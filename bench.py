@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- throughput of the clip.cpp encode path on N B200s of one node, one JSON line per run.
+"""bench.py -- throughput of the clip.cpp encode path on N H100s of one node, one JSON line per run.
 
     python bench.py --gpus 1 --steps 5 --warmup 3                    # headline: image-embeddings/sec, ViT-L/14 q4_0, b=512 per GPU
     python bench.py --config cfg2|cfg3|cfg4|cfg5                     # the other BASELINE.json configs (see CONFIGS)
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...      # one rank per GPU
     python bench.py --impl reference ...                             # the reference's CPU path on the host cores
+    python bench.py ... --dump-outputs DIR                           # also write what the last timed step computed, DIR/<name>.npy
 
 torch.distributed.run is only the LAUNCHER: the rank processes never import torch.  The library builds its own NCCL communicator
 from RANK / WORLD_SIZE / LOCAL_RANK / MASTER_PORT (clip_b200_dist_init: ncclCommInitRank, unique id through a rendezvous file), and
@@ -17,7 +18,8 @@ batch instead).
   e2e   : the same metric through the reference-facing C call with HOST buffers (H2D of the inputs, D2H of the embeddings timed)
 Timing: CUDA events on the library's launch stream (clip_b200_mark) around the K steps -- the NCCL all-gather is on that stream too
 -- bracketed by a barrier (all-reduce + device sync) on both sides, max over ranks (clip_b200_dist_max_f64).  Inputs per step exceed
-the 126 MB L2 for the image configs (308 MB / 154 MB of pixels); cfg4's token ids are tiny, its activations (> 1 GB per pass) are not.
+the H100's 50 MB L2 for the image configs (308 MB / 154 MB of pixels); cfg4's token ids are tiny, its activations (> 1 GB per pass) are not.
+Inputs are synthetic and seeded: the same arguments give the same inputs on every run, so two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -56,10 +58,6 @@ CONFIGS = {
                           "all-gathered, device logits + softmax + top-5 (BASELINE.json configs[4]); global sizes fixed"),
 }
 FTYPE_ID = {"f32": 0, "f16": 1, "q4_0": 2, "q4_1": 3, "q5_0": 6, "q5_1": 7, "q8_0": 8}
-
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of gemm_dq_kernel from the committed `ncu --set full` captures
-# (profiles/): mean over the four layer-GEMM shapes of the configuration's micro-batch; None = not captured for this config.
-NCU_GEMM_TRAFFIC = {"headline": (694_300_000, 742_900_000, "profiles/r02_gemm.md")}
 
 
 def log(*a):
@@ -103,7 +101,7 @@ def quantize_with_reference(src, dst, itype):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -146,7 +144,7 @@ def peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j.get("bf16_tflops_sustained", j.get("bf16_tflops", 1590.0))), "MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)"
-    return 1400.0, "fallback (B200_PROFILING.md: ~1.4 PFLOP/s sustained)"
+    return 989.0, "NVIDIA H100 SXM data sheet, dense BF16 (700 W part; not a measured rate)"
 
 
 # ---- CPU side: the reference's own implementation on a bounded sample ---------------------------------------------------
@@ -267,6 +265,12 @@ class Bench:
             out[nm] = {"ms_per_step": ms / steps, "launches_per_step": kcount.value / steps}
         return out
 
+    def fetch(self, d_ptr, shape):
+        """device fp32 buffer -> host array (after the stream has drained)"""
+        a = np.empty(shape, np.float32)
+        assert self.L.clip_b200_synchronize(self.ctx) and self.L.clip_b200_memcpy_d2h(self.ctx, a.ctypes.data, d_ptr, a.nbytes), self.lib.last_error()
+        return a
+
     def pinned(self, shape, dtype):
         n = int(np.prod(shape)) * np.dtype(dtype).itemsize
         p = self.L.clip_b200_host_malloc(n)
@@ -306,11 +310,12 @@ def bench_image(b, units):
     launches = (L.clip_b200_kernel_launches(ctx) - l0) + (args.steps if world > 1 else 0)
     clocks = sampler.stop() if rank == 0 else None
     kinds = b.kinds(args.steps)
+    dump = {"image_embeddings": b.fetch(d_all, (B * world, d))} if args.dump_outputs else {}
     for _ in range(2):
         step_e2e()
     ms_e2e, _ = b.timed(step_e2e, max(2, args.steps // 2))
     b.drop_profile()
-    res = {"ms_step": ms_step, "ms_wall": ms_wall, "launches": launches, "clocks": clocks, "kinds": kinds,
+    res = {"dump": dump, "ms_step": ms_step, "ms_wall": ms_wall, "launches": launches, "clocks": clocks, "kinds": kinds,
            "e2e": {"value": B * world / (ms_e2e / 1e3), "unit": "img/s", "h2d_bytes_per_step": B * per * 4, "d2h_bytes_per_step": B * world * d * 4,
                    "ms_per_step": ms_e2e, "call": "clip_b200_image_batch_encode_all" if world > 1 else "clip_image_batch_encode",
                    "host_buffers": "pinned (cudaMallocHost)"}}
@@ -385,12 +390,13 @@ def bench_text(b, units):
     launches = (L.clip_b200_kernel_launches(ctx) - l0) + (args.steps if world > 1 else 0)
     clocks = sampler.stop() if rank == 0 else None
     kinds = b.kinds(args.steps)
+    dump = {"text_embeddings": b.fetch(d_all, (TB * world, d))} if args.dump_outputs else {}
     for _ in range(2):
         step_e2e()
     ms_e2e, _ = b.timed(step_e2e, max(2, args.steps // 2))
     b.drop_profile()
     T_pad = (TL + 7) // 8 * 8 if TL < 77 else 77
-    return {"ms_step": ms_step, "ms_wall": ms_wall, "launches": launches, "clocks": clocks, "kinds": kinds,
+    return {"dump": dump, "ms_step": ms_step, "ms_wall": ms_wall, "launches": launches, "clocks": clocks, "kinds": kinds,
             "e2e": {"value": TB * world / (ms_e2e / 1e3), "unit": "seq/s", "h2d_bytes_per_step": TB * T_pad * 4 + TB * 4,
                     "d2h_bytes_per_step": TB * world * d * 4, "ms_per_step": ms_e2e,
                     "call": "clip_b200_text_batch_encode_all" if world > 1 else "clip_text_batch_encode", "host_buffers": "pageable clip_tokens arrays"}}
@@ -438,12 +444,14 @@ def bench_zsl(b, n_img_global, n_lab_global):
     launches = (L.clip_b200_kernel_launches(ctx) - l0) + (args.steps if world > 1 else 0)
     clocks = sampler.stop() if rank == 0 else None
     kinds = b.kinds(args.steps)
+    dump = {"image_embeddings": b.fetch(d_img, (B, d)), "label_embeddings": b.fetch(d_txt, (NL * world, d)),
+            "top5_scores": scores.copy(), "top5_labels": idx.astype(np.float64)} if args.dump_outputs else {}
     for _ in range(2):
         step_e2e()
     same = bool(np.array_equal(idx, ref_idx))
     ms_e2e, _ = b.timed(step_e2e, max(2, args.steps // 2))
     b.drop_profile()
-    return {"ms_step": ms_step, "ms_wall": ms_wall, "launches": launches, "clocks": clocks, "kinds": kinds, "units": B,
+    return {"dump": dump, "ms_step": ms_step, "ms_wall": ms_wall, "launches": launches, "clocks": clocks, "kinds": kinds, "units": B,
             "e2e": {"value": B * world / (ms_e2e / 1e3), "unit": "img/s", "h2d_bytes_per_step": B * per * 4 + NL * 80 * 4,
                     "d2h_bytes_per_step": B * K * 8, "ms_per_step": ms_e2e, "call": "clip_b200_zero_shot_images",
                     "top5_identical_to_device_resident_path": same}}
@@ -486,6 +494,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--quick", action="store_true", help=argparse.SUPPRESS)        # skip the secondary legs (ncu captures, probes)
     ap.add_argument("--no-text", action="store_true", help=argparse.SUPPRESS)       # kept for old command lines: same as --quick
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the arrays the timed path returned in its last step as DIR/<name>.npy (float32/float64)")
     args = ap.parse_args()
     args.quick = args.quick or args.no_text
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
@@ -511,6 +521,11 @@ def main():
         res = bench_image(b, units) if kind == "image" else bench_text(b, units)
     ms_step = res["ms_step"]
     value = units * world / (ms_step / 1e3)
+    dump = res.pop("dump")
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in dump.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), arr)
 
     if rank == 0:
         peak, peak_src = peaks()
@@ -523,7 +538,6 @@ def main():
             gemm_flops += (ft_total - ft_attn) * (cfg["labels"] // world)
         gemm_ms = res["kinds"]["gemm"]["ms_per_step"]
         achieved = gemm_flops / (gemm_ms / 1e3) / 1e12 if gemm_ms > 0 else 0.0
-        traffic = NCU_GEMM_TRAFFIC.get(args.config if not args.batch and scaling == "weak" else None)
         parity = parity_check(b) if kind != "zsl" else None
         cpu = None
         if world == 1 and not args.no_cpu_baseline:
@@ -536,14 +550,12 @@ def main():
         out = {
             "metric": metric, "value": value, "unit": unit, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms_step, "higher_is_better": True, "scaling": scaling, "vs_baseline": None,
-            "dtype": "bf16 (%s blocks unpacked to bf16 in-kernel, fp32 accumulate in TMEM; fp32 residual stream)" % cfg["ftype"], "data": "synthetic",
+            "dtype": "bf16 (%s blocks unpacked to bf16 in-kernel, fp32 accumulate in registers; fp32 residual stream)" % cfg["ftype"], "data": "synthetic",
             "config": {"workload": cfg["workload"], "name": args.config, "global_batch": units * world, "per_gpu_batch": units, "parallelism": "dp%d" % world,
-                       "l2": "inputs per step exceed the 126 MB L2 (no flush needed)" if kind != "text" else "token ids are tiny; the activations of a pass (> 1 GB) exceed L2",
+                       "l2": "inputs per step exceed the 50 MB L2 (no flush needed)" if kind != "text" else "token ids are tiny; the activations of a pass (> 1 GB) exceed L2",
                        "collective": "1 in-place NCCL all-gather of the final embeddings per step, enqueued by the C++ library (no torch in the rank processes)" if world > 1 else "none (1 GPU)"},
             "clocks": res["clocks"], "e2e": res["e2e"], "gpu_launches": int(res["launches"]),
             "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak if peak else None,
-                         "traffic": traffic[0] if traffic else None,
-                         "traffic_unit": ("bytes/launch (dram read+write, mean of the 4 layer GEMM shapes; %s) vs %d algorithmic" % (traffic[2], traffic[1])) if traffic else None,
                          "kernel": "gemm_dq_kernel (all fused-dequant GEMMs of the step)", "flops_per_step": gemm_flops, "kernel_ms_per_step": gemm_ms,
                          "peak_source": peak_src, "whole_step_frac": (f_total * units / (ms_step / 1e3) / 1e12) / peak if kind != "zsl" else None},
             "kernel_time_ms_per_step": res["kinds"], "wall_ms_per_step": res["ms_wall"], "parity": parity, "cpu_baseline": cpu,

@@ -3,7 +3,7 @@
 The same `ClipLib` class drives either shared library, because the product keeps the reference's
 22 exported symbols and struct layouts byte for byte:
 
-  * `libclip_b200.so`        -- the B200-native product (this repository)
+  * `libclip_b200.so`        -- the H100-native product (this repository)
   * the unmodified reference built under oracle/ (path: oracle/ref_run.py REF_LIB) -- tests / bench use it as the checker
 
 It mirrors the shape of the reference's own Python binding
@@ -59,7 +59,7 @@ REFERENCE_SYMBOLS = [
     "clip_zero_shot_label_image", "clip_model_quantize",
 ]
 
-# additive B200 entry points (include/clip_b200.h); absent from the reference library
+# additive entry points of this library (include/clip_b200.h); absent from the reference library
 EXTENSION_SYMBOLS = [
     "clip_text_batch_encode", "clip_b200_image_encode_device", "clip_b200_text_encode_device",
     "clip_b200_zero_shot_batch", "clip_b200_device_malloc", "clip_b200_device_free",

@@ -238,13 +238,7 @@ bool ensure_ws(clip_ctx* c, Tower& tw, int items, int T, bool vision) {
         !dev_alloc(c, &w.g, rows * tw.ff) || !dev_alloc(c, &w.sel16, (size_t)items * h) || !dev_alloc(c, &w.sel32, (size_t)items * h) ||
         !dev_alloc(c, &w.proj32, (size_t)items * tw.proj)) return false;
     bool ok = make_tma_2d_16bit(&w.map_a, w.a, rows, h, h, GEMM_BN) && make_tma_2d_16bit(&w.map_g, w.g, rows, tw.ff, tw.ff, GEMM_BN) &&
-              make_tma_2d_16bit(&w.map_sel, w.sel16, items, h, h, GEMM_BN) &&
-              make_tma_2d_16bit(&w.map_a_half, w.a, rows, h, h, GEMM_BN / 2) && make_tma_2d_16bit(&w.map_g_half, w.g, rows, tw.ff, tw.ff, GEMM_BN / 2) &&
-              make_tma_2d_16bit(&w.map_q128, w.qkv, rows, 3 * h, 3 * h, 128) &&
-              make_tma_2d_16bit(&w.map_kv16, w.qkv, rows, 3 * h, 3 * h, 16) &&
-              make_tma_2d_16bit_plain(&w.map_out_qkv, w.qkv, rows, 3 * h, 3 * h, GEMM_OUT_BOX, GEMM_OUT_BOX) &&
-              make_tma_2d_f32_plain(&w.map_out_x32, w.x, rows, h, h, GEMM_OUT_BOX, GEMM_OUT_BOX) &&
-              make_tma_2d_16bit_plain(&w.map_out_g, w.g, rows, tw.ff, tw.ff, GEMM_OUT_BOX, GEMM_OUT_BOX);
+              make_tma_2d_16bit(&w.map_sel, w.sel16, items, h, h, GEMM_BN);
     if (vision) {
         const size_t per = (size_t)tw.image_size * tw.image_size * 3;
         if (!dev_alloc(c, &w.pixels[0], items * per) || !dev_alloc(c, &w.pixels[1], items * per) ||
@@ -258,7 +252,7 @@ bool ensure_ws(clip_ctx* c, Tower& tw, int items, int T, bool vision) {
 }
 
 bool run_linear(clip_ctx* c, const Linear& L, const TmaMap* xmap, const void* xptr, bool x_bf16, int M, void* out, int ldo, int epi,
-                int out_bf16, int scale_cols = 0, float scale = 1.f, const TmaMap* xmap_half = nullptr, const TmaMap* out_map = nullptr) {
+                int out_bf16, int scale_cols = 0, float scale = 1.f) {
     Scope s(c, K_GEMM);
     if (c->debug_naive) {
         launch_naive_gemm(xptr, x_bf16, L.d_raw, L.qtype, L.d_bias, out, M, L.N, L.K, ldo, epi, out_bf16, scale_cols, scale, c->stream);
@@ -266,39 +260,30 @@ bool run_linear(clip_ctx* c, const Linear& L, const TmaMap* xmap, const void* xp
         return true;
     }
     GemmArgs a;
-    a.x_map = xmap; a.x_half_map = xmap_half; a.w_map = &L.w_map; a.w_packed = L.d_w; a.qtype = L.qtype; a.operand_bf16 = x_bf16;
+    a.x_map = xmap; a.w_map = &L.w_map; a.w_packed = L.d_w; a.qtype = L.qtype; a.operand_bf16 = x_bf16;
     a.bias = L.d_bias; a.out = out; a.M = M; a.N = L.N; a.K = L.K; a.ldo = ldo; a.epi = epi; a.out_bf16 = out_bf16;
-    a.scale_cols = scale_cols; a.scale = scale; a.out_map = out_map;
+    a.scale_cols = scale_cols; a.scale = scale;
     CK(gemm_launch(a, c->stream, c->num_sms, nullptr));
     return true;
 }
 
 // The per-layer schedule shared by both towers (clip.cpp:1064-1143 text, 1342-1423 vision).
 bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal) {
-    // The residual stream x stays fp32 (as in the reference).  The branch GEMMs (out-proj, FC2) add their result INTO x themselves: the
-    // epilogue stages fp32 blocks in shared memory and a TMA tensor reduce-add (cp.reduce.async.bulk.tensor .add) performs x += acc + bias
-    // in the memory system -- the SMs never read x for it, and the traffic hides under the tensor-bound GEMM.  LayerNorm then only reads
-    // x and writes its 16-bit output: 6 B per element instead of the 12 B of the round-1 "deferred residual" scheme.
+    // The residual stream x stays fp32 (as in the reference).  The branch GEMMs (out-proj, FC2) add their result INTO x themselves
+    // (EPI_REDADD32): LayerNorm then only reads x and writes its 16-bit output.
     Workspace& w = tw.ws;
     const int M = nseq * T, h = tw.hidden;
     const int bf = c->operand_bf16 ? 1 : 0;
     const float qscale = 1.0f / sqrtf(64.0f);
     for (auto& l : tw.L) {
         { Scope s(c, K_LN); launch_layernorm(w.x, h, M, h, tw.eps, l.ln1_g, l.ln1_b, nullptr, w.a, bf, c->stream); }
-        if (!run_linear(c, l.qkv, &w.map_a, w.a, bf, M, w.qkv, 3 * h, EPI_STORE16, bf, h, qscale, &w.map_a_half, &w.map_out_qkv)) return false;
-        if (c->attn_tc && attention_tc_supported(T)) {
-            const int q_done = attention_tc_tiles(T) * 128;
-            { Scope s(c, K_ATTN); CK(launch_attention_tc(&w.map_q128, w.qkv, &w.map_kv16, w.a, nseq, T, tw.heads, causal ? 1 : 0, bf, c->num_sms, c->stream)); }
-            if (q_done < T) { Scope s(c, K_ATTN); launch_attention(w.qkv, w.a, nseq, T, tw.heads, causal ? 1 : 0, bf, q_done, c->stream); }
-        } else if (c->attn_tc && attention_tc_long_supported(T, causal ? 1 : 0)) {
-            Scope s(c, K_ATTN); CK(launch_attention_tc_long(&w.map_q128, w.qkv, w.a, nseq, T, tw.heads, bf, c->num_sms, c->stream));
-        } else {
-            Scope s(c, K_ATTN); launch_attention(w.qkv, w.a, nseq, T, tw.heads, causal ? 1 : 0, bf, 0, c->stream);
-        }
-        if (!run_linear(c, l.out, &w.map_a, w.a, bf, M, w.x, h, EPI_REDADD32, 0, 0, 1.f, &w.map_a_half, &w.map_out_x32)) return false;
+        if (!run_linear(c, l.qkv, &w.map_a, w.a, bf, M, w.qkv, 3 * h, EPI_STORE16, bf, h, qscale)) return false;
+        if (c->attn_tc) { Scope s(c, K_ATTN); CK(launch_attention_tc(w.qkv, w.a, nseq, T, tw.heads, causal ? 1 : 0, bf, c->stream)); }
+        else { Scope s(c, K_ATTN); launch_attention(w.qkv, w.a, nseq, T, tw.heads, causal ? 1 : 0, bf, c->stream); }
+        if (!run_linear(c, l.out, &w.map_a, w.a, bf, M, w.x, h, EPI_REDADD32, 0)) return false;
         { Scope s(c, K_LN); launch_layernorm(w.x, h, M, h, tw.eps, l.ln2_g, l.ln2_b, nullptr, w.a, bf, c->stream); }
-        if (!run_linear(c, l.fc1, &w.map_a, w.a, bf, M, w.g, tw.ff, c->use_gelu ? EPI_GELU16 : EPI_QGELU16, bf, 0, 1.f, &w.map_a_half, &w.map_out_g)) return false;
-        if (!run_linear(c, l.fc2, &w.map_g, w.g, bf, M, w.x, h, EPI_REDADD32, 0, 0, 1.f, &w.map_g_half, &w.map_out_x32)) return false;
+        if (!run_linear(c, l.fc1, &w.map_a, w.a, bf, M, w.g, tw.ff, c->use_gelu ? EPI_GELU16 : EPI_QGELU16, bf)) return false;
+        if (!run_linear(c, l.fc2, &w.map_g, w.g, bf, M, w.x, h, EPI_REDADD32, 0)) return false;
     }
     CK(cudaGetLastError());
     return true;
@@ -357,13 +342,11 @@ bool ensure_buf(clip_ctx* c, T** buf, size_t* cap, size_t count) {
 }
 bool ensure_out(clip_ctx* c, size_t floats) { return ensure_buf(c, &c->d_out, &c->d_out_cap, floats); }
 
-int default_micro_batch(int T) {   // 37 token tiles = 148/4: every N/128 that is a multiple of 4 fills whole waves
-    // measured on B200 (ViT-L/14 q4_0, b=512, final kernels): 3 -> 4914, 4 -> 5062, 8 -> 5219, 12 -> 5316 img/s, one chunk of 512 -> 5394
-    // device-resident but 5298 end to end (the H2D copy of a single chunk cannot hide under compute).  Fewer, longer launches: the
-    // ~3 us drain/fill gap per launch is paid 1200 times per 512 images at 3 waves.  12 waves = 331 ViT-L/14 images = 1.9 GB of workspace.
+int default_micro_batch(int T) {   // 33 token tiles = 132/4: every N/128 that is a multiple of 4 fills whole waves of the H100's SMs
+    // Fewer, longer launches: each launch pays a drain/fill gap of a few microseconds.  12 waves = 295 ViT-L/14 images = 1.7 GB of workspace.
     int waves = 12;
-    if (const char* e = getenv("CLIP_B200_TOKEN_TILES_X37")) waves = std::max(1, atoi(e));
-    const int mb = 37 * waves * GEMM_BN / T;
+    if (const char* e = getenv("CLIP_B200_TOKEN_TILES_X33")) waves = std::max(1, atoi(e));
+    const int mb = 33 * waves * GEMM_BN / T;
     return mb < 1 ? 1 : mb;
 }
 
@@ -444,7 +427,7 @@ bool host_ptr_is_pinned(const void* p) {
 extern "C" {
 
 const char* clip_b200_last_error(void) { return g_err.c_str(); }
-const char* clip_b200_version(void) { return "clip_b200 0.1 (sm_100a; tcgen05 fused-dequant GEMM)"; }
+const char* clip_b200_version(void) { return "clip_b200 0.1 (sm_90a; wgmma fused-dequant GEMM)"; }
 
 // one replica of the model on `device` (weights are <= 0.33 GB: replicated, never sharded -- SURVEY.md section 8e)
 static clip_ctx* load_on_device(const GgufFile& g, int device, const int verbosity) {
@@ -455,7 +438,7 @@ static clip_ctx* load_on_device(const GgufFile& g, int device, const int verbosi
         if (cudaSetDevice(c->device) != cudaSuccess) { set_err("cudaSetDevice failed"); return nullptr; }
         cudaDeviceProp prop;
         if (cudaGetDeviceProperties(&prop, c->device) != cudaSuccess) { set_err("cudaGetDeviceProperties failed"); return nullptr; }
-        if (prop.major != 10) { set_err(std::string("device '") + prop.name + "' is not sm_100: this library only contains sm_100a code"); return nullptr; }
+        if (prop.major != 9 || prop.minor != 0) { set_err(std::string("device '") + prop.name + "' is not sm_90: this library only contains sm_90a code"); return nullptr; }
         c->num_sms = prop.multiProcessorCount;
         c->debug_naive = getenv("CLIP_B200_DEBUG_NAIVE") && atoi(getenv("CLIP_B200_DEBUG_NAIVE")) != 0;
         c->profile = getenv("CLIP_B200_PROFILE") && atoi(getenv("CLIP_B200_PROFILE")) != 0;
@@ -1471,12 +1454,9 @@ int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int e
         if (bias) { cudaMalloc(&d_bias, (size_t)N * 4); cudaMemcpy(d_bias, bias, (size_t)N * 4, cudaMemcpyHostToDevice); }
         if (epi == EPI_REDADD32 && resid_in) cudaMemcpy(d_out, resid_in, out_bytes, cudaMemcpyHostToDevice);
         else cudaMemset(d_out, 0, out_bytes);
-        TmaMap xm, xh, wm, om;
+        TmaMap xm, wm;
         memset(&wm, 0, sizeof(wm));
-        const bool use_out_map = epi != EPI_STORE32 && !(getenv("CLIP_B200_DEBUG_DIRECT_STORE") && atoi(getenv("CLIP_B200_DEBUG_DIRECT_STORE")) != 0);
-        if (use_out_map && !(out32 ? make_tma_2d_f32_plain(&om, d_out, M, N, N, GEMM_OUT_BOX, GEMM_OUT_BOX)
-                                   : make_tma_2d_16bit_plain(&om, d_out, M, N, N, GEMM_OUT_BOX, GEMM_OUT_BOX))) { set_err("tensor map OUT failed"); rc = 4; break; }
-        if (!make_tma_2d_16bit(&xm, d_x, M, K, K, GEMM_BN) || !make_tma_2d_16bit(&xh, d_x, M, K, K, GEMM_BN / 2)) { set_err("tensor map X failed"); rc = 4; break; }
+        if (!make_tma_2d_16bit(&xm, d_x, M, K, K, GEMM_BN)) { set_err("tensor map X failed"); rc = 4; break; }
         if (eff_q == QT_F16 && !make_tma_2d_16bit(&wm, d_w, N, K, K, GEMM_BM)) { set_err("tensor map W failed"); rc = 4; break; }
         cudaEventRecord(e0, st);
         if (use_naive) {
@@ -1484,9 +1464,9 @@ int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int e
             e = cudaGetLastError();
         } else {
             GemmArgs a;
-            a.x_map = &xm; a.x_half_map = &xh; a.w_map = &wm; a.w_packed = (const uint8_t*)d_w; a.qtype = eff_q; a.operand_bf16 = operand_bf16 != 0;
+            a.x_map = &xm; a.w_map = &wm; a.w_packed = (const uint8_t*)d_w; a.qtype = eff_q; a.operand_bf16 = operand_bf16 != 0;
             a.bias = d_bias; a.out = d_out; a.M = M; a.N = N; a.K = K; a.ldo = N; a.epi = epi; a.out_bf16 = operand_bf16;
-            a.scale_cols = N / 2; a.scale = 0.125f; a.out_map = use_out_map ? &om : nullptr;
+            a.scale_cols = N / 2; a.scale = 0.125f;
             e = gemm_launch(a, st, prop.multiProcessorCount, nullptr);
         }
         cudaEventRecord(e1, st);
@@ -1514,11 +1494,6 @@ int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int e
 int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int causal, int use_legacy, const float* qkv, float* out, float* ms) {
     g_err.clear();
     if (attention_tc_init() != cudaSuccess) { set_err("attention_tc_init failed"); return 1; }
-    if (!use_legacy && !attention_tc_supported(T) && !attention_tc_long_supported(T, causal)) { set_err("T not supported by the tcgen05 attention kernels"); return 2; }
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceProp prop;
-    cudaGetDeviceProperties(&prop, dev);
     const size_t rows = (size_t)nseq * T, hid = (size_t)H * 64;
     std::vector<uint16_t> h16(rows * 3 * hid);
     for (size_t i = 0; i < h16.size(); i++) h16[i] = operand_bf16 ? f32_to_bf16(qkv[i]) : f32_to_f16(qkv[i]);
@@ -1528,22 +1503,18 @@ int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int caus
     int rc = 0;
     do {
         cudaError_t e;
-        // pad by one 272-row box: the K/V boxes of the last sequence read (and discard) rows past the end
-        if ((e = cudaMalloc(&d_qkv, (rows + 272) * 3 * hid * 2)) != cudaSuccess || (e = cudaMalloc(&d_out, rows * hid * 2)) != cudaSuccess) { set_err(std::string("cudaMalloc: ") + cudaGetErrorString(e)); rc = 3; break; }
+        // one 128-row box of padding past the last sequence
+        if ((e = cudaMalloc(&d_qkv, (rows + 128) * 3 * hid * 2)) != cudaSuccess || (e = cudaMalloc(&d_out, rows * hid * 2)) != cudaSuccess) { set_err(std::string("cudaMalloc: ") + cudaGetErrorString(e)); rc = 3; break; }
         // the padding is POISONED (0xFFFF = NaN in fp16 and bf16): rows past the last sequence are stale memory in the model path
         // (ensure_ws never initialises the workspace tail), and no output may depend on them
-        cudaMemset(d_qkv, 0xff, (rows + 272) * 3 * hid * 2);
+        cudaMemset(d_qkv, 0xff, (rows + 128) * 3 * hid * 2);
         cudaMemset(d_out, 0xff, rows * hid * 2);
         cudaMemcpy(d_qkv, h16.data(), h16.size() * 2, cudaMemcpyHostToDevice);
         cudaStreamCreate(&st); cudaEventCreate(&e0); cudaEventCreate(&e1);
-        TmaMap mq, m16;
-        if (!make_tma_2d_16bit(&mq, d_qkv, rows, 3 * hid, 3 * hid, 128) ||
-            !make_tma_2d_16bit(&m16, d_qkv, rows, 3 * hid, 3 * hid, 16)) { set_err("tensor map failed"); rc = 4; break; }
         for (int rep = 0; rep < (ms ? 3 : 1); rep++) {
             cudaEventRecord(e0, st);
-            if (use_legacy) { launch_attention(d_qkv, d_out, nseq, T, H, causal, operand_bf16, 0, st); e = cudaGetLastError(); }
-            else if (attention_tc_supported(T)) e = launch_attention_tc(&mq, d_qkv, &m16, d_out, nseq, T, H, causal, operand_bf16, prop.multiProcessorCount, st);
-            else e = launch_attention_tc_long(&mq, d_qkv, d_out, nseq, T, H, operand_bf16, prop.multiProcessorCount, st);
+            if (use_legacy) { launch_attention(d_qkv, d_out, nseq, T, H, causal, operand_bf16, st); e = cudaGetLastError(); }
+            else e = launch_attention_tc(d_qkv, d_out, nseq, T, H, causal, operand_bf16, st);
             cudaEventRecord(e1, st);
             if (e != cudaSuccess) break;
             if ((e = cudaStreamSynchronize(st)) != cudaSuccess) break;

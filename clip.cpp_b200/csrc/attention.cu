@@ -9,7 +9,7 @@
 // Layout: qkv is the fused QKV GEMM output [tokens, 3*hidden] (Q | K | V, 16-bit), out is [tokens, hidden].
 // head_dim = 64 (true for ViT-B/32, B/16, L/14, L/14-336 and their text towers).
 // Tensor-core path: warp-level mma.sync m16n8k16 (fp16 or bf16 inputs, fp32 accumulate).  Attention is ~4% of the
-// model FLOPs (SURVEY.md section 8d); the tcgen05/TMEM version is listed as follow-up work in DESIGN.md.
+// model FLOPs (SURVEY.md section 8d); the production path is the wgmma kernel in attention_tc.cu, this one is its cross-check.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -73,12 +73,12 @@ CB_DEVINL void load_tile(uint32_t smem_tile, const uint16_t* g, int ld, int row0
 
 template <bool BF>
 __global__ void __launch_bounds__(128) attention_kernel(const uint16_t* __restrict__ qkv, uint16_t* __restrict__ out, int T, int H,
-                                                        int causal, int qt0) {
+                                                        int causal) {
     __shared__ __align__(128) uint8_t sQ[TQ * 128];
     __shared__ __align__(128) uint8_t sK[2][TK * 128];
     __shared__ __align__(128) uint8_t sV[2][TK * 128];
 
-    const int qt = blockIdx.x + qt0, head = blockIdx.y, seq = blockIdx.z;   // qt0: first 64-query tile (rows before it are done by attention_tc.cu)
+    const int qt = blockIdx.x, head = blockIdx.y, seq = blockIdx.z;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t4 = lane & 3;
     const int hid = H * DH, ld = 3 * hid;
     const uint16_t* base = qkv + (size_t)seq * T * ld + head * DH;
@@ -213,18 +213,17 @@ __global__ void __launch_bounds__(128) attention_kernel(const uint16_t* __restri
 
 }  // namespace
 
-void launch_attention(const void* qkv16, void* out16, int nseq, int T, int H, int causal, int bf16, int q_start, cudaStream_t st) {
-    if (nseq <= 0 || q_start >= T) return;
-    const int qt0 = q_start / TQ;
+void launch_attention(const void* qkv16, void* out16, int nseq, int T, int H, int causal, int bf16, cudaStream_t st) {
+    if (nseq <= 0) return;
     // gridDim.z limit is 65535: chunk over sequences
     const int hid = H * DH;
     for (int s0 = 0; s0 < nseq; s0 += 65535) {
         const int ns = (nseq - s0) < 65535 ? (nseq - s0) : 65535;
-        dim3 grid((T + TQ - 1) / TQ - qt0, H, ns);
+        dim3 grid((T + TQ - 1) / TQ, H, ns);
         const uint16_t* q = (const uint16_t*)qkv16 + (size_t)s0 * T * 3 * hid;
         uint16_t* o = (uint16_t*)out16 + (size_t)s0 * T * hid;
-        if (bf16) attention_kernel<true><<<grid, 128, 0, st>>>(q, o, T, H, causal, qt0);
-        else attention_kernel<false><<<grid, 128, 0, st>>>(q, o, T, H, causal, qt0);
+        if (bf16) attention_kernel<true><<<grid, 128, 0, st>>>(q, o, T, H, causal);
+        else attention_kernel<false><<<grid, 128, 0, st>>>(q, o, T, H, causal);
     }
 }
 

@@ -1,69 +1,40 @@
-// attention_tc.cu -- K3 on tcgen05: S = Q K^T and O = P V as UMMA instructions with both accumulators in TENSOR MEMORY.
+// attention_tc.cu -- K3 on Hopper tensor cores: S = Q K^T and O = P V as warpgroup MMAs (wgmma), online softmax in registers.
 //
 // Reference semantics: clip.cpp:1082-1108 (text, causal) / 1363-1388 (vision); soft_max ggml.c:12201-12270.
-// One persistent CTA per SM (640 threads, all 512 TMEM columns, 180 KB shared memory) walks (sequence, head) items; K and V of an
-// item stay in shared memory for all of its 128-query tiles and the next item's K/V are prefetched into the second stage:
-//   warp 0      TMA: K and V boxes [256 (+16) keys x 64] straight out of the fused QKV activation matrix (3-D view, row stride 3*hidden),
-//               the item's LAST query row when T % 128 == 1, and its Q boxes [128 x 64] (two slots)
-//   warp 1      one elected thread: S[128 x <=256] = Q.K^T (SS form, 4 UMMA k-steps) into TMEM buffer g&1, then
-//               O[128 x 64] = P.V (TS form: A = P from TMEM, B = V taken MN-major from the same [key][dh] tile).  S of tile g+1
-//               is issued BEFORE P.V of tile g, so the tensor core works on the next scores while tile g is in softmax.
-//   warps 4-11 / 12-19   two softmax groups, one per TMEM buffer (even / odd tiles), TMEM lane == query row.  Two warps share
-//               each 32-row quarter and split the key chunks / output dims; they exchange row max and row sum through shared
-//               memory (named barrier per pair).  Pass 1 row max over tcgen05.ld chunks, pass 2 p = 2^((s-m)*log2e) -> bf16/fp16
-//               pairs written IN PLACE over consumed S columns (tcgen05.st), row sum in fp32; after the PV commit: O / l ->
-//               64-byte row stores.  Exact two-pass maximum: the result of a row does not depend on T or on the batch around it.
-//               Key 256 of ViT-L/14 (257 tokens) does not fit the 256-column S tile: its score and its p*V term are one 64-long
-//               dot product / axpy per row on the CUDA cores, straight from the shared-memory tiles.
-//   warps 2, 3  the 257th QUERY row (T % 128 == 1) on the CUDA cores, alternating items: 257 dot products, softmax, 257 axpys out
-//               of the K/V tiles in shared memory -- a third, 127/128-empty tensor-core tile would cost a full pipeline slot.
-//   warp 2      also TMEM alloc (per buffer: S columns [0,256); P [0,64) and [128,192) in place; O [192,256) once S is dead)
-// HBM traffic: Q, K, V read exactly once, O written once.  Limits: head_dim 64, T <= 257 for this kernel; attention_tc_long_kernel
-// further down covers 257 < T <= 640 (non-causal) with an online softmax over 192-key blocks.
-// K / V boxes come through a per-launch 3-D tensor map [sequence][token][column]: rows past a sequence's T tokens are zero-filled by
-// TMA, so padded keys can never inject another sequence's (or stale) NaN / Inf into P.V.  The MMA issuer is one elected thread.
-// History (ViT-L/14, 82 images per launch): mma.sync flash kernel 148 us -> v3 (serial phases, 2 CTAs/SM) 88 us -> v4 (K/V resident,
-// ping-pong groups) 78 us -> this kernel 65 us; profiles/r01_attention.md has the stall breakdown.  Per item the kernel needs
-// ~4.1 K MUFU cycles, ~5 K tcgen05.ld cycles and ~5.8 K issue cycles per scheduler; a single-pass variant with a lazily raised
-// exponent offset (one tcgen05.ld pass) was measured SLOWER (its per-chunk max -> exp dependency serialises each warp) and is
-// not batch-invariant, so the exact two-pass form stays.
+// One CTA per (128-query tile, head, sequence), 288 threads, 81 KB of shared memory:
+//   warp 8      producer, one thread: TMA of the Q tile [128 x 64], then K and V blocks [128 keys x 64] into a two-deep ring, all
+//               straight out of the fused QKV activation matrix through a 3-D view [sequence][token][column]: rows past a sequence's
+//               T tokens arrive as zeros, so padded keys can never inject another sequence's (or stale) NaN / Inf into P.V
+//   warps 0-7   two consumer warpgroups, 64 query rows each.  Per key block: S[64 x 128] = Q.K^T (4 wgmma m64n128k16, both operands
+//               from shared memory), length / causal mask, online softmax (running row max and sum, quad shuffles), the probabilities
+//               re-packed IN REGISTERS as 16-bit A fragments, O[64 x 64] += P.V (8 wgmma m64n64k16, A from registers, V read MN-major
+//               from the same [key][dh] tile).  O / l -> 32-bit stores.
+// HBM traffic: Q read once, K and V once per query tile, O written once.  head_dim 64, any T; a causal tile stops at its diagonal block.
 #include <cuda.h>
 
 #include "common.cuh"
 #include "gemm.h"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace cb {
 
 namespace {
 
-constexpr int AQ = 128, AKMAX = 272, DH = 64;
-constexpr uint32_t Q_BYTES = AQ * 128, KV_BYTES = AKMAX * 128;
-// shared memory: two K/V stages [K 272 rows | V 272 rows] (next (sequence, head) prefetched), two Q slots
-constexpr uint32_t Q_OFF = 4 * KV_BYTES;               // 139264
-constexpr uint32_t QX_OFF = Q_OFF + 2 * Q_BYTES;       // 172032: two 16-row boxes holding the LAST query row of an item (CUDA-core path)
-constexpr uint32_t BAR_OFF = QX_OFF + 2 * 2048;        // 176128
-constexpr uint32_t XM_OFF = BAR_OFF + 256;             // row max [group][half][128] then row sum [group][half][128], fp32
-constexpr uint32_t PB_OFF = XM_OFF + 4096, PB_BYTES = 1152;   // probabilities of the last-row path, one buffer per row warp
-constexpr uint32_t ATT_SMEM = PB_OFF + 2 * PB_BYTES + 1024;
-constexpr int ATT_THREADS = 640;                       // TMA, MMA, 2 last-row warps, 2 softmax groups of 8 warps
-// TMEM: two score buffers of 256 columns.  In each: S fp32 [0,256); P (16-bit pairs) overwrites [0,128); O fp32 [128,192) once S is dead
-constexpr uint32_t TMEM_COLS = 512, S_COLS = 256, O_COL = 192;
-static_assert(KV_BYTES % 1024 == 0 && Q_OFF % 1024 == 0, "tile alignment");
+constexpr int AQ = 128, AK = 128, DH = 64;
+constexpr uint32_t Q_BYTES = AQ * 128, KV_BYTES = AK * 128;
+constexpr uint32_t KV_OFF = Q_BYTES;                   // two stages [K | V]
+constexpr uint32_t BAR_OFF = KV_OFF + 4 * KV_BYTES;
+constexpr uint32_t ATT_SMEM = BAR_OFF + 64 + 1024;
+constexpr int ATT_THREADS = 288;                       // 2 consumer warpgroups + 1 producer warp
+static_assert(KV_OFF % 1024 == 0 && KV_BYTES % 1024 == 0, "tile alignment");
 
 struct AParams {
-    CUtensorMap tm_q, tm_kv256, tm_kv16;
+    CUtensorMap tm_qkv;
     uint16_t* out;
-    int T, H, nseq, causal, ntile, nk16, last_row, desc;
+    int T, H, ntile, causal;
 };
 
-CB_DEVINL void tmem_st_32x16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-        "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
 CB_DEVINL void tma_load_3d(uint32_t dst_smem, const void* tmap, int c0, int c1, int c2, uint32_t bar) {
     asm volatile(
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst_smem),
@@ -78,684 +49,140 @@ CB_DEVINL uint32_t pack2(float lo, float hi) {
     else asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
     return r;
 }
-// instruction descriptor with runtime N; bmn = B operand is MN-major (V tile [key][dh]: dh contiguous)
-CB_DEVINL uint32_t idesc_n(bool bf, int N, bool bmn) {
-    return (1u << 4) | ((bf ? 1u : 0u) << 7) | ((bf ? 1u : 0u) << 10) | ((bmn ? 1u : 0u) << 16) | ((uint32_t)(N >> 3) << 17) | ((128u >> 4) << 24);
-}
-// MN-major operand tile: rows = k (128 B each = 64 MN elements), 8-row swizzle groups 1024 B apart (SBO); one 64-wide MN block (LBO unused)
-CB_DEVINL uint64_t umma_desc_mn128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)(1024 >> 4) << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-// bf16 / fp16 pair -> two floats
-template <bool BF>
-CB_DEVINL float2 unpack2(uint32_t u) {
-    if constexpr (BF) return make_float2(__uint_as_float(u << 16), __uint_as_float(u & 0xffff0000u));
-    else { const __half2 h = *reinterpret_cast<const __half2*>(&u); return __half22float2(h); }
-}
-CB_DEVINL uint4 lds128a(uint32_t a) {
-    uint4 v;
-    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
-    return v;
-}
-
-CB_DEVINL void pair_bar_sync(int id) { asm volatile("bar.sync %0, 64;" ::"r"(id) : "memory"); }
-CB_DEVINL uint32_t lds32a(uint32_t a) { uint32_t v; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a)); return v; }
-CB_DEVINL float4 lds128f(uint32_t a) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
-    return v;
-}
-CB_DEVINL void sts32f(uint32_t a, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); }
-CB_DEVINL float lds32f(uint32_t a) { float v; asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a)); return v; }
-
 template <bool BF>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __grid_constant__ AParams p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     const uint32_t smem_base = smem_u32(smem);
-    const uint32_t bars = smem_base + BAR_OFF;
-    // two-deep rings everywhere: index [0|1] = +8 bytes
-    const uint32_t kv_full = bars, kv_empty = bars + 16, q_full = bars + 32, q_empty = bars + 48, s_full = bars + 64, p_full = bars + 80,
-                   o_full = bars + 96, s_free = bars + 112, qx_full = bars + 128, qx_empty = bars + 144;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + BAR_OFF + 192);
+    const uint32_t q_full = smem_base + BAR_OFF, kv_full = q_full + 8, kv_empty = q_full + 24;     // kv rings: [0|1] = +8 bytes
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int ntile = p.ntile;
-    const bool last_row = p.last_row != 0;                 // T % 128 == 1: the last query row is done on the CUDA cores (warps 2, 3)
+    const int qt = blockIdx.x % p.ntile, head = (blockIdx.x / p.ntile) % p.H, seq = blockIdx.x / (p.ntile * p.H);
     if (threadIdx.x == 0) {
-        for (int i = 0; i < 2; i++) {
-            mbar_init(kv_full + 8 * i, 1); mbar_init(kv_empty + 8 * i, 8 * ntile + (last_row ? 1 : 0));
-            mbar_init(q_full + 8 * i, 1);  mbar_init(q_empty + 8 * i, 8);
-            mbar_init(s_full + 8 * i, 1);  mbar_init(p_full + 8 * i, 8);
-            mbar_init(o_full + 8 * i, 1);  mbar_init(s_free + 8 * i, 8);
-            mbar_init(qx_full + 8 * i, 1); mbar_init(qx_empty + 8 * i, 1);
-        }
+        mbar_init(q_full, 1);
+        for (int i = 0; i < 2; i++) { mbar_init(kv_full + 8 * i, 1); mbar_init(kv_empty + 8 * i, 8); }   // released by each consumer warp
         mbar_fence_init();
-        tma_prefetch_desc(&p.tm_q); tma_prefetch_desc(&p.tm_kv256); tma_prefetch_desc(&p.tm_kv16);
+        tma_prefetch_desc(&p.tm_qkv);
     }
-    if (warp == 2) tmem_alloc(smem_u32(tmem_slot), TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_trigger();
     pdl_wait();      // qkv is read (and the output written) only after the QKV GEMM grid has completed
 
-    const int hid = p.H * DH, nitems = p.nseq * p.H;
-    const int n_local = (nitems - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;      // (sequence, head) items of this CTA
-    const int G = n_local * ntile;                                                              // query tiles of this CTA
-    const int nmma = p.nk16 < 256 ? p.nk16 : 256;          // keys whose scores come from the tensor core
-    const bool extra = p.T > 256;                          // key 256 (ViT-L/14: T = 257) is folded in on the CUDA cores
-    const uint32_t kv_tx = 32768u + (extra ? 2048u : 0u);
-    const int nch = (nmma + 31) >> 5;                      // 32-key chunks of a score row
-    const int nch_a = (nch + 1) >> 1;                      // chunks [0, nch_a) belong to the first warp of a row pair, the rest to the second
+    const int hid = p.H * DH, c = head * DH, q0 = qt * AQ;
+    const int kend = p.causal ? min(p.T, q0 + AQ) : p.T;      // keys any row of this tile can see
+    const int nkb = (kend + AK - 1) / AK;
 
-    if (warp == 0) {
-        // ------------------------------------------------------------------ TMA producer: K/V (+ the last query row) once per
-        // (sequence, head), then its 128-query tiles
-        int g = 0;
-        for (int i = 0; i < n_local; i++) {
-            const int item = p.desc ? nitems - 1 - ((int)blockIdx.x + i * (int)gridDim.x) : (int)blockIdx.x + i * (int)gridDim.x, head = item % p.H, seq = item / p.H;   // descending: the QKV GEMM's last rows are in L2
-            const uint32_t st = i & 1, k_s = smem_base + st * (2 * KV_BYTES), v_s = k_s + KV_BYTES;
-            const int row0 = seq * p.T, c = head * DH;
-            mbar_wait(kv_empty + 8 * st, ((i >> 1) & 1) ^ 1);
-            if (elect_one()) {
-                mbar_arrive_expect_tx(kv_full + 8 * st, 2 * kv_tx);
-                // 3-D view [sequence][token][column]: rows past THIS sequence's T tokens are out of bounds and arrive as zeros, so the
-                // padded keys of the P.V product can never pick up another sequence's (or stale) NaN / Inf through 0 * x
-                tma_load_3d(k_s, &p.tm_kv256, hid + c, 0, seq, kv_full + 8 * st);
-                tma_load_3d(v_s, &p.tm_kv256, 2 * hid + c, 0, seq, kv_full + 8 * st);
-                if (extra) {
-                    tma_load_2d(k_s + 32768, &p.tm_kv16, hid + c, row0 + 256, kv_full + 8 * st);
-                    tma_load_2d(v_s + 32768, &p.tm_kv16, 2 * hid + c, row0 + 256, kv_full + 8 * st);
-                }
-            }
-            __syncwarp();
-            if (last_row) {
-                mbar_wait(qx_empty + 8 * st, ((i >> 1) & 1) ^ 1);
-                if (elect_one()) {
-                    mbar_arrive_expect_tx(qx_full + 8 * st, 2048);
-                    tma_load_2d(smem_base + QX_OFF + st * 2048, &p.tm_kv16, c, row0 + p.T - 1, qx_full + 8 * st);
-                }
-                __syncwarp();
-            }
-            for (int qt = 0; qt < ntile; qt++, g++) {
-                const uint32_t sl = g & 1;
-                mbar_wait(q_empty + 8 * sl, ((g >> 1) & 1) ^ 1);
-                if (elect_one()) {
-                    mbar_arrive_expect_tx(q_full + 8 * sl, Q_BYTES);
-                    tma_load_2d(smem_base + Q_OFF + sl * Q_BYTES, &p.tm_q, c, row0 + qt * AQ, q_full + 8 * sl);
-                }
-                __syncwarp();
+    if (warp == 8) {
+        // ------------------------------------------------------------------ producer (one thread)
+        if (lane == 0) {
+            mbar_arrive_expect_tx(q_full, Q_BYTES);
+            tma_load_3d(smem_base, &p.tm_qkv, c, q0, seq, q_full);
+            for (int kb = 0; kb < nkb; kb++) {
+                const uint32_t s = kb & 1, k_s = smem_base + KV_OFF + s * (2 * KV_BYTES);
+                mbar_wait(kv_empty + 8 * s, ((kb >> 1) & 1) ^ 1);
+                mbar_arrive_expect_tx(kv_full + 8 * s, 2 * KV_BYTES);
+                tma_load_3d(k_s, &p.tm_qkv, hid + c, kb * AK, seq, kv_full + 8 * s);
+                tma_load_3d(k_s + KV_BYTES, &p.tm_qkv, 2 * hid + c, kb * AK, seq, kv_full + 8 * s);
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer.  S(g+1) is issued BEFORE P.V(g): the
-        // tensor core computes the next score tile while softmax group g&1 is busy, and the two groups keep the MUFU pipe fed.
-        // ONE elected thread runs the whole issue loop (no re-election / reconvergence per tile): the issuer shares its scheduler with
-        // four softmax warps, and every instruction it does not execute shortens the S -> softmax -> P.V chain (same finding as K1's issuer)
-        const uint32_t id_s = idesc_n(BF, nmma, false), id_pv = idesc_n(BF, DH, true);
-        const int npv = nmma >> 4;
-        if (elect_one()) {
-        auto issue_s = [&](int g) {
-            const uint32_t sl = g & 1, u = (g >> 1) & 1;
-            const int i = g / ntile, qt = g - i * ntile;
-            if (qt == 0) mbar_wait(kv_full + 8 * (i & 1), (i >> 1) & 1);
-            mbar_wait(q_full + 8 * sl, u);
-            mbar_wait(s_free + 8 * sl, u ^ 1);          // the epilogue of tile g-2 has read O out of this TMEM buffer
-            tc_fence_after();
-            const uint64_t dq = umma_desc_k128(smem_base + Q_OFF + sl * Q_BYTES), dk = umma_desc_k128(smem_base + (i & 1) * (2 * KV_BYTES));
-            const uint32_t d = tmem_base + sl * S_COLS;
-            umma_f16_init(d, dq, dk, id_s);
-            umma_f16_acc(d, dq + 2, dk + 2, id_s);
-            umma_f16_acc(d, dq + 4, dk + 4, id_s);
-            umma_f16_acc(d, dq + 6, dk + 6, id_s);
-            umma_commit(s_full + 8 * sl);
-        };
-        if (G > 0) issue_s(0);
-        for (int g = 0; g < G; g++) {
-            if (g + 1 < G) issue_s(g + 1);
-            const uint32_t sl = g & 1;
-            const int i = g / ntile;
-            mbar_wait(p_full + 8 * sl, (g >> 1) & 1);
-            tc_fence_after();
-            const uint64_t dv = umma_desc_mn128(smem_base + (i & 1) * (2 * KV_BYTES) + KV_BYTES);
-            const uint32_t pa = tmem_base + sl * S_COLS, d = pa + O_COL;
-            for (int ks = 0; ks < npv; ks++) {     // 16 keys per step: 8 packed TMEM columns of P, 16 rows (2048 B) of V
-                const int c = ks >> 1;
-                const uint32_t pcol = (c < nch_a ? 16 * c : 32 * nch_a + 16 * (c - nch_a)) + 8 * (ks & 1);
-                if (ks == 0) umma_f16_ts_init(d, pa + pcol, dv, id_pv);
-                else umma_f16_ts_acc(d, pa + pcol, dv + (uint64_t)ks * (2048 >> 4), id_pv);
-            }
-            umma_commit(o_full + 8 * sl);
-        }
-        }
-        __syncwarp();
-    } else if (warp < 4) {
-        // ------------------------------------------------------------------ last query row (T % 128 == 1, e.g. row 256 of a
-        // ViT-L/14 sequence) on the CUDA cores: warp 2 takes the even items of this CTA, warp 3 the odd ones
-        if (last_row) {
-            const float LOG2E = 1.4426950408889634f;
-            const uint32_t st = warp - 2, pb = smem_base + PB_OFF + st * PB_BYTES;
-            const uint32_t k_s = smem_base + st * (2 * KV_BYTES), v_s = k_s + KV_BYTES, qx = smem_base + QX_OFF + st * 2048;
-            int j = 0;
-            for (int i = st; i < n_local; i += 2, j++) {
-                const int item = p.desc ? nitems - 1 - ((int)blockIdx.x + i * (int)gridDim.x) : (int)blockIdx.x + i * (int)gridDim.x, head = item % p.H, seq = item / p.H;   // descending: the QKV GEMM's last rows are in L2
-                mbar_wait(kv_full + 8 * st, j & 1);
-                mbar_wait(qx_full + 8 * st, j & 1);
-                uint32_t qp[32];                            // the query row, packed 16-bit pairs (unpacked on the fly: registers are scarce)
+        return;
+    }
+
+    // ---------------------------------------------------------------------- consumers (fragment layout: wgmma.cuh)
+    const int wg = warp >> 2;
+    const int wrow0 = q0 + wg * 64 + (warp & 3) * 16;          // first query row of this warp
+    const int r0 = wrow0 + (lane >> 2), tc = 2 * (lane & 3);   // this thread: rows r0 and r0 + 8, columns 8j + tc + {0, 1}
+    const bool live = q0 + wg * 64 < p.T;                      // warpgroup-uniform: T = 257 leaves one of the last tile's groups idle
+    const float LOG2E = 1.4426950408889634f;
+    float o[32], m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    #pragma unroll
+    for (int i = 0; i < 32; i++) o[i] = 0.f;
+    mbar_wait(q_full, 0);
+    const uint64_t dq = wgmma_desc_sw128(smem_base + (uint32_t)wg * 64u * 128u);
+    for (int kb = 0; kb < nkb; kb++) {
+        const uint32_t s = kb & 1, k_s = smem_base + KV_OFF + s * (2 * KV_BYTES), v_s = k_s + KV_BYTES;
+        mbar_wait(kv_full + 8 * s, (kb >> 1) & 1);
+        if (live) {
+            float sc[64];
+            const uint64_t dk = wgmma_desc_sw128(k_s);
+            wgmma_fence();
+            #pragma unroll
+            for (int k = 0; k < DH / 16; k++) wgmma_ss_n128<BF>(sc, dq + 2 * k, dk + 2 * k, (uint32_t)k);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(sc);
+            const int key0 = kb * AK;
+            // masking is only needed in the last (ragged) key block and, for the causal text tower, on the diagonal block
+            if (key0 + AK > p.T || (p.causal && key0 + AK - 1 > wrow0)) {
                 #pragma unroll
-                for (int c = 0; c < 8; c++) {               // row 0 of the box: 16-byte chunk c is not displaced by the swizzle
-                    const uint4 a = lds128a(qx + (c << 4));
-                    qp[4 * c] = a.x; qp[4 * c + 1] = a.y; qp[4 * c + 2] = a.z; qp[4 * c + 3] = a.w;
-                }
-                float sc[9], m = -INFINITY;
-                #pragma unroll
-                for (int jj = 0; jj < 9; jj++) {             // key k = lane + 32 jj
-                    const int k = lane + 32 * jj;
-                    sc[jj] = -INFINITY;
-                    if (k < p.T) {
-                        const uint32_t row = k_s + (uint32_t)k * 128, sw = k & 7;      // key 256 sits right behind the 256-row box
-                        float acc = 0.f;
-                        #pragma unroll
-                        for (int c = 0; c < 8; c++) {
-                            const uint4 b = lds128a(row + ((c ^ sw) << 4));
-                            const uint32_t bw[4] = {b.x, b.y, b.z, b.w};
-                            #pragma unroll
-                            for (int i2 = 0; i2 < 4; i2++) {
-                                const float2 f = unpack2<BF>(bw[i2]), fq = unpack2<BF>(qp[4 * c + i2]);
-                                acc = fmaf(fq.x, f.x, acc); acc = fmaf(fq.y, f.y, acc);
-                            }
-                        }
-                        sc[jj] = acc;
-                        m = fmaxf(m, acc);
-                    }
-                }
-                #pragma unroll
-                for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-                const float mb = m * LOG2E;
-                float l = 0.f;
-                #pragma unroll
-                for (int jj = 0; jj < 9; jj++) {
-                    const int k = lane + 32 * jj;
-                    const float pv = (k < p.T) ? ex2f(sc[jj] * LOG2E - mb) : 0.f;
-                    l += pv;
-                    if (k < PB_BYTES / 4) sts32f(pb + 4 * k, pv);
-                }
-                #pragma unroll
-                for (int o = 16; o; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
-                __syncwarp();
-                // O[d] for d = 2*lane, 2*lane+1: 32-bit word `lane` of every V row
-                float o0 = 0.f, o1 = 0.f;
-                const uint32_t wsel = (lane & 3) * 4, csel = lane >> 2;
-                const int T4 = p.T & ~3;
-                for (int k = 0; k < T4; k += 4) {
-                    const float4 pk = lds128f(pb + 4 * k);
-                    const float pr[4] = {pk.x, pk.y, pk.z, pk.w};
+                for (int j = 0; j < AK / 8; j++) {
                     #pragma unroll
                     for (int e = 0; e < 4; e++) {
-                        const int kk = k + e;
-                        const float2 f = unpack2<BF>(lds32a(v_s + (uint32_t)kk * 128 + ((csel ^ (kk & 7)) << 4) + wsel));
-                        o0 = fmaf(pr[e], f.x, o0); o1 = fmaf(pr[e], f.y, o1);
+                        const int key = key0 + 8 * j + tc + (e & 1), row = r0 + 8 * (e >> 1);
+                        if (key >= p.T || (p.causal && key > row)) sc[4 * j + e] = -INFINITY;
                     }
                 }
-                for (int kk = T4; kk < p.T; kk++) {
-                    const float pr = lds32f(pb + 4 * kk);
-                    const float2 f = unpack2<BF>(lds32a(v_s + (uint32_t)kk * 128 + ((csel ^ (kk & 7)) << 4) + wsel));
-                    o0 = fmaf(pr, f.x, o0); o1 = fmaf(pr, f.y, o1);
-                }
-                const float inv = 1.0f / l;
-                uint32_t* orow = reinterpret_cast<uint32_t*>(p.out + ((size_t)seq * p.T + (p.T - 1)) * hid + head * DH);
-                orow[lane] = pack2<BF>(o0 * inv, o1 * inv);
-                __syncwarp();
-                if (lane == 0) { mbar_arrive(qx_empty + 8 * st); mbar_arrive(kv_empty + 8 * st); }
             }
-        }
-    } else {
-        // ------------------------------------------------------------------ softmax + epilogue (TMEM lane == query row).  Group 0
-        // (warps 4-11) owns TMEM buffer / Q slot 0 and the even tiles, group 1 (warps 12-19) buffer 1 and the odd tiles.  Inside
-        // a group TWO warps share each 32-row quarter: half 0 takes score chunks [0, nch_a) and output dims [0,32), half 1 the
-        // rest; they exchange the row max / row sum through shared memory.
-        const int grp = (warp - 4) >> 3, half = ((warp - 4) >> 2) & 1;
-        const int r = (warp & 3) * 32 + lane;
-        const uint32_t lane_addr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + grp * S_COLS;
-        const float LOG2E = 1.4426950408889634f;
-        const int c_lo = half ? nch_a : 0, c_hi = half ? nch : nch_a;
-        const uint32_t p_base = half ? 32 * nch_a : 0;                        // P columns of this half: p_base + 16 * (c - c_lo)
-        const uint32_t q_row = smem_base + Q_OFF + grp * Q_BYTES + r * 128, sw = r & 7;
-        const uint32_t xm_mine = smem_base + XM_OFF + ((grp * 2 + half) * 128 + r) * 4, xm_other = smem_base + XM_OFF + ((grp * 2 + (half ^ 1)) * 128 + r) * 4;
-        const uint32_t xl_mine = xm_mine + 2048, xl_other = xm_other + 2048;
-        const int bar_id = 1 + grp * 4 + (warp & 3);                            // named barrier of this row pair (64 threads)
-        for (int g = grp; g < G; g += 2) {
-            const uint32_t jp = (g >> 1) & 1;
-            const int i = g / ntile, qt = g - i * ntile;
-            const int item = p.desc ? nitems - 1 - ((int)blockIdx.x + i * (int)gridDim.x) : (int)blockIdx.x + i * (int)gridDim.x, head = item % p.H, seq = item / p.H;   // descending: the QKV GEMM's last rows are in L2
-            const uint32_t k_s = smem_base + (i & 1) * (2 * KV_BYTES), v_s = k_s + KV_BYTES;
-            const int qrow = qt * AQ + r;
-            const int klim = p.causal ? min(p.T, qrow + 1) : p.T;      // keys [0, klim) are visible to this row
-            const int klim_min = __shfl_sync(0xffffffffu, klim, 0);    // lane 0 holds the smallest row of the warp
-            const bool warp_live = (qt * AQ + (warp & 3) * 32) < p.T;  // warp-uniform: any valid query row in this warp?
-            mbar_wait(s_full + 8 * grp, jp);
-            tc_fence_after();
-            float l = 0.f, p_x = 0.f;
-            // ---- key 256: one dot product per row on the CUDA cores (Q row and K row 256 are in shared memory)
-            float s_x = -INFINITY;
-            if (warp_live && extra && 256 < klim) {
-                float acc = 0.f;
+            #pragma unroll
+            for (int h = 0; h < 2; h++) {
+                float mx = -INFINITY;
                 #pragma unroll
-                for (int c = 0; c < 8; c++) {
-                    const uint4 a = lds128a(q_row + ((c ^ sw) << 4)), b = lds128a(k_s + 32768 + (c << 4));
-                    const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
-                    #pragma unroll
-                    for (int i2 = 0; i2 < 4; i2++) {
-                        const float2 fa = unpack2<BF>(aw[i2]), fb = unpack2<BF>(bw[i2]);
-                        acc = fmaf(fa.x, fb.x, acc); acc = fmaf(fa.y, fb.y, acc);
-                    }
-                }
-                s_x = acc;
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(q_empty + 8 * grp);         // S is complete and the Q rows are consumed: slot free for tile g+2
-            if (warp_live) {
-                // ---- pass 1: row max over this half's chunks, then the pair's maximum
-                float m = s_x;
-                for (int c = c_lo; c < c_hi; c++) {
-                    uint32_t v[32];
-                    tmem_ld_32x32(lane_addr + c * 32, v);
-                    tmem_ld_wait();
-                    if (c * 32 + 32 <= klim_min) {                         // warp-uniform: every key of the chunk is visible
-                        #pragma unroll
-                        for (int i2 = 0; i2 < 32; i2++) m = fmaxf(m, __uint_as_float(v[i2]));
-                    } else {
-                        #pragma unroll
-                        for (int i2 = 0; i2 < 32; i2++)
-                            if (c * 32 + i2 < klim) m = fmaxf(m, __uint_as_float(v[i2]));
-                    }
-                }
-                sts32f(xm_mine, m);
-                pair_bar_sync(bar_id);
-                m = fmaxf(m, lds32f(xm_other));
-                if (m == -INFINITY) m = 0.f;                               // padded query rows past T
-                const float mb = m * LOG2E;
-                p_x = (s_x == -INFINITY) ? 0.f : ex2f(s_x * LOG2E - mb);
-                l = half ? 0.f : p_x;
-                // ---- pass 2: p = 2^(s*log2e - m*log2e); the packed 16-bit pairs overwrite S columns this warp has already
-                // consumed (chunk c -> p_base + 16 (c - c_lo) <= 32 c); the other half never reads or writes these columns
-                for (int c = c_lo; c < c_hi; c++) {
-                    uint32_t v[32], pk[16];
-                    tmem_ld_32x32(lane_addr + c * 32, v);
-                    tmem_ld_wait();
-                    if (c * 32 + 32 <= klim_min) {
-                        #pragma unroll
-                        for (int i2 = 0; i2 < 16; i2++) {
-                            const float p0 = ex2f(__uint_as_float(v[2 * i2]) * LOG2E - mb), p1 = ex2f(__uint_as_float(v[2 * i2 + 1]) * LOG2E - mb);
-                            l += p0 + p1;
-                            pk[i2] = pack2<BF>(p0, p1);
-                        }
-                    } else {
-                        #pragma unroll
-                        for (int i2 = 0; i2 < 16; i2++) {
-                            const int k0 = c * 32 + 2 * i2;
-                            const float p0 = (k0 < klim) ? ex2f(__uint_as_float(v[2 * i2]) * LOG2E - mb) : 0.f;
-                            const float p1 = (k0 + 1 < klim) ? ex2f(__uint_as_float(v[2 * i2 + 1]) * LOG2E - mb) : 0.f;
-                            l += p0 + p1;
-                            pk[i2] = pack2<BF>(p0, p1);
-                        }
-                    }
-                    tmem_st_32x16(lane_addr + p_base + (c - c_lo) * 16, pk);
-                }
-                tmem_st_wait();
-                sts32f(xl_mine, l);                                        // read by the partner after the o_full wait
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(p_full + 8 * grp);
-            // ---- O (+ p_256 * V[256]) / l -> global: this half's 32 output dims
-            mbar_wait(o_full + 8 * grp, jp);
-            tc_fence_after();
-            if (warp_live) {
-                const float inv = 1.0f / (l + lds32f(xl_other));
-                uint16_t* orow = p.out + ((size_t)seq * p.T + qrow) * hid + head * DH + half * 32;
-                uint32_t v[32];
-                tmem_ld_32x32(lane_addr + O_COL + half * 32, v);
-                tmem_ld_wait();
-                float o[32];
+                for (int j = 0; j < AK / 8; j++) mx = fmaxf(mx, fmaxf(sc[4 * j + 2 * h], sc[4 * j + 2 * h + 1]));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                // every row (padded rows past T included: zero queries) sees at least one unmasked key per visited block
+                const float m_new = fmaxf(m_run[h], mx);
+                const float alpha = ex2f((m_run[h] - m_new) * LOG2E), mb = m_new * LOG2E;
+                float rs = 0.f;
                 #pragma unroll
-                for (int i2 = 0; i2 < 32; i2++) o[i2] = __uint_as_float(v[i2]);
-                if (extra) {
-                    #pragma unroll
-                    for (int c = 0; c < 4; c++) {
-                        const uint4 b = lds128a(v_s + 32768 + ((half * 4 + c) << 4));     // V row 256, broadcast read
-                        const uint32_t bw[4] = {b.x, b.y, b.z, b.w};
-                        #pragma unroll
-                        for (int i2 = 0; i2 < 4; i2++) {
-                            const float2 fv = unpack2<BF>(bw[i2]);
-                            o[8 * c + 2 * i2] = fmaf(p_x, fv.x, o[8 * c + 2 * i2]);
-                            o[8 * c + 2 * i2 + 1] = fmaf(p_x, fv.y, o[8 * c + 2 * i2 + 1]);
-                        }
-                    }
+                for (int j = 0; j < AK / 8; j++) {
+                    const float p0 = ex2f(sc[4 * j + 2 * h] * LOG2E - mb), p1 = ex2f(sc[4 * j + 2 * h + 1] * LOG2E - mb);
+                    sc[4 * j + 2 * h] = p0; sc[4 * j + 2 * h + 1] = p1;
+                    rs += p0 + p1;
                 }
-                if (qrow < p.T - (last_row ? 1 : 0)) {
-                    #pragma unroll
-                    for (int i2 = 0; i2 < 4; i2++) {
-                        uint4 q4;
-                        q4.x = pack2<BF>(o[8 * i2 + 0] * inv, o[8 * i2 + 1] * inv);
-                        q4.y = pack2<BF>(o[8 * i2 + 2] * inv, o[8 * i2 + 3] * inv);
-                        q4.z = pack2<BF>(o[8 * i2 + 4] * inv, o[8 * i2 + 5] * inv);
-                        q4.w = pack2<BF>(o[8 * i2 + 6] * inv, o[8 * i2 + 7] * inv);
-                        *reinterpret_cast<uint4*>(orow + 8 * i2) = q4;
-                    }
-                }
+                l_run[h] = l_run[h] * alpha + rs;
+                m_run[h] = m_new;
+                #pragma unroll
+                for (int j = 0; j < DH / 8; j++) { o[4 * j + 2 * h] *= alpha; o[4 * j + 2 * h + 1] *= alpha; }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                mbar_arrive(s_free + 8 * grp);            // O has been read: TMEM buffer free for S of tile g+2
-                mbar_arrive(kv_empty + 8 * (i & 1));      // 8*ntile (+1) arrivals release the K/V stage of this (sequence, head)
+            // O += P.V: key step kk covers S n-tiles 2kk (A fragment registers 0, 1) and 2kk + 1 (registers 2, 3)
+            wgmma_fence();
+            #pragma unroll
+            for (int kk = 0; kk < AK / 16; kk++) {
+                const uint32_t a[4] = {pack2<BF>(sc[8 * kk], sc[8 * kk + 1]), pack2<BF>(sc[8 * kk + 2], sc[8 * kk + 3]),
+                                       pack2<BF>(sc[8 * kk + 4], sc[8 * kk + 5]), pack2<BF>(sc[8 * kk + 6], sc[8 * kk + 7])};
+                wgmma_rs_n64_bmn<BF>(o, a, wgmma_desc_sw128(v_s + (uint32_t)kk * 2048u), 1u);      // 16 keys = 2048 B of V
             }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, TMEM_COLS);
-}
-
-// =====================================================================================================================================
-// Long sequences (257 < T <= 640, non-causal: ViT-L/14@336 and ViT-B/16@384 have 577 tokens): the same tcgen05 data path with an
-// ONLINE softmax over key blocks of 192.  K and V of a (sequence, head) item stay in shared memory for all of its query tiles (one
-// stage: 2 x 80 KB), each softmax group owns 256 TMEM columns: S / P of the current key block in [0, 192), the running O in
-// [192, 256).  Per key block: S = Q.K_blk^T (SS UMMA) -> block row max, new running max m, alpha = 2^((m_old - m) log2e) -> P =
-// 2^((s - m) log2e) in place over S -> O *= alpha (tcgen05.ld / st of the group's 64 O columns, after the previous block's P.V has
-// completed) -> O += P.V_blk (TS UMMA).  The two groups work on different query tiles, so one group's S / P.V fill the other's
-// softmax time.  Replaces the warp-level mma.sync kernel (attention.cu) for these shapes.
-// =====================================================================================================================================
-constexpr int LKB = 192;                                   // keys per block
-constexpr int LKV_ROWS = 640;                              // K / V rows held per item (10 TMA boxes of 64 rows)
-constexpr uint32_t LK_OFF = 0, LV_OFF = LKV_ROWS * 128, LQ_OFF = 2 * LKV_ROWS * 128;           // 0, 81920, 163840
-constexpr uint32_t LBAR_OFF = LQ_OFF + 2 * Q_BYTES;        // 196608
-constexpr uint32_t LXM_OFF = LBAR_OFF + 256;               // [parity][group][half][128] block max, then [group][half][128] row sums
-constexpr uint32_t LONG_SMEM = LXM_OFF + 2 * 2048 + 2048 + 1024;
-constexpr int LONG_THREADS = 640;
-static_assert(LV_OFF % 1024 == 0 && LQ_OFF % 1024 == 0 && (LKB * 128) % 1024 == 0, "tile alignment");
-static_assert(LONG_SMEM <= 232448, "shared memory plan");
-
-struct LParams {
-    CUtensorMap tm_q, tm_kv64;
-    uint16_t* out;
-    int T, H, nseq, ntile, nblk;
-};
-
-template <bool BF>
-__global__ void __launch_bounds__(LONG_THREADS, 1) attention_tc_long_kernel(const __grid_constant__ LParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const uint32_t smem_base = smem_u32(smem);
-    const uint32_t bars = smem_base + LBAR_OFF;
-    const uint32_t kv_full = bars, kv_empty = bars + 8, q_full = bars + 16, q_empty = bars + 32, s_full = bars + 48, p_full = bars + 64,
-                   o_full = bars + 80, s_free = bars + 96;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + LBAR_OFF + 128);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int ntile = p.ntile, nblk = p.nblk;
-    if (threadIdx.x == 0) {
-        mbar_init(kv_full, 1); mbar_init(kv_empty, 8 * ntile);
-        for (int i = 0; i < 2; i++) {
-            mbar_init(q_full + 8 * i, 1);  mbar_init(q_empty + 8 * i, 8);
-            mbar_init(s_full + 8 * i, 1);  mbar_init(p_full + 8 * i, 8);
-            mbar_init(o_full + 8 * i, 1);  mbar_init(s_free + 8 * i, 8);
-        }
-        mbar_fence_init();
-        tma_prefetch_desc(&p.tm_q); tma_prefetch_desc(&p.tm_kv64);
-    }
-    if (warp == 2) tmem_alloc(smem_u32(tmem_slot), TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_trigger();
-    pdl_wait();
-
-    const int hid = p.H * DH, nitems = p.nseq * p.H;
-    const int n_local = (nitems - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-    const int G = n_local * ntile;                                         // query tiles of this CTA; tile g belongs to group g & 1
-    const int nbox = (p.T + 63) >> 6;
-
-    if (warp == 0) {
-        // ------------------------------------------------------------------ TMA producer (one thread): K / V of the item, then its Q tiles
-        if (elect_one()) {
-            int g = 0;
-            for (int i = 0; i < n_local; i++) {
-                const int item = (int)blockIdx.x + i * (int)gridDim.x, head = item % p.H, seq = item / p.H;
-                const int row0 = seq * p.T, c = head * DH;
-                mbar_wait(kv_empty, (i & 1) ^ 1);
-                mbar_arrive_expect_tx(kv_full, (uint32_t)(2 * nbox) * 8192u);
-                for (int b = 0; b < nbox; b++) {
-                    tma_load_3d(smem_base + LK_OFF + b * 8192, &p.tm_kv64, hid + c, b * 64, seq, kv_full);
-                    tma_load_3d(smem_base + LV_OFF + b * 8192, &p.tm_kv64, 2 * hid + c, b * 64, seq, kv_full);
-                }
-                for (int qt = 0; qt < ntile; qt++, g++) {
-                    const uint32_t sl = g & 1;
-                    mbar_wait(q_empty + 8 * sl, ((g >> 1) & 1) ^ 1);
-                    mbar_arrive_expect_tx(q_full + 8 * sl, Q_BYTES);
-                    tma_load_2d(smem_base + LQ_OFF + sl * Q_BYTES, &p.tm_q, c, row0 + qt * AQ, q_full + 8 * sl);
-                }
-            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(o);
         }
         __syncwarp();
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer (one thread).  Per group the chain is strictly
-        // S(b) -> softmax -> P.V(b) -> S(b+1).  The thread POLLS both groups and issues whichever next action is ready: with a single
-        // K / V stage one group can be waiting for the next item's K / V while the other still works on the current item, and a blocking
-        // wait on the first would starve the second (and the K / V stage would never be released).
-        if (elect_one()) {
-            const uint32_t id_pv = idesc_n(BF, DH, true);
-            const int steps_g[2] = {((G + 1) >> 1) * nblk, (G >> 1) * nblk};
-            int step[2] = {0, 0};
-            bool pv_next[2] = {false, false};
-            long long t_idle = clock64();
-            while (step[0] < steps_g[0] || step[1] < steps_g[1]) {
-                bool progressed = false;
-                #pragma unroll
-                for (int grp = 0; grp < 2; grp++) {
-                    const int n = step[grp];
-                    if (n >= steps_g[grp]) continue;
-                    const int k = n / nblk, b = n - k * nblk, g = grp + 2 * k, i = g / ntile;
-                    const int nk = min(LKB, p.T - b * LKB), nk16 = (nk + 15) & ~15;
-                    if (!pv_next[grp]) {
-                        const bool ready = (b == 0) ? (mbar_try_wait(kv_full, i & 1) && mbar_try_wait(q_full + 8 * grp, k & 1) &&
-                                                       mbar_try_wait(s_free + 8 * grp, (k & 1) ^ 1))      // K / V here, Q here, previous tile's O read
-                                                    : mbar_try_wait(o_full + 8 * grp, (n - 1) & 1);        // P.V of the previous block has read P
-                        if (!ready) continue;
-                        tc_fence_after();
-                        const uint32_t id_s = idesc_n(BF, nk16, false);
-                        const uint64_t dq = umma_desc_k128(smem_base + LQ_OFF + grp * Q_BYTES), dk = umma_desc_k128(smem_base + LK_OFF + b * (LKB * 128));
-                        const uint32_t d = tmem_base + grp * S_COLS;
-                        umma_f16_init(d, dq, dk, id_s);
-                        umma_f16_acc(d, dq + 2, dk + 2, id_s);
-                        umma_f16_acc(d, dq + 4, dk + 4, id_s);
-                        umma_f16_acc(d, dq + 6, dk + 6, id_s);
-                        umma_commit(s_full + 8 * grp);
-                        pv_next[grp] = true;
-                    } else {
-                        if (!mbar_try_wait(p_full + 8 * grp, n & 1)) continue;
-                        tc_fence_after();
-                        const int npv = nk16 >> 4, nch = (nk + 31) >> 5, nch_a = (nch + 1) >> 1;
-                        const uint64_t dv = umma_desc_mn128(smem_base + LV_OFF + b * (LKB * 128));
-                        const uint32_t pa = tmem_base + grp * S_COLS, d = pa + O_COL;
-                        for (int ks = 0; ks < npv; ks++) {
-                            const int c = ks >> 1;
-                            const uint32_t pcol = (c < nch_a ? 16 * c : 32 * nch_a + 16 * (c - nch_a)) + 8 * (ks & 1);
-                            if (ks == 0 && b == 0) umma_f16_ts_init(d, pa + pcol, dv, id_pv);
-                            else umma_f16_ts_acc(d, pa + pcol, dv + (uint64_t)ks * (2048 >> 4), id_pv);
-                        }
-                        umma_commit(o_full + 8 * grp);
-                        pv_next[grp] = false;
-                        step[grp] = n + 1;
-                    }
-                    progressed = true;
-                }
-                if (progressed) t_idle = clock64();
-                else if (clock64() - t_idle > CB_WAIT_TIMEOUT_CYCLES) __trap();
-            }
-        }
-        __syncwarp();
-    } else if (warp >= 4) {
-        // ------------------------------------------------------------------ softmax groups (TMEM lane == query row); two warps per 32-row
-        // quarter split the key chunks of a block and the output dims
-        const int grp = (warp - 4) >> 3, half = ((warp - 4) >> 2) & 1;
-        const int r = (warp & 3) * 32 + lane;
-        const uint32_t lane_addr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + grp * S_COLS;
-        const float LOG2E = 1.4426950408889634f;
-        const uint32_t xm_base = smem_base + LXM_OFF, xl_base = xm_base + 4096;
-        const uint32_t xl_mine = xl_base + ((grp * 2 + half) * 128 + r) * 4, xl_other = xl_base + ((grp * 2 + (half ^ 1)) * 128 + r) * 4;
-        const int bar_id = 1 + grp * 4 + (warp & 3);
-        int n = 0;                                                          // step counter of this group (tile-major, block-minor)
-        for (int g = grp; g < G; g += 2) {
-            const int i = g / ntile, qt = g - i * ntile;
-            const int item = (int)blockIdx.x + i * (int)gridDim.x, head = item % p.H, seq = item / p.H;
-            const int qrow = qt * AQ + r;
-            const bool warp_live = (qt * AQ + (warp & 3) * 32) < p.T;
-            float m_run = -INFINITY, l = 0.f;
-            for (int b = 0; b < nblk; b++, n++) {
-                const int klim = min(LKB, p.T - b * LKB);                   // valid keys of this block
-                const int nch = (klim + 31) >> 5, nch_a = (nch + 1) >> 1;
-                const int c_lo = half ? nch_a : 0, c_hi = half ? nch : nch_a;
-                const uint32_t p_base = half ? 32 * nch_a : 0;
-                const uint32_t xm_mine = xm_base + ((((b & 1) * 2 + grp) * 2 + half) * 128 + r) * 4, xm_other = xm_base + ((((b & 1) * 2 + grp) * 2 + (half ^ 1)) * 128 + r) * 4;
-                mbar_wait(s_full + 8 * grp, n & 1);
-                tc_fence_after();
-                if (b == nblk - 1) { __syncwarp(); if (lane == 0) mbar_arrive(q_empty + 8 * grp); }     // the last S of this tile has consumed Q
-                float alpha = 1.f;
-                if (warp_live) {
-                    float m = -INFINITY;
-                    for (int c = c_lo; c < c_hi; c++) {
-                        uint32_t v[32];
-                        tmem_ld_32x32(lane_addr + c * 32, v);
-                        tmem_ld_wait();
-                        if (c * 32 + 32 <= klim) {
-                            #pragma unroll
-                            for (int i2 = 0; i2 < 32; i2++) m = fmaxf(m, __uint_as_float(v[i2]));
-                        } else {
-                            #pragma unroll
-                            for (int i2 = 0; i2 < 32; i2++)
-                                if (c * 32 + i2 < klim) m = fmaxf(m, __uint_as_float(v[i2]));
-                        }
-                    }
-                    sts32f(xm_mine, m);
-                    pair_bar_sync(bar_id);
-                    m = fmaxf(fmaxf(m, lds32f(xm_other)), m_run);
-                    if (m == -INFINITY) m = 0.f;
-                    alpha = (m_run == -INFINITY) ? 0.f : ex2f((m_run - m) * LOG2E);
-                    m_run = m;
-                    const float mb = m * LOG2E;
-                    l *= alpha;
-                    for (int c = c_lo; c < c_hi; c++) {
-                        uint32_t v[32], pk[16];
-                        tmem_ld_32x32(lane_addr + c * 32, v);
-                        tmem_ld_wait();
-                        if (c * 32 + 32 <= klim) {
-                            #pragma unroll
-                            for (int i2 = 0; i2 < 16; i2++) {
-                                const float p0 = ex2f(__uint_as_float(v[2 * i2]) * LOG2E - mb), p1 = ex2f(__uint_as_float(v[2 * i2 + 1]) * LOG2E - mb);
-                                l += p0 + p1;
-                                pk[i2] = pack2<BF>(p0, p1);
-                            }
-                        } else {
-                            #pragma unroll
-                            for (int i2 = 0; i2 < 16; i2++) {
-                                const int k0 = c * 32 + 2 * i2;
-                                const float p0 = (k0 < klim) ? ex2f(__uint_as_float(v[2 * i2]) * LOG2E - mb) : 0.f;
-                                const float p1 = (k0 + 1 < klim) ? ex2f(__uint_as_float(v[2 * i2 + 1]) * LOG2E - mb) : 0.f;
-                                l += p0 + p1;
-                                pk[i2] = pack2<BF>(p0, p1);
-                            }
-                        }
-                        tmem_st_32x16(lane_addr + p_base + (c - c_lo) * 16, pk);
-                    }
-                    // a half that owns no chunk of a short last block still holds half of the P columns the MMA reads: none (npv covers
-                    // only ceil16(klim) keys, all inside chunks [0, nch)), so nothing to clear
-                    if (b > 0) {
-                        // running output *= alpha: this half's 32 output dims (P.V of the previous block completed before S of this
-                        // block was issued, so O is quiescent)
-                        uint32_t o[32];
-                        tmem_ld_32x32(lane_addr + O_COL + half * 32, o);
-                        tmem_ld_wait();
-                        #pragma unroll
-                        for (int i2 = 0; i2 < 32; i2++) o[i2] = __float_as_uint(__uint_as_float(o[i2]) * alpha);
-                        tmem_st_32x32(lane_addr + O_COL + half * 32, o);
-                    }
-                    tmem_st_wait();
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(p_full + 8 * grp);
-            }
-            // ---- epilogue of the tile: O / l -> global
-            mbar_wait(o_full + 8 * grp, (n - 1) & 1);
-            tc_fence_after();
-            if (warp_live) {
-                sts32f(xl_mine, l);
-                pair_bar_sync(bar_id);
-                const float inv = 1.0f / (l + lds32f(xl_other));
-                uint16_t* orow = p.out + ((size_t)seq * p.T + qrow) * hid + head * DH + half * 32;
-                uint32_t v[32];
-                tmem_ld_32x32(lane_addr + O_COL + half * 32, v);
-                tmem_ld_wait();
-                if (qrow < p.T) {
-                    #pragma unroll
-                    for (int i2 = 0; i2 < 4; i2++) {
-                        uint4 q4;
-                        q4.x = pack2<BF>(__uint_as_float(v[8 * i2 + 0]) * inv, __uint_as_float(v[8 * i2 + 1]) * inv);
-                        q4.y = pack2<BF>(__uint_as_float(v[8 * i2 + 2]) * inv, __uint_as_float(v[8 * i2 + 3]) * inv);
-                        q4.z = pack2<BF>(__uint_as_float(v[8 * i2 + 4]) * inv, __uint_as_float(v[8 * i2 + 5]) * inv);
-                        q4.w = pack2<BF>(__uint_as_float(v[8 * i2 + 6]) * inv, __uint_as_float(v[8 * i2 + 7]) * inv);
-                        *reinterpret_cast<uint4*>(orow + 8 * i2) = q4;
-                    }
-                }
-                pair_bar_sync(bar_id);                                      // the partner has read xl before the next tile rewrites it
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) { mbar_arrive(s_free + 8 * grp); mbar_arrive(kv_empty); }
+        if (lane == 0) mbar_arrive(kv_empty + 8 * s);
+    }
+    if (!live) return;
+    #pragma unroll
+    for (int h = 0; h < 2; h++) {
+        float l = l_run[h];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float inv = 1.0f / l;
+        const int row = r0 + 8 * h;
+        if (row < p.T) {
+            uint16_t* orow = p.out + ((size_t)seq * p.T + row) * hid + c;
+            #pragma unroll
+            for (int j = 0; j < DH / 8; j++)
+                *reinterpret_cast<uint32_t*>(orow + 8 * j + tc) = pack2<BF>(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, TMEM_COLS);
-}
-
-}  // namespace
-
-bool attention_tc_supported(int T) { return T >= 1 && T <= 257; }   // 256 keys on the tensor core + at most one folded in on the CUDA cores
-
-// query tiles handled by the tcgen05 kernel (all of them since v3: a ragged last tile only keeps its live warps busy)
-int attention_tc_tiles(int T) { return (T + AQ - 1) / AQ; }
-
-// long sequences: 257 < T <= 640, non-causal (the 640 rows of K and V an item may keep in shared memory)
-bool attention_tc_long_supported(int T, int causal) { return T > 257 && T <= LKV_ROWS && !causal; }
-
-cudaError_t attention_tc_init() {
-    cudaError_t e = cudaFuncSetAttribute(attention_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attention_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attention_tc_long_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LONG_SMEM);
-    if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(attention_tc_long_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LONG_SMEM);
 }
 
 typedef CUresult (*EncodeTiledFn3)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// [nseq][T][3*H*64] view of the fused QKV activations, box = 64 columns x 256 tokens x 1 sequence (128-byte swizzle, zero fill)
-static bool make_kv_map(CUtensorMap* out, const void* qkv16, int nseq, int T, int H, unsigned box_rows = 256) {
+// [nseq][T][3*H*64] view of the fused QKV activations, box = 64 columns x 128 tokens x 1 sequence (128-byte swizzle, zero fill)
+bool make_qkv_map(CUtensorMap* out, const void* qkv16, int nseq, int T, int H) {
     static EncodeTiledFn3 enc = nullptr;
     if (!enc) {
         void* f = nullptr;
@@ -766,48 +193,30 @@ static bool make_kv_map(CUtensorMap* out, const void* qkv16, int nseq, int T, in
     const cuuint64_t cols = (cuuint64_t)3 * H * DH;
     const cuuint64_t dims[3] = {cols, (cuuint64_t)T, (cuuint64_t)nseq};
     const cuuint64_t strides[2] = {cols * 2, cols * 2 * (cuuint64_t)T};
-    const cuuint32_t box[3] = {64, box_rows, 1}, estr[3] = {1, 1, 1};
+    const cuuint32_t box[3] = {64, (cuuint32_t)AK, 1}, estr[3] = {1, 1, 1};
     return enc(out, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<void*>(qkv16), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-cudaError_t launch_attention_tc(const TmaMap* map_q, const void* qkv16, const TmaMap* map_kv16, void* out16, int nseq, int T,
-                                int H, int causal, int bf16, int num_sms, cudaStream_t st) {
+}  // namespace
+
+cudaError_t attention_tc_init() {
+    cudaError_t e = cudaFuncSetAttribute(attention_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(attention_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM);
+}
+
+cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T, int H, int causal, int bf16, cudaStream_t st) {
     if (nseq <= 0) return cudaSuccess;
     AParams p;
-    memcpy(&p.tm_q, map_q, sizeof(CUtensorMap));
-    if (!make_kv_map(&p.tm_kv256, qkv16, nseq, T, H)) return cudaErrorInvalidValue;
-    memcpy(&p.tm_kv16, map_kv16, sizeof(CUtensorMap));
-    p.out = (uint16_t*)out16; p.T = T; p.H = H; p.nseq = nseq; p.causal = causal;
-    p.last_row = (T > 1 && T % AQ == 1) ? 1 : 0;      // e.g. 257 = 2 tensor-core tiles + one row on the CUDA cores
-    p.ntile = (T - p.last_row + AQ - 1) / AQ;
-    p.nk16 = ((T + 15) / 16) * 16;
-    static const int desc = (getenv("CLIP_B200_ORDER") && !strcmp(getenv("CLIP_B200_ORDER"), "attn_desc")) ? 1 : 0;      // A/B switch for measurements
-    p.desc = desc;
-    const int total = nseq * H;
-    const int grid = total < num_sms ? total : num_sms;      // one persistent CTA per SM, items = (sequence, head)
+    if (!make_qkv_map(&p.tm_qkv, qkv16, nseq, T, H)) return cudaErrorInvalidValue;
+    p.out = (uint16_t*)out16; p.T = T; p.H = H; p.causal = causal;
+    p.ntile = (T + AQ - 1) / AQ;
+    const long long grid = (long long)nseq * H * p.ntile;
+    if (grid > 0x7fffffffll) return cudaErrorInvalidValue;
     cudaError_t e = bf16 ? launch_pdl(attention_tc_kernel<true>, (unsigned)grid, (unsigned)ATT_THREADS, ATT_SMEM, st, 1, p)
                          : launch_pdl(attention_tc_kernel<false>, (unsigned)grid, (unsigned)ATT_THREADS, ATT_SMEM, st, 1, p);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 
-}  // namespace cb
-
-namespace cb {
-cudaError_t launch_attention_tc_long(const TmaMap* map_q, const void* qkv16, void* out16, int nseq, int T, int H, int bf16, int num_sms,
-                                     cudaStream_t st) {
-    if (nseq <= 0) return cudaSuccess;
-    if (!attention_tc_long_supported(T, 0)) return cudaErrorInvalidValue;
-    LParams p;
-    memcpy(&p.tm_q, map_q, sizeof(CUtensorMap));
-    if (!make_kv_map(&p.tm_kv64, qkv16, nseq, T, H, 64)) return cudaErrorInvalidValue;
-    p.out = (uint16_t*)out16; p.T = T; p.H = H; p.nseq = nseq;
-    p.ntile = (T + AQ - 1) / AQ;
-    p.nblk = (T + LKB - 1) / LKB;
-    const int total = nseq * H;
-    const int grid = total < num_sms ? total : num_sms;
-    cudaError_t e = bf16 ? launch_pdl(attention_tc_long_kernel<true>, (unsigned)grid, (unsigned)LONG_THREADS, LONG_SMEM, st, 1, p)
-                         : launch_pdl(attention_tc_long_kernel<false>, (unsigned)grid, (unsigned)LONG_THREADS, LONG_SMEM, st, 1, p);
-    return e != cudaSuccess ? e : cudaGetLastError();
-}
 }  // namespace cb

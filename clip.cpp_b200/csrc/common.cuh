@@ -1,8 +1,7 @@
-// common.cuh -- sm_100a PTX building blocks shared by the kernels of libclip_b200.so.
+// common.cuh -- sm_90a PTX building blocks shared by the kernels of libclip_b200.so.
 //
-// Everything here is hand-written inline PTX for Blackwell (tcgen05 / TMEM / TMA / mbarrier); there is
-// no CUTLASS/CuTe dependency.  Descriptor bit layouts follow the PTX ISA "tcgen05" matrix/instruction
-// descriptor tables (cross-checked against the field tables in the vendored CuTe headers).
+// Everything here is hand-written inline PTX for Hopper (TMA / mbarrier / programmatic dependent launch; the warpgroup MMA wrappers are
+// in wgmma.cuh); there is no CUTLASS/CuTe dependency.
 #pragma once
 #include <cstdlib>
 
@@ -24,7 +23,7 @@ enum Epi : int {
     EPI_STORE16 = 0,      // out16 = (acc + bias) [* scale for the first scale_cols features]
     EPI_GELU16 = 1,       // out16 = gelu_tanh(acc + bias)          (clip.use_gelu = true)
     EPI_QGELU16 = 2,      // out16 = quick_gelu(acc + bias)         (clip.use_gelu = false)
-    EPI_REDADD32 = 3,     // x32 += acc + bias  (fp32 residual stream): staged in shared memory, added by a TMA tensor REDUCE
+    EPI_REDADD32 = 3,     // x32 += acc + bias  (fp32 residual stream; every element has exactly one owner thread)
     EPI_STORE32 = 4,      // out32 = acc + bias
 };
 
@@ -34,13 +33,6 @@ enum Epi : int {
 // shared-memory address helpers
 // --------------------------------------------------------------------------------------------------
 CB_DEVINL uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-
-// exactly one lane of a converged warp returns true (elect.sync: ptxas treats the guarded code as single-threaded)
-CB_DEVINL bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
 
 // --------------------------------------------------------------------------------------------------
 // mbarrier
@@ -91,38 +83,14 @@ CB_DEVINL void mbar_wait(uint32_t bar, uint32_t parity) {
 
 // --------------------------------------------------------------------------------------------------
 // programmatic dependent launch: the hot kernels of a tower are launched with programmaticStreamSerialization, so the next
-// kernel's CTAs are placed (and run their barrier / TMEM / descriptor prologue) while the previous grid drains.  pdl_wait()
+// kernel's CTAs are placed (and run their barrier / descriptor prologue) while the previous grid drains.  pdl_wait()
 // blocks until the previous grid has completed and its writes are visible: NO global memory may be touched before it.
 // --------------------------------------------------------------------------------------------------
 CB_DEVINL void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 CB_DEVINL void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // --------------------------------------------------------------------------------------------------
-// CTA pairs (cluster of 2): rank, remote (cluster-scope) barrier arrive, cluster barrier
-// --------------------------------------------------------------------------------------------------
-CB_DEVINL uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-CB_DEVINL uint32_t mapa_rank0(uint32_t addr) {   // shared::cluster address of `addr` inside CTA rank 0 of this cluster
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, 0;" : "=r"(r) : "r"(addr));
-    return r;
-}
-CB_DEVINL void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-CB_DEVINL void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// --------------------------------------------------------------------------------------------------
-// proxies / fences
-// --------------------------------------------------------------------------------------------------
-// generic-proxy smem writes (st.shared) -> visible to the async proxy (UMMA operand reads, TMA stores)
-CB_DEVINL void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-CB_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-CB_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// --------------------------------------------------------------------------------------------------
-// TMA: tiled tensor load (UTMALDG) and 1-D bulk copy (UBLKCP), completion on an mbarrier
+// TMA: tiled tensor load and 1-D bulk copy, completion on an mbarrier
 // --------------------------------------------------------------------------------------------------
 CB_DEVINL void tma_prefetch_desc(const void* tmap) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
@@ -133,177 +101,12 @@ CB_DEVINL void tma_load_2d(uint32_t dst_smem, const void* tmap, int c0, int c1, 
         "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1)
         : "memory");
 }
-// CTA-pair variant: the data lands in THIS CTA's shared memory, the transaction bytes are credited to the mbarrier of the
-// pair's leader CTA (bar_cluster = mapa_rank0(local barrier address))
-CB_DEVINL void tma_load_2d_2sm(uint32_t dst_smem, const void* tmap, int c0, int c1, uint32_t bar_cluster) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst_smem),
-        "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar_cluster), "r"(c0), "r"(c1)
-        : "memory");
-}
 CB_DEVINL void bulk_load_1d(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
                  "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar)
                  : "memory");
 }
 
-// TMA tensor STORE (shared -> global) with bulk-group completion: the issuing thread commits a group and later waits until the
-// group has finished READING shared memory before the staging buffer is reused.  Rows / columns outside the tensor map are clipped.
-CB_DEVINL void tma_store_2d(const void* tmap, uint32_t src_smem, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(src_smem),
-                 "r"(c0), "r"(c1)
-                 : "memory");
-}
-// TMA tensor REDUCE (shared -> global, element-wise add performed by the memory system): out[box] += smem[box].  Each output element is
-// owned by exactly one CTA, so the result is deterministic.
-CB_DEVINL void tma_reduce_add_2d(const void* tmap, uint32_t src_smem, int c0, int c1) {
-    asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(tmap)),
-                 "r"(src_smem), "r"(c0), "r"(c1)
-                 : "memory");
-}
-CB_DEVINL void sts32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
-CB_DEVINL void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-CB_DEVINL void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-CB_DEVINL void sts16(uint32_t a, uint16_t v) { asm volatile("st.shared.u16 [%0], %1;" ::"r"(a), "h"(v) : "memory"); }
-
-// --------------------------------------------------------------------------------------------------
-// TMEM allocation (one warp, .sync.aligned) and loads
-// --------------------------------------------------------------------------------------------------
-CB_DEVINL void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-CB_DEVINL void tmem_alloc_2sm(uint32_t dst_smem, uint32_t ncols) {   // executed by the same warp id in BOTH CTAs of the pair
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-CB_DEVINL void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-CB_DEVINL void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives lane (base_lane + i)
-CB_DEVINL void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns, registers -> TMEM (thread i of the warp writes lane base_lane + i)
-CB_DEVINL void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-        "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-        "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-        "r"(r[31])
-        : "memory");
-}
-CB_DEVINL void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-CB_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// --------------------------------------------------------------------------------------------------
-// tcgen05.mma (kind::f16, operands in shared memory, fp32 accumulator in TMEM), single-CTA group
-// --------------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a K-major tile whose rows are 128 bytes (64 x 16-bit) with the
-// 128-byte swizzle: 8-row groups are 1024 B apart (SBO), LBO is unused for swizzled K-major (set 1),
-// descriptor version 1 (sm_100), layout type 2 = SWIZZLE_128B.  Tile base must be 1024-B aligned; the
-// K offset of a 16-element MMA step is applied by advancing the start address by 32 B.
-CB_DEVINL uint64_t umma_desc_k128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);   // start address  [0,14)
-    d |= (uint64_t)1 << 16;                         // LBO (16-B units) [16,30)
-    d |= (uint64_t)(1024 >> 4) << 32;               // SBO (16-B units) [32,46)
-    d |= (uint64_t)1 << 46;                         // version = 1      [46,48)
-    d |= (uint64_t)2 << 61;                         // SWIZZLE_128B     [61,64)
-    return d;
-}
-// Instruction descriptor: D = F32, A/B format (0 = F16, 1 = BF16), both K-major, N>>3 at [17,23), M>>4 at [24,29)
-constexpr uint32_t umma_idesc(bool bf16, int M, int N) {
-    return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) | ((uint32_t)(N >> 3) << 17) |
-           ((uint32_t)(M >> 4) << 24);
-}
-// enable-input-d predicate is a compile-time constant in each variant (folds to PT / !PT, no per-issue setp)
-CB_DEVINL void umma_f16_acc(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.eq.u32 p, 0, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc)
-        : "memory");
-}
-CB_DEVINL void umma_f16_init(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc) {   // D = A.B (overwrite)
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.u32 p, 0, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc)
-        : "memory");
-}
-// "TS" form: A operand from tensor memory (M lanes x K/2 32-bit columns, two 16-bit k-elements per column), B from smem
-CB_DEVINL void umma_f16_ts_acc(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.eq.u32 p, 0, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc)
-        : "memory");
-}
-CB_DEVINL void umma_f16_ts_init(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.u32 p, 0, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc)
-        : "memory");
-}
-// CTA-pair (cta_group::2) forms: ONE instruction from the leader drives both SMs' tensor cores (M = 256: each CTA supplies its
-// 128 A rows from its own TMEM and half of the B rows from its own shared memory); commits are multicast to both CTAs.
-CB_DEVINL void umma_f16_ts_2sm_acc(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.eq.u32 p, 0, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc)
-        : "memory");
-}
-CB_DEVINL void umma_f16_ts_2sm_init(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.u32 p, 0, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc)
-        : "memory");
-}
-// runtime accumulate flag (the first k-block of a tile overwrites D): one form for the unrolled issue loop of the pair kernel
-CB_DEVINL void umma_f16_ts_2sm(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.u32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-CB_DEVINL void umma_commit_2sm(uint32_t bar) {   // arrives on the barrier at this offset in BOTH CTAs of the pair
-    const uint16_t mask = 3;
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask)
-                 : "memory");
-}
-// commit all previously issued tcgen05 async ops of this thread; arrives (count 1) on the mbarrier when they finish.
-// Implies tcgen05.fence::before_thread_sync.
-CB_DEVINL void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 
 // --------------------------------------------------------------------------------------------------
 // packed 16-bit x2 arithmetic on raw b32 registers, selected by operand type (fp16 / bf16)

@@ -1,4 +1,4 @@
-// gemm.h -- host interface of the fused block-dequant tcgen05 GEMM (gemm_dq.cu).
+// gemm.h -- host interface of the fused block-dequant wgmma GEMM (gemm_dq.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -15,33 +15,19 @@ struct alignas(64) TmaMap {
 bool make_tma_2d_16bit(TmaMap* out, const void* gptr, uint64_t rows, uint64_t cols, uint64_t row_stride_elems,
                        uint32_t box_rows);
 
-// Plain (un-swizzled) tiled map over a row-major 16-bit matrix, box = [box_rows, box_cols]: the GEMM epilogue's TMA STORE target
-// (box 32 tokens x 32 features = 32 rows of 64 bytes).
-bool make_tma_2d_16bit_plain(TmaMap* out, const void* gptr, uint64_t rows, uint64_t cols, uint64_t row_stride_elems, uint32_t box_rows,
-                             uint32_t box_cols);
-// the same over an fp32 matrix: target of the EPI_REDADD32 epilogue's TMA reduce-add (the residual stream)
-bool make_tma_2d_f32_plain(TmaMap* out, const void* gptr, uint64_t rows, uint64_t cols, uint64_t row_stride_elems, uint32_t box_rows,
-                           uint32_t box_cols);
-constexpr int GEMM_OUT_BOX = 32;
-
-constexpr int GEMM_BM = 128;   // features per tile (UMMA M / TMEM lanes)
-constexpr int GEMM_BN = 192;   // tokens per tile   (UMMA N / TMEM columns; 2 x 192 accumulator columns + 128 A-operand columns = 512)
+constexpr int GEMM_BM = 128;   // features per tile (two wgmma M = 64 warpgroups)
+constexpr int GEMM_BN = 192;   // tokens per tile   (wgmma N; 96 fp32 accumulator registers per thread)
 constexpr int GEMM_BK = 64;
 
 struct GemmArgs {
     // Y[M tokens, N features] (+)= X[M, K] . W[N, K]^T (+ bias[N]),  computed as D[feature, token] tiles
     const TmaMap* x_map = nullptr;   // activations X, 16-bit, box rows = GEMM_BN
     const TmaMap* w_map = nullptr;   // QT_F16 only: weights W [N, K] fp16, box rows = GEMM_BM
-    const TmaMap* x_half_map = nullptr;   // optional: X with box rows = GEMM_BN/2 -> enables the CTA-pair (cta_group::2) kernel when N % 256 == 0
     const uint8_t* w_packed = nullptr;   // quantized types: re-tiled blocks (wpack.h)
     int qtype = 1;                   // cb::QType of W
     bool operand_bf16 = false;       // X (and the unpacked W) are bf16 instead of fp16; must be false for QT_F16
     const float* bias = nullptr;     // [N] or null
     void* out = nullptr;             // EPI_*16: 16-bit [M, ldo]; EPI_*32: fp32 [M, ldo]
-    const TmaMap* out_map = nullptr; // 16-bit epilogues (optional) and EPI_REDADD32 (required unless the direct path is wanted) of quantized
-                                     // GEMMs: plain map of `out` (16-bit, resp. fp32; box GEMM_OUT_BOX x GEMM_OUT_BOX): the
-                                     // epilogue stages 32 x 32 blocks in shared memory and stores them with TMA instead of 2-byte STGs.
-                                     // NOTE rows of the last token tile beyond M are written too when the map has more than M rows.
     int M = 0, N = 0, K = 0, ldo = 0;
     int epi = 0;                     // cb::Epi
     int out_bf16 = 0;                // 16-bit stores: bf16 (1) or fp16 (0)

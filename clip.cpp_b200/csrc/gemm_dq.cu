@@ -1,42 +1,29 @@
-// gemm_dq.cu -- K1: fused block-dequant GEMM on tcgen05 tensor cores (sm_100a).
+// gemm_dq.cu -- K1: fused block-dequant GEMM on Hopper warpgroup MMA (sm_90a wgmma).
 //
 // Replaces ggml_compute_forward_mul_mat + vec_dot_q*_q8_* (reference: ggml/src/ggml.c:11223-11437,
 // 2333-3624) for every weight GEMM of the ViT / text transformer (clip.cpp:1080-1137, 1360-1417).
 //
 //   Y[token, feature] = sum_k X[token, k] * W[feature, k]  (+ bias, + epilogue)
 //
-// computed "swap-AB": the WEIGHT tile is the UMMA A operand (M = 128 features = TMEM lanes), the ACTIVATION tile is
-// the B operand (N = 192 tokens = TMEM columns).  Quantized weights never touch shared memory in unpacked form: the
-// unpack warps write the dequantised fp16/bf16 tile straight into TENSOR MEMORY (tcgen05.st) and the MMA takes its A
-// operand from TMEM (tcgen05.mma "TS" form).  Shared memory then carries only the activation tile (TMA in, UMMA out) and
-// the packed 4-8 bit blocks -- it was the binding resource of the earlier smem->smem version (see DESIGN.md section 6).
-//
-// Warp roles (persistent CTA, 1 per SM, 512 threads; 256 for unquantized f16 weights).  For N % 256 == 0 (every layer GEMM) a CTA PAIR
-// (cluster of 2) owns a [256 features x 192 tokens] tile and the leader issues cta_group::2 UMMAs (M = 256):
-//   warp 0      X producer: activation box (UTMALDG, 128B swizzle); pair form: each CTA loads its HALF of the token tile (96 rows,
-//               12 KB per k-block) into a 12-deep ring, bytes credited to the leader's barrier                         -> x_full[s]
-//   warp 3      Q producer: ONE 1-D bulk copy (UBLKCP) per k-block of the packed 32-weight blocks + scales of
-//               the [128 x 64] weight tile (wpack.h); runs up to 8 k-blocks ahead                                      -> q_full[s]
-//   warps 8-15  unpack, 2 groups x 4 warps (one warp per TMEM lane quarter); group g owns k-blocks i = g (mod 2):
-//               thread = one weight row x 64 k: ld.shared packed q4_0/q4_1/q5_0/q5_1/q8_0 -> 32 registers of 16-bit
-//               pairs (one LOP3 + one sub + one mul per pair for q4_0) -> tcgen05.st.32x32b.x32 into A stage (i mod 4)  -> a_full[j]
-//   warp 1      ONE elected thread runs the whole issue loop: tcgen05.mma (N192 K16, kind::f16, A from TMEM, B from smem), fp32
-//               accumulators in TMEM; tcgen05.commit releases the X / A stages and signals the epilogue.  This thread is the
-//               kernel's critical path (it shares its scheduler with an epilogue warp and two unpack warps): its loop is unrolled
-//               over lcm(X ring, A ring) k-blocks so stage indices and barrier addresses are compile-time constants
-//   warps 4-7   epilogue: tcgen05.ld 32x32b.x32 -> bias / scale / GELU -> 2-byte (or fp32) st.shared into a [32 tokens x 32 features]
-//               block -> ONE TMA tensor store per block, or a TMA tensor REDUCE-ADD into the fp32 residual stream (EPI_REDADD32);
-//               double-buffered accumulators (2 x 192 TMEM columns) overlap it with the next tile's MMAs
-//   warp 2      TMEM alloc / dealloc   (TMEM map: acc0 [0,192) acc1 [192,384) A stages [384 + 32 j), j < 4)
-//
-// Unquantized (f16 / f32-rounded-to-f16) weights use the plain SS form: warp 0 TMA-loads X and W tiles, direct global stores.
-// gemm_dq2_kernel below is the "wide" form ([256 x 384] super-tiles, both accumulators live): measured slower, opt-in only.
-// Algorithmic bytes per launch (DESIGN.md section 5): packed W once + X once + Y once; FLOPs = 2*M*N*K.
+// computed "swap-AB": the WEIGHT tile is the wgmma A operand (M = 128 features, 64 per consumer warpgroup), the ACTIVATION tile is
+// the B operand (N = 192 tokens); fp32 accumulators live in registers (96 per thread).  Persistent CTA, one per SM, 384 threads; the
+// producer warpgroup hands its registers to the consumers (setmaxnreg 40 / 232):
+//   warp 8      producer, one thread: per k-block ONE 1-D bulk copy of the packed 32-weight blocks + scales of the [128 x 64] weight
+//               tile (wpack.h) into the Q ring, and a TMA box of the activation tile [192 tokens x 64 k] (128-B swizzle) into the X
+//               ring; unquantized f16 weights come as a second TMA box [128 features x 64 k] in the same X stage instead
+//   warps 0-7   two consumer warpgroups; group g owns features [64 g, 64 g + 64) of the tile.  Quantized weights never exist unpacked in
+//               shared memory: every lane dequantises exactly the 16-bit pairs of its own wgmma A fragments (2 rows x 16 k per k-block)
+//               from the packed chunk into registers, and the group issues 4 register-A wgmma m64n192k16 per k-block (B = activation
+//               tile from shared memory), keeping one k-block of MMAs in flight while it unpacks the next.  f16 weights: both operands
+//               from shared memory.  Epilogue straight from the accumulator registers: bias / scale / GELU and 16-bit or fp32 stores,
+//               or x += acc + bias into the fp32 residual stream (every element has exactly one owner thread: deterministic).
+// Bytes per launch (DESIGN.md section 5): packed W once per token tile, X once per feature tile, Y once; FLOPs = 2*M*N*K.
 #include <cuda.h>
 #include <stdlib.h>
 
 #include "common.cuh"
 #include "gemm.h"
+#include "wgmma.cuh"
 #include "wpack.h"
 
 namespace cb {
@@ -46,59 +33,36 @@ namespace {
 constexpr int BM = GEMM_BM, BN = GEMM_BN, BK = GEMM_BK;
 constexpr int X_STAGE = BN * BK * 2;   // 24576 B
 constexpr int W_STAGE = BM * BK * 2;   // 16384 B (f16 path only)
-constexpr int N_GROUPS = 2;            // unpack groups (4 warps each)
-constexpr int NA = 4;                  // A-operand stages in TMEM (32 columns each)
-constexpr int N_EPI_WARPS = 4;
-constexpr uint32_t TMEM_COLS = 512;
-constexpr uint32_t A_COL0 = 2 * BN;    // first TMEM column of the A stages
-static_assert(2 * BN + NA * 32 <= 512, "TMEM budget");
-static_assert(X_STAGE % 1024 == 0, "swizzled stage alignment");
+constexpr int THREADS = 384;           // 2 consumer warpgroups + 1 producer warpgroup (one thread of it issues the copies)
+static_assert(X_STAGE % 1024 == 0 && W_STAGE % 1024 == 0, "swizzled stage alignment");
 
 __host__ __device__ constexpr uint32_t chunk_bytes(int qt) {
     return qt == 2 ? 4608u : qt == 3 ? 5120u : qt == 6 ? 5632u : qt == 7 ? 6144u : qt == 8 ? 8704u : 0u;
 }
-// shared-memory plan per weight type and kernel form (all rings fit the 227 KB carve-out).  In the CTA-pair form each CTA stages only
-// ITS half of the token tile (96 rows = 12 KB per k-block), so the same space holds a ring twice as deep: 12 k-blocks of TMA latency
-// cover instead of 6.
-template <int QT, bool PAIR = false>
+// shared-memory plan per weight type (fits the 227 KB carve-out): X ring, packed-weight ring, barriers
+template <int QT>
 struct Cfg {
     static constexpr bool DQ = (QT != QT_F16);
     static constexpr uint32_t CHUNK = chunk_bytes(QT);
-    static constexpr int SX = DQ ? (PAIR ? (QT == QT_Q8_0 ? 10 : 12) : (QT == QT_Q8_0 ? 5 : 6)) : 5;   // X ring (f16: X + W per stage)
+    static constexpr int SX = DQ ? 6 : 5;                              // X ring (f16: X + W per stage)
     static constexpr int SQ = DQ ? 8 : 0;                              // packed-weight ring
-    static constexpr uint32_t XS = DQ ? (uint32_t)(PAIR ? X_STAGE / 2 : X_STAGE) : (uint32_t)(X_STAGE + W_STAGE);
+    static constexpr uint32_t XS = DQ ? (uint32_t)X_STAGE : (uint32_t)(X_STAGE + W_STAGE);
     static constexpr uint32_t Q_OFF = SX * XS;
-    static constexpr uint32_t OUT_OFF = Q_OFF + SQ * CHUNK;            // epilogue staging: 4 warps x 2 buffers x [32 tokens x 32 features] (16-bit or fp32)
-    static constexpr uint32_t OUT_BYTES = DQ ? 4 * 2 * 4096 : 0;
-    static constexpr uint32_t BAR_OFF = (OUT_OFF + OUT_BYTES + 127) / 128 * 128;
-    static constexpr uint32_t SMEM = BAR_OFF + 512 /*barriers*/ + 1024 /*align slack*/;
+    static constexpr uint32_t BAR_OFF = (Q_OFF + SQ * CHUNK + 127) / 128 * 128;
+    static constexpr uint32_t SMEM = BAR_OFF + 256 /*barriers*/ + 1024 /*align slack*/;
     static_assert(SMEM <= 232448, "shared memory plan exceeds 227 KB");
-    static_assert(XS % 1024 == 0, "stage alignment");
+    static_assert(16 * SX + 16 * SQ <= 256, "barrier area");
 };
-
-// Probe switches (KParams::dbg) exist only in experiment builds (make VARIANT=-DCB_GEMM_PROBE ...): the production kernels do not
-// carry their loads and branches in the issue loops.
-#ifdef CB_GEMM_PROBE
-#define CB_DBG(p, bit) ((p).dbg & (bit))
-#else
-#define CB_DBG(p, bit) 0
-#endif
 
 struct KParams {
     CUtensorMap tm_x;
     CUtensorMap tm_w;
-    CUtensorMap tm_xh;    // CTA-pair kernels: activation box of BN/2 = 96 tokens (each CTA of the pair loads half the B operand)
-    CUtensorMap tm_out;   // 16-bit epilogues through shared memory + TMA store (tma_out != 0)
-    int tma_out;
     const uint8_t* w_packed;
     const float* bias;
     void* out;
     int M, N, K, ldo;
     int epi, scale_cols;
     float scale;
-    int dbg;   // experiment switches (env CLIP_B200_GEMM_DBG, tools only; results are WRONG with any of them): 1 skip unpack math + tcgen05.st,
-               // 2 skip X loads, 4 skip Q loads, 8 skip epilogue, 16 epilogue reads TMEM but stores nothing, 32 unpack does not wait for a
-               // free A stage, 64 MMA does not wait for the A stage
 };
 
 // explicit .shared accesses on 32-bit shared-window addresses (generic ld/st would cost an address-space check)
@@ -134,52 +98,43 @@ CB_DEVINL uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
     return r;
 }
 
-// Unpack the 32-weight ggml block t (= half*128 + row) of a packed [128 x 64] tile (wpack.h) into 16 registers holding
-// the 32 weights as adjacent 16-bit pairs in k order (out[c] = {w[2c], w[2c+1]}) -- exactly one TMEM row segment of the
-// UMMA A operand.  Arithmetic matches dequantize_row_q* (ggml/src/ggml.c:1496-1606): (q - zero) * d  or  q * d + m,
-// with the integer part exact (magic-number int->float) and ONE rounding of the product to the operand type.
+// Unpack four 16-bit weight pairs of the 32-weight ggml block b (= half*128 + row) of a packed [128 x 64] tile (wpack.h): v[j] holds
+// block elements 8j + 2t and 8j + 2t + 1 (t = lane % 4), i.e. what one lane contributes to the wgmma A fragments of the block's two
+// 16-wide k steps.  Arithmetic matches dequantize_row_q* (ggml/src/ggml.c:1496-1606): (q - zero) * d  or  q * d + m, with the integer
+// part exact (magic-number int->float) and ONE rounding of the product to the operand type.
 template <int QT, bool BF>
-CB_DEVINL void unpack_block(uint32_t q, int t, uint32_t* __restrict__ out) {
+CB_DEVINL void unpack_pairs(uint32_t q, int b, int t, uint32_t (&v)[4]) {
     using P = P2<BF>;
     if constexpr (QT == QT_Q8_0) {
-        const uint4 qa = lds128(q + 16 * t), qb = lds128(q + 4096 + 16 * t);
-        const uint32_t d2 = P::splat_from_f16bits(lds16(q + 8192 + 2 * t));
-        const uint32_t words[8] = {qa.x, qa.y, qa.z, qa.w, qb.x, qb.y, qb.z, qb.w};
+        const uint32_t d2 = P::splat_from_f16bits(lds16(q + 8192 + 2 * b));
+        const uint32_t wa = q + 16 * b + 4 * (t >> 1), wb = wa + 4096;          // qa: elements 0..15, qb: 16..31, 4 per word
+        const uint32_t words[4] = {lds32(wa), lds32(wa + 8), lds32(wb), lds32(wb + 8)};
+        const uint32_t sel = (t & 1) ? 0x4342u : 0x4140u;                       // bytes of elements 2t, 2t+1 -> 16-bit lanes
         const uint32_t magic = opaque_const(P::MAGIC), c4380 = opaque_const(0x43804380u);
-        (void)c4380;
+        (void)magic; (void)c4380;
         #pragma unroll
-        for (int c = 0; c < 4; c++) {
-            uint32_t v[4];
-            #pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const uint32_t s = words[2 * c + h] ^ 0x80808080u;          // int8 -> biased 0..255
-                const uint32_t p01 = prmt(s, 0u, 0x4140u), p23 = prmt(s, 0u, 0x4342u);   // bytes -> 16-bit lanes
-                if constexpr (!BF) {   // fp16: 1024 + s is exact, minus 1152 = signed quant
-                    v[2 * h + 0] = P::mul(P::sub(p01 | P::MAGIC, 0x64806480u), d2);
-                    v[2 * h + 1] = P::mul(P::sub(p23 | P::MAGIC, 0x64806480u), d2);
-                } else {               // bf16 has 7 mantissa bits: 128 + (s & 127), minus 128 or 256 by bit 7
-                    const uint32_t m01 = and_or<0x007f007fu>(p01, magic), c01 = and_xor<0x00800080u>(p01, c4380);
-                    const uint32_t m23 = and_or<0x007f007fu>(p23, magic), c23 = and_xor<0x00800080u>(p23, c4380);
-                    v[2 * h + 0] = P::mul(P::sub(m01, c01), d2);
-                    v[2 * h + 1] = P::mul(P::sub(m23, c23), d2);
-                }
+        for (int j = 0; j < 4; j++) {
+            const uint32_t pr = prmt(words[j] ^ 0x80808080u, 0u, sel);          // int8 -> biased 0..255
+            if constexpr (!BF) {   // fp16: 1024 + s is exact, minus 1152 = signed quant
+                v[j] = P::mul(P::sub(pr | P::MAGIC, 0x64806480u), d2);
+            } else {               // bf16 has 7 mantissa bits: 128 + (s & 127), minus 128 or 256 by bit 7
+                v[j] = P::mul(P::sub(and_or<0x007f007fu>(pr, magic), and_xor<0x00800080u>(pr, c4380)), d2);
             }
-            out[4 * c + 0] = v[0]; out[4 * c + 1] = v[1]; out[4 * c + 2] = v[2]; out[4 * c + 3] = v[3];
         }
     } else {
         constexpr bool Q5 = (QT == QT_Q5_0 || QT == QT_Q5_1);
         constexpr bool AFFINE = (QT == QT_Q4_1 || QT == QT_Q5_1);
-        const uint4 qs = lds128(q + 16 * t);
+        const uint4 qs = lds128(q + 16 * b);
         uint32_t hq = 0;
         uint32_t off = 4096;
-        if constexpr (Q5) { hq = lds32(q + off + 4 * t); off += 1024; }
+        if constexpr (Q5) { hq = lds32(q + off + 4 * b); off += 1024; }
         uint32_t d2, m2 = 0;
         if constexpr (AFFINE) {
-            const uint32_t dm = lds32(q + off + 4 * t);
+            const uint32_t dm = lds32(q + off + 4 * b);
             d2 = P::splat_from_f16bits((uint16_t)(dm & 0xffffu));
             m2 = P::splat_from_f16bits((uint16_t)(dm >> 16));
         } else {
-            d2 = P::splat_from_f16bits(lds16(q + off + 2 * t));
+            d2 = P::splat_from_f16bits(lds16(q + off + 2 * b));
         }
         // zero point folded into the exact integer subtraction: 8 (q4_0), 16 (q5_0), 0 (q4_1 / q5_1)
         constexpr uint32_t ZP = (QT == QT_Q4_0) ? 8u : (QT == QT_Q5_0) ? 16u : 0u;
@@ -188,21 +143,47 @@ CB_DEVINL void unpack_block(uint32_t q, int t, uint32_t* __restrict__ out) {
         const uint32_t magic = opaque_const(P::MAGIC);
         #pragma unroll
         for (int j = 0; j < 4; j++) {
-            uint32_t v[4];
-            #pragma unroll
-            for (int i = 0; i < 4; i++) {
-                uint32_t x = and_or<0x000f000fu>(words[j] >> (4 * i), magic);
-                if constexpr (Q5) {
-                    const int sh = 4 * j + i;   // 5th bits of this pair sit at bits sh and sh+16 -> move to bits 4 / 20
-                    const uint32_t hb = (sh >= 4) ? (hq >> (sh - 4)) : (hq << (4 - sh));
-                    x = and_or<0x00100010u>(hb, x);
-                }
-                const uint32_t qv = P::sub(x, C2);
-                v[i] = AFFINE ? P::fma(qv, d2, m2) : P::mul(qv, d2);
+            uint32_t x = and_or<0x000f000fu>(words[j] >> (4 * t), magic);       // pair t of word j: elements 8j + 2t, 8j + 2t + 1
+            if constexpr (Q5) {
+                const int sh = 4 * j + t;   // 5th bits of this pair sit at bits sh and sh+16 -> move to bits 4 / 20
+                const uint32_t hb = (sh >= 4) ? (hq >> (sh - 4)) : (hq << (4 - sh));
+                x = and_or<0x00100010u>(hb, x);
             }
-            out[4 * j + 0] = v[0]; out[4 * j + 1] = v[1]; out[4 * j + 2] = v[2]; out[4 * j + 3] = v[3];
+            const uint32_t qv = P::sub(x, C2);
+            v[j] = AFFINE ? P::fma(qv, d2, m2) : P::mul(qv, d2);
         }
     }
+}
+
+// wgmma A fragments of one 64-deep k-block for this lane: tile rows r and r + 8, t = lane % 4.  k step s = 2 half + u covers elements
+// 16u .. 16u + 15 of ggml block (row, half); a[4s + 0 / 1] = rows r / r + 8 at k 2t, 2t + 1, a[4s + 2 / 3] = the same rows at k 2t + 8, 2t + 9.
+template <int QT, bool BF>
+CB_DEVINL void unpack_frag(uint32_t q, int r, int t, uint32_t (&a)[16]) {
+    #pragma unroll
+    for (int half = 0; half < 2; half++) {
+        #pragma unroll
+        for (int h8 = 0; h8 < 2; h8++) {
+            uint32_t v[4];
+            unpack_pairs<QT, BF>(q, half * 128 + r + 8 * h8, t, v);
+            #pragma unroll
+            for (int u = 0; u < 2; u++) {
+                a[4 * (2 * half + u) + h8] = v[2 * u];
+                a[4 * (2 * half + u) + 2 + h8] = v[2 * u + 1];
+            }
+        }
+    }
+}
+
+// register budget of the calling warpgroup (all its threads execute it): producer down, consumers up
+template <int N>
+CB_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+CB_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// keeps the compiler from reusing a register an in-flight wgmma may still read before the wgmma_wait that retires it
+CB_DEVINL void fence_frag(uint32_t (&a)[16]) {
+    #pragma unroll
+    for (int i = 0; i < 16; i++) asm volatile("" : "+r"(a[i])::"memory");
 }
 
 // 16-bit epilogue value of one accumulator element.  `bias` arrives PRE-MULTIPLIED by `mul` for EPI_STORE16 so that
@@ -219,572 +200,145 @@ CB_DEVINL float epi_value(float acc, float bias, float mul) {
     } else return fmaf(acc, mul, bias);
 }
 
-// Epilogue of one [128 features x 192 tokens] accumulator: this thread owns feature n (TMEM lane) and walks the token
-// columns 32 at a time.  For a fixed token the 32 lanes of a warp hold 32 consecutive features -> every global access
-// below is one fully coalesced 64-B (16-bit) or 128-B (fp32) request.  Specialised per epilogue kind at compile time;
-// element offsets are 32-bit (host checks M*ldo < 2^32) so each access costs one IADD + one IMAD.WIDE.
-template <int EPI, bool BF, bool FULL>
-CB_DEVINL void epilogue_chunk(const KParams& p, const uint32_t (&r)[32], uint32_t off, uint32_t ldo, int nvalid, float bias, float mul) {
-    if constexpr (EPI == EPI_STORE32) {
-        float* base = reinterpret_cast<float*>(p.out);
-        uint32_t o = off;
-        #pragma unroll
-        for (int j = 0; j < 32; j++, o += ldo)
-            if (FULL || j < nvalid) base[o] = __uint_as_float(r[j]) + bias;
-    } else if constexpr (EPI == EPI_REDADD32) {      // direct fallback (no output map): every element belongs to exactly one thread
-        float* base = reinterpret_cast<float*>(p.out);
-        uint32_t o = off;
-        #pragma unroll
-        for (int j = 0; j < 32; j++, o += ldo)
-            if (FULL || j < nvalid) base[o] += __uint_as_float(r[j]) + bias;
-    } else {
-        uint16_t* base = reinterpret_cast<uint16_t*>(p.out);
-        uint32_t o = off;
-        #pragma unroll
-        for (int j = 0; j < 32; j++, o += ldo) {
-            const float v = epi_value<EPI>(__uint_as_float(r[j]), bias, mul);
-            if (FULL || j < nvalid) base[o] = P2<BF>::from_float(v);
-        }
-    }
-}
-
-// 16-bit epilogue through shared memory: the warp (32 features of the tile = 32 TMEM lanes) converts one 32-token chunk, lane f
-// writes its feature's 32 values as 2-byte words into a [32 tokens x 32 features] block (row = token, 64 B: one conflict-free
-// wavefront per token), and ONE TMA store moves the block to out[tok0 + 32 c ..][n0 ..].  The 2-byte global stores this replaces
-// were the most expensive part of the epilogue for the mainloop (profiles/r02_gemm_probe.md: the STG stream, not the TMEM reads).
+// Epilogue of one consumer group's [64 features x 192 tokens] accumulator (fragment layout: wgmma.cuh).  This thread owns features
+// f and f + 8 and tokens 8j + tc + {0, 1}; element offsets are 32-bit (host checks M*ldo < 2^32).
 template <int EPI, bool BF>
-CB_DEVINL void epilogue_tile_tma(const KParams& p, uint32_t acc_addr, int tok0, int n0, float bias, float mul, uint32_t stage, uint32_t& cidx, int lane) {
+CB_DEVINL void epilogue_regs(const KParams& p, float (&acc)[BN / 2], int tok0, int f, int tc, const float (&bias)[2], const float (&mul)[2]) {
     const int ntok = min(BN, p.M - tok0);
-    #pragma unroll 1
-    for (int c = 0; c < BN / 32; c++) {
-        if (ntok - c * 32 <= 0) break;             // warp-uniform
-        const uint32_t buf = stage + (cidx & 1u) * 4096u;
-        cidx++;
-        if (lane == 0) bulk_wait_group_read<1>();  // the store that last used THIS buffer (two chunks ago) has read it
-        __syncwarp();
-        uint32_t r[32];
-        tmem_ld_32x32(acc_addr + c * 32, r);
-        tmem_ld_wait();
-        if constexpr (EPI == EPI_REDADD32) {
-            // fp32 residual stream: x[tok, n] += acc + bias.  Row = token (128 B: one conflict-free wavefront), then ONE TMA reduce-add.
-            #pragma unroll
-            for (int j = 0; j < 32; j++) sts32(buf + (uint32_t)j * 128u + (uint32_t)lane * 4u, __float_as_uint(__uint_as_float(r[j]) + bias));
-        } else {
-            #pragma unroll
-            for (int j = 0; j < 32; j++) sts16(buf + (uint32_t)j * 64u + (uint32_t)lane * 2u, P2<BF>::from_float(epi_value<EPI>(__uint_as_float(r[j]), bias, mul)));
-        }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-            if constexpr (EPI == EPI_REDADD32) tma_reduce_add_2d(&p.tm_out, buf, n0, tok0 + c * 32);
-            else tma_store_2d(&p.tm_out, buf, n0, tok0 + c * 32);
-            bulk_commit_group();
-        }
-    }
-}
-
-template <int EPI, bool BF>
-CB_DEVINL void epilogue_tile(const KParams& p, uint32_t acc_addr, int tok0, int n, float bias, float mul) {
     const uint32_t ldo = (uint32_t)p.ldo;
-    const int ntok = min(BN, p.M - tok0);
-    uint32_t off = (uint32_t)tok0 * ldo + (uint32_t)n;
-    #pragma unroll 1
-    for (int c = 0; c < BN / 32; c++, off += 32u * ldo) {
-        const int nvalid = ntok - c * 32;
-        if (nvalid <= 0) break;                    // warp-uniform
-        uint32_t r[32];
-        tmem_ld_32x32(acc_addr + c * 32, r);
-        tmem_ld_wait();
-        if (CB_DBG(p, 16)) { if (r[0] == 0x7fc12345u && r[31] == 0x7fc54321u) reinterpret_cast<uint32_t*>(p.out)[0] = r[5]; }   // keep the loads alive
-        else if (nvalid >= 32) epilogue_chunk<EPI, BF, true>(p, r, off, ldo, 32, bias, mul);
-        else epilogue_chunk<EPI, BF, false>(p, r, off, ldo, nvalid, bias, mul);
+    #pragma unroll
+    for (int j = 0; j < BN / 8; j++) {
+        #pragma unroll
+        for (int e = 0; e < 4; e++) {
+            const int t = 8 * j + tc + (e & 1), h = e >> 1;
+            if (t >= ntok) continue;
+            const uint32_t o = (uint32_t)(tok0 + t) * ldo + (uint32_t)(f + 8 * h);
+            const float a = acc[4 * j + e];
+            if constexpr (EPI == EPI_STORE32) reinterpret_cast<float*>(p.out)[o] = a + bias[h];
+            else if constexpr (EPI == EPI_REDADD32) reinterpret_cast<float*>(p.out)[o] += a + bias[h];
+            else reinterpret_cast<uint16_t*>(p.out)[o] = P2<BF>::from_float(epi_value<EPI>(a, bias[h], mul[h]));
+        }
     }
 }
 
-// PAIR = true: two CTAs (a cluster of 2 = one TPC) work on one [256 features x 192 tokens] tile with cta_group::2 UMMAs.  Each CTA
-// unpacks ITS 128 feature rows into ITS tensor memory and TMA-loads HALF of the token tile (96 rows); the leader CTA (rank 0)
-// issues every MMA (M = 256) and multicasts the commits; the peer's TMA bytes, A-stage arrivals and accumulator releases are
-// credited to the leader's mbarriers (cluster-scope arrive / cta_group::2 TMA).  Halves the activation traffic per CTA and lifts
-// the single-CTA UMMA issue ceiling measured in profiles/r01_gemm_probe.txt.
-template <int QT, bool BF, bool PAIR>
-__global__ void __launch_bounds__(QT == QT_F16 ? 256 : 512, 1) gemm_dq_kernel(const __grid_constant__ KParams p) {
-    using C = Cfg<QT, PAIR>;
+template <int QT, bool BF>
+__global__ void __launch_bounds__(THREADS, 1) gemm_dq_kernel(const __grid_constant__ KParams p) {
+    using C = Cfg<QT>;
     constexpr bool DQ = C::DQ;
-    static_assert(!PAIR || DQ, "pair kernels exist for the quantized (TS-form) path only");
     constexpr int SX = C::SX, SQ = DQ ? C::SQ : 1;
-    constexpr uint32_t IDESC = umma_idesc(BF, PAIR ? 2 * BM : BM, BN);
-    const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-    const bool leader = rank == 0;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     const uint32_t smem_base = smem_u32(smem);
     const uint32_t bars = smem_base + C::BAR_OFF;
     // barrier slots (8 B each)
-    const uint32_t x_full = bars, x_empty = x_full + 8 * SX, q_full = x_empty + 8 * SX, q_empty = q_full + 8 * SQ,
-                   a_full = q_empty + 8 * SQ, a_empty = a_full + 8 * NA, acc_full = a_empty + 8 * NA, acc_empty = acc_full + 16;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + C::BAR_OFF + 16 * SX + 16 * SQ + 16 * NA + 32);
-    static_assert(16 * C::SX + 16 * (DQ ? C::SQ : 1) + 16 * NA + 32 + 4 <= 512, "barrier area");
+    const uint32_t x_full = bars, x_empty = x_full + 8 * SX, q_full = x_empty + 8 * SX, q_empty = q_full + 8 * SQ;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < SX; i++) { mbar_init(x_full + 8 * i, 1); mbar_init(x_empty + 8 * i, 1); }
-        for (int i = 0; i < SQ; i++) { mbar_init(q_full + 8 * i, 1); mbar_init(q_empty + 8 * i, 4); }
-        for (int i = 0; i < NA; i++) { mbar_init(a_full + 8 * i, PAIR ? 8 : 4); mbar_init(a_empty + 8 * i, 1); }
-        for (int i = 0; i < 2; i++) { mbar_init(acc_full + 8 * i, 1); mbar_init(acc_empty + 8 * i, PAIR ? 2 * N_EPI_WARPS : N_EPI_WARPS); }
+        for (int i = 0; i < SX; i++) { mbar_init(x_full + 8 * i, 1); mbar_init(x_empty + 8 * i, 8); }   // released by each consumer warp
+        for (int i = 0; i < SQ; i++) { mbar_init(q_full + 8 * i, 1); mbar_init(q_empty + 8 * i, 8); }
         mbar_fence_init();
         tma_prefetch_desc(&p.tm_x);
         if (!DQ) tma_prefetch_desc(&p.tm_w);
-        if (PAIR) tma_prefetch_desc(&p.tm_xh);
-        if (DQ && p.tma_out) tma_prefetch_desc(&p.tm_out);
     }
-    if (warp == 2) { if constexpr (PAIR) tmem_alloc_2sm(smem_u32(tmem_slot), TMEM_COLS); else tmem_alloc(smem_u32(tmem_slot), TMEM_COLS); }
-    tc_fence_before();
     __syncthreads();
-    if constexpr (PAIR) cluster_sync_all();      // the peer's barriers must be initialised before anything arrives on them remotely
-    tc_fence_after();
     pdl_trigger();      // the next kernel of the stream may start placing CTAs as ours retire ...
     pdl_wait();         // ... and we touch global memory only after the previous grid has completed
-    const uint32_t tmem_base = *tmem_slot;
 
-    // work units: 1-CTA kernels walk [128 x 192] tiles with stride gridDim; pair kernels walk [256 x 192] tiles with stride gridDim/2
-    const int n_ft = p.N / (PAIR ? 2 * BM : BM), n_tt = (p.M + BN - 1) / BN, n_tiles = n_ft * n_tt, nkb = p.K / BK;
-    const int first = PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x, stride = PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-    const int my_tiles = (n_tiles - first + stride - 1) / stride;                              // tiles of this CTA (pair)
-    const int total_kb = my_tiles * nkb;                                                      // k-blocks of this CTA
+    // work units: [128 features x 192 tokens] tiles, feature tile fastest (CTAs running at the same time share their X tile in L2)
+    const int n_ft = p.N / BM, n_tt = (p.M + BN - 1) / BN, n_tiles = n_ft * n_tt, nkb = p.K / BK;
 
-    if (warp == 0) {
-        // ------------------------------------------------------------------ X producer (f16: X and W)
-        uint32_t s = 0, ph = 0;
-        for (int tile = first; tile < n_tiles; tile += stride) {
-            const int ft = tile % n_ft, tt = tile / n_ft;
-            for (int kb = 0; kb < nkb; kb++) {
-                mbar_wait(x_empty + 8 * s, ph ^ 1);
-                if (elect_one()) {
-                    const uint32_t dst = smem_base + s * C::XS;
-                    if constexpr (PAIR) {
-                        // both CTAs load their half of the token tile; all bytes are credited to the LEADER's x_full barrier
-                        if (CB_DBG(p, 2)) { if (leader) mbar_arrive(x_full + 8 * s); }
-                        else {
-                        if (leader) mbar_arrive_expect_tx(x_full + 8 * s, X_STAGE);
-                        tma_load_2d_2sm(dst, &p.tm_xh, kb * BK, tt * BN + (int)rank * (BN / 2), mapa_rank0(x_full + 8 * s));
-                        }
-                    } else if (CB_DBG(p, 2)) mbar_arrive(x_full + 8 * s);
-                    else {
-                        mbar_arrive_expect_tx(x_full + 8 * s, C::XS);
-                        tma_load_2d(dst, &p.tm_x, kb * BK, tt * BN, x_full + 8 * s);
-                        if constexpr (!DQ) tma_load_2d(dst + X_STAGE, &p.tm_w, kb * BK, ft * BM, x_full + 8 * s);
-                    }
-                }
-                __syncwarp();
-                if (++s == SX) { s = 0; ph ^= 1; }
-            }
-        }
-    } else if (warp == 3) {
-        // ------------------------------------------------------------------ Q producer (packed weight blocks)
-        if constexpr (DQ) {
-            uint32_t s = 0, ph = 0;
-            for (int tile = first; tile < n_tiles; tile += stride) {
-                const int ft = PAIR ? (tile % n_ft) * 2 + (int)rank : tile % n_ft;      // 128-row feature tile this CTA unpacks
-                const uint8_t* src = p.w_packed + (size_t)ft * nkb * C::CHUNK;
+    if (warp >= 8) {
+        // ------------------------------------------------------------------ producer (one thread)
+        setmaxnreg_dec<40>();
+        if (warp == 8 && lane == 0) {
+            uint32_t s = 0, ph = 0, qs = 0, qph = 0;
+            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+                const int ft = tile % n_ft, tt = tile / n_ft;
                 for (int kb = 0; kb < nkb; kb++) {
-                    mbar_wait(q_empty + 8 * s, ph ^ 1);
-                    if (elect_one()) {
-                        if (CB_DBG(p, 4)) mbar_arrive(q_full + 8 * s);
-                        else {
-                        mbar_arrive_expect_tx(q_full + 8 * s, C::CHUNK);
-                        bulk_load_1d(smem_base + C::Q_OFF + s * C::CHUNK, src + (size_t)kb * C::CHUNK, C::CHUNK, q_full + 8 * s);
-                        }
-                    }
-                    __syncwarp();
-                    if (++s == SQ) { s = 0; ph ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer: the warp walks the loop, ONE elected
-        // thread issues (elect.sync keeps descriptors in uniform registers: 4 UTCHMMA + 2-3 UTCBAR back to back per k-block)
-        const uint64_t dx0 = umma_desc_k128(smem_base);
-        const uint64_t dw0 = umma_desc_k128(smem_base + X_STAGE);    // f16 path: W tile follows the X tile in each stage
-        constexpr uint64_t X_STEP = C::XS >> 4;
-        if constexpr (PAIR) {
-            // The issuer is the serial heart of the kernel and shares its scheduler with an epilogue warp and two unpack warps: every
-            // instruction it does not execute is tensor time (tools/pipe_probe.cu: one busy ALU warp on its scheduler costs 25 %).  The
-            // ring walk is therefore unrolled over lcm(X ring, A ring) k-blocks: stage indices, barrier addresses and descriptor offsets
-            // are compile-time constants, the parities follow from the pass counter, and what remains per k-block is two barrier probes,
-            // four UMMAs and two or three commits.
-            constexpr int UNROLL = (SX % NA == 0) ? SX : (SX % 2 == 0 ? 2 * SX : 4 * SX);      // lcm(SX, 4)
-            static_assert(UNROLL % SX == 0 && UNROLL % NA == 0, "ring walk");
-            if (leader && elect_one()) {          // ONE thread runs the whole loop: no re-election, no reconvergence per k-block
-                const uint32_t total = (uint32_t)total_kb;
-                uint32_t i = 0, pass = 0, kb = 0, it = 0, d_tmem = tmem_base, as = 0;
-                while (i < total) {
-                    #pragma unroll
-                    for (int u = 0; u < UNROLL; u++) {
-                        const int s = u % SX, sa = u % NA;
-                        if (kb == 0) {
-                            if (i >= total) break;                 // the work list ends on a tile boundary
-                            as = it & 1u;
-                            d_tmem = tmem_base + as * BN;
-                            mbar_wait(acc_empty + 8 * as, ((it >> 1) & 1u) ^ 1u);
-                        }
-                        mbar_wait(x_full + 8 * s, (((uint32_t)(UNROLL / SX) * pass) + (uint32_t)(u / SX)) & 1u);
-                        if (!CB_DBG(p, 64)) mbar_wait(a_full + 8 * sa, (((uint32_t)(UNROLL / NA) * pass) + (uint32_t)(u / NA)) & 1u);
-                        tc_fence_after();
-                        const uint64_t db = dx0 + (uint64_t)s * X_STEP;
-                        const uint32_t a_t = tmem_base + A_COL0 + sa * 32;
-                        umma_f16_ts_2sm(d_tmem, a_t, db, IDESC, kb);
-                        umma_f16_ts_2sm_acc(d_tmem, a_t + 8, db + 2, IDESC);
-                        umma_f16_ts_2sm_acc(d_tmem, a_t + 16, db + 4, IDESC);
-                        umma_f16_ts_2sm_acc(d_tmem, a_t + 24, db + 6, IDESC);
-                        umma_commit_2sm(x_empty + 8 * s);
-                        umma_commit_2sm(a_empty + 8 * sa);
-                        if (kb == (uint32_t)nkb - 1) umma_commit_2sm(acc_full + 8 * as);
-                        i++;
-                        if (++kb == (uint32_t)nkb) { kb = 0; it++; }
-                    }
-                    pass++;
-                }
-            }
-            __syncwarp();
-        } else {
-        uint32_t s = 0, ph = 0, sa = 0, pa = 0;
-        int it = 0;
-        for (int tile = first; tile < n_tiles; tile += stride, it++) {
-            const uint32_t as = it & 1, aph = (it >> 1) & 1;
-            const uint32_t d_tmem = tmem_base + as * BN;
-            mbar_wait(acc_empty + 8 * as, aph ^ 1);
-            tc_fence_after();
-            for (int kb = 0; kb < nkb; kb++) {
-                mbar_wait(x_full + 8 * s, ph);
-                if constexpr (DQ) { if (!CB_DBG(p, 64)) mbar_wait(a_full + 8 * sa, pa); }
-                tc_fence_after();
-                const uint64_t db = dx0 + (uint64_t)s * X_STEP;
-                if (elect_one()) {
                     if constexpr (DQ) {
-                        const uint32_t a_t = tmem_base + A_COL0 + sa * 32;      // 16 k = 8 TMEM columns per MMA step
-                        if (kb == 0) umma_f16_ts_init(d_tmem, a_t, db, IDESC);
-                        else umma_f16_ts_acc(d_tmem, a_t, db, IDESC);
-                        umma_f16_ts_acc(d_tmem, a_t + 8, db + 2, IDESC);          // B: +16 elements = +32 B = +2 descriptor units
-                        umma_f16_ts_acc(d_tmem, a_t + 16, db + 4, IDESC);
-                        umma_f16_ts_acc(d_tmem, a_t + 24, db + 6, IDESC);
-                        umma_commit(x_empty + 8 * s);
-                        umma_commit(a_empty + 8 * sa);
-                    } else {
-                        const uint64_t da = dw0 + (uint64_t)s * X_STEP;
-                        if (kb == 0) umma_f16_init(d_tmem, da, db, IDESC);
-                        else umma_f16_acc(d_tmem, da, db, IDESC);
-                        umma_f16_acc(d_tmem, da + 2, db + 2, IDESC);
-                        umma_f16_acc(d_tmem, da + 4, db + 4, IDESC);
-                        umma_f16_acc(d_tmem, da + 6, db + 6, IDESC);
-                        umma_commit(x_empty + 8 * s);
+                        mbar_wait(q_empty + 8 * qs, qph ^ 1);
+                        mbar_arrive_expect_tx(q_full + 8 * qs, C::CHUNK);
+                        bulk_load_1d(smem_base + C::Q_OFF + qs * C::CHUNK, p.w_packed + ((size_t)ft * nkb + kb) * C::CHUNK, C::CHUNK, q_full + 8 * qs);
+                        if (++qs == SQ) { qs = 0; qph ^= 1; }
                     }
-                    if (kb == nkb - 1) umma_commit(acc_full + 8 * as);
-                }
-                __syncwarp();
-                if (++s == SX) { s = 0; ph ^= 1; }
-                if constexpr (DQ) { if (++sa == NA) { sa = 0; pa ^= 1; } }
-            }
-        }
-        }
-    } else if (warp >= 4 && warp < 8) {
-        // ------------------------------------------------------------------ epilogue
-        const int fr = (warp & 3) * 32 + lane;                     // feature row of the tile == TMEM lane
-        const uint32_t lane_addr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-        int it = 0;
-        uint32_t cidx = 0;
-        const uint32_t out_stage = smem_base + C::OUT_OFF + (uint32_t)(warp & 3) * 8192u;
-        const bool tma_out = DQ && p.tma_out && !(CB_DBG(p, 24));
-        for (int tile = first; tile < n_tiles; tile += stride, it++) {
-            const int ft = PAIR ? (tile % n_ft) * 2 + (int)rank : tile % n_ft, tt = tile / n_ft;
-            const uint32_t as = it & 1, aph = (it >> 1) & 1;
-            const int n = ft * BM + fr;
-            const float mul = (n < p.scale_cols) ? p.scale : 1.0f;
-            const float bias = (p.bias ? p.bias[n] : 0.0f) * ((p.epi == EPI_STORE16) ? mul : 1.0f);
-            mbar_wait(acc_full + 8 * as, aph);
-            tc_fence_after();
-            const int tok0 = tt * BN;
-            const uint32_t acc_addr = lane_addr + as * BN;
-            if (tma_out) {
-                const int n0 = ft * BM + (warp & 3) * 32;
-                switch (p.epi) {
-                case EPI_GELU16: epilogue_tile_tma<EPI_GELU16, BF>(p, acc_addr, tok0, n0, bias, mul, out_stage, cidx, lane); break;
-                case EPI_QGELU16: epilogue_tile_tma<EPI_QGELU16, BF>(p, acc_addr, tok0, n0, bias, mul, out_stage, cidx, lane); break;
-                case EPI_REDADD32: epilogue_tile_tma<EPI_REDADD32, BF>(p, acc_addr, tok0, n0, bias, mul, out_stage, cidx, lane); break;
-                default: epilogue_tile_tma<EPI_STORE16, BF>(p, acc_addr, tok0, n0, bias, mul, out_stage, cidx, lane); break;
-                }
-            } else
-            if (!(CB_DBG(p, 8))) switch (p.epi) {
-            case EPI_STORE16: epilogue_tile<EPI_STORE16, BF>(p, acc_addr, tok0, n, bias, mul); break;
-            case EPI_GELU16: epilogue_tile<EPI_GELU16, BF>(p, acc_addr, tok0, n, bias, mul); break;
-            case EPI_QGELU16: epilogue_tile<EPI_QGELU16, BF>(p, acc_addr, tok0, n, bias, mul); break;
-            case EPI_REDADD32: epilogue_tile<EPI_REDADD32, BF>(p, acc_addr, tok0, n, bias, mul); break;
-            default: epilogue_tile<EPI_STORE32, BF>(p, acc_addr, tok0, n, bias, mul); break;
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) { if constexpr (PAIR) mbar_arrive_cluster(mapa_rank0(acc_empty + 8 * as)); else mbar_arrive(acc_empty + 8 * as); }
-        }
-        if (lane == 0) bulk_wait_group_read<0>();      // no TMA store may still be reading the staging buffers when the CTA exits
-    } else if (warp >= 8) {
-        // ------------------------------------------------------------------ unpack groups: registers -> TMEM A stages
-        if constexpr (DQ) {
-            const int g = (warp - 8) >> 2;                        // group 0..1 owns k-blocks i = g (mod 2)
-            const int row = (warp & 3) * 32 + lane;               // weight row of the tile == TMEM lane (warp%4 = lane quarter)
-            const uint32_t a_lane = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + A_COL0;
-            uint32_t qs = g, qph = 0, sa = g, pa = 0;             // ring positions of k-block i = g
-            for (int i = g; i < total_kb; i += N_GROUPS) {
-                // the unpack math only needs the packed chunk: do it BEFORE waiting for the TMEM stage, so the a_empty -> a_full
-                // round trip seen by the MMA warp is just tcgen05.st + wait::st (matters most for the CTA-pair kernel)
-                mbar_wait(q_full + 8 * qs, qph);
-                const uint32_t qa = smem_base + C::Q_OFF + qs * C::CHUNK;
-                uint32_t v[32];
-                if (!(CB_DBG(p, 1))) {
-                    unpack_block<DQ ? QT : QT_Q4_0, BF>(qa, row, v);              // k  0..31 of this row
-                    unpack_block<DQ ? QT : QT_Q4_0, BF>(qa, 128 + row, v + 16);   // k 32..63
-                }
-                __syncwarp();
-                if (lane == 0) mbar_arrive(q_empty + 8 * qs);
-                if (!(CB_DBG(p, 32))) mbar_wait(a_empty + 8 * sa, pa ^ 1);
-                tc_fence_after();
-                if (!(CB_DBG(p, 1))) {
-                    tmem_st_32x32(a_lane + sa * 32, v);
-                    tmem_st_wait();
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) {
-                    if constexpr (PAIR) mbar_arrive_cluster(mapa_rank0(a_full + 8 * sa)); else mbar_arrive(a_full + 8 * sa);
-                }
-                qs += N_GROUPS; if (qs >= (uint32_t)SQ) { qs -= SQ; qph ^= 1; }
-                sa += N_GROUPS; if (sa >= (uint32_t)NA) { sa -= NA; pa ^= 1; }
-            }
-        }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if constexpr (PAIR) cluster_sync_all();      // neither CTA may exit (or free TMEM) while the pair's MMAs / multicasts are in flight
-    if (warp == 2) { if constexpr (PAIR) tmem_dealloc_2sm(tmem_base, TMEM_COLS); else tmem_dealloc(tmem_base, TMEM_COLS); }
-}
-
-// =====================================================================================================================================
-// The WIDE form (the one the layer GEMMs of a tower run): a CTA pair works on a [256 features x 384 tokens] super-tile, i.e. BOTH
-// accumulators are live at once and every dequantised A stage feeds EIGHT UMMAs (two token tiles) instead of four.  The warps of an SM
-// share four issue ports and the unpack arithmetic was taking ~160 of them per k-block next to a 384-cycle MMA budget (profiles/
-// r02_gemm_probe.md); amortising it over 768 MMA cycles is what lifts the tensor pipe.  The accumulators are no longer double-buffered
-// across tiles: the epilogue drains acc0 while the MMAs of the last k-block still run on acc1, and the next super-tile's acc0 MMAs start
-// as soon as acc0 is drained.  The tail of the work list is cut into HALF super-tiles (one accumulator, the old shape) so that the last
-// wave costs half a wave.
-// =====================================================================================================================================
-struct Work { int ft, tok0, nh; };      // feature-pair tile, first token, number of 192-token halves (0 = nothing to do)
-
-// work item g of the launch: super-tiles [0, full) first, then the remaining super-tiles as 2 half items each
-CB_DEVINL bool get_work(int g, int n_ft, int n_super, int full, int M, Work& w) {
-    int st, half = 0, nh = 2;
-    if (g < full) st = g;
-    else { const int h = g - full; st = full + (h >> 1); half = h & 1; nh = 1; }
-    if (st >= n_super) return false;
-    w.ft = st % n_ft;
-    w.tok0 = (st / n_ft) * (2 * BN) + half * BN;
-    w.nh = (w.tok0 >= M) ? 0 : ((nh == 2 && w.tok0 + BN < M) ? 2 : 1);
-    return true;
-}
-
-template <int QT, bool BF>
-__global__ void __launch_bounds__(512, 1) gemm_dq2_kernel(const __grid_constant__ KParams p) {
-    using C = Cfg<QT, true>;
-    constexpr int SX = C::SX, SQ = C::SQ;
-    constexpr uint32_t IDESC = umma_idesc(BF, 2 * BM, BN);
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const uint32_t smem_base = smem_u32(smem);
-    const uint32_t bars = smem_base + C::BAR_OFF;
-    const uint32_t x_full = bars, x_empty = x_full + 8 * SX, q_full = x_empty + 8 * SX, q_empty = q_full + 8 * SQ,
-                   a_full = q_empty + 8 * SQ, a_empty = a_full + 8 * NA, acc_full = a_empty + 8 * NA, acc_empty = acc_full + 16;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + C::BAR_OFF + 16 * SX + 16 * SQ + 16 * NA + 32);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < SX; i++) { mbar_init(x_full + 8 * i, 1); mbar_init(x_empty + 8 * i, 1); }
-        for (int i = 0; i < SQ; i++) { mbar_init(q_full + 8 * i, 1); mbar_init(q_empty + 8 * i, 4); }
-        for (int i = 0; i < NA; i++) { mbar_init(a_full + 8 * i, 8); mbar_init(a_empty + 8 * i, 1); }
-        for (int i = 0; i < 2; i++) { mbar_init(acc_full + 8 * i, 1); mbar_init(acc_empty + 8 * i, 2 * N_EPI_WARPS); }
-        mbar_fence_init();
-        tma_prefetch_desc(&p.tm_xh);
-        if (p.tma_out) tma_prefetch_desc(&p.tm_out);
-    }
-    if (warp == 2) tmem_alloc_2sm(smem_u32(tmem_slot), TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    pdl_trigger();
-    pdl_wait();
-    const uint32_t tmem_base = *tmem_slot;
-
-    const int n_ft = p.N / (2 * BM), n_super = n_ft * ((p.M + 2 * BN - 1) / (2 * BN)), nkb = p.K / BK;
-    const int first = (int)(blockIdx.x >> 1), stride = (int)(gridDim.x >> 1);
-    const int full = (n_super / stride) * stride;                 // whole waves of super-tiles; the rest is walked as half items
-    Work w;
-
-    if (warp == 0) {
-        // ------------------------------------------------------------------ X producer: per k-block one 96-token box per live half
-        uint32_t s = 0, ph = 0;
-        for (int g = first; get_work(g, n_ft, n_super, full, p.M, w); g += stride) {
-            for (int kb = 0; kb < nkb; kb++)
-                for (int h = 0; h < w.nh; h++) {
                     mbar_wait(x_empty + 8 * s, ph ^ 1);
-                    if (elect_one()) {
-                        if (CB_DBG(p, 2)) { if (leader) mbar_arrive(x_full + 8 * s); }
-                        else {
-                            if (leader) mbar_arrive_expect_tx(x_full + 8 * s, X_STAGE);
-                            tma_load_2d_2sm(smem_base + s * C::XS, &p.tm_xh, kb * BK, w.tok0 + h * BN + (int)rank * (BN / 2), mapa_rank0(x_full + 8 * s));
-                        }
-                    }
-                    __syncwarp();
+                    mbar_arrive_expect_tx(x_full + 8 * s, C::XS);      // rows past M are zero-filled and still counted
+                    tma_load_2d(smem_base + s * C::XS, &p.tm_x, kb * BK, tt * BN, x_full + 8 * s);
+                    if constexpr (!DQ) tma_load_2d(smem_base + s * C::XS + X_STAGE, &p.tm_w, kb * BK, ft * BM, x_full + 8 * s);
                     if (++s == SX) { s = 0; ph ^= 1; }
                 }
-        }
-    } else if (warp == 3) {
-        // ------------------------------------------------------------------ Q producer (packed weight blocks of this CTA's 128 rows)
-        uint32_t s = 0, ph = 0;
-        for (int g = first; get_work(g, n_ft, n_super, full, p.M, w); g += stride) {
-            if (w.nh == 0) continue;
-            const uint8_t* src = p.w_packed + (size_t)(w.ft * 2 + (int)rank) * nkb * C::CHUNK;
-            for (int kb = 0; kb < nkb; kb++) {
-                mbar_wait(q_empty + 8 * s, ph ^ 1);
-                if (elect_one()) {
-                    if (CB_DBG(p, 4)) mbar_arrive(q_full + 8 * s);
-                    else {
-                        mbar_arrive_expect_tx(q_full + 8 * s, C::CHUNK);
-                        bulk_load_1d(smem_base + C::Q_OFF + s * C::CHUNK, src + (size_t)kb * C::CHUNK, C::CHUNK, q_full + 8 * s);
-                    }
-                }
-                __syncwarp();
-                if (++s == SQ) { s = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer (leader CTA): 4 UMMAs per live half and k-block
-        if (leader) {
-            const uint64_t dx0 = umma_desc_k128(smem_base);
-            constexpr uint64_t X_STEP = C::XS >> 4;
-            uint32_t s = 0, ph = 0, sa = 0, pa = 0, u0 = 0, u1 = 0;      // u0 / u1: uses of accumulator 0 / 1 so far (barrier phases)
-            for (int g = first; get_work(g, n_ft, n_super, full, p.M, w); g += stride) {
-                if (w.nh == 0) continue;
-                mbar_wait(acc_empty + 0, (u0 & 1) ^ 1);
-                for (int kb = 0; kb < nkb; kb++) {
-                    if (!(CB_DBG(p, 64))) mbar_wait(a_full + 8 * sa, pa);
-                    const uint32_t a_t = tmem_base + A_COL0 + sa * 32;
-                    for (int h = 0; h < w.nh; h++) {
-                        mbar_wait(x_full + 8 * s, ph);
-                        if (h == 1 && kb == 0) mbar_wait(acc_empty + 8, (u1 & 1) ^ 1);
-                        tc_fence_after();
-                        const uint64_t db = dx0 + (uint64_t)s * X_STEP;
-                        const uint32_t d_tmem = tmem_base + h * BN;
-                        if (elect_one()) {
-                            if (kb == 0) umma_f16_ts_2sm_init(d_tmem, a_t, db, IDESC);
-                            else umma_f16_ts_2sm_acc(d_tmem, a_t, db, IDESC);
-                            umma_f16_ts_2sm_acc(d_tmem, a_t + 8, db + 2, IDESC);
-                            umma_f16_ts_2sm_acc(d_tmem, a_t + 16, db + 4, IDESC);
-                            umma_f16_ts_2sm_acc(d_tmem, a_t + 24, db + 6, IDESC);
-                            umma_commit_2sm(x_empty + 8 * s);
-                            if (h == w.nh - 1) umma_commit_2sm(a_empty + 8 * sa);
-                            if (kb == nkb - 1) umma_commit_2sm(acc_full + 8 * h);
-                        }
-                        __syncwarp();
-                        if (++s == SX) { s = 0; ph ^= 1; }
-                    }
-                    if (++sa == NA) { sa = 0; pa ^= 1; }
-                }
-                u0++;
-                if (w.nh == 2) u1++;
-            }
-        }
-    } else if (warp >= 4 && warp < 8) {
-        // ------------------------------------------------------------------ epilogue: acc0 first (while acc1's last MMAs still run), then acc1
-        const int fr = (warp & 3) * 32 + lane;
-        const uint32_t lane_addr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-        uint32_t cidx = 0, u0 = 0, u1 = 0;
-        const uint32_t out_stage = smem_base + C::OUT_OFF + (uint32_t)(warp & 3) * 8192u;
-        const bool tma_out = p.tma_out && !(CB_DBG(p, 24));
-        for (int g = first; get_work(g, n_ft, n_super, full, p.M, w); g += stride) {
-            if (w.nh == 0) continue;
-            const int ft = w.ft * 2 + (int)rank;
-            const int n = ft * BM + fr;
-            const float mul = (n < p.scale_cols) ? p.scale : 1.0f;
-            const float bias = (p.bias ? p.bias[n] : 0.0f) * ((p.epi == EPI_STORE16) ? mul : 1.0f);
-            for (int h = 0; h < w.nh; h++) {
-                mbar_wait(acc_full + 8 * h, (h ? u1 : u0) & 1);
-                tc_fence_after();
-                const int tok0 = w.tok0 + h * BN;
-                const uint32_t acc_addr = lane_addr + h * BN;
-                if (tma_out) {
-                    const int n0 = ft * BM + (warp & 3) * 32;
-                    switch (p.epi) {
-                    case EPI_GELU16: epilogue_tile_tma<EPI_GELU16, BF>(p, acc_addr, tok0, n0, bias, mul, out_stage, cidx, lane); break;
-                    case EPI_QGELU16: epilogue_tile_tma<EPI_QGELU16, BF>(p, acc_addr, tok0, n0, bias, mul, out_stage, cidx, lane); break;
-                    case EPI_REDADD32: epilogue_tile_tma<EPI_REDADD32, BF>(p, acc_addr, tok0, n0, bias, mul, out_stage, cidx, lane); break;
-                    default: epilogue_tile_tma<EPI_STORE16, BF>(p, acc_addr, tok0, n0, bias, mul, out_stage, cidx, lane); break;
-                    }
-                } else if (!(CB_DBG(p, 8))) switch (p.epi) {
-                case EPI_STORE16: epilogue_tile<EPI_STORE16, BF>(p, acc_addr, tok0, n, bias, mul); break;
-                case EPI_GELU16: epilogue_tile<EPI_GELU16, BF>(p, acc_addr, tok0, n, bias, mul); break;
-                case EPI_QGELU16: epilogue_tile<EPI_QGELU16, BF>(p, acc_addr, tok0, n, bias, mul); break;
-                case EPI_REDADD32: epilogue_tile<EPI_REDADD32, BF>(p, acc_addr, tok0, n, bias, mul); break;
-                default: epilogue_tile<EPI_STORE32, BF>(p, acc_addr, tok0, n, bias, mul); break;
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(mapa_rank0(acc_empty + 8 * h));
-            }
-            u0++;
-            if (w.nh == 2) u1++;
-        }
-        if (lane == 0) bulk_wait_group_read<0>();
-    } else if (warp >= 8) {
-        // ------------------------------------------------------------------ unpack groups: registers -> TMEM A stages (one stage per k-block,
-        // whatever the number of live halves)
-        int items = 0;
-        for (int g = first; get_work(g, n_ft, n_super, full, p.M, w); g += stride) items += (w.nh != 0);
-        const int total_kb = items * nkb;
-        const int grp = (warp - 8) >> 2;
-        const int row = (warp & 3) * 32 + lane;
-        const uint32_t a_lane = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + A_COL0;
-        uint32_t qs = grp, qph = 0, sa = grp, pa = 0;
-        for (int i = grp; i < total_kb; i += N_GROUPS) {
-            mbar_wait(q_full + 8 * qs, qph);
-            const uint32_t qa = smem_base + C::Q_OFF + qs * C::CHUNK;
-            uint32_t v[32];
-            if (!(CB_DBG(p, 1))) {
-                unpack_block<QT, BF>(qa, row, v);
-                unpack_block<QT, BF>(qa, 128 + row, v + 16);
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(q_empty + 8 * qs);
-            if (!(CB_DBG(p, 32))) mbar_wait(a_empty + 8 * sa, pa ^ 1);
-            tc_fence_after();
-            if (!(CB_DBG(p, 1))) {
-                tmem_st_32x32(a_lane + sa * 32, v);
-                tmem_st_wait();
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(mapa_rank0(a_full + 8 * sa));
-            qs += N_GROUPS; if (qs >= (uint32_t)SQ) { qs -= SQ; qph ^= 1; }
-            sa += N_GROUPS; if (sa >= (uint32_t)NA) { sa -= NA; pa ^= 1; }
-        }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 2) tmem_dealloc_2sm(tmem_base, TMEM_COLS);
+    // ---------------------------------------------------------------------- consumers
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int fr = (warp & 3) * 16 + (lane >> 2), tc = 2 * (lane & 3);   // accumulator row (feature in the group) and token column
+    uint32_t s = 0, ph = 0, qs = 0, qph = 0;
+    float acc[BN / 2];
+    uint32_t afr0[16], afr1[16];      // A fragments of two consecutive k-blocks: one is read by in-flight MMAs while the next is unpacked
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        const int ft = tile % n_ft, tt = tile / n_ft;
+        uint32_t prev = 0;
+        auto kblock = [&](uint32_t (&a)[16], uint32_t (&other)[16], int kb) {
+            if constexpr (DQ) {
+                mbar_wait(q_full + 8 * qs, qph);
+                unpack_frag<DQ ? QT : QT_Q4_0, BF>(smem_base + C::Q_OFF + qs * C::CHUNK, wg * 64 + fr, lane & 3, a);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(q_empty + 8 * qs);
+                if (++qs == SQ) { qs = 0; qph ^= 1; }
+            }
+            mbar_wait(x_full + 8 * s, ph);
+            const uint64_t db = wgmma_desc_sw128(smem_base + s * C::XS);
+            wgmma_fence();
+            if constexpr (DQ) {
+                #pragma unroll
+                for (int k = 0; k < BK / 16; k++) {
+                    const uint32_t ak[4] = {a[4 * k], a[4 * k + 1], a[4 * k + 2], a[4 * k + 3]};
+                    wgmma_rs_n192<BF>(acc, ak, db + 2 * k, (uint32_t)(kb | k));                      // B: +16 k = +32 B
+                }
+            } else {
+                const uint64_t da = wgmma_desc_sw128(smem_base + s * C::XS + X_STAGE + (uint32_t)wg * 64u * 128u);
+                #pragma unroll
+                for (int k = 0; k < BK / 16; k++) wgmma_ss_n192<BF>(acc, da + 2 * k, db + 2 * k, (uint32_t)(kb | k));
+            }
+            wgmma_commit();
+            wgmma_wait<1>();            // the MMAs of k-block kb-1 are done: release its X stage, its A fragments may be overwritten
+            fence_frag(other);
+            if (kb > 0) { __syncwarp(); if (lane == 0) mbar_arrive(x_empty + 8 * prev); }
+            prev = s;
+            if (++s == SX) { s = 0; ph ^= 1; }
+        };
+        int kb = 0;
+        for (; kb + 1 < nkb; kb += 2) { kblock(afr0, afr1, kb); kblock(afr1, afr0, kb + 1); }
+        if (kb < nkb) kblock(afr0, afr1, kb);
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        fence_frag(afr0);
+        fence_frag(afr1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(x_empty + 8 * prev);
+
+        const int tok0 = tt * BN, f = ft * BM + wg * 64 + fr;
+        float mul[2], bias[2];
+        #pragma unroll
+        for (int h = 0; h < 2; h++) {
+            mul[h] = (f + 8 * h < p.scale_cols) ? p.scale : 1.0f;
+            bias[h] = (p.bias ? p.bias[f + 8 * h] : 0.0f) * ((p.epi == EPI_STORE16) ? mul[h] : 1.0f);
+        }
+        switch (p.epi) {
+        case EPI_STORE16: epilogue_regs<EPI_STORE16, BF>(p, acc, tok0, f, tc, bias, mul); break;
+        case EPI_GELU16: epilogue_regs<EPI_GELU16, BF>(p, acc, tok0, f, tc, bias, mul); break;
+        case EPI_QGELU16: epilogue_regs<EPI_QGELU16, BF>(p, acc, tok0, f, tc, bias, mul); break;
+        case EPI_REDADD32: epilogue_regs<EPI_REDADD32, BF>(p, acc, tok0, f, tc, bias, mul); break;
+        default: epilogue_regs<EPI_STORE32, BF>(p, acc, tok0, f, tc, bias, mul); break;
+        }
+    }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -804,26 +358,11 @@ EncodeTiledFn get_encode() {
 
 template <int QT, bool BF>
 cudaError_t launch_t(const KParams& kp, int grid, cudaStream_t st) {
-    return launch_pdl(gemm_dq_kernel<QT, BF, false>, (unsigned)grid, QT == QT_F16 ? 256u : 512u, Cfg<QT>::SMEM, st, 1, kp);
-}
-template <int QT, bool BF>
-cudaError_t launch_pair_t(const KParams& kp, int grid, cudaStream_t st) {
-    return launch_pdl(gemm_dq_kernel<QT, BF, true>, (unsigned)grid, 512u, Cfg<QT, true>::SMEM, st, 2, kp);
-}
-template <int QT, bool BF>
-cudaError_t launch_wide_t(const KParams& kp, int grid, cudaStream_t st) {
-    return launch_pdl(gemm_dq2_kernel<QT, BF>, (unsigned)grid, 512u, Cfg<QT, true>::SMEM, st, 2, kp);
+    return launch_pdl(gemm_dq_kernel<QT, BF>, (unsigned)grid, (unsigned)THREADS, Cfg<QT>::SMEM, st, 1, kp);
 }
 template <int QT, bool BF>
 cudaError_t set_attr() {
-    cudaError_t e = cudaFuncSetAttribute(gemm_dq_kernel<QT, BF, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<QT>::SMEM);
-    if (e != cudaSuccess) return e;
-    if constexpr (QT != QT_F16) {
-        e = cudaFuncSetAttribute(gemm_dq_kernel<QT, BF, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<QT, true>::SMEM);
-        if (e != cudaSuccess) return e;
-        e = cudaFuncSetAttribute(gemm_dq2_kernel<QT, BF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<QT, true>::SMEM);
-    }
-    return e;
+    return cudaFuncSetAttribute(gemm_dq_kernel<QT, BF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<QT>::SMEM);
 }
 
 }  // namespace
@@ -840,32 +379,6 @@ bool make_tma_2d_16bit(TmaMap* out, const void* gptr, uint64_t rows, uint64_t co
     CUresult r = enc(reinterpret_cast<CUtensorMap*>(out), CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void*>(gptr), dims,
                      strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
-}
-
-bool make_tma_2d_16bit_plain(TmaMap* out, const void* gptr, uint64_t rows, uint64_t cols, uint64_t row_stride_elems, uint32_t box_rows,
-                             uint32_t box_cols) {
-    EncodeTiledFn enc = get_encode();
-    if (!enc) return false;
-    const cuuint64_t dims[2] = {cols, rows};
-    const cuuint64_t strides[1] = {row_stride_elems * 2};
-    const cuuint32_t box[2] = {box_cols, box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(reinterpret_cast<CUtensorMap*>(out), CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void*>(gptr), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
-}
-
-bool make_tma_2d_f32_plain(TmaMap* out, const void* gptr, uint64_t rows, uint64_t cols, uint64_t row_stride_elems, uint32_t box_rows,
-                           uint32_t box_cols) {
-    EncodeTiledFn enc = get_encode();
-    if (!enc) return false;
-    const cuuint64_t dims[2] = {cols, rows};
-    const cuuint64_t strides[1] = {row_stride_elems * 4};
-    const cuuint32_t box[2] = {box_cols, box_rows};
-    const cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(reinterpret_cast<CUtensorMap*>(out), CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(gptr), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS;
 }
 
@@ -891,51 +404,14 @@ cudaError_t gemm_launch(const GemmArgs& a, cudaStream_t stream, int num_sms, uin
     memcpy(&kp.tm_x, a.x_map, sizeof(CUtensorMap));
     if (a.w_map) memcpy(&kp.tm_w, a.w_map, sizeof(CUtensorMap));
     else memset(&kp.tm_w, 0, sizeof(CUtensorMap));
-    if (a.x_half_map) memcpy(&kp.tm_xh, a.x_half_map, sizeof(CUtensorMap));
-    else memset(&kp.tm_xh, 0, sizeof(CUtensorMap));
-    const bool epi16 = (a.epi == EPI_STORE16 || a.epi == EPI_GELU16 || a.epi == EPI_QGELU16);
-    static const bool tma_store_off = getenv("CLIP_B200_GEMM_TMA_STORE") && atoi(getenv("CLIP_B200_GEMM_TMA_STORE")) == 0;
-    kp.tma_out = (a.out_map && (epi16 || a.epi == EPI_REDADD32) && a.qtype != QT_F16 && !tma_store_off) ? 1 : 0;
-    if (kp.tma_out) memcpy(&kp.tm_out, a.out_map, sizeof(CUtensorMap));
-    else memset(&kp.tm_out, 0, sizeof(CUtensorMap));
     kp.w_packed = a.w_packed;
     kp.bias = a.bias;
     kp.out = a.out;
     kp.M = a.M; kp.N = a.N; kp.K = a.K; kp.ldo = a.ldo;
     kp.epi = a.epi; kp.scale_cols = a.scale_cols; kp.scale = a.scale;
-    static const int dbg_env = getenv("CLIP_B200_GEMM_DBG") ? atoi(getenv("CLIP_B200_GEMM_DBG")) : 0;
-    kp.dbg = dbg_env;
     const int n_tiles = (a.N / BM) * ((a.M + BN - 1) / BN);
     const int grid = n_tiles < num_sms ? n_tiles : num_sms;
     if (launches) ++*launches;
-    static const bool pair_off = getenv("CLIP_B200_GEMM_PAIR") && atoi(getenv("CLIP_B200_GEMM_PAIR")) == 0;
-    // the wide form measured SLOWER than the double-buffered pair form on every layer shape (profiles/r02_gemm_wide.md: its exposed
-    // epilogue costs more than the halved unpack work returns); kept selectable for experiments, off by default
-    const bool wide_on = getenv("CLIP_B200_GEMM_WIDE") && atoi(getenv("CLIP_B200_GEMM_WIDE")) != 0;
-    if (a.x_half_map && !pair_off && wide_on && a.qtype != QT_F16 && a.N % (2 * BM) == 0) {
-        // wide form: [256 x 384] super-tiles; worth it once every pair gets at least one of them
-        const int n_super = (a.N / (2 * BM)) * ((a.M + 2 * BN - 1) / (2 * BN));
-        int pairs = num_sms / 2;
-        if (n_super >= pairs) {
-            switch (a.qtype) {
-#define CB_WCASE(QT) case QT: return a.operand_bf16 ? launch_wide_t<QT, true>(kp, 2 * pairs, stream) : launch_wide_t<QT, false>(kp, 2 * pairs, stream);
-            CB_WCASE(QT_Q4_0) CB_WCASE(QT_Q4_1) CB_WCASE(QT_Q5_0) CB_WCASE(QT_Q5_1) CB_WCASE(QT_Q8_0)
-#undef CB_WCASE
-            default: return cudaErrorInvalidValue;
-            }
-        }
-    }
-    if (a.x_half_map && !pair_off && a.qtype != QT_F16 && a.N % (2 * BM) == 0) {
-        const int n_pairs_tiles = n_tiles / 2;
-        int pairs = num_sms / 2;
-        if (pairs > n_pairs_tiles) pairs = n_pairs_tiles;
-        switch (a.qtype) {
-#define CB_PCASE(QT) case QT: return a.operand_bf16 ? launch_pair_t<QT, true>(kp, 2 * pairs, stream) : launch_pair_t<QT, false>(kp, 2 * pairs, stream);
-        CB_PCASE(QT_Q4_0) CB_PCASE(QT_Q4_1) CB_PCASE(QT_Q5_0) CB_PCASE(QT_Q5_1) CB_PCASE(QT_Q8_0)
-#undef CB_PCASE
-        default: return cudaErrorInvalidValue;
-        }
-    }
     switch (a.qtype) {
     case QT_F16: return launch_t<QT_F16, false>(kp, grid, stream);
 #define CB_CASE(QT) case QT: return a.operand_bf16 ? launch_t<QT, true>(kp, grid, stream) : launch_t<QT, false>(kp, grid, stream);

@@ -37,8 +37,8 @@ CB_DEVINL void row_stats(Load load, int h4, int lane, float inv_h, float eps, fl
 
 // K2 LayerNorm.  One warp per row, the row lives in registers (h <= 2048): one read of x, mean and CENTRED variance as the reference
 // computes them (ggml.c:10822-10840), affine, 16-bit store.  The DELTA form (x_new = x + delta written back in fp32, delta = a 16-bit
-// branch output) is round 1's deferred residual add; since round 2 the out-proj / FC2 epilogues add into x themselves (TMA
-// reduce-add) and the model schedule always passes delta = NULL -- the form stays for callers of launch_layernorm that want it.
+// branch output) is an earlier deferred residual add; the out-proj / FC2 epilogues now add into x themselves and the model schedule
+// always passes delta = NULL -- the form stays for callers of launch_layernorm that want it.
 // MAXV = float4 per lane (row width h <= 128 * MAXV): specialised so a 1024-wide row costs 32 value registers, not 64 -- the kernel is
 // latency-bound on its loads (ncu: long_scoreboard), so resident warps per SM are what buys HBM bandwidth.
 template <bool BF, bool DELTA, int MAXV>
@@ -261,7 +261,7 @@ void launch_im2col(const float* pixels, int B, int S, int P, int kpad, void* pat
     const size_t total = (size_t)B * (S / P) * (S / P) * kpad;
     if (!total) return;
     size_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;      // grid-stride loop: 32 blocks per H100 SM
     im2col_kernel<<<(int)blocks, 256, 0, st>>>(pixels, B, S, P, kpad, (__half*)patches16);
 }
 

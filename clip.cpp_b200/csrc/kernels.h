@@ -27,22 +27,13 @@ void launch_text_embed(const int32_t* ids, const float* tok, const float* pos, i
 
 // K3 attention: softmax(Q K^T [causal]) V per (sequence, head); qkv 16-bit [nseq*T, 3*H*64] (Q pre-scaled),
 // out 16-bit [nseq*T, H*64].  head_dim is fixed at 64.  (clip.cpp:1100-1108, 1382-1388)
-// q_start (multiple of 64): first query row this launch computes (rows before it come from the tcgen05 kernel below).
-void launch_attention(const void* qkv16, void* out16, int nseq, int T, int H, int causal, int bf16, int q_start, cudaStream_t st);
+// launch_attention: warp-level mma.sync kernel (attention.cu), kept as the cross-check of the wgmma kernel (CLIP_B200_ATTN=legacy).
+void launch_attention(const void* qkv16, void* out16, int nseq, int T, int H, int causal, int bf16, cudaStream_t st);
 
-// K3 on tcgen05 (attention_tc.cu): 128-query tiles, S and O accumulators in TMEM.  map_q / map_kv16 are TMA views of the qkv matrix
-// [rows, 3*H*64] with box rows 128 / 16; the K / V boxes come from a per-launch 3-D view [sequence][token][column] of qkv16 (zero fill
-// past each sequence's T tokens).  Handles query tiles [0, attention_tc_tiles(T)); T must satisfy _supported().
-struct TmaMap;
-bool attention_tc_supported(int T);
-int attention_tc_tiles(int T);
+// K3 on wgmma (attention_tc.cu): 128-query tiles, online softmax over 128-key blocks, any T.  The Q / K / V boxes come from a
+// per-launch 3-D TMA view [sequence][token][column] of qkv16 (zero fill past each sequence's T tokens).
 cudaError_t attention_tc_init();
-cudaError_t launch_attention_tc(const TmaMap* map_q, const void* qkv16, const TmaMap* map_kv16, void* out16, int nseq, int T,
-                                int H, int causal, int bf16, int num_sms, cudaStream_t st);
-// long sequences (257 < T <= 640, non-causal; e.g. the 577 tokens of ViT-L/14@336): same data path, online softmax over 192-key blocks
-bool attention_tc_long_supported(int T, int causal);
-cudaError_t launch_attention_tc_long(const TmaMap* map_q, const void* qkv16, void* out16, int nseq, int T, int H, int bf16, int num_sms,
-                                     cudaStream_t st);
+cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T, int H, int causal, int bf16, cudaStream_t st);
 
 // K5 head tail: out[r,:] = normalize ? v / sqrt(sum v^2) : v    (clip.cpp:1163-1166, 1448-1455)
 void launch_l2norm(const float* v, float* out, int rows, int d, int normalize, cudaStream_t st);

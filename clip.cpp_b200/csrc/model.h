@@ -45,10 +45,6 @@ struct Workspace {
     int32_t* ids = nullptr;
     int32_t* last = nullptr;     // index of the EOT row per sequence (len - 1)
     TmaMap map_a, map_g, map_patches, map_sel;
-    TmaMap map_a_half, map_g_half;          // box of GEMM_BN/2 tokens: B-operand halves of the CTA-pair GEMM
-    TmaMap map_q128, map_kv16;              // views of qkv for the tcgen05 attention kernel (K / V: per-launch 3-D view)
-    TmaMap map_out_qkv, map_out_g;          // plain 32 x 32 boxes: TMA-store targets of the GEMM epilogue (16-bit)
-    TmaMap map_out_x32;                     // fp32 view of the residual stream x: TMA reduce-add target of the out-proj / FC2 epilogue
 };
 
 struct Tower {
@@ -89,7 +85,7 @@ struct clip_ctx {
     cb::Vocab vocab;
     cb::Tower vis, txt;
     bool operand_bf16 = false;   // 16-bit activation / unpacked-weight type of the towers
-    int device = 0, num_sms = 148;
+    int device = 0, num_sms = 132;
     cudaStream_t stream = nullptr, copy_stream = nullptr;
     cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_consumed[2] = {nullptr, nullptr}, ev_t0 = nullptr, ev_t1 = nullptr;
     std::vector<void*> allocs;   // every device allocation, freed in clip_free

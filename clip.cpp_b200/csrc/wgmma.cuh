@@ -1,0 +1,88 @@
+// wgmma.cuh -- warpgroup MMA (sm_90a wgmma.mma_async) wrappers used by the GEMM and attention kernels.
+//
+// A warpgroup (4 consecutive warps) computes D[64 x N] += A[64 x 16] . B[16 x N] with fp32 accumulators in registers.  Accumulator
+// fragment of thread (warp w of the group, lane l): n-tile j (8 columns) holds rows 16w + l/4 (d[4j], d[4j+1]) and 16w + l/4 + 8
+// (d[4j+2], d[4j+3]), columns 8j + 2(l%4) + {0, 1}.  Every call must sit between wgmma_fence() and wgmma_commit(); the accumulators
+// may only be read after the matching wgmma_wait().
+#pragma once
+#include "common.cuh"
+
+namespace cb {
+
+CB_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+CB_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+CB_DEVINL void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of accumulator registers across a wgmma_wait()
+template <int R>
+CB_DEVINL void wgmma_fence_regs(float (&d)[R]) {
+    #pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// Shared-memory matrix descriptor of a tile stored with the 128-byte swizzle (what TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): rows
+// of 128 B, 8-row groups 1024 B apart.  K-major operands use only the 8-row group stride; for an MN-major operand no wider than 64
+// elements the other offset is never used either, so both are 1024 B.  Tile bases are 1024-B aligned; a 16-element K step inside a
+// K-major tile advances the start address by 32 B, one inside an MN-major tile by 16 rows (2048 B).
+CB_DEVINL uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);   // start address       [0,14)
+    d |= (uint64_t)(1024 >> 4) << 16;               // leading byte offset [16,30)
+    d |= (uint64_t)(1024 >> 4) << 32;               // stride byte offset  [32,46)
+    d |= (uint64_t)1 << 62;                         // layout: 128-byte swizzle [62,64)
+    return d;
+}
+
+// D[64 x 192] (+)= A[64 x 16] . B[192 x 16]^T, both operands K-major in shared memory (descriptors), fp32 accumulators
+template <bool BF>
+CB_DEVINL void wgmma_ss_n192(float (&d)[96], uint64_t da, uint64_t db, uint32_t accumulate) {
+#define CB_WGMMA_SS_N192(TY)                                                                                 \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %98, 0;\n\t"                                                 \
+                 "wgmma.mma_async.sync.aligned.m64n192k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, %96, %97, p, 1, 1, 0, 0;\n\t}"  \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])  \
+                 : "l"(da), "l"(db), "r"(accumulate))
+    if constexpr (BF) CB_WGMMA_SS_N192("bf16");
+    else CB_WGMMA_SS_N192("f16");
+#undef CB_WGMMA_SS_N192
+}
+
+// D[64 x 192] (+)= A[64 x 16] . B[192 x 16]^T: A from registers (the m16n8k16 A-fragment layout per warp), B K-major in shared memory
+template <bool BF>
+CB_DEVINL void wgmma_rs_n192(float (&d)[96], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+#define CB_WGMMA_RSK_N192(TY)                                                                                 \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %101, 0;\n\t"                                                 \
+                 "wgmma.mma_async.sync.aligned.m64n192k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, {%96, %97, %98, %99}, %100, p, 1, 1, 0;\n\t}"  \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])  \
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate))
+    if constexpr (BF) CB_WGMMA_RSK_N192("bf16");
+    else CB_WGMMA_RSK_N192("f16");
+#undef CB_WGMMA_RSK_N192
+}
+
+// D[64 x 128] (+)= A[64 x 16] . B[128 x 16]^T, both operands K-major in shared memory (descriptors), fp32 accumulators
+template <bool BF>
+CB_DEVINL void wgmma_ss_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+#define CB_WGMMA_SS_N128(TY)                                                                                 \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %66, 0;\n\t"                                                 \
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"  \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])  \
+                 : "l"(da), "l"(db), "r"(accumulate))
+    if constexpr (BF) CB_WGMMA_SS_N128("bf16");
+    else CB_WGMMA_SS_N128("f16");
+#undef CB_WGMMA_SS_N128
+}
+
+// D[64 x 64] (+)= A[64 x 16] . B[16 x 64]: A from registers (the m16n8k16 A-fragment layout per warp), B MN-major in shared memory
+template <bool BF>
+CB_DEVINL void wgmma_rs_n64_bmn(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+#define CB_WGMMA_RS_N64(TY)                                                                                 \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %37, 0;\n\t"                                                 \
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"  \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])  \
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate))
+    if constexpr (BF) CB_WGMMA_RS_N64("bf16");
+    else CB_WGMMA_RS_N64("f16");
+#undef CB_WGMMA_RS_N64
+}
+
+}  // namespace cb

@@ -26,7 +26,7 @@
 
 namespace cb {
 
-constexpr int WPACK_ROWS = 128;   // features per tile (UMMA M)
+constexpr int WPACK_ROWS = 128;   // features per GEMM tile (two wgmma M = 64 warpgroups)
 constexpr int WPACK_K = 64;       // k per tile (one 128-B swizzle row of 16-bit operands)
 
 inline size_t wpack_chunk_bytes(int qtype) {

@@ -1,5 +1,5 @@
 /*
- * clip_b200.h -- C ABI of libclip_b200.so, the B200-native drop-in for monatis/clip.cpp's encode path.
+ * clip_b200.h -- C ABI of libclip_b200.so, the H100-native drop-in for monatis/clip.cpp's encode path.
  *
  * PART 1 re-declares, symbol for symbol and struct for struct, the reference's public interface
  * (reference: /root/reference/clip.h:8-113, 22 extern "C" functions + 8 POD structs) so that the reference's
@@ -155,7 +155,7 @@ bool clip_zero_shot_label_image(struct clip_ctx * ctx, const int n_threads, cons
 bool clip_model_quantize(const char * fname_inp, const char * fname_out, const int itype);
 
 /* =====================================================================================================
- * PART 2 -- additive B200 entry points (not in the reference)
+ * PART 2 -- additive entry points of this library (not in the reference)
  * ===================================================================================================== */
 
 /* n independent clip_text_encode calls in one launch sequence; seqs may be ragged (each <= context_length).
@@ -264,7 +264,7 @@ bool clip_b200_image_batch_preprocess_device(const struct clip_ctx * ctx, const 
 
 /* TEST HOOK: one attention launch (clip.cpp:1082-1108 / 1363-1388 semantics: softmax(Q K^T [+ causal mask]) V per head, head_dim 64).
  * qkv: fp32 host [nseq*T, 3*H*64], columns Q | K | V with the 1/sqrt(64) scale already applied to Q; out: fp32 host [nseq*T, H*64].
- * use_legacy=1 runs the warp-level mma.sync kernel instead of the tcgen05 one.  ms (optional): device time of the last of 3 launches. */
+ * use_legacy=1 runs the warp-level mma.sync kernel instead of the wgmma one.  ms (optional): device time of the last of 3 launches. */
 int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int causal, int use_legacy, const float * qkv, float * out,
                               float * ms);
 

@@ -16,6 +16,12 @@ TOK_LENS = [77, 5, 2, 33, 16, 77, 9, 64]
 TOL = {"f32": 1e-3, "f16": 1e-3, "q4_0": 1e-2, "q4_1": 1e-2, "q5_0": 1e-2, "q5_1": 1e-2, "q8_0": 1e-2}
 
 
+def reference_runs():
+    """what the reference returned for the inputs of the tests that compare against it (tests/golden/make_reference_runs.py)"""
+    z = np.load(os.path.join(GOLDEN, "reference_runs.npz"))
+    return {k: z[k] for k in z.files}
+
+
 def golden(geom):
     p = os.path.join(GOLDEN, "%s-s%d.npz" % (geom, SEED))
     if not os.path.exists(p):

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "clip.cpp_b200"), os.path.join(ROOT, "oracle"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with `-m gpu` on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a); run with `-m gpu` on a machine that has one")
     config.addinivalue_line("markers", "slow: full-size geometries")
 
 

@@ -1,6 +1,6 @@
-"""K3 (tcgen05 attention) against a numpy restatement of clip.cpp:1082-1108 / 1363-1388 (scaled Q.K^T, optional causal mask,
-soft_max ggml.c:12201-12270, .V), through the C-ABI test hook.  Includes score patterns that force the kernel's rare paths:
-the lazy exponent-offset rescale inside one half of a row pair, and the reconciliation between the two halves."""
+"""K3 (wgmma attention) against a numpy restatement of clip.cpp:1082-1108 / 1363-1388 (scaled Q.K^T, optional causal mask,
+soft_max ggml.c:12201-12270, .V), through the C-ABI test hook.  Includes score patterns whose row maximum moves from key block to key
+block, which exercises the online-softmax rescale."""
 import ctypes as C
 import numpy as np
 import pytest
@@ -91,7 +91,7 @@ def test_matches_legacy_kernel(prod):
 
 @pytest.mark.parametrize("T,causal,nseq,H", [(17, 0, 90, 4), (5, 0, 200, 2), (50, 0, 60, 12), (257, 0, 40, 8), (77, 1, 64, 8), (20, 1, 100, 3)])
 def test_many_items_per_cta(prod, T, causal, nseq, H):
-    """More (sequence, head) items than SMs: every CTA walks several items through both K/V stages and TMEM buffers."""
+    """More (sequence, head) items than SMs, several query tiles per item, both K/V ring stages."""
     rng = np.random.default_rng(T + nseq)
     qkv = rng.standard_normal((nseq * T, 3 * H * 64)).astype(np.float32)
     qkv[:, : H * 64] *= 0.3
@@ -100,7 +100,7 @@ def test_many_items_per_cta(prod, T, causal, nseq, H):
 
 @pytest.mark.parametrize("T,causal", [(300, 0), (577, 0), (100, 1)])
 def test_legacy_kernel_long_sequences(prod, T, causal):
-    """T > 257 (e.g. ViT-L/14@336: 577 tokens) is served by the warp-level mma.sync flash kernel."""
+    """the warp-level mma.sync flash kernel (the cross-check of the wgmma kernel) at T > 257 (e.g. ViT-L/14@336: 577 tokens)"""
     rng = np.random.default_rng(T)
     nseq, H = 2, 3
     qkv = rng.standard_normal((nseq * T, 3 * H * 64)).astype(np.float32)
@@ -114,8 +114,8 @@ def test_legacy_kernel_long_sequences(prod, T, causal):
 @pytest.mark.parametrize("T,nseq,H", [(258, 3, 2), (300, 2, 3), (384, 2, 2), (385, 2, 2), (577, 2, 3), (577, 40, 16), (640, 1, 2)])
 @pytest.mark.parametrize("bf", [1, 0])
 def test_long_sequences_on_tcgen05(prod, T, nseq, H, bf):
-    """257 < T <= 640 (ViT-L/14@336: 577 tokens): the long-sequence tcgen05 kernel -- online softmax over 192-key blocks, K / V resident per
-    item, several items per CTA in the (577, 40, 16) case -- against the numpy restatement and against the warp-level kernel it replaces."""
+    """257 < T <= 640 (ViT-L/14@336: 577 tokens): the wgmma kernel over several 128-key blocks, ragged last block, many (sequence, head)
+    items in the (577, 40, 16) case -- against the numpy restatement and against the warp-level kernel."""
     rng = np.random.default_rng(T + nseq)
     qkv = rng.standard_normal((nseq * T, 3 * H * 64)).astype(np.float32)
     qkv[:, : H * 64] *= 0.3

@@ -1,4 +1,4 @@
-"""K1 in isolation: the fused block-dequant tcgen05 GEMM through the C-ABI test hook, against a numpy restatement
+"""K1 in isolation: the fused block-dequant wgmma GEMM through the C-ABI test hook, against a numpy restatement
 built on the ORACLE's dequantizer (ggml.c:1496-1606 semantics).  The comparison emulates the kernel's declared
 rounding points exactly -- operands rounded to fp16/bf16, fp32 accumulation -- so the tolerance can be tight."""
 import ctypes as C
@@ -156,7 +156,7 @@ def test_gemm_token_tails_and_multi_tile(prod, M):
 
 
 def test_gemm_matches_scalar_debug_kernel(prod):
-    """tcgen05 path vs the scalar kernel that dequantises straight from ggml-format rows on the device."""
+    """wgmma path vs the scalar kernel that dequantises straight from ggml-format rows on the device."""
     rng = np.random.default_rng(4)
     M, N, K = 513, 256, 1024
     raw, _ = make_weight("q5_1", N, K, rng)
@@ -168,7 +168,7 @@ def test_gemm_matches_scalar_debug_kernel(prod):
 
 
 def test_gemm_large_persistent(prod):
-    """More tiles than SMs (persistent loop, TMEM double buffering, ring wrap-around) at a ViT-L/14 layer shape."""
+    """More tiles than SMs (persistent loop, ring wrap-around, A-buffer reuse across tiles) at a ViT-L/14 layer shape."""
     rng = np.random.default_rng(5)
     M, N, K = 257 * 40, 1024, 1024
     raw, deq = make_weight("q4_0", N, K, rng)
@@ -179,29 +179,11 @@ def test_gemm_large_persistent(prod):
     print("gemm %dx%dx%d q4_0: %.3f ms  %.1f TFLOP/s" % (M, N, K, ms, 2.0 * M * N * K / ms / 1e9))
 
 
-@pytest.mark.parametrize("epi", [EPI_STORE16, EPI_QGELU16, EPI_REDADD32])
-def test_gemm_direct_store_epilogue_still_matches(prod, epi, monkeypatch):
-    """16-bit epilogues normally leave through shared memory + TMA store; the direct 2-byte store path (no output tensor map, e.g.
-    an output buffer the caller did not describe) must give the same bits."""
-    rng = np.random.default_rng(8)
-    M, N, K = 333, 256, 256
-    raw, deq = make_weight("q4_0", N, K, rng)
-    x = rng.standard_normal((M, K)).astype(np.float32)
-    bias = rng.standard_normal(N).astype(np.float32)
-    resid = rng.standard_normal((M, N)).astype(np.float32)
-    a, _ = run_gemm(prod, "q4_0", True, M, N, K, epi, x, raw, bias, resid)
-    monkeypatch.setenv("CLIP_B200_DEBUG_DIRECT_STORE", "1")
-    b, _ = run_gemm(prod, "q4_0", True, M, N, K, epi, x, raw, bias, resid)
-    assert np.array_equal(a, b)
-
-
 @pytest.mark.parametrize("qt,bf16", [(qt, bf) for qt in ("q4_0", "q4_1", "q5_0", "q5_1", "q8_0") for bf in (True, False)])
-def test_gemm_wide_form_all_types(prod, qt, bf16, monkeypatch):
-    """Enough [256 x 384] super-tiles for every CTA pair -> the WIDE kernel (both accumulators live, 8 UMMAs per A stage).  M is chosen
-    so that the last super-tile has a ragged first half only and the tail of the work list is walked as half items."""
-    monkeypatch.setenv("CLIP_B200_GEMM_WIDE", "1")
+def test_gemm_wide_form_all_types(prod, qt, bf16):
+    """Every weight type over more tiles than SMs (each CTA walks several tiles, rings wrap around), with a ragged last token tile."""
     rng = np.random.default_rng(21)
-    M, N, K = 37 * 384 + 100, 512, 128           # 2 feature-pair tiles x 38 super-tiles = 76 >= 74 pairs
+    M, N, K = 37 * 384 + 100, 512, 128           # 4 feature tiles x 74 token tiles = 296 tiles: > 2 per CTA on 132 SMs
     raw, deq = make_weight(qt, N, K, rng)
     x = rng.standard_normal((M, K)).astype(np.float32)
     bias = rng.standard_normal(N).astype(np.float32)
@@ -212,9 +194,8 @@ def test_gemm_wide_form_all_types(prod, qt, bf16, monkeypatch):
 
 @pytest.mark.parametrize("M", [74 * 384, 74 * 384 + 1, 75 * 384 - 191, 75 * 384 + 193, 111 * 384 + 7])
 @pytest.mark.parametrize("epi", [EPI_STORE16, EPI_QGELU16, EPI_REDADD32])
-def test_gemm_wide_form_tails_and_epilogues(prod, M, epi, monkeypatch):
-    """wide kernel: exact multiples, one extra row, a lone first half, a ragged second half, 1.5 waves; 16-bit epilogues via TMA store"""
-    monkeypatch.setenv("CLIP_B200_GEMM_WIDE", "1")
+def test_gemm_wide_form_tails_and_epilogues(prod, M, epi):
+    """many token tiles: exact multiples of the tile, one extra row, ragged last tiles, partial last waves; 16-bit and residual epilogues"""
     rng = np.random.default_rng(M)
     N, K = 256, 192
     raw, deq = make_weight("q4_0", N, K, rng)

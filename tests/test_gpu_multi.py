@@ -1,4 +1,4 @@
-"""Multi-GPU inside the library (SURVEY.md section 8e), needs >= 2 B200s (`gpurun --gpus 2 -- python -m pytest tests -m gpu -k multi`):
+"""Multi-GPU inside the library (SURVEY.md section 8e), needs >= 2 H100s (`python -m pytest tests -m gpu -k multi`; skips on one GPU):
   * devices mode -- CLIP_B200_DEVICES at clip_model_load, one context drives every GPU, results identical to one GPU;
   * ranks mode   -- one process per GPU, NCCL communicator built by the library from the launcher's environment (no torch),
                     clip_b200_*_all return every rank's embeddings in rank order."""

@@ -1,5 +1,5 @@
 """Scoring entry points of the C ABI on the GPU: clip_compare_text_and_image (clip.cpp:1534-1571) and clip_zero_shot_label_image
-(clip.cpp:1624-1659) against the LIVE reference (oracle/_ref, one model per process), the device similarity / softmax / top-k
+(clip.cpp:1624-1659) against what the reference returned (tests/golden/reference_runs.npz), the device similarity / softmax / top-k
 kernels against numpy restatements of softmax_with_sorting (clip.cpp:1591-1622), the batched zero-shot call, the device-resident
 text entry point, and pinned vs pageable caller buffers."""
 import ctypes as C
@@ -7,9 +7,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import ref_run
 import synth_gguf as sg
-from _util import model_file, one_minus_cos, token_seqs
+from _util import check_sha, model_file, one_minus_cos, reference_runs, token_seqs
 
 pytestmark = pytest.mark.gpu
 
@@ -21,6 +20,10 @@ def _u8(nx, ny, seed):
     base = rng.integers(0, 256, (ny // 8 + 2, nx // 8 + 2, 3)).astype(np.float32)
     img = np.kron(base, np.ones((8, 8, 1), np.float32))[:ny, :nx] + rng.normal(0, 10, (ny, nx, 3))
     return np.clip(img, 0, 255).astype(np.uint8)
+
+
+def live_u8():
+    return _u8(120, 90, 5)
 
 
 def _softmax_sorted(s):
@@ -37,12 +40,13 @@ def _softmax_sorted(s):
 SCORE_TOL = {"f16": 5e-3, "q4_0": 1e-1}
 
 
-@pytest.mark.skipif(not ref_run.available(), reason="oracle/_ref not built")
 @pytest.mark.parametrize("ft", ["f16", "q4_0"])
 def test_compare_and_zero_shot_label_match_live_reference(prod, ft):
     path = model_file("tiny", ft, prod)
-    u8 = _u8(120, 90, 5)
-    ref = ref_run.run_reference(path, u8_image=u8, texts=TEXTS, n_threads=4)
+    u8 = live_u8()
+    r = reference_runs()
+    check_sha(path, r["scoring_%s_sha" % ft])
+    ref = {k: r["scoring_%s_%s" % (ft, k)] for k in ("cmp", "zsl_scores", "zsl_idx")}
     ctx = prod.load(path, 0)
     try:
         got_cmp = np.array([prod.compare_text_and_image(ctx, t, u8) for t in TEXTS], np.float32)

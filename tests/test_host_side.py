@@ -1,6 +1,5 @@
 """Host-side members of the interface (no GPU): file quantizer, weight re-tiling, tokenizer, preprocess -- each
-checked bit-exactly against vectors produced by the reference (tests/golden, oracle/_ref) and, when the reference
-library is present, against it live."""
+checked bit-exactly against vectors produced by the reference (tests/golden, made with oracle/_ref)."""
 import ctypes as C
 import hashlib
 import json
@@ -12,7 +11,7 @@ import pytest
 import binding as bd
 import ref_run
 import synth_gguf as sg
-from _util import FTYPES, GOLDEN, check_sha, golden, model_file
+from _util import FTYPES, GOLDEN, check_sha, golden, model_file, reference_runs
 
 HOST = json.load(open(os.path.join(GOLDEN, "host_ops.json")))
 
@@ -86,21 +85,21 @@ def test_preprocess_matches_reference_golden_bit_exactly(prod):
         assert hashlib.sha256(out.tobytes()).hexdigest() == e["sha256"], e
 
 
-@pytest.mark.skipif(not ref_run.available(), reason="oracle/_ref not built")
+LIVE_TEXTS = ["the red apple isn't a dog", "  double  spaces and 42 numbers!!", "mixed'case I'LL"]
+
+
+def live_u8():
+    return _synth_u8(123, 77, 99)
+
+
 def test_tokenizer_and_preprocess_match_live_reference(prod):
-    import subprocess, sys, tempfile
+    """tokens and preprocess output the reference returned for these inputs (tests/golden/reference_runs.npz)"""
     model = model_file("tiny", "f16", prod)
-    texts = ["the red apple isn't a dog", "  double  spaces and 42 numbers!!", "mixed'case I'LL"]
-    u8 = _synth_u8(123, 77, 99)
-    code = ("import sys, json, numpy as np; sys.path.insert(0, %r); sys.path.insert(0, %r); import binding as bd, ref_run; r = bd.ClipLib(ref_run.REF_LIB); c = r.load(%r, 0);"
-            "print(json.dumps({'tok': [[int(v) for v in r.tokenize(c, t)] for t in %r], 'pre': r.preprocess(c, np.load(sys.argv[1])).ravel().tolist()}))"
-            % (os.path.join(os.path.dirname(GOLDEN), "..", "clip.cpp_b200"), os.path.join(os.path.dirname(GOLDEN), "..", "oracle"), model, texts))
-    with tempfile.NamedTemporaryFile(suffix=".npy") as f:
-        np.save(f.name, u8)
-        res = json.loads(subprocess.run([sys.executable, "-c", code, f.name], capture_output=True, text=True, check=True).stdout.strip().splitlines()[-1])
-    for t, ids in zip(texts, res["tok"]):
-        assert _tokenize(prod, model, t) == ids
-    assert np.array_equal(_preprocess(prod, u8).ravel(), np.array(res["pre"], np.float32))
+    check_sha(model, HOST["model_sha"])
+    r = reference_runs()
+    for i, t in enumerate(LIVE_TEXTS):
+        assert _tokenize(prod, model, t) == r["tok_%d" % i].tolist(), repr(t)
+    assert np.array_equal(_preprocess(prod, live_u8()), r["preprocess"])
 
 
 def test_scoring_helpers_match_reference_arithmetic(prod):
@@ -151,19 +150,23 @@ def test_png_decode_matches_pil_and_rejects_unknown_formats(prod, tmp_path):
     assert _load_file(prod, g) is None and b"supported formats" in prod.lib.clip_b200_last_error()
 
 
-@pytest.mark.skipif(not ref_run.available(), reason="oracle/_ref not built")
-def test_png_decode_matches_live_reference(prod, tmp_path):
-    Image = pytest.importorskip("PIL.Image")
+def live_pngs():
+    from PIL import Image
     rng = np.random.default_rng(1)
-    ref = bd.ClipLib(ref_run.REF_LIB)
-    ims = {"g16.png": Image.fromarray(rng.integers(0, 65536, (11, 13), dtype=np.uint16)),
-           "la.png": Image.fromarray(rng.integers(0, 256, (20, 31, 2), dtype=np.uint8), "LA"),
-           "rgb.png": Image.fromarray(rng.integers(0, 256, (64, 48, 3), dtype=np.uint8))}
-    for name, im in ims.items():
+    return {"g16.png": Image.fromarray(rng.integers(0, 65536, (11, 13), dtype=np.uint16)),
+            "la.png": Image.fromarray(rng.integers(0, 256, (20, 31, 2), dtype=np.uint8), "LA"),
+            "rgb.png": Image.fromarray(rng.integers(0, 256, (64, 48, 3), dtype=np.uint8))}
+
+
+def test_png_decode_matches_live_reference(prod, tmp_path):
+    """PNG decode against the reference's pixels for the same (lossless) files (tests/golden/reference_runs.npz)"""
+    pytest.importorskip("PIL.Image")
+    r = reference_runs()
+    for name, im in live_pngs().items():
         p = str(tmp_path / name)
         im.save(p)
-        a, b = _load_file(prod, p), _load_file(ref, p)
-        assert a is not None and b is not None and np.array_equal(a, b), name
+        a = _load_file(prod, p)
+        assert a is not None and np.array_equal(a, r["png_" + name]), name
 
 
 def _write_png(path, arr, ctype, depth, interlace=False, palette=None):
@@ -489,31 +492,44 @@ def test_jpeg_decode_matches_reference_golden(prod):
         assert hashlib.sha256(got.tobytes()).hexdigest() == want["sha256"], (name, float(got.mean()), want["mean"])
 
 
-@pytest.mark.skipif(not ref_run.available(), reason="oracle/_ref not built")
-def test_jpeg_decode_matches_live_reference(prod, tmp_path):
-    """Same comparison against the reference library itself on freshly written files (sizes x sampling x mode x quality), and on the
-    two sample JPEGs the reference ships when its tree is present."""
-    Image = pytest.importorskip("PIL.Image")
+def live_jpeg_cases(tmp):
+    """(key, path) of every file of the comparison below: freshly written by PIL (sizes x sampling x mode x quality), then the two
+    sample JPEGs the reference ships (copied to tests/golden/jpeg/reference_*.jpg)."""
+    from PIL import Image
     rng = np.random.default_rng(5)
-    ref = bd.ClipLib(ref_run.REF_LIB)
-    p = str(tmp_path / "t.jpg")
+    p = os.path.join(tmp, "t.jpg")
     n = 0
     for (w, h) in [(1, 1), (8, 8), (15, 9), (33, 17), (100, 75), (224, 224), (1234, 901)]:       # the last one is > 1 MP: threaded IDCT / colour rows
         y, x = np.mgrid[0:h, 0:w]
         pics = [rng.integers(0, 256, (h, w, 3), dtype=np.uint8),
                 np.stack([np.sin(x / 3.0) * 127 + 128, np.cos(y / 5.0) * 127 + 128, ((x // 4 + y // 4) % 2) * 255], -1).astype(np.uint8)]
-        for pic in pics:
+        for k, pic in enumerate(pics):
             for sub in ("4:4:4", "4:2:2", "4:2:0"):
                 for prog in (False, True):
                     q = int(rng.integers(5, 100))
                     Image.fromarray(pic).save(p, quality=q, subsampling=sub, progressive=prog, optimize=bool(n & 1))
-                    a, b = _load_file(prod, p), _load_file(ref, p)
-                    assert a is not None and b is not None and np.array_equal(a, b), (w, h, sub, prog, q)
+                    yield "%dx%d_%d_%s_%d_q%d" % (w, h, k, sub, prog, q), p
                     n += 1
-    for f in ("/root/reference/tests/red_apple.jpg", "/root/reference/tests/white.jpg"):
-        if os.path.exists(f):
-            a, b = _load_file(prod, f), _load_file(ref, f)
-            assert a is not None and np.array_equal(a, b), f
+    for name in ("red_apple", "white"):
+        yield name, os.path.join(JPEG_GOLDEN, "reference_%s.jpg" % name)
+
+
+def test_jpeg_decode_matches_live_reference(prod, tmp_path):
+    """Same comparison on freshly written files and the reference's two sample JPEGs: the sha256 of each input file and of the pixels
+    the reference decoded from it are stored in tests/golden/reference_runs.npz."""
+    import hashlib
+    pytest.importorskip("PIL.Image")
+    r = reference_runs()
+    want = dict(zip(r["jpeg_keys"].tolist(), zip(r["jpeg_file_sha"].tolist(), r["jpeg_ref_sha"].tolist())))
+    n = 0
+    for key, p in live_jpeg_cases(str(tmp_path)):
+        file_sha, ref_sha = want[key]
+        assert hashlib.sha256(open(p, "rb").read()).hexdigest() == file_sha, \
+            (key, "PIL wrote a different file than the one the fixture was made from: re-run tests/golden/make_reference_runs.py")
+        a = _load_file(prod, p)
+        assert a is not None and hashlib.sha256(a.tobytes()).hexdigest() == ref_sha, key
+        n += 1
+    assert n == len(want)
 
 
 def test_jpeg_decoder_survives_corrupt_files(prod, tmp_path):

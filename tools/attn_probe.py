@@ -16,4 +16,4 @@ for i in range(3):
     assert rc == 0, lib.last_error()
     best = min(best, ms.value)
 flops = 4.0 * nseq * H * T * T * 64
-print("nseq=%d T=%d H=%d %s: %.1f us  %.0f TFLOP/s" % (nseq, T, H, "mma.sync kernel" if legacy else "tcgen05 kernel", best * 1e3, flops / best / 1e9))
+print("nseq=%d T=%d H=%d %s: %.1f us  %.0f TFLOP/s" % (nseq, T, H, "mma.sync kernel" if legacy else "wgmma kernel", best * 1e3, flops / best / 1e9))

@@ -1,7 +1,7 @@
 """Host-side members of the interface timed next to the reference's own implementation (no GPU involved): clip_image_load_from_file
 (JPEG) and clip_image_preprocess's arithmetic.  Needs oracle/_ref/libclip_ref.so (make -C oracle ref) and PIL for the test images.
 
-    python tools/host_timing.py            -> the table in profiles/r02_host_side.md
+    python tools/host_timing.py            -> a markdown table on stdout
 """
 import ctypes as C
 import os
