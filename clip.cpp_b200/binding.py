@@ -76,6 +76,9 @@ EXTENSION_SYMBOLS = [
     "clip_b200_dist_barrier", "clip_b200_dist_max_f64", "clip_b200_dist_all_gather", "clip_b200_image_encode_device_all",
     "clip_b200_text_encode_device_all", "clip_b200_image_batch_encode_all", "clip_b200_text_batch_encode_all",
     "clip_b200_debug_rendezvous", "clip_b200_debug_shard_bounds",
+    # row-kernel test hooks
+    "clip_b200_debug_layernorm", "clip_b200_debug_assemble_preln", "clip_b200_debug_im2col", "clip_b200_debug_text_embed",
+    "clip_b200_debug_gather_rows", "clip_b200_debug_l2norm", "clip_b200_debug_fill_last",
 ]
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -180,6 +183,16 @@ class ClipLib:
             L.clip_b200_debug_attention.argtypes = [ip, ip, ip, ip, ip, ip, fp, fp, C.POINTER(C.c_float)]
             L.clip_b200_debug_gemm.restype = C.c_int
             L.clip_b200_debug_gemm.argtypes = [ip, ip, ip, ip, ip, ip, ip, fp, vp, fp, fp, fp, C.POINTER(C.c_float)]
+            i32p = C.POINTER(C.c_int32)
+            for f, args in (("clip_b200_debug_layernorm", [ip, ip, C.c_size_t, C.c_float, fp, fp, fp, fp, ip, fp, fp]),
+                            ("clip_b200_debug_assemble_preln", [fp, fp, fp, ip, ip, ip, C.c_float, fp, fp, fp]),
+                            ("clip_b200_debug_im2col", [fp, ip, ip, ip, ip, fp]),
+                            ("clip_b200_debug_text_embed", [i32p, fp, fp, ip, ip, ip, ip, fp]),
+                            ("clip_b200_debug_gather_rows", [fp, ip, ip, ip, ip, i32p, fp, ip, fp]),
+                            ("clip_b200_debug_l2norm", [fp, ip, ip, ip, fp]),
+                            ("clip_b200_debug_fill_last", [i32p, ip, ip, i32p])):
+                getattr(L, f).restype = C.c_int
+                getattr(L, f).argtypes = args
             ipp = C.POINTER(C.c_int)
             L.clip_b200_topk_search.restype = C.c_bool
             L.clip_b200_topk_search.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, ip, fp, ipp]

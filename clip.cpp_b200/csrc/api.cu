@@ -1535,6 +1535,193 @@ int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int caus
     return rc;
 }
 
+}  // extern "C"
+
+namespace {
+// Device buffers and a private stream on device 0 for the row-kernel test hooks; everything is released when it goes out of scope.
+struct HookScratch {
+    std::vector<void*> bufs;
+    cudaStream_t st = nullptr;
+    bool ok = true;
+    HookScratch() {
+        cudaError_t e = cudaSetDevice(0);
+        if (e == cudaSuccess) e = cudaStreamCreate(&st);
+        if (e != cudaSuccess) { set_err(std::string("hook setup: ") + cudaGetErrorString(e)); ok = false; }
+    }
+    ~HookScratch() {
+        for (void* p : bufs) cudaFree(p);
+        if (st) cudaStreamDestroy(st);
+    }
+    // `bytes` of device memory, every byte set to `fill` (0xff poisons: NaN in fp32, fp16 and bf16), then `src` copied to its start
+    void* alloc(size_t bytes, int fill, const void* src = nullptr, size_t src_bytes = 0) {
+        if (!ok) return nullptr;
+        void* d = nullptr;
+        cudaError_t e = cudaMalloc(&d, std::max<size_t>(bytes, 256));
+        if (e == cudaSuccess) bufs.push_back(d);
+        if (e == cudaSuccess) e = cudaMemset(d, fill, std::max<size_t>(bytes, 256));
+        if (e == cudaSuccess && src && src_bytes) e = cudaMemcpy(d, src, src_bytes, cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) { set_err(std::string("hook alloc: ") + cudaGetErrorString(e)); ok = false; return nullptr; }
+        return d;
+    }
+    // the launch's own error, then the kernel's
+    bool finish(const char* what) {
+        if (!ok) return false;
+        cudaError_t e = cudaGetLastError();
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) { set_err(std::string(what) + ": " + cudaGetErrorString(e)); ok = false; }
+        return ok;
+    }
+    bool copy_back(void* dst, const void* src, size_t bytes) {
+        if (!ok) return false;
+        cudaError_t e = cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost);
+        if (e != cudaSuccess) { set_err(std::string("hook copy back: ") + cudaGetErrorString(e)); ok = false; }
+        return ok;
+    }
+};
+
+std::vector<uint16_t> to16(const float* x, size_t n, int bf16) {
+    std::vector<uint16_t> o(n);
+    for (size_t i = 0; i < n; i++) o[i] = bf16 ? f32_to_bf16(x[i]) : f32_to_f16(x[i]);
+    return o;
+}
+void from16(const uint16_t* x, size_t n, int bf16, float* out) {
+    for (size_t i = 0; i < n; i++) {
+        if (bf16) { uint32_t b = (uint32_t)x[i] << 16; memcpy(&out[i], &b, 4); }
+        else out[i] = f16_to_f32(x[i]);
+    }
+}
+}  // namespace
+
+extern "C" {
+
+int clip_b200_debug_layernorm(int rows, int h, size_t in_stride, float eps, const float* x, const float* gamma, const float* beta,
+                              const float* delta, int operand_bf16, float* y_out, float* x_out) {
+    g_err.clear();
+    if (rows <= 0 || h <= 0 || h % 4 || h > 2048 || in_stride < (size_t)h || in_stride % 4) { set_err("debug_layernorm: bad shape"); return 1; }
+    HookScratch s;
+    const size_t span = ((size_t)rows - 1) * in_stride + h, hb = (size_t)h * 4;
+    float* d_x = (float*)s.alloc(span * 4, 0xff);
+    uint16_t* d_delta = nullptr;
+    if (delta) {
+        const std::vector<uint16_t> d16 = to16(delta, (size_t)rows * h, operand_bf16);
+        d_delta = (uint16_t*)s.alloc(span * 2, 0xff);
+        if (s.ok && cudaMemcpy2D(d_delta, in_stride * 2, d16.data(), (size_t)h * 2, (size_t)h * 2, rows, cudaMemcpyHostToDevice) != cudaSuccess) {
+            set_err("debug_layernorm: upload delta");
+            return 3;
+        }
+    }
+    float* d_g = (float*)s.alloc(hb, 0, gamma, hb);
+    float* d_b = (float*)s.alloc(hb, 0, beta, hb);
+    uint16_t* d_y = (uint16_t*)s.alloc((size_t)rows * h * 2, 0xff);
+    if (s.ok && cudaMemcpy2D(d_x, in_stride * 4, x, hb, hb, rows, cudaMemcpyHostToDevice) != cudaSuccess) { set_err("debug_layernorm: upload"); return 3; }
+    if (!s.ok) return 3;
+    launch_layernorm(d_x, in_stride, rows, h, eps, d_g, d_b, d_delta, d_y, operand_bf16, s.st);
+    if (!s.finish("layernorm")) return 5;
+    std::vector<uint16_t> y16((size_t)rows * h);
+    if (!s.copy_back(y16.data(), d_y, y16.size() * 2)) return 6;
+    from16(y16.data(), y16.size(), operand_bf16, y_out);
+    if (x_out && cudaMemcpy2D(x_out, hb, d_x, in_stride * 4, hb, rows, cudaMemcpyDeviceToHost) != cudaSuccess) { set_err("debug_layernorm: copy back x"); return 6; }
+    return 0;
+}
+
+int clip_b200_debug_assemble_preln(const float* patch, const float* class_embd, const float* pos, int B, int T, int h, float eps,
+                                   const float* gamma, const float* beta, float* x_out) {
+    g_err.clear();
+    if (B <= 0 || T < 2 || h <= 0 || h % 4) { set_err("debug_assemble_preln: bad shape"); return 1; }
+    HookScratch s;
+    const size_t hb = (size_t)h * 4, np = (size_t)B * (T - 1);
+    float* d_patch = (float*)s.alloc(np * hb, 0, patch, np * hb);
+    float* d_cls = (float*)s.alloc(hb, 0, class_embd, hb);
+    float* d_pos = (float*)s.alloc((size_t)T * hb, 0, pos, (size_t)T * hb);
+    float* d_g = (float*)s.alloc(hb, 0, gamma, hb);
+    float* d_b = (float*)s.alloc(hb, 0, beta, hb);
+    float* d_x = (float*)s.alloc((size_t)B * T * hb, 0xff);
+    if (!s.ok) return 3;
+    launch_assemble_preln(d_patch, d_cls, d_pos, B, T, h, eps, d_g, d_b, d_x, s.st);
+    if (!s.finish("assemble_preln")) return 5;
+    return s.copy_back(x_out, d_x, (size_t)B * T * hb) ? 0 : 6;
+}
+
+int clip_b200_debug_im2col(const float* pixels, int B, int S, int P, int kpad, float* out) {
+    g_err.clear();
+    if (B <= 0 || P <= 0 || S % P || kpad < 3 * P * P) { set_err("debug_im2col: bad shape"); return 1; }
+    HookScratch s;
+    const size_t pb = (size_t)B * S * S * 3 * 4, n = (size_t)B * (S / P) * (S / P) * kpad;
+    float* d_px = (float*)s.alloc(pb, 0, pixels, pb);
+    uint16_t* d_out = (uint16_t*)s.alloc(n * 2, 0xff);
+    if (!s.ok) return 3;
+    launch_im2col(d_px, B, S, P, kpad, d_out, s.st);
+    if (!s.finish("im2col")) return 5;
+    std::vector<uint16_t> o16(n);
+    if (!s.copy_back(o16.data(), d_out, n * 2)) return 6;
+    from16(o16.data(), n, 0, out);
+    return 0;
+}
+
+int clip_b200_debug_text_embed(const int32_t* ids, const float* tok, const float* pos, int nseq, int T, int h, int n_vocab, float* x_out) {
+    g_err.clear();
+    if (nseq <= 0 || T <= 0 || h <= 0 || h % 4 || n_vocab <= 0) { set_err("debug_text_embed: bad shape"); return 1; }
+    HookScratch s;
+    const size_t hb = (size_t)h * 4, rows = (size_t)nseq * T;
+    int32_t* d_ids = (int32_t*)s.alloc(rows * 4, 0, ids, rows * 4);
+    float* d_tok = (float*)s.alloc((size_t)n_vocab * hb, 0, tok, (size_t)n_vocab * hb);
+    float* d_pos = (float*)s.alloc((size_t)T * hb, 0, pos, (size_t)T * hb);
+    float* d_x = (float*)s.alloc(rows * hb, 0xff);
+    if (!s.ok) return 3;
+    launch_text_embed(d_ids, d_tok, d_pos, nseq, T, h, n_vocab, d_x, s.st);
+    if (!s.finish("text_embed")) return 5;
+    return s.copy_back(x_out, d_x, rows * hb) ? 0 : 6;
+}
+
+int clip_b200_debug_gather_rows(const float* src, int src_rows, int rows, int h, int stride_rows, const int32_t* offs,
+                                const float* delta, int operand_bf16, float* out) {
+    g_err.clear();
+    if (src_rows <= 0 || rows <= 0 || h <= 0 || h % 4) { set_err("debug_gather_rows: bad shape"); return 1; }
+    for (int r = 0; r < rows; r++) {
+        const long long i = (long long)r * stride_rows + (offs ? offs[r] : 0);
+        if (i < 0 || i >= src_rows) { set_err("debug_gather_rows: row index out of range"); return 1; }
+    }
+    HookScratch s;
+    const size_t hb = (size_t)h * 4, sn = (size_t)src_rows * h;
+    float* d_src = (float*)s.alloc(sn * 4, 0, src, sn * 4);
+    int32_t* d_offs = offs ? (int32_t*)s.alloc((size_t)rows * 4, 0, offs, (size_t)rows * 4) : nullptr;
+    uint16_t* d_delta = nullptr;
+    if (delta) {
+        const std::vector<uint16_t> d16 = to16(delta, sn, operand_bf16);
+        d_delta = (uint16_t*)s.alloc(sn * 2, 0, d16.data(), sn * 2);
+    }
+    float* d_out = (float*)s.alloc((size_t)rows * hb, 0xff);
+    if (!s.ok) return 3;
+    launch_gather_rows(d_src, d_out, rows, h, stride_rows, d_offs, d_delta, operand_bf16, s.st);
+    if (!s.finish("gather_rows")) return 5;
+    return s.copy_back(out, d_out, (size_t)rows * hb) ? 0 : 6;
+}
+
+int clip_b200_debug_l2norm(const float* v, int rows, int d, int normalize, float* out) {
+    g_err.clear();
+    if (rows <= 0 || d <= 0) { set_err("debug_l2norm: bad shape"); return 1; }
+    HookScratch s;
+    const size_t n = (size_t)rows * d * 4;
+    float* d_v = (float*)s.alloc(n, 0, v, n);
+    float* d_out = (float*)s.alloc(n, 0xff);
+    if (!s.ok) return 3;
+    launch_l2norm(d_v, d_out, rows, d, normalize, s.st);
+    if (!s.finish("l2norm")) return 5;
+    return s.copy_back(out, d_out, n) ? 0 : 6;
+}
+
+int clip_b200_debug_fill_last(const int32_t* lens, int n, int seq_len, int32_t* last) {
+    g_err.clear();
+    if (n <= 0 || seq_len <= 0) { set_err("debug_fill_last: bad shape"); return 1; }
+    HookScratch s;
+    int32_t* d_lens = lens ? (int32_t*)s.alloc((size_t)n * 4, 0, lens, (size_t)n * 4) : nullptr;
+    int32_t* d_last = (int32_t*)s.alloc((size_t)n * 4, 0xff);
+    if (!s.ok) return 3;
+    launch_fill_last(d_lens, d_last, n, seq_len, s.st);
+    if (!s.finish("fill_last")) return 5;
+    return s.copy_back(last, d_last, (size_t)n * 4) ? 0 : 6;
+}
+
 
 // ---- CPU-only test hooks (no context / GPU needed) ----------------------------------------------------------
 // ranks-mode rendezvous of the NCCL unique id (dist.cpp) without a GPU: rank 0 publishes, the others read the same 128 bytes

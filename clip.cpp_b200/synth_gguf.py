@@ -84,6 +84,10 @@ GEOMETRIES = {
     # ViT-L/14@336 token count (24*24 + 1 = 577 > 257: the long-sequence attention path) at small width
     "small-p14-336": Geometry("small-p14-336", image_size=336, patch_size=14, v_hidden=128, v_ff=256, v_heads=2,
                               v_layers=12, t_hidden=128, t_ff=256, t_heads=2, t_layers=12, proj_dim=128),
+    # ViT-H/14 width (1280 > 1024: the 16-float4-per-lane LayerNorm) in both towers, FC2 depth 5120, patch 14 (kpad 640), only
+    # 2 layers; ~300 MB as f16
+    "wide-h1280": Geometry("wide-h1280", image_size=112, patch_size=14, v_hidden=1280, v_ff=5120, v_heads=20, v_layers=2,
+                           t_hidden=1280, t_ff=5120, t_heads=20, t_layers=2, proj_dim=1024),
 }
 
 

@@ -268,6 +268,31 @@ bool clip_b200_image_batch_preprocess_device(const struct clip_ctx * ctx, const 
 int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int causal, int use_legacy, const float * qkv, float * out,
                               float * ms);
 
+/* TEST HOOKS for the row kernels (csrc/kernels.cu): each runs one launcher on a private stream on device 0 and returns 0 on
+ * success (clip_b200_last_error says why not).  Host buffers are fp32 / int32; 16-bit inputs are rounded to the operand type
+ * (operand_bf16) on the way in and 16-bit outputs come back widened to fp32.  Device outputs start poisoned (all bits set).
+ *
+ * LayerNorm over rows x h of x (host [rows, h], placed on the device at row stride in_stride >= h with the gaps poisoned);
+ * delta (host [rows, h] or NULL) selects the form that first adds the 16-bit residual branch into x.  y_out [rows, h];
+ * x_out [rows, h] (optional): x after the kernel. */
+int clip_b200_debug_layernorm(int rows, int h, size_t in_stride, float eps, const float * x, const float * gamma, const float * beta,
+                              const float * delta, int operand_bf16, float * y_out, float * x_out);
+/* pre-LN assembly: patch [B*(T-1), h], class_embd [h], pos [T, h] -> x_out [B*T, h] fp32 */
+int clip_b200_debug_assemble_preln(const float * patch, const float * class_embd, const float * pos, int B, int T, int h, float eps,
+                                   const float * gamma, const float * beta, float * x_out);
+/* im2col: NHWC pixels [B, S, S, 3] -> fp16 patches [B*(S/P)^2, kpad] (widened to fp32 in out) */
+int clip_b200_debug_im2col(const float * pixels, int B, int S, int P, int kpad, float * out);
+/* text embedding: ids [nseq*T] (clamped to [0, n_vocab)), tok [n_vocab, h], pos [T, h] -> x_out [nseq*T, h] */
+int clip_b200_debug_text_embed(const int32_t * ids, const float * tok, const float * pos, int nseq, int T, int h, int n_vocab,
+                               float * x_out);
+/* row gather: out[r] = src[r*stride_rows + offs[r]] (+ delta[same row]); src and delta (optional) [src_rows, h], offs optional */
+int clip_b200_debug_gather_rows(const float * src, int src_rows, int rows, int h, int stride_rows, const int32_t * offs,
+                                const float * delta, int operand_bf16, float * out);
+/* L2 norm of each row of v [rows, d] (normalize = 0: plain copy) */
+int clip_b200_debug_l2norm(const float * v, int rows, int d, int normalize, float * out);
+/* EOT row index per sequence: last[i] = clamp(lens ? lens[i] : seq_len, 1, seq_len) - 1 */
+int clip_b200_debug_fill_last(const int32_t * lens, int n, int seq_len, int32_t * last);
+
 /* CPU-only TEST HOOKS (no context, no GPU): lossless re-tiling check, tokenizer and preprocess without a model context */
 int clip_b200_debug_repack_roundtrip(int qtype, const void * rows, int N, int K);
 int clip_b200_debug_rendezvous(int rank, int world, const char * path, void * out128);     /* ranks-mode id exchange (csrc/dist.cpp) */

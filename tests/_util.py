@@ -65,3 +65,42 @@ def one_minus_cos(a, b):
     num = (a * b).sum(-1)
     den = np.linalg.norm(a, axis=-1) * np.linalg.norm(b, axis=-1)
     return 1.0 - num / den
+
+
+# ---- LayerNorm test rows and their fp64 reference (tests/test_gpu_rows.py, tests/test_oracle_pin.py) ----------------------------
+# Row contents, each aimed at one way a LayerNorm goes subtly wrong:
+#   normal       standard normal
+#   offset       mean 1e3, std 1e-2: a one-pass E[x^2] - mean^2 variance cancels catastrophically
+#   eps_scale    std 3e-3, so the variance (9e-6) is about eps: a missing or misplaced eps moves every output
+#   const_half   constant 0.5, const_m3 constant -3: dyadic, so every partial sum is exact and the output is exactly beta
+#   outlier      standard normal with one +-1e4 element
+LN_KINDS = ("normal", "offset", "eps_scale", "const_half", "const_m3", "outlier")
+LN_KIND_SCALE = {"normal": 1.0, "offset": 1e-2, "eps_scale": 3e-3, "const_half": 0.0, "const_m3": 0.0, "outlier": 1.0}
+
+
+def ln_rows(rows, h, rng, first=0):
+    """x [rows, h] float32 whose row r has content LN_KINDS[(first + r) % len(LN_KINDS)]; returns (x, kind names)."""
+    kinds = [LN_KINDS[(first + r) % len(LN_KINDS)] for r in range(rows)]
+    x = rng.standard_normal((rows, h))
+    for r, k in enumerate(kinds):
+        if k == "offset":
+            x[r] = 1e3 + 1e-2 * x[r]
+        elif k == "eps_scale":
+            x[r] *= 3e-3
+        elif k == "const_half":
+            x[r] = 0.5
+        elif k == "const_m3":
+            x[r] = -3.0
+        elif k == "outlier":
+            x[r, rng.integers(h)] = 1e4 if r % 2 else -1e4
+    return x.astype(np.float32), kinds
+
+
+def ln_ref64(x, eps):
+    """fp64 LayerNorm without the affine, of the fp32 values in x: returns (x_hat, rstd [rows, 1], mean |x| [rows, 1]).
+    eps enters as the fp32 value the kernels add."""
+    x = np.asarray(x, np.float64)
+    mu = x.mean(-1, keepdims=True)
+    var = ((x - mu) ** 2).mean(-1, keepdims=True)
+    rstd = 1.0 / np.sqrt(var + float(np.float32(eps)))
+    return (x - mu) * rstd, rstd, np.abs(x).mean(-1, keepdims=True)

@@ -192,6 +192,93 @@ def test_gemm_wide_form_all_types(prod, qt, bf16):
     assert np.abs(y - ref).max() <= 2e-3 * max(1.0, np.abs(ref).max()), (qt, bf16)
 
 
+# ---- f16 weights: the form with both operands in shared memory (X box + W box per stage, a 5-deep ring) -------------------------
+# It only takes fp16 activations.  f16 model files use it for every linear layer, and every model uses it for the patch embedding.
+
+@pytest.mark.parametrize("epi", [EPI_STORE16, EPI_GELU16, EPI_QGELU16, EPI_REDADD32, EPI_STORE32])
+def test_gemm_f16_weights_epilogues(prod, epi):
+    """test_gemm_epilogues with f16 weights: STORE16 with the Q scale on the first N/2 features, both GELUs, the residual add"""
+    rng = np.random.default_rng(12)
+    M, N, K = 77, 128, 128
+    raw, deq = make_weight("f16", N, K, rng)
+    x = rng.standard_normal((M, K)).astype(np.float32)
+    bias = rng.standard_normal(N).astype(np.float32)
+    resid = rng.standard_normal((M, N)).astype(np.float32)
+    y, _ = run_gemm(prod, "f16", False, M, N, K, epi, x, raw, bias, resid)
+    ref = expected(x, deq, bias, False, epi, resid, N)
+    tol = 2e-2 if epi in (EPI_STORE16, EPI_GELU16, EPI_QGELU16) else 2e-3
+    assert np.abs(y - ref).max() <= tol * max(1.0, np.abs(ref).max()), (epi, np.abs(y - ref).max())
+
+
+def padded_f16_case(rng, M, N, K, K_real):
+    """x and an f16 weight whose columns K_real..K are zero, as the patch embedding pads 3 P^2 up to kpad (make_linear)"""
+    w = (rng.standard_normal((N, K)) * 0.05).astype(np.float16)
+    x = rng.standard_normal((M, K)).astype(np.float32)
+    w[:, K_real:] = 0
+    x[:, K_real:] = 0
+    return x, w.tobytes(), w.astype(np.float32)
+
+
+@pytest.mark.parametrize("K,K_real", [(128, 128), (640, 588)], ids=["K128", "K640-patch14"])
+def test_gemm_f16_weights_many_tiles(prod, K, K_real):
+    """4 feature tiles x 75 token tiles (the last one ragged) = 300 tiles over 132 SMs: each CTA walks 2-3 tiles, so the ring's
+    stage / phase bookkeeping carries across tiles.  K = 640 is the patch-embedding depth of a patch-14 model (588 + zero pad)."""
+    rng = np.random.default_rng(K)
+    M, N = 37 * 384 + 100, 512
+    x, raw, w = padded_f16_case(rng, M, N, K, K_real)
+    bias = rng.standard_normal(N).astype(np.float32)
+    y, _ = run_gemm(prod, "f16", False, M, N, K, EPI_STORE32, x, raw, bias)
+    ref = expected(x, w, bias, False, EPI_STORE32, None, N)
+    assert np.abs(y - ref).max() <= 2e-3 * max(1.0, np.abs(ref).max()), K
+
+
+# Bound at K = 5120 (the FC2 depth of a 1280-wide tower).  The reference is the fp64 product of the rounded operands, so only the
+# kernel's fp32 accumulation differs: the tensor core sums each 16-deep k-step, and the accumulator adds K/16 = 320 of them in
+# sequence, so |err| <= (320 + 4) u sum_k |x_k w_k|, u = 2^-24.  With |x| ~ N(0, 1) and |w| ~ 0.05 N(0, 1):
+# sum_k |x_k w_k| ~ 0.8 * 0.04 K = 163 while max |ref| >= ~3.5 sqrt(K) 0.05 = 12.5, so err / max|ref| <= 2.6e-4 in the worst case --
+# the 2e-3 bound used everywhere in this file still holds with room to spare.
+
+def test_gemm_f16_weights_deep_k(prod):
+    """K = 5120: 80 k-blocks, so the 5-stage ring wraps 16 times inside every tile"""
+    rng = np.random.default_rng(5120)
+    M, N, K = 1000, 512, 5120
+    raw, deq = make_weight("f16", N, K, rng)
+    x = rng.standard_normal((M, K)).astype(np.float32)
+    y, _ = run_gemm(prod, "f16", False, M, N, K, EPI_STORE32, x, raw, None)
+    ref = expected(x, deq, None, False, EPI_STORE32, None, N)
+    assert np.abs(y - ref).max() <= 2e-3 * max(1.0, np.abs(ref).max())
+
+
+@pytest.mark.parametrize("epi", [EPI_STORE16, EPI_REDADD32])
+def test_gemm_f16_weights_single_token(prod, epi):
+    """M = 1: one token row in a 192-row tile, the rest zero-filled by the TMA"""
+    rng = np.random.default_rng(1)
+    M, N, K = 1, 256, 640
+    raw, deq = make_weight("f16", N, K, rng)
+    x = rng.standard_normal((M, K)).astype(np.float32)
+    bias = rng.standard_normal(N).astype(np.float32)
+    resid = rng.standard_normal((M, N)).astype(np.float32)
+    y, _ = run_gemm(prod, "f16", False, M, N, K, epi, x, raw, bias, resid)
+    ref = expected(x, deq, bias, False, epi, resid, N)
+    tol = 2e-2 if epi == EPI_STORE16 else 2e-3
+    assert np.abs(y - ref).max() <= tol * max(1.0, np.abs(ref).max())
+
+
+@pytest.mark.parametrize("K,M", [(64, 333), (5120, 1000)], ids=["K64", "K5120"])
+@pytest.mark.parametrize("qt,bf16", [(qt, bf) for qt in ("q4_0", "q4_1", "q5_0", "q5_1", "q8_0") for bf in (True, False)])
+def test_gemm_k_depth_edges(prod, qt, bf16, K, M):
+    """K = 64 is a single k-block: only the tail kblock() after the paired loop runs.  K = 5120 is the FC2 depth of a 1280-wide
+    tower: the packed-weight and X rings wrap many times inside each tile (bound: see the note above test_gemm_f16_weights_deep_k)."""
+    rng = np.random.default_rng(K + M)
+    N = 256
+    raw, deq = make_weight(qt, N, K, rng)
+    x = rng.standard_normal((M, K)).astype(np.float32)
+    bias = rng.standard_normal(N).astype(np.float32)
+    y, _ = run_gemm(prod, qt, bf16, M, N, K, EPI_STORE32, x, raw, bias)
+    ref = expected(x, deq, bias, bf16, EPI_STORE32, None, N)
+    assert np.abs(y - ref).max() <= 2e-3 * max(1.0, np.abs(ref).max()), (qt, bf16, K)
+
+
 @pytest.mark.parametrize("M", [74 * 384, 74 * 384 + 1, 75 * 384 - 191, 75 * 384 + 193, 111 * 384 + 7])
 @pytest.mark.parametrize("epi", [EPI_STORE16, EPI_QGELU16, EPI_REDADD32])
 def test_gemm_wide_form_tails_and_epilogues(prod, M, epi):

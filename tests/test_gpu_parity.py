@@ -90,6 +90,34 @@ def test_against_cpu_oracle_unnormalized(prod):
         assert abs(np.linalg.norm(gt[i]) / np.linalg.norm(ot) - 1) < 0.05
 
 
+@pytest.mark.parametrize("ft", ["f16", "q4_0"])
+def test_wide_h1280_against_cpu_oracle(prod, ft):
+    """1280-wide towers (wide-h1280): the only place the 16-float4-per-lane LayerNorm runs in the model schedule -- pre-LN, ln1 /
+    ln2 and post-LN of both towers -- next to the f16 patch embedding at kpad 640 and FC2 at K = 5120.  No golden file: the
+    oracle restatement is the reference."""
+    import oracle as orc
+    path = model_file("wide-h1280", ft, prod)
+    imgs = sg.synth_images(3, 112, 1280)
+    seqs = [sg.synth_tokens(1, n, 1280 + n)[0] for n in (2, 33, 77)]
+    ctx = prod.load(path, 0)
+    try:
+        gi = prod.image_batch_encode(ctx, imgs, normalize=False)
+        gt = prod.text_batch_encode(ctx, seqs, normalize=False)
+        ni = prod.image_batch_encode(ctx, imgs)
+        nt = prod.text_batch_encode(ctx, seqs)
+    finally:
+        prod.free(ctx)
+    om = orc.OracleModel(path)
+    for i in range(3):
+        oi, ot = om.encode_image(imgs[i], normalize=False), om.encode_text(seqs[i], normalize=False)
+        di, dt = one_minus_cos(ni[i], oi), one_minus_cos(nt[i], ot)
+        print("wide-h1280 %s #%d  image 1-cos %.2e  text 1-cos %.2e" % (ft, i, di, dt))
+        assert di <= TOL[ft] and dt <= TOL[ft], (ft, i, di, dt)
+        assert abs(np.linalg.norm(gi[i]) / np.linalg.norm(oi) - 1) < 0.05
+        assert abs(np.linalg.norm(gt[i]) / np.linalg.norm(ot) - 1) < 0.05
+        assert one_minus_cos(gi[i], ni[i]) < 1e-6 and one_minus_cos(gt[i], nt[i]) < 1e-6
+
+
 def test_edge_cases(prod):
     import ctypes as C
     import binding as bd

@@ -3,7 +3,10 @@
   2. against what the reference returned for fresh inputs (tests/golden/reference_runs.npz, made by oracle/_ref);
   3. its block quantizer against the reference's quantized model files (sha256 of the whole GGUF).
 Tolerances: the oracle reproduces every rounding point of the reference, so only summation order differs; quantized
-paths re-quantize activations per layer, which turns ulp-level differences into occasional +-1 flips (observed 1e-5)."""
+paths re-quantize activations per layer, which turns ulp-level differences into occasional +-1 flips (observed 1e-5).
+It also checks the other way round: the fp64 LayerNorm that tests/test_gpu_rows.py holds the kernels to agrees with the
+oracle's orc_layer_norm on the same rows, so that reference is itself pinned on a machine without a GPU."""
+import ctypes as C
 import os
 
 import numpy as np
@@ -11,7 +14,7 @@ import pytest
 
 import oracle as orc
 import synth_gguf as sg
-from _util import FTYPES, check_sha, golden, model_file, one_minus_cos, reference_runs, token_seqs
+from _util import FTYPES, LN_KINDS, check_sha, golden, ln_ref64, ln_rows, model_file, one_minus_cos, reference_runs, token_seqs
 
 PIN_TOL = {"f32": 1e-5, "f16": 1e-5, "q4_0": 5e-4, "q4_1": 5e-4, "q5_0": 5e-4, "q5_1": 5e-4, "q8_0": 5e-4}
 
@@ -82,9 +85,31 @@ def test_oracle_quantizer_reproduces_reference_blocks(prod, ft):
     assert n == 4
 
 
+@pytest.mark.parametrize("eps", [1e-5, 1e-6])
+@pytest.mark.parametrize("h", [128, 384, 512, 640, 1024, 1152, 1280, 1664, 2048])
+def test_layer_norm_reference_matches_oracle(h, eps):
+    """ln_ref64 (fp64) against orc_layer_norm, every row content of LN_KINDS.  The oracle's rounding points: the mean is the
+    fp32 rounding of a double sum (off by <= 1 fp32 ulp of mean), x - mean is one fp32 rounding, the variance a double sum of fp32
+    squares rounded to fp32, then + eps, sqrtf, 1/ and one product: <= 8 fp32 units u = 2^-24 relative on x_hat.  The mean's
+    error shifts x_hat by rstd * dmu, and adds dmu^2 to the variance."""
+    rng = np.random.default_rng(h)
+    x, kinds = ln_rows(4 * len(LN_KINDS), h, rng)
+    y = np.empty_like(x)
+    fp = C.POINTER(C.c_float)
+    orc.lib().orc_layer_norm(x.ctypes.data_as(fp), y.ctypes.data_as(fp), x.shape[0], h, eps)
+    xh, rstd, _ = ln_ref64(x, eps)
+    u = 2.0 ** -24
+    dmu = np.spacing(np.abs(x.astype(np.float64).mean(-1, keepdims=True)).astype(np.float32)).astype(np.float64)
+    tol = 8 * u * np.abs(xh) + rstd * dmu + 0.5 * (rstd * dmu) ** 2 * np.abs(xh)
+    err = np.abs(y - xh)
+    assert (err <= tol).all(), (h, eps, [kinds[r] for r in np.unique(np.nonzero(err > tol)[0])], (err / tol).max())
+    for r, k in enumerate(kinds):
+        if k.startswith("const"):
+            assert not y[r].any(), (h, k)          # a constant row normalises to exactly 0
+
+
 def test_oracle_dequant_matches_format_definition():
     """Hand-built q4_0 / q8_0 blocks with known values (ggml.c:1496-1512, 1599-1605)."""
-    import ctypes as C
     blk = np.zeros(18, np.uint8)
     blk[0:2] = np.array([0.5], np.float16).view(np.uint8)
     blk[2:] = np.arange(16, dtype=np.uint8) | ((15 - np.arange(16, dtype=np.uint8)) << 4)
