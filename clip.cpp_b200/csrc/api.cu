@@ -211,9 +211,11 @@ bool load_blocks(clip_ctx* c, const GgufFile& g, const char* p, Tower& tw) {
     return true;
 }
 
-bool check_geometry(const char* what, const Tower& t) {
+bool check_geometry(const clip_ctx* c, const char* what, const Tower& t) {
     if (t.hidden <= 0 || t.ff <= 0 || t.heads <= 0 || t.layers < 0 || t.layers > 1024 || t.proj <= 0 || !(t.eps >= 0.f)) { set_err(std::string(what) + ": non-positive hyper-parameter in the file"); return false; }
-    if (t.heads <= 0 || t.hidden % t.heads || t.hidden / t.heads != 64) { set_err(std::string(what) + ": head_dim must be 64 (hidden " + std::to_string(t.hidden) + ", heads " + std::to_string(t.heads) + ")"); return false; }
+    const std::string hh = " (hidden " + std::to_string(t.hidden) + ", heads " + std::to_string(t.heads) + ")";
+    if (t.heads <= 0 || t.hidden % t.heads || (t.hidden / t.heads != 64 && t.hidden / t.heads != 80)) { set_err(std::string(what) + ": head_dim must be 64 or 80" + hh); return false; }
+    if (!c->attn_tc && t.hidden / t.heads != 64) { set_err(std::string(what) + ": the legacy attention kernel (CLIP_B200_ATTN=legacy) supports head_dim 64 only" + hh); return false; }
     if (t.hidden > 2048) { set_err(std::string(what) + ": hidden size > 2048 is not supported by the register-resident LayerNorm"); return false; }
     if (t.hidden % 128 || t.ff % 128 || t.proj % 128) { set_err(std::string(what) + ": hidden/ff/projection sizes must be multiples of 128"); return false; }
     return true;
@@ -274,11 +276,12 @@ bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal) {
     Workspace& w = tw.ws;
     const int M = nseq * T, h = tw.hidden;
     const int bf = c->operand_bf16 ? 1 : 0;
-    const float qscale = 1.0f / sqrtf(64.0f);
+    const int dh = h / tw.heads;                      // 64 or 80 (check_geometry)
+    const float qscale = 1.0f / sqrtf((float)dh);     // clip.cpp:1082, 1363
     for (auto& l : tw.L) {
         { Scope s(c, K_LN); launch_layernorm(w.x, h, M, h, tw.eps, l.ln1_g, l.ln1_b, nullptr, w.a, bf, c->stream); }
         if (!run_linear(c, l.qkv, &w.map_a, w.a, bf, M, w.qkv, 3 * h, EPI_STORE16, bf, h, qscale)) return false;
-        if (c->attn_tc) { Scope s(c, K_ATTN); CK(launch_attention_tc(w.qkv, w.a, nseq, T, tw.heads, causal ? 1 : 0, bf, c->stream)); }
+        if (c->attn_tc) { Scope s(c, K_ATTN); CK(launch_attention_tc(w.qkv, w.a, nseq, T, tw.heads, dh, causal ? 1 : 0, bf, c->stream)); }
         else { Scope s(c, K_ATTN); launch_attention(w.qkv, w.a, nseq, T, tw.heads, causal ? 1 : 0, bf, c->stream); }
         if (!run_linear(c, l.out, &w.map_a, w.a, bf, M, w.x, h, EPI_REDADD32, 0)) return false;
         { Scope s(c, K_LN); launch_layernorm(w.x, h, M, h, tw.eps, l.ln2_g, l.ln2_b, nullptr, w.a, bf, c->stream); }
@@ -485,7 +488,7 @@ static clip_ctx* load_on_device(const GgufFile& g, int device, const int verbosi
             t.present = true; t.hidden = hp.hidden_size; t.ff = hp.n_intermediate; t.heads = hp.n_head; t.layers = hp.n_layer;
             t.proj = hp.projection_dim; t.eps = hp.eps; t.n_vocab = hp.n_vocab; t.n_ctx = hp.num_positions;
             if (t.n_ctx <= 0 || t.n_ctx > 4096 || t.n_vocab <= 0) { set_err("text tower: bad context_length / vocabulary size"); return nullptr; }
-            if (!check_geometry("text tower", t)) return nullptr;
+            if (!check_geometry(c, "text tower", t)) return nullptr;
             if (!upload_f32(c, g, "t.token_embd.weight", &t.tok, (int64_t)t.n_vocab * t.hidden) ||
                 !upload_f32(c, g, "t.position_embd.weight", &t.pos, (int64_t)t.n_ctx * t.hidden) ||
                 !upload_f32(c, g, "t.post_ln.weight", &t.post_g, t.hidden) || !upload_f32(c, g, "t.post_ln.bias", &t.post_b, t.hidden)) return nullptr;
@@ -516,7 +519,7 @@ static clip_ctx* load_on_device(const GgufFile& g, int device, const int verbosi
             t.n_patches = (t.image_size / t.patch) * (t.image_size / t.patch);
             t.T = t.n_patches + 1;
             t.kpad = (3 * t.patch * t.patch + GEMM_BK - 1) / GEMM_BK * GEMM_BK;
-            if (!check_geometry("vision tower", t)) return nullptr;
+            if (!check_geometry(c, "vision tower", t)) return nullptr;
             if (!make_linear(c, g, {"v.patch_embd.weight"}, {}, t.patch_w, t.kpad)) return nullptr;
             if (t.patch_w.N != t.hidden) { set_err("v.patch_embd.weight shape mismatch"); return nullptr; }
             if (!upload_f32(c, g, "v.class_embd", &t.class_embd, t.hidden) ||
@@ -1489,12 +1492,15 @@ int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int e
 }
 
 
-// TEST HOOK: one attention launch on device 0.  qkv: fp32 host [nseq*T, 3*H*64] (columns Q | K | V, the Q columns already scaled),
-// rounded to the operand type on the way in; out: fp32 host [nseq*T, H*64].  use_legacy=1 runs the mma.sync flash kernel.
-int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int causal, int use_legacy, const float* qkv, float* out, float* ms) {
+// TEST HOOK: one attention launch on device 0.  qkv: fp32 host [nseq*T, 3*H*dh] (columns Q | K | V, the Q columns already scaled),
+// rounded to the operand type on the way in; out: fp32 host [nseq*T, H*dh].  use_legacy=1 runs the mma.sync flash kernel (dh 64).
+int clip_b200_debug_attention_hd(int operand_bf16, int nseq, int T, int H, int head_dim, int causal, int use_legacy, const float* qkv,
+                                 float* out, float* ms) {
     g_err.clear();
+    if (head_dim != 64 && head_dim != 80) { set_err("attention: head_dim must be 64 or 80"); return 2; }
+    if (use_legacy && head_dim != 64) { set_err("attention: the legacy kernel supports head_dim 64 only"); return 2; }
     if (attention_tc_init() != cudaSuccess) { set_err("attention_tc_init failed"); return 1; }
-    const size_t rows = (size_t)nseq * T, hid = (size_t)H * 64;
+    const size_t rows = (size_t)nseq * T, hid = (size_t)H * head_dim;
     std::vector<uint16_t> h16(rows * 3 * hid);
     for (size_t i = 0; i < h16.size(); i++) h16[i] = operand_bf16 ? f32_to_bf16(qkv[i]) : f32_to_f16(qkv[i]);
     uint16_t *d_qkv = nullptr, *d_out = nullptr;
@@ -1514,7 +1520,7 @@ int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int caus
         for (int rep = 0; rep < (ms ? 3 : 1); rep++) {
             cudaEventRecord(e0, st);
             if (use_legacy) { launch_attention(d_qkv, d_out, nseq, T, H, causal, operand_bf16, st); e = cudaGetLastError(); }
-            else e = launch_attention_tc(d_qkv, d_out, nseq, T, H, causal, operand_bf16, st);
+            else e = launch_attention_tc(d_qkv, d_out, nseq, T, H, head_dim, causal, operand_bf16, st);
             cudaEventRecord(e1, st);
             if (e != cudaSuccess) break;
             if ((e = cudaStreamSynchronize(st)) != cudaSuccess) break;
@@ -1533,6 +1539,10 @@ int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int caus
     if (e1) cudaEventDestroy(e1);
     if (st) cudaStreamDestroy(st);
     return rc;
+}
+
+int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int causal, int use_legacy, const float* qkv, float* out, float* ms) {
+    return clip_b200_debug_attention_hd(operand_bf16, nseq, T, H, 64, causal, use_legacy, qkv, out, ms);
 }
 
 }  // extern "C"

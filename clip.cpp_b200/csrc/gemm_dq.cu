@@ -186,8 +186,9 @@ CB_DEVINL void fence_frag(uint32_t (&a)[16]) {
     for (int i = 0; i < 16; i++) asm volatile("" : "+r"(a[i])::"memory");
 }
 
-// 16-bit epilogue value of one accumulator element.  `bias` arrives PRE-MULTIPLIED by `mul` for EPI_STORE16 so that
-// (acc + b) * mul becomes one FFMA (the Q scale 1/sqrt(64) = 0.125 is a power of two: bit-identical to the two-step form);
+// 16-bit epilogue value of one accumulator element.  EPI_STORE16 rounds (acc + b) to fp32 before the scale, the reference's order
+// (ggml_add then ggml_scale, clip.cpp:1082, 1363): the Q scale 1/sqrt(80) of head_dim 80 is not a power of two, so a single FFMA
+// with a pre-scaled bias would round differently.  For 1/sqrt(64) = 0.125 the two forms give the same bits.
 // quick-GELU x * sigmoid(1.702 x) = h + h * tanh(0.851 x) with h = x / 2.
 template <int EPI>
 CB_DEVINL float epi_value(float acc, float bias, float mul) {
@@ -197,7 +198,7 @@ CB_DEVINL float epi_value(float acc, float bias, float mul) {
         float t;
         asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.851f * x));
         return fmaf(h, t, h);
-    } else return fmaf(acc, mul, bias);
+    } else return (acc + bias) * mul;
 }
 
 // Epilogue of one consumer group's [64 features x 192 tokens] accumulator (fragment layout: wgmma.cuh).  This thread owns features
@@ -329,7 +330,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_dq_kernel(const __grid_consta
         #pragma unroll
         for (int h = 0; h < 2; h++) {
             mul[h] = (f + 8 * h < p.scale_cols) ? p.scale : 1.0f;
-            bias[h] = (p.bias ? p.bias[f + 8 * h] : 0.0f) * ((p.epi == EPI_STORE16) ? mul[h] : 1.0f);
+            bias[h] = p.bias ? p.bias[f + 8 * h] : 0.0f;
         }
         switch (p.epi) {
         case EPI_STORE16: epilogue_regs<EPI_STORE16, BF>(p, acc, tok0, f, tc, bias, mul); break;

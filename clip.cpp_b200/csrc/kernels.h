@@ -25,15 +25,17 @@ void launch_assemble_preln(const float* patch, const float* class_embd, const fl
 void launch_text_embed(const int32_t* ids, const float* tok, const float* pos, int nseq, int T, int h, int n_vocab, float* x,
                        cudaStream_t st);
 
-// K3 attention: softmax(Q K^T [causal]) V per (sequence, head); qkv 16-bit [nseq*T, 3*H*64] (Q pre-scaled),
-// out 16-bit [nseq*T, H*64].  head_dim is fixed at 64.  (clip.cpp:1100-1108, 1382-1388)
-// launch_attention: warp-level mma.sync kernel (attention.cu), kept as the cross-check of the wgmma kernel (CLIP_B200_ATTN=legacy).
+// K3 attention: softmax(Q K^T [causal]) V per (sequence, head); qkv 16-bit [nseq*T, 3*H*dh] (Q pre-scaled by 1/sqrt(dh)),
+// out 16-bit [nseq*T, H*dh].  (clip.cpp:1100-1108, 1382-1388)
+// launch_attention: warp-level mma.sync kernel (attention.cu), head_dim 64 only, kept as the cross-check of the wgmma kernel
+// (CLIP_B200_ATTN=legacy).
 void launch_attention(const void* qkv16, void* out16, int nseq, int T, int H, int causal, int bf16, cudaStream_t st);
 
-// K3 on wgmma (attention_tc.cu): 128-query tiles, online softmax over 128-key blocks, any T.  The Q / K / V boxes come from a
-// per-launch 3-D TMA view [sequence][token][column] of qkv16 (zero fill past each sequence's T tokens).
+// K3 on wgmma (attention_tc.cu): head_dim dh = 64 or 80 (anything else: cudaErrorInvalidValue), 128-query tiles, online softmax
+// over 128-key blocks, any T.  The Q / K / V boxes come from per-launch 3-D TMA views [sequence][token][column] of qkv16 (zero
+// fill past each sequence's T tokens).
 cudaError_t attention_tc_init();
-cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T, int H, int causal, int bf16, cudaStream_t st);
+cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T, int H, int dh, int causal, int bf16, cudaStream_t st);
 
 // K5 head tail: out[r,:] = normalize ? v / sqrt(sum v^2) : v    (clip.cpp:1163-1166, 1448-1455)
 void launch_l2norm(const float* v, float* out, int rows, int d, int normalize, cudaStream_t st);

@@ -33,6 +33,18 @@ CB_DEVINL uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
     return d;
 }
 
+// The same for a tile 16 elements wide stored with the 32-byte swizzle (CU_TENSOR_MAP_SWIZZLE_32B): rows of 32 B, 8-row groups
+// 256 B apart.  A K-major operand of one 16-deep k step and an MN-major operand 16 wide both fit in one swizzle atom across, so
+// only the 8-row group stride is used.  Tile bases are 256-B aligned; a 16-row step (keys of an MN-major tile) is 512 B.
+CB_DEVINL uint64_t wgmma_desc_sw32(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);   // start address       [0,14)
+    d |= (uint64_t)(256 >> 4) << 16;                // leading byte offset [16,30)
+    d |= (uint64_t)(256 >> 4) << 32;                // stride byte offset  [32,46)
+    d |= (uint64_t)3 << 62;                         // layout: 32-byte swizzle [62,64)
+    return d;
+}
+
 // D[64 x 192] (+)= A[64 x 16] . B[192 x 16]^T, both operands K-major in shared memory (descriptors), fp32 accumulators
 template <bool BF>
 CB_DEVINL void wgmma_ss_n192(float (&d)[96], uint64_t da, uint64_t db, uint32_t accumulate) {
@@ -83,6 +95,19 @@ CB_DEVINL void wgmma_rs_n64_bmn(float (&d)[32], const uint32_t (&a)[4], uint64_t
     if constexpr (BF) CB_WGMMA_RS_N64("bf16");
     else CB_WGMMA_RS_N64("f16");
 #undef CB_WGMMA_RS_N64
+}
+
+// D[64 x 16] (+)= A[64 x 16] . B[16 x 16]: A from registers, B MN-major in shared memory (the 16-column tail of an 80-wide head)
+template <bool BF>
+CB_DEVINL void wgmma_rs_n16_bmn(float (&d)[8], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+#define CB_WGMMA_RS_N16(TY)                                                                                 \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %13, 0;\n\t"                                                 \
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 1;\n\t}"  \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])  \
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate))
+    if constexpr (BF) CB_WGMMA_RS_N16("bf16");
+    else CB_WGMMA_RS_N16("f16");
+#undef CB_WGMMA_RS_N16
 }
 
 }  // namespace cb

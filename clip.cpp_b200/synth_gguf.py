@@ -9,7 +9,7 @@ written in exactly the on-disk contract the reference's loader reads:
   * tensor names:                     /root/reference/clip.cpp:64-79
   * dtype rules of the HF converter:  /root/reference/models/convert_hf_to_gguf.py:173-206
     (2-D `*.weight` -> f16/f32, `v.patch_embd.weight` always f16, everything else f32)
-  * tensor counts the reference accepts (397 two-tower base, 589 two-tower large):
+  * tensor counts the reference accepts (397 two-tower base, 589 two-tower large, 909 two-tower huge):
                                       /root/reference/clip.cpp:261-294
 
 Weights are drawn from a seeded numpy PCG64 stream, so a (geometry, seed) pair
@@ -71,6 +71,9 @@ GEOMETRIES = {
     "vit-b32": Geometry("vit-b32"),
     "vit-l14": Geometry("vit-l14", patch_size=14, v_hidden=1024, v_ff=4096, v_heads=16, v_layers=24,
                         t_hidden=768, t_ff=3072, t_heads=12, t_layers=12, proj_dim=768),
+    # LAION ViT-H/14: vision head_dim 1280 / 16 = 80, text head_dim 1024 / 16 = 64, GELU
+    "vit-h14": Geometry("vit-h14", patch_size=14, v_hidden=1280, v_ff=5120, v_heads=16, v_layers=32,
+                        t_hidden=1024, t_ff=4096, t_heads=16, t_layers=24, proj_dim=1024, use_gelu=True),
     # small models for unit tests: same tensor counts as base (397) so the reference accepts them,
     # head_dim = 64 like every real CLIP model
     "tiny": Geometry("tiny", image_size=64, patch_size=16, v_hidden=128, v_ff=256, v_heads=2, v_layers=12,
@@ -88,6 +91,10 @@ GEOMETRIES = {
     # 2 layers; ~300 MB as f16
     "wide-h1280": Geometry("wide-h1280", image_size=112, patch_size=14, v_hidden=1280, v_ff=5120, v_heads=20, v_layers=2,
                            t_hidden=1280, t_ff=5120, t_heads=20, t_layers=2, proj_dim=1024),
+    # the huge tensor counts (32 + 24 layers, 909 tensors) at low width, so the reference accepts it: vision head_dim 640 / 8 = 80
+    # over 257 positions, GELU
+    "huge-w640": Geometry("huge-w640", image_size=224, patch_size=14, v_hidden=640, v_ff=1280, v_heads=8, v_layers=32,
+                          t_hidden=128, t_ff=256, t_heads=2, t_layers=24, proj_dim=128, use_gelu=True),
 }
 
 

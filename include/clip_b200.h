@@ -267,6 +267,10 @@ bool clip_b200_image_batch_preprocess_device(const struct clip_ctx * ctx, const 
  * use_legacy=1 runs the warp-level mma.sync kernel instead of the wgmma one.  ms (optional): device time of the last of 3 launches. */
 int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int causal, int use_legacy, const float * qkv, float * out,
                               float * ms);
+/* The same for head_dim 64 or 80: qkv [nseq*T, 3*H*head_dim], the 1/sqrt(head_dim) scale already applied to Q; out [nseq*T, H*head_dim].
+ * Returns 2 with a message for any other head_dim, and for use_legacy=1 with head_dim 80 (the legacy kernel is head_dim 64 only). */
+int clip_b200_debug_attention_hd(int operand_bf16, int nseq, int T, int H, int head_dim, int causal, int use_legacy, const float * qkv,
+                                 float * out, float * ms);
 
 /* TEST HOOKS for the row kernels (csrc/kernels.cu): each runs one launcher on a private stream on device 0 and returns 0 on
  * success (clip_b200_last_error says why not).  Host buffers are fp32 / int32; 16-bit inputs are rounded to the operand type
