@@ -16,7 +16,8 @@
 //               from the packed chunk into registers, and the group issues 4 register-A wgmma m64n192k16 per k-block (B = activation
 //               tile from shared memory), keeping one k-block of MMAs in flight while it unpacks the next.  f16 weights: both operands
 //               from shared memory.  Epilogue straight from the accumulator registers: bias / scale / GELU and 16-bit or fp32 stores,
-//               or x += acc + bias into the fp32 residual stream (every element has exactly one owner thread: deterministic).
+//               or x += acc + bias into the fp32 residual stream (every element has exactly one owner thread: deterministic), its x
+//               values read in four batches of independent loads (epilogue_regs).
 // Bytes per launch (DESIGN.md section 5): packed W once per token tile, X once per feature tile, Y once; FLOPs = 2*M*N*K.
 #include <cuda.h>
 #include <stdlib.h>
@@ -201,23 +202,63 @@ CB_DEVINL float epi_value(float acc, float bias, float mul) {
     } else return (acc + bias) * mul;
 }
 
+// Global accesses of the epilogue, predicated on `ok` (token rows past M) inside one asm: no branch per element.  All are volatile, so
+// they reach ptxas in source order: the residual loads of a batch are issued before any of its stores.
+CB_DEVINL float ldg_f32_if(const float* a, bool ok) {
+    float v = 0.f;
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p ld.global.f32 %0, [%1];\n\t}" : "+f"(v) : "l"(a), "r"((int)ok));
+    return v;
+}
+CB_DEVINL void stg_f32_if(float* a, float v, bool ok) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.global.f32 [%0], %1;\n\t}" ::"l"(a), "f"(v), "r"((int)ok));
+}
+CB_DEVINL void stg_u16_if(uint16_t* a, uint16_t v, bool ok) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.global.u16 [%0], %1;\n\t}" ::"l"(a), "h"(v), "r"((int)ok));
+}
+
 // Epilogue of one consumer group's [64 features x 192 tokens] accumulator (fragment layout: wgmma.cuh).  This thread owns features
 // f and f + 8 and tokens 8j + tc + {0, 1}; element offsets are 32-bit (host checks M*ldo < 2^32).
+// The residual add x += acc + bias reads its 96 x values in four batches of 24, each batch loaded completely before the first of its
+// stores: four memory round trips per tile instead of a chain of 96 dependent ones (with loads and stores through one pointer the
+// compiler cannot prove them disjoint, so written as x[o] += v it keeps every load behind the previous store).
 template <int EPI, bool BF>
-CB_DEVINL void epilogue_regs(const KParams& p, float (&acc)[BN / 2], int tok0, int f, int tc, const float (&bias)[2], const float (&mul)[2]) {
-    const int ntok = min(BN, p.M - tok0);
-    const uint32_t ldo = (uint32_t)p.ldo;
-    #pragma unroll
-    for (int j = 0; j < BN / 8; j++) {
+CB_DEVINL void epilogue_regs(void* out, int M, int ldo_, float (&acc)[BN / 2], int tok0, int f, int tc, const float (&bias)[2],
+                             const float (&mul)[2]) {
+    const int nt = min(BN, M - tok0) - tc;     // this thread's token 8j + tc + e1 is in range iff 8j + e1 < nt
+    const uint32_t ldo = (uint32_t)ldo_;
+    const uint32_t o0 = (uint32_t)(tok0 + tc) * ldo + (uint32_t)f;
+    auto off = [&](int j, int e) { return o0 + (uint32_t)(8 * j + (e & 1)) * ldo + 8u * (uint32_t)(e >> 1); };
+    if constexpr (EPI == EPI_REDADD32) {
+        float* x = reinterpret_cast<float*>(out);
+        constexpr int JB = 6;                  // 6 token groups = 24 elements per batch: the most that fits 168 registers without spills
         #pragma unroll
-        for (int e = 0; e < 4; e++) {
-            const int t = 8 * j + tc + (e & 1), h = e >> 1;
-            if (t >= ntok) continue;
-            const uint32_t o = (uint32_t)(tok0 + t) * ldo + (uint32_t)(f + 8 * h);
-            const float a = acc[4 * j + e];
-            if constexpr (EPI == EPI_STORE32) reinterpret_cast<float*>(p.out)[o] = a + bias[h];
-            else if constexpr (EPI == EPI_REDADD32) reinterpret_cast<float*>(p.out)[o] += a + bias[h];
-            else reinterpret_cast<uint16_t*>(p.out)[o] = P2<BF>::from_float(epi_value<EPI>(a, bias[h], mul[h]));
+        for (int b = 0; b < BN / 8 / JB; b++) {
+            float r[4 * JB];
+            #pragma unroll
+            for (int jj = 0; jj < JB; jj++) {
+                #pragma unroll
+                for (int e = 0; e < 4; e++) r[4 * jj + e] = ldg_f32_if(x + off(b * JB + jj, e), 8 * (b * JB + jj) + (e & 1) < nt);
+            }
+            #pragma unroll
+            for (int jj = 0; jj < JB; jj++) {
+                #pragma unroll
+                for (int e = 0; e < 4; e++) {
+                    const int j = b * JB + jj;
+                    stg_f32_if(x + off(j, e), r[4 * jj + e] + (acc[4 * j + e] + bias[e >> 1]), 8 * j + (e & 1) < nt);
+                }
+            }
+        }
+    } else {
+        #pragma unroll
+        for (int j = 0; j < BN / 8; j++) {
+            #pragma unroll
+            for (int e = 0; e < 4; e++) {
+                const int h = e >> 1;
+                const bool ok = 8 * j + (e & 1) < nt;
+                const float a = acc[4 * j + e];
+                if constexpr (EPI == EPI_STORE32) stg_f32_if(reinterpret_cast<float*>(out) + off(j, e), a + bias[h], ok);
+                else stg_u16_if(reinterpret_cast<uint16_t*>(out) + off(j, e), P2<BF>::from_float(epi_value<EPI>(a, bias[h], mul[h])), ok);
+            }
         }
     }
 }
@@ -332,12 +373,13 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_dq_kernel(const __grid_consta
             mul[h] = (f + 8 * h < p.scale_cols) ? p.scale : 1.0f;
             bias[h] = p.bias ? p.bias[f + 8 * h] : 0.0f;
         }
+        void* const out = p.out;
         switch (p.epi) {
-        case EPI_STORE16: epilogue_regs<EPI_STORE16, BF>(p, acc, tok0, f, tc, bias, mul); break;
-        case EPI_GELU16: epilogue_regs<EPI_GELU16, BF>(p, acc, tok0, f, tc, bias, mul); break;
-        case EPI_QGELU16: epilogue_regs<EPI_QGELU16, BF>(p, acc, tok0, f, tc, bias, mul); break;
-        case EPI_REDADD32: epilogue_regs<EPI_REDADD32, BF>(p, acc, tok0, f, tc, bias, mul); break;
-        default: epilogue_regs<EPI_STORE32, BF>(p, acc, tok0, f, tc, bias, mul); break;
+        case EPI_STORE16: epilogue_regs<EPI_STORE16, BF>(out, p.M, p.ldo, acc, tok0, f, tc, bias, mul); break;
+        case EPI_GELU16: epilogue_regs<EPI_GELU16, BF>(out, p.M, p.ldo, acc, tok0, f, tc, bias, mul); break;
+        case EPI_QGELU16: epilogue_regs<EPI_QGELU16, BF>(out, p.M, p.ldo, acc, tok0, f, tc, bias, mul); break;
+        case EPI_REDADD32: epilogue_regs<EPI_REDADD32, BF>(out, p.M, p.ldo, acc, tok0, f, tc, bias, mul); break;
+        default: epilogue_regs<EPI_STORE32, BF>(out, p.M, p.ldo, acc, tok0, f, tc, bias, mul); break;
         }
     }
 }
