@@ -2,6 +2,7 @@
 // host<->device plumbing.  No graph, no dispatch: each encode call issues a fixed sequence of kernel launches on
 // one stream.  There is NO CPU path -- if CUDA is unavailable clip_model_load fails loudly.
 #include <chrono>
+#include <float.h>
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -1031,7 +1032,9 @@ static bool score_topk_locked(clip_ctx* c, const float* d_q, size_t nq, const fl
     const int SL = topk_slice();
     const size_t budget = (size_t)32 << 20;                               // floats of similarity scratch per pass (128 MB)
     size_t CH = std::min(ndb, std::max<size_t>(budget / std::min<size_t>(nq, 256), (size_t)SL));
-    if (softmax) CH = ndb;                                                // the normalisation needs whole rows
+    // whole rows: the normalisation needs them, and so does the host ranking taken when top_k > 1024 (a ranking per chunk would
+    // keep only the last chunk's best, numbered within that chunk)
+    if (softmax || k > 1024) CH = ndb;
     const size_t RB = std::max<size_t>(1, std::min<size_t>({nq, budget / CH + 1, (size_t)32768}));
     size_t nsl = 0;
     for (size_t c0 = 0; c0 < ndb; c0 += CH) nsl += (std::min(CH, ndb - c0) + SL - 1) / SL;
@@ -1059,10 +1062,13 @@ static bool score_topk_locked(clip_ctx* c, const float* d_q, size_t nq, const fl
                 launch_topk_stage(c->d_logits, nullptr, CH, rows, cols, (int)c0, kk, c->d_cand_v[0], c->d_cand_i[0], cand_ld, (int)(sl0 * kk), c->stream);
                 sl0 += ((size_t)cols + SL - 1) / SL;
             } else {
-                // full ranking of rows longer than one sort slice (top_k > 1024): ranked on the host, as the reference does
+                // full ranking of rows longer than one sort slice (top_k > 1024): ranked on the host, as the reference does.  cols
+                // is the whole row (CH = ndb above) and k <= ndb.  NaN becomes -FLT_MAX as in topk_stage_kernel: it ranks last, ties
+                // by index, and the comparator stays a strict weak order.
                 hrow.resize((size_t)rows * cols);
                 CK(cudaMemcpy2DAsync(hrow.data(), (size_t)cols * 4, c->d_logits, CH * 4, (size_t)cols * 4, rows, cudaMemcpyDeviceToHost, c->stream));
                 CK(cudaStreamSynchronize(c->stream));
+                for (float& v : hrow) if (v != v) v = -FLT_MAX;
                 hidx.resize(cols);
                 for (int i = 0; i < rows; i++) {
                     const float* r = hrow.data() + (size_t)i * cols;
@@ -1351,9 +1357,18 @@ void* clip_b200_device_malloc(const struct clip_ctx* c, size_t bytes) {
 void clip_b200_device_free(const struct clip_ctx* c, void* p) { if (c) cudaSetDevice(c->device); cudaFree(p); }
 void* clip_b200_host_malloc(size_t bytes) { void* p = nullptr; if (cudaMallocHost(&p, bytes) != cudaSuccess) return nullptr; return p; }
 void clip_b200_host_free(void* p) { cudaFreeHost(p); }
+// Returns once the bytes are on the device.  A plain cudaMemcpy from pageable memory may return while its last DMA is still in
+// flight, and the context's streams are non-blocking (not ordered after the legacy default stream), so the next launch could read
+// the buffer's tail before it lands.  The copy therefore goes on the context's stream, which every later launch is ordered after.
 bool clip_b200_memcpy_h2d(const struct clip_ctx* c, void* d, const void* h, size_t bytes) {
-    if (c) cudaSetDevice(c->device);
-    CK(cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice));
+    if (!c) {
+        CK(cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice));
+        CK(cudaDeviceSynchronize());
+        return true;
+    }
+    CK(cudaSetDevice(c->device));
+    CK(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
     return true;
 }
 bool clip_b200_memcpy_d2h(const struct clip_ctx* c, void* h, const void* d, size_t bytes) {

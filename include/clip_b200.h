@@ -173,12 +173,17 @@ bool clip_b200_text_encode_device(const struct clip_ctx * ctx, const void * d_id
                                   int seq_len, void * d_vec, bool normalize);
 
 /* Batched zero-shot scoring on the device (clip.cpp:1624-1659 semantics per image): d_img_vec [n_img, d], d_txt_vec [n_txt, d]
- * -> host scores/indices [n_img, top_k], best first; similarity matrix, softmax and top-k selection all run on the GPU. */
+ * -> host scores/indices [n_img, top_k], best first; similarity matrix, softmax and top-k selection all run on the GPU.
+ * Ranking (here and in clip_b200_topk_search): top_k <= 0 or top_k > n_txt means all n_txt, and row i of the output starts at
+ * i * (that clamped top_k).  Equal scores are ordered by lower index first.  A NaN score ranks last and is reported as -FLT_MAX. */
 bool clip_b200_zero_shot_batch(const struct clip_ctx * ctx, const void * d_img_vec, size_t n_img, const void * d_txt_vec,
                                size_t n_txt, float * scores, int * indices, int top_k);
 
 /* Nearest-neighbour search on the device (stands in for USearch in examples/image-search/search.cpp:114-158): raw dot products
- * (cosine similarity for normalised embeddings) of n_queries x n_db device-resident vectors, best top_k per query to the host. */
+ * (cosine similarity for normalised embeddings) of n_queries x n_db device-resident vectors, best top_k per query to the host.
+ * Each score is one sequential fmaf chain over the d features.  top_k <= 0 or top_k > n_db means all n_db, and row i of the output
+ * starts at i * (that clamped top_k).  Equal scores are ordered by lower index first.  A NaN score ranks last and is reported as
+ * -FLT_MAX. */
 bool clip_b200_topk_search(const struct clip_ctx * ctx, const void * d_queries, size_t n_queries, const void * d_db, size_t n_db,
                            int top_k, float * scores, int * indices);
 
@@ -221,7 +226,8 @@ bool clip_b200_image_batch_encode_all(const struct clip_ctx * ctx, const int n_t
 bool clip_b200_text_batch_encode_all(const struct clip_ctx * ctx, const int n_threads, const struct clip_tokens * seqs,
                                      const size_t n, float * vec_all, const bool normalize);
 
-/* memory + stream helpers so that a plain C caller needs no CUDA headers */
+/* memory + stream helpers so that a plain C caller needs no CUDA headers.  clip_b200_memcpy_h2d returns once the bytes are on the
+ * device, so the context's next call reads all of them, pageable source or not. */
 void * clip_b200_device_malloc(const struct clip_ctx * ctx, size_t bytes);
 void   clip_b200_device_free(const struct clip_ctx * ctx, void * p);
 void * clip_b200_host_malloc(size_t bytes);            /* pinned */

@@ -59,6 +59,53 @@ def token_seqs(n, tok_seed=99):
     return [sg.synth_tokens(1, TOK_LENS[i % len(TOK_LENS)], tok_seed + i)[0] for i in range(n)]
 
 
+# ---- device scoring references (tests/test_gpu_scoring.py, tests/test_gpu_scoring_exact.py) -----------------------------------
+def fmaf32(a, b, c):
+    """fmaf(a, b, c) of float32 values (numpy arrays, broadcast), correctly rounded to nearest even, as float32.  The product of
+    two float32 is exact in fp64 (24 + 24 <= 53 bits).  The fp64 sum p + c is then rounded to odd: TwoSum gives its rounding
+    error, and a nonzero error on an even mantissa moves the sum one ulp towards it.  Rounding that once to float32 is the
+    correctly rounded fma, because 53 >= 24 + 2 (a plain fp64 sum could land on a float32 tie the exact value is not on)."""
+    p = np.asarray(a, np.float64) * np.asarray(b, np.float64)
+    c = np.asarray(c, np.float64)
+    s = p + c
+    t = s - p
+    err = (p - (s - t)) + (c - t)
+    bits = s.view(np.int64)
+    odd = (err != 0) & ((bits & 1) == 0) & np.isfinite(s)
+    bits += odd * np.where((err > 0) == (s > 0), 1, -1)
+    return s.astype(np.float32)
+
+
+def fmaf_chain_dot(a, b):
+    """S[i, j] = acc after acc = fmaf(a[i, k], b[j, k], acc) for k = 0 .. d-1 from acc = +0, as float32 [len(a), len(b)]: one
+    sequential fused chain per entry, the order csrc/search.cu's sim_kernel accumulates in."""
+    a = np.asarray(a, np.float64)
+    bt = np.ascontiguousarray(np.asarray(b, np.float64).T)
+    s = np.empty((len(a), bt.shape[1]), np.float32)
+    rows = max(1, 32768 // bt.shape[1])                      # a few rows at a time keep the working set in cache
+    for r0 in range(0, len(a), rows):
+        acc = np.zeros((len(a[r0:r0 + rows]), bt.shape[1]), np.float32)
+        for k in range(a.shape[1]):
+            acc = fmaf32(a[r0:r0 + rows, k:k + 1], bt[k], acc)
+        s[r0:r0 + rows] = acc
+    return s
+
+
+def softmax_sorted(s):
+    """softmax_with_sorting's arithmetic (clip.cpp:1599-1607) per row -- e = float32(exp(float64(s)) + 1e-9), the sum of the
+    rounded e in fp64, p = float32(e / sum) -- sorted by (p descending, index ascending): returns (p sorted, order)."""
+    s = np.asarray(s, np.float32)
+    e = (np.exp(s.astype(np.float64)) + 1e-9).astype(np.float32)
+    p = (e.astype(np.float64) / e.astype(np.float64).sum(-1, keepdims=True)).astype(np.float32)
+    order = np.argsort(-p, axis=-1, kind="stable")
+    return np.take_along_axis(p, order, -1), order
+
+
+def ulp_dist(a, b):
+    """|a - b| in float32 ulps, for float32 arrays of one sign (the integer views are then ordered like the values)"""
+    return np.abs(np.asarray(a, np.float32).view(np.int32).astype(np.int64) - np.asarray(b, np.float32).view(np.int32))
+
+
 def one_minus_cos(a, b):
     a = np.asarray(a, np.float64)
     b = np.asarray(b, np.float64)

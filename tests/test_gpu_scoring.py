@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 import synth_gguf as sg
-from _util import check_sha, model_file, one_minus_cos, reference_runs, token_seqs
+from _util import check_sha, fmaf_chain_dot, model_file, one_minus_cos, reference_runs, softmax_sorted, token_seqs, ulp_dist
 
 pytestmark = pytest.mark.gpu
 
@@ -24,15 +24,6 @@ def _u8(nx, ny, seed):
 
 def live_u8():
     return _u8(120, 90, 5)
-
-
-def _softmax_sorted(s):
-    """softmax_with_sorting's arithmetic (clip.cpp:1599-1607) with a stable, index-ascending tie order."""
-    s = np.asarray(s, np.float32)
-    e = (np.exp(s.astype(np.float64)) + 1e-9).astype(np.float32)
-    p = (e.astype(np.float64) / e.astype(np.float64).sum(-1, keepdims=True)).astype(np.float32)
-    order = np.argsort(-p, axis=-1, kind="stable")
-    return np.take_along_axis(p, order, -1), order
 
 
 # |score - reference| bounds: the two embeddings may each differ by the north-star tolerance (1 - cos <= 1e-3 / 1e-2, i.e. an angle
@@ -90,16 +81,11 @@ def test_zero_shot_batch_device_topk(prod, n_img, n_txt, k):
         prod.lib.clip_b200_device_free(ctx, d_t)
     finally:
         prod.free(ctx)
-    s = (img.astype(np.float64) @ txt.astype(np.float64).T).astype(np.float32)
-    p_sorted, order = _softmax_sorted(s)
-    assert np.allclose(scores, p_sorted[:, :k], rtol=2e-4, atol=1e-9)
-    # identical ranking, except that labels whose probabilities agree to rounding may swap places
-    p_full = (np.exp(s.astype(np.float64)) + 1e-9) / (np.exp(s.astype(np.float64)) + 1e-9).sum(1, keepdims=True)
-    r, c = np.nonzero(idx != order[:, :k])
-    for ri, ci in zip(r, c):
-        assert np.isclose(p_full[ri, idx[ri, ci]], p_full[ri, order[ri, ci]], rtol=2e-4), (ri, ci)
-    assert len(r) <= 0.02 * idx.size + 2
-    assert (np.sort(idx, 1)[:, 1:] != np.sort(idx, 1)[:, :-1]).all()           # no index reported twice
+    # the device's similarities are these fmaf chains bit for bit (tests/test_gpu_scoring_exact.py), so the softmax reference
+    # sees the same logits: the ranking is exact and each probability within 1 ulp (fp64 sums in another order)
+    p_sorted, order = softmax_sorted(fmaf_chain_dot(img, txt))
+    assert np.array_equal(idx, order[:, :k]), (idx != order[:, :k]).sum()
+    assert ulp_dist(scores, p_sorted[:, :k]).max() <= 1
 
 
 @pytest.mark.parametrize("nq,ndb,k", [(1, 300, 10), (3, 20000, 10), (70, 4097, 1)])
@@ -121,12 +107,11 @@ def test_topk_search_raw_similarity(prod, nq, ndb, k):
                                               idx.ctypes.data_as(C.POINTER(C.c_int))), prod.last_error()
     finally:
         prod.free(ctx)
-    s = q.astype(np.float64) @ db.astype(np.float64).T
+    s = fmaf_chain_dot(q, db)                                # the device's similarities, bit for bit
     order = np.argsort(-s, axis=1, kind="stable")[:, :k]
     assert idx[0, 0] == 123 % ndb and abs(scores[0, 0] - 1.0) < 1e-5
-    assert np.allclose(scores, np.take_along_axis(s, order, 1), atol=2e-6)
-    agree = (idx == order).mean()
-    assert agree > 0.95, agree                               # fp32 vs fp64 may swap near-equal neighbours
+    assert np.array_equal(idx, order), (idx != order).sum()
+    assert np.array_equal(scores, np.take_along_axis(s, order, 1))
 
 
 def test_zero_shot_images_single_gpu_equals_composition(prod):
@@ -139,7 +124,7 @@ def test_zero_shot_images_single_gpu_equals_composition(prod):
             sc, ix = prod.zero_shot_images(ctx, imgs, labels, 4, normalize=normalize)
             iv = prod.image_batch_encode(ctx, imgs, normalize=normalize)
             tv = prod.text_batch_encode(ctx, labels, normalize=normalize)
-            p, order = _softmax_sorted(iv @ tv.T)
+            p, order = softmax_sorted(iv @ tv.T)
             assert np.array_equal(ix, order[:, :4])
             assert np.allclose(sc, p[:, :4], rtol=1e-4)
     finally:
