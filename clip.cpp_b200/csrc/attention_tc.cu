@@ -1,19 +1,29 @@
 // attention_tc.cu -- K3 on Hopper tensor cores: S = Q K^T and O = P V as warpgroup MMAs (wgmma), online softmax in registers.
 //
 // Reference semantics: clip.cpp:1082-1108 (text, causal) / 1363-1388 (vision); soft_max ggml.c:12201-12270.
-// One CTA per (128-query tile, head, sequence), 288 threads, 81 KB (head_dim 64) or 101 KB (head_dim 80) of shared memory:
-//   warp 8      producer, one thread: TMA of the Q tile [128 x dh], then K and V blocks [128 keys x dh] into a two-deep ring, all
-//               straight out of the fused QKV activation matrix through a 3-D view [sequence][token][column]: rows past a sequence's
-//               T tokens arrive as zeros, so padded keys can never inject another sequence's (or stale) NaN / Inf into P.V
-//   warps 0-7   two consumer warpgroups, 64 query rows each.  Per key block: S[64 x 128] = Q.K^T (wgmma m64n128k16, both operands
-//               from shared memory), length / causal mask, online softmax (running row max and sum, quad shuffles), the probabilities
-//               re-packed IN REGISTERS as 16-bit A fragments, O[64 x dh] += P.V (wgmma m64n64k16 per 16 keys, A from registers, V read
-//               MN-major from the same [key][dh] tile).  O / l -> 16-bit stores.
+// Persistent: min(iterations, SMs) CTAs of 288 threads, 161 KB (head_dim 64) or 201 KB (head_dim 80) of shared memory.  The work unit is
+// a GROUP of 64 query rows, numbered in (sequence, head, group) order; iteration `it` of the launch takes groups 2it and 2it + 1, one
+// per consumer warpgroup, and CTA b runs iterations b, b + grid, ...  So the CTAs running at one time cover consecutive groups, and the
+// K / V blocks of a (sequence, head) are read from HBM about once and then from L2.  A group never holds a row past T; only the odd
+// group at the very end leaves a warpgroup without work.
+//   warp 8      producer, one thread: TMA of both groups' Q rows into a two-deep Q ring, then K and V in 128-key blocks into a two-deep
+//               ring whose stages have a slot per head: when the two groups belong to two (sequence, head)s, both heads' blocks are
+//               loaded.  All straight out of the fused QKV activation matrix through a 3-D view [sequence][token][column], in boxes of
+//               64 rows: rows past a sequence's T tokens arrive as zeros, so padded keys can never inject another sequence's (or stale)
+//               NaN / Inf into P.V, and a box wholly past the last key a group uses is not loaded.  The producer's ring positions run on
+//               across iterations, so the next item's Q and first K / V blocks arrive while the consumers finish the current one.
+//   warps 0-7   two consumer warpgroups, one group each.  Per key block: S[64 x W] = Q.K^T (wgmma m64nWk16, both operands from shared
+//               memory; W = 128 except in the last block, where it is the least of 16, 32, 64, 128 that covers the keys left), length /
+//               causal mask, online softmax (running row max and sum, quad shuffles), the probabilities re-packed IN REGISTERS as
+//               16-bit A fragments, O[64 x dh] += P.V (wgmma m64n64k16 per 16 keys, A from registers, V read MN-major from the same
+//               [key][dh] tile, 8 NT / 16 steps).  O / l -> 16-bit stores.
+// Trimmed keys only ever contributed -inf to a row maximum and exact zeros to sums, so every output has the bits of the full-width
+// computation.
 // head_dim 80 (ViT-H/14): a 128-byte-swizzle box holds at most 64 sixteen-bit columns, and a wider box would reach into the next
-// head (the tensor map's zero fill stops only at token and matrix ends, not at head boundaries).  So every Q / K / V tile arrives
+// head (the tensor map's zero fill stops only at token and matrix ends, not at head boundaries).  So every Q / K / V box arrives
 // as two pieces from two tensor maps over the same buffer: columns 0-63 (128-byte swizzle) and 64-79 (32-byte swizzle).  S takes
 // one extra k16 step on the tail pieces, O one extra m64n16k16 wgmma per 16 keys into 8 more accumulators per thread.
-// HBM traffic: Q read once, K and V once per query tile, O written once.  Any T; a causal tile stops at its diagonal block.
+// Any T; a causal group stops at its own diagonal.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -25,27 +35,32 @@ namespace cb {
 
 namespace {
 
-constexpr int AQ = 128, AK = 128;
+constexpr int AG = 64, AK = 128;                       // query rows per group, keys per block
+constexpr int ABOX = 64;                               // rows per TMA box
 constexpr int ATT_THREADS = 288;                       // 2 consumer warpgroups + 1 producer warp
 
-// Shared-memory layout for one head_dim: every Q, K or V tile is [128 rows x 64 columns] (128-byte swizzle), followed for
-// head_dim 80 by [128 rows x 16 columns] (32-byte swizzle).  Q tile, then two stages [K | V].
+// Shared-memory layout for one head_dim.  A TILE is [128 rows x 64 columns] (128-byte swizzle), followed for head_dim 80 by
+// [128 rows x 16 columns] (32-byte swizzle); a 64-row box fills half of each part.  Two Q tiles (rows 0-63: the first group, 64-127: the
+// second), then two stages of two head slots [K | V].
 template <int DH>
 struct AttnGeo {
     static_assert(DH == 64 || DH == 80, "head_dim 64 or 80");
     static constexpr bool TAIL = DH == 80;
     static constexpr uint32_t MAIN = AK * 128, TILE = MAIN + (TAIL ? AK * 32 : 0);
-    static constexpr uint32_t KV_OFF = TILE;
-    static constexpr uint32_t BAR_OFF = KV_OFF + 4 * TILE;
+    static constexpr uint32_t BOX_BYTES = ABOX * (128 + (TAIL ? 32 : 0));      // one 64-row box, both pieces
+    static constexpr uint32_t KV_OFF = 2 * TILE;
+    static constexpr uint32_t BAR_OFF = KV_OFF + 8 * TILE;
     static constexpr uint32_t SMEM = BAR_OFF + 64 + 1024;
-    static_assert(AQ == AK && MAIN % 1024 == 0 && TILE % 1024 == 0, "tile alignment");
+    static_assert(2 * AG == AK && 2 * ABOX == AK && MAIN % 1024 == 0 && TILE % 1024 == 0, "tile alignment");
 };
 
 struct AParams {
     CUtensorMap tm_qkv;     // boxes of columns 0-63 of a head
     CUtensorMap tm_tail;    // head_dim 80: boxes of columns 64-79
     uint16_t* out;
-    int T, H, ntile, causal;
+    int T, H, causal;
+    int ngrp;               // 64-row groups per (sequence, head)
+    int ngroups, niter;     // groups in the launch, iterations (pairs of groups)
 };
 
 CB_DEVINL void tma_load_3d(uint32_t dst_smem, const void* tmap, int c0, int c1, int c2, uint32_t bar) {
@@ -62,19 +77,147 @@ CB_DEVINL uint32_t pack2(float lo, float hi) {
     else asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
     return r;
 }
+
+// One group of 64 query rows: its (sequence, head), first row and the end of the keys any of its rows can see
+struct Group {
+    int seq, head, g0, kend;
+};
+CB_DEVINL Group group_of(const AParams& p, int g) {
+    const int sh = g / p.ngrp;
+    Group r;
+    r.g0 = (g - sh * p.ngrp) * AG;
+    r.head = sh % p.H;
+    r.seq = sh / p.H;
+    r.kend = p.causal ? min(p.T, r.g0 + AG) : p.T;
+    return r;
+}
+
+// The two groups of iteration `it` and what the K / V stages hold for them: slot 0 the first group's head (and the second's, when it
+// is the same (sequence, head) or there is no second group), slot 1 the second group's head otherwise.  kend0 / kend1: the keys a
+// slot must hold (0: slot unused); nkb: key blocks of the iteration.
+struct Iter {
+    Group a, b;
+    bool has_b, shared;
+    int kend0, kend1, nkb;
+};
+CB_DEVINL Iter iter_of(const AParams& p, int it) {
+    Iter r;
+    r.has_b = 2 * it + 1 < p.ngroups;
+    r.a = group_of(p, 2 * it);
+    r.b = group_of(p, r.has_b ? 2 * it + 1 : 2 * it);
+    r.shared = r.a.seq == r.b.seq && r.a.head == r.b.head;
+    r.kend0 = r.shared ? max(r.a.kend, r.b.kend) : r.a.kend;
+    r.kend1 = r.shared ? 0 : r.b.kend;
+    r.nkb = (max(r.kend0, r.kend1) + AK - 1) / AK;
+    return r;
+}
+
+// 64-row boxes of key block kb that a slot holding keys [0, kend) needs
+CB_DEVINL int kv_boxes(int kend, int kb) {
+    const int key0 = kb * AK;
+    return key0 >= kend ? 0 : key0 + ABOX >= kend ? 1 : 2;
+}
+
+// one 64-row box (both pieces at head_dim 80) into box `b` of the tile at `tile`
+template <int DH>
+CB_DEVINL void load_box(uint32_t tile, int b, const AParams& p, int col, int row, int seq, uint32_t bar) {
+    using G = AttnGeo<DH>;
+    tma_load_3d(tile + (uint32_t)b * (ABOX * 128), &p.tm_qkv, col, row, seq, bar);
+    if constexpr (G::TAIL) tma_load_3d(tile + G::MAIN + (uint32_t)b * (ABOX * 32), &p.tm_tail, col + 64, row, seq, bar);
+}
+
+template <bool BF, int NT>
+CB_DEVINL void wgmma_ss_nt(float (&d)[4 * NT], uint64_t da, uint64_t db, uint32_t accumulate) {
+    if constexpr (NT == 16) wgmma_ss_n128<BF>(d, da, db, accumulate);
+    else if constexpr (NT == 8) wgmma_ss_n64<BF>(d, da, db, accumulate);
+    else if constexpr (NT == 4) wgmma_ss_n32<BF>(d, da, db, accumulate);
+    else wgmma_ss_n16<BF>(d, da, db, accumulate);
+}
+
+// One key block of one consumer warpgroup, S NT n-tiles (8 keys each) wide: keys [key0, key0 + 8 NT) of the stage at k_s / v_s.
+// The same operations in the same order as the full 128-key block: the keys past 8 NT would only have been masked to -inf.
+template <bool BF, int DH, int NT>
+CB_DEVINL void attend_block(float (&o)[32], float (&ot)[8], float (&m_run)[2], float (&l_run)[2], uint64_t dq, uint64_t dq_t,
+                            uint32_t k_s, uint32_t v_s, int key0, int T, int causal, int wrow0, int r0, int tc) {
+    using G = AttnGeo<DH>;
+    constexpr float LOG2E = 1.4426950408889634f;
+    float sc[4 * NT];
+    const uint64_t dk = wgmma_desc_sw128(k_s);
+    wgmma_fence();
+    #pragma unroll
+    for (int k = 0; k < 4; k++) wgmma_ss_nt<BF, NT>(sc, dq + 2 * k, dk + 2 * k, (uint32_t)k);
+    if constexpr (G::TAIL) wgmma_ss_nt<BF, NT>(sc, dq_t, wgmma_desc_sw32(k_s + G::MAIN), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sc);
+    // masking is only needed in the last (ragged) key block and, for the causal text tower, on the diagonal block
+    if (key0 + 8 * NT > T || (causal && key0 + 8 * NT - 1 > wrow0)) {
+        #pragma unroll
+        for (int j = 0; j < NT; j++) {
+            #pragma unroll
+            for (int e = 0; e < 4; e++) {
+                const int key = key0 + 8 * j + tc + (e & 1), row = r0 + 8 * (e >> 1);
+                if (key >= T || (causal && key > row)) sc[4 * j + e] = -INFINITY;
+            }
+        }
+    }
+    #pragma unroll
+    for (int h = 0; h < 2; h++) {
+        float mx = -INFINITY;
+        #pragma unroll
+        for (int j = 0; j < NT; j++) mx = fmaxf(mx, fmaxf(sc[4 * j + 2 * h], sc[4 * j + 2 * h + 1]));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        // every row (padded rows past T included: zero queries) sees at least one unmasked key per visited block
+        const float m_new = fmaxf(m_run[h], mx);
+        const float alpha = ex2f((m_run[h] - m_new) * LOG2E), mb = m_new * LOG2E;
+        float rs = 0.f;
+        #pragma unroll
+        for (int j = 0; j < NT; j++) {
+            const float p0 = ex2f(sc[4 * j + 2 * h] * LOG2E - mb), p1 = ex2f(sc[4 * j + 2 * h + 1] * LOG2E - mb);
+            sc[4 * j + 2 * h] = p0; sc[4 * j + 2 * h + 1] = p1;
+            rs += p0 + p1;
+        }
+        l_run[h] = l_run[h] * alpha + rs;
+        m_run[h] = m_new;
+        #pragma unroll
+        for (int j = 0; j < 8; j++) { o[4 * j + 2 * h] *= alpha; o[4 * j + 2 * h + 1] *= alpha; }
+        if constexpr (G::TAIL) {
+            #pragma unroll
+            for (int j = 0; j < 2; j++) { ot[4 * j + 2 * h] *= alpha; ot[4 * j + 2 * h + 1] *= alpha; }
+        }
+    }
+    // O += P.V: key step kk covers S n-tiles 2kk (A fragment registers 0, 1) and 2kk + 1 (registers 2, 3).  Keys in [kend, key0 + 8 NT)
+    // have P = 0 and zero-filled V rows (they lie past T); a data-dependent skip of their steps would make ptxas serialize the chain.
+    wgmma_fence();
+    #pragma unroll
+    for (int kk = 0; kk < NT / 2; kk++) {
+        const uint32_t a[4] = {pack2<BF>(sc[8 * kk], sc[8 * kk + 1]), pack2<BF>(sc[8 * kk + 2], sc[8 * kk + 3]),
+                               pack2<BF>(sc[8 * kk + 4], sc[8 * kk + 5]), pack2<BF>(sc[8 * kk + 6], sc[8 * kk + 7])};
+        wgmma_rs_n64_bmn<BF>(o, a, wgmma_desc_sw128(v_s + (uint32_t)kk * 2048u), 1u);      // 16 keys = 2048 B of V
+        if constexpr (G::TAIL) wgmma_rs_n16_bmn<BF>(ot, a, wgmma_desc_sw32(v_s + G::MAIN + (uint32_t)kk * 512u), 1u);   // 512 B
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    if constexpr (G::TAIL) wgmma_fence_regs(ot);
+}
+
 template <bool BF, int DH>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __grid_constant__ AParams p) {
     using G = AttnGeo<DH>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     const uint32_t smem_base = smem_u32(smem);
-    const uint32_t q_full = smem_base + G::BAR_OFF, kv_full = q_full + 8, kv_empty = q_full + 24;     // kv rings: [0|1] = +8 bytes
+    // rings of two, [0|1] = +8 bytes: Q tile full / empty, K-V stage full / empty
+    const uint32_t q_full = smem_base + G::BAR_OFF, q_empty = q_full + 16, kv_full = q_full + 32, kv_empty = q_full + 48;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int qt = blockIdx.x % p.ntile, head = (blockIdx.x / p.ntile) % p.H, seq = blockIdx.x / (p.ntile * p.H);
     if (threadIdx.x == 0) {
-        mbar_init(q_full, 1);
-        for (int i = 0; i < 2; i++) { mbar_init(kv_full + 8 * i, 1); mbar_init(kv_empty + 8 * i, 8); }   // released by each consumer warp
+        for (int i = 0; i < 2; i++) {
+            mbar_init(q_full + 8 * i, 1); mbar_init(q_empty + 8 * i, 8);          // released by each consumer warp
+            mbar_init(kv_full + 8 * i, 1); mbar_init(kv_empty + 8 * i, 8);
+        }
         mbar_fence_init();
         tma_prefetch_desc(&p.tm_qkv);
         if constexpr (G::TAIL) tma_prefetch_desc(&p.tm_tail);
@@ -83,24 +226,36 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __gr
     pdl_trigger();
     pdl_wait();      // qkv is read (and the output written) only after the QKV GEMM grid has completed
 
-    const int hid = p.H * DH, c = head * DH, q0 = qt * AQ;
-    const int kend = p.causal ? min(p.T, q0 + AQ) : p.T;      // keys any row of this tile can see
-    const int nkb = (kend + AK - 1) / AK;
-
+    const int hid = p.H * DH;
+    // Ring positions run on across iterations: the i-th iteration of this CTA uses Q tile i % 2 (its (i / 2)-th use), the n-th key
+    // block of this CTA stage n % 2 (its (n / 2)-th use).  A use waits for full with the use's parity and, in the producer, for the
+    // release of the previous use of the slot (parity flipped: the first wait on a fresh barrier passes).
     if (warp == 8) {
         // ------------------------------------------------------------------ producer (one thread)
         if (lane == 0) {
-            mbar_arrive_expect_tx(q_full, G::TILE);
-            tma_load_3d(smem_base, &p.tm_qkv, c, q0, seq, q_full);
-            if constexpr (G::TAIL) tma_load_3d(smem_base + G::MAIN, &p.tm_tail, c + 64, q0, seq, q_full);
-            for (int kb = 0; kb < nkb; kb++) {
-                const uint32_t s = kb & 1, k_s = smem_base + G::KV_OFF + s * (2 * G::TILE);
-                mbar_wait(kv_empty + 8 * s, ((kb >> 1) & 1) ^ 1);
-                mbar_arrive_expect_tx(kv_full + 8 * s, 2 * G::TILE);
-                tma_load_3d(k_s, &p.tm_qkv, hid + c, kb * AK, seq, kv_full + 8 * s);
-                if constexpr (G::TAIL) tma_load_3d(k_s + G::MAIN, &p.tm_tail, hid + c + 64, kb * AK, seq, kv_full + 8 * s);
-                tma_load_3d(k_s + G::TILE, &p.tm_qkv, 2 * hid + c, kb * AK, seq, kv_full + 8 * s);
-                if constexpr (G::TAIL) tma_load_3d(k_s + G::TILE + G::MAIN, &p.tm_tail, 2 * hid + c + 64, kb * AK, seq, kv_full + 8 * s);
+            uint32_t n = 0, i = 0;
+            for (int it = blockIdx.x; it < p.niter; it += gridDim.x, i++) {
+                const Iter w = iter_of(p, it);
+                const uint32_t qb = i & 1, q_s = smem_base + qb * G::TILE;
+                mbar_wait(q_empty + 8 * qb, ((i >> 1) & 1) ^ 1);
+                mbar_arrive_expect_tx(q_full + 8 * qb, (w.has_b ? 2 : 1) * G::BOX_BYTES);
+                load_box<DH>(q_s, 0, p, w.a.head * DH, w.a.g0, w.a.seq, q_full + 8 * qb);
+                if (w.has_b) load_box<DH>(q_s, 1, p, w.b.head * DH, w.b.g0, w.b.seq, q_full + 8 * qb);
+                for (int kb = 0; kb < w.nkb; kb++, n++) {
+                    const uint32_t s = n & 1, bar = kv_full + 8 * s;
+                    const int nb0 = kv_boxes(w.kend0, kb), nb1 = kv_boxes(w.kend1, kb);
+                    mbar_wait(kv_empty + 8 * s, ((n >> 1) & 1) ^ 1);
+                    mbar_arrive_expect_tx(bar, (uint32_t)(nb0 + nb1) * 2 * G::BOX_BYTES);
+                    const uint32_t slot0 = smem_base + G::KV_OFF + s * (4 * G::TILE), slot1 = slot0 + 2 * G::TILE;
+                    for (int b = 0; b < nb0; b++) {
+                        load_box<DH>(slot0, b, p, hid + w.a.head * DH, kb * AK + b * ABOX, w.a.seq, bar);
+                        load_box<DH>(slot0 + G::TILE, b, p, 2 * hid + w.a.head * DH, kb * AK + b * ABOX, w.a.seq, bar);
+                    }
+                    for (int b = 0; b < nb1; b++) {
+                        load_box<DH>(slot1, b, p, hid + w.b.head * DH, kb * AK + b * ABOX, w.b.seq, bar);
+                        load_box<DH>(slot1 + G::TILE, b, p, 2 * hid + w.b.head * DH, kb * AK + b * ABOX, w.b.seq, bar);
+                    }
+                }
             }
         }
         return;
@@ -108,104 +263,61 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __gr
 
     // ---------------------------------------------------------------------- consumers (fragment layout: wgmma.cuh)
     const int wg = warp >> 2;
-    const int wrow0 = q0 + wg * 64 + (warp & 3) * 16;          // first query row of this warp
-    const int r0 = wrow0 + (lane >> 2), tc = 2 * (lane & 3);   // this thread: rows r0 and r0 + 8, columns 8j + tc + {0, 1}
-    const bool live = q0 + wg * 64 < p.T;                      // warpgroup-uniform: T = 257 leaves one of the last tile's groups idle
-    const float LOG2E = 1.4426950408889634f;
-    // o: columns 0-63, ot: columns 64-79 (head_dim 80 only)
-    float o[32], ot[8], m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-    #pragma unroll
-    for (int i = 0; i < 32; i++) o[i] = 0.f;
-    #pragma unroll
-    for (int i = 0; i < 8; i++) ot[i] = 0.f;
-    mbar_wait(q_full, 0);
-    const uint64_t dq = wgmma_desc_sw128(smem_base + (uint32_t)wg * 64u * 128u);
-    const uint64_t dq_t = wgmma_desc_sw32(smem_base + G::MAIN + (uint32_t)wg * 64u * 32u);
-    for (int kb = 0; kb < nkb; kb++) {
-        const uint32_t s = kb & 1, k_s = smem_base + G::KV_OFF + s * (2 * G::TILE), v_s = k_s + G::TILE;
-        mbar_wait(kv_full + 8 * s, (kb >> 1) & 1);
-        if (live) {
-            float sc[64];
-            const uint64_t dk = wgmma_desc_sw128(k_s);
-            wgmma_fence();
-            #pragma unroll
-            for (int k = 0; k < 4; k++) wgmma_ss_n128<BF>(sc, dq + 2 * k, dk + 2 * k, (uint32_t)k);
-            if constexpr (G::TAIL) wgmma_ss_n128<BF>(sc, dq_t, wgmma_desc_sw32(k_s + G::MAIN), 1u);
-            wgmma_commit();
-            wgmma_wait<0>();
-            wgmma_fence_regs(sc);
-            const int key0 = kb * AK;
-            // masking is only needed in the last (ragged) key block and, for the causal text tower, on the diagonal block
-            if (key0 + AK > p.T || (p.causal && key0 + AK - 1 > wrow0)) {
-                #pragma unroll
-                for (int j = 0; j < AK / 8; j++) {
-                    #pragma unroll
-                    for (int e = 0; e < 4; e++) {
-                        const int key = key0 + 8 * j + tc + (e & 1), row = r0 + 8 * (e >> 1);
-                        if (key >= p.T || (p.causal && key > row)) sc[4 * j + e] = -INFINITY;
-                    }
-                }
+    const int tc = 2 * (lane & 3);                             // this thread: columns 8j + tc + {0, 1}
+    uint32_t n = 0, i = 0;
+    for (int it = blockIdx.x; it < p.niter; it += gridDim.x, i++) {
+        const Iter w = iter_of(p, it);
+        const Group g = group_of(p, min(2 * it + wg, p.ngroups - 1));
+        const bool live = wg == 0 || w.has_b;                  // warpgroup-uniform: only the launch's last, odd group leaves one idle
+        const uint32_t slot = (wg == 0 || w.shared) ? 0u : 1u;
+        const int nkb = (g.kend + AK - 1) / AK;
+        const int wrow0 = g.g0 + (warp & 3) * 16;              // first query row of this warp
+        const int r0 = wrow0 + (lane >> 2);                    // this thread: rows r0 and r0 + 8
+        // o: columns 0-63, ot: columns 64-79 (head_dim 80 only)
+        float o[32], ot[8], m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+        #pragma unroll
+        for (int j = 0; j < 32; j++) o[j] = 0.f;
+        #pragma unroll
+        for (int j = 0; j < 8; j++) ot[j] = 0.f;
+        const uint32_t qb = i & 1, q_s = smem_base + qb * G::TILE;
+        mbar_wait(q_full + 8 * qb, (i >> 1) & 1);
+        const uint64_t dq = wgmma_desc_sw128(q_s + (uint32_t)wg * 64u * 128u);
+        const uint64_t dq_t = wgmma_desc_sw32(q_s + G::MAIN + (uint32_t)wg * 64u * 32u);
+        for (int kb = 0; kb < w.nkb; kb++, n++) {
+            const uint32_t s = n & 1;
+            const uint32_t k_s = smem_base + G::KV_OFF + s * (4 * G::TILE) + slot * (2 * G::TILE), v_s = k_s + G::TILE;
+            mbar_wait(kv_full + 8 * s, (n >> 1) & 1);
+            if (live && kb < nkb) {
+                const int key0 = kb * AK, rem = g.kend - key0;
+                if (rem > 64) attend_block<BF, DH, 16>(o, ot, m_run, l_run, dq, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
+                else if (rem > 32) attend_block<BF, DH, 8>(o, ot, m_run, l_run, dq, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
+                else if (rem > 16) attend_block<BF, DH, 4>(o, ot, m_run, l_run, dq, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
+                else attend_block<BF, DH, 2>(o, ot, m_run, l_run, dq, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
             }
-            #pragma unroll
-            for (int h = 0; h < 2; h++) {
-                float mx = -INFINITY;
+            __syncwarp();
+            if (lane == 0) mbar_arrive(kv_empty + 8 * s);
+        }
+        // every S product that read this Q tile has completed (wgmma_wait<0> in attend_block)
+        __syncwarp();
+        if (lane == 0) mbar_arrive(q_empty + 8 * qb);
+        if (!live) continue;
+        #pragma unroll
+        for (int h = 0; h < 2; h++) {
+            float l = l_run[h];
+            l += __shfl_xor_sync(0xffffffffu, l, 1);
+            l += __shfl_xor_sync(0xffffffffu, l, 2);
+            const float inv = 1.0f / l;
+            const int row = r0 + 8 * h;
+            if (row < p.T) {
+                uint16_t* orow = p.out + ((size_t)g.seq * p.T + row) * hid + g.head * DH;
                 #pragma unroll
-                for (int j = 0; j < AK / 8; j++) mx = fmaxf(mx, fmaxf(sc[4 * j + 2 * h], sc[4 * j + 2 * h + 1]));
-                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-                // every row (padded rows past T included: zero queries) sees at least one unmasked key per visited block
-                const float m_new = fmaxf(m_run[h], mx);
-                const float alpha = ex2f((m_run[h] - m_new) * LOG2E), mb = m_new * LOG2E;
-                float rs = 0.f;
-                #pragma unroll
-                for (int j = 0; j < AK / 8; j++) {
-                    const float p0 = ex2f(sc[4 * j + 2 * h] * LOG2E - mb), p1 = ex2f(sc[4 * j + 2 * h + 1] * LOG2E - mb);
-                    sc[4 * j + 2 * h] = p0; sc[4 * j + 2 * h + 1] = p1;
-                    rs += p0 + p1;
-                }
-                l_run[h] = l_run[h] * alpha + rs;
-                m_run[h] = m_new;
-                #pragma unroll
-                for (int j = 0; j < 8; j++) { o[4 * j + 2 * h] *= alpha; o[4 * j + 2 * h + 1] *= alpha; }
+                for (int j = 0; j < 8; j++)
+                    *reinterpret_cast<uint32_t*>(orow + 8 * j + tc) = pack2<BF>(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
                 if constexpr (G::TAIL) {
                     #pragma unroll
-                    for (int j = 0; j < 2; j++) { ot[4 * j + 2 * h] *= alpha; ot[4 * j + 2 * h + 1] *= alpha; }
+                    for (int j = 0; j < 2; j++)
+                        *reinterpret_cast<uint32_t*>(orow + 64 + 8 * j + tc) = pack2<BF>(ot[4 * j + 2 * h] * inv, ot[4 * j + 2 * h + 1] * inv);
                 }
-            }
-            // O += P.V: key step kk covers S n-tiles 2kk (A fragment registers 0, 1) and 2kk + 1 (registers 2, 3)
-            wgmma_fence();
-            #pragma unroll
-            for (int kk = 0; kk < AK / 16; kk++) {
-                const uint32_t a[4] = {pack2<BF>(sc[8 * kk], sc[8 * kk + 1]), pack2<BF>(sc[8 * kk + 2], sc[8 * kk + 3]),
-                                       pack2<BF>(sc[8 * kk + 4], sc[8 * kk + 5]), pack2<BF>(sc[8 * kk + 6], sc[8 * kk + 7])};
-                wgmma_rs_n64_bmn<BF>(o, a, wgmma_desc_sw128(v_s + (uint32_t)kk * 2048u), 1u);      // 16 keys = 2048 B of V
-                if constexpr (G::TAIL) wgmma_rs_n16_bmn<BF>(ot, a, wgmma_desc_sw32(v_s + G::MAIN + (uint32_t)kk * 512u), 1u);   // 512 B
-            }
-            wgmma_commit();
-            wgmma_wait<0>();
-            wgmma_fence_regs(o);
-            if constexpr (G::TAIL) wgmma_fence_regs(ot);
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(kv_empty + 8 * s);
-    }
-    if (!live) return;
-    #pragma unroll
-    for (int h = 0; h < 2; h++) {
-        float l = l_run[h];
-        l += __shfl_xor_sync(0xffffffffu, l, 1);
-        l += __shfl_xor_sync(0xffffffffu, l, 2);
-        const float inv = 1.0f / l;
-        const int row = r0 + 8 * h;
-        if (row < p.T) {
-            uint16_t* orow = p.out + ((size_t)seq * p.T + row) * hid + c;
-            #pragma unroll
-            for (int j = 0; j < 8; j++)
-                *reinterpret_cast<uint32_t*>(orow + 8 * j + tc) = pack2<BF>(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
-            if constexpr (G::TAIL) {
-                #pragma unroll
-                for (int j = 0; j < 2; j++)
-                    *reinterpret_cast<uint32_t*>(orow + 64 + 8 * j + tc) = pack2<BF>(ot[4 * j + 2 * h] * inv, ot[4 * j + 2 * h + 1] * inv);
             }
         }
     }
@@ -215,7 +327,7 @@ typedef CUresult (*EncodeTiledFn3)(CUtensorMap*, CUtensorMapDataType, cuuint32_t
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// [nseq][T][3*H*dh] view of the fused QKV activations, box = `box_cols` columns x 128 tokens x 1 sequence (zero fill past T):
+// [nseq][T][3*H*dh] view of the fused QKV activations, box = `box_cols` columns x 64 tokens x 1 sequence (zero fill past T):
 // 64 columns with the 128-byte swizzle, or the 16-column tail of an 80-wide head with the 32-byte swizzle
 bool make_qkv_map(CUtensorMap* out, const void* qkv16, int nseq, int T, int H, int dh, int box_cols, CUtensorMapSwizzle swz) {
     static EncodeTiledFn3 enc = nullptr;
@@ -228,7 +340,7 @@ bool make_qkv_map(CUtensorMap* out, const void* qkv16, int nseq, int T, int H, i
     const cuuint64_t cols = (cuuint64_t)3 * H * dh;
     const cuuint64_t dims[3] = {cols, (cuuint64_t)T, (cuuint64_t)nseq};
     const cuuint64_t strides[2] = {cols * 2, cols * 2 * (cuuint64_t)T};
-    const cuuint32_t box[3] = {(cuuint32_t)box_cols, (cuuint32_t)AK, 1}, estr[3] = {1, 1, 1};
+    const cuuint32_t box[3] = {(cuuint32_t)box_cols, (cuuint32_t)ABOX, 1}, estr[3] = {1, 1, 1};
     return enc(out, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<void*>(qkv16), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
@@ -262,10 +374,18 @@ cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T,
     if (!make_qkv_map(&p.tm_qkv, qkv16, nseq, T, H, dh, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return cudaErrorInvalidValue;
     if (dh == 80 && !make_qkv_map(&p.tm_tail, qkv16, nseq, T, H, dh, 16, CU_TENSOR_MAP_SWIZZLE_32B)) return cudaErrorInvalidValue;
     p.out = (uint16_t*)out16; p.T = T; p.H = H; p.causal = causal;
-    p.ntile = (T + AQ - 1) / AQ;
-    const long long grid = (long long)nseq * H * p.ntile;
-    if (grid > 0x7fffffffll) return cudaErrorInvalidValue;
-    const cudaError_t e = dh == 80 ? launch_dh<80>(p, (unsigned)grid, bf16, st) : launch_dh<64>(p, (unsigned)grid, bf16, st);
+    p.ngrp = (T + AG - 1) / AG;
+    const long long ngroups = (long long)nseq * H * p.ngrp;
+    if (ngroups > 0x7ffffffell) return cudaErrorInvalidValue;
+    p.ngroups = (int)ngroups;
+    p.niter = (p.ngroups + 1) / 2;
+    // persistent: at most one CTA per SM (the shared memory admits no second one)
+    int dev = 0, sms = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) return e;
+    const unsigned grid = (unsigned)min(p.niter, sms);
+    e = dh == 80 ? launch_dh<80>(p, grid, bf16, st) : launch_dh<64>(p, grid, bf16, st);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 

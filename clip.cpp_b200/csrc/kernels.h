@@ -31,8 +31,8 @@ void launch_text_embed(const int32_t* ids, const float* tok, const float* pos, i
 // (CLIP_B200_ATTN=legacy).
 void launch_attention(const void* qkv16, void* out16, int nseq, int T, int H, int causal, int bf16, cudaStream_t st);
 
-// K3 on wgmma (attention_tc.cu): head_dim dh = 64 or 80 (anything else: cudaErrorInvalidValue), 128-query tiles, online softmax
-// over 128-key blocks, any T.  The Q / K / V boxes come from per-launch 3-D TMA views [sequence][token][column] of qkv16 (zero
+// K3 on wgmma (attention_tc.cu): head_dim dh = 64 or 80 (anything else: cudaErrorInvalidValue), a persistent grid over
+// 64-row query groups, online softmax over 128-key blocks, any T.  The Q / K / V boxes come from per-launch 3-D TMA views [sequence][token][column] of qkv16 (zero
 // fill past each sequence's T tokens).
 cudaError_t attention_tc_init();
 cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T, int H, int dh, int causal, int bf16, cudaStream_t st);

@@ -84,6 +84,42 @@ CB_DEVINL void wgmma_ss_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t 
 #undef CB_WGMMA_SS_N128
 }
 
+// D[64 x 64], D[64 x 32] and D[64 x 16] (+)= A[64 x 16] . B[N x 16]^T, both operands K-major in shared memory: the narrower S
+// products of the attention kernel's ragged last key block
+template <bool BF>
+CB_DEVINL void wgmma_ss_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+#define CB_WGMMA_SS_N64(TY)                                                                                 \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %34, 0;\n\t"                                                 \
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"  \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])  \
+                 : "l"(da), "l"(db), "r"(accumulate))
+    if constexpr (BF) CB_WGMMA_SS_N64("bf16");
+    else CB_WGMMA_SS_N64("f16");
+#undef CB_WGMMA_SS_N64
+}
+template <bool BF>
+CB_DEVINL void wgmma_ss_n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+#define CB_WGMMA_SS_N32(TY)                                                                                 \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %18, 0;\n\t"                                                 \
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"  \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])  \
+                 : "l"(da), "l"(db), "r"(accumulate))
+    if constexpr (BF) CB_WGMMA_SS_N32("bf16");
+    else CB_WGMMA_SS_N32("f16");
+#undef CB_WGMMA_SS_N32
+}
+template <bool BF>
+CB_DEVINL void wgmma_ss_n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t accumulate) {
+#define CB_WGMMA_SS_N16(TY)                                                                                 \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %10, 0;\n\t"                                                 \
+                 "wgmma.mma_async.sync.aligned.m64n16k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"  \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])  \
+                 : "l"(da), "l"(db), "r"(accumulate))
+    if constexpr (BF) CB_WGMMA_SS_N16("bf16");
+    else CB_WGMMA_SS_N16("f16");
+#undef CB_WGMMA_SS_N16
+}
+
 // D[64 x 64] (+)= A[64 x 16] . B[16 x 64]: A from registers (the m16n8k16 A-fragment layout per warp), B MN-major in shared memory
 template <bool BF>
 CB_DEVINL void wgmma_rs_n64_bmn(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
