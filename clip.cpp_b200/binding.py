@@ -79,7 +79,15 @@ EXTENSION_SYMBOLS = [
     # row-kernel test hooks
     "clip_b200_debug_layernorm", "clip_b200_debug_assemble_preln", "clip_b200_debug_im2col", "clip_b200_debug_text_embed",
     "clip_b200_debug_gather_rows", "clip_b200_debug_l2norm", "clip_b200_debug_fill_last",
+    # per-token hidden states
+    "clip_b200_image_tokens", "clip_b200_image_tokens_device", "clip_b200_text_tokens", "clip_b200_text_tokens_device",
+    "clip_b200_debug_token_rows",
 ]
+
+# include/clip_b200.h: output types and flags of the *_tokens entry points
+OUT_F32, OUT_F16, OUT_BF16 = 0, 1, 2
+OUT_DTYPES = {OUT_F32: np.float32, OUT_F16: np.float16, OUT_BF16: np.uint16}      # bf16 comes back as its raw 16-bit pattern
+TOKENS_POST_LN, TOKENS_PROJECT, TOKENS_NORMALIZE, TOKENS_NO_CLS = 1, 2, 4, 8
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 PRODUCT_LIB = os.environ.get("CLIP_B200_LIB") or os.path.join(HERE, "libclip_b200.so")     # CLIP_B200_LIB: experiment builds only
@@ -192,9 +200,18 @@ class ClipLib:
                             ("clip_b200_debug_text_embed", [i32p, fp, fp, ip, ip, ip, ip, fp]),
                             ("clip_b200_debug_gather_rows", [fp, ip, ip, ip, ip, i32p, fp, ip, fp]),
                             ("clip_b200_debug_l2norm", [fp, ip, ip, ip, fp]),
-                            ("clip_b200_debug_fill_last", [i32p, ip, ip, i32p])):
+                            ("clip_b200_debug_fill_last", [i32p, ip, ip, i32p]),
+                            ("clip_b200_debug_token_rows", [ip, ip, ip, C.c_size_t, ip, C.c_float, fp, fp, fp, ip, vp])):
                 getattr(L, f).restype = C.c_int
                 getattr(L, f).argtypes = args
+            L.clip_b200_image_tokens.restype = C.c_bool
+            L.clip_b200_image_tokens.argtypes = [vp, C.POINTER(clip_image_f32_batch), ip, ip, ip, vp]
+            L.clip_b200_image_tokens_device.restype = C.c_bool
+            L.clip_b200_image_tokens_device.argtypes = [vp, vp, C.c_size_t, ip, ip, ip, vp]
+            L.clip_b200_text_tokens.restype = C.c_bool
+            L.clip_b200_text_tokens.argtypes = [vp, i32p, C.c_size_t, ip, ip, ip, ip, vp]
+            L.clip_b200_text_tokens_device.restype = C.c_bool
+            L.clip_b200_text_tokens_device.argtypes = [vp, vp, C.c_size_t, ip, ip, ip, ip, vp]
             ipp = C.POINTER(C.c_int)
             L.clip_b200_topk_search.restype = C.c_bool
             L.clip_b200_topk_search.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, ip, fp, ipp]
@@ -320,6 +337,32 @@ class ClipLib:
                                              out.ctypes.data_as(C.POINTER(C.c_float)), normalize)
         if not ok:
             raise RuntimeError("clip_text_batch_encode failed: " + self.last_error())
+        return out
+
+    # ---- per-token hidden states (include/clip_b200.h) ------------------------------------------------------------------------
+    def token_shape(self, ctx, vision: bool, n: int, rows: int, flags: int):
+        """shape of a *_tokens output: [n, rows (T, T - 1 with NO_CLS, or seq_len), hidden_size or projection_dim]"""
+        hp = self.vision_hparams(ctx) if vision else self.text_hparams(ctx)
+        width = hp.projection_dim if flags & TOKENS_PROJECT else hp.hidden_size
+        return (n, rows - (1 if flags & TOKENS_NO_CLS else 0), width)
+
+    def image_tokens(self, ctx, images: np.ndarray, layer: int = -1, flags: int = 0, out_type: int = OUT_F32) -> np.ndarray:
+        """images [n, S, S, 3] float32 -> rows of every image after `layer`: [n, T or T - 1, width] of OUT_DTYPES[out_type]"""
+        batch, keep = self.make_image_batch(images)
+        hp = self.vision_hparams(ctx)
+        T = (hp.image_size // hp.patch_size) ** 2 + 1
+        out = np.empty(self.token_shape(ctx, True, images.shape[0], T, flags), OUT_DTYPES.get(out_type, np.float32))
+        if not self.lib.clip_b200_image_tokens(ctx, C.byref(batch), layer, flags, out_type, out.ctypes.data):
+            raise RuntimeError("clip_b200_image_tokens failed: " + self.last_error())
+        return out
+
+    def text_tokens(self, ctx, ids: np.ndarray, layer: int = -1, flags: int = 0, out_type: int = OUT_F32) -> np.ndarray:
+        """ids [n, seq_len] int32, padded by the caller -> [n, seq_len, width] of OUT_DTYPES[out_type]"""
+        ids = np.ascontiguousarray(ids, np.int32)
+        out = np.empty(self.token_shape(ctx, False, ids.shape[0], ids.shape[1], flags), OUT_DTYPES.get(out_type, np.float32))
+        if not self.lib.clip_b200_text_tokens(ctx, ids.ctypes.data_as(C.POINTER(C.c_int32)), ids.shape[0], ids.shape[1], layer, flags,
+                                              out_type, out.ctypes.data):
+            raise RuntimeError("clip_b200_text_tokens failed: " + self.last_error())
         return out
 
     @staticmethod

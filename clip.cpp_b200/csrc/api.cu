@@ -86,7 +86,7 @@ struct Scope {
         }
     }
 };
-enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3 };
+enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4 };
 
 // ---- tensor lookup helpers ---------------------------------------------------------------------------------
 const GgufTensor* need(const GgufFile& g, const std::string& name) {
@@ -270,8 +270,8 @@ bool run_linear(clip_ctx* c, const Linear& L, const TmaMap* xmap, const void* xp
     return true;
 }
 
-// The per-layer schedule shared by both towers (clip.cpp:1064-1143 text, 1342-1423 vision).
-bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal) {
+// The per-layer schedule shared by both towers (clip.cpp:1064-1143 text, 1342-1423 vision): blocks 0 .. n_blocks-1.
+bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal, int n_blocks) {
     // The residual stream x stays fp32 (as in the reference).  The branch GEMMs (out-proj, FC2) add their result INTO x themselves
     // (EPI_REDADD32): LayerNorm then only reads x and writes its 16-bit output.
     Workspace& w = tw.ws;
@@ -279,7 +279,8 @@ bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal) {
     const int bf = c->operand_bf16 ? 1 : 0;
     const int dh = h / tw.heads;                      // 64 or 80 (check_geometry)
     const float qscale = 1.0f / sqrtf((float)dh);     // clip.cpp:1082, 1363
-    for (auto& l : tw.L) {
+    for (int il = 0; il < n_blocks; il++) {
+        const Layer& l = tw.L[il];
         { Scope s(c, K_LN); launch_layernorm(w.x, h, M, h, tw.eps, l.ln1_g, l.ln1_b, nullptr, w.a, bf, c->stream); }
         if (!run_linear(c, l.qkv, &w.map_a, w.a, bf, M, w.qkv, 3 * h, EPI_STORE16, bf, h, qscale)) return false;
         if (c->attn_tc) { Scope s(c, K_ATTN); CK(launch_attention_tc(w.qkv, w.a, nseq, T, tw.heads, dh, causal ? 1 : 0, bf, c->stream)); }
@@ -293,16 +294,25 @@ bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal) {
     return true;
 }
 
+// Vision embedding of nb images resident at d_pixels (NHWC f32): ws.x = pre_ln(class | patch embedding + position), the input of block 0.
+bool vision_embed(clip_ctx* c, const float* d_pixels, int nb) {
+    Tower& tw = c->vis;
+    Workspace& w = tw.ws;
+    const int h = tw.hidden;
+    { Scope s(c, K_OTHER); launch_im2col(d_pixels, nb, tw.image_size, tw.patch, tw.kpad, w.patches, c->stream); }
+    // patch embedding = stride-P conv = GEMM over fp16 patches, fp16 weights, fp32 out, no bias (clip.cpp:1309)
+    if (!run_linear(c, tw.patch_w, &w.map_patches, w.patches, false, nb * tw.n_patches, w.patch32, h, EPI_STORE32, 0)) return false;
+    { Scope s(c, K_OTHER); launch_assemble_preln(w.patch32, tw.class_embd, tw.pos, nb, tw.T, h, tw.eps, tw.pre_g, tw.pre_b, w.x, c->stream); }
+    return true;
+}
+
 // Vision tower on nb images already resident at d_pixels (NHWC f32); writes d_out [nb, proj].
 bool vision_forward(clip_ctx* c, const float* d_pixels, int nb, float* d_out, bool normalize) {
     Tower& tw = c->vis;
     Workspace& w = tw.ws;
     const int h = tw.hidden, bf = c->operand_bf16 ? 1 : 0;
-    { Scope s(c, K_OTHER); launch_im2col(d_pixels, nb, tw.image_size, tw.patch, tw.kpad, w.patches, c->stream); }
-    // patch embedding = stride-P conv = GEMM over fp16 patches, fp16 weights, fp32 out, no bias (clip.cpp:1309)
-    if (!run_linear(c, tw.patch_w, &w.map_patches, w.patches, false, nb * tw.n_patches, w.patch32, h, EPI_STORE32, 0)) return false;
-    { Scope s(c, K_OTHER); launch_assemble_preln(w.patch32, tw.class_embd, tw.pos, nb, tw.T, h, tw.eps, tw.pre_g, tw.pre_b, w.x, c->stream); }
-    if (!run_blocks(c, tw, nb, tw.T, false)) return false;
+    if (!vision_embed(c, d_pixels, nb)) return false;
+    if (!run_blocks(c, tw, nb, tw.T, false, tw.layers)) return false;
     // CLS rows -> post-LN -> projection -> (L2 norm)   (clip.cpp:1426-1455)
     { Scope s(c, K_LN); launch_layernorm(w.x, (size_t)tw.T * h, nb, h, tw.eps, tw.post_g, tw.post_b, nullptr, w.sel16, bf, c->stream); }
     if (!run_linear(c, tw.proj_w, &w.map_sel, w.sel16, bf, nb, w.proj32, tw.proj, EPI_STORE32, 0)) return false;
@@ -317,7 +327,7 @@ bool text_forward(clip_ctx* c, int nb, int T, float* d_out, bool normalize) {
     Workspace& w = tw.ws;
     const int h = tw.hidden, bf = c->operand_bf16 ? 1 : 0;
     { Scope s(c, K_OTHER); launch_text_embed(w.ids, tw.tok, tw.pos, nb, T, h, tw.n_vocab, w.x, c->stream); }
-    if (!run_blocks(c, tw, nb, T, true)) return false;
+    if (!run_blocks(c, tw, nb, T, true, tw.layers)) return false;
     // final LN is row-wise, so LN(select(EOT)) == select(LN(all)) (clip.cpp:1146-1155)
     { Scope s(c, K_OTHER); launch_gather_rows(w.x, w.sel32, nb, h, T, w.last, nullptr, bf, c->stream); }
     { Scope s(c, K_LN); launch_layernorm(w.sel32, h, nb, h, tw.eps, tw.post_g, tw.post_b, nullptr, w.sel16, bf, c->stream); }
@@ -325,6 +335,74 @@ bool text_forward(clip_ctx* c, int nb, int T, float* d_out, bool normalize) {
     { Scope s(c, K_OTHER); launch_l2norm(w.proj32, d_out, nb, tw.proj, normalize ? 1 : 0, c->stream); }
     CK(cudaGetLastError());
     return true;
+}
+
+// ---- per-token hidden states (clip_b200_image_tokens / clip_b200_text_tokens) ----------------------------------------------------
+// What a tokens call asks for, checked and resolved: how many blocks to run, which rows of each item, how wide and how many bytes.
+struct TokenReq {
+    int blocks = 0, skip = 0, width = 0, esize = 4, flags = 0, out_type = 0;
+    size_t item_bytes = 0;     // one item's rows in the output
+};
+
+bool token_request(const clip_ctx* c, bool vision, int layer, int flags, int out_type, int T, TokenReq& q, const char* who) {
+    const Tower& tw = vision ? c->vis : c->txt;
+    if (!tw.present) { set_err(std::string(who) + ": this model has no " + (vision ? "vision" : "text") + " encoder"); return false; }
+    const int nl = tw.layers;
+    if (layer < -(nl + 1) || layer > nl) {
+        set_err(std::string(who) + ": layer " + std::to_string(layer) + " is outside [" + std::to_string(-(nl + 1)) + ", " + std::to_string(nl) + "]");
+        return false;
+    }
+    if (flags & ~(CLIP_B200_TOKENS_POST_LN | CLIP_B200_TOKENS_PROJECT | CLIP_B200_TOKENS_NORMALIZE | CLIP_B200_TOKENS_NO_CLS)) { set_err(std::string(who) + ": unknown flag bits"); return false; }
+    if ((flags & CLIP_B200_TOKENS_NO_CLS) && !vision) { set_err(std::string(who) + ": CLIP_B200_TOKENS_NO_CLS is for the vision tower only"); return false; }
+    if ((flags & CLIP_B200_TOKENS_NORMALIZE) && !(flags & CLIP_B200_TOKENS_PROJECT)) { set_err(std::string(who) + ": CLIP_B200_TOKENS_NORMALIZE needs CLIP_B200_TOKENS_PROJECT"); return false; }
+    if (out_type != CLIP_B200_OUT_F32 && out_type != CLIP_B200_OUT_F16 && out_type != CLIP_B200_OUT_BF16) { set_err(std::string(who) + ": unknown out_type " + std::to_string(out_type)); return false; }
+    // PROJECT keeps the projected rows in the qkv and g buffers, free once the blocks have run (every CLIP geometry: d <= h, ff = 4h)
+    if ((flags & CLIP_B200_TOKENS_PROJECT) && (2 * (size_t)tw.proj > 3 * (size_t)tw.hidden || 2 * (size_t)tw.proj > (size_t)tw.ff)) {
+        set_err(std::string(who) + ": CLIP_B200_TOKENS_PROJECT needs projection_dim <= 1.5 hidden_size and <= feed_forward_length / 2");
+        return false;
+    }
+    q.blocks = layer < 0 ? nl + 1 + layer : layer;
+    q.skip = (flags & CLIP_B200_TOKENS_NO_CLS) ? 1 : 0;
+    q.width = (flags & CLIP_B200_TOKENS_PROJECT) ? tw.proj : tw.hidden;
+    q.esize = out_type == CLIP_B200_OUT_F32 ? 4 : 2;
+    q.flags = flags; q.out_type = out_type;
+    q.item_bytes = (size_t)(T - q.skip) * q.width * q.esize;
+    return true;
+}
+
+// After the blocks: the requested rows of ws.x for nb items of T rows -> dst (device), item-major, q.item_bytes per item.
+// PROJECT runs today's pooled tail on every row -- K2 post_ln into the 16-bit operand type, K1 projection (fp32), l2norm -- so the
+// CLS / EOT rows come out bit-identical to clip_image_batch_encode / clip_text_batch_encode; K7 then picks and converts the rows.
+bool token_rows_tail(clip_ctx* c, Tower& tw, int nb, int T, const TokenReq& q, void* dst) {
+    Workspace& w = tw.ws;
+    const int h = tw.hidden, M = nb * T, bf = c->operand_bf16 ? 1 : 0;
+    const bool ln = q.flags & (CLIP_B200_TOKENS_POST_LN | CLIP_B200_TOKENS_PROJECT);
+    if (!(q.flags & CLIP_B200_TOKENS_PROJECT)) {
+        Scope s(c, K_TOKEN_ROWS);
+        launch_token_rows(w.x, h, nb, T, q.skip, h, ln ? tw.post_g : nullptr, tw.post_b, tw.eps, q.out_type, dst, c->stream);
+    } else {
+        float* p32 = reinterpret_cast<float*>(w.qkv);     // [M, proj] fp32 in the [M, 3h] 16-bit buffer
+        float* n32 = reinterpret_cast<float*>(w.g);       // [M, proj] fp32 in the [M, ff] 16-bit buffer
+        { Scope s(c, K_LN); launch_layernorm(w.x, h, M, h, tw.eps, tw.post_g, tw.post_b, nullptr, w.a, bf, c->stream); }
+        if (!run_linear(c, tw.proj_w, &w.map_a, w.a, bf, M, p32, tw.proj, EPI_STORE32, 0)) return false;
+        if (q.flags & CLIP_B200_TOKENS_NORMALIZE) { Scope s(c, K_OTHER); launch_l2norm(p32, n32, M, tw.proj, 1, c->stream); p32 = n32; }
+        { Scope s(c, K_TOKEN_ROWS); launch_token_rows(p32, tw.proj, nb, T, q.skip, tw.proj, nullptr, nullptr, 0.f, q.out_type, dst, c->stream); }
+    }
+    CK(cudaGetLastError());
+    return true;
+}
+
+// nb images at d_pixels through q.blocks blocks -> dst
+bool vision_tokens(clip_ctx* c, const float* d_pixels, int nb, const TokenReq& q, void* dst) {
+    Tower& tw = c->vis;
+    return vision_embed(c, d_pixels, nb) && run_blocks(c, tw, nb, tw.T, false, q.blocks) && token_rows_tail(c, tw, nb, tw.T, q, dst);
+}
+
+// nb sequences of T ids already in ws.ids through q.blocks blocks -> dst
+bool text_tokens(clip_ctx* c, int nb, int T, const TokenReq& q, void* dst) {
+    Tower& tw = c->txt;
+    { Scope s(c, K_OTHER); launch_text_embed(tw.ws.ids, tw.tok, tw.pos, nb, T, tw.hidden, tw.n_vocab, tw.ws.x, c->stream); }
+    return run_blocks(c, tw, nb, T, true, q.blocks) && token_rows_tail(c, tw, nb, T, q, dst);
 }
 
 void dev_free(clip_ctx* c, void* p) {
@@ -960,6 +1038,122 @@ bool clip_b200_text_encode_device(const struct clip_ctx* cctx, const void* d_ids
     CK(cudaSetDevice(c->device));
     // lengths stay on the device: a tiny kernel turns them into EOT-row indices per micro-batch (clamped to [1, seq_len])
     return text_encode_impl(c, nullptr, nullptr, (const int32_t*)d_ids, (const int32_t*)d_lens, n, seq_len, nullptr, (float*)d_vec, normalize);
+}
+
+// ---- per-token hidden states ----------------------------------------------------------------------------------------------------
+// One GPU, host buffers: each micro-batch's inputs go up on the launch stream, its rows come back straight into the caller's `out`
+// (a staging buffer of one micro-batch on the device; the whole output is never held there).
+static bool image_tokens_one(clip_ctx* c, const clip_image_f32* imgs, size_t n, const TokenReq& q, char* out) {
+    Tower& tw = c->vis;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    if (!ensure_ws(c, tw, tw.micro_batch, tw.T, true)) return false;
+    size_t n_chunks, chunk;
+    chunking(n, tw.micro_batch, n_chunks, chunk);
+    if (!ensure_out(c, (chunk * q.item_bytes + 3) / 4)) return false;
+    const size_t per = (size_t)tw.image_size * tw.image_size * 3;
+    CK(cudaEventRecord(c->ev_t0, c->stream));
+    for (size_t i0 = 0; i0 < n; i0 += chunk) {
+        const int nb = (int)std::min(chunk, n - i0);
+        for (int j = 0; j < nb; j++)
+            CK(cudaMemcpyAsync(tw.ws.pixels[0] + (size_t)j * per, imgs[i0 + j].data, per * 4, cudaMemcpyHostToDevice, c->stream));
+        if (!vision_tokens(c, tw.ws.pixels[0], nb, q, c->d_out)) return false;
+        CK(cudaMemcpyAsync(out + i0 * q.item_bytes, c->d_out, nb * q.item_bytes, cudaMemcpyDeviceToHost, c->stream));
+    }
+    CK(cudaEventRecord(c->ev_t1, c->stream));
+    return sync_and_time(c);
+}
+
+bool clip_b200_image_tokens(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, int layer, int flags, int out_type, void* out) {
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    TokenReq q;
+    if (!c) { set_err("clip_b200_image_tokens: null context"); return false; }
+    if (!token_request(c, true, layer, flags, out_type, c->vis.T, q, "clip_b200_image_tokens")) return false;
+    const size_t n = imgs ? imgs->size : 0;
+    if (n == 0) return true;
+    if (!out) { set_err("clip_b200_image_tokens: null output"); return false; }
+    if (!check_images(c, imgs->data, n, "clip_b200_image_tokens")) return false;
+    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
+        // devices mode: contiguous shards, every GPU copies its slice of the rows into the caller's buffer
+        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
+            return hi == lo || image_tokens_one(r, imgs->data + lo, hi - lo, q, (char*)out + lo * q.item_bytes);
+        });
+    }
+    return image_tokens_one(c, imgs->data, n, q, (char*)out);
+}
+
+bool clip_b200_image_tokens_device(const struct clip_ctx* cctx, const void* d_pixels, size_t n, int layer, int flags, int out_type, void* d_out) {
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    TokenReq q;
+    if (!c) { set_err("clip_b200_image_tokens_device: null context"); return false; }
+    if (!token_request(c, true, layer, flags, out_type, c->vis.T, q, "clip_b200_image_tokens_device")) return false;
+    if (n == 0) return true;
+    if (!d_pixels || !d_out) { set_err("clip_b200_image_tokens_device: null device pointer"); return false; }
+    Tower& tw = c->vis;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    if (!ensure_ws(c, tw, tw.micro_batch, tw.T, true)) return false;
+    size_t n_chunks, chunk;
+    chunking(n, tw.micro_batch, n_chunks, chunk);
+    const size_t per = (size_t)tw.image_size * tw.image_size * 3;
+    CK(cudaEventRecord(c->ev_t0, c->stream));
+    for (size_t i0 = 0; i0 < n; i0 += chunk) {
+        const int nb = (int)std::min(chunk, n - i0);
+        if (!vision_tokens(c, (const float*)d_pixels + i0 * per, nb, q, (char*)d_out + i0 * q.item_bytes)) return false;
+    }
+    CK(cudaEventRecord(c->ev_t1, c->stream));
+    return sync_and_time(c);
+}
+
+// n padded sequences of seq_len ids, on the host (h_ids) or the device (d_ids) -> rows at out (host) or d_out (device)
+static bool text_tokens_impl(clip_ctx* c, const int32_t* h_ids, const int32_t* d_ids, size_t n, int seq_len, const TokenReq& q, char* out,
+                             char* d_out) {
+    Tower& tw = c->txt;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    if (!ensure_ws(c, tw, tw.micro_batch, tw.n_ctx, false)) return false;
+    size_t n_chunks, chunk;
+    chunking(n, tw.micro_batch, n_chunks, chunk);
+    if (!d_out && !ensure_out(c, (chunk * q.item_bytes + 3) / 4)) return false;
+    CK(cudaEventRecord(c->ev_t0, c->stream));
+    for (size_t i0 = 0; i0 < n; i0 += chunk) {
+        const int nb = (int)std::min(chunk, n - i0);
+        const size_t id_bytes = (size_t)nb * seq_len * 4;
+        if (h_ids) CK(cudaMemcpyAsync(tw.ws.ids, h_ids + i0 * seq_len, id_bytes, cudaMemcpyHostToDevice, c->stream));
+        else CK(cudaMemcpyAsync(tw.ws.ids, d_ids + i0 * seq_len, id_bytes, cudaMemcpyDeviceToDevice, c->stream));
+        if (!text_tokens(c, nb, seq_len, q, d_out ? d_out + i0 * q.item_bytes : (void*)c->d_out)) return false;
+        if (!d_out) CK(cudaMemcpyAsync(out + i0 * q.item_bytes, c->d_out, nb * q.item_bytes, cudaMemcpyDeviceToHost, c->stream));
+    }
+    CK(cudaEventRecord(c->ev_t1, c->stream));
+    return sync_and_time(c);
+}
+
+bool clip_b200_text_tokens(const struct clip_ctx* cctx, const int32_t* ids, size_t n, int seq_len, int layer, int flags, int out_type, void* out) {
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    TokenReq q;
+    if (!c) { set_err("clip_b200_text_tokens: null context"); return false; }
+    if (!token_request(c, false, layer, flags, out_type, seq_len, q, "clip_b200_text_tokens")) return false;
+    if (n == 0) return true;
+    if (seq_len < 1 || seq_len > c->txt.n_ctx) { set_err("clip_b200_text_tokens: seq_len must be in [1, context_length]"); return false; }
+    if (!ids || !out) { set_err("clip_b200_text_tokens: null pointer"); return false; }
+    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
+        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
+            return hi == lo || text_tokens_impl(r, ids + lo * seq_len, nullptr, hi - lo, seq_len, q, (char*)out + lo * q.item_bytes, nullptr);
+        });
+    }
+    return text_tokens_impl(c, ids, nullptr, n, seq_len, q, (char*)out, nullptr);
+}
+
+bool clip_b200_text_tokens_device(const struct clip_ctx* cctx, const void* d_ids, size_t n, int seq_len, int layer, int flags, int out_type,
+                                  void* d_out) {
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    TokenReq q;
+    if (!c) { set_err("clip_b200_text_tokens_device: null context"); return false; }
+    if (!token_request(c, false, layer, flags, out_type, seq_len, q, "clip_b200_text_tokens_device")) return false;
+    if (n == 0) return true;
+    if (seq_len < 1 || seq_len > c->txt.n_ctx) { set_err("clip_b200_text_tokens_device: seq_len must be in [1, context_length]"); return false; }
+    if (!d_ids || !d_out) { set_err("clip_b200_text_tokens_device: null device pointer"); return false; }
+    return text_tokens_impl(c, nullptr, (const int32_t*)d_ids, n, seq_len, q, nullptr, (char*)d_out);
 }
 
 float clip_similarity_score(const float* vec1, const float* vec2, const int vec_dim) {
@@ -1745,6 +1939,28 @@ int clip_b200_debug_fill_last(const int32_t* lens, int n, int seq_len, int32_t* 
     launch_fill_last(d_lens, d_last, n, seq_len, s.st);
     if (!s.finish("fill_last")) return 5;
     return s.copy_back(last, d_last, (size_t)n * 4) ? 0 : 6;
+}
+
+int clip_b200_debug_token_rows(int n, int T, int h, size_t in_stride, int no_cls, float eps, const float* x, const float* gamma,
+                               const float* beta, int out_type, void* out) {
+    g_err.clear();
+    const int skip = no_cls ? 1 : 0;
+    if (n <= 0 || T <= skip || h <= 0 || h % 4 || h > 2048 || in_stride < (size_t)h || in_stride % 4 || out_type < 0 || out_type > 2) {
+        set_err("debug_token_rows: bad shape");
+        return 1;
+    }
+    HookScratch s;
+    const size_t rows = (size_t)n * T, hb = (size_t)h * 4, span = (rows - 1) * in_stride + h;
+    const size_t out_bytes = (size_t)n * (T - skip) * h * (out_type == 0 ? 4 : 2);
+    float* d_x = (float*)s.alloc(span * 4, 0xff);
+    float* d_g = gamma ? (float*)s.alloc(hb, 0, gamma, hb) : nullptr;
+    float* d_b = gamma ? (float*)s.alloc(hb, 0, beta, hb) : nullptr;
+    void* d_out = s.alloc(out_bytes, 0xff);
+    if (s.ok && cudaMemcpy2D(d_x, in_stride * 4, x, hb, hb, rows, cudaMemcpyHostToDevice) != cudaSuccess) { set_err("debug_token_rows: upload"); return 3; }
+    if (!s.ok) return 3;
+    launch_token_rows(d_x, in_stride, n, T, skip, h, d_g, d_b, eps, out_type, d_out, s.st);
+    if (!s.finish("token_rows")) return 5;
+    return s.copy_back(out, d_out, out_bytes) ? 0 : 6;
 }
 
 

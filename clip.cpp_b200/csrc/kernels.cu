@@ -1,5 +1,5 @@
 // kernels.cu -- the memory-bound kernels around the GEMMs: LayerNorm (K2), im2col (K0a), embedding assembly (K4),
-// L2-normalise (K5), plus a scalar debug GEMM (scoring lives in search.cu).  All are HBM-bound streaming kernels: one warp per
+// L2-normalise (K5), per-token output rows (K7), plus a scalar debug GEMM (scoring lives in search.cu).  All are HBM-bound streaming kernels: one warp per
 // row, 128-bit coalesced loads, warp-shuffle reductions, no shared memory.
 #include <stdlib.h>
 #include <string.h>
@@ -93,6 +93,67 @@ __global__ void __launch_bounds__(256) layernorm_kernel(float* __restrict__ x, s
             pk.x = (uint32_t)P2<BF>::from_float(o0) | ((uint32_t)P2<BF>::from_float(o1) << 16);
             pk.y = (uint32_t)P2<BF>::from_float(o2) | ((uint32_t)P2<BF>::from_float(o3) << 16);
             *reinterpret_cast<uint2*>(yr + 4 * i) = pk;
+        }
+    }
+}
+
+// Token rows (K7): out[r, :] = the r-th requested row of x, optionally through post_ln, as the caller's type.  Output row r of item
+// i = r / rows_out takes x row i * T + skip + r % rows_out (skip = 1 drops the CLS row), rows in_stride floats apart.  With LN the
+// arithmetic is K2's, expression for expression (per-lane sums, warp_sum, rsqrtf, (v - mean) * rstd * g + b in fp32), so the 16-bit
+// output of the operand type equals layernorm_kernel's bit for bit.  OT: 0 fp32, 1 fp16, 2 bf16, each rounded to nearest even.
+template <int OT, bool LN, int MAXV>
+__global__ void __launch_bounds__(256) token_rows_kernel(const float* __restrict__ x, size_t in_stride, int rows, int rows_out, int T,
+                                                         int skip, int h, float eps, const float* __restrict__ gamma,
+                                                         const float* __restrict__ beta, void* __restrict__ out) {
+    // last row first, as K2: the GEMM before this kernel wrote x in ascending token order, so its last rows are still in L2
+    const int lin = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (lin >= rows) return;
+    const int r = rows - 1 - lin;
+    const float* xr = x + ((size_t)(r / rows_out) * T + skip + r % rows_out) * in_stride;
+    const int h4 = h >> 2;
+    float4 v[MAXV];
+    float s = 0.f;
+    #pragma unroll
+    for (int j = 0; j < MAXV; j++) {
+        const int i = lane + 32 * j;
+        if (i < h4) {
+            v[j] = ld4(xr + 4 * i);
+            s += (v[j].x + v[j].y) + (v[j].z + v[j].w);
+        }
+    }
+    float mean = 0.f, rstd = 1.f;
+    if constexpr (LN) {
+        mean = warp_sum(s) / (float)h;
+        float q = 0.f;
+        #pragma unroll
+        for (int j = 0; j < MAXV; j++) {
+            if (lane + 32 * j < h4) {
+                const float a = v[j].x - mean, b = v[j].y - mean, c = v[j].z - mean, d = v[j].w - mean;
+                q += (a * a + b * b) + (c * c + d * d);
+            }
+        }
+        rstd = rsqrtf(warp_sum(q) / (float)h + eps);
+    }
+    #pragma unroll
+    for (int j = 0; j < MAXV; j++) {
+        const int i = lane + 32 * j;
+        if (i < h4) {
+            float4 o = v[j];
+            if constexpr (LN) {
+                const float4 g = ld4(gamma + 4 * i), b = ld4(beta + 4 * i);
+                o.x = (v[j].x - mean) * rstd * g.x + b.x; o.y = (v[j].y - mean) * rstd * g.y + b.y;
+                o.z = (v[j].z - mean) * rstd * g.z + b.z; o.w = (v[j].w - mean) * rstd * g.w + b.w;
+            }
+            const size_t e = (size_t)r * h + 4 * i;
+            if constexpr (OT == 0) {
+                *reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + e) = o;
+            } else {
+                using C = P2<OT == 2>;
+                uint2 pk;
+                pk.x = (uint32_t)C::from_float(o.x) | ((uint32_t)C::from_float(o.y) << 16);
+                pk.y = (uint32_t)C::from_float(o.z) | ((uint32_t)C::from_float(o.w) << 16);
+                *reinterpret_cast<uint2*>(reinterpret_cast<uint16_t*>(out) + e) = pk;
+            }
         }
     }
 }
@@ -255,6 +316,21 @@ void launch_layernorm(float* x, size_t in_stride, int rows, int h, float eps, co
     else      { if (d) CB_LN_W(false, true); else CB_LN_W(false, false); }
 #undef CB_LN_W
 #undef CB_LN
+}
+
+void launch_token_rows(const float* x, size_t in_stride, int n, int T, int skip, int h, const float* gamma, const float* beta, float eps,
+                       int out_type, void* out, cudaStream_t st) {
+    const int rows_out = T - skip, rows = n * rows_out;
+    if (rows <= 0) return;
+    const int grid = rows_grid(rows, 8);
+#define CB_TR(OT, LN, MV) token_rows_kernel<OT, LN, MV><<<grid, 256, 0, st>>>(x, in_stride, rows, rows_out, T, skip, h, eps, gamma, beta, out)
+#define CB_TR_W(OT, LN) do { if (h <= 512) CB_TR(OT, LN, 4); else if (h <= 1024) CB_TR(OT, LN, 8); else CB_TR(OT, LN, 16); } while (0)
+#define CB_TR_T(LN) do { if (out_type == 0) CB_TR_W(0, LN); else if (out_type == 1) CB_TR_W(1, LN); else CB_TR_W(2, LN); } while (0)
+    if (gamma) CB_TR_T(true);
+    else CB_TR_T(false);
+#undef CB_TR_T
+#undef CB_TR_W
+#undef CB_TR
 }
 
 void launch_im2col(const float* pixels, int B, int S, int P, int kpad, void* patches16, cudaStream_t st) {

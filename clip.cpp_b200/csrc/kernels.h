@@ -12,6 +12,12 @@ namespace cb {
 void launch_layernorm(float* x, size_t in_stride, int rows, int h, float eps, const float* gamma, const float* beta,
                       const void* delta16, void* y16, int bf16, cudaStream_t st);
 
+// K7 token rows: for each of n items, rows skip .. T-1 of x (item i's row t at x + (i*T + t)*in_stride) -> out [n*(T-skip), h],
+// contiguous, as out_type (0 fp32, 1 fp16, 2 bf16; round to nearest even).  gamma != NULL applies LayerNorm (gamma, beta, eps) first,
+// with K2's arithmetic: the 16-bit output of the operand type equals launch_layernorm's bit for bit.  h % 4 == 0, h <= 2048.
+void launch_token_rows(const float* x, size_t in_stride, int n, int T, int skip, int h, const float* gamma, const float* beta, float eps,
+                       int out_type, void* out, cudaStream_t st);
+
 // K0a im2col for the stride-P patch conv: pixels NHWC f32 [B,S,S,3] -> fp16 [B*Np, kpad], k = c*P*P + ky*P + kx,
 // zero padded to kpad (reference conv_2d im2col, ggml.c:13595-13631; pixel -> fp16 rounding ggml.c:13623).
 void launch_im2col(const float* pixels, int B, int S, int P, int kpad, void* patches16, cudaStream_t st);

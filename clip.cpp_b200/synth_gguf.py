@@ -71,6 +71,9 @@ GEOMETRIES = {
     "vit-b32": Geometry("vit-b32"),
     "vit-l14": Geometry("vit-l14", patch_size=14, v_hidden=1024, v_ff=4096, v_heads=16, v_layers=24,
                         t_hidden=768, t_ff=3072, t_heads=12, t_layers=12, proj_dim=768),
+    # ViT-L/14@336 (LLaVA-1.5's vision tower): 24 * 24 + 1 = 577 positions
+    "vit-l14-336": Geometry("vit-l14-336", image_size=336, patch_size=14, v_hidden=1024, v_ff=4096, v_heads=16, v_layers=24,
+                            t_hidden=768, t_ff=3072, t_heads=12, t_layers=12, proj_dim=768),
     # LAION ViT-H/14: vision head_dim 1280 / 16 = 80, text head_dim 1024 / 16 = 64, GELU
     "vit-h14": Geometry("vit-h14", patch_size=14, v_hidden=1280, v_ff=5120, v_heads=16, v_layers=32,
                         t_hidden=1024, t_ff=4096, t_heads=16, t_layers=24, proj_dim=1024, use_gelu=True),

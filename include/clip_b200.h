@@ -172,6 +172,37 @@ bool clip_b200_image_encode_device(const struct clip_ctx * ctx, const void * d_p
 bool clip_b200_text_encode_device(const struct clip_ctx * ctx, const void * d_ids, const void * d_lens, size_t n,
                                   int seq_len, void * d_vec, bool normalize);
 
+/* Per-token hidden states of either tower (HF output_hidden_states, open_clip forward_intermediates): every row of the residual
+ * stream after a chosen layer, for vision-language front ends (LLaVA reads the patch rows of the penultimate layer) and diffusion
+ * text conditioning (Stable Diffusion reads all 77 rows, post_ln applied).
+ *   layer    HF hidden_states numbering: 0 = the input of block 0 (vision: the pre_ln output; text: token + position embeddings),
+ *            i = the output of block i (1 .. n_layer), negative counts from the end (-1 = the last block, -2 = the penultimate one).
+ *            Only the blocks up to `layer` run.  Outside [-(n_layer + 1), n_layer]: refused.
+ *   flags    CLIP_B200_TOKENS_* below, or 0 for the raw residual rows.
+ *   out      item-major, row-major: vision [n, T or T - 1, width] with T = (image_size / patch_size)^2 + 1, CLS first; text
+ *            [n, seq_len, width].  width = hidden_size, or projection_dim with PROJECT.  Elements of out_type, rounded to nearest even.
+ * With PROJECT the CLS row of an image (row 0) and the EOT row of a sequence (row len - 1) equal clip_image_batch_encode /
+ * clip_text_batch_encode's embedding bit for bit (normalize = whether NORMALIZE is set).  Text ids are padded by the caller (any pad id
+ * of the caller's model; causal attention keeps the rows before the padding independent of it).
+ * Refused with a message in clip_b200_last_error(): a bad layer, unknown flag bits or out_type, NO_CLS on text, NORMALIZE without
+ * PROJECT, a model without the tower.  n == 0 returns true.
+ * Host variants: devices mode (CLIP_B200_DEVICES) shards the batch like clip_image_batch_encode, each GPU copying its slice into out;
+ * each micro-batch's rows are copied straight into out (the whole output is never held on the device).  Device variants: pointers on
+ * the context's GPU, d_out 16-byte aligned (any cudaMalloc pointer is). */
+enum { CLIP_B200_OUT_F32 = 0, CLIP_B200_OUT_F16 = 1, CLIP_B200_OUT_BF16 = 2 };
+#define CLIP_B200_TOKENS_POST_LN    1  /* the tower's final LayerNorm (post_ln) on every returned row               */
+#define CLIP_B200_TOKENS_PROJECT    2  /* post_ln + projection: rows of projection_dim instead of hidden_size        */
+#define CLIP_B200_TOKENS_NORMALIZE  4  /* with PROJECT: L2-normalise each row (as normalize=true does)               */
+#define CLIP_B200_TOKENS_NO_CLS     8  /* vision only: patch tokens, T-1 rows per image                               */
+bool clip_b200_image_tokens(const struct clip_ctx * ctx, const struct clip_image_f32_batch * imgs, int layer, int flags, int out_type,
+                            void * out);
+bool clip_b200_image_tokens_device(const struct clip_ctx * ctx, const void * d_pixels, size_t n, int layer, int flags, int out_type,
+                                   void * d_out);
+bool clip_b200_text_tokens(const struct clip_ctx * ctx, const int32_t * ids, size_t n, int seq_len, int layer, int flags, int out_type,
+                           void * out);
+bool clip_b200_text_tokens_device(const struct clip_ctx * ctx, const void * d_ids, size_t n, int seq_len, int layer, int flags,
+                                  int out_type, void * d_out);
+
 /* Batched zero-shot scoring on the device (clip.cpp:1624-1659 semantics per image): d_img_vec [n_img, d], d_txt_vec [n_txt, d]
  * -> host scores/indices [n_img, top_k], best first; similarity matrix, softmax and top-k selection all run on the GPU.
  * Ranking (here and in clip_b200_topk_search): top_k <= 0 or top_k > n_txt means all n_txt, and row i of the output starts at
@@ -245,7 +276,7 @@ void   clip_b200_set_micro_batch(const struct clip_ctx * ctx, int images, int se
 uint64_t clip_b200_kernel_launches(const struct clip_ctx * ctx);   /* kernels launched by this context so far */
 float    clip_b200_last_device_ms(const struct clip_ctx * ctx);    /* CUDA-event time of the last encode's kernels */
 /* per-kernel-class CUDA-event time accumulated since the last call with the same kind (0 GEMM, 1 attention,
- * 2 layernorm, 3 other); *count receives the number of launches.  Enabled by env CLIP_B200_PROFILE=1. */
+ * 2 layernorm, 3 other, 4 the token-row kernel of the *_tokens calls); *count receives the number of launches.  Enabled by env CLIP_B200_PROFILE=1. */
 float    clip_b200_kernel_ms(const struct clip_ctx * ctx, int kind, uint64_t * count);
 /* CUDA-event stopwatch on the launch stream: mark(slot 0..3), then elapsed(a, b) in ms (-1 on error) */
 bool     clip_b200_mark(const struct clip_ctx * ctx, int slot);
@@ -302,6 +333,11 @@ int clip_b200_debug_gather_rows(const float * src, int src_rows, int rows, int h
 int clip_b200_debug_l2norm(const float * v, int rows, int d, int normalize, float * out);
 /* EOT row index per sequence: last[i] = clamp(lens ? lens[i] : seq_len, 1, seq_len) - 1 */
 int clip_b200_debug_fill_last(const int32_t * lens, int n, int seq_len, int32_t * last);
+/* token rows (K7): x host [n*T, h] placed at row stride in_stride (gaps poisoned); out receives rows 1 .. T-1 (no_cls) or 0 .. T-1
+ * of each item, [n, T or T-1, h], as out_type (0 fp32, 1 fp16, 2 bf16: raw 16-bit values, not widened); gamma = NULL: no
+ * LayerNorm, otherwise post_ln with gamma, beta, eps */
+int clip_b200_debug_token_rows(int n, int T, int h, size_t in_stride, int no_cls, float eps, const float * x, const float * gamma,
+                               const float * beta, int out_type, void * out);
 
 /* CPU-only TEST HOOKS (no context, no GPU): lossless re-tiling check, tokenizer and preprocess without a model context */
 int clip_b200_debug_repack_roundtrip(int qtype, const void * rows, int N, int K);
