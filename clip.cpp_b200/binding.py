@@ -82,6 +82,9 @@ EXTENSION_SYMBOLS = [
     # per-token hidden states
     "clip_b200_image_tokens", "clip_b200_image_tokens_device", "clip_b200_text_tokens", "clip_b200_text_tokens_device",
     "clip_b200_debug_token_rows",
+    # any patch-multiple image size (interpolated position table)
+    "clip_b200_image_encode_device_hw", "clip_b200_image_tokens_device_hw", "clip_b200_image_batch_encode_hw", "clip_b200_image_tokens_hw",
+    "clip_b200_debug_im2col_hw", "clip_b200_debug_pos_resample",
 ]
 
 # include/clip_b200.h: output types and flags of the *_tokens entry points
@@ -201,7 +204,9 @@ class ClipLib:
                             ("clip_b200_debug_gather_rows", [fp, ip, ip, ip, ip, i32p, fp, ip, fp]),
                             ("clip_b200_debug_l2norm", [fp, ip, ip, ip, fp]),
                             ("clip_b200_debug_fill_last", [i32p, ip, ip, i32p]),
-                            ("clip_b200_debug_token_rows", [ip, ip, ip, C.c_size_t, ip, C.c_float, fp, fp, fp, ip, vp])):
+                            ("clip_b200_debug_token_rows", [ip, ip, ip, C.c_size_t, ip, C.c_float, fp, fp, fp, ip, vp]),
+                            ("clip_b200_debug_im2col_hw", [fp, ip, ip, ip, ip, ip, fp]),
+                            ("clip_b200_debug_pos_resample", [fp, ip, ip, ip, ip, fp])):
                 getattr(L, f).restype = C.c_int
                 getattr(L, f).argtypes = args
             L.clip_b200_image_tokens.restype = C.c_bool
@@ -212,6 +217,14 @@ class ClipLib:
             L.clip_b200_text_tokens.argtypes = [vp, i32p, C.c_size_t, ip, ip, ip, ip, vp]
             L.clip_b200_text_tokens_device.restype = C.c_bool
             L.clip_b200_text_tokens_device.argtypes = [vp, vp, C.c_size_t, ip, ip, ip, ip, vp]
+            L.clip_b200_image_encode_device_hw.restype = C.c_bool
+            L.clip_b200_image_encode_device_hw.argtypes = [vp, vp, C.c_size_t, ip, ip, vp, C.c_bool]
+            L.clip_b200_image_tokens_device_hw.restype = C.c_bool
+            L.clip_b200_image_tokens_device_hw.argtypes = [vp, vp, C.c_size_t, ip, ip, ip, ip, ip, vp]
+            L.clip_b200_image_batch_encode_hw.restype = C.c_bool
+            L.clip_b200_image_batch_encode_hw.argtypes = [vp, C.POINTER(clip_image_f32_batch), fp, C.c_bool]
+            L.clip_b200_image_tokens_hw.restype = C.c_bool
+            L.clip_b200_image_tokens_hw.argtypes = [vp, C.POINTER(clip_image_f32_batch), ip, ip, ip, vp]
             ipp = C.POINTER(C.c_int)
             L.clip_b200_topk_search.restype = C.c_bool
             L.clip_b200_topk_search.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, ip, fp, ipp]
@@ -277,15 +290,15 @@ class ClipLib:
     # ---- encoders (host buffers; the reference-facing calls) ---------------------------------------
     @staticmethod
     def make_image_batch(images: np.ndarray):
-        """images: [n, S, S, 3] float32 C-contiguous -> (batch struct, keep-alive tuple)."""
+        """images: [n, H, W, 3] float32 C-contiguous (H = W = image_size for the native calls) -> (batch struct, keep-alive tuple)."""
         assert images.dtype == np.float32 and images.flags["C_CONTIGUOUS"] and images.ndim == 4
-        n, s = images.shape[0], images.shape[1]
+        n, hgt, wid = images.shape[:3]
         arr = (clip_image_f32 * n)()
-        per = s * s * 3
+        per = hgt * wid * 3
         base = images.ctypes.data
         for i in range(n):
-            arr[i].nx = s
-            arr[i].ny = s
+            arr[i].nx = wid
+            arr[i].ny = hgt
             arr[i].size = per
             arr[i].data = C.cast(base + i * per * 4, C.POINTER(C.c_float))
         batch = clip_image_f32_batch(arr, n)
@@ -354,6 +367,25 @@ class ClipLib:
         out = np.empty(self.token_shape(ctx, True, images.shape[0], T, flags), OUT_DTYPES.get(out_type, np.float32))
         if not self.lib.clip_b200_image_tokens(ctx, C.byref(batch), layer, flags, out_type, out.ctypes.data):
             raise RuntimeError("clip_b200_image_tokens failed: " + self.last_error())
+        return out
+
+    # ---- any patch-multiple image size (include/clip_b200.h: *_hw) --------------------------------------------------------------
+    def image_batch_encode_hw(self, ctx, images: np.ndarray, normalize=True) -> np.ndarray:
+        """images [n, H, W, 3] float32, H and W multiples of patch_size -> [n, projection_dim] (position table resampled to the grid)"""
+        batch, keep = self.make_image_batch(images)
+        out = np.empty((images.shape[0], self.vision_hparams(ctx).projection_dim), np.float32)
+        if not self.lib.clip_b200_image_batch_encode_hw(ctx, C.byref(batch), out.ctypes.data_as(C.POINTER(C.c_float)), normalize):
+            raise RuntimeError("clip_b200_image_batch_encode_hw failed: " + self.last_error())
+        return out
+
+    def image_tokens_hw(self, ctx, images: np.ndarray, layer: int = -1, flags: int = 0, out_type: int = OUT_F32) -> np.ndarray:
+        """images [n, H, W, 3] float32 -> [n, T or T - 1, width], T = (H / P) * (W / P) + 1, patch rows in row-major grid order"""
+        batch, keep = self.make_image_batch(images)
+        P = self.vision_hparams(ctx).patch_size
+        T = (images.shape[1] // P) * (images.shape[2] // P) + 1
+        out = np.empty(self.token_shape(ctx, True, images.shape[0], T, flags), OUT_DTYPES.get(out_type, np.float32))
+        if not self.lib.clip_b200_image_tokens_hw(ctx, C.byref(batch), layer, flags, out_type, out.ctypes.data):
+            raise RuntimeError("clip_b200_image_tokens_hw failed: " + self.last_error())
         return out
 
     def text_tokens(self, ctx, ids: np.ndarray, layer: int = -1, flags: int = 0, out_type: int = OUT_F32) -> np.ndarray:

@@ -86,7 +86,7 @@ struct Scope {
         }
     }
 };
-enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4 };
+enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4, K_POS_RESAMPLE = 5 };
 
 // ---- tensor lookup helpers ---------------------------------------------------------------------------------
 const GgufTensor* need(const GgufFile& g, const std::string& name) {
@@ -294,27 +294,40 @@ bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal, int n_bloc
     return true;
 }
 
+// The image size of one vision call: H x W pixels, T = (H/P)(W/P) + 1 rows per image, the position table of that grid ([T, h]).
+// The model's own size is H = W = image_size with the loaded table; the *_hw entry points pass others (plan_call).
+struct VisCall {
+    int H = 0, W = 0, T = 0;
+    const float* pos = nullptr;
+    size_t per() const { return (size_t)H * W * 3; }     // floats of one NHWC image
+};
+VisCall native_call(const Tower& tw) {
+    VisCall v;
+    v.H = v.W = tw.image_size; v.T = tw.T; v.pos = tw.pos;
+    return v;
+}
+
 // Vision embedding of nb images resident at d_pixels (NHWC f32): ws.x = pre_ln(class | patch embedding + position), the input of block 0.
-bool vision_embed(clip_ctx* c, const float* d_pixels, int nb) {
+bool vision_embed(clip_ctx* c, const float* d_pixels, int nb, const VisCall& v) {
     Tower& tw = c->vis;
     Workspace& w = tw.ws;
     const int h = tw.hidden;
-    { Scope s(c, K_OTHER); launch_im2col(d_pixels, nb, tw.image_size, tw.patch, tw.kpad, w.patches, c->stream); }
+    { Scope s(c, K_OTHER); launch_im2col(d_pixels, nb, v.H, v.W, tw.patch, tw.kpad, w.patches, c->stream); }
     // patch embedding = stride-P conv = GEMM over fp16 patches, fp16 weights, fp32 out, no bias (clip.cpp:1309)
-    if (!run_linear(c, tw.patch_w, &w.map_patches, w.patches, false, nb * tw.n_patches, w.patch32, h, EPI_STORE32, 0)) return false;
-    { Scope s(c, K_OTHER); launch_assemble_preln(w.patch32, tw.class_embd, tw.pos, nb, tw.T, h, tw.eps, tw.pre_g, tw.pre_b, w.x, c->stream); }
+    if (!run_linear(c, tw.patch_w, &w.map_patches, w.patches, false, nb * (v.T - 1), w.patch32, h, EPI_STORE32, 0)) return false;
+    { Scope s(c, K_OTHER); launch_assemble_preln(w.patch32, tw.class_embd, v.pos, nb, v.T, h, tw.eps, tw.pre_g, tw.pre_b, w.x, c->stream); }
     return true;
 }
 
 // Vision tower on nb images already resident at d_pixels (NHWC f32); writes d_out [nb, proj].
-bool vision_forward(clip_ctx* c, const float* d_pixels, int nb, float* d_out, bool normalize) {
+bool vision_forward(clip_ctx* c, const float* d_pixels, int nb, const VisCall& v, float* d_out, bool normalize) {
     Tower& tw = c->vis;
     Workspace& w = tw.ws;
     const int h = tw.hidden, bf = c->operand_bf16 ? 1 : 0;
-    if (!vision_embed(c, d_pixels, nb)) return false;
-    if (!run_blocks(c, tw, nb, tw.T, false, tw.layers)) return false;
+    if (!vision_embed(c, d_pixels, nb, v)) return false;
+    if (!run_blocks(c, tw, nb, v.T, false, tw.layers)) return false;
     // CLS rows -> post-LN -> projection -> (L2 norm)   (clip.cpp:1426-1455)
-    { Scope s(c, K_LN); launch_layernorm(w.x, (size_t)tw.T * h, nb, h, tw.eps, tw.post_g, tw.post_b, nullptr, w.sel16, bf, c->stream); }
+    { Scope s(c, K_LN); launch_layernorm(w.x, (size_t)v.T * h, nb, h, tw.eps, tw.post_g, tw.post_b, nullptr, w.sel16, bf, c->stream); }
     if (!run_linear(c, tw.proj_w, &w.map_sel, w.sel16, bf, nb, w.proj32, tw.proj, EPI_STORE32, 0)) return false;
     { Scope s(c, K_OTHER); launch_l2norm(w.proj32, d_out, nb, tw.proj, normalize ? 1 : 0, c->stream); }
     CK(cudaGetLastError());
@@ -393,9 +406,9 @@ bool token_rows_tail(clip_ctx* c, Tower& tw, int nb, int T, const TokenReq& q, v
 }
 
 // nb images at d_pixels through q.blocks blocks -> dst
-bool vision_tokens(clip_ctx* c, const float* d_pixels, int nb, const TokenReq& q, void* dst) {
+bool vision_tokens(clip_ctx* c, const float* d_pixels, int nb, const VisCall& v, const TokenReq& q, void* dst) {
     Tower& tw = c->vis;
-    return vision_embed(c, d_pixels, nb) && run_blocks(c, tw, nb, tw.T, false, q.blocks) && token_rows_tail(c, tw, nb, tw.T, q, dst);
+    return vision_embed(c, d_pixels, nb, v) && run_blocks(c, tw, nb, v.T, false, q.blocks) && token_rows_tail(c, tw, nb, v.T, q, dst);
 }
 
 // nb sequences of T ids already in ws.ids through q.blocks blocks -> dst
@@ -457,16 +470,67 @@ bool sync_and_time(clip_ctx* c) {
     return true;
 }
 
-bool image_encode_device_locked(clip_ctx* c, const float* d_pixels, size_t n, float* d_vec, bool normalize) {
+// H x W = 0 x 0 or (image_size x image_size): T, the position table and the images per pass of the model's own size
+// (micro_batch).  Another size (already checked by check_hw_size): T = (H/P)(W/P) + 1, the table resampled to that grid (K8, cached
+// for the last size), and as many images per pass as fit every workspace buffer.  The workspace itself is always sized for
+// micro_batch images of the native T, at the first call of the context whatever its size, so a native call after a *_hw one finds
+// it as it would have.  Caller holds c->mu and has set the device.
+bool plan_call(clip_ctx* c, int H, int W, VisCall& v, int& mb, const char* who) {
     Tower& tw = c->vis;
     if (!ensure_ws(c, tw, tw.micro_batch, tw.T, true)) return false;
+    if (H == 0 || (H == tw.image_size && W == tw.image_size)) {
+        v = native_call(tw);
+        mb = tw.micro_batch;
+        return true;
+    }
+    const int g = tw.image_size / tw.patch, gh = H / tw.patch, gw = W / tw.patch, h = tw.hidden;
+    v.H = H; v.W = W; v.T = gh * gw + 1;
+    // rows of x / a / qkv / g, the sel / proj rows, and the patch rows of patches / patch32 (the pixel buffers hold exactly P*P*3
+    // floats per patch row, so they fit whenever the patch rows do)
+    const Workspace& w = tw.ws;
+    const size_t fit = std::min({(size_t)w.cap_rows / v.T, (size_t)w.cap_items, (size_t)w.cap_items * tw.n_patches / (v.T - 1)});
+    if (fit < 1) {
+        set_err(std::string(who) + ": one " + std::to_string(H) + " x " + std::to_string(W) + " image needs " + std::to_string(v.T) +
+                " rows, more than the workspace holds (" + std::to_string(w.cap_rows) + "); raise clip_b200_set_micro_batch before the first encode");
+        return false;
+    }
+    mb = (int)fit;
+    if (c->pos_gh != gh || c->pos_gw != gw) {
+        c->pos_gh = c->pos_gw = 0;
+        if (!ensure_buf(c, &c->pos_hw, &c->pos_hw_cap, (size_t)v.T * h)) return false;
+        CK(cudaMemcpyAsync(c->pos_hw, tw.pos, (size_t)h * 4, cudaMemcpyDeviceToDevice, c->stream));     // the CLS row as it is
+        { Scope s(c, K_POS_RESAMPLE); launch_pos_resample(tw.pos + h, g, h, gh, gw, c->pos_hw + h, c->stream); }
+        CK(cudaGetLastError());
+        c->pos_gh = gh; c->pos_gw = gw;
+    }
+    v.pos = c->pos_hw;
+    return true;
+}
+
+// a *_hw size: positive multiples of patch_size, at most 4096 on each side
+bool check_hw_size(const clip_ctx* c, int H, int W, const char* who) {
+    const int P = c->vis.patch;
+    if (H <= 0 || W <= 0 || H % P || W % P || H > 4096 || W > 4096) {
+        set_err(std::string(who) + ": height and width must be positive multiples of patch_size (" + std::to_string(P) + ") and at most 4096, not " +
+                std::to_string(H) + " x " + std::to_string(W));
+        return false;
+    }
+    return true;
+}
+
+bool image_encode_device_locked(clip_ctx* c, const float* d_pixels, size_t n, float* d_vec, bool normalize, int H = 0, int W = 0,
+                                const char* who = "clip_b200_image_encode_device") {
+    Tower& tw = c->vis;
+    VisCall v;
+    int mb = 0;
+    if (!plan_call(c, H, W, v, mb, who)) return false;
     size_t n_chunks, chunk;
-    chunking(n, tw.micro_batch, n_chunks, chunk);
-    const size_t per = (size_t)tw.image_size * tw.image_size * 3;
+    chunking(n, mb, n_chunks, chunk);
+    const size_t per = v.per();
     CK(cudaEventRecord(c->ev_t0, c->stream));
     for (size_t i0 = 0; i0 < n; i0 += chunk) {
         const int nb = (int)std::min(chunk, n - i0);
-        if (!vision_forward(c, d_pixels + i0 * per, nb, d_vec + i0 * tw.proj, normalize)) return false;
+        if (!vision_forward(c, d_pixels + i0 * per, nb, v, d_vec + i0 * tw.proj, normalize)) return false;
     }
     CK(cudaEventRecord(c->ev_t1, c->stream));
     return true;
@@ -801,7 +865,7 @@ static bool preprocess_chunks(clip_ctx* c, const clip_image_u8* imgs, size_t n, 
         std::string err;
         if (!preprocess_device(c, imgs + i0, nb, b, tw.ws.pixels[b], c->copy_stream, c->ev_copied[b], c->stream, err)) { set_err(err); return false; }
         if (h_pixels_out) CK(cudaMemcpyAsync(h_pixels_out + i0 * per, tw.ws.pixels[b], (size_t)nb * per * 4, cudaMemcpyDeviceToHost, c->stream));
-        if (vec && !vision_forward(c, tw.ws.pixels[b], nb, c->d_out + i0 * tw.proj, normalize)) return false;
+        if (vec && !vision_forward(c, tw.ws.pixels[b], nb, native_call(tw), c->d_out + i0 * tw.proj, normalize)) return false;
         CK(cudaEventRecord(c->ev_consumed[b], c->stream));
     }
     CK(cudaEventRecord(c->ev_t1, c->stream));
@@ -859,28 +923,44 @@ bool clip_b200_image_encode_device(const struct clip_ctx* cctx, const void* d_pi
     return sync_and_time(c);
 }
 
+bool clip_b200_image_encode_device_hw(const struct clip_ctx* cctx, const void* d_pixels, size_t n, int height, int width, void* d_vec,
+                                      bool normalize) {
+    const char* who = "clip_b200_image_encode_device_hw";
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    if (!c || !c->has_vision) { set_err(std::string(who) + ": this model has no vision encoder"); return false; }
+    if (!check_hw_size(c, height, width, who)) return false;
+    if (n == 0) return true;
+    if (!d_pixels || !d_vec) { set_err(std::string(who) + ": null device pointer"); return false; }
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    if (!image_encode_device_locked(c, (const float*)d_pixels, n, (float*)d_vec, normalize, height, width, who)) return false;
+    return sync_and_time(c);
+}
+
 // One GPU: n host images -> embeddings at d_vec (device, may be null) and / or vec (host, may be null).  Host pixels travel on the
 // copy stream, double-buffered against the kernels of the previous micro-batch.  Pinned / registered caller buffers are copied
 // directly; PAGEABLE ones (what clip_image_preprocess returns: new float[]) are first gathered into a pinned arena by host threads,
 // in sub-batches so the H2D of sub-batch k overlaps the memcpy of k+1 -- a pageable cudaMemcpyAsync would be staged synchronously
 // by the driver, one 602 KB image at a time.
 static bool image_batch_encode_one(clip_ctx* c, int n_threads, const clip_image_f32* imgs, size_t n, float* vec, float* d_vec, bool normalize,
-                                   bool sync) {
+                                   bool sync, int H = 0, int W = 0, const char* who = "clip_image_batch_encode") {
     Tower& tw = c->vis;
     std::lock_guard<std::mutex> lk(c->mu);
     CK(cudaSetDevice(c->device));
-    if (!ensure_ws(c, tw, tw.micro_batch, tw.T, true)) return false;
+    VisCall v;
+    int mb = 0;
+    if (!plan_call(c, H, W, v, mb, who)) return false;
     if (!d_vec) { if (!ensure_out(c, n * tw.proj)) return false; d_vec = c->d_out; }
-    const std::vector<size_t> bounds = host_chunk_bounds(n, tw.micro_batch);
-    const size_t per = (size_t)tw.image_size * tw.image_size * 3;
+    const std::vector<size_t> bounds = host_chunk_bounds(n, mb);
+    const size_t per = v.per();
     bool pinned = true;
     for (size_t i = 0; i < n && pinned; i++) pinned = host_ptr_is_pinned(imgs[i].data);
-    if (!pinned && c->h_stage_cap < (size_t)tw.micro_batch * per) {
+    if (!pinned && c->h_stage_cap < (size_t)mb * per) {
         for (int b = 0; b < 2; b++) {
             if (c->h_stage[b]) { cudaFreeHost(c->h_stage[b]); c->h_stage[b] = nullptr; }
-            CK(cudaMallocHost((void**)&c->h_stage[b], (size_t)tw.micro_batch * per * 4));
+            CK(cudaMallocHost((void**)&c->h_stage[b], (size_t)mb * per * 4));
         }
-        c->h_stage_cap = (size_t)tw.micro_batch * per;
+        c->h_stage_cap = (size_t)mb * per;
     }
     const int nt = std::max(1, std::min({std::max(n_threads, 4), 16, (int)std::thread::hardware_concurrency()}));
     CK(cudaEventRecord(c->ev_t0, c->stream));
@@ -911,7 +991,7 @@ static bool image_batch_encode_one(clip_ctx* c, int n_threads, const clip_image_
         }
         CK(cudaEventRecord(c->ev_copied[b], c->copy_stream));
         CK(cudaStreamWaitEvent(c->stream, c->ev_copied[b], 0));
-        if (!vision_forward(c, tw.ws.pixels[b], nb, d_vec + i0 * tw.proj, normalize)) return false;
+        if (!vision_forward(c, tw.ws.pixels[b], nb, v, d_vec + i0 * tw.proj, normalize)) return false;
         CK(cudaEventRecord(c->ev_consumed[b], c->stream));
     }
     CK(cudaEventRecord(c->ev_t1, c->stream));
@@ -923,6 +1003,20 @@ static bool check_images(clip_ctx* c, const clip_image_f32* imgs, size_t n, cons
     for (size_t i = 0; i < n; i++)
         if (imgs[i].nx != c->vis.image_size || imgs[i].ny != c->vis.image_size || !imgs[i].data) { set_err(std::string(who) + ": every image must be image_size x image_size"); return false; }
     return true;
+}
+
+// host *_hw forms: the size is the images' own (ny rows of nx pixels), the same for every image of the call
+static bool check_images_hw(clip_ctx* c, const clip_image_f32* imgs, size_t n, int& H, int& W, const char* who) {
+    H = imgs[0].ny; W = imgs[0].nx;
+    for (size_t i = 0; i < n; i++) {
+        if (!imgs[i].data) { set_err(std::string(who) + ": image " + std::to_string(i) + " has no pixels"); return false; }
+        if (imgs[i].ny != H || imgs[i].nx != W) {
+            set_err(std::string(who) + ": every image of one call must have the same size (height x width: image 0 is " + std::to_string(H) + " x " +
+                    std::to_string(W) + ", image " + std::to_string(i) + " is " + std::to_string(imgs[i].ny) + " x " + std::to_string(imgs[i].nx) + ")");
+            return false;
+        }
+    }
+    return check_hw_size(c, H, W, who);
 }
 
 bool clip_image_batch_encode(const struct clip_ctx* cctx, const int n_threads, const struct clip_image_f32_batch* imgs, float* vec,
@@ -940,6 +1034,24 @@ bool clip_image_batch_encode(const struct clip_ctx* cctx, const int n_threads, c
         });
     }
     return image_batch_encode_one(c, n_threads, imgs->data, n, vec, nullptr, normalize, true);
+}
+
+bool clip_b200_image_batch_encode_hw(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, float* vec, bool normalize) {
+    const char* who = "clip_b200_image_batch_encode_hw";
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    if (!c || !c->has_vision) { set_err(std::string(who) + ": this model has no vision encoder"); return false; }
+    const size_t n = imgs ? imgs->size : 0;
+    if (n == 0) return true;
+    if (!vec) { set_err(std::string(who) + ": null output"); return false; }
+    int H = 0, W = 0;
+    if (!check_images_hw(c, imgs->data, n, H, W, who)) return false;
+    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
+        const int d = c->vis.proj;
+        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
+            return hi == lo || image_batch_encode_one(r, 4, imgs->data + lo, hi - lo, vec + lo * d, nullptr, normalize, true, H, W, who);
+        });
+    }
+    return image_batch_encode_one(c, 4, imgs->data, n, vec, nullptr, normalize, true, H, W, who);
 }
 
 bool clip_image_encode(const struct clip_ctx* ctx, const int n_threads, struct clip_image_f32* img, float* vec, const bool normalize) {
@@ -1043,22 +1155,44 @@ bool clip_b200_text_encode_device(const struct clip_ctx* cctx, const void* d_ids
 // ---- per-token hidden states ----------------------------------------------------------------------------------------------------
 // One GPU, host buffers: each micro-batch's inputs go up on the launch stream, its rows come back straight into the caller's `out`
 // (a staging buffer of one micro-batch on the device; the whole output is never held there).
-static bool image_tokens_one(clip_ctx* c, const clip_image_f32* imgs, size_t n, const TokenReq& q, char* out) {
+static bool image_tokens_one(clip_ctx* c, const clip_image_f32* imgs, size_t n, const TokenReq& q, char* out, int H = 0, int W = 0,
+                             const char* who = "clip_b200_image_tokens") {
     Tower& tw = c->vis;
     std::lock_guard<std::mutex> lk(c->mu);
     CK(cudaSetDevice(c->device));
-    if (!ensure_ws(c, tw, tw.micro_batch, tw.T, true)) return false;
+    VisCall v;
+    int mb = 0;
+    if (!plan_call(c, H, W, v, mb, who)) return false;
     size_t n_chunks, chunk;
-    chunking(n, tw.micro_batch, n_chunks, chunk);
+    chunking(n, mb, n_chunks, chunk);
     if (!ensure_out(c, (chunk * q.item_bytes + 3) / 4)) return false;
-    const size_t per = (size_t)tw.image_size * tw.image_size * 3;
+    const size_t per = v.per();
     CK(cudaEventRecord(c->ev_t0, c->stream));
     for (size_t i0 = 0; i0 < n; i0 += chunk) {
         const int nb = (int)std::min(chunk, n - i0);
         for (int j = 0; j < nb; j++)
             CK(cudaMemcpyAsync(tw.ws.pixels[0] + (size_t)j * per, imgs[i0 + j].data, per * 4, cudaMemcpyHostToDevice, c->stream));
-        if (!vision_tokens(c, tw.ws.pixels[0], nb, q, c->d_out)) return false;
+        if (!vision_tokens(c, tw.ws.pixels[0], nb, v, q, c->d_out)) return false;
         CK(cudaMemcpyAsync(out + i0 * q.item_bytes, c->d_out, nb * q.item_bytes, cudaMemcpyDeviceToHost, c->stream));
+    }
+    CK(cudaEventRecord(c->ev_t1, c->stream));
+    return sync_and_time(c);
+}
+
+// n images of H x W (0 x 0: the model's size) resident at d_pixels -> rows at d_out
+static bool image_tokens_device_impl(clip_ctx* c, const float* d_pixels, size_t n, const TokenReq& q, char* d_out, int H, int W, const char* who) {
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    VisCall v;
+    int mb = 0;
+    if (!plan_call(c, H, W, v, mb, who)) return false;
+    size_t n_chunks, chunk;
+    chunking(n, mb, n_chunks, chunk);
+    const size_t per = v.per();
+    CK(cudaEventRecord(c->ev_t0, c->stream));
+    for (size_t i0 = 0; i0 < n; i0 += chunk) {
+        const int nb = (int)std::min(chunk, n - i0);
+        if (!vision_tokens(c, d_pixels + i0 * per, nb, v, q, d_out + i0 * q.item_bytes)) return false;
     }
     CK(cudaEventRecord(c->ev_t1, c->stream));
     return sync_and_time(c);
@@ -1089,20 +1223,41 @@ bool clip_b200_image_tokens_device(const struct clip_ctx* cctx, const void* d_pi
     if (!token_request(c, true, layer, flags, out_type, c->vis.T, q, "clip_b200_image_tokens_device")) return false;
     if (n == 0) return true;
     if (!d_pixels || !d_out) { set_err("clip_b200_image_tokens_device: null device pointer"); return false; }
-    Tower& tw = c->vis;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    if (!ensure_ws(c, tw, tw.micro_batch, tw.T, true)) return false;
-    size_t n_chunks, chunk;
-    chunking(n, tw.micro_batch, n_chunks, chunk);
-    const size_t per = (size_t)tw.image_size * tw.image_size * 3;
-    CK(cudaEventRecord(c->ev_t0, c->stream));
-    for (size_t i0 = 0; i0 < n; i0 += chunk) {
-        const int nb = (int)std::min(chunk, n - i0);
-        if (!vision_tokens(c, (const float*)d_pixels + i0 * per, nb, q, (char*)d_out + i0 * q.item_bytes)) return false;
+    return image_tokens_device_impl(c, (const float*)d_pixels, n, q, (char*)d_out, 0, 0, "clip_b200_image_tokens_device");
+}
+
+bool clip_b200_image_tokens_hw(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, int layer, int flags, int out_type, void* out) {
+    const char* who = "clip_b200_image_tokens_hw";
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    TokenReq q;
+    if (!c) { set_err(std::string(who) + ": null context"); return false; }
+    if (!c->has_vision) { set_err(std::string(who) + ": this model has no vision encoder"); return false; }
+    const size_t n = imgs ? imgs->size : 0;
+    if (n == 0) return token_request(c, true, layer, flags, out_type, c->vis.T, q, who);
+    if (!out) { set_err(std::string(who) + ": null output"); return false; }
+    int H = 0, W = 0;
+    if (!check_images_hw(c, imgs->data, n, H, W, who)) return false;
+    if (!token_request(c, true, layer, flags, out_type, (H / c->vis.patch) * (W / c->vis.patch) + 1, q, who)) return false;
+    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
+        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
+            return hi == lo || image_tokens_one(r, imgs->data + lo, hi - lo, q, (char*)out + lo * q.item_bytes, H, W, who);
+        });
     }
-    CK(cudaEventRecord(c->ev_t1, c->stream));
-    return sync_and_time(c);
+    return image_tokens_one(c, imgs->data, n, q, (char*)out, H, W, who);
+}
+
+bool clip_b200_image_tokens_device_hw(const struct clip_ctx* cctx, const void* d_pixels, size_t n, int height, int width, int layer, int flags,
+                                      int out_type, void* d_out) {
+    const char* who = "clip_b200_image_tokens_device_hw";
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    TokenReq q;
+    if (!c) { set_err(std::string(who) + ": null context"); return false; }
+    if (!c->has_vision) { set_err(std::string(who) + ": this model has no vision encoder"); return false; }
+    if (!check_hw_size(c, height, width, who)) return false;
+    if (!token_request(c, true, layer, flags, out_type, (height / c->vis.patch) * (width / c->vis.patch) + 1, q, who)) return false;
+    if (n == 0) return true;
+    if (!d_pixels || !d_out) { set_err(std::string(who) + ": null device pointer"); return false; }
+    return image_tokens_device_impl(c, (const float*)d_pixels, n, q, (char*)d_out, height, width, who);
 }
 
 // n padded sequences of seq_len ids, on the host (h_ids) or the device (d_ids) -> rows at out (host) or d_out (device)
@@ -1869,12 +2024,41 @@ int clip_b200_debug_im2col(const float* pixels, int B, int S, int P, int kpad, f
     float* d_px = (float*)s.alloc(pb, 0, pixels, pb);
     uint16_t* d_out = (uint16_t*)s.alloc(n * 2, 0xff);
     if (!s.ok) return 3;
-    launch_im2col(d_px, B, S, P, kpad, d_out, s.st);
+    launch_im2col(d_px, B, S, S, P, kpad, d_out, s.st);
     if (!s.finish("im2col")) return 5;
     std::vector<uint16_t> o16(n);
     if (!s.copy_back(o16.data(), d_out, n * 2)) return 6;
     from16(o16.data(), n, 0, out);
     return 0;
+}
+
+int clip_b200_debug_im2col_hw(const float* pixels, int B, int H, int W, int P, int kpad, float* out) {
+    g_err.clear();
+    if (B <= 0 || P <= 0 || H <= 0 || W <= 0 || H % P || W % P || kpad < 3 * P * P) { set_err("debug_im2col_hw: bad shape"); return 1; }
+    HookScratch s;
+    const size_t pb = (size_t)B * H * W * 3 * 4, n = (size_t)B * (H / P) * (W / P) * kpad;
+    float* d_px = (float*)s.alloc(pb, 0, pixels, pb);
+    uint16_t* d_out = (uint16_t*)s.alloc(n * 2, 0xff);
+    if (!s.ok) return 3;
+    launch_im2col(d_px, B, H, W, P, kpad, d_out, s.st);
+    if (!s.finish("im2col")) return 5;
+    std::vector<uint16_t> o16(n);
+    if (!s.copy_back(o16.data(), d_out, n * 2)) return 6;
+    from16(o16.data(), n, 0, out);
+    return 0;
+}
+
+int clip_b200_debug_pos_resample(const float* table, int g, int h, int gh, int gw, float* out) {
+    g_err.clear();
+    if (g <= 0 || h <= 0 || gh <= 0 || gw <= 0) { set_err("debug_pos_resample: bad shape"); return 1; }
+    HookScratch s;
+    const size_t tb = (size_t)g * g * h * 4, ob = (size_t)gh * gw * h * 4;
+    float* d_t = (float*)s.alloc(tb, 0, table, tb);
+    float* d_out = (float*)s.alloc(ob, 0xff);
+    if (!s.ok) return 3;
+    launch_pos_resample(d_t, g, h, gh, gw, d_out, s.st);
+    if (!s.finish("pos_resample")) return 5;
+    return s.copy_back(out, d_out, ob) ? 0 : 6;
 }
 
 int clip_b200_debug_text_embed(const int32_t* ids, const float* tok, const float* pos, int nseq, int T, int h, int n_vocab, float* x_out) {

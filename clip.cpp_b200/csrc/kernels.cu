@@ -1,5 +1,5 @@
 // kernels.cu -- the memory-bound kernels around the GEMMs: LayerNorm (K2), im2col (K0a), embedding assembly (K4),
-// L2-normalise (K5), per-token output rows (K7), plus a scalar debug GEMM (scoring lives in search.cu).  All are HBM-bound streaming kernels: one warp per
+// L2-normalise (K5), per-token output rows (K7), position-table resample (K8), plus a scalar debug GEMM (scoring lives in search.cu).  All are HBM-bound streaming kernels: one warp per
 // row, 128-bit coalesced loads, warp-shuffle reductions, no shared memory.
 #include <stdlib.h>
 #include <string.h>
@@ -158,21 +158,61 @@ __global__ void __launch_bounds__(256) token_rows_kernel(const float* __restrict
     }
 }
 
-__global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ px, int B, int S, int P, int kpad,
+__global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ px, int B, int H, int W, int P, int kpad,
                                                      __half* __restrict__ out) {
-    const int np1 = S / P, K = 3 * P * P;
-    const size_t total = (size_t)B * np1 * np1 * kpad;
+    const int gh = H / P, gw = W / P, np = gh * gw, K = 3 * P * P;
+    const size_t total = (size_t)B * np * kpad;
     for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
         const int k = (int)(idx % kpad);
         const size_t rowi = idx / kpad;
         float v = 0.f;
         if (k < K) {
-            const int p = (int)(rowi % (np1 * np1)), b = (int)(rowi / (np1 * np1));
-            const int py = p / np1, pxx = p % np1;
+            const int p = (int)(rowi % np), b = (int)(rowi / np);
+            const int py = p / gw, pxx = p % gw;
             const int c = k / (P * P), rem = k % (P * P), ky = rem / P, kx = rem % P;
-            v = px[(((size_t)b * S + (py * P + ky)) * S + (pxx * P + kx)) * 3 + c];
+            v = px[(((size_t)b * H + (py * P + ky)) * W + (pxx * P + kx)) * 3 + c];
         }
         out[idx] = __float2half_rn(v);
+    }
+}
+
+// K8 bicubic weights (torch's upsample_bicubic2d, A = -0.75) of the output index o on an axis of g -> go, in fp64 with every
+// operation rounded on its own (no contraction), so that a numpy restatement reproduces them bit for bit.
+CB_DEVINL void cubic_taps(int o, int g, int go, int idx[4], double w[4]) {
+    const double src = __dadd_rn(__dmul_rn(__ddiv_rn((double)g, (double)go), __dadd_rn((double)o, 0.5)), -0.5);   // not clamped
+    const double fi = floor(src), t = __dadd_rn(src, -fi), s = __dadd_rn(1.0, -t);
+    // cc1(x) = ((A+2) x - (A+3)) x x + 1,  cc2(x) = ((A x - 5A) x + 8A) x - 4A
+    auto cc1 = [](double x) { return __dadd_rn(__dmul_rn(__dmul_rn(__dadd_rn(__dmul_rn(1.25, x), -2.25), x), x), 1.0); };
+    auto cc2 = [](double x) { return __dadd_rn(__dmul_rn(__dadd_rn(__dmul_rn(__dadd_rn(__dmul_rn(-0.75, x), 3.75), x), -6.0), x), 3.0); };
+    w[0] = cc2(__dadd_rn(t, 1.0)); w[1] = cc1(t); w[2] = cc1(s); w[3] = cc2(__dadd_rn(s, 1.0));
+    const int i = (int)fi;
+    #pragma unroll
+    for (int k = 0; k < 4; k++) idx[k] = min(max(i - 1 + k, 0), g - 1);
+}
+
+// K8 position-table resample: out[(oy*gw + ox), c] from table [g*g, h] (row-major grid y, then x).  One thread per output element,
+// c fastest, so a warp reads and writes consecutive columns; each output reads 16 table elements (L1 / L2 hits: the table is at
+// most a few MB) and is written once.  Horizontal pass first per source row, then the vertical one, each a left-to-right sum.
+__global__ void __launch_bounds__(256) pos_resample_kernel(const float* __restrict__ table, int g, int h, int gh, int gw,
+                                                           float* __restrict__ out) {
+    const size_t total = (size_t)gh * gw * h;
+    for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+        const int c = (int)(e % h), o = (int)(e / h), oy = o / gw, ox = o % gw;
+        int iy[4], ix[4];
+        double wy[4], wx[4];
+        cubic_taps(oy, g, gh, iy, wy);
+        cubic_taps(ox, g, gw, ix, wx);
+        double acc = 0.0;
+        #pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const float* r = table + (size_t)iy[j] * g * h + c;
+            double row = __dmul_rn((double)r[(size_t)ix[0] * h], wx[0]);
+            row = __dadd_rn(row, __dmul_rn((double)r[(size_t)ix[1] * h], wx[1]));
+            row = __dadd_rn(row, __dmul_rn((double)r[(size_t)ix[2] * h], wx[2]));
+            row = __dadd_rn(row, __dmul_rn((double)r[(size_t)ix[3] * h], wx[3]));
+            acc = j == 0 ? __dmul_rn(row, wy[0]) : __dadd_rn(acc, __dmul_rn(row, wy[j]));
+        }
+        out[e] = __double2float_rn(acc);
     }
 }
 
@@ -333,12 +373,20 @@ void launch_token_rows(const float* x, size_t in_stride, int n, int T, int skip,
 #undef CB_TR
 }
 
-void launch_im2col(const float* pixels, int B, int S, int P, int kpad, void* patches16, cudaStream_t st) {
-    const size_t total = (size_t)B * (S / P) * (S / P) * kpad;
+void launch_im2col(const float* pixels, int B, int H, int W, int P, int kpad, void* patches16, cudaStream_t st) {
+    const size_t total = (size_t)B * (H / P) * (W / P) * kpad;
     if (!total) return;
     size_t blocks = (total + 255) / 256;
     if (blocks > 132 * 32) blocks = 132 * 32;      // grid-stride loop: 32 blocks per H100 SM
-    im2col_kernel<<<(int)blocks, 256, 0, st>>>(pixels, B, S, P, kpad, (__half*)patches16);
+    im2col_kernel<<<(int)blocks, 256, 0, st>>>(pixels, B, H, W, P, kpad, (__half*)patches16);
+}
+
+void launch_pos_resample(const float* table, int g, int h, int gh, int gw, float* out, cudaStream_t st) {
+    const size_t total = (size_t)gh * gw * h;
+    if (!total) return;
+    size_t blocks = (total + 255) / 256;
+    if (blocks > 132 * 8) blocks = 132 * 8;
+    pos_resample_kernel<<<(int)blocks, 256, 0, st>>>(table, g, h, gh, gw, out);
 }
 
 void launch_assemble_preln(const float* patch, const float* class_embd, const float* pos, int B, int T, int h, float eps,

@@ -18,9 +18,16 @@ void launch_layernorm(float* x, size_t in_stride, int rows, int h, float eps, co
 void launch_token_rows(const float* x, size_t in_stride, int n, int T, int skip, int h, const float* gamma, const float* beta, float eps,
                        int out_type, void* out, cudaStream_t st);
 
-// K0a im2col for the stride-P patch conv: pixels NHWC f32 [B,S,S,3] -> fp16 [B*Np, kpad], k = c*P*P + ky*P + kx,
-// zero padded to kpad (reference conv_2d im2col, ggml.c:13595-13631; pixel -> fp16 rounding ggml.c:13623).
-void launch_im2col(const float* pixels, int B, int S, int P, int kpad, void* patches16, cudaStream_t st);
+// K0a im2col for the stride-P patch conv: pixels NHWC f32 [B,H,W,3] -> fp16 [B*Np, kpad], Np = (H/P)(W/P) patches in row-major
+// grid order, k = c*P*P + ky*P + kx, zero padded to kpad (reference conv_2d im2col, ggml.c:13595-13631; pixel -> fp16 rounding
+// ggml.c:13623).  The model's own size passes H = W = image_size.
+void launch_im2col(const float* pixels, int B, int H, int W, int P, int kpad, void* patches16, cudaStream_t st);
+
+// K8 position-table resample (HF interpolate_pos_encoding): table fp32 [g*g, h] (the patch rows of a g x g grid) -> out fp32
+// [gh*gw, h], torch's upsample_bicubic2d (A = -0.75, align_corners = False, taps clamped to the edge) evaluated in fp64 without
+// contraction, horizontal pass first, rounded once to fp32.  Torch evaluates the same formula in fp32, so the two agree within
+// the rounding of torch's fp32 coordinates, weights and sums (tests/test_pos_resample.py), not bit for bit.
+void launch_pos_resample(const float* table, int g, int h, int gh, int gw, float* out, cudaStream_t st);
 
 // K4v assemble + pre-LN: x[b,t,:] = LN( (t==0 ? class_embd : patch[b*Np+t-1,:]) + pos[t,:] ) * g + b  -> fp32
 // (clip.cpp:1315-1339)

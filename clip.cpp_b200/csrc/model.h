@@ -107,6 +107,9 @@ struct clip_ctx {
     float* d_logits = nullptr; size_t d_logits_cap = 0;
     float* d_cand_v[2] = {nullptr, nullptr}; int* d_cand_i[2] = {nullptr, nullptr}; size_t d_cand_cap = 0;
     float* d_emb[2] = {nullptr, nullptr}; size_t d_emb_cap[2] = {0, 0};     // image / text embeddings kept on the device (zero-shot)
+    // the last position table resampled for a non-native image size (*_hw calls): CLS row + gh*gw patch rows [T, h], grow-only
+    float* pos_hw = nullptr; size_t pos_hw_cap = 0;
+    int pos_gh = 0, pos_gw = 0;
     double* d_scalars = nullptr;            // 16 doubles for the tiny all-reduces (barrier, max over ranks)
     // ---- multi-GPU (dist.h) ------------------------------------------------------------------------------------------
     cb::DistComm dist;                      // this replica's NCCL communicator (ranks mode or devices mode); world == 1: none

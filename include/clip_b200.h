@@ -203,6 +203,31 @@ bool clip_b200_text_tokens(const struct clip_ctx * ctx, const int32_t * ids, siz
 bool clip_b200_text_tokens_device(const struct clip_ctx * ctx, const void * d_ids, size_t n, int seq_len, int layer, int flags,
                                   int out_type, void * d_out);
 
+/* Vision tower at height x width pixels (both positive multiples of patch_size, <= 4096; rectangular allowed) -- HF
+ * CLIPVisionModel(..., interpolate_pos_encoding=True).  The patch grid is gh x gw = height/P x width/P, T = gh*gw + 1.  Patch rows of
+ * the position table are resampled to gh x gw as HF's interpolate_pos_encoding does (bicubic, A = -0.75, align_corners = False);
+ * the CLS row is unchanged.  The resample is evaluated in fp64 and rounded once to fp32, where torch evaluates it in fp32: the table
+ * agrees with HF's to within the fp32 rounding of torch's source coordinates, weights and sums (up to ~25 ulps of the table's
+ * largest entry in tests/test_pos_resample.py), not bit for bit.  At height = width = image_size no resampling happens and every result equals
+ * the existing entry point's bit for bit.
+ *   pixels   NHWC f32 [n, height, width, 3], already normalised, as for the entry points above.
+ *   d_vec    [n, projection_dim];  token rows [n, T or T - 1, width], patch rows in row-major grid order (y, then x), as HF's
+ *            flatten(2) gives them.  layer, flags and out_type are those of clip_b200_image_tokens, with the same refusals.
+ * The workspace is sized as for the model's own size (micro_batch images of the native T, clip_b200_set_micro_batch); a call at
+ * another size runs as many images per pass as fit it.  The context keeps the last resampled table, so a call at a new size costs
+ * one resample launch.  Refused with a message in clip_b200_last_error(): a size that is not a positive multiple of patch_size or
+ * is above 4096, mixed sizes in one host call, a model without a vision tower, a size too large for even one image to fit the
+ * workspace.  n == 0 returns true.  Host forms: the size is the images' own (ny rows of nx pixels), every image of one call must
+ * have the same size; devices mode (CLIP_B200_DEVICES) shards the batch as clip_image_batch_encode does. */
+bool clip_b200_image_encode_device_hw(const struct clip_ctx * ctx, const void * d_pixels, size_t n, int height, int width,
+                                      void * d_vec, bool normalize);
+bool clip_b200_image_tokens_device_hw(const struct clip_ctx * ctx, const void * d_pixels, size_t n, int height, int width,
+                                      int layer, int flags, int out_type, void * d_out);
+bool clip_b200_image_batch_encode_hw(const struct clip_ctx * ctx, const struct clip_image_f32_batch * imgs, float * vec,
+                                     bool normalize);
+bool clip_b200_image_tokens_hw(const struct clip_ctx * ctx, const struct clip_image_f32_batch * imgs, int layer, int flags,
+                               int out_type, void * out);
+
 /* Batched zero-shot scoring on the device (clip.cpp:1624-1659 semantics per image): d_img_vec [n_img, d], d_txt_vec [n_txt, d]
  * -> host scores/indices [n_img, top_k], best first; similarity matrix, softmax and top-k selection all run on the GPU.
  * Ranking (here and in clip_b200_topk_search): top_k <= 0 or top_k > n_txt means all n_txt, and row i of the output starts at
@@ -276,7 +301,8 @@ void   clip_b200_set_micro_batch(const struct clip_ctx * ctx, int images, int se
 uint64_t clip_b200_kernel_launches(const struct clip_ctx * ctx);   /* kernels launched by this context so far */
 float    clip_b200_last_device_ms(const struct clip_ctx * ctx);    /* CUDA-event time of the last encode's kernels */
 /* per-kernel-class CUDA-event time accumulated since the last call with the same kind (0 GEMM, 1 attention,
- * 2 layernorm, 3 other, 4 the token-row kernel of the *_tokens calls); *count receives the number of launches.  Enabled by env CLIP_B200_PROFILE=1. */
+ * 2 layernorm, 3 other, 4 the token-row kernel of the *_tokens calls, 5 the position-table resample of the *_hw calls); *count
+ * receives the number of launches.  Enabled by env CLIP_B200_PROFILE=1. */
 float    clip_b200_kernel_ms(const struct clip_ctx * ctx, int kind, uint64_t * count);
 /* CUDA-event stopwatch on the launch stream: mark(slot 0..3), then elapsed(a, b) in ms (-1 on error) */
 bool     clip_b200_mark(const struct clip_ctx * ctx, int slot);
@@ -323,6 +349,10 @@ int clip_b200_debug_assemble_preln(const float * patch, const float * class_embd
                                    const float * gamma, const float * beta, float * x_out);
 /* im2col: NHWC pixels [B, S, S, 3] -> fp16 patches [B*(S/P)^2, kpad] (widened to fp32 in out) */
 int clip_b200_debug_im2col(const float * pixels, int B, int S, int P, int kpad, float * out);
+/* the same for rectangles: [B, H, W, 3] -> [B*(H/P)*(W/P), kpad], patches in row-major grid order */
+int clip_b200_debug_im2col_hw(const float * pixels, int B, int H, int W, int P, int kpad, float * out);
+/* position-table resample (K8): table [g*g, h] (patch rows only) -> out [gh*gw, h], as the *_hw entry points resample */
+int clip_b200_debug_pos_resample(const float * table, int g, int h, int gh, int gw, float * out);
 /* text embedding: ids [nseq*T] (clamped to [0, n_vocab)), tok [n_vocab, h], pos [T, h] -> x_out [nseq*T, h] */
 int clip_b200_debug_text_embed(const int32_t * ids, const float * tok, const float * pos, int nseq, int T, int h, int n_vocab,
                                float * x_out);
