@@ -85,6 +85,9 @@ EXTENSION_SYMBOLS = [
     # any patch-multiple image size (interpolated position table)
     "clip_b200_image_encode_device_hw", "clip_b200_image_tokens_device_hw", "clip_b200_image_batch_encode_hw", "clip_b200_image_tokens_hw",
     "clip_b200_debug_im2col_hw", "clip_b200_debug_pos_resample",
+    # several layers' token rows from one forward pass
+    "clip_b200_image_tokens_layers", "clip_b200_image_tokens_layers_device", "clip_b200_text_tokens_layers",
+    "clip_b200_text_tokens_layers_device",
 ]
 
 # include/clip_b200.h: output types and flags of the *_tokens entry points
@@ -225,6 +228,15 @@ class ClipLib:
             L.clip_b200_image_batch_encode_hw.argtypes = [vp, C.POINTER(clip_image_f32_batch), fp, C.c_bool]
             L.clip_b200_image_tokens_hw.restype = C.c_bool
             L.clip_b200_image_tokens_hw.argtypes = [vp, C.POINTER(clip_image_f32_batch), ip, ip, ip, vp]
+            intp = C.POINTER(C.c_int)
+            L.clip_b200_image_tokens_layers.restype = C.c_bool
+            L.clip_b200_image_tokens_layers.argtypes = [vp, C.POINTER(clip_image_f32_batch), intp, intp, ip, ip, vp]
+            L.clip_b200_image_tokens_layers_device.restype = C.c_bool
+            L.clip_b200_image_tokens_layers_device.argtypes = [vp, vp, C.c_size_t, ip, ip, intp, intp, ip, ip, vp]
+            L.clip_b200_text_tokens_layers.restype = C.c_bool
+            L.clip_b200_text_tokens_layers.argtypes = [vp, i32p, C.c_size_t, ip, intp, intp, ip, ip, vp]
+            L.clip_b200_text_tokens_layers_device.restype = C.c_bool
+            L.clip_b200_text_tokens_layers_device.argtypes = [vp, vp, C.c_size_t, ip, intp, intp, ip, ip, vp]
             ipp = C.POINTER(C.c_int)
             L.clip_b200_topk_search.restype = C.c_bool
             L.clip_b200_topk_search.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, ip, fp, ipp]
@@ -396,6 +408,79 @@ class ClipLib:
                                               out_type, out.ctypes.data):
             raise RuntimeError("clip_b200_text_tokens failed: " + self.last_error())
         return out
+
+    # ---- several layers from one forward pass (include/clip_b200.h: *_tokens_layers) ----------------------------------------------
+    def _layers_call(self, ctx, vision, n, rows, layers, flags, out_type, out, call, name):
+        """run call(c_layers, c_flags, n_layers, out) and return the per-entry views of the layer-major output, each shaped as the
+        single-layer wrapper shapes its result.  flags None is passed as NULL (0 for every entry).  `out`: a flat buffer of the
+        output dtype to write into (for example pinned memory), or None for a new numpy array."""
+        layers = [int(l) for l in layers]
+        k = max(len(layers), 1)
+        c_layers = (C.c_int * k)(*layers)
+        fl = [0] * len(layers) if flags is None else [int(f) for f in flags]
+        c_flags = None if flags is None else (C.c_int * max(len(fl), 1))(*fl)
+        shapes = [self.token_shape(ctx, vision, n, rows, f) for f in fl[:len(layers)]]
+        sizes = [int(np.prod(s)) for s in shapes]
+        if out is None:
+            out = np.empty(sum(sizes), OUT_DTYPES.get(out_type, np.float32))
+        assert out.flags["C_CONTIGUOUS"] and out.size >= sum(sizes)
+        if not call(c_layers, c_flags, len(layers), out):
+            raise RuntimeError(name + " failed: " + self.last_error())
+        flat, views, o = out.reshape(-1), [], 0
+        for s, z in zip(shapes, sizes):
+            views.append(flat[o:o + z].reshape(s))
+            o += z
+        return views
+
+    def _via_device(self, ctx, inp, out, fn):
+        """upload inp, fn(d_in, d_out) into a device buffer of out.nbytes, download into out"""
+        d_in = self.lib.clip_b200_device_malloc(ctx, max(inp.nbytes, 1))
+        d_out = self.lib.clip_b200_device_malloc(ctx, max(out.nbytes, 1))
+        try:
+            if not (d_in and d_out and self.lib.clip_b200_memcpy_h2d(ctx, d_in, inp.ctypes.data, inp.nbytes)):
+                return False
+            if not fn(d_in, d_out):
+                return False
+            return self.lib.clip_b200_memcpy_d2h(ctx, out.ctypes.data, d_out, out.nbytes)
+        finally:
+            self.lib.clip_b200_device_free(ctx, d_in)
+            self.lib.clip_b200_device_free(ctx, d_out)
+
+    def image_tokens_layers(self, ctx, images: np.ndarray, layers, flags=None, out_type: int = OUT_F32, out=None):
+        """images [n, H, W, 3] float32 -> one [n, T or T - 1, width] array per entry (layers[j], flags[j]), from one forward pass"""
+        batch, keep = self.make_image_batch(images)
+        P = self.vision_hparams(ctx).patch_size
+        T = (images.shape[1] // P) * (images.shape[2] // P) + 1
+        return self._layers_call(ctx, True, images.shape[0], T, layers, flags, out_type, out,
+                                 lambda ls, fs, k, o: self.lib.clip_b200_image_tokens_layers(ctx, C.byref(batch), ls, fs, k, out_type, o.ctypes.data),
+                                 "clip_b200_image_tokens_layers")
+
+    def image_tokens_layers_device(self, ctx, images: np.ndarray, layers, flags=None, out_type: int = OUT_F32):
+        """image_tokens_layers through the device form: images uploaded, the slabs written on the GPU and downloaded"""
+        images = np.ascontiguousarray(images, np.float32)
+        n, H, W = images.shape[:3]
+        P = self.vision_hparams(ctx).patch_size
+        return self._layers_call(ctx, True, n, (H // P) * (W // P) + 1, layers, flags, out_type, None,
+                                 lambda ls, fs, k, o: self._via_device(ctx, images, o, lambda di, do: self.lib.clip_b200_image_tokens_layers_device(
+                                     ctx, di, n, H, W, ls, fs, k, out_type, do)),
+                                 "clip_b200_image_tokens_layers_device")
+
+    def text_tokens_layers(self, ctx, ids: np.ndarray, layers, flags=None, out_type: int = OUT_F32, out=None):
+        """ids [n, seq_len] int32, padded by the caller -> one [n, seq_len, width] array per entry, from one forward pass"""
+        ids = np.ascontiguousarray(ids, np.int32)
+        return self._layers_call(ctx, False, ids.shape[0], ids.shape[1], layers, flags, out_type, out,
+                                 lambda ls, fs, k, o: self.lib.clip_b200_text_tokens_layers(
+                                     ctx, ids.ctypes.data_as(C.POINTER(C.c_int32)), ids.shape[0], ids.shape[1], ls, fs, k, out_type, o.ctypes.data),
+                                 "clip_b200_text_tokens_layers")
+
+    def text_tokens_layers_device(self, ctx, ids: np.ndarray, layers, flags=None, out_type: int = OUT_F32):
+        """text_tokens_layers through the device form"""
+        ids = np.ascontiguousarray(ids, np.int32)
+        n, S = ids.shape
+        return self._layers_call(ctx, False, n, S, layers, flags, out_type, None,
+                                 lambda ls, fs, k, o: self._via_device(ctx, ids, o, lambda di, do: self.lib.clip_b200_text_tokens_layers_device(
+                                     ctx, di, n, S, ls, fs, k, out_type, do)),
+                                 "clip_b200_text_tokens_layers_device")
 
     @staticmethod
     def make_token_array(seqs):

@@ -270,8 +270,9 @@ bool run_linear(clip_ctx* c, const Linear& L, const TmaMap* xmap, const void* xp
     return true;
 }
 
-// The per-layer schedule shared by both towers (clip.cpp:1064-1143 text, 1342-1423 vision): blocks 0 .. n_blocks-1.
-bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal, int n_blocks) {
+// The per-layer schedule shared by both towers (clip.cpp:1064-1143 text, 1342-1423 vision): blocks first .. end-1 on ws.x (a
+// multi-layer tokens call resumes where its previous stop left x).
+bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal, int first, int end) {
     // The residual stream x stays fp32 (as in the reference).  The branch GEMMs (out-proj, FC2) add their result INTO x themselves
     // (EPI_REDADD32): LayerNorm then only reads x and writes its 16-bit output.
     Workspace& w = tw.ws;
@@ -279,7 +280,7 @@ bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal, int n_bloc
     const int bf = c->operand_bf16 ? 1 : 0;
     const int dh = h / tw.heads;                      // 64 or 80 (check_geometry)
     const float qscale = 1.0f / sqrtf((float)dh);     // clip.cpp:1082, 1363
-    for (int il = 0; il < n_blocks; il++) {
+    for (int il = first; il < end; il++) {
         const Layer& l = tw.L[il];
         { Scope s(c, K_LN); launch_layernorm(w.x, h, M, h, tw.eps, l.ln1_g, l.ln1_b, nullptr, w.a, bf, c->stream); }
         if (!run_linear(c, l.qkv, &w.map_a, w.a, bf, M, w.qkv, 3 * h, EPI_STORE16, bf, h, qscale)) return false;
@@ -325,7 +326,7 @@ bool vision_forward(clip_ctx* c, const float* d_pixels, int nb, const VisCall& v
     Workspace& w = tw.ws;
     const int h = tw.hidden, bf = c->operand_bf16 ? 1 : 0;
     if (!vision_embed(c, d_pixels, nb, v)) return false;
-    if (!run_blocks(c, tw, nb, v.T, false, tw.layers)) return false;
+    if (!run_blocks(c, tw, nb, v.T, false, 0, tw.layers)) return false;
     // CLS rows -> post-LN -> projection -> (L2 norm)   (clip.cpp:1426-1455)
     { Scope s(c, K_LN); launch_layernorm(w.x, (size_t)v.T * h, nb, h, tw.eps, tw.post_g, tw.post_b, nullptr, w.sel16, bf, c->stream); }
     if (!run_linear(c, tw.proj_w, &w.map_sel, w.sel16, bf, nb, w.proj32, tw.proj, EPI_STORE32, 0)) return false;
@@ -340,7 +341,7 @@ bool text_forward(clip_ctx* c, int nb, int T, float* d_out, bool normalize) {
     Workspace& w = tw.ws;
     const int h = tw.hidden, bf = c->operand_bf16 ? 1 : 0;
     { Scope s(c, K_OTHER); launch_text_embed(w.ids, tw.tok, tw.pos, nb, T, h, tw.n_vocab, w.x, c->stream); }
-    if (!run_blocks(c, tw, nb, T, true, tw.layers)) return false;
+    if (!run_blocks(c, tw, nb, T, true, 0, tw.layers)) return false;
     // final LN is row-wise, so LN(select(EOT)) == select(LN(all)) (clip.cpp:1146-1155)
     { Scope s(c, K_OTHER); launch_gather_rows(w.x, w.sel32, nb, h, T, w.last, nullptr, bf, c->stream); }
     { Scope s(c, K_LN); launch_layernorm(w.sel32, h, nb, h, tw.eps, tw.post_g, tw.post_b, nullptr, w.sel16, bf, c->stream); }
@@ -405,18 +406,118 @@ bool token_rows_tail(clip_ctx* c, Tower& tw, int nb, int T, const TokenReq& q, v
     return true;
 }
 
-// nb images at d_pixels through q.blocks blocks -> dst
-bool vision_tokens(clip_ctx* c, const float* d_pixels, int nb, const VisCall& v, const TokenReq& q, void* dst) {
-    Tower& tw = c->vis;
-    return vision_embed(c, d_pixels, nb, v) && run_blocks(c, tw, nb, v.T, false, q.blocks) && token_rows_tail(c, tw, nb, v.T, q, dst);
+// The entries of one tokens call (one for the single-layer calls), for nb items whose embedding is in ws.x: the blocks run once, up
+// to the deepest entry, each run resuming where the previous stop left x; after each block count some entry asks for, emit(j) writes
+// entry j's rows (token_rows_tail) while x holds that layer.  Between stops only x is live, so a PROJECT tail may use a, qkv and g.
+template <class Emit>
+bool token_stops(clip_ctx* c, Tower& tw, int nb, int T, bool causal, const std::vector<TokenReq>& qs, Emit emit) {
+    std::vector<int> order(qs.size());
+    std::iota(order.begin(), order.end(), 0);
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return qs[a].blocks < qs[b].blocks; });
+    int done = 0;
+    for (int j : order) {
+        if (qs[j].blocks > done) {
+            if (!run_blocks(c, tw, nb, T, causal, done, qs[j].blocks)) return false;
+            done = qs[j].blocks;
+        }
+        if (!emit(j)) return false;
+    }
+    return true;
 }
 
-// nb sequences of T ids already in ws.ids through q.blocks blocks -> dst
-bool text_tokens(clip_ctx* c, int nb, int T, const TokenReq& q, void* dst) {
+// nb images at d_pixels through the blocks of every entry -> emit(j)
+template <class Emit>
+bool vision_tokens(clip_ctx* c, const float* d_pixels, int nb, const VisCall& v, const std::vector<TokenReq>& qs, Emit emit) {
+    return vision_embed(c, d_pixels, nb, v) && token_stops(c, c->vis, nb, v.T, false, qs, emit);
+}
+
+// nb sequences of T ids already in ws.ids through the blocks of every entry -> emit(j)
+template <class Emit>
+bool text_tokens(clip_ctx* c, int nb, int T, const std::vector<TokenReq>& qs, Emit emit) {
     Tower& tw = c->txt;
     { Scope s(c, K_OTHER); launch_text_embed(tw.ws.ids, tw.tok, tw.pos, nb, T, tw.hidden, tw.n_vocab, tw.ws.x, c->stream); }
-    return run_blocks(c, tw, nb, T, true, q.blocks) && token_rows_tail(c, tw, nb, T, q, dst);
+    return token_stops(c, tw, nb, T, true, qs, emit);
 }
+
+// Layer-major output of a tokens call: entry j's slab of n items starts at n * (item_bytes of the entries before it); the shard of
+// items lo .. of a devices-mode GPU starts lo * item_bytes_j into each slab.
+std::vector<char*> slab_bases(const std::vector<TokenReq>& qs, char* out, size_t n, size_t lo) {
+    std::vector<char*> b;
+    size_t off = 0;
+    for (const TokenReq& q : qs) { b.push_back(out + off + lo * q.item_bytes); off += n * q.item_bytes; }
+    return b;
+}
+
+// memcpy split over up to nt host threads
+void parallel_copy(char* dst, const char* src, size_t bytes, int nt) {
+    const size_t part = (bytes + nt - 1) / nt;
+    if (nt <= 1 || bytes < ((size_t)4 << 20)) { memcpy(dst, src, bytes); return; }
+    std::vector<std::thread> th;
+    for (size_t o = 0; o < bytes; o += part) th.emplace_back([=]() { memcpy(dst + o, src + o, std::min(part, bytes - o)); });
+    for (auto& t : th) t.join();
+}
+
+template <class T>
+bool ensure_buf(clip_ctx* c, T** buf, size_t* cap, size_t count);
+bool host_ptr_is_pinned(const void* p);
+
+// Host forms: rows leave the device through a two-slot ring (c->d_ring) instead of holding the launch stream on PCIe.  K7 fills slot
+// s on the launch stream; the copy stream takes it to the host once K7 is done (ev_ring_rows[s]), so the D2H of one stop runs under
+// the blocks of the next, and the tail into slot s first waits for that slot's previous D2H (ev_ring_free[s]).  A pinned `out`
+// receives the D2H directly.  A pageable one cannot take an async D2H, so the rows land in a pinned bounce slot (c->h_ring) that host
+// threads drain into `out` before that slot is copied into again (image_batch_encode_one's arena, the other way round).
+// Caller holds c->mu and has set the device.
+struct RowRing {
+    clip_ctx* c;
+    bool pinned = true;
+    size_t slot = 0;            // bytes per slot: one micro-batch of the widest entry
+    unsigned k = 0;             // stops so far; stop k uses slot k & 1
+    int nt = 1;
+    char* pend[2] = {nullptr, nullptr};
+    size_t pend_bytes[2] = {0, 0};
+
+    bool init(size_t slot_bytes, const void* out) {
+        slot = (slot_bytes + 255) / 256 * 256;
+        pinned = host_ptr_is_pinned(out);
+        nt = std::max(1, std::min(16, (int)std::thread::hardware_concurrency()));
+        if (!ensure_buf(c, &c->d_ring, &c->d_ring_cap, 2 * slot)) return false;
+        if (!pinned && c->h_ring_cap < 2 * slot) {
+            if (c->h_ring) { cudaFreeHost(c->h_ring); c->h_ring = nullptr; c->h_ring_cap = 0; }
+            CK(cudaMallocHost((void**)&c->h_ring, 2 * slot));
+            c->h_ring_cap = 2 * slot;
+        }
+        return true;
+    }
+    // rows of entry q for nb items -> dst (host)
+    bool put(Tower& tw, int nb, int T, const TokenReq& q, char* dst) {
+        const int s = (int)(k++ & 1);
+        char* d = c->d_ring + s * slot;
+        CK(cudaStreamWaitEvent(c->stream, c->ev_ring_free[s], 0));
+        if (!token_rows_tail(c, tw, nb, T, q, d)) return false;
+        CK(cudaEventRecord(c->ev_ring_rows[s], c->stream));
+        if (!drain(s)) return false;
+        const size_t bytes = (size_t)nb * q.item_bytes;
+        CK(cudaStreamWaitEvent(c->copy_stream, c->ev_ring_rows[s], 0));
+        CK(cudaMemcpyAsync(pinned ? dst : c->h_ring + s * slot, d, bytes, cudaMemcpyDeviceToHost, c->copy_stream));
+        CK(cudaEventRecord(c->ev_ring_free[s], c->copy_stream));
+        if (!pinned) { pend[s] = dst; pend_bytes[s] = bytes; }
+        return true;
+    }
+    // bounce slot s -> its destination, once its D2H has landed
+    bool drain(int s) {
+        if (!pend[s]) return true;
+        CK(cudaEventSynchronize(c->ev_ring_free[s]));
+        parallel_copy(pend[s], c->h_ring + s * slot, pend_bytes[s], nt);
+        pend[s] = nullptr;
+        return true;
+    }
+    // the launch stream waits for the last D2Hs, so the call's end event (and its synchronisation) covers them
+    bool close() {
+        for (int s = 0; s < 2; s++) CK(cudaStreamWaitEvent(c->stream, c->ev_ring_free[s], 0));
+        return true;
+    }
+    bool drain_all() { return drain((int)(k & 1)) && drain((int)((k + 1) & 1)); }     // the older slot first
+};
 
 void dev_free(clip_ctx* c, void* p) {
     if (!p) return;
@@ -593,6 +694,8 @@ static clip_ctx* load_on_device(const GgufFile& g, int device, const int verbosi
         for (int i = 0; i < 2; i++) {
             cudaEventCreateWithFlags(&c->ev_copied[i], cudaEventDisableTiming);
             cudaEventCreateWithFlags(&c->ev_consumed[i], cudaEventDisableTiming);
+            cudaEventCreateWithFlags(&c->ev_ring_rows[i], cudaEventDisableTiming);
+            cudaEventCreateWithFlags(&c->ev_ring_free[i], cudaEventDisableTiming);
         }
         cudaEventCreate(&c->ev_t0);
         cudaEventCreate(&c->ev_t1);
@@ -768,9 +871,11 @@ void clip_free(struct clip_ctx* c) {
     preprocess_release(c);
     for (void* p : c->allocs) cudaFree(p);
     for (int i = 0; i < 2; i++) if (c->h_stage[i]) cudaFreeHost(c->h_stage[i]);
+    if (c->h_ring) cudaFreeHost(c->h_ring);
     for (auto& p : c->prof) { cudaEventDestroy(p.e0); cudaEventDestroy(p.e1); }
     for (auto e : c->ev_pool) cudaEventDestroy(e);
     for (int i = 0; i < 2; i++) { if (c->ev_copied[i]) cudaEventDestroy(c->ev_copied[i]); if (c->ev_consumed[i]) cudaEventDestroy(c->ev_consumed[i]); }
+    for (int i = 0; i < 2; i++) { if (c->ev_ring_rows[i]) cudaEventDestroy(c->ev_ring_rows[i]); if (c->ev_ring_free[i]) cudaEventDestroy(c->ev_ring_free[i]); }
     for (int i = 0; i < 4; i++) if (c->marks[i]) cudaEventDestroy(c->marks[i]);
     if (c->ev_t0) cudaEventDestroy(c->ev_t0);
     if (c->ev_t1) cudaEventDestroy(c->ev_t1);
@@ -1153,10 +1258,10 @@ bool clip_b200_text_encode_device(const struct clip_ctx* cctx, const void* d_ids
 }
 
 // ---- per-token hidden states ----------------------------------------------------------------------------------------------------
-// One GPU, host buffers: each micro-batch's inputs go up on the launch stream, its rows come back straight into the caller's `out`
-// (a staging buffer of one micro-batch on the device; the whole output is never held there).
-static bool image_tokens_one(clip_ctx* c, const clip_image_f32* imgs, size_t n, const TokenReq& q, char* out, int H = 0, int W = 0,
-                             const char* who = "clip_b200_image_tokens") {
+// One GPU, host buffers: each micro-batch's inputs go up on the launch stream; the rows of every entry leave through the RowRing into
+// that entry's slab of the caller's buffer (bases[j] = item 0 of this call in slab j), so the whole output is never held on the device.
+static bool image_tokens_one(clip_ctx* c, const clip_image_f32* imgs, size_t n, const std::vector<TokenReq>& qs, const std::vector<char*>& bases,
+                             int H = 0, int W = 0, const char* who = "clip_b200_image_tokens") {
     Tower& tw = c->vis;
     std::lock_guard<std::mutex> lk(c->mu);
     CK(cudaSetDevice(c->device));
@@ -1165,22 +1270,27 @@ static bool image_tokens_one(clip_ctx* c, const clip_image_f32* imgs, size_t n, 
     if (!plan_call(c, H, W, v, mb, who)) return false;
     size_t n_chunks, chunk;
     chunking(n, mb, n_chunks, chunk);
-    if (!ensure_out(c, (chunk * q.item_bytes + 3) / 4)) return false;
+    size_t widest = 0;
+    for (const TokenReq& q : qs) widest = std::max(widest, q.item_bytes);
+    RowRing ring{c};
+    if (!ring.init(chunk * widest, bases[0])) return false;
     const size_t per = v.per();
     CK(cudaEventRecord(c->ev_t0, c->stream));
     for (size_t i0 = 0; i0 < n; i0 += chunk) {
         const int nb = (int)std::min(chunk, n - i0);
         for (int j = 0; j < nb; j++)
             CK(cudaMemcpyAsync(tw.ws.pixels[0] + (size_t)j * per, imgs[i0 + j].data, per * 4, cudaMemcpyHostToDevice, c->stream));
-        if (!vision_tokens(c, tw.ws.pixels[0], nb, v, q, c->d_out)) return false;
-        CK(cudaMemcpyAsync(out + i0 * q.item_bytes, c->d_out, nb * q.item_bytes, cudaMemcpyDeviceToHost, c->stream));
+        if (!vision_tokens(c, tw.ws.pixels[0], nb, v, qs, [&](int j) { return ring.put(tw, nb, v.T, qs[j], bases[j] + i0 * qs[j].item_bytes); }))
+            return false;
     }
+    if (!ring.close()) return false;
     CK(cudaEventRecord(c->ev_t1, c->stream));
-    return sync_and_time(c);
+    return sync_and_time(c) && ring.drain_all();
 }
 
-// n images of H x W (0 x 0: the model's size) resident at d_pixels -> rows at d_out
-static bool image_tokens_device_impl(clip_ctx* c, const float* d_pixels, size_t n, const TokenReq& q, char* d_out, int H, int W, const char* who) {
+// n images of H x W (0 x 0: the model's size) resident at d_pixels -> the slabs at bases (device)
+static bool image_tokens_device_impl(clip_ctx* c, const float* d_pixels, size_t n, const std::vector<TokenReq>& qs, const std::vector<char*>& bases,
+                                     int H, int W, const char* who) {
     std::lock_guard<std::mutex> lk(c->mu);
     CK(cudaSetDevice(c->device));
     VisCall v;
@@ -1192,10 +1302,41 @@ static bool image_tokens_device_impl(clip_ctx* c, const float* d_pixels, size_t 
     CK(cudaEventRecord(c->ev_t0, c->stream));
     for (size_t i0 = 0; i0 < n; i0 += chunk) {
         const int nb = (int)std::min(chunk, n - i0);
-        if (!vision_tokens(c, d_pixels + i0 * per, nb, v, q, d_out + i0 * q.item_bytes)) return false;
+        auto emit = [&](int j) { return token_rows_tail(c, c->vis, nb, v.T, qs[j], bases[j] + i0 * qs[j].item_bytes); };
+        if (!vision_tokens(c, d_pixels + i0 * per, nb, v, qs, emit)) return false;
     }
     CK(cudaEventRecord(c->ev_t1, c->stream));
     return sync_and_time(c);
+}
+
+// The entries of a multi-layer call, each checked and resolved by token_request as the single-layer call would be; the message of a
+// refused entry names its index.
+static bool token_requests(const clip_ctx* c, bool vision, const int* layers, const int* flags, int n_layers, int out_type, int T,
+                           std::vector<TokenReq>& qs, const char* who) {
+    if (!(vision ? c->vis : c->txt).present) { set_err(std::string(who) + ": this model has no " + (vision ? "vision" : "text") + " encoder"); return false; }
+    if (n_layers < 1 || n_layers > CLIP_B200_TOKENS_MAX_LAYERS) {
+        set_err(std::string(who) + ": n_layers must be in [1, " + std::to_string(CLIP_B200_TOKENS_MAX_LAYERS) + "], not " + std::to_string(n_layers));
+        return false;
+    }
+    if (!layers) { set_err(std::string(who) + ": null layers"); return false; }
+    qs.assign((size_t)n_layers, TokenReq());
+    for (int j = 0; j < n_layers; j++) {
+        const std::string w = std::string(who) + ": entry " + std::to_string(j);
+        if (!token_request(c, vision, layers[j], flags ? flags[j] : 0, out_type, T, qs[j], w.c_str())) return false;
+    }
+    return true;
+}
+
+// host image forms, one layer or several: shard over the GPUs in devices mode, each writing its items into every slab
+static bool image_tokens_host(clip_ctx* c, const clip_image_f32_batch* imgs, const std::vector<TokenReq>& qs, char* out, int H, int W, const char* who) {
+    const size_t n = imgs->size;
+    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
+        // devices mode: contiguous shards, every GPU copies its slice of the rows into the caller's buffer
+        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
+            return hi == lo || image_tokens_one(r, imgs->data + lo, hi - lo, qs, slab_bases(qs, out, n, lo), H, W, who);
+        });
+    }
+    return image_tokens_one(c, imgs->data, n, qs, slab_bases(qs, out, n, 0), H, W, who);
 }
 
 bool clip_b200_image_tokens(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, int layer, int flags, int out_type, void* out) {
@@ -1207,13 +1348,7 @@ bool clip_b200_image_tokens(const struct clip_ctx* cctx, const struct clip_image
     if (n == 0) return true;
     if (!out) { set_err("clip_b200_image_tokens: null output"); return false; }
     if (!check_images(c, imgs->data, n, "clip_b200_image_tokens")) return false;
-    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
-        // devices mode: contiguous shards, every GPU copies its slice of the rows into the caller's buffer
-        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
-            return hi == lo || image_tokens_one(r, imgs->data + lo, hi - lo, q, (char*)out + lo * q.item_bytes);
-        });
-    }
-    return image_tokens_one(c, imgs->data, n, q, (char*)out);
+    return image_tokens_host(c, imgs, {q}, (char*)out, 0, 0, "clip_b200_image_tokens");
 }
 
 bool clip_b200_image_tokens_device(const struct clip_ctx* cctx, const void* d_pixels, size_t n, int layer, int flags, int out_type, void* d_out) {
@@ -1223,7 +1358,7 @@ bool clip_b200_image_tokens_device(const struct clip_ctx* cctx, const void* d_pi
     if (!token_request(c, true, layer, flags, out_type, c->vis.T, q, "clip_b200_image_tokens_device")) return false;
     if (n == 0) return true;
     if (!d_pixels || !d_out) { set_err("clip_b200_image_tokens_device: null device pointer"); return false; }
-    return image_tokens_device_impl(c, (const float*)d_pixels, n, q, (char*)d_out, 0, 0, "clip_b200_image_tokens_device");
+    return image_tokens_device_impl(c, (const float*)d_pixels, n, {q}, {(char*)d_out}, 0, 0, "clip_b200_image_tokens_device");
 }
 
 bool clip_b200_image_tokens_hw(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, int layer, int flags, int out_type, void* out) {
@@ -1238,12 +1373,7 @@ bool clip_b200_image_tokens_hw(const struct clip_ctx* cctx, const struct clip_im
     int H = 0, W = 0;
     if (!check_images_hw(c, imgs->data, n, H, W, who)) return false;
     if (!token_request(c, true, layer, flags, out_type, (H / c->vis.patch) * (W / c->vis.patch) + 1, q, who)) return false;
-    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
-        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
-            return hi == lo || image_tokens_one(r, imgs->data + lo, hi - lo, q, (char*)out + lo * q.item_bytes, H, W, who);
-        });
-    }
-    return image_tokens_one(c, imgs->data, n, q, (char*)out, H, W, who);
+    return image_tokens_host(c, imgs, {q}, (char*)out, H, W, who);
 }
 
 bool clip_b200_image_tokens_device_hw(const struct clip_ctx* cctx, const void* d_pixels, size_t n, int height, int width, int layer, int flags,
@@ -1257,30 +1387,48 @@ bool clip_b200_image_tokens_device_hw(const struct clip_ctx* cctx, const void* d
     if (!token_request(c, true, layer, flags, out_type, (height / c->vis.patch) * (width / c->vis.patch) + 1, q, who)) return false;
     if (n == 0) return true;
     if (!d_pixels || !d_out) { set_err(std::string(who) + ": null device pointer"); return false; }
-    return image_tokens_device_impl(c, (const float*)d_pixels, n, q, (char*)d_out, height, width, who);
+    return image_tokens_device_impl(c, (const float*)d_pixels, n, {q}, {(char*)d_out}, height, width, who);
 }
 
-// n padded sequences of seq_len ids, on the host (h_ids) or the device (d_ids) -> rows at out (host) or d_out (device)
-static bool text_tokens_impl(clip_ctx* c, const int32_t* h_ids, const int32_t* d_ids, size_t n, int seq_len, const TokenReq& q, char* out,
-                             char* d_out) {
+// n padded sequences of seq_len ids, on the host (h_ids) or the device (d_ids) -> the slabs at bases, host memory (through the
+// RowRing) when `host_out`, else device memory
+static bool text_tokens_impl(clip_ctx* c, const int32_t* h_ids, const int32_t* d_ids, size_t n, int seq_len, const std::vector<TokenReq>& qs,
+                             const std::vector<char*>& bases, bool host_out) {
     Tower& tw = c->txt;
     std::lock_guard<std::mutex> lk(c->mu);
     CK(cudaSetDevice(c->device));
     if (!ensure_ws(c, tw, tw.micro_batch, tw.n_ctx, false)) return false;
     size_t n_chunks, chunk;
     chunking(n, tw.micro_batch, n_chunks, chunk);
-    if (!d_out && !ensure_out(c, (chunk * q.item_bytes + 3) / 4)) return false;
+    size_t widest = 0;
+    for (const TokenReq& q : qs) widest = std::max(widest, q.item_bytes);
+    RowRing ring{c};
+    if (host_out && !ring.init(chunk * widest, bases[0])) return false;
     CK(cudaEventRecord(c->ev_t0, c->stream));
     for (size_t i0 = 0; i0 < n; i0 += chunk) {
         const int nb = (int)std::min(chunk, n - i0);
         const size_t id_bytes = (size_t)nb * seq_len * 4;
         if (h_ids) CK(cudaMemcpyAsync(tw.ws.ids, h_ids + i0 * seq_len, id_bytes, cudaMemcpyHostToDevice, c->stream));
         else CK(cudaMemcpyAsync(tw.ws.ids, d_ids + i0 * seq_len, id_bytes, cudaMemcpyDeviceToDevice, c->stream));
-        if (!text_tokens(c, nb, seq_len, q, d_out ? d_out + i0 * q.item_bytes : (void*)c->d_out)) return false;
-        if (!d_out) CK(cudaMemcpyAsync(out + i0 * q.item_bytes, c->d_out, nb * q.item_bytes, cudaMemcpyDeviceToHost, c->stream));
+        auto emit = [&](int j) {
+            char* dst = bases[j] + i0 * qs[j].item_bytes;
+            return host_out ? ring.put(tw, nb, seq_len, qs[j], dst) : token_rows_tail(c, tw, nb, seq_len, qs[j], dst);
+        };
+        if (!text_tokens(c, nb, seq_len, qs, emit)) return false;
     }
+    if (host_out && !ring.close()) return false;
     CK(cudaEventRecord(c->ev_t1, c->stream));
-    return sync_and_time(c);
+    return sync_and_time(c) && ring.drain_all();
+}
+
+// host text forms, one layer or several: shard over the GPUs in devices mode, each writing its sequences into every slab
+static bool text_tokens_host(clip_ctx* c, const int32_t* ids, size_t n, int seq_len, const std::vector<TokenReq>& qs, char* out) {
+    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
+        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
+            return hi == lo || text_tokens_impl(r, ids + lo * seq_len, nullptr, hi - lo, seq_len, qs, slab_bases(qs, out, n, lo), true);
+        });
+    }
+    return text_tokens_impl(c, ids, nullptr, n, seq_len, qs, slab_bases(qs, out, n, 0), true);
 }
 
 bool clip_b200_text_tokens(const struct clip_ctx* cctx, const int32_t* ids, size_t n, int seq_len, int layer, int flags, int out_type, void* out) {
@@ -1291,12 +1439,7 @@ bool clip_b200_text_tokens(const struct clip_ctx* cctx, const int32_t* ids, size
     if (n == 0) return true;
     if (seq_len < 1 || seq_len > c->txt.n_ctx) { set_err("clip_b200_text_tokens: seq_len must be in [1, context_length]"); return false; }
     if (!ids || !out) { set_err("clip_b200_text_tokens: null pointer"); return false; }
-    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
-        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
-            return hi == lo || text_tokens_impl(r, ids + lo * seq_len, nullptr, hi - lo, seq_len, q, (char*)out + lo * q.item_bytes, nullptr);
-        });
-    }
-    return text_tokens_impl(c, ids, nullptr, n, seq_len, q, (char*)out, nullptr);
+    return text_tokens_host(c, ids, n, seq_len, {q}, (char*)out);
 }
 
 bool clip_b200_text_tokens_device(const struct clip_ctx* cctx, const void* d_ids, size_t n, int seq_len, int layer, int flags, int out_type,
@@ -1308,7 +1451,64 @@ bool clip_b200_text_tokens_device(const struct clip_ctx* cctx, const void* d_ids
     if (n == 0) return true;
     if (seq_len < 1 || seq_len > c->txt.n_ctx) { set_err("clip_b200_text_tokens_device: seq_len must be in [1, context_length]"); return false; }
     if (!d_ids || !d_out) { set_err("clip_b200_text_tokens_device: null device pointer"); return false; }
-    return text_tokens_impl(c, nullptr, (const int32_t*)d_ids, n, seq_len, q, nullptr, (char*)d_out);
+    return text_tokens_impl(c, nullptr, (const int32_t*)d_ids, n, seq_len, {q}, {(char*)d_out}, false);
+}
+
+// ---- several layers from one forward pass (clip_b200_*_tokens_layers) ------------------------------------------------------------
+bool clip_b200_image_tokens_layers(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, const int* layers, const int* flags,
+                                   int n_layers, int out_type, void* out) {
+    const char* who = "clip_b200_image_tokens_layers";
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    std::vector<TokenReq> qs;
+    if (!c) { set_err(std::string(who) + ": null context"); return false; }
+    const size_t n = imgs ? imgs->size : 0;
+    if (n == 0) return token_requests(c, true, layers, flags, n_layers, out_type, c->vis.T, qs, who);
+    if (!c->has_vision) { set_err(std::string(who) + ": this model has no vision encoder"); return false; }
+    if (!out) { set_err(std::string(who) + ": null output"); return false; }
+    int H = 0, W = 0;
+    if (!check_images_hw(c, imgs->data, n, H, W, who)) return false;
+    if (!token_requests(c, true, layers, flags, n_layers, out_type, (H / c->vis.patch) * (W / c->vis.patch) + 1, qs, who)) return false;
+    return image_tokens_host(c, imgs, qs, (char*)out, H, W, who);
+}
+
+bool clip_b200_image_tokens_layers_device(const struct clip_ctx* cctx, const void* d_pixels, size_t n, int height, int width, const int* layers,
+                                          const int* flags, int n_layers, int out_type, void* d_out) {
+    const char* who = "clip_b200_image_tokens_layers_device";
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    std::vector<TokenReq> qs;
+    if (!c) { set_err(std::string(who) + ": null context"); return false; }
+    if (!c->has_vision) { set_err(std::string(who) + ": this model has no vision encoder"); return false; }
+    if (!check_hw_size(c, height, width, who)) return false;
+    if (!token_requests(c, true, layers, flags, n_layers, out_type, (height / c->vis.patch) * (width / c->vis.patch) + 1, qs, who)) return false;
+    if (n == 0) return true;
+    if (!d_pixels || !d_out) { set_err(std::string(who) + ": null device pointer"); return false; }
+    return image_tokens_device_impl(c, (const float*)d_pixels, n, qs, slab_bases(qs, (char*)d_out, n, 0), height, width, who);
+}
+
+bool clip_b200_text_tokens_layers(const struct clip_ctx* cctx, const int32_t* ids, size_t n, int seq_len, const int* layers, const int* flags,
+                                  int n_layers, int out_type, void* out) {
+    const char* who = "clip_b200_text_tokens_layers";
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    std::vector<TokenReq> qs;
+    if (!c) { set_err(std::string(who) + ": null context"); return false; }
+    if (!token_requests(c, false, layers, flags, n_layers, out_type, seq_len, qs, who)) return false;
+    if (n == 0) return true;
+    if (seq_len < 1 || seq_len > c->txt.n_ctx) { set_err(std::string(who) + ": seq_len must be in [1, context_length]"); return false; }
+    if (!ids || !out) { set_err(std::string(who) + ": null pointer"); return false; }
+    return text_tokens_host(c, ids, n, seq_len, qs, (char*)out);
+}
+
+bool clip_b200_text_tokens_layers_device(const struct clip_ctx* cctx, const void* d_ids, size_t n, int seq_len, const int* layers, const int* flags,
+                                         int n_layers, int out_type, void* d_out) {
+    const char* who = "clip_b200_text_tokens_layers_device";
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    std::vector<TokenReq> qs;
+    if (!c) { set_err(std::string(who) + ": null context"); return false; }
+    if (!token_requests(c, false, layers, flags, n_layers, out_type, seq_len, qs, who)) return false;
+    if (n == 0) return true;
+    if (seq_len < 1 || seq_len > c->txt.n_ctx) { set_err(std::string(who) + ": seq_len must be in [1, context_length]"); return false; }
+    if (!d_ids || !d_out) { set_err(std::string(who) + ": null device pointer"); return false; }
+    return text_tokens_impl(c, nullptr, (const int32_t*)d_ids, n, seq_len, qs, slab_bases(qs, (char*)d_out, n, 0), false);
 }
 
 float clip_similarity_score(const float* vec1, const float* vec2, const int vec_dim) {

@@ -103,6 +103,11 @@ struct clip_ctx {
     // H2D per micro-batch -- pageable cudaMemcpyAsync would be staged synchronously by the driver, image by image
     float* h_stage[2] = {nullptr, nullptr};
     size_t h_stage_cap = 0;                 // floats per buffer
+    // host *_tokens calls: the two-slot ring their rows leave the device through (RowRing in api.cu), grow-only; h_ring is the
+    // pinned bounce for pageable caller buffers.  ev_ring_rows[s]: K7 has filled slot s; ev_ring_free[s]: its D2H has finished.
+    char* d_ring = nullptr; size_t d_ring_cap = 0;
+    char* h_ring = nullptr; size_t h_ring_cap = 0;
+    cudaEvent_t ev_ring_rows[2] = {nullptr, nullptr}, ev_ring_free[2] = {nullptr, nullptr};
     // scoring scratch (search.cu), grow-only
     float* d_logits = nullptr; size_t d_logits_cap = 0;
     float* d_cand_v[2] = {nullptr, nullptr}; int* d_cand_i[2] = {nullptr, nullptr}; size_t d_cand_cap = 0;

@@ -228,6 +228,33 @@ bool clip_b200_image_batch_encode_hw(const struct clip_ctx * ctx, const struct c
 bool clip_b200_image_tokens_hw(const struct clip_ctx * ctx, const struct clip_image_f32_batch * imgs, int layer, int flags,
                                int out_type, void * out);
 
+/* Several layers' token rows from ONE forward pass of a tower (HF output_hidden_states returns all n_layer + 1; multi-layer VLM
+ * connectors read 3 or 4 vision layers; SDXL reads layer -2 raw and the projected EOT row of layer -1 of the same text pass).
+ *   layers[j], flags[j]  entry j: a layer and CLIP_B200_TOKENS_* flags exactly as `layer` / `flags` of the single-layer calls above.
+ *            Any order, duplicates allowed.  flags == NULL: 0 for every entry.  Only blocks 0 .. deepest - 1 run, each once.
+ *   n_layers 1 .. CLIP_B200_TOKENS_MAX_LAYERS;  out_type applies to every entry.
+ *   out      layer-major: entry j is one slab of n * item_bytes_j bytes at offset n * (item_bytes_0 + ... + item_bytes_{j-1}), laid
+ *            out as the single-layer call lays out its whole output (item_bytes_j = rows x width x element size of that entry).
+ * Slab j equals, byte for byte, the single-layer call with (layers[j], flags[j], out_type) on the same inputs: the same kernels run
+ * on the same residual stream.  Image size: the host form takes it from the images, as clip_b200_image_tokens_hw does (at
+ * image_size x image_size that is the native path); the device form takes height x width (image_size x image_size: native).  Every
+ * *_hw rule applies.  Refused with a message in clip_b200_last_error(): n_layers outside [1, CLIP_B200_TOKENS_MAX_LAYERS], NULL
+ * layers or output, any entry the single-layer call would refuse (the message names the entry's index), a bad image size or mixed
+ * sizes in one host call, a model without the tower.  n == 0 returns true.
+ * Host forms: rows leave the device through a two-slot staging ring on a copy stream, so one layer's device-to-host copy runs under
+ * the next layer's blocks; a pinned `out` (clip_b200_host_malloc) receives them directly, a pageable one through a pinned bounce
+ * buffer (two micro-batches of the widest entry, grow-only).  Devices mode (CLIP_B200_DEVICES) shards the items as the single-layer
+ * host forms do, each GPU writing its items into every slab.  Device forms: pointers on the context's GPU, d_out 16-byte aligned. */
+#define CLIP_B200_TOKENS_MAX_LAYERS 4096
+bool clip_b200_image_tokens_layers(const struct clip_ctx * ctx, const struct clip_image_f32_batch * imgs,
+                                   const int * layers, const int * flags, int n_layers, int out_type, void * out);
+bool clip_b200_image_tokens_layers_device(const struct clip_ctx * ctx, const void * d_pixels, size_t n, int height, int width,
+                                          const int * layers, const int * flags, int n_layers, int out_type, void * d_out);
+bool clip_b200_text_tokens_layers(const struct clip_ctx * ctx, const int32_t * ids, size_t n, int seq_len,
+                                  const int * layers, const int * flags, int n_layers, int out_type, void * out);
+bool clip_b200_text_tokens_layers_device(const struct clip_ctx * ctx, const void * d_ids, size_t n, int seq_len,
+                                         const int * layers, const int * flags, int n_layers, int out_type, void * d_out);
+
 /* Batched zero-shot scoring on the device (clip.cpp:1624-1659 semantics per image): d_img_vec [n_img, d], d_txt_vec [n_txt, d]
  * -> host scores/indices [n_img, top_k], best first; similarity matrix, softmax and top-k selection all run on the GPU.
  * Ranking (here and in clip_b200_topk_search): top_k <= 0 or top_k > n_txt means all n_txt, and row i of the output starts at
