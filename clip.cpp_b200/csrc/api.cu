@@ -3,6 +3,7 @@
 // one stream.  There is NO CPU path -- if CUDA is unavailable clip_model_load fails loudly.
 #include <chrono>
 #include <float.h>
+#include <limits.h>
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -235,8 +236,18 @@ bool ensure_ws(clip_ctx* c, Tower& tw, int items, int T, bool vision) {
     if (w.cap_items >= items && w.T == T) return true;
     if (w.cap_items) { set_err("workspace re-sizing is not supported after the first encode"); return false; }
     const int h = tw.hidden;
-    w.cap_items = items; w.T = T; w.cap_rows = items * T;
-    const size_t rows = (size_t)w.cap_rows;
+    // Row counts are ints, and every GEMM of a pass addresses its output (and the patch GEMM its input) with 32-bit element offsets
+    // (gemm_launch): refuse a micro_batch past either limit here, before anything is allocated, so the context stays usable.
+    const size_t rows = (size_t)items * (size_t)T;
+    const size_t widest = std::max({(size_t)3 * h, (size_t)tw.ff, (size_t)tw.proj, vision ? (size_t)tw.kpad : (size_t)0});
+    if (rows > (size_t)INT_MAX || rows * widest >= ((size_t)1 << 32)) {
+        const size_t limit = std::min((size_t)INT_MAX / T, (((size_t)1 << 32) - 1) / (widest * T));
+        set_err(std::string(vision ? "vision" : "text") + " micro_batch " + std::to_string(items) + " is too large: " + std::to_string(rows) +
+                " rows of " + std::to_string(T) + " per " + (vision ? "image" : "sequence") + " x " + std::to_string(widest) +
+                " columns exceed 32-bit offsets; the limit is " + std::to_string(limit) + " (clip_b200_set_micro_batch)");
+        return false;
+    }
+    w.cap_items = items; w.T = T; w.cap_rows = (int)rows;
     if (!dev_alloc(c, &w.x, rows * h) || !dev_alloc(c, &w.a, rows * h) || !dev_alloc(c, &w.qkv, rows * 3 * h) ||
         !dev_alloc(c, &w.g, rows * tw.ff) || !dev_alloc(c, &w.sel16, (size_t)items * h) || !dev_alloc(c, &w.sel32, (size_t)items * h) ||
         !dev_alloc(c, &w.proj32, (size_t)items * tw.proj)) return false;

@@ -321,7 +321,11 @@ bool   clip_b200_synchronize(const struct clip_ctx * ctx);
 void * clip_b200_get_stream(const struct clip_ctx * ctx);          /* the cudaStream_t every kernel is launched on */
 
 /* images (vision) / sequences (text) processed per pass through the layer stack; 0 keeps the current value.  Workspaces are sized
- * once, at the first encode of a tower: a call after that is ignored for that tower. */
+ * once, at the first encode of a tower: a call after that is ignored for that tower.  A pass must fit 32-bit element offsets:
+ * micro_batch x T rows (T = the native token count, or context_length for text) times the widest activation of the tower (3 x
+ * hidden, ff, projection_dim, and for vision the padded patch width) must stay below 2^32, e.g. at most 4 080 ViT-L/14 images.
+ * A larger value is accepted here but the first encode of that tower is refused with a message naming micro_batch and the limit,
+ * before anything is allocated; a smaller value set after that refusal takes effect. */
 void   clip_b200_set_micro_batch(const struct clip_ctx * ctx, int images, int sequences);
 
 /* measurement hooks */

@@ -12,9 +12,9 @@ pytestmark = pytest.mark.gpu
 
 H = 3          # odd: with an odd number of groups per head, every other warpgroup pair straddles two heads
 SMS = 132
-# T (64-row groups per head: 1 1 1 1 1 1 2 2 2 3 3 4 5 5 10), causal
+# T (64-row groups per head: 1 1 1 1 1 1 2 2 2 3 3 4 5 5 10 17 4 16 33), causal
 CASES = [(1, 0), (16, 0), (17, 0), (50, 0), (63, 0), (64, 0), (65, 0), (77, 1), (128, 0), (129, 0), (192, 0), (256, 0), (257, 0),
-         (320, 0), (577, 0)]
+         (320, 0), (577, 0), (1025, 0), (248, 1), (1000, 1), (2049, 1)]
 # groups in the launch against 2 x 132 (one pair per SM): below, about at, several times above
 GROUPS = {"below": 40, "at": 2 * SMS, "above": 8 * SMS}
 
