@@ -2015,6 +2015,8 @@ int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int e
     void *d_x = nullptr, *d_w = nullptr, *d_raw = nullptr, *d_out = nullptr;
     float* d_bias = nullptr;
     const size_t out_bytes = (size_t)M * N * (out32 ? 4 : 2);
+    // one token tile of guard rows past row M, filled with 0xFF: the GEMM must leave them untouched
+    const size_t guard_bytes = (size_t)GEMM_BN * N * (out32 ? 4 : 2);
     int rc = 0;
     cudaStream_t st = nullptr;
     cudaEvent_t e0, e1;
@@ -2023,7 +2025,8 @@ int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int e
     cudaError_t e;
     do {
         if ((e = cudaMalloc(&d_x, x16.size() * 2)) != cudaSuccess) { fail("malloc x", e); break; }
-        if ((e = cudaMalloc(&d_out, out_bytes)) != cudaSuccess) { fail("malloc out", e); break; }
+        if ((e = cudaMalloc(&d_out, out_bytes + guard_bytes)) != cudaSuccess) { fail("malloc out", e); break; }
+        cudaMemset((uint8_t*)d_out + out_bytes, 0xFF, guard_bytes);
         if ((e = cudaMalloc(&d_raw, raw_bytes)) != cudaSuccess) { fail("malloc raw", e); break; }
         cudaMemcpy(d_x, x16.data(), x16.size() * 2, cudaMemcpyHostToDevice);
         cudaMemcpy(d_raw, eff_q == QT_F16 ? (const void*)wf16.data() : w_rows, raw_bytes, cudaMemcpyHostToDevice);
@@ -2051,6 +2054,9 @@ int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int e
         if (e != cudaSuccess) { fail("launch", e); break; }
         if ((e = cudaStreamSynchronize(st)) != cudaSuccess) { fail("kernel", e); break; }
         if (ms) cudaEventElapsedTime(ms, e0, e1);
+        std::vector<uint8_t> guard(guard_bytes);
+        cudaMemcpy(guard.data(), (uint8_t*)d_out + out_bytes, guard_bytes, cudaMemcpyDeviceToHost);
+        if (std::any_of(guard.begin(), guard.end(), [](uint8_t b) { return b != 0xFF; })) { set_err("GEMM wrote past row M"); rc = 5; break; }
         if (out32) cudaMemcpy(y_out, d_out, out_bytes, cudaMemcpyDeviceToHost);
         else {
             std::vector<uint16_t> o16((size_t)M * N);

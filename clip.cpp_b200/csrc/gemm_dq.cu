@@ -15,9 +15,10 @@
 //               shared memory: every lane dequantises exactly the 16-bit pairs of its own wgmma A fragments (2 rows x 16 k per k-block)
 //               from the packed chunk into registers, and the group issues 4 register-A wgmma m64n192k16 per k-block (B = activation
 //               tile from shared memory), keeping one k-block of MMAs in flight while it unpacks the next.  f16 weights: both operands
-//               from shared memory.  Epilogue straight from the accumulator registers: bias / scale / GELU and 16-bit or fp32 stores,
-//               or x += acc + bias into the fp32 residual stream (every element has exactly one owner thread: deterministic), its x
-//               values read in four batches of independent loads (epilogue_regs).
+//               from shared memory.  Epilogue: bias / scale / GELU computed from the accumulator registers, written in chunks into a
+//               ring of swizzled staging slots in shared memory and sent out by bulk tensor stores that drain while the group runs
+//               the next tile's main loop; x += acc + bias into the fp32 residual stream adds to x that TMA brought into the slot
+//               (every element has exactly one owner thread: deterministic).  See epilogue_staged.
 // Bytes per launch (DESIGN.md section 5): packed W once per token tile, X once per feature tile, Y once; FLOPs = 2*M*N*K.
 #include <cuda.h>
 #include <stdlib.h>
@@ -40,28 +41,34 @@ static_assert(X_STAGE % 1024 == 0 && W_STAGE % 1024 == 0, "swizzled stage alignm
 __host__ __device__ constexpr uint32_t chunk_bytes(int qt) {
     return qt == 2 ? 4608u : qt == 3 ? 5120u : qt == 6 ? 5632u : qt == 7 ? 6144u : qt == 8 ? 8704u : 0u;
 }
-// shared-memory plan per weight type (fits the 227 KB carve-out): X ring, packed-weight ring, barriers
+constexpr uint32_t E_SLOT = 4096;   // one epilogue staging slot (epilogue_staged)
+// shared-memory plan per weight type (fits the 227 KB carve-out): X ring, packed-weight ring, epilogue staging (SE slots per consumer
+// group, as many as the rings leave room for), barriers.  q8_0's Q ring is one chunk shallower than the others' to make room for two
+// slots per group: the producer issues Q(kb) just before it waits for X(kb)'s stage, and the consumers release a Q chunk a k-block
+// before its X stage, so with 6 X stages no more than 7 Q chunks are ever in use.
 template <int QT>
 struct Cfg {
     static constexpr bool DQ = (QT != QT_F16);
     static constexpr uint32_t CHUNK = chunk_bytes(QT);
     static constexpr int SX = DQ ? 6 : 5;                              // X ring (f16: X + W per stage)
-    static constexpr int SQ = DQ ? 8 : 0;                              // packed-weight ring
+    static constexpr int SQ = !DQ ? 0 : QT == QT_Q8_0 ? 7 : 8;         // packed-weight ring
+    static constexpr int SE = !DQ ? 3 : QT == QT_Q8_0 ? 2 : (QT == QT_Q4_0 || QT == QT_Q4_1) ? 5 : 4;
     static constexpr uint32_t XS = DQ ? (uint32_t)X_STAGE : (uint32_t)(X_STAGE + W_STAGE);
     static constexpr uint32_t Q_OFF = SX * XS;
-    static constexpr uint32_t BAR_OFF = (Q_OFF + SQ * CHUNK + 127) / 128 * 128;
-    static constexpr uint32_t SMEM = BAR_OFF + 256 /*barriers*/ + 1024 /*align slack*/;
+    static constexpr uint32_t E_OFF = (Q_OFF + SQ * CHUNK + 1023) / 1024 * 1024;   // swizzled slots: 1024-byte aligned
+    static constexpr uint32_t BAR_OFF = E_OFF + 2 * SE * E_SLOT;
+    static constexpr uint32_t SMEM = BAR_OFF + 512 /*barriers*/ + 1024 /*align slack*/;
     static_assert(SMEM <= 232448, "shared memory plan exceeds 227 KB");
-    static_assert(16 * SX + 16 * SQ <= 256, "barrier area");
+    static_assert(16 * SX + 16 * SQ + 16 * SE <= 512, "barrier area");
 };
 
 struct KParams {
     CUtensorMap tm_x;
     CUtensorMap tm_w;
+    CUtensorMap tm_out;   // Y [M, N]: exactly M rows, so bulk stores clip a ragged last tile; boxes of one staging chunk
     const uint8_t* w_packed;
     const float* bias;
-    void* out;
-    int M, N, K, ldo;
+    int M, N, K;
     int epi, scale_cols;
     float scale;
 };
@@ -202,64 +209,138 @@ CB_DEVINL float epi_value(float acc, float bias, float mul) {
     } else return (acc + bias) * mul;
 }
 
-// Global accesses of the epilogue, predicated on `ok` (token rows past M) inside one asm: no branch per element.  All are volatile, so
-// they reach ptxas in source order: the residual loads of a batch are issued before any of its stores.
-CB_DEVINL float ldg_f32_if(const float* a, bool ok) {
-    float v = 0.f;
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p ld.global.f32 %0, [%1];\n\t}" : "+f"(v) : "l"(a), "r"((int)ok));
-    return v;
+// ---- epilogue staging: bulk tensor stores (and, for the residual add, loads) between the staging slots and the output matrix
+CB_DEVINL void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+CB_DEVINL void group_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }   // the 128 threads of one group
+CB_DEVINL void tma_store_2d(const void* tmap, uint32_t src_smem, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(tmap)),
+                 "r"(src_smem), "r"(c0), "r"(c1)
+                 : "memory");
 }
-CB_DEVINL void stg_f32_if(float* a, float v, bool ok) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.global.f32 [%0], %1;\n\t}" ::"l"(a), "f"(v), "r"((int)ok));
+CB_DEVINL void tma_prefetch_l2(const void* tmap, int c0, int c1) {
+    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1)
+                 : "memory");
 }
-CB_DEVINL void stg_u16_if(uint16_t* a, uint16_t v, bool ok) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %2, 0;\n\t@p st.global.u16 [%0], %1;\n\t}" ::"l"(a), "h"(v), "r"((int)ok));
+CB_DEVINL void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+CB_DEVINL void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }   // sources reusable
+CB_DEVINL void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }                // writes complete
+CB_DEVINL float lds_f32(uint32_t a) { float v; asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a)); return v; }
+CB_DEVINL void sts_f32(uint32_t a, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); }
+// four 8x8 16-bit matrices from accumulator-layout fragments, each stored transposed: row i of matrix m (address of lane 8m + i)
+// receives column i of the fragment, i.e. 8 features of one token
+CB_DEVINL void stmatrix_x4_trans(uint32_t a, const uint32_t (&r)[4]) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(r[0]), "r"(r[1]), "r"(r[2]),
+                 "r"(r[3])
+                 : "memory");
 }
 
-// Epilogue of one consumer group's [64 features x 192 tokens] accumulator (fragment layout: wgmma.cuh).  This thread owns features
-// f and f + 8 and tokens 8j + tc + {0, 1}; element offsets are 32-bit (host checks M*ldo < 2^32).
-// The residual add x += acc + bias reads its 96 x values in four batches of 24, each batch loaded completely before the first of its
-// stores: four memory round trips per tile instead of a chain of 96 dependent ones (with loads and stores through one pointer the
-// compiler cannot prove them disjoint, so written as x[o] += v it keeps every load behind the previous store).
-template <int EPI, bool BF>
-CB_DEVINL void epilogue_regs(void* out, int M, int ldo_, float (&acc)[BN / 2], int tok0, int f, int tc, const float (&bias)[2],
-                             const float (&mul)[2]) {
-    const int nt = min(BN, M - tok0) - tc;     // this thread's token 8j + tc + e1 is in range iff 8j + e1 < nt
-    const uint32_t ldo = (uint32_t)ldo_;
-    const uint32_t o0 = (uint32_t)(tok0 + tc) * ldo + (uint32_t)f;
-    auto off = [&](int j, int e) { return o0 + (uint32_t)(8 * j + (e & 1)) * ldo + 8u * (uint32_t)(e >> 1); };
-    if constexpr (EPI == EPI_REDADD32) {
-        float* x = reinterpret_cast<float*>(out);
-        constexpr int JB = 6;                  // 6 token groups = 24 elements per batch: the most that fits 168 registers without spills
-        #pragma unroll
-        for (int b = 0; b < BN / 8 / JB; b++) {
-            float r[4 * JB];
+// Output rectangle of one consumer group: [192 tokens x 64 features] of Y, staged through a ring of SE slots of E_SLOT bytes in
+// shared memory, laid out [token][feature] with the 128-byte swizzle of the output tensor map (rows of 128 B, 16-byte piece p of row
+// r at p ^ (r & 7)).  A chunk fills one slot: 32 tokens x 64 features of 16-bit values (one box), or 16 tokens x 64 features of fp32
+// (two boxes of 32 features).  Chunks past the last token are skipped; the map's M rows clip the rest of a ragged tile.
+constexpr int TC16 = E_SLOT / 128, TC32 = E_SLOT / 256;   // tokens per chunk
+template <int EPI>
+struct EpiShape {
+    static constexpr bool F32 = (EPI == EPI_STORE32 || EPI == EPI_REDADD32);
+    static constexpr int TC = F32 ? TC32 : TC16;
+    static constexpr int CH = BN / TC;                     // chunks per tile
+};
+CB_DEVINL int epi_chunks(int m_left, int tc) { return min(BN / tc, (m_left + tc - 1) / tc); }
+
+// x of the residual add: the leader thread loads chunk n of the tile (sequence number e) into its slot
+template <int SE>
+CB_DEVINL void load_x_chunk(const KParams& p, uint32_t ring, uint32_t full, uint32_t e, int tok0, int f0, int n) {
+    const uint32_t s = e % SE, dst = ring + s * E_SLOT;
+    mbar_arrive_expect_tx(full + 8 * s, E_SLOT);          // rows past M are zero-filled and still counted
+    tma_load_2d(dst, &p.tm_out, f0, tok0 + n * TC32, full + 8 * s);
+    tma_load_2d(dst + E_SLOT / 2, &p.tm_out, f0 + 32, tok0 + n * TC32, full + 8 * s);
+}
+// Residual add, from the middle of a tile's main loop: the leader loads the tile's first SE chunks of x into the group's slots (the
+// previous tile's stores read them long ago) and has L2 fetch the others, which the epilogue then loads from L2.
+template <int SE>
+CB_DEVINL void prefetch_x(const KParams& p, uint32_t ring, uint32_t full, uint32_t e, int tok0, int f0) {
+    const int nch = epi_chunks(p.M - tok0, TC32);
+    bulk_wait_read<0>();
+    for (int n = 0; n < nch; n++) {
+        if (n < SE) {
+            load_x_chunk<SE>(p, ring, full, e + n, tok0, f0, n);
+        } else {
+            tma_prefetch_l2(&p.tm_out, f0, tok0 + n * TC32);
+            tma_prefetch_l2(&p.tm_out, f0 + 32, tok0 + n * TC32);
+        }
+    }
+}
+
+// Epilogue of one consumer group's [64 features x 192 tokens] accumulator (fragment layout: wgmma.cuh): this thread (warp w of the
+// group) owns features 16w + lane/4 (+ 8) and tokens 8j + 2 (lane % 4) + {0, 1}.  Per chunk: the values go into the slot, every
+// thread fences them to the async proxy, the group syncs and its leader thread issues the bulk store; nobody waits for the store.
+// A slot is written again only after the store that read it is past its source (the leader's wait_group.read before the group
+// barrier).  Residual add: the slot already holds the chunk's x (load_x_chunk: the first SE chunks during the main loop, chunk n + SE
+// once the store of chunk n has read the slot); x + (acc + bias) is written back in place.  `e` numbers this group's chunks.
+template <int EPI, bool BF, int SE>
+CB_DEVINL void epilogue_staged(const KParams& p, const float (&acc)[BN / 2], int tok0, int f0, int w, int lane, const float (&bias)[2],
+                               const float (&mul)[2], uint32_t ring, uint32_t full, uint32_t& e, bool leader, int bar_id) {
+    using S = EpiShape<EPI>;
+    static_assert(SE >= 2, "a staging ring needs two slots");
+    const int nch = epi_chunks(p.M - tok0, S::TC);
+    #pragma unroll
+    for (int c = 0; c < S::CH; c++) {
+        if (c >= nch) break;
+        const uint32_t slot = ring + (e % SE) * E_SLOT;
+        if constexpr (!S::F32) {
+            const int m = lane >> 3, rr = lane & 7;
             #pragma unroll
-            for (int jj = 0; jj < JB; jj++) {
+            for (int jp = 0; jp < TC16 / 16; jp++) {
+                const int j = c * (TC16 / 8) + 2 * jp;     // token groups j and j + 1: matrices (j, f), (j, f + 8), (j + 1, f), (j + 1, f + 8)
+                uint32_t r[4];
                 #pragma unroll
-                for (int e = 0; e < 4; e++) r[4 * jj + e] = ldg_f32_if(x + off(b * JB + jj, e), 8 * (b * JB + jj) + (e & 1) < nt);
+                for (int q = 0; q < 4; q++) {
+                    const int i = 4 * (j + (q >> 1)) + 2 * (q & 1), h = q & 1;
+                    r[q] = (uint32_t)P2<BF>::from_float(epi_value<EPI>(acc[i], bias[h], mul[h])) |
+                           ((uint32_t)P2<BF>::from_float(epi_value<EPI>(acc[i + 1], bias[h], mul[h])) << 16);
+                }
+                const uint32_t row = 16 * jp + 8 * (m >> 1) + rr;
+                stmatrix_x4_trans(slot + row * 128 + ((uint32_t)((2 * w + (m & 1)) ^ rr) << 4), r);
             }
+        } else {
+            if constexpr (EPI == EPI_REDADD32) mbar_wait(full + 8 * (e % SE), (e / SE) & 1);
             #pragma unroll
-            for (int jj = 0; jj < JB; jj++) {
+            for (int jj = 0; jj < TC32 / 8; jj++) {
                 #pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    const int j = b * JB + jj;
-                    stg_f32_if(x + off(j, e), r[4 * jj + e] + (acc[4 * j + e] + bias[e >> 1]), 8 * j + (e & 1) < nt);
+                for (int q = 0; q < 4; q++) {
+                    const uint32_t row = 8 * jj + 2 * (lane & 3) + (q & 1);
+                    const uint32_t piece = 4 * (w & 1) + 2 * (q >> 1) + (lane >> 4);
+                    const uint32_t a = slot + (w >> 1) * (E_SLOT / 2) + row * 128 + ((piece ^ (row & 7)) << 4) + 4 * ((lane >> 2) & 3);
+                    const float v = acc[4 * (c * (TC32 / 8) + jj) + q] + bias[q >> 1];
+                    if constexpr (EPI == EPI_REDADD32) sts_f32(a, lds_f32(a) + v);
+                    else sts_f32(a, v);
                 }
             }
         }
-    } else {
-        #pragma unroll
-        for (int j = 0; j < BN / 8; j++) {
-            #pragma unroll
-            for (int e = 0; e < 4; e++) {
-                const int h = e >> 1;
-                const bool ok = 8 * j + (e & 1) < nt;
-                const float a = acc[4 * j + e];
-                if constexpr (EPI == EPI_STORE32) stg_f32_if(reinterpret_cast<float*>(out) + off(j, e), a + bias[h], ok);
-                else stg_u16_if(reinterpret_cast<uint16_t*>(out) + off(j, e), P2<BF>::from_float(epi_value<EPI>(a, bias[h], mul[h])), ok);
+        fence_proxy_async();
+        if constexpr (EPI != EPI_REDADD32) {
+            if (leader) bulk_wait_read<SE - 2>();          // the store of chunk e + 1 - SE has read the slot chunk e + 1 will write
+        }
+        group_bar(bar_id);
+        if (leader) {
+            const int row = tok0 + c * S::TC;
+            if constexpr (S::F32) {
+                tma_store_2d(&p.tm_out, slot, f0, row);
+                tma_store_2d(&p.tm_out, slot + E_SLOT / 2, f0 + 32, row);
+            } else {
+                tma_store_2d(&p.tm_out, slot, f0, row);
+            }
+            bulk_commit();
+            if constexpr (EPI == EPI_REDADD32) {
+                if (c >= 1 && c - 1 + SE < nch) {              // the slot of chunk c - 1 is free once its store has read it
+                    bulk_wait_read<1>();
+                    load_x_chunk<SE>(p, ring, full, e - 1 + SE, tok0, f0, c - 1 + SE);
+                }
             }
         }
+        __syncwarp();
+        e++;
     }
 }
 
@@ -267,23 +348,26 @@ template <int QT, bool BF>
 __global__ void __launch_bounds__(THREADS, 1) gemm_dq_kernel(const __grid_constant__ KParams p) {
     using C = Cfg<QT>;
     constexpr bool DQ = C::DQ;
-    constexpr int SX = C::SX, SQ = DQ ? C::SQ : 1;
+    constexpr int SX = C::SX, SQ = DQ ? C::SQ : 1, SE = C::SE;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     const uint32_t smem_base = smem_u32(smem);
     const uint32_t bars = smem_base + C::BAR_OFF;
-    // barrier slots (8 B each)
-    const uint32_t x_full = bars, x_empty = x_full + 8 * SX, q_full = x_empty + 8 * SX, q_empty = q_full + 8 * SQ;
+    // barrier slots (8 B each); e_full: x of the residual add arrived in a staging slot (SE per consumer group)
+    const uint32_t x_full = bars, x_empty = x_full + 8 * SX, q_full = x_empty + 8 * SX, q_empty = q_full + 8 * SQ,
+                   e_full = q_empty + 8 * SQ;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < SX; i++) { mbar_init(x_full + 8 * i, 1); mbar_init(x_empty + 8 * i, 8); }   // released by each consumer warp
         for (int i = 0; i < SQ; i++) { mbar_init(q_full + 8 * i, 1); mbar_init(q_empty + 8 * i, 8); }
+        for (int i = 0; i < 2 * SE; i++) mbar_init(e_full + 8 * i, 1);
         mbar_fence_init();
         tma_prefetch_desc(&p.tm_x);
         if (!DQ) tma_prefetch_desc(&p.tm_w);
+        tma_prefetch_desc(&p.tm_out);
     }
     __syncthreads();
     pdl_trigger();      // the next kernel of the stream may start placing CTAs as ours retire ...
@@ -320,12 +404,15 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_dq_kernel(const __grid_consta
     // ---------------------------------------------------------------------- consumers
     setmaxnreg_inc<232>();
     const int wg = warp >> 2;
-    const int fr = (warp & 3) * 16 + (lane >> 2), tc = 2 * (lane & 3);   // accumulator row (feature in the group) and token column
-    uint32_t s = 0, ph = 0, qs = 0, qph = 0;
+    const int fr = (warp & 3) * 16 + (lane >> 2);   // accumulator row (feature in the group)
+    const bool leader = (threadIdx.x & 127) == 0;   // issues this group's bulk stores and residual loads
+    const uint32_t ring = smem_base + C::E_OFF + (uint32_t)wg * SE * E_SLOT, ring_full = e_full + 8 * SE * wg;
+    uint32_t s = 0, ph = 0, qs = 0, qph = 0, e = 0;
     float acc[BN / 2];
     uint32_t afr0[16], afr1[16];      // A fragments of two consecutive k-blocks: one is read by in-flight MMAs while the next is unpacked
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int ft = tile % n_ft, tt = tile / n_ft;
+        const int tok0 = tt * BN, f0 = ft * BM + wg * 64;
         uint32_t prev = 0;
         auto kblock = [&](uint32_t (&a)[16], uint32_t (&other)[16], int kb) {
             if constexpr (DQ) {
@@ -355,6 +442,10 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_dq_kernel(const __grid_consta
             if (kb > 0) { __syncwarp(); if (lane == 0) mbar_arrive(x_empty + 8 * prev); }
             prev = s;
             if (++s == SX) { s = 0; ph ^= 1; }
+            if (p.epi == EPI_REDADD32 && kb == nkb / 2) {
+                if (leader) prefetch_x<SE>(p, ring, ring_full, e, tok0, f0);
+                __syncwarp();
+            }
         };
         int kb = 0;
         for (; kb + 1 < nkb; kb += 2) { kblock(afr0, afr1, kb); kblock(afr1, afr0, kb + 1); }
@@ -366,21 +457,25 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_dq_kernel(const __grid_consta
         __syncwarp();
         if (lane == 0) mbar_arrive(x_empty + 8 * prev);
 
-        const int tok0 = tt * BN, f = ft * BM + wg * 64 + fr;
+        const int f = f0 + fr;
         float mul[2], bias[2];
         #pragma unroll
         for (int h = 0; h < 2; h++) {
             mul[h] = (f + 8 * h < p.scale_cols) ? p.scale : 1.0f;
             bias[h] = p.bias ? p.bias[f + 8 * h] : 0.0f;
         }
-        void* const out = p.out;
+#define CB_EPI(E) epilogue_staged<E, BF, SE>(p, acc, tok0, f0, warp & 3, lane, bias, mul, ring, ring_full, e, leader, 1 + wg)
         switch (p.epi) {
-        case EPI_STORE16: epilogue_regs<EPI_STORE16, BF>(out, p.M, p.ldo, acc, tok0, f, tc, bias, mul); break;
-        case EPI_GELU16: epilogue_regs<EPI_GELU16, BF>(out, p.M, p.ldo, acc, tok0, f, tc, bias, mul); break;
-        case EPI_QGELU16: epilogue_regs<EPI_QGELU16, BF>(out, p.M, p.ldo, acc, tok0, f, tc, bias, mul); break;
-        case EPI_REDADD32: epilogue_regs<EPI_REDADD32, BF>(out, p.M, p.ldo, acc, tok0, f, tc, bias, mul); break;
-        default: epilogue_regs<EPI_STORE32, BF>(out, p.M, p.ldo, acc, tok0, f, tc, bias, mul); break;
+        case EPI_STORE16: CB_EPI(EPI_STORE16); break;
+        case EPI_GELU16: CB_EPI(EPI_GELU16); break;
+        case EPI_QGELU16: CB_EPI(EPI_QGELU16); break;
+        case EPI_REDADD32: CB_EPI(EPI_REDADD32); break;
+        default: CB_EPI(EPI_STORE32); break;
         }
+#undef CB_EPI
+        // the last tile's stores have written Y before the grid counts as complete (and shared memory goes away).  Inside the loop:
+        // the same wait after it makes ptxas serialize the wgmmas for want of registers.
+        if (leader && tile + (int)gridDim.x >= n_tiles) bulk_wait_all();
     }
 }
 
@@ -443,14 +538,30 @@ cudaError_t gemm_launch(const GemmArgs& a, cudaStream_t stream, int num_sms, uin
     if ((a.epi == EPI_STORE16 || a.epi == EPI_GELU16 || a.epi == EPI_QGELU16) && (a.out_bf16 != 0) != a.operand_bf16) return cudaErrorInvalidValue;
     if (a.qtype == QT_F16 && (a.operand_bf16 || !a.w_map)) return cudaErrorInvalidValue;
     if (a.qtype != QT_F16 && !a.w_packed) return cudaErrorInvalidValue;
+    // the output map: Y [M, N] with row stride ldo, one staging chunk per box (epilogue_staged); a bulk tensor copy needs a 16-byte
+    // aligned base and row stride
+    const bool out32 = (a.epi == EPI_STORE32 || a.epi == EPI_REDADD32);
+    const uint64_t row_bytes = (uint64_t)a.ldo * (out32 ? 4 : 2);
+    if (a.ldo < a.N || reinterpret_cast<uintptr_t>(a.out) % 16 || row_bytes % 16) return cudaErrorInvalidValue;
+    EncodeTiledFn enc = get_encode();
+    if (!enc) return cudaErrorInvalidValue;
     KParams kp;
+    {
+        const cuuint64_t dims[2] = {(cuuint64_t)a.N, (cuuint64_t)a.M};
+        const cuuint64_t strides[1] = {row_bytes};
+        const cuuint32_t box[2] = {out32 ? 32u : 64u, (cuuint32_t)(out32 ? TC32 : TC16)};
+        const cuuint32_t estr[2] = {1, 1};
+        if (enc(&kp.tm_out, out32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, a.out, dims, strides, box, estr,
+                CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+            return cudaErrorInvalidValue;
+    }
     memcpy(&kp.tm_x, a.x_map, sizeof(CUtensorMap));
     if (a.w_map) memcpy(&kp.tm_w, a.w_map, sizeof(CUtensorMap));
     else memset(&kp.tm_w, 0, sizeof(CUtensorMap));
     kp.w_packed = a.w_packed;
     kp.bias = a.bias;
-    kp.out = a.out;
-    kp.M = a.M; kp.N = a.N; kp.K = a.K; kp.ldo = a.ldo;
+    kp.M = a.M; kp.N = a.N; kp.K = a.K;
     kp.epi = a.epi; kp.scale_cols = a.scale_cols; kp.scale = a.scale;
     const int n_tiles = (a.N / BM) * ((a.M + BN - 1) / BN);
     const int grid = n_tiles < num_sms ? n_tiles : num_sms;

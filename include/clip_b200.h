@@ -343,7 +343,8 @@ const char * clip_b200_version(void);
 
 /* TEST HOOK: run one fused-dequant GEMM  Y[M,N] = X[M,K] . W[N,K]^T (+bias) on device 0.
  * w_rows: ggml-format rows of type qtype; x: fp32 host [M,K] (rounded to the operand type on the way in);
- * y_out: fp32 host [M,N].  use_naive=1 runs the scalar debug kernel instead.  Returns 0 on success. */
+ * y_out: fp32 host [M,N].  use_naive=1 runs the scalar debug kernel instead.  Returns 0 on success, 5 if the GEMM wrote into the
+ * poisoned guard rows that follow row M of its output buffer. */
 int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int epi, int use_naive, const float * x,
                          const void * w_rows, const float * bias, const float * resid_in, float * y_out, float * ms);
 
