@@ -88,12 +88,27 @@ EXTENSION_SYMBOLS = [
     # several layers' token rows from one forward pass
     "clip_b200_image_tokens_layers", "clip_b200_image_tokens_layers_device", "clip_b200_text_tokens_layers",
     "clip_b200_text_tokens_layers_device",
+    # attention probabilities (TOKENS_ATTENTION entries)
+    "clip_b200_debug_attention_probs",
 ]
 
 # include/clip_b200.h: output types and flags of the *_tokens entry points
 OUT_F32, OUT_F16, OUT_BF16 = 0, 1, 2
 OUT_DTYPES = {OUT_F32: np.float32, OUT_F16: np.float16, OUT_BF16: np.uint16}      # bf16 comes back as its raw 16-bit pattern
 TOKENS_POST_LN, TOKENS_PROJECT, TOKENS_NORMALIZE, TOKENS_NO_CLS = 1, 2, 4, 8
+TOKENS_ATTENTION, TOKENS_ATTENTION_CLS = 32, 64      # bit 16 stays unassigned
+
+
+def slab_offsets(nbytes, flags):
+    """byte offsets of the slabs of a *_tokens_layers output: slab j follows slab j - 1, except that the slab after an ATTENTION
+    slab starts at the next multiple of 16 bytes.  nbytes[j]: slab j's size, flags[j]: its flags."""
+    offs, o = [], 0
+    for b, f in zip(nbytes, flags):
+        offs.append(o)
+        o += b
+        if f & TOKENS_ATTENTION:
+            o = (o + 15) // 16 * 16
+    return offs
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 PRODUCT_LIB = os.environ.get("CLIP_B200_LIB") or os.path.join(HERE, "libclip_b200.so")     # CLIP_B200_LIB: experiment builds only
@@ -197,6 +212,8 @@ class ClipLib:
             L.clip_b200_debug_attention.argtypes = [ip, ip, ip, ip, ip, ip, fp, fp, C.POINTER(C.c_float)]
             L.clip_b200_debug_attention_hd.restype = C.c_int
             L.clip_b200_debug_attention_hd.argtypes = [ip, ip, ip, ip, ip, ip, ip, fp, fp, C.POINTER(C.c_float)]
+            L.clip_b200_debug_attention_probs.restype = C.c_int
+            L.clip_b200_debug_attention_probs.argtypes = [ip, ip, ip, ip, ip, ip, ip, ip, fp, vp]
             L.clip_b200_debug_gemm.restype = C.c_int
             L.clip_b200_debug_gemm.argtypes = [ip, ip, ip, ip, ip, ip, ip, fp, vp, fp, fp, fp, C.POINTER(C.c_float)]
             i32p = C.POINTER(C.c_int32)
@@ -366,8 +383,11 @@ class ClipLib:
 
     # ---- per-token hidden states (include/clip_b200.h) ------------------------------------------------------------------------
     def token_shape(self, ctx, vision: bool, n: int, rows: int, flags: int):
-        """shape of a *_tokens output: [n, rows (T, T - 1 with NO_CLS, or seq_len), hidden_size or projection_dim]"""
+        """shape of a *_tokens output: [n, rows (T, T - 1 with NO_CLS, or seq_len), hidden_size or projection_dim]; with ATTENTION
+        [n, n_head, rows or 1 (ATTENTION_CLS), rows]"""
         hp = self.vision_hparams(ctx) if vision else self.text_hparams(ctx)
+        if flags & TOKENS_ATTENTION:
+            return (n, hp.n_head, 1 if flags & TOKENS_ATTENTION_CLS else rows, rows)
         width = hp.projection_dim if flags & TOKENS_PROJECT else hp.hidden_size
         return (n, rows - (1 if flags & TOKENS_NO_CLS else 0), width)
 
@@ -421,16 +441,16 @@ class ClipLib:
         c_flags = None if flags is None else (C.c_int * max(len(fl), 1))(*fl)
         shapes = [self.token_shape(ctx, vision, n, rows, f) for f in fl[:len(layers)]]
         sizes = [int(np.prod(s)) for s in shapes]
+        dtype = np.dtype(OUT_DTYPES.get(out_type, np.float32))
+        offs = [b // dtype.itemsize for b in slab_offsets([z * dtype.itemsize for z in sizes], fl)]
+        total = offs[-1] + sizes[-1] if sizes else 0
         if out is None:
-            out = np.empty(sum(sizes), OUT_DTYPES.get(out_type, np.float32))
-        assert out.flags["C_CONTIGUOUS"] and out.size >= sum(sizes)
+            out = np.empty(total, dtype)
+        assert out.flags["C_CONTIGUOUS"] and out.size >= total
         if not call(c_layers, c_flags, len(layers), out):
             raise RuntimeError(name + " failed: " + self.last_error())
-        flat, views, o = out.reshape(-1), [], 0
-        for s, z in zip(shapes, sizes):
-            views.append(flat[o:o + z].reshape(s))
-            o += z
-        return views
+        flat = out.reshape(-1)
+        return [flat[o:o + z].reshape(s) for o, z, s in zip(offs, sizes, shapes)]
 
     def _via_device(self, ctx, inp, out, fn):
         """upload inp, fn(d_in, d_out) into a device buffer of out.nbytes, download into out"""

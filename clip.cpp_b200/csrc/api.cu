@@ -87,7 +87,7 @@ struct Scope {
         }
     }
 };
-enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4, K_POS_RESAMPLE = 5 };
+enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4, K_POS_RESAMPLE = 5, K_ATTN_PROBS = 6 };
 
 // ---- tensor lookup helpers ---------------------------------------------------------------------------------
 const GgufTensor* need(const GgufFile& g, const std::string& name) {
@@ -366,7 +366,8 @@ bool text_forward(clip_ctx* c, int nb, int T, float* d_out, bool normalize) {
 // What a tokens call asks for, checked and resolved: how many blocks to run, which rows of each item, how wide and how many bytes.
 struct TokenReq {
     int blocks = 0, skip = 0, width = 0, esize = 4, flags = 0, out_type = 0;
-    size_t item_bytes = 0;     // one item's rows in the output
+    int attn = 0;              // ATTENTION entry: 1 full maps, 2 the CLS row only (K9 instead of the rows of x)
+    size_t item_bytes = 0;     // one item's rows (or attention maps) in the output
 };
 
 bool token_request(const clip_ctx* c, bool vision, int layer, int flags, int out_type, int T, TokenReq& q, const char* who) {
@@ -377,7 +378,20 @@ bool token_request(const clip_ctx* c, bool vision, int layer, int flags, int out
         set_err(std::string(who) + ": layer " + std::to_string(layer) + " is outside [" + std::to_string(-(nl + 1)) + ", " + std::to_string(nl) + "]");
         return false;
     }
-    if (flags & ~(CLIP_B200_TOKENS_POST_LN | CLIP_B200_TOKENS_PROJECT | CLIP_B200_TOKENS_NORMALIZE | CLIP_B200_TOKENS_NO_CLS)) { set_err(std::string(who) + ": unknown flag bits"); return false; }
+    if (flags & ~(CLIP_B200_TOKENS_POST_LN | CLIP_B200_TOKENS_PROJECT | CLIP_B200_TOKENS_NORMALIZE | CLIP_B200_TOKENS_NO_CLS |
+                  CLIP_B200_TOKENS_ATTENTION | CLIP_B200_TOKENS_ATTENTION_CLS)) { set_err(std::string(who) + ": unknown flag bits"); return false; }
+    if (flags & (CLIP_B200_TOKENS_ATTENTION | CLIP_B200_TOKENS_ATTENTION_CLS)) {
+        if (!(flags & CLIP_B200_TOKENS_ATTENTION)) { set_err(std::string(who) + ": CLIP_B200_TOKENS_ATTENTION_CLS needs CLIP_B200_TOKENS_ATTENTION"); return false; }
+        if (flags & (CLIP_B200_TOKENS_POST_LN | CLIP_B200_TOKENS_PROJECT | CLIP_B200_TOKENS_NORMALIZE | CLIP_B200_TOKENS_NO_CLS)) {
+            set_err(std::string(who) + ": CLIP_B200_TOKENS_ATTENTION cannot be combined with POST_LN, PROJECT, NORMALIZE or NO_CLS");
+            return false;
+        }
+        if ((flags & CLIP_B200_TOKENS_ATTENTION_CLS) && !vision) { set_err(std::string(who) + ": CLIP_B200_TOKENS_ATTENTION_CLS is for the vision tower only"); return false; }
+        if (layer == 0 || layer == -(nl + 1)) {
+            set_err(std::string(who) + ": CLIP_B200_TOKENS_ATTENTION needs layer >= 1 (or -n_layer .. -1): layer " + std::to_string(layer) + " is before the first block");
+            return false;
+        }
+    }
     if ((flags & CLIP_B200_TOKENS_NO_CLS) && !vision) { set_err(std::string(who) + ": CLIP_B200_TOKENS_NO_CLS is for the vision tower only"); return false; }
     if ((flags & CLIP_B200_TOKENS_NORMALIZE) && !(flags & CLIP_B200_TOKENS_PROJECT)) { set_err(std::string(who) + ": CLIP_B200_TOKENS_NORMALIZE needs CLIP_B200_TOKENS_PROJECT"); return false; }
     if (out_type != CLIP_B200_OUT_F32 && out_type != CLIP_B200_OUT_F16 && out_type != CLIP_B200_OUT_BF16) { set_err(std::string(who) + ": unknown out_type " + std::to_string(out_type)); return false; }
@@ -392,17 +406,25 @@ bool token_request(const clip_ctx* c, bool vision, int layer, int flags, int out
     q.esize = out_type == CLIP_B200_OUT_F32 ? 4 : 2;
     q.flags = flags; q.out_type = out_type;
     q.item_bytes = (size_t)(T - q.skip) * q.width * q.esize;
+    if (flags & CLIP_B200_TOKENS_ATTENTION) {
+        q.attn = (flags & CLIP_B200_TOKENS_ATTENTION_CLS) ? 2 : 1;
+        q.item_bytes = (size_t)tw.heads * (q.attn == 2 ? 1 : T) * T * q.esize;
+    }
     return true;
 }
 
 // After the blocks: the requested rows of ws.x for nb items of T rows -> dst (device), item-major, q.item_bytes per item.
 // PROJECT runs today's pooled tail on every row -- K2 post_ln into the 16-bit operand type, K1 projection (fp32), l2norm -- so the
 // CLS / EOT rows come out bit-identical to clip_image_batch_encode / clip_text_batch_encode; K7 then picks and converts the rows.
+// An ATTENTION entry runs K9 on ws.qkv, which still holds the last block's Q | K | V (token_stops emits it before any PROJECT tail).
 bool token_rows_tail(clip_ctx* c, Tower& tw, int nb, int T, const TokenReq& q, void* dst) {
     Workspace& w = tw.ws;
     const int h = tw.hidden, M = nb * T, bf = c->operand_bf16 ? 1 : 0;
     const bool ln = q.flags & (CLIP_B200_TOKENS_POST_LN | CLIP_B200_TOKENS_PROJECT);
-    if (!(q.flags & CLIP_B200_TOKENS_PROJECT)) {
+    if (q.attn) {
+        Scope s(c, K_ATTN_PROBS);
+        CK(launch_attention_probs(w.qkv, dst, q.out_type, nb, T, tw.heads, h / tw.heads, &tw == &c->txt ? 1 : 0, q.attn == 2 ? 1 : 0, bf, c->stream));
+    } else if (!(q.flags & CLIP_B200_TOKENS_PROJECT)) {
         Scope s(c, K_TOKEN_ROWS);
         launch_token_rows(w.x, h, nb, T, q.skip, h, ln ? tw.post_g : nullptr, tw.post_b, tw.eps, q.out_type, dst, c->stream);
     } else {
@@ -419,12 +441,16 @@ bool token_rows_tail(clip_ctx* c, Tower& tw, int nb, int T, const TokenReq& q, v
 
 // The entries of one tokens call (one for the single-layer calls), for nb items whose embedding is in ws.x: the blocks run once, up
 // to the deepest entry, each run resuming where the previous stop left x; after each block count some entry asks for, emit(j) writes
-// entry j's rows (token_rows_tail) while x holds that layer.  Between stops only x is live, so a PROJECT tail may use a, qkv and g.
+// entry j's rows (token_rows_tail) while x holds that layer.  Between stops x is live, and so is qkv until the stop's ATTENTION
+// entries have run: the last block's QKV GEMM wrote it and nothing after K3 in a block writes it.  So at one stop the ATTENTION
+// entries come first, and only then may a PROJECT tail use a, qkv and g as scratch.
 template <class Emit>
 bool token_stops(clip_ctx* c, Tower& tw, int nb, int T, bool causal, const std::vector<TokenReq>& qs, Emit emit) {
     std::vector<int> order(qs.size());
     std::iota(order.begin(), order.end(), 0);
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return qs[a].blocks < qs[b].blocks; });
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) {
+        return qs[a].blocks != qs[b].blocks ? qs[a].blocks < qs[b].blocks : (qs[a].attn != 0) > (qs[b].attn != 0);
+    });
     int done = 0;
     for (int j : order) {
         if (qs[j].blocks > done) {
@@ -451,11 +477,16 @@ bool text_tokens(clip_ctx* c, int nb, int T, const std::vector<TokenReq>& qs, Em
 }
 
 // Layer-major output of a tokens call: entry j's slab of n items starts at n * (item_bytes of the entries before it); the shard of
-// items lo .. of a devices-mode GPU starts lo * item_bytes_j into each slab.
+// items lo .. of a devices-mode GPU starts lo * item_bytes_j into each slab.  The slab after an ATTENTION slab starts at the next
+// multiple of 16 bytes: attention items are H x R x T elements, often an odd count, and K7's vector stores need the alignment.
 std::vector<char*> slab_bases(const std::vector<TokenReq>& qs, char* out, size_t n, size_t lo) {
     std::vector<char*> b;
     size_t off = 0;
-    for (const TokenReq& q : qs) { b.push_back(out + off + lo * q.item_bytes); off += n * q.item_bytes; }
+    for (const TokenReq& q : qs) {
+        b.push_back(out + off + lo * q.item_bytes);
+        off += n * q.item_bytes;
+        if (q.attn) off = (off + 15) / 16 * 16;
+    }
     return b;
 }
 
@@ -2361,6 +2392,32 @@ int clip_b200_debug_token_rows(int n, int T, int h, size_t in_stride, int no_cls
     if (!s.ok) return 3;
     launch_token_rows(d_x, in_stride, n, T, skip, h, d_g, d_b, eps, out_type, d_out, s.st);
     if (!s.finish("token_rows")) return 5;
+    return s.copy_back(out, d_out, out_bytes) ? 0 : 6;
+}
+
+// K9 on qkv (fp32 host [nseq*T, 3*H*head_dim], rounded to the operand type on the way in; one 128-row box of poisoned rows follows
+// the last sequence, as in clip_b200_debug_attention_hd).  Poisoned guard bytes follow the output.
+int clip_b200_debug_attention_probs(int operand_bf16, int nseq, int T, int H, int head_dim, int causal, int cls_row, int out_type,
+                                    const float* qkv, void* out) {
+    g_err.clear();
+    if ((head_dim != 64 && head_dim != 80) || nseq <= 0 || T <= 0 || H <= 0 || out_type < 0 || out_type > 2 || !qkv || !out) {
+        set_err("debug_attention_probs: bad arguments (head_dim 64 or 80, positive sizes, out_type 0..2)");
+        return 2;
+    }
+    HookScratch s;
+    if (s.ok && attention_tc_init() != cudaSuccess) { set_err("attention_tc_init failed"); return 1; }
+    const size_t rows = (size_t)nseq * T, cols = (size_t)3 * H * head_dim, guard = 4096;
+    const size_t out_bytes = (size_t)nseq * H * (cls_row ? 1 : T) * T * (out_type == 0 ? 4 : 2);
+    const std::vector<uint16_t> q16 = to16(qkv, rows * cols, operand_bf16);
+    void* d_qkv = s.alloc((rows + 128) * cols * 2, 0xff, q16.data(), q16.size() * 2);
+    uint8_t* d_out = (uint8_t*)s.alloc(out_bytes + guard, 0xff);
+    if (!s.ok) return 3;
+    const cudaError_t e = launch_attention_probs(d_qkv, d_out, out_type, nseq, T, H, head_dim, causal ? 1 : 0, cls_row ? 1 : 0, operand_bf16 ? 1 : 0, s.st);
+    if (e != cudaSuccess) { set_err(std::string("attention_probs launch: ") + cudaGetErrorString(e)); return 4; }
+    if (!s.finish("attention_probs")) return 4;
+    std::vector<uint8_t> g(guard);
+    if (!s.copy_back(g.data(), d_out + out_bytes, guard)) return 6;
+    if (std::any_of(g.begin(), g.end(), [](uint8_t b) { return b != 0xFF; })) { set_err("attention_probs wrote past the output"); return 5; }
     return s.copy_back(out, d_out, out_bytes) ? 0 : 6;
 }
 

@@ -323,6 +323,220 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __gr
     }
 }
 
+// ---- K9: the attention probabilities themselves (the *_tokens calls' ATTENTION entries) ------------------------------------------
+// softmax(Q.K^T [causal]) of one block, recomputed from the qkv matrix K3 read (Q scaled by 1/sqrt(dh) and rounded, K 16-bit) through
+// the same 3-D maps, as rows of T elements.  CTA = one consumer warpgroup (warps 0-3) + one producer warp (warp 4); work unit = one
+// (sequence, head, 64-row query group), in CLS mode one (sequence, head), group 0, of which only row 0 is written.
+//   producer  one thread: the group's Q box, then K only (V is never loaded) in 128-key blocks into a two-deep ring, every block twice.
+//   pass 1    per key block: S = Q.K^T (wgmma, K3's widths 16 / 32 / 64 / 128 and masks), running row max and sum with K3's arithmetic.
+//   pass 2    the blocks again: p = ex2(s log2e - m log2e) * (1 / l) in fp32 (a 16-bit output is the RNE of that fp32 value), masked
+//             keys +0.  Each [64 x <= 128] block is staged in shared memory and leaves as row segments of coalesced element stores:
+//             rows are T elements long and T is mostly odd, so no store wider than one element is aligned.  The keys of a causal
+//             group past its diagonal block are written as +0 without being computed.
+constexpr int PROBS_THREADS = 160;
+constexpr int PSTRIDE = AK + 8;          // staging row stride in elements: a warp's fragment stores of 4 rows fill 32 distinct banks
+
+template <int DH>
+struct ProbsGeo {
+    using G = AttnGeo<DH>;
+    static constexpr uint32_t K_OFF = G::TILE;                        // Q: box 0 of one tile; then the two K stages
+    static constexpr uint32_t STAGE_OFF = K_OFF + 2 * G::TILE;        // [64][PSTRIDE] elements of up to 4 bytes
+    static constexpr uint32_t BAR_OFF = STAGE_OFF + AG * PSTRIDE * 4;
+    static constexpr uint32_t SMEM = BAR_OFF + 64 + 1024;
+};
+
+struct PParams {
+    AParams a;              // maps, T, H, causal; ngrp = 64-row groups per (sequence, head), 1 in CLS mode
+    void* out;              // [nseq, H, rows, T] of otype
+    int otype, rows;        // 0 f32, 1 f16, 2 bf16;  rows = T, or 1 (CLS)
+};
+
+CB_DEVINL void probs_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }      // the consumer warpgroup only
+
+// S of one key block, NT n-tiles wide, masked as in attend_block
+template <bool BF, int DH, int NT>
+CB_DEVINL void probs_scores(float (&sc)[4 * NT], uint64_t dq, uint64_t dq_t, uint32_t k_s, int key0, int T, int causal, int wrow0, int r0,
+                            int tc) {
+    using G = AttnGeo<DH>;
+    const uint64_t dk = wgmma_desc_sw128(k_s);
+    wgmma_fence();
+    #pragma unroll
+    for (int k = 0; k < 4; k++) wgmma_ss_nt<BF, NT>(sc, dq + 2 * k, dk + 2 * k, (uint32_t)k);
+    if constexpr (G::TAIL) wgmma_ss_nt<BF, NT>(sc, dq_t, wgmma_desc_sw32(k_s + G::MAIN), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sc);
+    if (key0 + 8 * NT > T || (causal && key0 + 8 * NT - 1 > wrow0)) {
+        #pragma unroll
+        for (int j = 0; j < NT; j++) {
+            #pragma unroll
+            for (int e = 0; e < 4; e++) {
+                const int key = key0 + 8 * j + tc + (e & 1), row = r0 + 8 * (e >> 1);
+                if (key >= T || (causal && key > row)) sc[4 * j + e] = -INFINITY;
+            }
+        }
+    }
+}
+
+// pass 1: the running row max and sum over one key block, exactly as attend_block updates them
+template <bool BF, int DH, int NT>
+CB_DEVINL void probs_stats(float (&m_run)[2], float (&l_run)[2], uint64_t dq, uint64_t dq_t, uint32_t k_s, int key0, int T, int causal,
+                           int wrow0, int r0, int tc) {
+    constexpr float LOG2E = 1.4426950408889634f;
+    float sc[4 * NT];
+    probs_scores<BF, DH, NT>(sc, dq, dq_t, k_s, key0, T, causal, wrow0, r0, tc);
+    #pragma unroll
+    for (int h = 0; h < 2; h++) {
+        float mx = -INFINITY;
+        #pragma unroll
+        for (int j = 0; j < NT; j++) mx = fmaxf(mx, fmaxf(sc[4 * j + 2 * h], sc[4 * j + 2 * h + 1]));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        const float m_new = fmaxf(m_run[h], mx);
+        const float alpha = ex2f((m_run[h] - m_new) * LOG2E), mb = m_new * LOG2E;
+        float rs = 0.f;
+        #pragma unroll
+        for (int j = 0; j < NT; j++) rs += ex2f(sc[4 * j + 2 * h] * LOG2E - mb) + ex2f(sc[4 * j + 2 * h + 1] * LOG2E - mb);
+        l_run[h] = l_run[h] * alpha + rs;
+        m_run[h] = m_new;
+    }
+}
+
+// pass 2: the probabilities of one key block into the staging buffer (row lr0 + 8h, columns 8j + tc + {0, 1}); the K stage is
+// released as soon as S is in registers
+template <bool BF, int DH, int NT>
+CB_DEVINL void probs_block(const float (&mb)[2], const float (&inv)[2], uint64_t dq, uint64_t dq_t, uint32_t k_s, int key0, int T, int causal,
+                           int wrow0, int r0, int tc, int lr0, uint8_t* stage, int otype, uint32_t release, int lane) {
+    constexpr float LOG2E = 1.4426950408889634f;
+    float sc[4 * NT];
+    probs_scores<BF, DH, NT>(sc, dq, dq_t, k_s, key0, T, causal, wrow0, r0, tc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(release);
+    probs_bar();                                               // the previous block's stores have read the staging buffer
+    #pragma unroll
+    for (int h = 0; h < 2; h++) {
+        const int lr = lr0 + 8 * h;
+        #pragma unroll
+        for (int j = 0; j < NT; j++) {
+            const float p0 = ex2f(sc[4 * j + 2 * h] * LOG2E - mb[h]) * inv[h], p1 = ex2f(sc[4 * j + 2 * h + 1] * LOG2E - mb[h]) * inv[h];
+            const int e = lr * PSTRIDE + 8 * j + tc;
+            if (otype == 0) *reinterpret_cast<float2*>(stage + 4 * e) = make_float2(p0, p1);
+            else *reinterpret_cast<uint32_t*>(stage + 2 * e) = otype == 2 ? pack2<true>(p0, p1) : pack2<false>(p0, p1);
+        }
+    }
+    probs_bar();
+}
+
+template <bool BF, int DH>
+__global__ void __launch_bounds__(PROBS_THREADS, 1) attention_probs_kernel(const __grid_constant__ PParams p) {
+    using G = AttnGeo<DH>;
+    using PG = ProbsGeo<DH>;
+    constexpr float LOG2E = 1.4426950408889634f;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    const uint32_t smem_base = smem_u32(smem);
+    // Q full, K stage full [0|1], K stage empty [0|1]
+    const uint32_t q_full = smem_base + PG::BAR_OFF, kv_full = q_full + 8, kv_empty = q_full + 24;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        mbar_init(q_full, 1);
+        for (int i = 0; i < 2; i++) { mbar_init(kv_full + 8 * i, 1); mbar_init(kv_empty + 8 * i, 4); }     // released by each consumer warp
+        mbar_fence_init();
+        tma_prefetch_desc(&p.a.tm_qkv);
+        if constexpr (G::TAIL) tma_prefetch_desc(&p.a.tm_tail);
+    }
+    __syncthreads();
+    pdl_trigger();
+    pdl_wait();      // qkv is read (and the output written) only after the kernels before this one have completed
+
+    const int T = p.a.T;
+    const int sh = blockIdx.x / p.a.ngrp;                     // (sequence, head)
+    const int g0 = (blockIdx.x - sh * p.a.ngrp) * AG, head = sh % p.a.H, seq = sh / p.a.H;
+    const int kend = p.a.causal ? min(T, g0 + AG) : T;
+    const int nkb = (kend + AK - 1) / AK;
+    if (warp == 4) {
+        // ------------------------------------------------------------------ producer (one thread): Q, then K blocks 0 .. nkb-1 twice
+        if (lane == 0) {
+            mbar_arrive_expect_tx(q_full, G::BOX_BYTES);
+            load_box<DH>(smem_base, 0, p.a, head * DH, g0, seq, q_full);
+            const int kcol = p.a.H * DH + head * DH;
+            for (int n = 0; n < 2 * nkb; n++) {
+                const int kb = n < nkb ? n : n - nkb, nb = kv_boxes(kend, kb);
+                const uint32_t s = n & 1, bar = kv_full + 8 * s;
+                mbar_wait(kv_empty + 8 * s, ((n >> 1) & 1) ^ 1);
+                mbar_arrive_expect_tx(bar, (uint32_t)nb * G::BOX_BYTES);
+                for (int b = 0; b < nb; b++) load_box<DH>(smem_base + PG::K_OFF + s * G::TILE, b, p.a, kcol, kb * AK + b * ABOX, seq, bar);
+            }
+        }
+        return;
+    }
+
+    // ---------------------------------------------------------------------- consumers (fragment layout: wgmma.cuh)
+    const int tc = 2 * (lane & 3);
+    const int lr0 = warp * 16 + (lane >> 2);                  // this thread: group rows lr0 and lr0 + 8
+    const int wrow0 = g0 + warp * 16, r0 = g0 + lr0;
+    mbar_wait(q_full, 0);
+    const uint64_t dq = wgmma_desc_sw128(smem_base), dq_t = wgmma_desc_sw32(smem_base + G::MAIN);
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    uint32_t n = 0;
+    for (int kb = 0; kb < nkb; kb++, n++) {
+        const uint32_t s = n & 1, k_s = smem_base + PG::K_OFF + s * G::TILE;
+        mbar_wait(kv_full + 8 * s, (n >> 1) & 1);
+        const int key0 = kb * AK, rem = kend - key0;
+        if (rem > 64) probs_stats<BF, DH, 16>(m_run, l_run, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc);
+        else if (rem > 32) probs_stats<BF, DH, 8>(m_run, l_run, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc);
+        else if (rem > 16) probs_stats<BF, DH, 4>(m_run, l_run, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc);
+        else probs_stats<BF, DH, 2>(m_run, l_run, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(kv_empty + 8 * s);
+    }
+    float mb[2], inv[2];
+    #pragma unroll
+    for (int h = 0; h < 2; h++) {
+        float l = l_run[h];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        inv[h] = 1.0f / l;
+        mb[h] = m_run[h] * LOG2E;
+    }
+
+    uint8_t* stage = smem + PG::STAGE_OFF;
+    const int nrows = p.rows == 1 ? 1 : min(AG, T - g0);
+    const size_t obase = ((size_t)sh * p.rows + g0) * T;      // element offset of the group's first row
+    for (int kb = 0; kb < nkb; kb++, n++) {
+        const uint32_t s = n & 1, k_s = smem_base + PG::K_OFF + s * G::TILE, release = kv_empty + 8 * s;
+        mbar_wait(kv_full + 8 * s, (n >> 1) & 1);
+        const int key0 = kb * AK, rem = kend - key0;
+        if (rem > 64) probs_block<BF, DH, 16>(mb, inv, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc, lr0, stage, p.otype, release, lane);
+        else if (rem > 32) probs_block<BF, DH, 8>(mb, inv, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc, lr0, stage, p.otype, release, lane);
+        else if (rem > 16) probs_block<BF, DH, 4>(mb, inv, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc, lr0, stage, p.otype, release, lane);
+        else probs_block<BF, DH, 2>(mb, inv, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc, lr0, stage, p.otype, release, lane);
+        // columns key0 .. min(key0 + 128, kend) - 1 of every row, one warp per row
+        const int cw = min(AK, rem);
+        if (p.otype == 0) {
+            const float* sf = reinterpret_cast<const float*>(stage);
+            float* o = reinterpret_cast<float*>(p.out) + obase + key0;
+            for (int r = warp; r < nrows; r += 4)
+                for (int c = lane; c < cw; c += 32) o[(size_t)r * T + c] = sf[r * PSTRIDE + c];
+        } else {
+            const uint16_t* sh16 = reinterpret_cast<const uint16_t*>(stage);
+            uint16_t* o = reinterpret_cast<uint16_t*>(p.out) + obase + key0;
+            for (int r = warp; r < nrows; r += 4)
+                for (int c = lane; c < cw; c += 32) o[(size_t)r * T + c] = sh16[r * PSTRIDE + c];
+        }
+    }
+    // a causal group's keys past its diagonal block: +0
+    if (kend < T) {
+        for (int r = warp; r < nrows; r += 4) {
+            const size_t o = obase + (size_t)r * T;
+            for (int c = kend + lane; c < T; c += 32) {
+                if (p.otype == 0) reinterpret_cast<float*>(p.out)[o + c] = 0.f;
+                else reinterpret_cast<uint16_t*>(p.out)[o + c] = 0;
+            }
+        }
+    }
+}
+
 typedef CUresult (*EncodeTiledFn3)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -349,7 +563,11 @@ template <int DH>
 cudaError_t set_smem() {
     cudaError_t e = cudaFuncSetAttribute(attention_tc_kernel<true, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AttnGeo<DH>::SMEM);
     if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(attention_tc_kernel<false, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AttnGeo<DH>::SMEM);
+    e = cudaFuncSetAttribute(attention_tc_kernel<false, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AttnGeo<DH>::SMEM);
+    if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(attention_probs_kernel<true, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ProbsGeo<DH>::SMEM);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(attention_probs_kernel<false, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ProbsGeo<DH>::SMEM);
 }
 
 template <int DH>
@@ -386,6 +604,28 @@ cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T,
     if (e != cudaSuccess) return e;
     const unsigned grid = (unsigned)min(p.niter, sms);
     e = dh == 80 ? launch_dh<80>(p, grid, bf16, st) : launch_dh<64>(p, grid, bf16, st);
+    return e != cudaSuccess ? e : cudaGetLastError();
+}
+
+cudaError_t launch_attention_probs(const void* qkv16, void* out, int elem_type, int nseq, int T, int H, int dh, int causal, int cls_only,
+                                   int bf16, cudaStream_t st) {
+    if ((dh != 64 && dh != 80) || elem_type < 0 || elem_type > 2) return cudaErrorInvalidValue;
+    if (nseq <= 0 || T <= 0) return cudaSuccess;
+    PParams p;
+    memset(&p, 0, sizeof(p));
+    if (!make_qkv_map(&p.a.tm_qkv, qkv16, nseq, T, H, dh, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return cudaErrorInvalidValue;
+    if (dh == 80 && !make_qkv_map(&p.a.tm_tail, qkv16, nseq, T, H, dh, 16, CU_TENSOR_MAP_SWIZZLE_32B)) return cudaErrorInvalidValue;
+    p.a.T = T; p.a.H = H; p.a.causal = causal;
+    p.a.ngrp = cls_only ? 1 : (T + AG - 1) / AG;
+    p.out = out; p.otype = elem_type; p.rows = cls_only ? 1 : T;
+    const long long units = (long long)nseq * H * p.a.ngrp;
+    if (units > 0x7fffffffll) return cudaErrorInvalidValue;
+    const unsigned grid = (unsigned)units;
+    cudaError_t e;
+    if (dh == 80) e = bf16 ? launch_pdl(attention_probs_kernel<true, 80>, grid, (unsigned)PROBS_THREADS, ProbsGeo<80>::SMEM, st, 1, p)
+                           : launch_pdl(attention_probs_kernel<false, 80>, grid, (unsigned)PROBS_THREADS, ProbsGeo<80>::SMEM, st, 1, p);
+    else e = bf16 ? launch_pdl(attention_probs_kernel<true, 64>, grid, (unsigned)PROBS_THREADS, ProbsGeo<64>::SMEM, st, 1, p)
+                  : launch_pdl(attention_probs_kernel<false, 64>, grid, (unsigned)PROBS_THREADS, ProbsGeo<64>::SMEM, st, 1, p);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 

@@ -50,6 +50,12 @@ void launch_attention(const void* qkv16, void* out16, int nseq, int T, int H, in
 cudaError_t attention_tc_init();
 cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T, int H, int dh, int causal, int bf16, cudaStream_t st);
 
+// K9 attention probabilities (attention_tc.cu): the softmax(Q K^T [causal]) K3 computes internally, from the same qkv16, written out:
+// out [nseq, H, R, T] of elem_type (0 fp32, 1 fp16, 2 bf16: RNE of the fp32 value), R = T, or 1 with cls_only (query row 0 alone).
+// Masked keys are +0.  Any T, head_dim 64 or 80; out needs only the element type's alignment.
+cudaError_t launch_attention_probs(const void* qkv16, void* out, int elem_type, int nseq, int T, int H, int dh, int causal, int cls_only,
+                                   int bf16, cudaStream_t st);
+
 // K5 head tail: out[r,:] = normalize ? v / sqrt(sum v^2) : v    (clip.cpp:1163-1166, 1448-1455)
 void launch_l2norm(const float* v, float* out, int rows, int d, int normalize, cudaStream_t st);
 

@@ -194,6 +194,23 @@ enum { CLIP_B200_OUT_F32 = 0, CLIP_B200_OUT_F16 = 1, CLIP_B200_OUT_BF16 = 2 };
 #define CLIP_B200_TOKENS_PROJECT    2  /* post_ln + projection: rows of projection_dim instead of hidden_size        */
 #define CLIP_B200_TOKENS_NORMALIZE  4  /* with PROJECT: L2-normalise each row (as normalize=true does)               */
 #define CLIP_B200_TOKENS_NO_CLS     8  /* vision only: patch tokens, T-1 rows per image                               */
+/* bit 16 is deliberately left unassigned (tests use it as an unknown flag); new flags take bits above 64 */
+#define CLIP_B200_TOKENS_ATTENTION      32  /* the softmax probabilities of block `layer` instead of its residual rows        */
+#define CLIP_B200_TOKENS_ATTENTION_CLS  64  /* with ATTENTION, vision only: query row 0 (CLS) only                            */
+/* ATTENTION entries (HF output_attentions): `layer` l >= 1, or negative (-1 = the last block), returns the attention of the l-th
+ * block, HF's attentions[l - 1]; only blocks 0 .. l - 1 run.  Layer 0 and -(n_layer + 1) are refused (no block has run).
+ *   out      per item [H, R, T] row-major (item-major [n, H, R, T], HF's layout), R = T, or 1 with ATTENTION_CLS; elements of
+ *            out_type, rounded to nearest even.  Text rows use the causal mask: entries above the diagonal are exactly +0.  Padding is
+ *            the caller's, as for hidden states: the rows before a sequence's padding do not depend on it.
+ *   flags    ATTENTION cannot be combined with POST_LN, PROJECT, NORMALIZE or NO_CLS; ATTENTION_CLS needs ATTENTION and is refused on
+ *            text.
+ * Numerics: the scores are those of the attention kernel -- Q already scaled by 1/sqrt(head_dim) and rounded to the 16-bit operand
+ * type, K 16-bit, products accumulated in fp32 -- and the softmax runs in fp32 with ex2: p = ex2(s log2e - m log2e) * (1 / l), m the
+ * row max, l the sum of ex2(s log2e - m log2e) accumulated block by block as the attention kernel accumulates it.  16-bit outputs are
+ * the RNE of that fp32 value.  Not bit-identical to the P the attention kernel multiplies V with: that one is rescaled online and
+ * rounded to 16 bits (tests/_attention_probs_bound.py derives the element-wise bound against an fp64 softmax of the same operands).
+ * Memory: full maps are large (ViT-L/14 at 224: 16 x 257 x 257 elements per image and layer, 2.1 MB in f16); the host forms stage
+ * one micro-batch of the widest entry twice on the device (see *_tokens_layers). */
 bool clip_b200_image_tokens(const struct clip_ctx * ctx, const struct clip_image_f32_batch * imgs, int layer, int flags, int out_type,
                             void * out);
 bool clip_b200_image_tokens_device(const struct clip_ctx * ctx, const void * d_pixels, size_t n, int layer, int flags, int out_type,
@@ -234,7 +251,10 @@ bool clip_b200_image_tokens_hw(const struct clip_ctx * ctx, const struct clip_im
  *            Any order, duplicates allowed.  flags == NULL: 0 for every entry.  Only blocks 0 .. deepest - 1 run, each once.
  *   n_layers 1 .. CLIP_B200_TOKENS_MAX_LAYERS;  out_type applies to every entry.
  *   out      layer-major: entry j is one slab of n * item_bytes_j bytes at offset n * (item_bytes_0 + ... + item_bytes_{j-1}), laid
- *            out as the single-layer call lays out its whole output (item_bytes_j = rows x width x element size of that entry).
+ *            out as the single-layer call lays out its whole output (item_bytes_j = rows x width x element size of that entry;
+ *            H x R x T x element size for an ATTENTION entry).  After an ATTENTION slab the next slab starts at the next multiple of
+ *            16 bytes (from out), so that the vector stores of the slab after an odd-sized attention slab stay aligned; only
+ *            attention slabs are padded, and a list without ATTENTION entries is laid out as above, byte for byte.
  * Slab j equals, byte for byte, the single-layer call with (layers[j], flags[j], out_type) on the same inputs: the same kernels run
  * on the same residual stream.  Image size: the host form takes it from the images, as clip_b200_image_tokens_hw does (at
  * image_size x image_size that is the native path); the device form takes height x width (image_size x image_size: native).  Every
@@ -332,7 +352,8 @@ void   clip_b200_set_micro_batch(const struct clip_ctx * ctx, int images, int se
 uint64_t clip_b200_kernel_launches(const struct clip_ctx * ctx);   /* kernels launched by this context so far */
 float    clip_b200_last_device_ms(const struct clip_ctx * ctx);    /* CUDA-event time of the last encode's kernels */
 /* per-kernel-class CUDA-event time accumulated since the last call with the same kind (0 GEMM, 1 attention,
- * 2 layernorm, 3 other, 4 the token-row kernel of the *_tokens calls, 5 the position-table resample of the *_hw calls); *count
+ * 2 layernorm, 3 other, 4 the token-row kernel of the *_tokens calls, 5 the position-table resample of the *_hw calls, 6 the
+ * attention-probability kernel of ATTENTION entries); *count
  * receives the number of launches.  Enabled by env CLIP_B200_PROFILE=1. */
 float    clip_b200_kernel_ms(const struct clip_ctx * ctx, int kind, uint64_t * count);
 /* CUDA-event stopwatch on the launch stream: mark(slot 0..3), then elapsed(a, b) in ms (-1 on error) */
@@ -366,6 +387,12 @@ int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int caus
  * Returns 2 with a message for any other head_dim, and for use_legacy=1 with head_dim 80 (the legacy kernel is head_dim 64 only). */
 int clip_b200_debug_attention_hd(int operand_bf16, int nseq, int T, int H, int head_dim, int causal, int use_legacy, const float * qkv,
                                  float * out, float * ms);
+/* The attention probabilities of the same qkv (the kernel behind CLIP_B200_TOKENS_ATTENTION): out [nseq, H, R, T] with R = T, or 1
+ * with cls_row (query row 0 only), of out_type (0 fp32, 1 fp16, 2 bf16: raw 16-bit values, not widened).  Runs on device 0.  Returns
+ * 2 for bad arguments (head_dim other than 64 / 80, a non-positive size, an unknown out_type), 5 if the kernel wrote into the
+ * poisoned guard bytes that follow the output. */
+int clip_b200_debug_attention_probs(int operand_bf16, int nseq, int T, int H, int head_dim, int causal, int cls_row, int out_type,
+                                    const float * qkv, void * out);
 
 /* TEST HOOKS for the row kernels (csrc/kernels.cu): each runs one launcher on a private stream on device 0 and returns 0 on
  * success (clip_b200_last_error says why not).  Host buffers are fp32 / int32; 16-bit inputs are rounded to the operand type
