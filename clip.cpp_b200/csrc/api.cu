@@ -363,16 +363,15 @@ bool text_forward(clip_ctx* c, int nb, int T, float* d_out, bool normalize) {
 }
 
 // ---- per-token hidden states (clip_b200_image_tokens / clip_b200_text_tokens) ----------------------------------------------------
-// What a tokens call asks for, checked and resolved: how many blocks to run, which rows of each item, how wide and how many bytes.
+// What a tokens call asks for, checked and resolved: how many blocks to run, which rows of each item, how wide.
 struct TokenReq {
     int blocks = 0, skip = 0, width = 0, esize = 4, flags = 0, out_type = 0;
     int attn = 0;              // ATTENTION entry: 1 full maps, 2 the CLS row only (K9 instead of the rows of x)
-    size_t item_bytes = 0;     // one item's rows (or attention maps) in the output
 };
 
-bool token_request(const clip_ctx* c, bool vision, int layer, int flags, int out_type, int T, TokenReq& q, const char* who) {
+// One entry of a tokens call on a tower that is present.
+bool token_request(const clip_ctx* c, bool vision, int layer, int flags, int out_type, TokenReq& q, const char* who) {
     const Tower& tw = vision ? c->vis : c->txt;
-    if (!tw.present) { set_err(std::string(who) + ": this model has no " + (vision ? "vision" : "text") + " encoder"); return false; }
     const int nl = tw.layers;
     if (layer < -(nl + 1) || layer > nl) {
         set_err(std::string(who) + ": layer " + std::to_string(layer) + " is outside [" + std::to_string(-(nl + 1)) + ", " + std::to_string(nl) + "]");
@@ -405,15 +404,17 @@ bool token_request(const clip_ctx* c, bool vision, int layer, int flags, int out
     q.width = (flags & CLIP_B200_TOKENS_PROJECT) ? tw.proj : tw.hidden;
     q.esize = out_type == CLIP_B200_OUT_F32 ? 4 : 2;
     q.flags = flags; q.out_type = out_type;
-    q.item_bytes = (size_t)(T - q.skip) * q.width * q.esize;
-    if (flags & CLIP_B200_TOKENS_ATTENTION) {
-        q.attn = (flags & CLIP_B200_TOKENS_ATTENTION_CLS) ? 2 : 1;
-        q.item_bytes = (size_t)tw.heads * (q.attn == 2 ? 1 : T) * T * q.esize;
-    }
+    if (flags & CLIP_B200_TOKENS_ATTENTION) q.attn = (flags & CLIP_B200_TOKENS_ATTENTION_CLS) ? 2 : 1;
     return true;
 }
 
-// After the blocks: the requested rows of ws.x for nb items of T rows -> dst (device), item-major, q.item_bytes per item.
+// one item's rows (or attention maps) of entry q in the output of a call of T rows per item
+size_t item_bytes(const TokenReq& q, const Tower& tw, int T) {
+    if (q.attn) return (size_t)tw.heads * (q.attn == 2 ? 1 : T) * T * q.esize;
+    return (size_t)(T - q.skip) * q.width * q.esize;
+}
+
+// After the blocks: the requested rows of ws.x for nb items of T rows -> dst (device), item-major, item_bytes per item.
 // PROJECT runs today's pooled tail on every row -- K2 post_ln into the 16-bit operand type, K1 projection (fp32), l2norm -- so the
 // CLS / EOT rows come out bit-identical to clip_image_batch_encode / clip_text_batch_encode; K7 then picks and converts the rows.
 // An ATTENTION entry runs K9 on ws.qkv, which still holds the last block's Q | K | V (token_stops emits it before any PROJECT tail).
@@ -462,29 +463,17 @@ bool token_stops(clip_ctx* c, Tower& tw, int nb, int T, bool causal, const std::
     return true;
 }
 
-// nb images at d_pixels through the blocks of every entry -> emit(j)
-template <class Emit>
-bool vision_tokens(clip_ctx* c, const float* d_pixels, int nb, const VisCall& v, const std::vector<TokenReq>& qs, Emit emit) {
-    return vision_embed(c, d_pixels, nb, v) && token_stops(c, c->vis, nb, v.T, false, qs, emit);
-}
-
-// nb sequences of T ids already in ws.ids through the blocks of every entry -> emit(j)
-template <class Emit>
-bool text_tokens(clip_ctx* c, int nb, int T, const std::vector<TokenReq>& qs, Emit emit) {
-    Tower& tw = c->txt;
-    { Scope s(c, K_OTHER); launch_text_embed(tw.ws.ids, tw.tok, tw.pos, nb, T, tw.hidden, tw.n_vocab, tw.ws.x, c->stream); }
-    return token_stops(c, tw, nb, T, true, qs, emit);
-}
-
-// Layer-major output of a tokens call: entry j's slab of n items starts at n * (item_bytes of the entries before it); the shard of
-// items lo .. of a devices-mode GPU starts lo * item_bytes_j into each slab.  The slab after an ATTENTION slab starts at the next
-// multiple of 16 bytes: attention items are H x R x T elements, often an odd count, and K7's vector stores need the alignment.
-std::vector<char*> slab_bases(const std::vector<TokenReq>& qs, char* out, size_t n, size_t lo) {
+// Layer-major output of a tokens call of T rows per item: entry j's slab of n items starts at n * (item_bytes of the entries before
+// it); the shard of items lo .. of a devices-mode GPU starts lo * item_bytes_j into each slab.  The slab after an ATTENTION slab
+// starts at the next multiple of 16 bytes: attention items are H x R x T elements, often an odd count, and K7's vector stores need
+// the alignment.
+std::vector<char*> slab_bases(const std::vector<TokenReq>& qs, const Tower& tw, int T, char* out, size_t n, size_t lo) {
     std::vector<char*> b;
     size_t off = 0;
     for (const TokenReq& q : qs) {
-        b.push_back(out + off + lo * q.item_bytes);
-        off += n * q.item_bytes;
+        const size_t ib = item_bytes(q, tw, T);
+        b.push_back(out + off + lo * ib);
+        off += n * ib;
         if (q.attn) off = (off + 15) / 16 * 16;
     }
     return b;
@@ -538,7 +527,7 @@ struct RowRing {
         if (!token_rows_tail(c, tw, nb, T, q, d)) return false;
         CK(cudaEventRecord(c->ev_ring_rows[s], c->stream));
         if (!drain(s)) return false;
-        const size_t bytes = (size_t)nb * q.item_bytes;
+        const size_t bytes = (size_t)nb * item_bytes(q, tw, T);
         CK(cudaStreamWaitEvent(c->copy_stream, c->ev_ring_rows[s], 0));
         CK(cudaMemcpyAsync(pinned ? dst : c->h_ring + s * slot, d, bytes, cudaMemcpyDeviceToHost, c->copy_stream));
         CK(cudaEventRecord(c->ev_ring_free[s], c->copy_stream));
@@ -1299,258 +1288,186 @@ bool clip_b200_text_encode_device(const struct clip_ctx* cctx, const void* d_ids
     return text_encode_impl(c, nullptr, nullptr, (const int32_t*)d_ids, (const int32_t*)d_lens, n, seq_len, nullptr, (float*)d_vec, normalize);
 }
 
-// ---- per-token hidden states ----------------------------------------------------------------------------------------------------
-// One GPU, host buffers: each micro-batch's inputs go up on the launch stream; the rows of every entry leave through the RowRing into
-// that entry's slab of the caller's buffer (bases[j] = item 0 of this call in slab j), so the whole output is never held on the device.
-static bool image_tokens_one(clip_ctx* c, const clip_image_f32* imgs, size_t n, const std::vector<TokenReq>& qs, const std::vector<char*>& bases,
-                             int H = 0, int W = 0, const char* who = "clip_b200_image_tokens") {
-    Tower& tw = c->vis;
+// ---- per-token hidden states: the ten clip_b200_*_tokens* forms -------------------------------------------------------------------
+// What one tokens call reads, as its public form received it.  Each form fills one and calls tokens_call, so every form checks its
+// arguments in the same order (include/clip_b200.h) and runs the same pass driver.
+struct TokensCall {
+    const char* who;                              // the public name, for messages
+    bool vision, host;                            // the tower; inputs and out in host memory (else device memory)
+    bool hw = false;                              // vision: any patch-multiple size, H x W given (device) or the images' own (host)
+    const clip_image_f32_batch* imgs = nullptr;   // vision, host: the images, n = imgs->size
+    const void* in = nullptr;                     // vision, device: NHWC f32 pixels; text: ids [n, seq_len]
+    size_t n = 0;
+    int H = 0, W = 0, seq_len = 0;
+    const int* layers = nullptr;                  // n_layers entries; a single-layer form passes its one (layer, flags)
+    const int* flags = nullptr;                   // NULL: 0 for every entry
+    int n_layers = 1;
+    bool list = false;                            // a *_layers form: n_layers and layers are checked, messages name the entry
+    int out_type = 0;
+    void* out = nullptr;
+};
+
+// One GPU, items lo .. hi of a checked call.  Per micro-batch: stage its inputs (host images go up one copy per image on the launch
+// stream into ws.pixels[0], device pixels are read in place, ids are copied into ws.ids), embed them, then token_stops; each entry's
+// rows go to its slab (bases[j] = item lo in slab j), through the RowRing for host memory, so the whole output is never held on the
+// device.
+static bool tokens_pass(clip_ctx* c, const TokensCall& a, const std::vector<TokenReq>& qs, size_t lo, size_t hi) {
+    Tower& tw = a.vision ? c->vis : c->txt;
     std::lock_guard<std::mutex> lk(c->mu);
     CK(cudaSetDevice(c->device));
     VisCall v;
-    int mb = 0;
-    if (!plan_call(c, H, W, v, mb, who)) return false;
+    int mb = tw.micro_batch, T = a.seq_len;
+    if (a.vision) {
+        if (!plan_call(c, a.H, a.W, v, mb, a.who)) return false;
+        T = v.T;
+    } else if (!ensure_ws(c, tw, tw.micro_batch, tw.n_ctx, false)) {
+        return false;
+    }
+    const size_t n = hi - lo;
     size_t n_chunks, chunk;
     chunking(n, mb, n_chunks, chunk);
-    size_t widest = 0;
-    for (const TokenReq& q : qs) widest = std::max(widest, q.item_bytes);
+    const std::vector<char*> bases = slab_bases(qs, tw, T, (char*)a.out, a.n, lo);
     RowRing ring{c};
-    if (!ring.init(chunk * widest, bases[0])) return false;
+    if (a.host) {
+        size_t widest = 0;
+        for (const TokenReq& q : qs) widest = std::max(widest, item_bytes(q, tw, T));
+        if (!ring.init(chunk * widest, bases[0])) return false;
+    }
     const size_t per = v.per();
     CK(cudaEventRecord(c->ev_t0, c->stream));
     for (size_t i0 = 0; i0 < n; i0 += chunk) {
         const int nb = (int)std::min(chunk, n - i0);
-        for (int j = 0; j < nb; j++)
-            CK(cudaMemcpyAsync(tw.ws.pixels[0] + (size_t)j * per, imgs[i0 + j].data, per * 4, cudaMemcpyHostToDevice, c->stream));
-        if (!vision_tokens(c, tw.ws.pixels[0], nb, v, qs, [&](int j) { return ring.put(tw, nb, v.T, qs[j], bases[j] + i0 * qs[j].item_bytes); }))
-            return false;
+        const size_t i = lo + i0;     // the call's index of the micro-batch's first item
+        if (a.vision && a.host) {
+            for (int j = 0; j < nb; j++)
+                CK(cudaMemcpyAsync(tw.ws.pixels[0] + (size_t)j * per, a.imgs->data[i + j].data, per * 4, cudaMemcpyHostToDevice, c->stream));
+            if (!vision_embed(c, tw.ws.pixels[0], nb, v)) return false;
+        } else if (a.vision) {
+            if (!vision_embed(c, (const float*)a.in + i * per, nb, v)) return false;
+        } else {
+            CK(cudaMemcpyAsync(tw.ws.ids, (const int32_t*)a.in + i * T, (size_t)nb * T * 4,
+                               a.host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, c->stream));
+            { Scope s(c, K_OTHER); launch_text_embed(tw.ws.ids, tw.tok, tw.pos, nb, T, tw.hidden, tw.n_vocab, tw.ws.x, c->stream); }
+        }
+        auto emit = [&](int j) {
+            char* dst = bases[j] + i0 * item_bytes(qs[j], tw, T);
+            return a.host ? ring.put(tw, nb, T, qs[j], dst) : token_rows_tail(c, tw, nb, T, qs[j], dst);
+        };
+        if (!token_stops(c, tw, nb, T, !a.vision, qs, emit)) return false;
     }
-    if (!ring.close()) return false;
+    if (a.host && !ring.close()) return false;
     CK(cudaEventRecord(c->ev_t1, c->stream));
     return sync_and_time(c) && ring.drain_all();
 }
 
-// n images of H x W (0 x 0: the model's size) resident at d_pixels -> the slabs at bases (device)
-static bool image_tokens_device_impl(clip_ctx* c, const float* d_pixels, size_t n, const std::vector<TokenReq>& qs, const std::vector<char*>& bases,
-                                     int H, int W, const char* who) {
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    VisCall v;
-    int mb = 0;
-    if (!plan_call(c, H, W, v, mb, who)) return false;
-    size_t n_chunks, chunk;
-    chunking(n, mb, n_chunks, chunk);
-    const size_t per = v.per();
-    CK(cudaEventRecord(c->ev_t0, c->stream));
-    for (size_t i0 = 0; i0 < n; i0 += chunk) {
-        const int nb = (int)std::min(chunk, n - i0);
-        auto emit = [&](int j) { return token_rows_tail(c, c->vis, nb, v.T, qs[j], bases[j] + i0 * qs[j].item_bytes); };
-        if (!vision_tokens(c, d_pixels + i0 * per, nb, v, qs, emit)) return false;
-    }
-    CK(cudaEventRecord(c->ev_t1, c->stream));
-    return sync_and_time(c);
-}
-
-// The entries of a multi-layer call, each checked and resolved by token_request as the single-layer call would be; the message of a
-// refused entry names its index.
-static bool token_requests(const clip_ctx* c, bool vision, const int* layers, const int* flags, int n_layers, int out_type, int T,
-                           std::vector<TokenReq>& qs, const char* who) {
-    if (!(vision ? c->vis : c->txt).present) { set_err(std::string(who) + ": this model has no " + (vision ? "vision" : "text") + " encoder"); return false; }
-    if (n_layers < 1 || n_layers > CLIP_B200_TOKENS_MAX_LAYERS) {
-        set_err(std::string(who) + ": n_layers must be in [1, " + std::to_string(CLIP_B200_TOKENS_MAX_LAYERS) + "], not " + std::to_string(n_layers));
+// Every tokens form: the arguments checked in one order, the first fault refused (include/clip_b200.h), then the pass; devices mode
+// shards the host forms' items over the GPUs, each writing its items into every slab.
+static bool tokens_call(const clip_ctx* cctx, TokensCall a) {
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    const std::string who = a.who;
+    if (!c) { set_err(who + ": null context"); return false; }
+    const Tower& tw = a.vision ? c->vis : c->txt;
+    if (!tw.present) { set_err(who + ": this model has no " + (a.vision ? "vision" : "text") + " encoder"); return false; }
+    if (a.hw && !a.host && !check_hw_size(c, a.H, a.W, a.who)) return false;
+    if (a.list && (a.n_layers < 1 || a.n_layers > CLIP_B200_TOKENS_MAX_LAYERS)) {
+        set_err(who + ": n_layers must be in [1, " + std::to_string(CLIP_B200_TOKENS_MAX_LAYERS) + "], not " + std::to_string(a.n_layers));
         return false;
     }
-    if (!layers) { set_err(std::string(who) + ": null layers"); return false; }
-    qs.assign((size_t)n_layers, TokenReq());
-    for (int j = 0; j < n_layers; j++) {
-        const std::string w = std::string(who) + ": entry " + std::to_string(j);
-        if (!token_request(c, vision, layers[j], flags ? flags[j] : 0, out_type, T, qs[j], w.c_str())) return false;
+    if (!a.layers) { set_err(who + ": null layers"); return false; }
+    std::vector<TokenReq> qs((size_t)a.n_layers);
+    for (int j = 0; j < a.n_layers; j++) {
+        const std::string w = a.list ? who + ": entry " + std::to_string(j) : who;
+        if (!token_request(c, a.vision, a.layers[j], a.flags ? a.flags[j] : 0, a.out_type, qs[j], w.c_str())) return false;
     }
-    return true;
-}
-
-// host image forms, one layer or several: shard over the GPUs in devices mode, each writing its items into every slab
-static bool image_tokens_host(clip_ctx* c, const clip_image_f32_batch* imgs, const std::vector<TokenReq>& qs, char* out, int H, int W, const char* who) {
-    const size_t n = imgs->size;
-    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
-        // devices mode: contiguous shards, every GPU copies its slice of the rows into the caller's buffer
-        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
-            return hi == lo || image_tokens_one(r, imgs->data + lo, hi - lo, qs, slab_bases(qs, out, n, lo), H, W, who);
-        });
+    if (a.imgs) a.n = a.imgs->size;
+    if (a.n == 0) return true;
+    if (!a.vision && (a.seq_len < 1 || a.seq_len > tw.n_ctx)) { set_err(who + ": seq_len must be in [1, context_length]"); return false; }
+    if (!a.out || (!a.in && !a.imgs)) {
+        set_err(who + (!a.host ? ": null device pointer" : a.vision ? ": null output" : ": null pointer"));
+        return false;
     }
-    return image_tokens_one(c, imgs->data, n, qs, slab_bases(qs, out, n, 0), H, W, who);
+    if (a.imgs && !a.hw && !check_images(c, a.imgs->data, a.n, a.who)) return false;
+    if (a.imgs && a.hw && !check_images_hw(c, a.imgs->data, a.n, a.H, a.W, a.who)) return false;
+    if (a.host && c->replicas.size() > 1 && a.n >= c->replicas.size())
+        return for_each_replica(c, a.n, [&](clip_ctx* r, int, size_t lo, size_t hi) { return hi == lo || tokens_pass(r, a, qs, lo, hi); });
+    return tokens_pass(c, a, qs, 0, a.n);
 }
 
 bool clip_b200_image_tokens(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, int layer, int flags, int out_type, void* out) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    TokenReq q;
-    if (!c) { set_err("clip_b200_image_tokens: null context"); return false; }
-    if (!token_request(c, true, layer, flags, out_type, c->vis.T, q, "clip_b200_image_tokens")) return false;
-    const size_t n = imgs ? imgs->size : 0;
-    if (n == 0) return true;
-    if (!out) { set_err("clip_b200_image_tokens: null output"); return false; }
-    if (!check_images(c, imgs->data, n, "clip_b200_image_tokens")) return false;
-    return image_tokens_host(c, imgs, {q}, (char*)out, 0, 0, "clip_b200_image_tokens");
+    TokensCall a{"clip_b200_image_tokens", true, true};
+    a.imgs = imgs;
+    a.layers = &layer; a.flags = &flags; a.out_type = out_type; a.out = out;
+    return tokens_call(cctx, a);
 }
 
 bool clip_b200_image_tokens_device(const struct clip_ctx* cctx, const void* d_pixels, size_t n, int layer, int flags, int out_type, void* d_out) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    TokenReq q;
-    if (!c) { set_err("clip_b200_image_tokens_device: null context"); return false; }
-    if (!token_request(c, true, layer, flags, out_type, c->vis.T, q, "clip_b200_image_tokens_device")) return false;
-    if (n == 0) return true;
-    if (!d_pixels || !d_out) { set_err("clip_b200_image_tokens_device: null device pointer"); return false; }
-    return image_tokens_device_impl(c, (const float*)d_pixels, n, {q}, {(char*)d_out}, 0, 0, "clip_b200_image_tokens_device");
+    TokensCall a{"clip_b200_image_tokens_device", true, false};
+    a.in = d_pixels; a.n = n;
+    a.layers = &layer; a.flags = &flags; a.out_type = out_type; a.out = d_out;
+    return tokens_call(cctx, a);
 }
 
 bool clip_b200_image_tokens_hw(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, int layer, int flags, int out_type, void* out) {
-    const char* who = "clip_b200_image_tokens_hw";
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    TokenReq q;
-    if (!c) { set_err(std::string(who) + ": null context"); return false; }
-    if (!c->has_vision) { set_err(std::string(who) + ": this model has no vision encoder"); return false; }
-    const size_t n = imgs ? imgs->size : 0;
-    if (n == 0) return token_request(c, true, layer, flags, out_type, c->vis.T, q, who);
-    if (!out) { set_err(std::string(who) + ": null output"); return false; }
-    int H = 0, W = 0;
-    if (!check_images_hw(c, imgs->data, n, H, W, who)) return false;
-    if (!token_request(c, true, layer, flags, out_type, (H / c->vis.patch) * (W / c->vis.patch) + 1, q, who)) return false;
-    return image_tokens_host(c, imgs, {q}, (char*)out, H, W, who);
+    TokensCall a{"clip_b200_image_tokens_hw", true, true, true};
+    a.imgs = imgs;
+    a.layers = &layer; a.flags = &flags; a.out_type = out_type; a.out = out;
+    return tokens_call(cctx, a);
 }
 
 bool clip_b200_image_tokens_device_hw(const struct clip_ctx* cctx, const void* d_pixels, size_t n, int height, int width, int layer, int flags,
                                       int out_type, void* d_out) {
-    const char* who = "clip_b200_image_tokens_device_hw";
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    TokenReq q;
-    if (!c) { set_err(std::string(who) + ": null context"); return false; }
-    if (!c->has_vision) { set_err(std::string(who) + ": this model has no vision encoder"); return false; }
-    if (!check_hw_size(c, height, width, who)) return false;
-    if (!token_request(c, true, layer, flags, out_type, (height / c->vis.patch) * (width / c->vis.patch) + 1, q, who)) return false;
-    if (n == 0) return true;
-    if (!d_pixels || !d_out) { set_err(std::string(who) + ": null device pointer"); return false; }
-    return image_tokens_device_impl(c, (const float*)d_pixels, n, {q}, {(char*)d_out}, height, width, who);
-}
-
-// n padded sequences of seq_len ids, on the host (h_ids) or the device (d_ids) -> the slabs at bases, host memory (through the
-// RowRing) when `host_out`, else device memory
-static bool text_tokens_impl(clip_ctx* c, const int32_t* h_ids, const int32_t* d_ids, size_t n, int seq_len, const std::vector<TokenReq>& qs,
-                             const std::vector<char*>& bases, bool host_out) {
-    Tower& tw = c->txt;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    if (!ensure_ws(c, tw, tw.micro_batch, tw.n_ctx, false)) return false;
-    size_t n_chunks, chunk;
-    chunking(n, tw.micro_batch, n_chunks, chunk);
-    size_t widest = 0;
-    for (const TokenReq& q : qs) widest = std::max(widest, q.item_bytes);
-    RowRing ring{c};
-    if (host_out && !ring.init(chunk * widest, bases[0])) return false;
-    CK(cudaEventRecord(c->ev_t0, c->stream));
-    for (size_t i0 = 0; i0 < n; i0 += chunk) {
-        const int nb = (int)std::min(chunk, n - i0);
-        const size_t id_bytes = (size_t)nb * seq_len * 4;
-        if (h_ids) CK(cudaMemcpyAsync(tw.ws.ids, h_ids + i0 * seq_len, id_bytes, cudaMemcpyHostToDevice, c->stream));
-        else CK(cudaMemcpyAsync(tw.ws.ids, d_ids + i0 * seq_len, id_bytes, cudaMemcpyDeviceToDevice, c->stream));
-        auto emit = [&](int j) {
-            char* dst = bases[j] + i0 * qs[j].item_bytes;
-            return host_out ? ring.put(tw, nb, seq_len, qs[j], dst) : token_rows_tail(c, tw, nb, seq_len, qs[j], dst);
-        };
-        if (!text_tokens(c, nb, seq_len, qs, emit)) return false;
-    }
-    if (host_out && !ring.close()) return false;
-    CK(cudaEventRecord(c->ev_t1, c->stream));
-    return sync_and_time(c) && ring.drain_all();
-}
-
-// host text forms, one layer or several: shard over the GPUs in devices mode, each writing its sequences into every slab
-static bool text_tokens_host(clip_ctx* c, const int32_t* ids, size_t n, int seq_len, const std::vector<TokenReq>& qs, char* out) {
-    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
-        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
-            return hi == lo || text_tokens_impl(r, ids + lo * seq_len, nullptr, hi - lo, seq_len, qs, slab_bases(qs, out, n, lo), true);
-        });
-    }
-    return text_tokens_impl(c, ids, nullptr, n, seq_len, qs, slab_bases(qs, out, n, 0), true);
+    TokensCall a{"clip_b200_image_tokens_device_hw", true, false, true};
+    a.in = d_pixels; a.n = n; a.H = height; a.W = width;
+    a.layers = &layer; a.flags = &flags; a.out_type = out_type; a.out = d_out;
+    return tokens_call(cctx, a);
 }
 
 bool clip_b200_text_tokens(const struct clip_ctx* cctx, const int32_t* ids, size_t n, int seq_len, int layer, int flags, int out_type, void* out) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    TokenReq q;
-    if (!c) { set_err("clip_b200_text_tokens: null context"); return false; }
-    if (!token_request(c, false, layer, flags, out_type, seq_len, q, "clip_b200_text_tokens")) return false;
-    if (n == 0) return true;
-    if (seq_len < 1 || seq_len > c->txt.n_ctx) { set_err("clip_b200_text_tokens: seq_len must be in [1, context_length]"); return false; }
-    if (!ids || !out) { set_err("clip_b200_text_tokens: null pointer"); return false; }
-    return text_tokens_host(c, ids, n, seq_len, {q}, (char*)out);
+    TokensCall a{"clip_b200_text_tokens", false, true};
+    a.in = ids; a.n = n; a.seq_len = seq_len;
+    a.layers = &layer; a.flags = &flags; a.out_type = out_type; a.out = out;
+    return tokens_call(cctx, a);
 }
 
 bool clip_b200_text_tokens_device(const struct clip_ctx* cctx, const void* d_ids, size_t n, int seq_len, int layer, int flags, int out_type,
                                   void* d_out) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    TokenReq q;
-    if (!c) { set_err("clip_b200_text_tokens_device: null context"); return false; }
-    if (!token_request(c, false, layer, flags, out_type, seq_len, q, "clip_b200_text_tokens_device")) return false;
-    if (n == 0) return true;
-    if (seq_len < 1 || seq_len > c->txt.n_ctx) { set_err("clip_b200_text_tokens_device: seq_len must be in [1, context_length]"); return false; }
-    if (!d_ids || !d_out) { set_err("clip_b200_text_tokens_device: null device pointer"); return false; }
-    return text_tokens_impl(c, nullptr, (const int32_t*)d_ids, n, seq_len, {q}, {(char*)d_out}, false);
+    TokensCall a{"clip_b200_text_tokens_device", false, false};
+    a.in = d_ids; a.n = n; a.seq_len = seq_len;
+    a.layers = &layer; a.flags = &flags; a.out_type = out_type; a.out = d_out;
+    return tokens_call(cctx, a);
 }
 
 // ---- several layers from one forward pass (clip_b200_*_tokens_layers) ------------------------------------------------------------
 bool clip_b200_image_tokens_layers(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, const int* layers, const int* flags,
                                    int n_layers, int out_type, void* out) {
-    const char* who = "clip_b200_image_tokens_layers";
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    std::vector<TokenReq> qs;
-    if (!c) { set_err(std::string(who) + ": null context"); return false; }
-    const size_t n = imgs ? imgs->size : 0;
-    if (n == 0) return token_requests(c, true, layers, flags, n_layers, out_type, c->vis.T, qs, who);
-    if (!c->has_vision) { set_err(std::string(who) + ": this model has no vision encoder"); return false; }
-    if (!out) { set_err(std::string(who) + ": null output"); return false; }
-    int H = 0, W = 0;
-    if (!check_images_hw(c, imgs->data, n, H, W, who)) return false;
-    if (!token_requests(c, true, layers, flags, n_layers, out_type, (H / c->vis.patch) * (W / c->vis.patch) + 1, qs, who)) return false;
-    return image_tokens_host(c, imgs, qs, (char*)out, H, W, who);
+    TokensCall a{"clip_b200_image_tokens_layers", true, true, true};
+    a.imgs = imgs;
+    a.layers = layers; a.flags = flags; a.n_layers = n_layers; a.list = true; a.out_type = out_type; a.out = out;
+    return tokens_call(cctx, a);
 }
 
 bool clip_b200_image_tokens_layers_device(const struct clip_ctx* cctx, const void* d_pixels, size_t n, int height, int width, const int* layers,
                                           const int* flags, int n_layers, int out_type, void* d_out) {
-    const char* who = "clip_b200_image_tokens_layers_device";
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    std::vector<TokenReq> qs;
-    if (!c) { set_err(std::string(who) + ": null context"); return false; }
-    if (!c->has_vision) { set_err(std::string(who) + ": this model has no vision encoder"); return false; }
-    if (!check_hw_size(c, height, width, who)) return false;
-    if (!token_requests(c, true, layers, flags, n_layers, out_type, (height / c->vis.patch) * (width / c->vis.patch) + 1, qs, who)) return false;
-    if (n == 0) return true;
-    if (!d_pixels || !d_out) { set_err(std::string(who) + ": null device pointer"); return false; }
-    return image_tokens_device_impl(c, (const float*)d_pixels, n, qs, slab_bases(qs, (char*)d_out, n, 0), height, width, who);
+    TokensCall a{"clip_b200_image_tokens_layers_device", true, false, true};
+    a.in = d_pixels; a.n = n; a.H = height; a.W = width;
+    a.layers = layers; a.flags = flags; a.n_layers = n_layers; a.list = true; a.out_type = out_type; a.out = d_out;
+    return tokens_call(cctx, a);
 }
 
 bool clip_b200_text_tokens_layers(const struct clip_ctx* cctx, const int32_t* ids, size_t n, int seq_len, const int* layers, const int* flags,
                                   int n_layers, int out_type, void* out) {
-    const char* who = "clip_b200_text_tokens_layers";
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    std::vector<TokenReq> qs;
-    if (!c) { set_err(std::string(who) + ": null context"); return false; }
-    if (!token_requests(c, false, layers, flags, n_layers, out_type, seq_len, qs, who)) return false;
-    if (n == 0) return true;
-    if (seq_len < 1 || seq_len > c->txt.n_ctx) { set_err(std::string(who) + ": seq_len must be in [1, context_length]"); return false; }
-    if (!ids || !out) { set_err(std::string(who) + ": null pointer"); return false; }
-    return text_tokens_host(c, ids, n, seq_len, qs, (char*)out);
+    TokensCall a{"clip_b200_text_tokens_layers", false, true};
+    a.in = ids; a.n = n; a.seq_len = seq_len;
+    a.layers = layers; a.flags = flags; a.n_layers = n_layers; a.list = true; a.out_type = out_type; a.out = out;
+    return tokens_call(cctx, a);
 }
 
 bool clip_b200_text_tokens_layers_device(const struct clip_ctx* cctx, const void* d_ids, size_t n, int seq_len, const int* layers, const int* flags,
                                          int n_layers, int out_type, void* d_out) {
-    const char* who = "clip_b200_text_tokens_layers_device";
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    std::vector<TokenReq> qs;
-    if (!c) { set_err(std::string(who) + ": null context"); return false; }
-    if (!token_requests(c, false, layers, flags, n_layers, out_type, seq_len, qs, who)) return false;
-    if (n == 0) return true;
-    if (seq_len < 1 || seq_len > c->txt.n_ctx) { set_err(std::string(who) + ": seq_len must be in [1, context_length]"); return false; }
-    if (!d_ids || !d_out) { set_err(std::string(who) + ": null device pointer"); return false; }
-    return text_tokens_impl(c, nullptr, (const int32_t*)d_ids, n, seq_len, qs, slab_bases(qs, (char*)d_out, n, 0), false);
+    TokensCall a{"clip_b200_text_tokens_layers_device", false, false};
+    a.in = d_ids; a.n = n; a.seq_len = seq_len;
+    a.layers = layers; a.flags = flags; a.n_layers = n_layers; a.list = true; a.out_type = out_type; a.out = d_out;
+    return tokens_call(cctx, a);
 }
 
 float clip_similarity_score(const float* vec1, const float* vec2, const int vec_dim) {

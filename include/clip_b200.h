@@ -186,6 +186,11 @@ bool clip_b200_text_encode_device(const struct clip_ctx * ctx, const void * d_id
  * of the caller's model; causal attention keeps the rows before the padding independent of it).
  * Refused with a message in clip_b200_last_error(): a bad layer, unknown flag bits or out_type, NO_CLS on text, NORMALIZE without
  * PROJECT, a model without the tower.  n == 0 returns true.
+ * Every tokens form (these four, the *_hw and the *_tokens_layers forms below) checks its arguments in one order and reports the
+ * first fault: 1. a null context; 2. the tower; 3. height x width where they are arguments (the device *_hw and *_layers forms);
+ * 4. the request: n_layers, NULL layers, then each entry in order; 5. n == 0 returns true here; 6. seq_len in [1, context_length];
+ * 7. null input or output pointers; 8. the host images: image_size x image_size for clip_b200_image_tokens, one patch-multiple size
+ * for the host *_hw and *_layers forms.
  * Host variants: devices mode (CLIP_B200_DEVICES) shards the batch like clip_image_batch_encode, each GPU copying its slice into out;
  * each micro-batch's rows are copied straight into out (the whole output is never held on the device).  Device variants: pointers on
  * the context's GPU, d_out 16-byte aligned (any cudaMalloc pointer is). */
