@@ -496,7 +496,7 @@ bool host_ptr_is_pinned(const void* p);
 // s on the launch stream; the copy stream takes it to the host once K7 is done (ev_ring_rows[s]), so the D2H of one stop runs under
 // the blocks of the next, and the tail into slot s first waits for that slot's previous D2H (ev_ring_free[s]).  A pinned `out`
 // receives the D2H directly.  A pageable one cannot take an async D2H, so the rows land in a pinned bounce slot (c->h_ring) that host
-// threads drain into `out` before that slot is copied into again (image_batch_encode_one's arena, the other way round).
+// threads drain into `out` before that slot is copied into again (encode_pass's arena for host images, the other way round).
 // Caller holds c->mu and has set the device.
 struct RowRing {
     clip_ctx* c;
@@ -650,24 +650,6 @@ bool check_hw_size(const clip_ctx* c, int H, int W, const char* who) {
     return true;
 }
 
-bool image_encode_device_locked(clip_ctx* c, const float* d_pixels, size_t n, float* d_vec, bool normalize, int H = 0, int W = 0,
-                                const char* who = "clip_b200_image_encode_device") {
-    Tower& tw = c->vis;
-    VisCall v;
-    int mb = 0;
-    if (!plan_call(c, H, W, v, mb, who)) return false;
-    size_t n_chunks, chunk;
-    chunking(n, mb, n_chunks, chunk);
-    const size_t per = v.per();
-    CK(cudaEventRecord(c->ev_t0, c->stream));
-    for (size_t i0 = 0; i0 < n; i0 += chunk) {
-        const int nb = (int)std::min(chunk, n - i0);
-        if (!vision_forward(c, d_pixels + i0 * per, nb, v, d_vec + i0 * tw.proj, normalize)) return false;
-    }
-    CK(cudaEventRecord(c->ev_t1, c->stream));
-    return true;
-}
-
 // ---- devices mode helper: f(replica, r, lo, hi) on one host thread per GPU, contiguous balanced shards of n items --------------
 template <class F>
 bool for_each_replica(clip_ctx* c, size_t n, F f) {
@@ -688,6 +670,18 @@ bool for_each_replica(clip_ctx* c, size_t n, F f) {
     cudaSetDevice(c->device);
     for (int r = 0; r < w; r++)
         if (!ok[r]) { set_err("device " + std::to_string(c->replicas[r]->device) + ": " + errs[r]); return false; }
+    return true;
+}
+
+bool ranks_mode(const clip_ctx* c) { return c->replicas.size() <= 1 && c->dist.comm && c->dist.world > 1; }
+
+// ranks mode: every rank encodes ITS n_local items and ends with ALL world * n_local embeddings, rank-major.  The last kernel of
+// the tower (K5 l2norm) writes straight into this rank's slot of the gather buffer; the all-gather runs in place on the launch stream.
+bool gather_in_place(clip_ctx* c, float* d_all, size_t n_local, int d) {
+    if (!ranks_mode(c)) return true;
+    std::string e;
+    const size_t bytes = n_local * (size_t)d * 4;
+    if (!dist_all_gather(c->dist, (const char*)d_all + (size_t)c->dist.rank * bytes, d_all, bytes, c->stream, e)) { set_err(e); return false; }
     return true;
 }
 
@@ -984,157 +978,7 @@ void clip_image_batch_preprocess(const struct clip_ctx* ctx, const int n_threads
     for (auto& t : th) t.join();
 }
 
-// ---- N1 (SURVEY.md section 8f): preprocess on the device -------------------------------------------------------------------------
-// Shared driver: micro-batches of raw u8 images -> pixel staging buffer (preprocess.cu) -> optional vision forward.
-static bool preprocess_chunks(clip_ctx* c, const clip_image_u8* imgs, size_t n, float* h_pixels_out, float* vec, bool normalize) {
-    Tower& tw = c->vis;
-    if (!ensure_ws(c, tw, tw.micro_batch, tw.T, true)) return false;
-    if (vec && !ensure_out(c, n * tw.proj)) return false;
-    size_t n_chunks, chunk;
-    chunking(n, tw.micro_batch, n_chunks, chunk);
-    const size_t per = (size_t)tw.image_size * tw.image_size * 3;
-    CK(cudaEventRecord(c->ev_t0, c->stream));
-    size_t ci = 0;
-    for (size_t i0 = 0; i0 < n; i0 += chunk, ci++) {
-        const int nb = (int)std::min(chunk, n - i0), b = (int)(ci & 1);
-        if (ci >= 2) CK(cudaEventSynchronize(c->ev_consumed[b]));      // arena b is rewritten on the host below
-        std::string err;
-        if (!preprocess_device(c, imgs + i0, nb, b, tw.ws.pixels[b], c->copy_stream, c->ev_copied[b], c->stream, err)) { set_err(err); return false; }
-        if (h_pixels_out) CK(cudaMemcpyAsync(h_pixels_out + i0 * per, tw.ws.pixels[b], (size_t)nb * per * 4, cudaMemcpyDeviceToHost, c->stream));
-        if (vec && !vision_forward(c, tw.ws.pixels[b], nb, native_call(tw), c->d_out + i0 * tw.proj, normalize)) return false;
-        CK(cudaEventRecord(c->ev_consumed[b], c->stream));
-    }
-    CK(cudaEventRecord(c->ev_t1, c->stream));
-    if (vec) CK(cudaMemcpyAsync(vec, c->d_out, n * tw.proj * 4, cudaMemcpyDeviceToHost, c->stream));
-    return sync_and_time(c);
-}
-
-bool clip_b200_image_batch_encode_u8(const struct clip_ctx* cctx, const struct clip_image_u8_batch* imgs, float* vec, const bool normalize) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c || !c->has_vision) { set_err("no vision encoder"); return false; }
-    if (!imgs || imgs->size == 0) return true;
-    if (c->replicas.size() > 1 && imgs->size >= c->replicas.size()) {
-        const int d = c->vis.proj;
-        return for_each_replica(c, imgs->size, [&](clip_ctx* r, int, size_t lo, size_t hi) {
-            if (hi == lo) return true;
-            std::lock_guard<std::mutex> lk(r->mu);
-            CK(cudaSetDevice(r->device));
-            return preprocess_chunks(r, imgs->data + lo, hi - lo, nullptr, vec + lo * d, normalize);
-        });
-    }
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    return preprocess_chunks(c, imgs->data, imgs->size, nullptr, vec, normalize);
-}
-
-bool clip_b200_image_batch_preprocess_device(const struct clip_ctx* cctx, const struct clip_image_u8_batch* in, struct clip_image_f32_batch* out) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c || !c->has_vision) { set_err("no vision encoder"); return false; }
-    out->size = in->size;
-    const size_t n = in->size;
-    if (n == 0) return true;
-    const int S = c->vhp.image_size;
-    const size_t per = (size_t)3 * S * S;
-    std::vector<float> host(n * per);
-    {
-        std::lock_guard<std::mutex> lk(c->mu);
-        CK(cudaSetDevice(c->device));
-        if (!preprocess_chunks(c, in->data, n, host.data(), nullptr, false)) return false;
-    }
-    for (size_t i = 0; i < n; i++) {        // same ownership convention as clip_image_preprocess: data is new[]-allocated here
-        out->data[i].nx = S; out->data[i].ny = S; out->data[i].size = per;
-        out->data[i].data = new float[per];
-        memcpy(out->data[i].data, host.data() + i * per, per * 4);
-    }
-    return true;
-}
-
-bool clip_b200_image_encode_device(const struct clip_ctx* cctx, const void* d_pixels, size_t n, void* d_vec, bool normalize) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c || !c->has_vision) { set_err("no vision encoder"); return false; }
-    if (n == 0) return true;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    if (!image_encode_device_locked(c, (const float*)d_pixels, n, (float*)d_vec, normalize)) return false;
-    return sync_and_time(c);
-}
-
-bool clip_b200_image_encode_device_hw(const struct clip_ctx* cctx, const void* d_pixels, size_t n, int height, int width, void* d_vec,
-                                      bool normalize) {
-    const char* who = "clip_b200_image_encode_device_hw";
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c || !c->has_vision) { set_err(std::string(who) + ": this model has no vision encoder"); return false; }
-    if (!check_hw_size(c, height, width, who)) return false;
-    if (n == 0) return true;
-    if (!d_pixels || !d_vec) { set_err(std::string(who) + ": null device pointer"); return false; }
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    if (!image_encode_device_locked(c, (const float*)d_pixels, n, (float*)d_vec, normalize, height, width, who)) return false;
-    return sync_and_time(c);
-}
-
-// One GPU: n host images -> embeddings at d_vec (device, may be null) and / or vec (host, may be null).  Host pixels travel on the
-// copy stream, double-buffered against the kernels of the previous micro-batch.  Pinned / registered caller buffers are copied
-// directly; PAGEABLE ones (what clip_image_preprocess returns: new float[]) are first gathered into a pinned arena by host threads,
-// in sub-batches so the H2D of sub-batch k overlaps the memcpy of k+1 -- a pageable cudaMemcpyAsync would be staged synchronously
-// by the driver, one 602 KB image at a time.
-static bool image_batch_encode_one(clip_ctx* c, int n_threads, const clip_image_f32* imgs, size_t n, float* vec, float* d_vec, bool normalize,
-                                   bool sync, int H = 0, int W = 0, const char* who = "clip_image_batch_encode") {
-    Tower& tw = c->vis;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    VisCall v;
-    int mb = 0;
-    if (!plan_call(c, H, W, v, mb, who)) return false;
-    if (!d_vec) { if (!ensure_out(c, n * tw.proj)) return false; d_vec = c->d_out; }
-    const std::vector<size_t> bounds = host_chunk_bounds(n, mb);
-    const size_t per = v.per();
-    bool pinned = true;
-    for (size_t i = 0; i < n && pinned; i++) pinned = host_ptr_is_pinned(imgs[i].data);
-    if (!pinned && c->h_stage_cap < (size_t)mb * per) {
-        for (int b = 0; b < 2; b++) {
-            if (c->h_stage[b]) { cudaFreeHost(c->h_stage[b]); c->h_stage[b] = nullptr; }
-            CK(cudaMallocHost((void**)&c->h_stage[b], (size_t)mb * per * 4));
-        }
-        c->h_stage_cap = (size_t)mb * per;
-    }
-    const int nt = std::max(1, std::min({std::max(n_threads, 4), 16, (int)std::thread::hardware_concurrency()}));
-    CK(cudaEventRecord(c->ev_t0, c->stream));
-    for (size_t ci = 0; ci + 1 < bounds.size(); ci++) {
-        const size_t i0 = bounds[ci];
-        const int nb = (int)(bounds[ci + 1] - i0), b = (int)(ci & 1);
-        if (ci >= 2) CK(cudaStreamWaitEvent(c->copy_stream, c->ev_consumed[b], 0));
-        if (pinned) {
-            for (int j = 0; j < nb; j++)
-                CK(cudaMemcpyAsync(tw.ws.pixels[b] + (size_t)j * per, imgs[i0 + j].data, per * 4, cudaMemcpyHostToDevice, c->copy_stream));
-        } else {
-            if (ci >= 2) CK(cudaEventSynchronize(c->ev_copied[b]));      // the arena's previous H2D has left the host buffer
-            const int sub = 32;
-            for (int j0 = 0; j0 < nb; j0 += sub) {
-                const int ns = std::min(sub, nb - j0);
-                float* dst = c->h_stage[b] + (size_t)j0 * per;
-                const clip_image_f32* src = imgs + i0 + j0;
-                const int t_use = std::min(nt, ns);
-                if (t_use <= 1) { for (int j = 0; j < ns; j++) memcpy(dst + (size_t)j * per, src[j].data, per * 4); }
-                else {
-                    std::vector<std::thread> th;
-                    for (int t = 0; t < t_use; t++)
-                        th.emplace_back([=]() { for (int j = t; j < ns; j += t_use) memcpy(dst + (size_t)j * per, src[j].data, per * 4); });
-                    for (auto& t : th) t.join();
-                }
-                CK(cudaMemcpyAsync(tw.ws.pixels[b] + (size_t)j0 * per, dst, (size_t)ns * per * 4, cudaMemcpyHostToDevice, c->copy_stream));
-            }
-        }
-        CK(cudaEventRecord(c->ev_copied[b], c->copy_stream));
-        CK(cudaStreamWaitEvent(c->stream, c->ev_copied[b], 0));
-        if (!vision_forward(c, tw.ws.pixels[b], nb, v, d_vec + i0 * tw.proj, normalize)) return false;
-        CK(cudaEventRecord(c->ev_consumed[b], c->stream));
-    }
-    CK(cudaEventRecord(c->ev_t1, c->stream));
-    if (vec) CK(cudaMemcpyAsync(vec, d_vec, n * tw.proj * 4, cudaMemcpyDeviceToHost, c->stream));
-    return sync ? sync_and_time(c) : true;
-}
-
+// ---- pooled embeddings: the clip_*_encode* forms and the u8 forms ----------------------------------------------------------------
 static bool check_images(clip_ctx* c, const clip_image_f32* imgs, size_t n, const char* who) {
     for (size_t i = 0; i < n; i++)
         if (imgs[i].nx != c->vis.image_size || imgs[i].ny != c->vis.image_size || !imgs[i].data) { set_err(std::string(who) + ": every image must be image_size x image_size"); return false; }
@@ -1155,84 +999,22 @@ static bool check_images_hw(clip_ctx* c, const clip_image_f32* imgs, size_t n, i
     return check_hw_size(c, H, W, who);
 }
 
-bool clip_image_batch_encode(const struct clip_ctx* cctx, const int n_threads, const struct clip_image_f32_batch* imgs, float* vec,
-                             const bool normalize) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c || !c->has_vision) { printf("This gguf file seems to have no vision encoder\n"); return false; }
-    const size_t n = imgs->size;
-    if (n == 0) return true;
-    if (!check_images(c, imgs->data, n, "clip_image_batch_encode")) return false;
-    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
-        // devices mode: contiguous shards, every GPU copies its slice of the result straight into the caller's vec (no exchange needed)
-        const int d = c->vis.proj;
-        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
-            return hi == lo || image_batch_encode_one(r, n_threads, imgs->data + lo, hi - lo, vec + lo * d, nullptr, normalize, true);
-        });
-    }
-    return image_batch_encode_one(c, n_threads, imgs->data, n, vec, nullptr, normalize, true);
-}
-
-bool clip_b200_image_batch_encode_hw(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, float* vec, bool normalize) {
-    const char* who = "clip_b200_image_batch_encode_hw";
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c || !c->has_vision) { set_err(std::string(who) + ": this model has no vision encoder"); return false; }
-    const size_t n = imgs ? imgs->size : 0;
-    if (n == 0) return true;
-    if (!vec) { set_err(std::string(who) + ": null output"); return false; }
-    int H = 0, W = 0;
-    if (!check_images_hw(c, imgs->data, n, H, W, who)) return false;
-    if (c->replicas.size() > 1 && n >= c->replicas.size()) {
-        const int d = c->vis.proj;
-        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
-            return hi == lo || image_batch_encode_one(r, 4, imgs->data + lo, hi - lo, vec + lo * d, nullptr, normalize, true, H, W, who);
-        });
-    }
-    return image_batch_encode_one(c, 4, imgs->data, n, vec, nullptr, normalize, true, H, W, who);
-}
-
-bool clip_image_encode(const struct clip_ctx* ctx, const int n_threads, struct clip_image_f32* img, float* vec, const bool normalize) {
-    if (!ctx || !ctx->has_vision) { printf("This gguf file seems to have no vision encoder\n"); return false; }
-    clip_image_f32_batch b;
-    b.data = img; b.size = 1;
-    return clip_image_batch_encode(ctx, n_threads, &b, vec, normalize);
-}
-
-// n sequences padded to T tokens on the host (h_ids / h_last) or on the device (d_ids / d_lens) -> d_out_dev (device) and / or vec_host
-static bool text_encode_impl(clip_ctx* c, const int32_t* h_ids, const int32_t* h_last, const int32_t* d_ids, const int32_t* d_lens,
-                             size_t n, int T, float* vec_host, float* vec_dev, bool normalize, bool sync = true) {
-    Tower& tw = c->txt;
-    // the padded length is fixed per context so that one workspace serves every call
-    if (T > tw.n_ctx) { set_err("sequence longer than context_length"); return false; }
-    if (!ensure_ws(c, tw, tw.micro_batch, tw.n_ctx, false)) return false;
-    float* d_out = vec_dev;
-    if (!d_out) { if (!ensure_out(c, n * tw.proj)) return false; d_out = c->d_out; }
-    size_t n_chunks, chunk;
-    chunking(n, tw.micro_batch, n_chunks, chunk);
-    CK(cudaEventRecord(c->ev_t0, c->stream));
-    for (size_t i0 = 0; i0 < n; i0 += chunk) {
-        const int nb = (int)std::min(chunk, n - i0);
-        if (h_ids) {
-            CK(cudaMemcpyAsync(tw.ws.ids, h_ids + i0 * T, (size_t)nb * T * 4, cudaMemcpyHostToDevice, c->stream));
-            CK(cudaMemcpyAsync(tw.ws.last, h_last + i0, (size_t)nb * 4, cudaMemcpyHostToDevice, c->stream));
-        } else {
-            CK(cudaMemcpyAsync(tw.ws.ids, d_ids + i0 * T, (size_t)nb * T * 4, cudaMemcpyDeviceToDevice, c->stream));
-            launch_fill_last(d_lens ? d_lens + i0 : nullptr, tw.ws.last, nb, T, c->stream);
-        }
-        if (!text_forward(c, nb, T, d_out + i0 * tw.proj, normalize)) return false;
-    }
-    CK(cudaEventRecord(c->ev_t1, c->stream));
-    if (vec_host) CK(cudaMemcpyAsync(vec_host, d_out, n * tw.proj * 4, cudaMemcpyDeviceToHost, c->stream));
-    return sync ? sync_and_time(c) : true;
-}
-
-// host token sequences -> padded id matrix + EOT row indices.  Padding to a multiple of 8 tokens is causally invisible to the EOT row.
-static bool pack_tokens(clip_ctx* c, const clip_tokens* seqs, size_t n, std::vector<int32_t>& ids, std::vector<int32_t>& last, int& T_out) {
+// host token sequences: none empty, none longer than context_length
+static bool check_tokens(const clip_ctx* c, const clip_tokens* seqs, size_t n, const char* who) {
     size_t T = 0;
     for (size_t i = 0; i < n; i++) {
-        if (seqs[i].size == 0 || !seqs[i].data) { set_err("empty token sequence"); return false; }
+        if (seqs[i].size == 0 || !seqs[i].data) { set_err(std::string(who) + ": empty token sequence"); return false; }
         T = std::max(T, seqs[i].size);
     }
-    if ((int)T > c->txt.n_ctx) { set_err("token sequence longer than context_length (" + std::to_string(c->txt.n_ctx) + ")"); return false; }
+    if (T > (size_t)c->txt.n_ctx) { set_err(std::string(who) + ": token sequence longer than context_length (" + std::to_string(c->txt.n_ctx) + ")"); return false; }
+    return true;
+}
+
+// checked host token sequences -> padded id matrix + EOT row indices.  Padding to a multiple of 8 tokens is causally invisible to the
+// EOT row.
+static void pack_tokens(const clip_ctx* c, const clip_tokens* seqs, size_t n, std::vector<int32_t>& ids, std::vector<int32_t>& last, int& T_out) {
+    size_t T = 0;
+    for (size_t i = 0; i < n; i++) T = std::max(T, seqs[i].size);
     T = std::min<size_t>((T + 7) / 8 * 8, (size_t)c->txt.n_ctx);
     ids.assign(n * T, 0);
     last.resize(n);
@@ -1241,51 +1023,265 @@ static bool pack_tokens(clip_ctx* c, const clip_tokens* seqs, size_t n, std::vec
         last[i] = (int32_t)seqs[i].size - 1;     // the reference selects row N-1 (clip.cpp:1154-1155)
     }
     T_out = (int)T;
+}
+
+// What one pooled call reads, as its public form received it.  Each form fills one and calls encode_call, so every form checks its
+// arguments in the same order (include/clip_b200.h) and runs the same pass driver.
+struct EncodeCall {
+    enum Input { F32_IMAGES, U8_IMAGES, DEVICE_PIXELS, TOKENS, DEVICE_IDS };
+    const char* who;                              // the public name, for messages
+    Input input;
+    const void* in = nullptr;                     // host: clip_image_f32 / clip_image_u8 / clip_tokens [n]; device: NHWC f32 pixels or ids [n, seq_len]
+    const int32_t* d_lens = nullptr;              // DEVICE_IDS: true lengths [n] (NULL: all seq_len)
+    size_t n = 0;
+    bool hw = false;                              // any patch-multiple size, H x W given (device) or the images' own (host)
+    int H = 0, W = 0, seq_len = 0;
+    int n_threads = 4;                            // host threads that gather pageable f32 images into the pinned arena
+    bool normalize = true;
+    float* vec = nullptr;                         // host output [n, proj]
+    float* d_vec = nullptr;                       // device output [n, proj]; an *_all form's is [world * n, proj]
+    clip_image_f32_batch* pixels = nullptr;       // the preprocessed u8 images, copied back to the host instead of any forward
+    bool all = false;                             // an *_all form: in ranks mode, every rank's embeddings out
+    bool reference = false;                       // a form of the reference's clip.h: prints the reference's line for a missing tower
+    bool vision() const { return input <= DEVICE_PIXELS; }
+    void batch(const clip_image_f32_batch* b) { if (b) { in = b->data; n = b->size; } }     // a NULL batch is an empty one
+    void batch(const clip_image_u8_batch* b) { if (b) { in = b->data; n = b->size; } }
+};
+
+// One GPU, items lo .. hi of a checked call: their embeddings into d_vec (device; NULL: the context's own buffer when vec is set, and no
+// forward at all when it is not), then into vec (host) unless it is NULL; sync: synchronise the launch stream and time the call.  Only
+// staging a micro-batch differs by input kind.  Host f32 pixels travel on the copy stream, double-buffered against the kernels of the
+// previous micro-batch.  Pinned / registered caller buffers are copied directly; PAGEABLE ones (what clip_image_preprocess returns:
+// new float[]) are first gathered into a pinned arena by host threads, in sub-batches so the H2D of sub-batch k overlaps the memcpy of
+// k+1 -- a pageable cudaMemcpyAsync would be staged synchronously by the driver, one 602 KB image at a time.
+static bool encode_pass(clip_ctx* c, const EncodeCall& a, size_t lo, size_t hi, float* vec, float* d_vec, bool sync) {
+    Tower& tw = a.vision() ? c->vis : c->txt;
+    const size_t n = hi - lo;
+    // ids / last are pageable vectors: the async copies below return only after the driver has staged them, so they may go out of
+    // scope when this function returns even with sync == false
+    std::vector<int32_t> ids, last;
+    int T = a.seq_len;
+    if (a.input == EncodeCall::TOKENS) pack_tokens(c, (const clip_tokens*)a.in + lo, n, ids, last, T);
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    VisCall v;
+    int mb = tw.micro_batch;
+    // the padded text length is fixed per context so that one workspace serves every call
+    if (a.vision() ? !plan_call(c, a.H, a.W, v, mb, a.who) : !ensure_ws(c, tw, tw.micro_batch, tw.n_ctx, false)) return false;
+    if (!d_vec && vec) {
+        if (!ensure_out(c, n * tw.proj)) return false;
+        d_vec = c->d_out;
+    }
+    std::vector<size_t> bounds{0};
+    if (a.input == EncodeCall::F32_IMAGES) {
+        bounds = host_chunk_bounds(n, mb);
+    } else {
+        size_t n_chunks, chunk;
+        chunking(n, mb, n_chunks, chunk);
+        for (size_t i0 = 0; i0 < n; i0 += chunk) bounds.push_back(std::min(n, i0 + chunk));
+    }
+    const size_t per = v.per();
+    const clip_image_f32* imgs = a.input == EncodeCall::F32_IMAGES ? (const clip_image_f32*)a.in + lo : nullptr;
+    bool pinned = true;
+    int nt = 1;
+    if (imgs) {
+        for (size_t i = 0; i < n && pinned; i++) pinned = host_ptr_is_pinned(imgs[i].data);
+        if (!pinned && c->h_stage_cap < (size_t)mb * per) {
+            for (int b = 0; b < 2; b++) {
+                if (c->h_stage[b]) { cudaFreeHost(c->h_stage[b]); c->h_stage[b] = nullptr; }
+                CK(cudaMallocHost((void**)&c->h_stage[b], (size_t)mb * per * 4));
+            }
+            c->h_stage_cap = (size_t)mb * per;
+        }
+        nt = std::max(1, std::min({std::max(a.n_threads, 4), 16, (int)std::thread::hardware_concurrency()}));
+    }
+    std::vector<float> h_pixels(a.pixels ? n * per : 0);
+    CK(cudaEventRecord(c->ev_t0, c->stream));
+    for (size_t ci = 0; ci + 1 < bounds.size(); ci++) {
+        const size_t i0 = bounds[ci];
+        const int nb = (int)(bounds[ci + 1] - i0), b = (int)(ci & 1);
+        const float* px = tw.ws.pixels[b];
+        if (a.input == EncodeCall::F32_IMAGES) {
+            if (ci >= 2) CK(cudaStreamWaitEvent(c->copy_stream, c->ev_consumed[b], 0));
+            if (pinned) {
+                for (int j = 0; j < nb; j++)
+                    CK(cudaMemcpyAsync(tw.ws.pixels[b] + (size_t)j * per, imgs[i0 + j].data, per * 4, cudaMemcpyHostToDevice, c->copy_stream));
+            } else {
+                if (ci >= 2) CK(cudaEventSynchronize(c->ev_copied[b]));      // the arena's previous H2D has left the host buffer
+                const int sub = 32;
+                for (int j0 = 0; j0 < nb; j0 += sub) {
+                    const int ns = std::min(sub, nb - j0);
+                    float* dst = c->h_stage[b] + (size_t)j0 * per;
+                    const clip_image_f32* src = imgs + i0 + j0;
+                    const int t_use = std::min(nt, ns);
+                    if (t_use <= 1) { for (int j = 0; j < ns; j++) memcpy(dst + (size_t)j * per, src[j].data, per * 4); }
+                    else {
+                        std::vector<std::thread> th;
+                        for (int t = 0; t < t_use; t++)
+                            th.emplace_back([=]() { for (int j = t; j < ns; j += t_use) memcpy(dst + (size_t)j * per, src[j].data, per * 4); });
+                        for (auto& t : th) t.join();
+                    }
+                    CK(cudaMemcpyAsync(tw.ws.pixels[b] + (size_t)j0 * per, dst, (size_t)ns * per * 4, cudaMemcpyHostToDevice, c->copy_stream));
+                }
+            }
+            CK(cudaEventRecord(c->ev_copied[b], c->copy_stream));
+            CK(cudaStreamWaitEvent(c->stream, c->ev_copied[b], 0));
+        } else if (a.input == EncodeCall::U8_IMAGES) {
+            if (ci >= 2) CK(cudaEventSynchronize(c->ev_consumed[b]));      // arena b is rewritten on the host below
+            std::string err;
+            if (!preprocess_device(c, (const clip_image_u8*)a.in + lo + i0, nb, b, tw.ws.pixels[b], c->copy_stream, c->ev_copied[b], c->stream, err)) {
+                set_err(std::string(a.who) + ": " + err);
+                return false;
+            }
+            if (a.pixels) CK(cudaMemcpyAsync(h_pixels.data() + i0 * per, tw.ws.pixels[b], (size_t)nb * per * 4, cudaMemcpyDeviceToHost, c->stream));
+        } else if (a.input == EncodeCall::DEVICE_PIXELS) {
+            px = (const float*)a.in + (lo + i0) * per;
+        } else if (a.input == EncodeCall::TOKENS) {
+            CK(cudaMemcpyAsync(tw.ws.ids, ids.data() + i0 * T, (size_t)nb * T * 4, cudaMemcpyHostToDevice, c->stream));
+            CK(cudaMemcpyAsync(tw.ws.last, last.data() + i0, (size_t)nb * 4, cudaMemcpyHostToDevice, c->stream));
+        } else {
+            // lengths stay on the device: a tiny kernel turns them into EOT-row indices (clamped to [1, seq_len])
+            CK(cudaMemcpyAsync(tw.ws.ids, (const int32_t*)a.in + (lo + i0) * T, (size_t)nb * T * 4, cudaMemcpyDeviceToDevice, c->stream));
+            launch_fill_last(a.d_lens ? a.d_lens + lo + i0 : nullptr, tw.ws.last, nb, T, c->stream);
+        }
+        if (d_vec && !(a.vision() ? vision_forward(c, px, nb, v, d_vec + i0 * tw.proj, a.normalize)
+                                  : text_forward(c, nb, T, d_vec + i0 * tw.proj, a.normalize))) return false;
+        if (a.input == EncodeCall::F32_IMAGES || a.input == EncodeCall::U8_IMAGES) CK(cudaEventRecord(c->ev_consumed[b], c->stream));
+    }
+    CK(cudaEventRecord(c->ev_t1, c->stream));
+    if (vec) CK(cudaMemcpyAsync(vec, d_vec, n * tw.proj * 4, cudaMemcpyDeviceToHost, c->stream));
+    if (sync && !sync_and_time(c)) return false;
+    if (a.pixels)
+        for (size_t i = 0; i < n; i++) {        // same ownership convention as clip_image_preprocess: data is new[]-allocated here
+            clip_image_f32& o = a.pixels->data[lo + i];
+            o.nx = v.W; o.ny = v.H; o.size = per;
+            o.data = new float[per];
+            memcpy(o.data, h_pixels.data() + i * per, per * 4);
+        }
     return true;
 }
 
-static bool text_batch_encode_one(clip_ctx* c, const clip_tokens* seqs, size_t n, float* vec, float* d_vec, bool normalize, bool sync) {
-    std::vector<int32_t> ids, last;
-    int T = 0;
-    if (!pack_tokens(c, seqs, n, ids, last, T)) return false;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    // ids / last are pageable vectors: the async copies inside return only after the driver has staged them, so they may go out of
-    // scope when this function returns even with sync == false
-    return text_encode_impl(c, ids.data(), last.data(), nullptr, nullptr, n, T, vec, d_vec, normalize, sync);
+// Devices mode shards a text call only from this many sequences per GPU: a sequence is a fraction of an image's work (77 rows against
+// 257 for ViT-L/14, on a smaller tower), so a GPU needs more of them before its share outweighs the fixed cost of its host thread,
+// launches and synchronise.
+const size_t TEXT_SHARD_MIN = 8;
+
+// Every pooled form: the arguments checked in one order, the first fault refused (include/clip_b200.h), then the pass.  Devices mode
+// shards the forms with a host output over the GPUs, each GPU copying its slice into vec; an *_all form encodes this rank's items into
+// its slot of the gather buffer and all-gathers every rank's (outside ranks mode the device forms run the same steps without the
+// exchange, and the host forms are the plain ones).
+static bool encode_call(const clip_ctx* cctx, EncodeCall a) {
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    const std::string who = a.who;
+    if (a.reference && !(c && (a.vision() ? c->has_vision : c->has_text))) {
+        printf(a.vision() ? "This gguf file seems to have no vision encoder\n" : "This GGUF file seems to have no text encoder\n");
+        return false;
+    }
+    if (!c) { set_err(who + ": null context"); return false; }
+    const Tower& tw = a.vision() ? c->vis : c->txt;
+    if (!tw.present) { set_err(who + ": this model has no " + (a.vision() ? "vision" : "text") + " encoder"); return false; }
+    const bool device = a.input == EncodeCall::DEVICE_PIXELS || a.input == EncodeCall::DEVICE_IDS;
+    if (a.hw && device && !check_hw_size(c, a.H, a.W, a.who)) return false;
+    const bool ranks = a.all && ranks_mode(c);
+    if (a.pixels) a.pixels->size = a.n;
+    if (a.n == 0) {
+        if (!ranks) return true;
+        set_err(who + ": every rank must pass the same, non-zero number of " + (a.vision() ? "images" : "sequences"));
+        return false;
+    }
+    if (a.input == EncodeCall::DEVICE_IDS && (a.seq_len < 1 || a.seq_len > tw.n_ctx)) { set_err(who + ": seq_len must be in [1, context_length]"); return false; }
+    if (!a.in || !(a.vec || a.d_vec || a.pixels)) {
+        set_err(who + (device ? ": null device pointer" : a.in ? ": null output" : ": null input"));
+        return false;
+    }
+    if (a.input == EncodeCall::F32_IMAGES) {
+        const clip_image_f32* imgs = (const clip_image_f32*)a.in;
+        if (!(a.hw ? check_images_hw(c, imgs, a.n, a.H, a.W, a.who) : check_images(c, imgs, a.n, a.who))) return false;
+    }
+    if (a.input == EncodeCall::TOKENS && !check_tokens(c, (const clip_tokens*)a.in, a.n, a.who)) return false;
+    const int d = tw.proj;
+    if (a.all && (device || ranks)) {
+        const int w = ranks ? c->dist.world : 1, rank = ranks ? c->dist.rank : 0;
+        float* all = a.d_vec;
+        if (!all) {
+            std::lock_guard<std::mutex> lk(c->mu);
+            CK(cudaSetDevice(c->device));
+            if (!ensure_out(c, (size_t)w * a.n * d)) return false;
+            all = c->d_out;
+        }
+        if (!encode_pass(c, a, 0, a.n, nullptr, all + (size_t)rank * a.n * d, false)) return false;
+        std::lock_guard<std::mutex> lk(c->mu);
+        if (!gather_in_place(c, all, a.n, d)) return false;
+        CK(cudaEventRecord(c->ev_t1, c->stream));
+        if (a.vec) CK(cudaMemcpyAsync(a.vec, all, (size_t)w * a.n * d * 4, cudaMemcpyDeviceToHost, c->stream));
+        return sync_and_time(c);
+    }
+    if (a.vec && c->replicas.size() > 1 && a.n >= (a.vision() ? 1 : TEXT_SHARD_MIN) * c->replicas.size())
+        return for_each_replica(c, a.n, [&](clip_ctx* r, int, size_t lo, size_t hi) { return hi == lo || encode_pass(r, a, lo, hi, a.vec + lo * d, nullptr, true); });
+    return encode_pass(c, a, 0, a.n, a.vec, a.d_vec, true);
+}
+
+bool clip_b200_image_batch_encode_u8(const struct clip_ctx* cctx, const struct clip_image_u8_batch* imgs, float* vec, const bool normalize) {
+    EncodeCall a{"clip_b200_image_batch_encode_u8", EncodeCall::U8_IMAGES};
+    a.batch(imgs); a.normalize = normalize; a.vec = vec;
+    return encode_call(cctx, a);
+}
+
+bool clip_b200_image_batch_preprocess_device(const struct clip_ctx* cctx, const struct clip_image_u8_batch* in, struct clip_image_f32_batch* out) {
+    EncodeCall a{"clip_b200_image_batch_preprocess_device", EncodeCall::U8_IMAGES};
+    a.batch(in); a.pixels = out;
+    return encode_call(cctx, a);
+}
+
+bool clip_b200_image_encode_device(const struct clip_ctx* cctx, const void* d_pixels, size_t n, void* d_vec, bool normalize) {
+    EncodeCall a{"clip_b200_image_encode_device", EncodeCall::DEVICE_PIXELS};
+    a.in = d_pixels; a.n = n; a.normalize = normalize; a.d_vec = (float*)d_vec;
+    return encode_call(cctx, a);
+}
+
+bool clip_b200_image_encode_device_hw(const struct clip_ctx* cctx, const void* d_pixels, size_t n, int height, int width, void* d_vec,
+                                      bool normalize) {
+    EncodeCall a{"clip_b200_image_encode_device_hw", EncodeCall::DEVICE_PIXELS};
+    a.in = d_pixels; a.n = n; a.hw = true; a.H = height; a.W = width; a.normalize = normalize; a.d_vec = (float*)d_vec;
+    return encode_call(cctx, a);
+}
+
+bool clip_image_batch_encode(const struct clip_ctx* cctx, const int n_threads, const struct clip_image_f32_batch* imgs, float* vec,
+                             const bool normalize) {
+    EncodeCall a{"clip_image_batch_encode", EncodeCall::F32_IMAGES};
+    a.batch(imgs); a.n_threads = n_threads; a.normalize = normalize; a.vec = vec; a.reference = true;
+    return encode_call(cctx, a);
+}
+
+bool clip_b200_image_batch_encode_hw(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, float* vec, bool normalize) {
+    EncodeCall a{"clip_b200_image_batch_encode_hw", EncodeCall::F32_IMAGES};
+    a.batch(imgs); a.hw = true; a.normalize = normalize; a.vec = vec;
+    return encode_call(cctx, a);
+}
+
+bool clip_image_encode(const struct clip_ctx* ctx, const int n_threads, struct clip_image_f32* img, float* vec, const bool normalize) {
+    clip_image_f32_batch b;
+    b.data = img; b.size = 1;
+    return clip_image_batch_encode(ctx, n_threads, &b, vec, normalize);
 }
 
 bool clip_text_batch_encode(const struct clip_ctx* cctx, const int n_threads, const struct clip_tokens* seqs, const size_t n, float* vec,
                             const bool normalize) {
     (void)n_threads;
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c || !c->has_text) { printf("This GGUF file seems to have no text encoder\n"); return false; }
-    if (n == 0) return true;
-    if (c->replicas.size() > 1 && n >= 8 * c->replicas.size()) {
-        const int d = c->txt.proj;
-        return for_each_replica(c, n, [&](clip_ctx* r, int, size_t lo, size_t hi) {
-            return hi == lo || text_batch_encode_one(r, seqs + lo, hi - lo, vec + lo * d, nullptr, normalize, true);
-        });
-    }
-    return text_batch_encode_one(c, seqs, n, vec, nullptr, normalize, true);
+    EncodeCall a{"clip_text_batch_encode", EncodeCall::TOKENS};
+    a.in = seqs; a.n = n; a.normalize = normalize; a.vec = vec; a.reference = true;
+    return encode_call(cctx, a);
 }
 
 bool clip_text_encode(const struct clip_ctx* ctx, const int n_threads, const struct clip_tokens* tokens, float* vec, const bool normalize) {
-    if (!ctx || !ctx->has_text) { printf("This GGUF file seems to have no text encoder\n"); return false; }
     return clip_text_batch_encode(ctx, n_threads, tokens, 1, vec, normalize);
 }
 
 bool clip_b200_text_encode_device(const struct clip_ctx* cctx, const void* d_ids, const void* d_lens, size_t n, int seq_len, void* d_vec,
                                   bool normalize) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c || !c->has_text) { set_err("no text encoder"); return false; }
-    if (n == 0) return true;
-    if (seq_len < 1 || seq_len > c->txt.n_ctx) { set_err("clip_b200_text_encode_device: seq_len must be in [1, context_length]"); return false; }
-    if (!d_ids || !d_vec) { set_err("clip_b200_text_encode_device: null device pointer"); return false; }
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    // lengths stay on the device: a tiny kernel turns them into EOT-row indices per micro-batch (clamped to [1, seq_len])
-    return text_encode_impl(c, nullptr, nullptr, (const int32_t*)d_ids, (const int32_t*)d_lens, n, seq_len, nullptr, (float*)d_vec, normalize);
+    EncodeCall a{"clip_b200_text_encode_device", EncodeCall::DEVICE_IDS};
+    a.in = d_ids; a.d_lens = (const int32_t*)d_lens; a.n = n; a.seq_len = seq_len; a.normalize = normalize; a.d_vec = (float*)d_vec;
+    return encode_call(cctx, a);
 }
 
 // ---- per-token hidden states: the ten clip_b200_*_tokens* forms -------------------------------------------------------------------
@@ -1662,8 +1658,6 @@ int clip_b200_device_count(const struct clip_ctx* c) { return c ? std::max<int>(
 int clip_b200_nccl_version(void) { return dist_nccl_version(); }
 int clip_b200_cuda_device_count(void) { int n = 0; if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; } return n; }
 
-static bool ranks_mode(const clip_ctx* c) { return c->replicas.size() <= 1 && c->dist.comm && c->dist.world > 1; }
-
 static bool ensure_scalars(clip_ctx* c) {
     if (c->d_scalars) return true;
     return dev_alloc(c, &c->d_scalars, 16);
@@ -1708,78 +1702,33 @@ bool clip_b200_dist_barrier(const struct clip_ctx* cctx) {
     return true;
 }
 
-// ranks mode: every rank encodes ITS n_local items and ends with ALL world * n_local embeddings, rank-major.  The last kernel of
-// the tower (K5 l2norm) writes straight into this rank's slot of the gather buffer; the all-gather runs in place on the launch stream.
-static bool gather_in_place(clip_ctx* c, float* d_all, size_t n_local, int d) {
-    if (!ranks_mode(c)) return true;
-    std::string e;
-    const size_t bytes = n_local * (size_t)d * 4;
-    if (!dist_all_gather(c->dist, (const char*)d_all + (size_t)c->dist.rank * bytes, d_all, bytes, c->stream, e)) { set_err(e); return false; }
-    return true;
-}
-
 bool clip_b200_image_encode_device_all(const struct clip_ctx* cctx, const void* d_pixels, size_t n_local, void* d_vec_all, bool normalize) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c || !c->has_vision) { set_err("no vision encoder"); return false; }
-    if (n_local == 0) return true;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    const int d = c->vis.proj;
-    float* slot = (float*)d_vec_all + (ranks_mode(c) ? (size_t)c->dist.rank * n_local * d : 0);
-    if (!image_encode_device_locked(c, (const float*)d_pixels, n_local, slot, normalize)) return false;
-    if (!gather_in_place(c, (float*)d_vec_all, n_local, d)) return false;
-    CK(cudaEventRecord(c->ev_t1, c->stream));
-    return sync_and_time(c);
+    EncodeCall a{"clip_b200_image_encode_device_all", EncodeCall::DEVICE_PIXELS};
+    a.in = d_pixels; a.n = n_local; a.normalize = normalize; a.d_vec = (float*)d_vec_all; a.all = true;
+    return encode_call(cctx, a);
 }
 
 bool clip_b200_image_batch_encode_all(const struct clip_ctx* cctx, const int n_threads, const struct clip_image_f32_batch* imgs, float* vec_all,
                                       const bool normalize) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c || !c->has_vision) { set_err("no vision encoder"); return false; }
-    if (!ranks_mode(c)) return clip_image_batch_encode(c, n_threads, imgs, vec_all, normalize);
-    const size_t n = imgs->size;
-    if (n == 0) { set_err("clip_b200_image_batch_encode_all: every rank must pass the same, non-zero number of images"); return false; }
-    if (!check_images(c, imgs->data, n, "clip_b200_image_batch_encode_all")) return false;
-    const int d = c->vis.proj, w = c->dist.world;
-    { std::lock_guard<std::mutex> lk(c->mu); CK(cudaSetDevice(c->device)); if (!ensure_out(c, (size_t)w * n * d)) return false; }
-    if (!image_batch_encode_one(c, n_threads, imgs->data, n, nullptr, c->d_out + (size_t)c->dist.rank * n * d, normalize, false)) return false;
-    std::lock_guard<std::mutex> lk(c->mu);
-    if (!gather_in_place(c, c->d_out, n, d)) return false;
-    CK(cudaEventRecord(c->ev_t1, c->stream));
-    CK(cudaMemcpyAsync(vec_all, c->d_out, (size_t)w * n * d * 4, cudaMemcpyDeviceToHost, c->stream));
-    return sync_and_time(c);
+    EncodeCall a{"clip_b200_image_batch_encode_all", EncodeCall::F32_IMAGES};
+    a.batch(imgs); a.n_threads = n_threads; a.normalize = normalize; a.vec = vec_all; a.all = true;
+    return encode_call(cctx, a);
 }
 
 bool clip_b200_text_batch_encode_all(const struct clip_ctx* cctx, const int n_threads, const struct clip_tokens* seqs, const size_t n, float* vec_all,
                                      const bool normalize) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c || !c->has_text) { set_err("no text encoder"); return false; }
-    if (!ranks_mode(c)) return clip_text_batch_encode(c, n_threads, seqs, n, vec_all, normalize);
-    if (n == 0) { set_err("clip_b200_text_batch_encode_all: every rank must pass the same, non-zero number of sequences"); return false; }
-    const int d = c->txt.proj, w = c->dist.world;
-    { std::lock_guard<std::mutex> lk(c->mu); CK(cudaSetDevice(c->device)); if (!ensure_out(c, (size_t)w * n * d)) return false; }
-    if (!text_batch_encode_one(c, seqs, n, nullptr, c->d_out + (size_t)c->dist.rank * n * d, normalize, false)) return false;
-    std::lock_guard<std::mutex> lk(c->mu);
-    if (!gather_in_place(c, c->d_out, n, d)) return false;
-    CK(cudaEventRecord(c->ev_t1, c->stream));
-    CK(cudaMemcpyAsync(vec_all, c->d_out, (size_t)w * n * d * 4, cudaMemcpyDeviceToHost, c->stream));
-    return sync_and_time(c);
+    (void)n_threads;
+    EncodeCall a{"clip_b200_text_batch_encode_all", EncodeCall::TOKENS};
+    a.in = seqs; a.n = n; a.normalize = normalize; a.vec = vec_all; a.all = true;
+    return encode_call(cctx, a);
 }
 
 bool clip_b200_text_encode_device_all(const struct clip_ctx* cctx, const void* d_ids, const void* d_lens, size_t n_local, int seq_len,
                                       void* d_vec_all, bool normalize) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c || !c->has_text) { set_err("no text encoder"); return false; }
-    if (n_local == 0) return true;
-    if (seq_len < 1 || seq_len > c->txt.n_ctx || !d_ids || !d_vec_all) { set_err("clip_b200_text_encode_device_all: bad arguments"); return false; }
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    const int d = c->txt.proj;
-    float* slot = (float*)d_vec_all + (ranks_mode(c) ? (size_t)c->dist.rank * n_local * d : 0);
-    if (!text_encode_impl(c, nullptr, nullptr, (const int32_t*)d_ids, (const int32_t*)d_lens, n_local, seq_len, nullptr, slot, normalize, false)) return false;
-    if (!gather_in_place(c, (float*)d_vec_all, n_local, d)) return false;
-    CK(cudaEventRecord(c->ev_t1, c->stream));
-    return sync_and_time(c);
+    EncodeCall a{"clip_b200_text_encode_device_all", EncodeCall::DEVICE_IDS};
+    a.in = d_ids; a.d_lens = (const int32_t*)d_lens; a.n = n_local; a.seq_len = seq_len; a.normalize = normalize; a.d_vec = (float*)d_vec_all;
+    a.all = true;
+    return encode_call(cctx, a);
 }
 
 // Batched zero-shot labelling (BASELINE.json configs[4]; per image the arithmetic of clip_zero_shot_label_image, clip.cpp:1624-1659):
@@ -1792,10 +1741,14 @@ bool clip_b200_zero_shot_images(const struct clip_ctx* cctx, const int n_threads
                                 const struct clip_tokens* labels, const size_t n_labels, const bool normalize, int top_k, float* scores,
                                 int* indices) {
     clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    const char* who = "clip_b200_zero_shot_images";
     if (!c || !(c->has_text && c->has_vision)) { set_err("clip_b200_zero_shot_images needs a two-tower model"); return false; }
     const size_t n = imgs ? imgs->size : 0;
     if (n == 0 || n_labels == 0) return n == 0;
-    if (!check_images(c, imgs->data, n, "clip_b200_zero_shot_images")) return false;
+    if (!check_images(c, imgs->data, n, who) || !check_tokens(c, labels, n_labels, who)) return false;
+    EncodeCall ai{who, EncodeCall::F32_IMAGES}, at{who, EncodeCall::TOKENS};
+    ai.batch(imgs); ai.n_threads = n_threads; ai.normalize = normalize;
+    at.in = labels; at.n = n_labels; at.normalize = normalize;
     const int d = c->vis.proj;
     if (c->replicas.size() > 1) {
         const int w = (int)c->replicas.size();
@@ -1809,9 +1762,9 @@ bool clip_b200_zero_shot_images(const struct clip_ctx* cctx, const int n_threads
                     if (!ensure_buf(r, &r->d_emb[0], &r->d_emb_cap[0], std::max<size_t>(hi - lo, 1) * d) || !ensure_buf(r, &r->d_emb[1], &r->d_emb_cap[1], tot * d)) return false;
                     CK(cudaMemsetAsync(r->d_emb[1], 0, tot * d * 4, r->stream));
                 }
-                if (hi > lo && !image_batch_encode_one(r, n_threads, imgs->data + lo, hi - lo, nullptr, r->d_emb[0], normalize, false)) return false;
+                if (hi > lo && !encode_pass(r, ai, lo, hi, nullptr, r->d_emb[0], false)) return false;
                 const size_t l0 = std::min(n_labels, (size_t)ri * per), l1 = std::min(n_labels, l0 + per);
-                if (l1 > l0 && !text_batch_encode_one(r, labels + l0, l1 - l0, nullptr, r->d_emb[1] + (size_t)ri * per * d, normalize, false)) return false;
+                if (l1 > l0 && !encode_pass(r, at, l0, l1, nullptr, r->d_emb[1] + (size_t)ri * per * d, false)) return false;
                 return true;
             })) return false;
         // phase 2: ONE all-gather of the label embeddings, in place on every GPU (group call: one thread drives all communicators)
@@ -1839,8 +1792,8 @@ bool clip_b200_zero_shot_images(const struct clip_ctx* cctx, const int n_threads
         CK(cudaSetDevice(c->device));
         if (!ensure_buf(c, &c->d_emb[0], &c->d_emb_cap[0], n * d) || !ensure_buf(c, &c->d_emb[1], &c->d_emb_cap[1], n_all * d)) return false;
     }
-    if (!image_batch_encode_one(c, n_threads, imgs->data, n, nullptr, c->d_emb[0], normalize, false)) return false;
-    if (!text_batch_encode_one(c, labels, n_labels, nullptr, c->d_emb[1] + (size_t)rank * n_labels * d, normalize, false)) return false;
+    if (!encode_pass(c, ai, 0, n, nullptr, c->d_emb[0], false)) return false;
+    if (!encode_pass(c, at, 0, n_labels, nullptr, c->d_emb[1] + (size_t)rank * n_labels * d, false)) return false;
     std::lock_guard<std::mutex> lk(c->mu);
     CK(cudaSetDevice(c->device));
     if (!gather_in_place(c, c->d_emb[1], n_labels, d)) return false;

@@ -172,6 +172,15 @@ bool clip_b200_image_encode_device(const struct clip_ctx * ctx, const void * d_p
 bool clip_b200_text_encode_device(const struct clip_ctx * ctx, const void * d_ids, const void * d_lens, size_t n,
                                   int seq_len, void * d_vec, bool normalize);
 
+/* Every pooled form -- clip_image_batch_encode and clip_text_batch_encode (and clip_image_encode / clip_text_encode through them), the
+ * two above, the *_hw, *_all and u8 forms and clip_b200_image_batch_preprocess_device -- checks its arguments in one order and
+ * reports the first fault: 1. a null context; 2. the tower; 3. height x width of clip_b200_image_encode_device_hw; 4. n == 0 (a NULL
+ * batch is an empty one) returns true here, except in the *_all forms in ranks mode, which refuse it; 5. seq_len in [1,
+ * context_length] of the device text forms; 6. null input or output pointers; 7. the host inputs: image_size x image_size images (one
+ * patch-multiple size for clip_b200_image_batch_encode_hw), token sequences neither empty nor longer than context_length.  Messages
+ * start with the form's name, except for 1 and 2 in the reference's four forms, which print the reference's line to stdout and leave
+ * clip_b200_last_error as it was.  Devices mode checks a call once, before it shards it. */
+
 /* Per-token hidden states of either tower (HF output_hidden_states, open_clip forward_intermediates): every row of the residual
  * stream after a chosen layer, for vision-language front ends (LLaVA reads the patch rows of the penultimate layer) and diffusion
  * text conditioning (Stable Diffusion reads all 77 rows, post_ln applied).
