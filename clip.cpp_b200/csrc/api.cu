@@ -87,7 +87,7 @@ struct Scope {
         }
     }
 };
-enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4, K_POS_RESAMPLE = 5, K_ATTN_PROBS = 6 };
+enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4, K_POS_RESAMPLE = 5, K_ATTN_PROBS = 6, K_KNN16 = 7 };
 
 // ---- tensor lookup helpers ---------------------------------------------------------------------------------
 const GgufTensor* need(const GgufFile& g, const std::string& name) {
@@ -1525,6 +1525,31 @@ bool clip_zero_shot_label_image(struct clip_ctx* ctx, const int n_threads, const
 // =====================================================================================================================
 // Scoring on the device (search.cu): similarity matrix -> [softmax_with_sorting arithmetic] -> top-k, results to the host
 // =====================================================================================================================
+// Merge stages over d_cand_v/i[0] [rows, cand_ld]: nsl sorted runs of kk candidates (value, index) compete again until one run of kk
+// is left.  Returns the buffer (0 or 1) that holds each row's best kk, best first.
+static int merge_candidates(clip_ctx* c, int rows, size_t cand_ld, size_t nsl, int kk) {
+    const int SL = topk_slice();
+    int cur = 0;
+    size_t cur_n = cand_ld;
+    while (cur_n > (size_t)SL || (cur_n > (size_t)kk && nsl > 1)) {      // merge stages: candidates of all slices compete again
+        const size_t nslices = (cur_n + SL - 1) / SL;
+        { Scope s(c, K_OTHER); launch_topk_stage(c->d_cand_v[cur], c->d_cand_i[cur], cand_ld, rows, (int)cur_n, 0, kk, c->d_cand_v[cur ^ 1], c->d_cand_i[cur ^ 1], cand_ld, 0, c->stream); }
+        cur ^= 1;
+        cur_n = nslices * (size_t)kk;
+        if (nslices == 1) break;
+    }
+    return cur;
+}
+
+// grow the four candidate buffers to `count` entries each
+static bool ensure_cand(clip_ctx* c, size_t count) {
+    size_t cap0 = c->d_cand_cap, cap1 = c->d_cand_cap, cap2 = c->d_cand_cap, cap3 = c->d_cand_cap;
+    if (!ensure_buf(c, &c->d_cand_v[0], &cap0, count) || !ensure_buf(c, &c->d_cand_v[1], &cap1, count) ||
+        !ensure_buf(c, &c->d_cand_i[0], &cap2, count) || !ensure_buf(c, &c->d_cand_i[1], &cap3, count)) return false;
+    c->d_cand_cap = std::min(std::min(cap0, cap1), std::min(cap2, cap3));
+    return true;
+}
+
 // d_q [nq, d] x d_db [ndb, d] -> host scores / indices [nq, k], best first (ties: lower index first).  softmax: p = (exp(s)+1e-9)/sum
 // over the whole row first (clip.cpp:1591-1622); otherwise the raw dot products are ranked (nearest-neighbour search).
 // The stream is synchronised on return.  Caller holds c->mu and has set the device.
@@ -1546,12 +1571,7 @@ static bool score_topk_locked(clip_ctx* c, const float* d_q, size_t nq, const fl
     const bool device_select = nsl == 1 || k <= 1024;                    // each stage must shrink the candidate set
     if (!ensure_buf(c, &c->d_logits, &c->d_logits_cap, RB * CH)) return false;
     const size_t cand_ld = nsl * (size_t)kk;
-    if (device_select) {
-        size_t cap0 = c->d_cand_cap, cap1 = c->d_cand_cap, cap2 = c->d_cand_cap, cap3 = c->d_cand_cap;
-        if (!ensure_buf(c, &c->d_cand_v[0], &cap0, RB * cand_ld) || !ensure_buf(c, &c->d_cand_v[1], &cap1, RB * cand_ld) ||
-            !ensure_buf(c, &c->d_cand_i[0], &cap2, RB * cand_ld) || !ensure_buf(c, &c->d_cand_i[1], &cap3, RB * cand_ld)) return false;
-        c->d_cand_cap = std::min(std::min(cap0, cap1), std::min(cap2, cap3));
-    }
+    if (device_select && !ensure_cand(c, RB * cand_ld)) return false;
     std::vector<float> hrow;
     std::vector<int> hidx;
     for (size_t r0 = 0; r0 < nq; r0 += RB) {
@@ -1583,15 +1603,7 @@ static bool score_topk_locked(clip_ctx* c, const float* d_q, size_t nq, const fl
             }
         }
         if (!device_select) continue;
-        int cur = 0;
-        size_t cur_n = cand_ld;
-        while (cur_n > (size_t)SL || (cur_n > (size_t)kk && nsl > 1)) {      // merge stages: candidates of all slices compete again
-            const size_t nslices = (cur_n + SL - 1) / SL;
-            { Scope s(c, K_OTHER); launch_topk_stage(c->d_cand_v[cur], c->d_cand_i[cur], cand_ld, rows, (int)cur_n, 0, kk, c->d_cand_v[cur ^ 1], c->d_cand_i[cur ^ 1], cand_ld, 0, c->stream); }
-            cur ^= 1;
-            cur_n = nslices * (size_t)kk;
-            if (nslices == 1) break;
-        }
+        const int cur = merge_candidates(c, rows, cand_ld, nsl, kk);
         CK(cudaMemcpy2DAsync(scores + r0 * k, (size_t)k * 4, c->d_cand_v[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaMemcpy2DAsync(indices + r0 * k, (size_t)k * 4, c->d_cand_i[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaStreamSynchronize(c->stream));
@@ -1618,6 +1630,64 @@ bool clip_b200_topk_search(const struct clip_ctx* cctx, const void* d_queries, s
     CK(cudaSetDevice(c->device));
     const int d = c->has_vision ? c->vhp.projection_dim : c->thp.projection_dim;
     return score_topk_locked(c, (const float*)d_queries, n_queries, (const float*)d_db, n_db, d, top_k, false, scores, indices);
+}
+
+// ---- 16-bit nearest-neighbour search (K10, search.cu) ---------------------------------------------------------------
+bool clip_b200_rows_to_16bit(const struct clip_ctx* cctx, const void* d_src, size_t n, int dim, int out_type, void* d_dst) {
+    static const char* F = "clip_b200_rows_to_16bit: ";
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    if (!c) { set_err(std::string(F) + "null context"); return false; }
+    if (out_type != CLIP_B200_OUT_F16 && out_type != CLIP_B200_OUT_BF16) { set_err(std::string(F) + "out_type must be CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16"); return false; }
+    if (dim < 4 || dim > 2048 || dim % 4) { set_err(std::string(F) + "dim must be a multiple of 4 in [4, 2048]"); return false; }
+    if (n > 0x7fffffffull) { set_err(std::string(F) + "n must be below 2^31"); return false; }
+    if (n == 0) return true;
+    if (!d_src || !d_dst || ((uintptr_t)d_src | (uintptr_t)d_dst) % 16) { set_err(std::string(F) + "null or not 16-byte aligned pointer"); return false; }
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    // K7 with one row per item, no CLS skip and no LayerNorm: an RNE copy.  Its offsets are size_t, so n * dim may pass 2^32.
+    { Scope s(c, K_TOKEN_ROWS); launch_token_rows((const float*)d_src, (size_t)dim, (int)n, 1, 0, dim, nullptr, nullptr, 0.f, out_type, d_dst, c->stream); }
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(c->stream));
+    return true;
+}
+
+bool clip_b200_topk_search_16(const struct clip_ctx* cctx, const void* d_queries, size_t n_queries, const void* d_db, size_t n_db, int dim,
+                              int in_type, int top_k, float* scores, int* indices) {
+    static const char* F = "clip_b200_topk_search_16: ";
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    if (!c) { set_err(std::string(F) + "null context"); return false; }
+    if (in_type != CLIP_B200_OUT_F16 && in_type != CLIP_B200_OUT_BF16) { set_err(std::string(F) + "in_type must be CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16"); return false; }
+    if (dim < 8 || dim > 2048 || dim % 8) { set_err(std::string(F) + "dim must be a multiple of 8 in [8, 2048]"); return false; }
+    if (top_k < 1 || top_k > 1024) { set_err(std::string(F) + "top_k must be in [1, 1024]"); return false; }
+    if (n_queries > 0x7fffffffull || n_db > 0x7fffffffull) { set_err(std::string(F) + "n_queries and n_db must be below 2^31"); return false; }
+    if (n_queries == 0 || n_db == 0) return true;
+    if (!d_queries || !d_db || ((uintptr_t)d_queries | (uintptr_t)d_db) % 16) { set_err(std::string(F) + "null or not 16-byte aligned device pointer"); return false; }
+    if (!scores || !indices) { set_err(std::string(F) + "null output"); return false; }
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
+    const int k = (int)std::min<size_t>((size_t)top_k, n_db), ndb = (int)n_db;
+    const size_t QB = 32768;                                              // queries per launch (the merge grid's row limit)
+    const uint16_t* q16 = (const uint16_t*)d_queries;
+    for (size_t r0 = 0; r0 < n_queries; r0 += QB) {
+        const int rows = (int)std::min(QB, n_queries - r0);
+        const Knn16Plan pl = knn16_plan(rows, ndb, k, sms);
+        const size_t cand_ld = (size_t)pl.parts * k;
+        if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * pl.buf_entries) || !ensure_cand(c, (size_t)rows * cand_ld)) return false;
+        {
+            Scope s(c, K_KNN16);
+            const cudaError_t e = launch_knn16(q16 + r0 * dim, rows, d_db, ndb, dim, in_type == CLIP_B200_OUT_BF16, k, pl, c->d_knn,
+                                               c->d_cand_v[0], c->d_cand_i[0], cand_ld, c->stream);
+            if (e != cudaSuccess) { set_err(std::string(F) + "launch: " + cudaGetErrorString(e)); return false; }
+        }
+        const int cur = merge_candidates(c, rows, cand_ld, (size_t)pl.parts, k);
+        CK(cudaMemcpy2DAsync(scores + r0 * k, (size_t)k * 4, c->d_cand_v[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpy2DAsync(indices + r0 * k, (size_t)k * 4, c->d_cand_i[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+    }
+    CK(cudaGetLastError());
+    return true;
 }
 
 // =====================================================================================================================

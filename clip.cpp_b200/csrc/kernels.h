@@ -77,6 +77,18 @@ int topk_slice();
 void launch_topk_stage(const float* vals, const int* in_idx, size_t ld, int rows, int n, int idx_base, int kk, float* out_v, int* out_i,
                        size_t out_ld, int out_off, cudaStream_t st);
 
+// K10 16-bit nearest-neighbour search (search.cu): q [nq, dim] x db [ndb, dim], f16 or bf16, 16-byte aligned, dim % 8 == 0, dim <= 2048.
+// Writes each query's best kk (<= 1024) per database partition, sorted, to out[query, partition * kk ...] (row stride out_ld >=
+// parts * kk); padding entries are (-inf, INT_MAX).  The plan fixes the query tile (8 nt queries), the partitions and the scratch
+// `buf` of buf_entries (value, index) pairs the launch needs.
+struct Knn16Plan {
+    int nt, parts, rows_per_part, grid, cap;
+    size_t buf_entries;
+};
+Knn16Plan knn16_plan(int nq, int ndb, int kk, int sms);
+cudaError_t launch_knn16(const void* q, int nq, const void* db, int ndb, int dim, int bf16, int kk, const Knn16Plan& pl, void* buf,
+                         float* out_v, int* out_i, size_t out_ld, cudaStream_t st);
+
 }  // namespace cb
 struct clip_ctx;
 struct clip_image_u8;

@@ -6,10 +6,18 @@
 // 4096 x 1000 x 768 zero-shot problem is 6.3 GFLOP (0.008 % of the encode that produced the embeddings) and the ranking must not
 // move in the 4th digit, which bf16 tensor-core products would do.  Each dot product is ONE sequential fmaf chain over k, the same
 // order the reference's scalar loop uses.
+//
+// K10 (knn16_kernel, below) is the separate, opt-in search over a database stored in 16 bits: tensor-core scores and a top-k kept
+// inside the kernel, so no score matrix ever reaches memory.  It shares the candidate order and the merge stage with the fp32 path.
+#include <cuda.h>
 #include <float.h>
+#include <string.h>
+
+#include <algorithm>
 
 #include "common.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace cb {
 
@@ -122,6 +130,237 @@ __global__ void __launch_bounds__(256) topk_stage_kernel(const float* __restrict
     }
 }
 
+// ---- K10: nearest-neighbour search over a 16-bit database on the tensor cores ---------------------------------------------------
+// CTA = two consumer warpgroups (warps 0-7) + one producer warp (warp 8).  Work unit = (query tile of NQ = 8 NT <= 128 queries, database
+// partition of rows_per_part rows); the partition is walked in tiles of KB = 128 rows, 64 per consumer warpgroup.
+//   producer  one thread: per tile and per 64-column chunk of dim, the tile's database box [128 x 64] and the query box [NQ x 64]
+//             (TMA, 128-byte swizzle, zero fill past n_db / n_q / dim) into a KSTAGES-deep mbarrier ring.
+//             (NQ stops at 128: nine warps put three on one SM sub-partition, which leaves 168 registers a thread, too few for
+//             n256's 128 accumulators.)
+//   MMA       S[64 x NQ] = X.Q^T, database rows on the M side, queries on the N side, both K-major in shared memory: k16 steps in
+//             dim order, fp32 accumulators.  The last chunk's zero-filled columns past dim add exact zeros (four steps per chunk
+//             always: a data-dependent step count would serialise the wgmma chain).  A score's operations do not depend on where its row lies in the tile, the
+//             partition or the database, so its bits depend on the query and the row alone.
+//   select    per query the CTA keeps a candidate buffer in global memory (cap = kk + 2 KB entries) and a threshold theta in shared
+//             memory: the kk-th best of the buffer after its last compaction (-inf before).  A score (NaN read as -FLT_MAX) enters
+//             iff it is >= theta (ties are kept: the index order is settled by the sort).  A query whose buffer passed kk + KB entries
+//             is compacted after the tile (bitonic sort in shared memory, best kk kept, theta raised), so one tile never overflows it.
+//   end       every query's buffer is sorted once more and its best kk (padded with (-inf, INT_MAX)) go to the candidate matrix at
+//             [query, partition * kk]; launch_topk_stage's merge passes finish the ranking across partitions.
+constexpr int KB = 128, KC = 64, KSTAGES = 4, KSORT = 2048;      // rows per tile, columns per chunk, ring depth, sort capacity
+constexpr int KNN_THREADS = 288;
+constexpr uint32_t KDB_BYTES = KB * KC * 2;
+
+template <int NT>
+struct KnnGeo {
+    static constexpr int NQ = 8 * NT;
+    static constexpr uint32_t Q_BYTES = NQ * KC * 2, STAGE = KDB_BYTES + Q_BYTES;
+    static constexpr uint32_t SORT_OFF = KSTAGES * STAGE;                     // Cand[KSORT]
+    static constexpr uint32_t THETA_OFF = SORT_OFF + KSORT * 8;               // float[128]
+    static constexpr uint32_t CNT_OFF = THETA_OFF + 128 * 4;                  // int[128]
+    static constexpr uint32_t FLAG_OFF = CNT_OFF + 128 * 4;                   // uint32[4]: queries to compact
+    static constexpr uint32_t BAR_OFF = FLAG_OFF + 32;                        // full[KSTAGES], empty[KSTAGES]
+    static constexpr uint32_t SMEM = BAR_OFF + 16 * KSTAGES + 1024;
+    static_assert(Q_BYTES % 1024 == 0 && STAGE % 1024 == 0 && SMEM <= 227 * 1024, "K10 shared memory");
+};
+
+struct KParams {
+    CUtensorMap tm_db, tm_q;
+    Cand* buf;                      // [grid][NQ][cap]
+    float* out_v; int* out_i;       // [nq, parts * kk], row stride out_ld
+    size_t out_ld;
+    int nq, ndb, nchunks, rows_per_part, parts, kk, cap;
+};
+
+CB_DEVINL void knn_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }        // both consumer warpgroups
+
+template <bool BF, int NT>
+CB_DEVINL void knn_mma(float (&d)[4 * NT], uint64_t da, uint64_t db, uint32_t accumulate) {
+    if constexpr (NT == 16) wgmma_ss_n128<BF>(d, da, db, accumulate);
+    else if constexpr (NT == 8) wgmma_ss_n64<BF>(d, da, db, accumulate);
+    else if constexpr (NT == 4) wgmma_ss_n32<BF>(d, da, db, accumulate);
+    else if constexpr (NT == 2) wgmma_ss_n16<BF>(d, da, db, accumulate);
+    else wgmma_ss_n8<BF>(d, da, db, accumulate);
+}
+
+// Sort query q's n buffered candidates (256 consumer threads) and keep the best kk: back into the buffer with theta raised
+// (final = false), or into the candidate matrix row `orow` (final = true).
+CB_DEVINL void knn_sort_keep(Cand* sc, Cand* b, int n, int kk, bool final, float* theta, int* cnt, float* ov, int* oi) {
+    const int t = threadIdx.x;
+    int m = 1;
+    while (m < n) m <<= 1;
+    for (int e = t; e < m; e += 256) sc[e] = e < n ? b[e] : Cand{-INFINITY, 0x7fffffff};
+    knn_bar();
+    for (int size = 2; size <= m; size <<= 1)
+        for (int stride = size >> 1; stride > 0; stride >>= 1) {
+            for (int u = t; u < (m >> 1); u += 256) {
+                const int lo = 2 * u - (u & (stride - 1)), hi = lo + stride;
+                const bool desc = (lo & size) == 0;
+                const Cand x = sc[lo], y = sc[hi];
+                if (before(y, x) == desc) { sc[lo] = y; sc[hi] = x; }
+            }
+            knn_bar();
+        }
+    if (final) {
+        for (int e = t; e < kk; e += 256) {
+            const Cand x = e < n ? sc[e] : Cand{-INFINITY, 0x7fffffff};
+            ov[e] = x.v; oi[e] = x.i;
+        }
+    } else {
+        for (int e = t; e < kk; e += 256) b[e] = sc[e];
+        if (t == 0) { *theta = sc[kk - 1].v; *cnt = kk; }
+    }
+    knn_bar();
+}
+
+template <bool BF, int NT>
+__global__ void __launch_bounds__(KNN_THREADS, 1) knn16_kernel(const __grid_constant__ KParams p) {
+    using G = KnnGeo<NT>;
+    constexpr int NQ = G::NQ;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    const uint32_t smem_base = smem_u32(smem);
+    const uint32_t full = smem_base + G::BAR_OFF, empty = full + 8 * KSTAGES;
+    Cand* sort_s = reinterpret_cast<Cand*>(smem + G::SORT_OFF);
+    float* theta = reinterpret_cast<float*>(smem + G::THETA_OFF);
+    int* cnt = reinterpret_cast<int*>(smem + G::CNT_OFF);
+    uint32_t* flags = reinterpret_cast<uint32_t*>(smem + G::FLAG_OFF);
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int qt = blockIdx.x / p.parts, part = blockIdx.x - qt * p.parts;
+    const int q0 = qt * NQ, nqv = min(NQ, p.nq - q0);
+    const int row_begin = part * p.rows_per_part, row_end = min(p.ndb, row_begin + p.rows_per_part);
+    const int ntiles = (row_end - row_begin + KB - 1) / KB;
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < KSTAGES; i++) { mbar_init(full + 8 * i, 1); mbar_init(empty + 8 * i, 8); }
+        mbar_fence_init();
+        tma_prefetch_desc(&p.tm_db);
+        tma_prefetch_desc(&p.tm_q);
+    }
+    if (threadIdx.x < 128) { theta[threadIdx.x] = -INFINITY; cnt[threadIdx.x] = 0; }
+    if (threadIdx.x < 4) flags[threadIdx.x] = 0;
+    __syncthreads();
+
+    if (warp == 8) {
+        // ------------------------------------------------------------------ producer (one thread)
+        if (lane == 0) {
+            uint32_t n = 0;
+            for (int t = 0; t < ntiles; t++)
+                for (int c = 0; c < p.nchunks; c++, n++) {
+                    const uint32_t s = n % KSTAGES, st = smem_base + s * G::STAGE;
+                    mbar_wait(empty + 8 * s, ((n / KSTAGES) & 1) ^ 1);
+                    mbar_arrive_expect_tx(full + 8 * s, G::STAGE);
+                    tma_load_2d(st, &p.tm_db, c * KC, row_begin + t * KB, full + 8 * s);
+                    tma_load_2d(st + KDB_BYTES, &p.tm_q, c * KC, q0, full + 8 * s);
+                }
+        }
+        return;
+    }
+
+    // ---------------------------------------------------------------------- consumers (fragment layout: wgmma.cuh)
+    const int wg = warp >> 2, tc = 2 * (lane & 3);
+    const int rr = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // this thread: tile rows rr and rr + 8
+    Cand* const bufq = p.buf + (size_t)blockIdx.x * NQ * p.cap;
+    float d[4 * NT];
+    uint32_t n = 0;
+    for (int t = 0; t < ntiles; t++) {
+        uint32_t prev = 0;
+        for (int c = 0; c < p.nchunks; c++, n++) {
+            const uint32_t s = n % KSTAGES, st = smem_base + s * G::STAGE;
+            mbar_wait(full + 8 * s, (n / KSTAGES) & 1);
+            const uint64_t da = wgmma_desc_sw128(st + (uint32_t)wg * 64u * 128u), dq = wgmma_desc_sw128(st + KDB_BYTES);
+            wgmma_fence();
+            #pragma unroll
+            for (int k = 0; k < 4; k++) knn_mma<BF, NT>(d, da + 2 * k, dq + 2 * k, (uint32_t)(c | k));
+            wgmma_commit();
+            if (c > 0) {                                           // the previous chunk's MMAs have read their stage
+                wgmma_wait<1>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty + 8 * prev);
+            }
+            prev = s;
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(d);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty + 8 * prev);
+
+        // candidates of this tile
+        const int row0 = row_begin + t * KB + rr;
+        #pragma unroll
+        for (int j = 0; j < NT; j++) {
+            #pragma unroll
+            for (int e = 0; e < 4; e++) {
+                const int q = 8 * j + tc + (e & 1), row = row0 + 8 * (e >> 1);
+                float v = d[4 * j + e];
+                v = v != v ? -FLT_MAX : v;
+                if (q < nqv && row < row_end && v >= theta[q]) {
+                    const int pos = atomicAdd(&cnt[q], 1);
+                    *reinterpret_cast<float2*>(bufq + (size_t)q * p.cap + pos) = make_float2(v, __int_as_float(row));
+                    if (pos == p.kk + KB) atomicOr(&flags[q >> 5], 1u << (q & 31));
+                }
+            }
+        }
+        knn_bar();
+        uint32_t fl[(NQ + 31) / 32];
+        bool any = false;
+        #pragma unroll
+        for (int w = 0; w < (NQ + 31) / 32; w++) { fl[w] = flags[w]; any |= fl[w] != 0; }
+        knn_bar();
+        if (any) {                                                 // block-uniform
+            if (threadIdx.x < 4) flags[threadIdx.x] = 0;
+            #pragma unroll
+            for (int w = 0; w < (NQ + 31) / 32; w++)
+                for (uint32_t f = fl[w]; f; f &= f - 1) {
+                    const int q = 32 * w + __ffs(f) - 1;
+                    knn_sort_keep(sort_s, bufq + (size_t)q * p.cap, cnt[q], p.kk, false, &theta[q], &cnt[q], nullptr, nullptr);
+                }
+        }
+    }
+    for (int q = 0; q < nqv; q++) {
+        const size_t o = (size_t)(q0 + q) * p.out_ld + (size_t)part * p.kk;
+        knn_sort_keep(sort_s, bufq + (size_t)q * p.cap, cnt[q], p.kk, true, nullptr, nullptr, p.out_v + o, p.out_i + o);
+    }
+}
+
+typedef CUresult (*EncodeTiledFnK)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+// [rows, dim] 16-bit row-major, boxes of 64 columns x box_rows rows, 128-byte swizzle, zero fill past both ends
+bool make_rows_map(CUtensorMap* out, const void* base, int rows, int dim, int box_rows) {
+    static EncodeTiledFnK enc = nullptr;
+    if (!enc) {
+        void* f = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) return false;
+        enc = reinterpret_cast<EncodeTiledFnK>(f);
+    }
+    const cuuint64_t dims[2] = {(cuuint64_t)dim, (cuuint64_t)rows}, strides[1] = {(cuuint64_t)dim * 2};
+    const cuuint32_t box[2] = {(cuuint32_t)KC, (cuuint32_t)box_rows}, estr[2] = {1, 1};
+    return enc(out, CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+template <bool BF, int NT>
+cudaError_t knn16_launch(const KParams& p, unsigned grid, cudaStream_t st) {
+    constexpr uint32_t smem = KnnGeo<NT>::SMEM;
+    cudaError_t e = cudaFuncSetAttribute(knn16_kernel<BF, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    knn16_kernel<BF, NT><<<grid, KNN_THREADS, smem, st>>>(p);
+    return cudaGetLastError();
+}
+template <bool BF>
+cudaError_t knn16_launch_nt(int nt, const KParams& p, unsigned grid, cudaStream_t st) {
+    switch (nt) {
+        case 1: return knn16_launch<BF, 1>(p, grid, st);
+        case 2: return knn16_launch<BF, 2>(p, grid, st);
+        case 4: return knn16_launch<BF, 4>(p, grid, st);
+        case 8: return knn16_launch<BF, 8>(p, grid, st);
+        default: return knn16_launch<BF, 16>(p, grid, st);
+    }
+}
+
 }  // namespace
 
 void launch_similarity(const float* a, const float* b, float* s, int na, int nb, int d, size_t lds, cudaStream_t st) {
@@ -142,6 +381,36 @@ void launch_topk_stage(const float* vals, const int* in_idx, size_t ld, int rows
     if (rows <= 0 || n <= 0) return;
     dim3 grid((n + SL - 1) / SL, rows);
     topk_stage_kernel<<<grid, 256, 0, st>>>(vals, in_idx, ld, n, idx_base, kk, out_v, out_i, out_ld, out_off);
+}
+
+Knn16Plan knn16_plan(int nq, int ndb, int kk, int sms) {
+    Knn16Plan pl;
+    const int nqc = std::min(nq, 128);
+    pl.nt = 1;
+    while (8 * pl.nt < nqc) pl.nt <<= 1;
+    const int qtiles = (nq + 8 * pl.nt - 1) / (8 * pl.nt);
+    const int max_parts = (ndb + KB - 1) / KB;
+    pl.parts = std::min(std::max(1, sms / qtiles), max_parts);
+    pl.rows_per_part = ((ndb + pl.parts - 1) / pl.parts + KB - 1) / KB * KB;
+    pl.parts = (ndb + pl.rows_per_part - 1) / pl.rows_per_part;
+    pl.grid = qtiles * pl.parts;
+    pl.cap = kk + 2 * KB;
+    pl.buf_entries = (size_t)pl.grid * 8 * pl.nt * pl.cap;
+    return pl;
+}
+
+cudaError_t launch_knn16(const void* q, int nq, const void* db, int ndb, int dim, int bf16, int kk, const Knn16Plan& pl, void* buf,
+                         float* out_v, int* out_i, size_t out_ld, cudaStream_t st) {
+    if (nq <= 0 || ndb <= 0) return cudaSuccess;
+    KParams p;
+    memset(&p, 0, sizeof(p));
+    if (!make_rows_map(&p.tm_db, db, ndb, dim, KB) || !make_rows_map(&p.tm_q, q, nq, dim, 8 * pl.nt)) return cudaErrorInvalidValue;
+    p.buf = reinterpret_cast<Cand*>(buf);
+    p.out_v = out_v; p.out_i = out_i; p.out_ld = out_ld;
+    p.nq = nq; p.ndb = ndb;
+    p.nchunks = (dim + KC - 1) / KC;
+    p.rows_per_part = pl.rows_per_part; p.parts = pl.parts; p.kk = kk; p.cap = pl.cap;
+    return bf16 ? knn16_launch_nt<true>(pl.nt, p, (unsigned)pl.grid, st) : knn16_launch_nt<false>(pl.nt, p, (unsigned)pl.grid, st);
 }
 
 }  // namespace cb

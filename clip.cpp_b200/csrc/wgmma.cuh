@@ -146,4 +146,18 @@ CB_DEVINL void wgmma_rs_n16_bmn(float (&d)[8], const uint32_t (&a)[4], uint64_t 
 #undef CB_WGMMA_RS_N16
 }
 
+// D[64 x 8] (+)= A[64 x 16] . B[8 x 16]^T, both operands K-major in shared memory: the one-query tile of the 16-bit search kernel
+// (search.cu)
+template <bool BF>
+CB_DEVINL void wgmma_ss_n8(float (&d)[4], uint64_t da, uint64_t db, uint32_t accumulate) {
+#define CB_WGMMA_SS_N8(TY)                                                                                 \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %6, 0;\n\t"                                                 \
+                 "wgmma.mma_async.sync.aligned.m64n8k16.f32." TY "." TY " {%0, %1, %2, %3}, %4, %5, p, 1, 1, 0, 0;\n\t}"  \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])  \
+                 : "l"(da), "l"(db), "r"(accumulate))
+    if constexpr (BF) CB_WGMMA_SS_N8("bf16");
+    else CB_WGMMA_SS_N8("f16");
+#undef CB_WGMMA_SS_N8
+}
+
 }  // namespace cb

@@ -304,6 +304,35 @@ bool clip_b200_zero_shot_batch(const struct clip_ctx * ctx, const void * d_img_v
 bool clip_b200_topk_search(const struct clip_ctx * ctx, const void * d_queries, size_t n_queries, const void * d_db, size_t n_db,
                            int top_k, float * scores, int * indices);
 
+/* f32 rows -> f16 / bf16 rows (round to nearest even), device to device: how pooled embeddings (or token rows) become a 16-bit
+ * database or query set for clip_b200_topk_search_16.  d_src [n, dim] f32 and d_dst [n, dim] of out_type (CLIP_B200_OUT_F16 or
+ * CLIP_B200_OUT_BF16), row-major, on the context's GPU, 16-byte aligned; dim a multiple of 4 in [4, 2048]; n < 2^31 (n * dim may
+ * exceed 2^32).  n == 0 returns true.  Returns once the rows are written.  Its time is kernel class 4. */
+bool clip_b200_rows_to_16bit(const struct clip_ctx * ctx, const void * d_src, size_t n, int dim, int out_type, void * d_dst);
+
+/* Nearest-neighbour search over a 16-bit database on the tensor cores (kernel K10), the opt-in companion of clip_b200_topk_search
+ * for databases stored in 16 bits.  No score matrix is written: each CTA keeps its own top_k while it scores.
+ * - Inputs: in_type is CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16.  d_queries [n_queries, dim] and d_db [n_db, dim] are row-major, of
+ *   that type, on the context's GPU, 16-byte aligned.  dim is a multiple of 8 in [8, 2048]; it is an argument, not the model's
+ *   projection_dim (patch-token features can be searched too), and the model's towers are not used.
+ * - Scores: the dot product of the 16-bit query and row; the products are exact in fp32 and accumulated in fp32 on the tensor
+ *   cores, in k16 steps.  Each score lies within (2 * ceil(dim / 16) + 4) * 2^-24 * sum_i |q_i x_i| of the exact value.  A score
+ *   depends only on the query and the row: it has the same bits on every call, whatever n_db, top_k or the row's position.
+ * - Ranking: the best top_k of all n_db scores, score descending, then lower index first, host [n_queries, top_k], row i at
+ *   i * top_k.  A NaN score ranks last and is reported as -FLT_MAX.
+ * - top_k must be in [1, 1024]; a value above n_db means n_db.  Unlike clip_b200_topk_search there is no "all rows" ranking
+ *   on the host: top_k <= 0 or > 1024 is refused.
+ * - Refusals, with a message in clip_b200_last_error, in this order: null context; in_type; dim; top_k; n_queries or n_db >= 2^31;
+ *   then, when there is work (n_queries == 0 or n_db == 0 returns true and writes nothing), null or misaligned device pointers
+ *   and null outputs.
+ * - Runs on the context's first GPU (in devices mode too); the database is not sharded.
+ * - Workspace, grow-only, on the context: per launch of up to 32768 queries (Q of them), with the plan's query tile N = the least
+ *   power of two >= min(Q, 128), at least 8, P partitions and G CTAs (G <= max(#SMs, Q / 128 rounded up), P * ceil(Q / N) = G):
+ *   G * N * (top_k + 256) * 8 bytes of per-CTA candidates, plus 4 * Q * P * top_k * 4 bytes of merge buffers (shared with
+ *   clip_b200_topk_search). */
+bool clip_b200_topk_search_16(const struct clip_ctx * ctx, const void * d_queries, size_t n_queries, const void * d_db, size_t n_db,
+                              int dim, int in_type, int top_k, float * scores, int * indices);
+
 /* Batched zero-shot labelling, the batch form of clip_zero_shot_label_image (clip.h:106-107, clip.cpp:1624-1659): n images x
  * n_labels token sequences -> scores / indices [n, top_k], best first (p = (exp(s)+1e-9)/sum over ALL labels, clip.cpp:1591-1622).
  * normalize = false reproduces the reference (un-normalised embeddings).  Works in every multi-GPU mode (see below): in devices
@@ -367,7 +396,7 @@ uint64_t clip_b200_kernel_launches(const struct clip_ctx * ctx);   /* kernels la
 float    clip_b200_last_device_ms(const struct clip_ctx * ctx);    /* CUDA-event time of the last encode's kernels */
 /* per-kernel-class CUDA-event time accumulated since the last call with the same kind (0 GEMM, 1 attention,
  * 2 layernorm, 3 other, 4 the token-row kernel of the *_tokens calls, 5 the position-table resample of the *_hw calls, 6 the
- * attention-probability kernel of ATTENTION entries); *count
+ * attention-probability kernel of ATTENTION entries, 7 the 16-bit search kernel of clip_b200_topk_search_16); *count
  * receives the number of launches.  Enabled by env CLIP_B200_PROFILE=1. */
 float    clip_b200_kernel_ms(const struct clip_ctx * ctx, int kind, uint64_t * count);
 /* CUDA-event stopwatch on the launch stream: mark(slot 0..3), then elapsed(a, b) in ms (-1 on error) */
