@@ -66,7 +66,7 @@ EXTENSION_SYMBOLS = [
     "clip_b200_host_malloc", "clip_b200_host_free", "clip_b200_memcpy_h2d", "clip_b200_memcpy_d2h",
     "clip_b200_synchronize", "clip_b200_last_error", "clip_b200_kernel_launches",
     "clip_b200_last_device_ms", "clip_b200_version", "clip_b200_set_micro_batch",
-    "clip_b200_debug_gemm", "clip_b200_debug_attention", "clip_b200_debug_attention_hd", "clip_b200_image_batch_encode_u8",
+    "clip_b200_debug_gemm", "clip_b200_debug_gemm_scaled", "clip_b200_debug_attention", "clip_b200_debug_attention_hd", "clip_b200_image_batch_encode_u8",
     "clip_b200_image_batch_preprocess_device", "clip_b200_get_stream", "clip_b200_kernel_ms",
     "clip_b200_debug_repack_roundtrip", "clip_b200_debug_tokenize", "clip_b200_debug_preprocess",
     "clip_b200_mark", "clip_b200_mark_elapsed_ms",
@@ -216,6 +216,8 @@ class ClipLib:
             L.clip_b200_debug_attention_probs.argtypes = [ip, ip, ip, ip, ip, ip, ip, ip, fp, vp]
             L.clip_b200_debug_gemm.restype = C.c_int
             L.clip_b200_debug_gemm.argtypes = [ip, ip, ip, ip, ip, ip, ip, fp, vp, fp, fp, fp, C.POINTER(C.c_float)]
+            L.clip_b200_debug_gemm_scaled.restype = C.c_int
+            L.clip_b200_debug_gemm_scaled.argtypes = [ip, ip, ip, ip, ip, ip, ip, C.c_float, fp, vp, fp, fp, fp, C.POINTER(C.c_float)]
             i32p = C.POINTER(C.c_int32)
             for f, args in (("clip_b200_debug_layernorm", [ip, ip, C.c_size_t, C.c_float, fp, fp, fp, fp, ip, fp, fp]),
                             ("clip_b200_debug_assemble_preln", [fp, fp, fp, ip, ip, ip, C.c_float, fp, fp, fp]),

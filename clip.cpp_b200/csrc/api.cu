@@ -1957,8 +1957,8 @@ float clip_b200_kernel_ms(const struct clip_ctx* cc, int kind, uint64_t* count) 
     return total;
 }
 
-int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int epi, int use_naive, const float* x, const void* w_rows,
-                         const float* bias, const float* resid_in, float* y_out, float* ms) {
+int clip_b200_debug_gemm_scaled(int qtype, int operand_bf16, int M, int N, int K, int epi, int use_naive, float scale, const float* x,
+                                const void* w_rows, const float* bias, const float* resid_in, float* y_out, float* ms) {
     g_err.clear();
     if (gemm_init() != cudaSuccess) { set_err("gemm_init failed"); return 1; }
     int dev = 0;
@@ -2012,13 +2012,13 @@ int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int e
         if (eff_q == QT_F16 && !make_tma_2d_16bit(&wm, d_w, N, K, K, GEMM_BM)) { set_err("tensor map W failed"); rc = 4; break; }
         cudaEventRecord(e0, st);
         if (use_naive) {
-            launch_naive_gemm(d_x, operand_bf16, d_raw, eff_q, d_bias, d_out, M, N, K, N, epi, operand_bf16, N / 2, 0.125f, st);
+            launch_naive_gemm(d_x, operand_bf16, d_raw, eff_q, d_bias, d_out, M, N, K, N, epi, operand_bf16, N / 2, scale, st);
             e = cudaGetLastError();
         } else {
             GemmArgs a;
             a.x_map = &xm; a.w_map = &wm; a.w_packed = (const uint8_t*)d_w; a.qtype = eff_q; a.operand_bf16 = operand_bf16 != 0;
             a.bias = d_bias; a.out = d_out; a.M = M; a.N = N; a.K = K; a.ldo = N; a.epi = epi; a.out_bf16 = operand_bf16;
-            a.scale_cols = N / 2; a.scale = 0.125f;
+            a.scale_cols = N / 2; a.scale = scale;
             e = gemm_launch(a, st, prop.multiProcessorCount, nullptr);
         }
         cudaEventRecord(e1, st);
@@ -2041,6 +2041,11 @@ int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int e
     cudaFree(d_x); cudaFree(d_out); cudaFree(d_raw); if (d_w && d_w != d_raw) cudaFree(d_w); cudaFree(d_bias);
     cudaEventDestroy(e0); cudaEventDestroy(e1); cudaStreamDestroy(st);
     return rc;
+}
+
+int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int epi, int use_naive, const float* x, const void* w_rows,
+                         const float* bias, const float* resid_in, float* y_out, float* ms) {
+    return clip_b200_debug_gemm_scaled(qtype, operand_bf16, M, N, K, epi, use_naive, 0.125f, x, w_rows, bias, resid_in, y_out, ms);
 }
 
 

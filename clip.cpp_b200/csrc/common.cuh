@@ -139,17 +139,24 @@ struct P2<true> {    // bf16: 0x4300 = 128.0, one ulp = 1
     CB_DEVINL static float to_float(uint16_t b) { return __uint_as_float((uint32_t)b << 16); }
 };
 
-CB_DEVINL float gelu_tanh(float x) {   // reference formula: ggml/src/ggml.c:3756-3758
-    const float u = 0.79788456080286535587989211986876f * x * (1.0f + 0.044715f * x * x);
-    float t;
-    asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(u));
-    return 0.5f * x * (1.0f + t);
+// x * sigmoid(y) for a = y log2(e): x / (1 + 2^-a) when a >= 0, x 2^a / (1 + 2^a) when a < 0, so the one exponential is
+// e = 2^-|a| in (0, 1] and the denominator stays in [1, 2].  Not 0.5 x (1 + tanh(y / 2)): for y < 0 that cancels, and the
+// absolute error of tanh.approx (relative 2^-11 near -1) becomes a relative error of the result that grows without bound.
+// ex2.approx.ftz (relative error 2^-22) computes 2^64 e, so that e down to 2^-190 stays normal: x e is then right wherever a
+// 16-bit result can be normal.  1/d by rcp.approx (relative error about 2^-23): two MUFU operations per element where tanh.approx
+// took one.  A reciprocal from a linear start and two Newton steps on the FMA pipe instead measured slower in K1's epilogue (DESIGN
+// section 6).  a = +-inf gives x and -+0.
+CB_DEVINL float mul_sigmoid_exp2(float x, float a) {
+    float es, r;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(es) : "f"(64.0f - fabsf(a)));
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(fmaf(es, 0x1p-64f, 1.0f)));
+    return (a >= 0.0f ? x : (x * es) * 0x1p-64f) * r;
 }
-CB_DEVINL float gelu_quick(float x) {  // x * sigmoid(1.702 x): ggml/src/ggml.c:3783-3785; sigmoid(z) = 0.5 + 0.5 tanh(z/2): one MUFU
-    float t;
-    asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.851f * x));
-    return x * fmaf(0.5f, t, 0.5f);
-}
+// tanh-GELU, reference formula ggml/src/ggml.c:3756-3758: 0.5 x (1 + tanh(u)) = x sigmoid(2u), u = sqrt(2/pi) x (1 + 0.044715 x^2);
+// 2u log2(e) = x (C0 + C1 x^2) with C0 = 2 sqrt(2/pi) log2(e), C1 = 0.044715 C0
+CB_DEVINL float gelu_tanh(float x) { return mul_sigmoid_exp2(x, x * fmaf(0.10294323958f, x * x, 2.3022081981f)); }
+// quick-GELU x sigmoid(1.702 x), ggml/src/ggml.c:3783-3785; 1.702 log2(e) = 2.45546695959
+CB_DEVINL float gelu_quick(float x) { return mul_sigmoid_exp2(x, 2.4554669596f * x); }
 
 
 // host side: launch with the PDL attribute (and optionally as clusters of `cluster_x` CTAs)

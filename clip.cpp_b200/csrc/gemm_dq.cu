@@ -196,17 +196,13 @@ CB_DEVINL void fence_frag(uint32_t (&a)[16]) {
 
 // 16-bit epilogue value of one accumulator element.  EPI_STORE16 rounds (acc + b) to fp32 before the scale, the reference's order
 // (ggml_add then ggml_scale, clip.cpp:1082, 1363): the Q scale 1/sqrt(80) of head_dim 80 is not a power of two, so a single FFMA
-// with a pre-scaled bias would round differently.  For 1/sqrt(64) = 0.125 the two forms give the same bits.
-// quick-GELU x * sigmoid(1.702 x) = h + h * tanh(0.851 x) with h = x / 2.
+// with a pre-scaled bias would round differently.  For 1/sqrt(64) = 0.125 the two forms give the same bits.  The GELUs are
+// common.cuh's, which the scalar debug kernel runs too.
 template <int EPI>
 CB_DEVINL float epi_value(float acc, float bias, float mul) {
     if constexpr (EPI == EPI_GELU16) return gelu_tanh(acc + bias);
-    else if constexpr (EPI == EPI_QGELU16) {
-        const float x = acc + bias, h = 0.5f * x;
-        float t;
-        asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.851f * x));
-        return fmaf(h, t, h);
-    } else return (acc + bias) * mul;
+    else if constexpr (EPI == EPI_QGELU16) return gelu_quick(acc + bias);
+    else return (acc + bias) * mul;
 }
 
 // ---- epilogue staging: bulk tensor stores (and, for the residual add, loads) between the staging slots and the output matrix

@@ -407,10 +407,16 @@ const char * clip_b200_version(void);
 
 /* TEST HOOK: run one fused-dequant GEMM  Y[M,N] = X[M,K] . W[N,K]^T (+bias) on device 0.
  * w_rows: ggml-format rows of type qtype; x: fp32 host [M,K] (rounded to the operand type on the way in);
- * y_out: fp32 host [M,N].  use_naive=1 runs the scalar debug kernel instead.  Returns 0 on success, 5 if the GEMM wrote into the
- * poisoned guard rows that follow row M of its output buffer. */
+ * y_out: fp32 host [M,N].  use_naive=1 runs the scalar debug kernel instead.  EPI_STORE16 scales the first N/2 features by 0.125
+ * (the Q scale of head_dim 64).  Returns 0 on success, 5 if the GEMM wrote into the poisoned guard rows that follow row M of its
+ * output buffer. */
 int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int epi, int use_naive, const float * x,
                          const void * w_rows, const float * bias, const float * resid_in, float * y_out, float * ms);
+/* the same with the Q scale as an argument: EPI_STORE16 writes (acc + bias) * scale on the first N/2 features, as the fused QKV
+ * GEMM does with 1/sqrt(head_dim) (1/sqrt(80) for head_dim 80 is not a power of two) */
+int clip_b200_debug_gemm_scaled(int qtype, int operand_bf16, int M, int N, int K, int epi, int use_naive, float scale,
+                                const float * x, const void * w_rows, const float * bias, const float * resid_in, float * y_out,
+                                float * ms);
 
 /* N1 (SURVEY.md section 8f) -- clip_image_batch_preprocess (clip.h:98, clip.cpp:963-1008) on the device, fused with the encode:
  * raw u8 RGB images of any size are uploaded (3 B/pixel), resized (PIL-style antialiased bicubic, a = -0.5), centre-cropped and

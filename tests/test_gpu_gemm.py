@@ -6,6 +6,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import _epilogue_rule as rule
 import oracle as orc
 
 pytestmark = pytest.mark.gpu
@@ -83,16 +84,25 @@ def unpacked(wdesc, bf16):
     return round16((q.astype(np.float64) * d16 + m16).astype(np.float32), bf16)
 
 
-def run_gemm(prod, qt, bf16, M, N, K, epi, x, raw, bias, resid=None, naive=0):
+def run_gemm(prod, qt, bf16, M, N, K, epi, x, raw, bias, resid=None, naive=0, scale=0.125):
+    """scale: the Q scale EPI_STORE16 applies to the first N/2 features (0.125 = 1/sqrt(64) unless a test asks otherwise)"""
     y = np.empty((M, N), np.float32)
     ms = C.c_float(0)
     fp = C.POINTER(C.c_float)
     buf = np.frombuffer(raw, np.uint8)
-    rc = prod.lib.clip_b200_debug_gemm(QT[qt], int(bf16), M, N, K, epi, naive, x.ctypes.data_as(fp), buf.ctypes.data,
-                                       bias.ctypes.data_as(fp) if bias is not None else None,
-                                       resid.ctypes.data_as(fp) if resid is not None else None, y.ctypes.data_as(fp), C.byref(ms))
+    rc = prod.lib.clip_b200_debug_gemm_scaled(QT[qt], int(bf16), M, N, K, epi, naive, scale, x.ctypes.data_as(fp), buf.ctypes.data,
+                                              bias.ctypes.data_as(fp) if bias is not None else None,
+                                              resid.ctypes.data_as(fp) if resid is not None else None, y.ctypes.data_as(fp),
+                                              C.byref(ms))
     assert rc == 0, prod.last_error()
     return y, ms.value
+
+
+def check_gelu(prod, qt, bf16, M, N, K, epi, x, raw, bias, y):
+    """a GELU epilogue's 16-bit result y against the rule of tests/_epilogue_rule.py, at the fp32 value v that EPI_STORE32 gives for
+    the same call (the same accumulator: tests/test_gpu_gemm_epilogue_exact.py)"""
+    v, _ = run_gemm(prod, qt, bf16, M, N, K, EPI_STORE32, x, raw, bias)
+    return rule.check(y, v, "gelu" if epi == EPI_GELU16 else "qgelu", bf16, (qt, M, N, K))
 
 
 def expected(x, deq, bias, bf16, epi, resid, N):
@@ -139,6 +149,8 @@ def test_gemm_epilogues(prod, epi, bf16):
     bias = rng.standard_normal(N).astype(np.float32)
     resid = rng.standard_normal((M, N)).astype(np.float32)
     y, _ = run_gemm(prod, "q4_0", bf16, M, N, K, epi, x, raw, bias, resid)
+    if epi in (EPI_GELU16, EPI_QGELU16):
+        check_gelu(prod, "q4_0", bf16, M, N, K, epi, x, raw, bias, y)
     ref = expected(x, deq, bias, bf16, epi, resid, N)
     tol = 2e-2 if epi in (EPI_STORE16, EPI_GELU16, EPI_QGELU16) else 2e-3     # one 16-bit output ulp at |v|~2
     assert np.abs(y - ref).max() <= tol * max(1.0, np.abs(ref).max()), (epi, bf16, np.abs(y - ref).max())
@@ -205,6 +217,8 @@ def test_gemm_f16_weights_epilogues(prod, epi):
     bias = rng.standard_normal(N).astype(np.float32)
     resid = rng.standard_normal((M, N)).astype(np.float32)
     y, _ = run_gemm(prod, "f16", False, M, N, K, epi, x, raw, bias, resid)
+    if epi in (EPI_GELU16, EPI_QGELU16):
+        check_gelu(prod, "f16", False, M, N, K, epi, x, raw, bias, y)
     ref = expected(x, deq, bias, False, epi, resid, N)
     tol = 2e-2 if epi in (EPI_STORE16, EPI_GELU16, EPI_QGELU16) else 2e-3
     assert np.abs(y - ref).max() <= tol * max(1.0, np.abs(ref).max()), (epi, np.abs(y - ref).max())
@@ -290,5 +304,7 @@ def test_gemm_wide_form_tails_and_epilogues(prod, M, epi):
     bias = rng.standard_normal(N).astype(np.float32)
     resid = rng.standard_normal((M, N)).astype(np.float32)
     y, _ = run_gemm(prod, "q4_0", True, M, N, K, epi, x, raw, bias, resid)
+    if epi == EPI_QGELU16:
+        check_gelu(prod, "q4_0", True, M, N, K, epi, x, raw, bias, y)
     ref = expected(x, deq, bias, True, epi, resid, N)
     assert np.abs(y - ref).max() <= 2e-2 * max(1.0, np.abs(ref).max())

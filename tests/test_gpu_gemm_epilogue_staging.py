@@ -5,9 +5,12 @@ several tiles and reuses each slot many times.  The hook fills one token tile pa
 any of it changes, so every call here also checks that rows past M are never written.
 
 STORE32 is checked against an fp64 restatement; the other epilogues against STORE32 from the same call site: the residual add bit for
-bit as x0 + v, the 16-bit store bit for bit as v times the column scale rounded once, the GELUs to one 16-bit ulp."""
+bit as x0 + v, the 16-bit store bit for bit as v times the column scale rounded once, the GELUs by the rule of
+tests/_epilogue_rule.py at v (one 16-bit ulp where the result is normal)."""
 import numpy as np
 import pytest
+
+import _epilogue_rule as rule
 
 from test_gpu_gemm import (EPI_GELU16, EPI_QGELU16, EPI_REDADD32, EPI_STORE16, EPI_STORE32, expected, make_weight, round16,
                            run_gemm)
@@ -46,11 +49,6 @@ def test_staged_epilogues(prod, qt, bf16, N, tail):
     s[:, :N // 2] *= np.float32(0.125)   # the hook's Q scale on the first N/2 features: a power of two, exact
     assert same_bits(y, round16(s, bf16)), (qt, N, M)
 
-    for epi in (EPI_GELU16, EPI_QGELU16):
+    for fn, epi in (("gelu", EPI_GELU16), ("qgelu", EPI_QGELU16)):
         y, _ = run_gemm(prod, qt, bf16, M, N, K, epi, x, raw, bias)
-        if epi == EPI_GELU16:
-            want = 0.5 * v * (1 + np.tanh(0.7978845608 * v * (1 + 0.044715 * v * v)))
-        else:
-            want = v / (1 + np.exp(-1.702 * v))
-        want = round16(want.astype(np.float32), bf16)
-        assert np.abs(y - want).max() <= 2e-2 * max(1.0, np.abs(want).max()), (qt, N, M, epi)
+        rule.check(y, v, fn, bf16, (qt, N, M))

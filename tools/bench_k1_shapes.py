@@ -20,8 +20,9 @@ sys.path.insert(0, os.path.join(ROOT, "clip.cpp_b200"))
 import binding  # noqa: E402
 
 EPI = {"STORE16": 0, "GELU16": 1, "QGELU16": 2, "REDADD32": 3, "STORE32": 4}
+# (N, K, epilogue); the last four are the FC1 GEMMs of ViT-L/14 (4096 x 1024) and ViT-H/14 (5120 x 1280) under both GELUs
 SHAPES = [(1024, 1024, "REDADD32"), (1024, 1024, "STORE32"), (1024, 4096, "REDADD32"), (1024, 4096, "STORE32"),
-          (3072, 1024, "STORE16"), (4096, 1024, "QGELU16")]
+          (3072, 1024, "STORE16"), (4096, 1024, "QGELU16"), (4096, 1024, "GELU16"), (5120, 1280, "GELU16"), (5120, 1280, "QGELU16")]
 
 
 def q4_0_rows(N, K, rng):
@@ -37,6 +38,7 @@ def main():
     ap.add_argument("--lib", default=binding.PRODUCT_LIB)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--M", type=int, default=132 * 192)
+    ap.add_argument("--epi", default="", help="comma-separated epilogues to run (default: every shape)")
     args = ap.parse_args()
     lib = binding.ClipLib(args.lib)
     rng = np.random.default_rng(0)
@@ -44,6 +46,8 @@ def main():
     fp = C.POINTER(C.c_float)
     out = {"lib": os.path.basename(args.lib), "M": M, "shapes": []}
     for N, K, epi in SHAPES:
+        if args.epi and epi not in args.epi.split(","):
+            continue
         x = rng.standard_normal((M, K)).astype(np.float32)
         raw = np.frombuffer(q4_0_rows(N, K, rng), np.uint8)
         bias = rng.standard_normal(N).astype(np.float32)
