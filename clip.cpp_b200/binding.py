@@ -90,6 +90,8 @@ EXTENSION_SYMBOLS = [
     "clip_b200_text_tokens_layers_device",
     # attention probabilities (TOKENS_ATTENTION entries)
     "clip_b200_debug_attention_probs",
+    # head_dim 104 (ViT-bigG/14): the loader's QKV row padding
+    "clip_b200_debug_pad_qkv",
 ]
 
 # include/clip_b200.h: output types and flags of the *_tokens entry points
@@ -279,6 +281,8 @@ class ClipLib:
             L.clip_b200_nccl_version.argtypes = []
             L.clip_b200_cuda_device_count.restype = C.c_int
             L.clip_b200_cuda_device_count.argtypes = []
+            L.clip_b200_debug_pad_qkv.restype = C.c_int
+            L.clip_b200_debug_pad_qkv.argtypes = [ip, ip, ip, ip, ip, vp, vp]
             L.clip_b200_debug_rendezvous.restype = C.c_int
             L.clip_b200_debug_rendezvous.argtypes = [ip, ip, C.c_char_p, vp]
             L.clip_b200_debug_shard_bounds.restype = None

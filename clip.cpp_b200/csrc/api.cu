@@ -127,18 +127,36 @@ bool upload_f32(clip_ctx* c, const GgufFile& g, const std::string& name, float**
     return upload(c, out, h.data(), h.size() * 4);
 }
 
-// GEMM weight from one or more row-concatenated tensors (fused QKV).  kpad > 0 zero-pads K (patch embedding).
+// Columns of a tower's fused QKV activations: Q | K | V, each heads x qkv_head_cols(head_dim) (head_dim 104 pads each head to 112).
+int qkv_width(const Tower& tw) { return 3 * tw.heads * qkv_head_cols(tw.hidden / tw.heads); }
+
+// GEMM weight from one or more row-concatenated tensors (fused QKV).  kpad > 0 zero-pads K (patch embedding).  head_dim > 0 pads
+// the rows (and bias) of every part to qkv_head_cols(head_dim) per head of head_dim rows, with zero rows (pad_head_rows).
 bool make_linear(clip_ctx* c, const GgufFile& g, const std::vector<std::string>& wn, const std::vector<std::string>& bn, Linear& L,
-                 int kpad = 0) {
+                 int kpad = 0, int head_dim = 0) {
     std::vector<const GgufTensor*> ts;
     for (auto& n : wn) { const GgufTensor* t = need(g, n); if (!t) return false; ts.push_back(t); }
     const uint32_t type = ts[0]->type;
     int64_t K = 1;
     for (uint32_t d = 0; d + 1 < std::max(ts[0]->n_dims, 2u); d++) K *= (int64_t)ts[0]->ne[d];   // 4-D conv weight: K = P*P*3
+    const int dhp = head_dim > 0 ? qkv_head_cols(head_dim) : 0;
+    const bool pad = dhp > head_dim;
     int64_t N = 0;
-    for (auto* t : ts) {
+    std::vector<std::vector<uint8_t>> padded(ts.size());
+    std::vector<const uint8_t*> src(ts.size());       // each part's rows, padded if asked
+    std::vector<int64_t> part_rows(ts.size());
+    for (size_t i = 0; i < ts.size(); i++) {
+        const GgufTensor* t = ts[i];
         if (t->type != type || (int64_t)(t->nelements() / (t->ne[ts[0]->n_dims - 1])) != K) { set_err("inconsistent fused weight " + wn[0]); return false; }
-        N += (int64_t)t->ne[t->n_dims - 1];
+        const int64_t rows = (int64_t)t->ne[t->n_dims - 1];
+        src[i] = t->data; part_rows[i] = rows;
+        if (pad) {
+            const size_t rb = t->nbytes / (size_t)rows;
+            padded[i].resize((size_t)(rows / head_dim) * dhp * rb);
+            if (!pad_head_rows(t->data, rb, rows, head_dim, dhp, padded[i].data())) { set_err("weight " + wn[i] + " is not a whole number of heads"); return false; }
+            src[i] = padded[i].data(); part_rows[i] = rows / head_dim * dhp;
+        }
+        N += part_rows[i];
     }
     const int64_t Kp = kpad > 0 ? kpad : K;
     if (N % GEMM_BM || Kp % GEMM_BK) { set_err("weight " + wn[0] + ": shape [" + std::to_string(N) + "," + std::to_string(Kp) + "] is not tileable (N%128, K%64)"); return false; }
@@ -147,12 +165,12 @@ bool make_linear(clip_ctx* c, const GgufFile& g, const std::vector<std::string>&
         L.qtype = QT_F16;
         std::vector<uint16_t> h((size_t)N * Kp, 0);
         int64_t r0 = 0;
-        for (auto* t : ts) {
-            const int64_t rows = (int64_t)t->ne[t->n_dims - 1];
+        for (size_t i = 0; i < ts.size(); i++) {
+            const int64_t rows = part_rows[i];
             for (int64_t r = 0; r < rows; r++) {
                 uint16_t* dst = h.data() + (size_t)(r0 + r) * Kp;
-                if (type == 1) memcpy(dst, t->data + (size_t)r * K * 2, (size_t)K * 2);
-                else { const float* s = (const float*)(t->data) + (size_t)r * K; for (int64_t k = 0; k < K; k++) dst[k] = f32_to_f16(s[k]); }
+                if (type == 1) memcpy(dst, src[i] + (size_t)r * K * 2, (size_t)K * 2);
+                else { const float* s = (const float*)(src[i]) + (size_t)r * K; for (int64_t k = 0; k < K; k++) dst[k] = f32_to_f16(s[k]); }
             }
             r0 += rows;
         }
@@ -166,17 +184,21 @@ bool make_linear(clip_ctx* c, const GgufFile& g, const std::vector<std::string>&
         if (!chunk) { set_err("unsupported weight type in " + wn[0]); return false; }
         std::vector<uint8_t> packed(wpack_total_bytes((int)type, N, K));
         int64_t r0 = 0;
-        for (auto* t : ts) {
-            const int64_t rows = (int64_t)t->ne[1];
+        for (size_t i = 0; i < ts.size(); i++) {
+            const int64_t rows = part_rows[i];
             if (rows % GEMM_BM) { set_err("fused part of " + wn[0] + " is not a multiple of 128 rows"); return false; }
-            if (!wpack_repack((int)type, t->data, rows, K, packed.data() + (size_t)(r0 / GEMM_BM) * (K / GEMM_BK) * chunk)) { set_err("re-tiling failed for " + wn[0]); return false; }
+            if (!wpack_repack((int)type, src[i], rows, K, packed.data() + (size_t)(r0 / GEMM_BM) * (K / GEMM_BK) * chunk)) { set_err("re-tiling failed for " + wn[0]); return false; }
             r0 += rows;
         }
         if (!upload(c, &L.d_w, packed.data(), packed.size())) return false;
         if (c->debug_naive) {
             std::vector<uint8_t> raw((size_t)N * (K / 32) * bb);
             size_t o = 0;
-            for (auto* t : ts) { memcpy(raw.data() + o, t->data, t->nbytes); o += t->nbytes; }
+            for (size_t i = 0; i < ts.size(); i++) {
+                const size_t nb = (size_t)part_rows[i] * (K / 32) * bb;
+                memcpy(raw.data() + o, src[i], nb);
+                o += nb;
+            }
             if (!upload(c, &L.d_raw, raw.data(), raw.size())) return false;
         }
     }
@@ -186,8 +208,15 @@ bool make_linear(clip_ctx* c, const GgufFile& g, const std::vector<std::string>&
             const GgufTensor* t = need(g, n);
             if (!t) return false;
             if (t->type != 0) { set_err("bias " + n + " must be f32"); return false; }
-            const float* p = (const float*)t->data;
-            hb.insert(hb.end(), p, p + t->nelements());
+            const int64_t ne = (int64_t)t->nelements();
+            if (pad) {
+                std::vector<float> pb((size_t)(ne / head_dim) * dhp);
+                if (!pad_head_rows(t->data, 4, ne, head_dim, dhp, reinterpret_cast<uint8_t*>(pb.data()))) { set_err("bias " + n + " is not a whole number of heads"); return false; }
+                hb.insert(hb.end(), pb.begin(), pb.end());
+            } else {
+                const float* p = (const float*)t->data;
+                hb.insert(hb.end(), p, p + ne);
+            }
         }
         if ((int64_t)hb.size() != N) { set_err("bias size mismatch for " + wn[0]); return false; }
         if (!upload(c, &L.d_bias, hb.data(), hb.size() * 4)) return false;
@@ -201,11 +230,11 @@ bool load_blocks(clip_ctx* c, const GgufFile& g, const char* p, Tower& tw) {
         const std::string b = std::string(p) + ".blk." + std::to_string(il) + ".";
         Layer& l = tw.L[il];
         if (!make_linear(c, g, {b + "attn_q.weight", b + "attn_k.weight", b + "attn_v.weight"},
-                         {b + "attn_q.bias", b + "attn_k.bias", b + "attn_v.bias"}, l.qkv)) return false;
+                         {b + "attn_q.bias", b + "attn_k.bias", b + "attn_v.bias"}, l.qkv, 0, tw.hidden / tw.heads)) return false;
         if (!make_linear(c, g, {b + "attn_out.weight"}, {b + "attn_out.bias"}, l.out)) return false;
         if (!make_linear(c, g, {b + "ffn_down.weight"}, {b + "ffn_down.bias"}, l.fc1)) return false;   // HF fc1: h -> f
         if (!make_linear(c, g, {b + "ffn_up.weight"}, {b + "ffn_up.bias"}, l.fc2)) return false;       // HF fc2: f -> h
-        if (l.qkv.N != 3 * tw.hidden || l.qkv.K != tw.hidden || l.out.N != tw.hidden || l.out.K != tw.hidden ||
+        if (l.qkv.N != qkv_width(tw) || l.qkv.K != tw.hidden || l.out.N != tw.hidden || l.out.K != tw.hidden ||
             l.fc1.N != tw.ff || l.fc1.K != tw.hidden || l.fc2.N != tw.hidden || l.fc2.K != tw.ff) { set_err("layer shape mismatch in " + b); return false; }
         if (!upload_f32(c, g, b + "ln1.weight", &l.ln1_g, tw.hidden) || !upload_f32(c, g, b + "ln1.bias", &l.ln1_b, tw.hidden) ||
             !upload_f32(c, g, b + "ln2.weight", &l.ln2_g, tw.hidden) || !upload_f32(c, g, b + "ln2.bias", &l.ln2_b, tw.hidden)) return false;
@@ -216,7 +245,8 @@ bool load_blocks(clip_ctx* c, const GgufFile& g, const char* p, Tower& tw) {
 bool check_geometry(const clip_ctx* c, const char* what, const Tower& t) {
     if (t.hidden <= 0 || t.ff <= 0 || t.heads <= 0 || t.layers < 0 || t.layers > 1024 || t.proj <= 0 || !(t.eps >= 0.f)) { set_err(std::string(what) + ": non-positive hyper-parameter in the file"); return false; }
     const std::string hh = " (hidden " + std::to_string(t.hidden) + ", heads " + std::to_string(t.heads) + ")";
-    if (t.heads <= 0 || t.hidden % t.heads || (t.hidden / t.heads != 64 && t.hidden / t.heads != 80)) { set_err(std::string(what) + ": head_dim must be 64 or 80" + hh); return false; }
+    const int dh = t.heads > 0 && t.hidden % t.heads == 0 ? t.hidden / t.heads : 0;
+    if (dh != 64 && dh != 80 && dh != 104) { set_err(std::string(what) + ": head_dim must be 64 or 80 (ViT-B/L/H) or 104 (ViT-bigG/14)" + hh); return false; }
     if (!c->attn_tc && t.hidden / t.heads != 64) { set_err(std::string(what) + ": the legacy attention kernel (CLIP_B200_ATTN=legacy) supports head_dim 64 only" + hh); return false; }
     if (t.hidden > 2048) { set_err(std::string(what) + ": hidden size > 2048 is not supported by the register-resident LayerNorm"); return false; }
     if (t.hidden % 128 || t.ff % 128 || t.proj % 128) { set_err(std::string(what) + ": hidden/ff/projection sizes must be multiples of 128"); return false; }
@@ -239,7 +269,7 @@ bool ensure_ws(clip_ctx* c, Tower& tw, int items, int T, bool vision) {
     // Row counts are ints, and every GEMM of a pass addresses its output (and the patch GEMM its input) with 32-bit element offsets
     // (gemm_launch): refuse a micro_batch past either limit here, before anything is allocated, so the context stays usable.
     const size_t rows = (size_t)items * (size_t)T;
-    const size_t widest = std::max({(size_t)3 * h, (size_t)tw.ff, (size_t)tw.proj, vision ? (size_t)tw.kpad : (size_t)0});
+    const size_t widest = std::max({(size_t)qkv_width(tw), (size_t)tw.ff, (size_t)tw.proj, vision ? (size_t)tw.kpad : (size_t)0});
     if (rows > (size_t)INT_MAX || rows * widest >= ((size_t)1 << 32)) {
         const size_t limit = std::min((size_t)INT_MAX / T, (((size_t)1 << 32) - 1) / (widest * T));
         set_err(std::string(vision ? "vision" : "text") + " micro_batch " + std::to_string(items) + " is too large: " + std::to_string(rows) +
@@ -248,7 +278,7 @@ bool ensure_ws(clip_ctx* c, Tower& tw, int items, int T, bool vision) {
         return false;
     }
     w.cap_items = items; w.T = T; w.cap_rows = (int)rows;
-    if (!dev_alloc(c, &w.x, rows * h) || !dev_alloc(c, &w.a, rows * h) || !dev_alloc(c, &w.qkv, rows * 3 * h) ||
+    if (!dev_alloc(c, &w.x, rows * h) || !dev_alloc(c, &w.a, rows * h) || !dev_alloc(c, &w.qkv, rows * qkv_width(tw)) ||
         !dev_alloc(c, &w.g, rows * tw.ff) || !dev_alloc(c, &w.sel16, (size_t)items * h) || !dev_alloc(c, &w.sel32, (size_t)items * h) ||
         !dev_alloc(c, &w.proj32, (size_t)items * tw.proj)) return false;
     bool ok = make_tma_2d_16bit(&w.map_a, w.a, rows, h, h, GEMM_BN) && make_tma_2d_16bit(&w.map_g, w.g, rows, tw.ff, tw.ff, GEMM_BN) &&
@@ -289,12 +319,13 @@ bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal, int first,
     Workspace& w = tw.ws;
     const int M = nseq * T, h = tw.hidden;
     const int bf = c->operand_bf16 ? 1 : 0;
-    const int dh = h / tw.heads;                      // 64 or 80 (check_geometry)
-    const float qscale = 1.0f / sqrtf((float)dh);     // clip.cpp:1082, 1363
+    const int dh = h / tw.heads;                      // 64, 80 or 104 (check_geometry)
+    const float qscale = 1.0f / sqrtf((float)dh);     // clip.cpp:1082, 1363: the real head_dim, not the padded one
+    const int qw = qkv_width(tw);
     for (int il = first; il < end; il++) {
         const Layer& l = tw.L[il];
         { Scope s(c, K_LN); launch_layernorm(w.x, h, M, h, tw.eps, l.ln1_g, l.ln1_b, nullptr, w.a, bf, c->stream); }
-        if (!run_linear(c, l.qkv, &w.map_a, w.a, bf, M, w.qkv, 3 * h, EPI_STORE16, bf, h, qscale)) return false;
+        if (!run_linear(c, l.qkv, &w.map_a, w.a, bf, M, w.qkv, qw, EPI_STORE16, bf, qw / 3, qscale)) return false;
         if (c->attn_tc) { Scope s(c, K_ATTN); CK(launch_attention_tc(w.qkv, w.a, nseq, T, tw.heads, dh, causal ? 1 : 0, bf, c->stream)); }
         else { Scope s(c, K_ATTN); launch_attention(w.qkv, w.a, nseq, T, tw.heads, causal ? 1 : 0, bf, c->stream); }
         if (!run_linear(c, l.out, &w.map_a, w.a, bf, M, w.x, h, EPI_REDADD32, 0)) return false;
@@ -701,7 +732,7 @@ extern "C" {
 const char* clip_b200_last_error(void) { return g_err.c_str(); }
 const char* clip_b200_version(void) { return "clip_b200 0.1 (sm_90a; wgmma fused-dequant GEMM)"; }
 
-// one replica of the model on `device` (weights are <= 0.33 GB: replicated, never sharded -- SURVEY.md section 8e)
+// one replica of the model on `device` (weights, at most about 5 GB for ViT-bigG/14 in f16: replicated, never sharded -- SURVEY.md section 8e)
 static clip_ctx* load_on_device(const GgufFile& g, int device, const int verbosity) {
     {
         std::unique_ptr<clip_ctx, void (*)(clip_ctx*)> guard(new clip_ctx, [](clip_ctx* p) { clip_free(p); });
@@ -2049,17 +2080,32 @@ int clip_b200_debug_gemm(int qtype, int operand_bf16, int M, int N, int K, int e
 }
 
 
+// The hooks' qkv [rows, 3*H*dh] (fp32) as the model's 16-bit QKV activations: rounded to the operand type, and each head padded to
+// qkv_head_cols(dh) columns with zeros, as the loader's padded QKV projection leaves them.
+static std::vector<uint16_t> qkv_to16_padded(const float* qkv, size_t rows, int H, int dh, int bf16) {
+    const int dhp = qkv_head_cols(dh);
+    const size_t parts = (size_t)3 * H, src_cols = parts * dh, cols = parts * dhp;
+    std::vector<uint16_t> h16(rows * cols, 0);
+    for (size_t r = 0; r < rows; r++)
+        for (size_t ph = 0; ph < parts; ph++)
+            for (int d = 0; d < dh; d++) {
+                const float v = qkv[r * src_cols + ph * dh + d];
+                h16[r * cols + ph * dhp + d] = bf16 ? f32_to_bf16(v) : f32_to_f16(v);
+            }
+    return h16;
+}
+
 // TEST HOOK: one attention launch on device 0.  qkv: fp32 host [nseq*T, 3*H*dh] (columns Q | K | V, the Q columns already scaled),
-// rounded to the operand type on the way in; out: fp32 host [nseq*T, H*dh].  use_legacy=1 runs the mma.sync flash kernel (dh 64).
+// rounded to the operand type on the way in (and padded as qkv_to16_padded does); out: fp32 host [nseq*T, H*dh].  use_legacy=1 runs
+// the mma.sync flash kernel (dh 64).
 int clip_b200_debug_attention_hd(int operand_bf16, int nseq, int T, int H, int head_dim, int causal, int use_legacy, const float* qkv,
                                  float* out, float* ms) {
     g_err.clear();
-    if (head_dim != 64 && head_dim != 80) { set_err("attention: head_dim must be 64 or 80"); return 2; }
+    if (head_dim != 64 && head_dim != 80 && head_dim != 104) { set_err("attention: head_dim must be 64 or 80 (ViT-B/L/H) or 104 (ViT-bigG/14)"); return 2; }
     if (use_legacy && head_dim != 64) { set_err("attention: the legacy kernel supports head_dim 64 only"); return 2; }
     if (attention_tc_init() != cudaSuccess) { set_err("attention_tc_init failed"); return 1; }
-    const size_t rows = (size_t)nseq * T, hid = (size_t)H * head_dim;
-    std::vector<uint16_t> h16(rows * 3 * hid);
-    for (size_t i = 0; i < h16.size(); i++) h16[i] = operand_bf16 ? f32_to_bf16(qkv[i]) : f32_to_f16(qkv[i]);
+    const size_t rows = (size_t)nseq * T, hid = (size_t)H * head_dim, qcols = (size_t)3 * H * qkv_head_cols(head_dim);
+    const std::vector<uint16_t> h16 = qkv_to16_padded(qkv, rows, H, head_dim, operand_bf16);
     uint16_t *d_qkv = nullptr, *d_out = nullptr;
     cudaStream_t st = nullptr;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -2067,10 +2113,10 @@ int clip_b200_debug_attention_hd(int operand_bf16, int nseq, int T, int H, int h
     do {
         cudaError_t e;
         // one 128-row box of padding past the last sequence
-        if ((e = cudaMalloc(&d_qkv, (rows + 128) * 3 * hid * 2)) != cudaSuccess || (e = cudaMalloc(&d_out, rows * hid * 2)) != cudaSuccess) { set_err(std::string("cudaMalloc: ") + cudaGetErrorString(e)); rc = 3; break; }
+        if ((e = cudaMalloc(&d_qkv, (rows + 128) * qcols * 2)) != cudaSuccess || (e = cudaMalloc(&d_out, rows * hid * 2)) != cudaSuccess) { set_err(std::string("cudaMalloc: ") + cudaGetErrorString(e)); rc = 3; break; }
         // the padding is POISONED (0xFFFF = NaN in fp16 and bf16): rows past the last sequence are stale memory in the model path
         // (ensure_ws never initialises the workspace tail), and no output may depend on them
-        cudaMemset(d_qkv, 0xff, (rows + 128) * 3 * hid * 2);
+        cudaMemset(d_qkv, 0xff, (rows + 128) * qcols * 2);
         cudaMemset(d_out, 0xff, rows * hid * 2);
         cudaMemcpy(d_qkv, h16.data(), h16.size() * 2, cudaMemcpyHostToDevice);
         cudaStreamCreate(&st); cudaEventCreate(&e0); cudaEventCreate(&e1);
@@ -2340,20 +2386,20 @@ int clip_b200_debug_token_rows(int n, int T, int h, size_t in_stride, int no_cls
     return s.copy_back(out, d_out, out_bytes) ? 0 : 6;
 }
 
-// K9 on qkv (fp32 host [nseq*T, 3*H*head_dim], rounded to the operand type on the way in; one 128-row box of poisoned rows follows
-// the last sequence, as in clip_b200_debug_attention_hd).  Poisoned guard bytes follow the output.
+// K9 on qkv (fp32 host [nseq*T, 3*H*head_dim], rounded to the operand type and padded on the way in; one 128-row box of poisoned
+// rows follows the last sequence, as in clip_b200_debug_attention_hd).  Poisoned guard bytes follow the output.
 int clip_b200_debug_attention_probs(int operand_bf16, int nseq, int T, int H, int head_dim, int causal, int cls_row, int out_type,
                                     const float* qkv, void* out) {
     g_err.clear();
-    if ((head_dim != 64 && head_dim != 80) || nseq <= 0 || T <= 0 || H <= 0 || out_type < 0 || out_type > 2 || !qkv || !out) {
-        set_err("debug_attention_probs: bad arguments (head_dim 64 or 80, positive sizes, out_type 0..2)");
+    if ((head_dim != 64 && head_dim != 80 && head_dim != 104) || nseq <= 0 || T <= 0 || H <= 0 || out_type < 0 || out_type > 2 || !qkv || !out) {
+        set_err("debug_attention_probs: bad arguments (head_dim 64 or 80, or 104; positive sizes, out_type 0..2)");
         return 2;
     }
     HookScratch s;
     if (s.ok && attention_tc_init() != cudaSuccess) { set_err("attention_tc_init failed"); return 1; }
-    const size_t rows = (size_t)nseq * T, cols = (size_t)3 * H * head_dim, guard = 4096;
+    const size_t rows = (size_t)nseq * T, cols = (size_t)3 * H * qkv_head_cols(head_dim), guard = 4096;
     const size_t out_bytes = (size_t)nseq * H * (cls_row ? 1 : T) * T * (out_type == 0 ? 4 : 2);
-    const std::vector<uint16_t> q16 = to16(qkv, rows * cols, operand_bf16);
+    const std::vector<uint16_t> q16 = qkv_to16_padded(qkv, rows, H, head_dim, operand_bf16);
     void* d_qkv = s.alloc((rows + 128) * cols * 2, 0xff, q16.data(), q16.size() * 2);
     uint8_t* d_out = (uint8_t*)s.alloc(out_bytes + guard, 0xff);
     if (!s.ok) return 3;
@@ -2368,6 +2414,17 @@ int clip_b200_debug_attention_probs(int operand_bf16, int nseq, int T, int H, in
 
 
 // ---- CPU-only test hooks (no context / GPU needed) ----------------------------------------------------------
+// The loader's QKV row padding (pad_head_rows) on one fused part or the whole Q | K | V: src holds 3*H*dh rows of a [*, K] weight of
+// ggml type qtype (0 f32, 1 f16, or a block type; qtype 0 with K = 1 is a bias), out receives 3*H*dhp rows.  dhp must be
+// qkv_head_cols(dh) or any other value >= dh.
+int clip_b200_debug_pad_qkv(int qtype, int H, int dh, int dhp, int K, const void* src, void* out) {
+    g_err.clear();
+    const size_t bb = qtype == 0 ? 4 : qtype == 1 ? 2 : wpack_ggml_block_bytes(qtype), be = qtype <= 1 ? 1 : 32;
+    if (H <= 0 || dh <= 0 || dhp < dh || K <= 0 || !bb || K % be || !src || !out) { set_err("debug_pad_qkv: bad arguments"); return 1; }
+    const size_t rb = (size_t)K / be * bb;
+    return pad_head_rows((const uint8_t*)src, rb, (int64_t)3 * H * dh, dh, dhp, (uint8_t*)out) ? 0 : 1;
+}
+
 // ranks-mode rendezvous of the NCCL unique id (dist.cpp) without a GPU: rank 0 publishes, the others read the same 128 bytes
 int clip_b200_debug_rendezvous(int rank, int world, const char* path, void* out128) {
     std::string e;

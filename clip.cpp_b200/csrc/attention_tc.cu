@@ -1,7 +1,8 @@
 // attention_tc.cu -- K3 on Hopper tensor cores: S = Q K^T and O = P V as warpgroup MMAs (wgmma), online softmax in registers.
 //
 // Reference semantics: clip.cpp:1082-1108 (text, causal) / 1363-1388 (vision); soft_max ggml.c:12201-12270.
-// Persistent: min(iterations, SMs) CTAs of 288 threads, 161 KB (head_dim 64) or 201 KB (head_dim 80) of shared memory.  The work unit is
+// Persistent: min(iterations, SMs) CTAs of 288 threads, 161 KB (head_dim 64), 201 KB (head_dim 80) or 225 KB (head_dim 104) of
+// shared memory.  The work unit is
 // a GROUP of 64 query rows, numbered in (sequence, head, group) order; iteration `it` of the launch takes groups 2it and 2it + 1, one
 // per consumer warpgroup, and CTA b runs iterations b, b + grid, ...  So the CTAs running at one time cover consecutive groups, and the
 // K / V blocks of a (sequence, head) are read from HBM about once and then from L2.  A group never holds a row past T; only the odd
@@ -23,6 +24,11 @@
 // head (the tensor map's zero fill stops only at token and matrix ends, not at head boundaries).  So every Q / K / V box arrives
 // as two pieces from two tensor maps over the same buffer: columns 0-63 (128-byte swizzle) and 64-79 (32-byte swizzle).  S takes
 // one extra k16 step on the tail pieces, O one extra m64n16k16 wgmma per 16 keys into 8 more accumulators per thread.
+// head_dim 104 (ViT-bigG/14): the loader pads each head of the QKV projection to 112 columns, the last 8 exactly zero
+// (qkv_head_cols), and every box arrives as three pieces: columns 0-63 (128-byte swizzle), 64-95 (64-byte swizzle) and 96-111
+// (32-byte swizzle).  The zero columns add exact zeros to S and give O columns that are never stored, and no piece reaches into
+// the next head.  S takes 4 + 2 + 1 k16 steps, O n64 + n32 + n16 per 16 keys (56 accumulators).  A 224-byte row makes a 128-key
+// K / V tile 28 KB, so this instance runs 64-key blocks in a ring of three stages (225 KB of shared memory in all).
 // Any T; a causal group stops at its own diagonal.
 #include <cuda.h>
 
@@ -39,24 +45,37 @@ constexpr int AG = 64, AK = 128;                       // query rows per group, 
 constexpr int ABOX = 64;                               // rows per TMA box
 constexpr int ATT_THREADS = 288;                       // 2 consumer warpgroups + 1 producer warp
 
-// Shared-memory layout for one head_dim.  A TILE is [128 rows x 64 columns] (128-byte swizzle), followed for head_dim 80 by
-// [128 rows x 16 columns] (32-byte swizzle); a 64-row box fills half of each part.  Two Q tiles (rows 0-63: the first group, 64-127: the
-// second), then two stages of two head slots [K | V].
+// Shared-memory layout for one head_dim.  A head's columns arrive as up to three pieces, each a row-major block of its own: columns
+// 0-63 (128-byte swizzle), at head_dim 104 columns 64-95 (64-byte swizzle), and the last 16 columns (32-byte swizzle: 64-79 at
+// head_dim 80, 96-111 of the 112-column padded head at 104).  A tile of R rows is the R-row blocks of its pieces one after the
+// other; a 64-row box fills a 64-row slice of each.  Two Q tiles of 128 rows (rows 0-63: the first group, 64-127: the second), then
+// NST stages of two head slots [K | V], each tile KB keys.  Head_dim 104 takes 64-key blocks: its 224-byte rows would need 280 KB
+// at 128 keys and two stages.
 template <int DH>
 struct AttnGeo {
-    static_assert(DH == 64 || DH == 80, "head_dim 64 or 80");
-    static constexpr bool TAIL = DH == 80;
-    static constexpr uint32_t MAIN = AK * 128, TILE = MAIN + (TAIL ? AK * 32 : 0);
-    static constexpr uint32_t BOX_BYTES = ABOX * (128 + (TAIL ? 32 : 0));      // one 64-row box, both pieces
+    static_assert(DH == 64 || DH == 80 || DH == 104, "head_dim 64, 80 or 104");
+    static constexpr bool MID = DH == 104, TAIL = DH != 64;
+    static constexpr int DHP = qkv_head_cols(DH);                   // columns per head in the qkv matrix
+    static constexpr int tail_col() { return MID ? 96 : 64; }       // first column of the 16-column tail piece
+    static constexpr uint32_t ROW_BYTES = 128 + (MID ? 64 : 0) + (TAIL ? 32 : 0);
+    static constexpr int KB = MID ? 64 : AK;                        // keys per K / V block
+    static constexpr int NST = MID ? 3 : 2;                         // K / V ring stages
+    static constexpr uint32_t MAIN = AK * 128, TILE = AK * ROW_BYTES;          // a 128-row (Q) tile: its first piece, all of it
+    static constexpr uint32_t KTILE = KB * ROW_BYTES;                          // a K or V tile
+    static constexpr uint32_t BOX_BYTES = ABOX * ROW_BYTES;                    // one 64-row box, every piece
     static constexpr uint32_t KV_OFF = 2 * TILE;
-    static constexpr uint32_t BAR_OFF = KV_OFF + 8 * TILE;
-    static constexpr uint32_t SMEM = BAR_OFF + 64 + 1024;
-    static_assert(2 * AG == AK && 2 * ABOX == AK && MAIN % 1024 == 0 && TILE % 1024 == 0, "tile alignment");
+    static constexpr uint32_t BAR_OFF = KV_OFF + NST * 4 * KTILE;
+    static constexpr uint32_t SMEM = BAR_OFF + 32 + 16 * NST + 1024;
+    // offsets of the mid and tail pieces in a tile of `rows` rows
+    static constexpr uint32_t mid_off(int rows) { return (uint32_t)rows * 128; }
+    static constexpr uint32_t tail_off(int rows) { return (uint32_t)rows * (128 + (MID ? 64 : 0)); }
+    static_assert(2 * AG == AK && 2 * ABOX == AK && MAIN % 1024 == 0 && TILE % 1024 == 0 && KTILE % 1024 == 0, "tile alignment");
+    static_assert(SMEM <= 227 * 1024, "shared memory per block");
 };
 
 struct AParams {
     CUtensorMap tm_qkv;     // boxes of columns 0-63 of a head
-    CUtensorMap tm_tail;    // head_dim 80: boxes of columns 64-79
+    CUtensorMap tm_tail;    // head_dim 80 / 104: boxes of the 16-column tail piece
     uint16_t* out;
     int T, H, causal;
     int ngrp;               // 64-row groups per (sequence, head)
@@ -94,12 +113,13 @@ CB_DEVINL Group group_of(const AParams& p, int g) {
 
 // The two groups of iteration `it` and what the K / V stages hold for them: slot 0 the first group's head (and the second's, when it
 // is the same (sequence, head) or there is no second group), slot 1 the second group's head otherwise.  kend0 / kend1: the keys a
-// slot must hold (0: slot unused); nkb: key blocks of the iteration.
+// slot must hold (0: slot unused); nkb: key blocks (of KB keys) of the iteration.
 struct Iter {
     Group a, b;
     bool has_b, shared;
     int kend0, kend1, nkb;
 };
+template <int KB>
 CB_DEVINL Iter iter_of(const AParams& p, int it) {
     Iter r;
     r.has_b = 2 * it + 1 < p.ngroups;
@@ -108,22 +128,24 @@ CB_DEVINL Iter iter_of(const AParams& p, int it) {
     r.shared = r.a.seq == r.b.seq && r.a.head == r.b.head;
     r.kend0 = r.shared ? max(r.a.kend, r.b.kend) : r.a.kend;
     r.kend1 = r.shared ? 0 : r.b.kend;
-    r.nkb = (max(r.kend0, r.kend1) + AK - 1) / AK;
+    r.nkb = (max(r.kend0, r.kend1) + KB - 1) / KB;
     return r;
 }
 
-// 64-row boxes of key block kb that a slot holding keys [0, kend) needs
+// 64-row boxes of key block kb (KB keys) that a slot holding keys [0, kend) needs
+template <int KB>
 CB_DEVINL int kv_boxes(int kend, int kb) {
-    const int key0 = kb * AK;
-    return key0 >= kend ? 0 : key0 + ABOX >= kend ? 1 : 2;
+    const int key0 = kb * KB;
+    return key0 >= kend ? 0 : (KB == ABOX || key0 + ABOX >= kend) ? 1 : 2;
 }
 
-// one 64-row box (both pieces at head_dim 80) into box `b` of the tile at `tile`
-template <int DH>
-CB_DEVINL void load_box(uint32_t tile, int b, const AParams& p, int col, int row, int seq, uint32_t bar) {
+// one 64-row box (every piece) into box `b` of the `rows`-row tile at `tile`; tm_mid: the head_dim 104 map of columns 64-95
+template <int DH, int ROWS>
+CB_DEVINL void load_box(uint32_t tile, int b, const AParams& p, const CUtensorMap& tm_mid, int col, int row, int seq, uint32_t bar) {
     using G = AttnGeo<DH>;
     tma_load_3d(tile + (uint32_t)b * (ABOX * 128), &p.tm_qkv, col, row, seq, bar);
-    if constexpr (G::TAIL) tma_load_3d(tile + G::MAIN + (uint32_t)b * (ABOX * 32), &p.tm_tail, col + 64, row, seq, bar);
+    if constexpr (G::MID) tma_load_3d(tile + G::mid_off(ROWS) + (uint32_t)b * (ABOX * 64), &tm_mid, col + 64, row, seq, bar);
+    if constexpr (G::TAIL) tma_load_3d(tile + G::tail_off(ROWS) + (uint32_t)b * (ABOX * 32), &p.tm_tail, col + G::tail_col(), row, seq, bar);
 }
 
 template <bool BF, int NT>
@@ -137,8 +159,8 @@ CB_DEVINL void wgmma_ss_nt(float (&d)[4 * NT], uint64_t da, uint64_t db, uint32_
 // One key block of one consumer warpgroup, S NT n-tiles (8 keys each) wide: keys [key0, key0 + 8 NT) of the stage at k_s / v_s.
 // The same operations in the same order as the full 128-key block: the keys past 8 NT would only have been masked to -inf.
 template <bool BF, int DH, int NT>
-CB_DEVINL void attend_block(float (&o)[32], float (&ot)[8], float (&m_run)[2], float (&l_run)[2], uint64_t dq, uint64_t dq_t,
-                            uint32_t k_s, uint32_t v_s, int key0, int T, int causal, int wrow0, int r0, int tc) {
+CB_DEVINL void attend_block(float (&o)[32], float (&om)[16], float (&ot)[8], float (&m_run)[2], float (&l_run)[2], uint64_t dq,
+                            uint64_t dq_m, uint64_t dq_t, uint32_t k_s, uint32_t v_s, int key0, int T, int causal, int wrow0, int r0, int tc) {
     using G = AttnGeo<DH>;
     constexpr float LOG2E = 1.4426950408889634f;
     float sc[4 * NT];
@@ -146,7 +168,12 @@ CB_DEVINL void attend_block(float (&o)[32], float (&ot)[8], float (&m_run)[2], f
     wgmma_fence();
     #pragma unroll
     for (int k = 0; k < 4; k++) wgmma_ss_nt<BF, NT>(sc, dq + 2 * k, dk + 2 * k, (uint32_t)k);
-    if constexpr (G::TAIL) wgmma_ss_nt<BF, NT>(sc, dq_t, wgmma_desc_sw32(k_s + G::MAIN), 1u);
+    if constexpr (G::MID) {
+        const uint64_t dkm = wgmma_desc_sw64(k_s + G::mid_off(G::KB));
+        #pragma unroll
+        for (int k = 0; k < 2; k++) wgmma_ss_nt<BF, NT>(sc, dq_m + 2 * k, dkm + 2 * k, 1u);
+    }
+    if constexpr (G::TAIL) wgmma_ss_nt<BF, NT>(sc, dq_t, wgmma_desc_sw32(k_s + G::tail_off(G::KB)), 1u);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs(sc);
@@ -182,6 +209,10 @@ CB_DEVINL void attend_block(float (&o)[32], float (&ot)[8], float (&m_run)[2], f
         m_run[h] = m_new;
         #pragma unroll
         for (int j = 0; j < 8; j++) { o[4 * j + 2 * h] *= alpha; o[4 * j + 2 * h + 1] *= alpha; }
+        if constexpr (G::MID) {
+            #pragma unroll
+            for (int j = 0; j < 4; j++) { om[4 * j + 2 * h] *= alpha; om[4 * j + 2 * h + 1] *= alpha; }
+        }
         if constexpr (G::TAIL) {
             #pragma unroll
             for (int j = 0; j < 2; j++) { ot[4 * j + 2 * h] *= alpha; ot[4 * j + 2 * h + 1] *= alpha; }
@@ -195,65 +226,69 @@ CB_DEVINL void attend_block(float (&o)[32], float (&ot)[8], float (&m_run)[2], f
         const uint32_t a[4] = {pack2<BF>(sc[8 * kk], sc[8 * kk + 1]), pack2<BF>(sc[8 * kk + 2], sc[8 * kk + 3]),
                                pack2<BF>(sc[8 * kk + 4], sc[8 * kk + 5]), pack2<BF>(sc[8 * kk + 6], sc[8 * kk + 7])};
         wgmma_rs_n64_bmn<BF>(o, a, wgmma_desc_sw128(v_s + (uint32_t)kk * 2048u), 1u);      // 16 keys = 2048 B of V
-        if constexpr (G::TAIL) wgmma_rs_n16_bmn<BF>(ot, a, wgmma_desc_sw32(v_s + G::MAIN + (uint32_t)kk * 512u), 1u);   // 512 B
+        if constexpr (G::MID) wgmma_rs_n32_bmn<BF>(om, a, wgmma_desc_sw64(v_s + G::mid_off(G::KB) + (uint32_t)kk * 1024u), 1u);   // 1024 B
+        if constexpr (G::TAIL) wgmma_rs_n16_bmn<BF>(ot, a, wgmma_desc_sw32(v_s + G::tail_off(G::KB) + (uint32_t)kk * 512u), 1u);  // 512 B
     }
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs(o);
+    if constexpr (G::MID) wgmma_fence_regs(om);
     if constexpr (G::TAIL) wgmma_fence_regs(ot);
 }
 
+// tm_mid: head_dim 104's map of columns 64-95 (unused otherwise; a parameter of its own, so AParams keeps its layout)
 template <bool BF, int DH>
-__global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __grid_constant__ AParams p) {
+__global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __grid_constant__ AParams p, const __grid_constant__ CUtensorMap tm_mid) {
     using G = AttnGeo<DH>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     const uint32_t smem_base = smem_u32(smem);
-    // rings of two, [0|1] = +8 bytes: Q tile full / empty, K-V stage full / empty
-    const uint32_t q_full = smem_base + G::BAR_OFF, q_empty = q_full + 16, kv_full = q_full + 32, kv_empty = q_full + 48;
+    // [i] = +8i bytes: Q tile full / empty (rings of two), K-V stage full / empty (rings of NST)
+    const uint32_t q_full = smem_base + G::BAR_OFF, q_empty = q_full + 16, kv_full = q_full + 32, kv_empty = kv_full + 8 * G::NST;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        for (int i = 0; i < 2; i++) {
-            mbar_init(q_full + 8 * i, 1); mbar_init(q_empty + 8 * i, 8);          // released by each consumer warp
+        for (int i = 0; i < G::NST; i++) {
+            if (i < 2) { mbar_init(q_full + 8 * i, 1); mbar_init(q_empty + 8 * i, 8); }      // released by each consumer warp
             mbar_init(kv_full + 8 * i, 1); mbar_init(kv_empty + 8 * i, 8);
         }
         mbar_fence_init();
         tma_prefetch_desc(&p.tm_qkv);
+        if constexpr (G::MID) tma_prefetch_desc(&tm_mid);
         if constexpr (G::TAIL) tma_prefetch_desc(&p.tm_tail);
     }
     __syncthreads();
     pdl_trigger();
     pdl_wait();      // qkv is read (and the output written) only after the QKV GEMM grid has completed
 
-    const int hid = p.H * DH;
+    const int hid = p.H * DH, qcols = p.H * G::DHP;           // output row, and Q / K / V part of a qkv row
     // Ring positions run on across iterations: the i-th iteration of this CTA uses Q tile i % 2 (its (i / 2)-th use), the n-th key
-    // block of this CTA stage n % 2 (its (n / 2)-th use).  A use waits for full with the use's parity and, in the producer, for the
+    // block of this CTA stage n % NST (its (n / NST)-th use).  A use waits for full with the use's parity and, in the producer, for the
     // release of the previous use of the slot (parity flipped: the first wait on a fresh barrier passes).
     if (warp == 8) {
         // ------------------------------------------------------------------ producer (one thread)
         if (lane == 0) {
             uint32_t n = 0, i = 0;
             for (int it = blockIdx.x; it < p.niter; it += gridDim.x, i++) {
-                const Iter w = iter_of(p, it);
+                const Iter w = iter_of<G::KB>(p, it);
                 const uint32_t qb = i & 1, q_s = smem_base + qb * G::TILE;
                 mbar_wait(q_empty + 8 * qb, ((i >> 1) & 1) ^ 1);
                 mbar_arrive_expect_tx(q_full + 8 * qb, (w.has_b ? 2 : 1) * G::BOX_BYTES);
-                load_box<DH>(q_s, 0, p, w.a.head * DH, w.a.g0, w.a.seq, q_full + 8 * qb);
-                if (w.has_b) load_box<DH>(q_s, 1, p, w.b.head * DH, w.b.g0, w.b.seq, q_full + 8 * qb);
+                load_box<DH, AK>(q_s, 0, p, tm_mid, w.a.head * G::DHP, w.a.g0, w.a.seq, q_full + 8 * qb);
+                if (w.has_b) load_box<DH, AK>(q_s, 1, p, tm_mid, w.b.head * G::DHP, w.b.g0, w.b.seq, q_full + 8 * qb);
                 for (int kb = 0; kb < w.nkb; kb++, n++) {
-                    const uint32_t s = n & 1, bar = kv_full + 8 * s;
-                    const int nb0 = kv_boxes(w.kend0, kb), nb1 = kv_boxes(w.kend1, kb);
-                    mbar_wait(kv_empty + 8 * s, ((n >> 1) & 1) ^ 1);
+                    const uint32_t s = n % G::NST, bar = kv_full + 8 * s;
+                    const int nb0 = kv_boxes<G::KB>(w.kend0, kb), nb1 = kv_boxes<G::KB>(w.kend1, kb);
+                    mbar_wait(kv_empty + 8 * s, ((n / G::NST) & 1) ^ 1);
                     mbar_arrive_expect_tx(bar, (uint32_t)(nb0 + nb1) * 2 * G::BOX_BYTES);
-                    const uint32_t slot0 = smem_base + G::KV_OFF + s * (4 * G::TILE), slot1 = slot0 + 2 * G::TILE;
+                    const uint32_t slot0 = smem_base + G::KV_OFF + s * (4 * G::KTILE), slot1 = slot0 + 2 * G::KTILE;
                     for (int b = 0; b < nb0; b++) {
-                        load_box<DH>(slot0, b, p, hid + w.a.head * DH, kb * AK + b * ABOX, w.a.seq, bar);
-                        load_box<DH>(slot0 + G::TILE, b, p, 2 * hid + w.a.head * DH, kb * AK + b * ABOX, w.a.seq, bar);
+                        load_box<DH, G::KB>(slot0, b, p, tm_mid, qcols + w.a.head * G::DHP, kb * G::KB + b * ABOX, w.a.seq, bar);
+                        load_box<DH, G::KB>(slot0 + G::KTILE, b, p, tm_mid, 2 * qcols + w.a.head * G::DHP, kb * G::KB + b * ABOX, w.a.seq, bar);
                     }
                     for (int b = 0; b < nb1; b++) {
-                        load_box<DH>(slot1, b, p, hid + w.b.head * DH, kb * AK + b * ABOX, w.b.seq, bar);
-                        load_box<DH>(slot1 + G::TILE, b, p, 2 * hid + w.b.head * DH, kb * AK + b * ABOX, w.b.seq, bar);
+                        load_box<DH, G::KB>(slot1, b, p, tm_mid, qcols + w.b.head * G::DHP, kb * G::KB + b * ABOX, w.b.seq, bar);
+                        load_box<DH, G::KB>(slot1 + G::KTILE, b, p, tm_mid, 2 * qcols + w.b.head * G::DHP, kb * G::KB + b * ABOX, w.b.seq, bar);
                     }
                 }
             }
@@ -266,33 +301,37 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __gr
     const int tc = 2 * (lane & 3);                             // this thread: columns 8j + tc + {0, 1}
     uint32_t n = 0, i = 0;
     for (int it = blockIdx.x; it < p.niter; it += gridDim.x, i++) {
-        const Iter w = iter_of(p, it);
+        const Iter w = iter_of<G::KB>(p, it);
         const Group g = group_of(p, min(2 * it + wg, p.ngroups - 1));
         const bool live = wg == 0 || w.has_b;                  // warpgroup-uniform: only the launch's last, odd group leaves one idle
         const uint32_t slot = (wg == 0 || w.shared) ? 0u : 1u;
-        const int nkb = (g.kend + AK - 1) / AK;
+        const int nkb = (g.kend + G::KB - 1) / G::KB;
         const int wrow0 = g.g0 + (warp & 3) * 16;              // first query row of this warp
         const int r0 = wrow0 + (lane >> 2);                    // this thread: rows r0 and r0 + 8
-        // o: columns 0-63, ot: columns 64-79 (head_dim 80 only)
-        float o[32], ot[8], m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+        // o: columns 0-63, om: 64-95 (head_dim 104 only), ot: the 16-column tail (head_dim 80, 104)
+        float o[32], om[16], ot[8], m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
         #pragma unroll
         for (int j = 0; j < 32; j++) o[j] = 0.f;
+        #pragma unroll
+        for (int j = 0; j < 16; j++) om[j] = 0.f;
         #pragma unroll
         for (int j = 0; j < 8; j++) ot[j] = 0.f;
         const uint32_t qb = i & 1, q_s = smem_base + qb * G::TILE;
         mbar_wait(q_full + 8 * qb, (i >> 1) & 1);
         const uint64_t dq = wgmma_desc_sw128(q_s + (uint32_t)wg * 64u * 128u);
-        const uint64_t dq_t = wgmma_desc_sw32(q_s + G::MAIN + (uint32_t)wg * 64u * 32u);
+        const uint64_t dq_m = wgmma_desc_sw64(q_s + G::mid_off(AK) + (uint32_t)wg * 64u * 64u);
+        const uint64_t dq_t = wgmma_desc_sw32(q_s + G::tail_off(AK) + (uint32_t)wg * 64u * 32u);
         for (int kb = 0; kb < w.nkb; kb++, n++) {
-            const uint32_t s = n & 1;
-            const uint32_t k_s = smem_base + G::KV_OFF + s * (4 * G::TILE) + slot * (2 * G::TILE), v_s = k_s + G::TILE;
-            mbar_wait(kv_full + 8 * s, (n >> 1) & 1);
+            const uint32_t s = n % G::NST;
+            const uint32_t k_s = smem_base + G::KV_OFF + s * (4 * G::KTILE) + slot * (2 * G::KTILE), v_s = k_s + G::KTILE;
+            mbar_wait(kv_full + 8 * s, (n / G::NST) & 1);
             if (live && kb < nkb) {
-                const int key0 = kb * AK, rem = g.kend - key0;
-                if (rem > 64) attend_block<BF, DH, 16>(o, ot, m_run, l_run, dq, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
-                else if (rem > 32) attend_block<BF, DH, 8>(o, ot, m_run, l_run, dq, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
-                else if (rem > 16) attend_block<BF, DH, 4>(o, ot, m_run, l_run, dq, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
-                else attend_block<BF, DH, 2>(o, ot, m_run, l_run, dq, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
+                const int key0 = kb * G::KB, rem = g.kend - key0;
+                // S at the narrowest width that covers the keys left (a 64-key block never needs 128)
+                if (G::KB == 128 && rem > 64) attend_block<BF, DH, 16>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
+                else if (rem > 32) attend_block<BF, DH, 8>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
+                else if (rem > 16) attend_block<BF, DH, 4>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
+                else attend_block<BF, DH, 2>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(kv_empty + 8 * s);
@@ -313,10 +352,16 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __gr
                 #pragma unroll
                 for (int j = 0; j < 8; j++)
                     *reinterpret_cast<uint32_t*>(orow + 8 * j + tc) = pack2<BF>(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
-                if constexpr (G::TAIL) {
+                if constexpr (G::MID) {
                     #pragma unroll
-                    for (int j = 0; j < 2; j++)
-                        *reinterpret_cast<uint32_t*>(orow + 64 + 8 * j + tc) = pack2<BF>(ot[4 * j + 2 * h] * inv, ot[4 * j + 2 * h + 1] * inv);
+                    for (int j = 0; j < 4; j++)
+                        *reinterpret_cast<uint32_t*>(orow + 64 + 8 * j + tc) = pack2<BF>(om[4 * j + 2 * h] * inv, om[4 * j + 2 * h + 1] * inv);
+                }
+                if constexpr (G::TAIL) {
+                    // the real tail columns only: at head_dim 104, columns 104-111 are the padding
+                    #pragma unroll
+                    for (int j = 0; j < (DH - G::tail_col()) / 8; j++)
+                        *reinterpret_cast<uint32_t*>(orow + G::tail_col() + 8 * j + tc) = pack2<BF>(ot[4 * j + 2 * h] * inv, ot[4 * j + 2 * h + 1] * inv);
                 }
             }
         }
@@ -336,10 +381,13 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __gr
 constexpr int PROBS_THREADS = 160;
 constexpr int PSTRIDE = AK + 8;          // staging row stride in elements: a warp's fragment stores of 4 rows fill 32 distinct banks
 
+// Q: one box in a tile of QROWS rows (head_dim 104: a 64-row tile, so that two CTAs fit on an SM; 64 and 80 keep the half-used
+// 128-row tile they always had); then the two K stages of 128-row tiles.
 template <int DH>
 struct ProbsGeo {
     using G = AttnGeo<DH>;
-    static constexpr uint32_t K_OFF = G::TILE;                        // Q: box 0 of one tile; then the two K stages
+    static constexpr int QROWS = G::MID ? ABOX : AK;
+    static constexpr uint32_t K_OFF = QROWS * G::ROW_BYTES;
     static constexpr uint32_t STAGE_OFF = K_OFF + 2 * G::TILE;        // [64][PSTRIDE] elements of up to 4 bytes
     static constexpr uint32_t BAR_OFF = STAGE_OFF + AG * PSTRIDE * 4;
     static constexpr uint32_t SMEM = BAR_OFF + 64 + 1024;
@@ -355,14 +403,19 @@ CB_DEVINL void probs_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }   
 
 // S of one key block, NT n-tiles wide, masked as in attend_block
 template <bool BF, int DH, int NT>
-CB_DEVINL void probs_scores(float (&sc)[4 * NT], uint64_t dq, uint64_t dq_t, uint32_t k_s, int key0, int T, int causal, int wrow0, int r0,
-                            int tc) {
+CB_DEVINL void probs_scores(float (&sc)[4 * NT], uint64_t dq, uint64_t dq_m, uint64_t dq_t, uint32_t k_s, int key0, int T, int causal,
+                            int wrow0, int r0, int tc) {
     using G = AttnGeo<DH>;
     const uint64_t dk = wgmma_desc_sw128(k_s);
     wgmma_fence();
     #pragma unroll
     for (int k = 0; k < 4; k++) wgmma_ss_nt<BF, NT>(sc, dq + 2 * k, dk + 2 * k, (uint32_t)k);
-    if constexpr (G::TAIL) wgmma_ss_nt<BF, NT>(sc, dq_t, wgmma_desc_sw32(k_s + G::MAIN), 1u);
+    if constexpr (G::MID) {
+        const uint64_t dkm = wgmma_desc_sw64(k_s + G::mid_off(AK));
+        #pragma unroll
+        for (int k = 0; k < 2; k++) wgmma_ss_nt<BF, NT>(sc, dq_m + 2 * k, dkm + 2 * k, 1u);
+    }
+    if constexpr (G::TAIL) wgmma_ss_nt<BF, NT>(sc, dq_t, wgmma_desc_sw32(k_s + G::tail_off(AK)), 1u);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs(sc);
@@ -380,11 +433,11 @@ CB_DEVINL void probs_scores(float (&sc)[4 * NT], uint64_t dq, uint64_t dq_t, uin
 
 // pass 1: the running row max and sum over one key block, exactly as attend_block updates them
 template <bool BF, int DH, int NT>
-CB_DEVINL void probs_stats(float (&m_run)[2], float (&l_run)[2], uint64_t dq, uint64_t dq_t, uint32_t k_s, int key0, int T, int causal,
-                           int wrow0, int r0, int tc) {
+CB_DEVINL void probs_stats(float (&m_run)[2], float (&l_run)[2], uint64_t dq, uint64_t dq_m, uint64_t dq_t, uint32_t k_s, int key0, int T,
+                           int causal, int wrow0, int r0, int tc) {
     constexpr float LOG2E = 1.4426950408889634f;
     float sc[4 * NT];
-    probs_scores<BF, DH, NT>(sc, dq, dq_t, k_s, key0, T, causal, wrow0, r0, tc);
+    probs_scores<BF, DH, NT>(sc, dq, dq_m, dq_t, k_s, key0, T, causal, wrow0, r0, tc);
     #pragma unroll
     for (int h = 0; h < 2; h++) {
         float mx = -INFINITY;
@@ -405,11 +458,11 @@ CB_DEVINL void probs_stats(float (&m_run)[2], float (&l_run)[2], uint64_t dq, ui
 // pass 2: the probabilities of one key block into the staging buffer (row lr0 + 8h, columns 8j + tc + {0, 1}); the K stage is
 // released as soon as S is in registers
 template <bool BF, int DH, int NT>
-CB_DEVINL void probs_block(const float (&mb)[2], const float (&inv)[2], uint64_t dq, uint64_t dq_t, uint32_t k_s, int key0, int T, int causal,
-                           int wrow0, int r0, int tc, int lr0, uint8_t* stage, int otype, uint32_t release, int lane) {
+CB_DEVINL void probs_block(const float (&mb)[2], const float (&inv)[2], uint64_t dq, uint64_t dq_m, uint64_t dq_t, uint32_t k_s, int key0,
+                           int T, int causal, int wrow0, int r0, int tc, int lr0, uint8_t* stage, int otype, uint32_t release, int lane) {
     constexpr float LOG2E = 1.4426950408889634f;
     float sc[4 * NT];
-    probs_scores<BF, DH, NT>(sc, dq, dq_t, k_s, key0, T, causal, wrow0, r0, tc);
+    probs_scores<BF, DH, NT>(sc, dq, dq_m, dq_t, k_s, key0, T, causal, wrow0, r0, tc);
     __syncwarp();
     if (lane == 0) mbar_arrive(release);
     probs_bar();                                               // the previous block's stores have read the staging buffer
@@ -428,7 +481,7 @@ CB_DEVINL void probs_block(const float (&mb)[2], const float (&inv)[2], uint64_t
 }
 
 template <bool BF, int DH>
-__global__ void __launch_bounds__(PROBS_THREADS, 1) attention_probs_kernel(const __grid_constant__ PParams p) {
+__global__ void __launch_bounds__(PROBS_THREADS, 1) attention_probs_kernel(const __grid_constant__ PParams p, const __grid_constant__ CUtensorMap tm_mid) {
     using G = AttnGeo<DH>;
     using PG = ProbsGeo<DH>;
     constexpr float LOG2E = 1.4426950408889634f;
@@ -443,6 +496,7 @@ __global__ void __launch_bounds__(PROBS_THREADS, 1) attention_probs_kernel(const
         for (int i = 0; i < 2; i++) { mbar_init(kv_full + 8 * i, 1); mbar_init(kv_empty + 8 * i, 4); }     // released by each consumer warp
         mbar_fence_init();
         tma_prefetch_desc(&p.a.tm_qkv);
+        if constexpr (G::MID) tma_prefetch_desc(&tm_mid);
         if constexpr (G::TAIL) tma_prefetch_desc(&p.a.tm_tail);
     }
     __syncthreads();
@@ -458,14 +512,14 @@ __global__ void __launch_bounds__(PROBS_THREADS, 1) attention_probs_kernel(const
         // ------------------------------------------------------------------ producer (one thread): Q, then K blocks 0 .. nkb-1 twice
         if (lane == 0) {
             mbar_arrive_expect_tx(q_full, G::BOX_BYTES);
-            load_box<DH>(smem_base, 0, p.a, head * DH, g0, seq, q_full);
-            const int kcol = p.a.H * DH + head * DH;
+            load_box<DH, PG::QROWS>(smem_base, 0, p.a, tm_mid, head * G::DHP, g0, seq, q_full);
+            const int kcol = p.a.H * G::DHP + head * G::DHP;
             for (int n = 0; n < 2 * nkb; n++) {
-                const int kb = n < nkb ? n : n - nkb, nb = kv_boxes(kend, kb);
+                const int kb = n < nkb ? n : n - nkb, nb = kv_boxes<AK>(kend, kb);
                 const uint32_t s = n & 1, bar = kv_full + 8 * s;
                 mbar_wait(kv_empty + 8 * s, ((n >> 1) & 1) ^ 1);
                 mbar_arrive_expect_tx(bar, (uint32_t)nb * G::BOX_BYTES);
-                for (int b = 0; b < nb; b++) load_box<DH>(smem_base + PG::K_OFF + s * G::TILE, b, p.a, kcol, kb * AK + b * ABOX, seq, bar);
+                for (int b = 0; b < nb; b++) load_box<DH, AK>(smem_base + PG::K_OFF + s * G::TILE, b, p.a, tm_mid, kcol, kb * AK + b * ABOX, seq, bar);
             }
         }
         return;
@@ -476,17 +530,18 @@ __global__ void __launch_bounds__(PROBS_THREADS, 1) attention_probs_kernel(const
     const int lr0 = warp * 16 + (lane >> 2);                  // this thread: group rows lr0 and lr0 + 8
     const int wrow0 = g0 + warp * 16, r0 = g0 + lr0;
     mbar_wait(q_full, 0);
-    const uint64_t dq = wgmma_desc_sw128(smem_base), dq_t = wgmma_desc_sw32(smem_base + G::MAIN);
+    const uint64_t dq = wgmma_desc_sw128(smem_base), dq_m = wgmma_desc_sw64(smem_base + G::mid_off(PG::QROWS));
+    const uint64_t dq_t = wgmma_desc_sw32(smem_base + G::tail_off(PG::QROWS));
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
     uint32_t n = 0;
     for (int kb = 0; kb < nkb; kb++, n++) {
         const uint32_t s = n & 1, k_s = smem_base + PG::K_OFF + s * G::TILE;
         mbar_wait(kv_full + 8 * s, (n >> 1) & 1);
         const int key0 = kb * AK, rem = kend - key0;
-        if (rem > 64) probs_stats<BF, DH, 16>(m_run, l_run, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc);
-        else if (rem > 32) probs_stats<BF, DH, 8>(m_run, l_run, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc);
-        else if (rem > 16) probs_stats<BF, DH, 4>(m_run, l_run, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc);
-        else probs_stats<BF, DH, 2>(m_run, l_run, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc);
+        if (rem > 64) probs_stats<BF, DH, 16>(m_run, l_run, dq, dq_m, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc);
+        else if (rem > 32) probs_stats<BF, DH, 8>(m_run, l_run, dq, dq_m, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc);
+        else if (rem > 16) probs_stats<BF, DH, 4>(m_run, l_run, dq, dq_m, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc);
+        else probs_stats<BF, DH, 2>(m_run, l_run, dq, dq_m, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc);
         __syncwarp();
         if (lane == 0) mbar_arrive(kv_empty + 8 * s);
     }
@@ -507,10 +562,10 @@ __global__ void __launch_bounds__(PROBS_THREADS, 1) attention_probs_kernel(const
         const uint32_t s = n & 1, k_s = smem_base + PG::K_OFF + s * G::TILE, release = kv_empty + 8 * s;
         mbar_wait(kv_full + 8 * s, (n >> 1) & 1);
         const int key0 = kb * AK, rem = kend - key0;
-        if (rem > 64) probs_block<BF, DH, 16>(mb, inv, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc, lr0, stage, p.otype, release, lane);
-        else if (rem > 32) probs_block<BF, DH, 8>(mb, inv, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc, lr0, stage, p.otype, release, lane);
-        else if (rem > 16) probs_block<BF, DH, 4>(mb, inv, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc, lr0, stage, p.otype, release, lane);
-        else probs_block<BF, DH, 2>(mb, inv, dq, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc, lr0, stage, p.otype, release, lane);
+        if (rem > 64) probs_block<BF, DH, 16>(mb, inv, dq, dq_m, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc, lr0, stage, p.otype, release, lane);
+        else if (rem > 32) probs_block<BF, DH, 8>(mb, inv, dq, dq_m, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc, lr0, stage, p.otype, release, lane);
+        else if (rem > 16) probs_block<BF, DH, 4>(mb, inv, dq, dq_m, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc, lr0, stage, p.otype, release, lane);
+        else probs_block<BF, DH, 2>(mb, inv, dq, dq_m, dq_t, k_s, key0, T, p.a.causal, wrow0, r0, tc, lr0, stage, p.otype, release, lane);
         // columns key0 .. min(key0 + 128, kend) - 1 of every row, one warp per row
         const int cw = min(AK, rem);
         if (p.otype == 0) {
@@ -541,8 +596,8 @@ typedef CUresult (*EncodeTiledFn3)(CUtensorMap*, CUtensorMapDataType, cuuint32_t
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// [nseq][T][3*H*dh] view of the fused QKV activations, box = `box_cols` columns x 64 tokens x 1 sequence (zero fill past T):
-// 64 columns with the 128-byte swizzle, or the 16-column tail of an 80-wide head with the 32-byte swizzle
+// [nseq][T][3*H*dhp] view of the fused QKV activations (dhp = qkv_head_cols(dh)), box = `box_cols` columns x 64 tokens x 1
+// sequence (zero fill past T): 64 columns with the 128-byte swizzle, 32 with the 64-byte swizzle, or 16 with the 32-byte swizzle
 bool make_qkv_map(CUtensorMap* out, const void* qkv16, int nseq, int T, int H, int dh, int box_cols, CUtensorMapSwizzle swz) {
     static EncodeTiledFn3 enc = nullptr;
     if (!enc) {
@@ -551,12 +606,20 @@ bool make_qkv_map(CUtensorMap* out, const void* qkv16, int nseq, int T, int H, i
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) return false;
         enc = reinterpret_cast<EncodeTiledFn3>(f);
     }
-    const cuuint64_t cols = (cuuint64_t)3 * H * dh;
+    const cuuint64_t cols = (cuuint64_t)3 * H * qkv_head_cols(dh);
     const cuuint64_t dims[3] = {cols, (cuuint64_t)T, (cuuint64_t)nseq};
     const cuuint64_t strides[2] = {cols * 2, cols * 2 * (cuuint64_t)T};
     const cuuint32_t box[3] = {(cuuint32_t)box_cols, (cuuint32_t)ABOX, 1}, estr[3] = {1, 1, 1};
     return enc(out, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<void*>(qkv16), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// the maps of every piece of a dh-wide head (AttnGeo): tm_mid is left zero unless dh == 104
+bool make_piece_maps(AParams& p, CUtensorMap& tm_mid, const void* qkv16, int nseq, int T, int H, int dh) {
+    memset(&tm_mid, 0, sizeof(tm_mid));
+    if (!make_qkv_map(&p.tm_qkv, qkv16, nseq, T, H, dh, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return false;
+    if (dh == 104 && !make_qkv_map(&tm_mid, qkv16, nseq, T, H, dh, 32, CU_TENSOR_MAP_SWIZZLE_64B)) return false;
+    return dh == 64 || make_qkv_map(&p.tm_tail, qkv16, nseq, T, H, dh, 16, CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
 template <int DH>
@@ -571,26 +634,36 @@ cudaError_t set_smem() {
 }
 
 template <int DH>
-cudaError_t launch_dh(const AParams& p, unsigned grid, int bf16, cudaStream_t st) {
+cudaError_t launch_dh(const AParams& p, const CUtensorMap& tm_mid, unsigned grid, int bf16, cudaStream_t st) {
     constexpr uint32_t smem = AttnGeo<DH>::SMEM;
-    return bf16 ? launch_pdl(attention_tc_kernel<true, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p)
-                : launch_pdl(attention_tc_kernel<false, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p);
+    return bf16 ? launch_pdl(attention_tc_kernel<true, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid)
+                : launch_pdl(attention_tc_kernel<false, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid);
 }
+
+template <int DH>
+cudaError_t launch_probs_dh(const PParams& p, const CUtensorMap& tm_mid, unsigned grid, int bf16, cudaStream_t st) {
+    constexpr uint32_t smem = ProbsGeo<DH>::SMEM;
+    return bf16 ? launch_pdl(attention_probs_kernel<true, DH>, grid, (unsigned)PROBS_THREADS, smem, st, 1, p, tm_mid)
+                : launch_pdl(attention_probs_kernel<false, DH>, grid, (unsigned)PROBS_THREADS, smem, st, 1, p, tm_mid);
+}
+
+bool supported_dh(int dh) { return dh == 64 || dh == 80 || dh == 104; }
 
 }  // namespace
 
 cudaError_t attention_tc_init() {
     cudaError_t e = set_smem<64>();
-    return e != cudaSuccess ? e : set_smem<80>();
+    if (e == cudaSuccess) e = set_smem<80>();
+    return e != cudaSuccess ? e : set_smem<104>();
 }
 
 cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T, int H, int dh, int causal, int bf16, cudaStream_t st) {
-    if (dh != 64 && dh != 80) return cudaErrorInvalidValue;
+    if (!supported_dh(dh)) return cudaErrorInvalidValue;
     if (nseq <= 0) return cudaSuccess;
     AParams p;
+    CUtensorMap tm_mid;
     memset(&p, 0, sizeof(p));
-    if (!make_qkv_map(&p.tm_qkv, qkv16, nseq, T, H, dh, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return cudaErrorInvalidValue;
-    if (dh == 80 && !make_qkv_map(&p.tm_tail, qkv16, nseq, T, H, dh, 16, CU_TENSOR_MAP_SWIZZLE_32B)) return cudaErrorInvalidValue;
+    if (!make_piece_maps(p, tm_mid, qkv16, nseq, T, H, dh)) return cudaErrorInvalidValue;
     p.out = (uint16_t*)out16; p.T = T; p.H = H; p.causal = causal;
     p.ngrp = (T + AG - 1) / AG;
     const long long ngroups = (long long)nseq * H * p.ngrp;
@@ -603,29 +676,26 @@ cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T,
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (e != cudaSuccess) return e;
     const unsigned grid = (unsigned)min(p.niter, sms);
-    e = dh == 80 ? launch_dh<80>(p, grid, bf16, st) : launch_dh<64>(p, grid, bf16, st);
+    e = dh == 104 ? launch_dh<104>(p, tm_mid, grid, bf16, st) : dh == 80 ? launch_dh<80>(p, tm_mid, grid, bf16, st) : launch_dh<64>(p, tm_mid, grid, bf16, st);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 cudaError_t launch_attention_probs(const void* qkv16, void* out, int elem_type, int nseq, int T, int H, int dh, int causal, int cls_only,
                                    int bf16, cudaStream_t st) {
-    if ((dh != 64 && dh != 80) || elem_type < 0 || elem_type > 2) return cudaErrorInvalidValue;
+    if (!supported_dh(dh) || elem_type < 0 || elem_type > 2) return cudaErrorInvalidValue;
     if (nseq <= 0 || T <= 0) return cudaSuccess;
     PParams p;
+    CUtensorMap tm_mid;
     memset(&p, 0, sizeof(p));
-    if (!make_qkv_map(&p.a.tm_qkv, qkv16, nseq, T, H, dh, 64, CU_TENSOR_MAP_SWIZZLE_128B)) return cudaErrorInvalidValue;
-    if (dh == 80 && !make_qkv_map(&p.a.tm_tail, qkv16, nseq, T, H, dh, 16, CU_TENSOR_MAP_SWIZZLE_32B)) return cudaErrorInvalidValue;
+    if (!make_piece_maps(p.a, tm_mid, qkv16, nseq, T, H, dh)) return cudaErrorInvalidValue;
     p.a.T = T; p.a.H = H; p.a.causal = causal;
     p.a.ngrp = cls_only ? 1 : (T + AG - 1) / AG;
     p.out = out; p.otype = elem_type; p.rows = cls_only ? 1 : T;
     const long long units = (long long)nseq * H * p.a.ngrp;
     if (units > 0x7fffffffll) return cudaErrorInvalidValue;
     const unsigned grid = (unsigned)units;
-    cudaError_t e;
-    if (dh == 80) e = bf16 ? launch_pdl(attention_probs_kernel<true, 80>, grid, (unsigned)PROBS_THREADS, ProbsGeo<80>::SMEM, st, 1, p)
-                           : launch_pdl(attention_probs_kernel<false, 80>, grid, (unsigned)PROBS_THREADS, ProbsGeo<80>::SMEM, st, 1, p);
-    else e = bf16 ? launch_pdl(attention_probs_kernel<true, 64>, grid, (unsigned)PROBS_THREADS, ProbsGeo<64>::SMEM, st, 1, p)
-                  : launch_pdl(attention_probs_kernel<false, 64>, grid, (unsigned)PROBS_THREADS, ProbsGeo<64>::SMEM, st, 1, p);
+    const cudaError_t e = dh == 104 ? launch_probs_dh<104>(p, tm_mid, grid, bf16, st)
+                          : dh == 80 ? launch_probs_dh<80>(p, tm_mid, grid, bf16, st) : launch_probs_dh<64>(p, tm_mid, grid, bf16, st);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 

@@ -2,7 +2,7 @@
 //
 // Two ways to get more than one GPU behind the C ABI:
 //   * "devices" mode  -- ONE process drives several GPUs: CLIP_B200_DEVICES=0,1,...|all at clip_model_load creates a replica of
-//                        the model per device (weights are <= 0.33 GB) and one NCCL communicator per replica (ncclCommInitAll);
+//                        the model per device (weights: at most about 5 GB, ViT-bigG/14 f16) and one NCCL communicator per replica (ncclCommInitAll);
 //   * "ranks" mode    -- one process per GPU (torchrun / mpirun / any launcher): clip_b200_dist_init(ctx, rank, world, ...) joins
 //                        a communicator with ncclCommInitRank; the 128-byte unique id travels through a rendezvous file on the
 //                        node (or through the caller's own channel: clip_b200_dist_unique_id + clip_b200_dist_init_with_id).

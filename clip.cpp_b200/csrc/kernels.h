@@ -44,15 +44,20 @@ void launch_text_embed(const int32_t* ids, const float* tok, const float* pos, i
 // (CLIP_B200_ATTN=legacy).
 void launch_attention(const void* qkv16, void* out16, int nseq, int T, int H, int causal, int bf16, cudaStream_t st);
 
-// K3 on wgmma (attention_tc.cu): head_dim dh = 64 or 80 (anything else: cudaErrorInvalidValue), a persistent grid over
-// 64-row query groups, online softmax over 128-key blocks, any T.  The Q / K / V boxes come from per-launch 3-D TMA views [sequence][token][column] of qkv16 (zero
-// fill past each sequence's T tokens).
+// Columns a head of head_dim dh takes in the fused QKV matrix: dh, except 104 (ViT-bigG/14), which the loader pads to 112 with 8
+// exactly-zero columns per head so that the attention kernels' pieces (64 + 32 + 16 columns) never reach into the next head.
+constexpr int qkv_head_cols(int dh) { return dh == 104 ? 112 : dh; }
+
+// K3 on wgmma (attention_tc.cu): head_dim dh = 64, 80 or 104 (anything else: cudaErrorInvalidValue), a persistent grid over
+// 64-row query groups, online softmax over 128-key blocks (64-key at 104), any T.  qkv16 is [nseq*T, 3*H*qkv_head_cols(dh)]; out
+// stays [nseq*T, H*dh].  The Q / K / V boxes come from per-launch 3-D TMA views [sequence][token][column] of qkv16 (zero fill past
+// each sequence's T tokens).
 cudaError_t attention_tc_init();
 cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T, int H, int dh, int causal, int bf16, cudaStream_t st);
 
 // K9 attention probabilities (attention_tc.cu): the softmax(Q K^T [causal]) K3 computes internally, from the same qkv16, written out:
 // out [nseq, H, R, T] of elem_type (0 fp32, 1 fp16, 2 bf16: RNE of the fp32 value), R = T, or 1 with cls_only (query row 0 alone).
-// Masked keys are +0.  Any T, head_dim 64 or 80; out needs only the element type's alignment.
+// Masked keys are +0.  Any T, head_dim 64, 80 or 104 (qkv16 laid out as for K3); out needs only the element type's alignment.
 cudaError_t launch_attention_probs(const void* qkv16, void* out, int elem_type, int nseq, int T, int H, int dh, int causal, int cls_only,
                                    int bf16, cudaStream_t st);
 

@@ -45,6 +45,18 @@ CB_DEVINL uint64_t wgmma_desc_sw32(uint32_t smem_addr) {
     return d;
 }
 
+// The same for a tile 32 elements wide stored with the 64-byte swizzle (CU_TENSOR_MAP_SWIZZLE_64B): rows of 64 B, 8-row groups
+// 512 B apart.  A K-major operand steps 16 elements (32 B) inside the row, and an MN-major operand 32 wide is one swizzle atom
+// across, so only the 8-row group stride is used.  Tile bases are 512-B aligned; a 16-row step (keys of an MN-major tile) is 1024 B.
+CB_DEVINL uint64_t wgmma_desc_sw64(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);   // start address       [0,14)
+    d |= (uint64_t)(512 >> 4) << 16;                // leading byte offset [16,30)
+    d |= (uint64_t)(512 >> 4) << 32;                // stride byte offset  [32,46)
+    d |= (uint64_t)2 << 62;                         // layout: 64-byte swizzle [62,64)
+    return d;
+}
+
 // D[64 x 192] (+)= A[64 x 16] . B[192 x 16]^T, both operands K-major in shared memory (descriptors), fp32 accumulators
 template <bool BF>
 CB_DEVINL void wgmma_ss_n192(float (&d)[96], uint64_t da, uint64_t db, uint32_t accumulate) {
@@ -133,7 +145,21 @@ CB_DEVINL void wgmma_rs_n64_bmn(float (&d)[32], const uint32_t (&a)[4], uint64_t
 #undef CB_WGMMA_RS_N64
 }
 
-// D[64 x 16] (+)= A[64 x 16] . B[16 x 16]: A from registers, B MN-major in shared memory (the 16-column tail of an 80-wide head)
+// D[64 x 32] (+)= A[64 x 16] . B[16 x 32]: A from registers, B MN-major in shared memory (columns 64-95 of a 104-wide head)
+template <bool BF>
+CB_DEVINL void wgmma_rs_n32_bmn(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+#define CB_WGMMA_RS_N32(TY)                                                                                 \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %21, 0;\n\t"                                                 \
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 1;\n\t}"  \
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])  \
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate))
+    if constexpr (BF) CB_WGMMA_RS_N32("bf16");
+    else CB_WGMMA_RS_N32("f16");
+#undef CB_WGMMA_RS_N32
+}
+
+// D[64 x 16] (+)= A[64 x 16] . B[16 x 16]: A from registers, B MN-major in shared memory (the 16-column tail of an 80- or 104-wide
+// head)
 template <bool BF>
 CB_DEVINL void wgmma_rs_n16_bmn(float (&d)[8], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
 #define CB_WGMMA_RS_N16(TY)                                                                                 \

@@ -147,4 +147,15 @@ bool wpack_unpack(int qt, const uint8_t* packed, int64_t N, int64_t K, uint8_t* 
     return true;
 }
 
+bool pad_head_rows(const uint8_t* src, size_t row_bytes, int64_t rows, int dh, int dhp, uint8_t* dst) {
+    if (dh <= 0 || dhp < dh || rows % dh) return false;
+    const size_t head = (size_t)dh * row_bytes, pad = (size_t)(dhp - dh) * row_bytes;
+    for (int64_t h = 0; h < rows / dh; h++) {
+        uint8_t* d = dst + (size_t)h * (head + pad);
+        memcpy(d, src + (size_t)h * head, head);
+        memset(d + head, 0, pad);
+    }
+    return true;
+}
+
 }  // namespace cb

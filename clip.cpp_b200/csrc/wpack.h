@@ -57,6 +57,12 @@ inline size_t wpack_total_bytes(int qtype, int64_t N, int64_t K) {
 // Returns false if the shape cannot be tiled.
 bool wpack_repack(int qtype, const uint8_t* src, int64_t N, int64_t K, uint8_t* dst);
 
+// Row padding of the fused QKV projection (kernels.h: qkv_head_cols): `rows` rows of `row_bytes` bytes, in groups of dh rows (one
+// head of Q, K or V), become groups of dhp rows: the dh source rows, then dhp - dh rows of zero bytes.  All-zero bytes are an exact
+// zero in f32, f16 and every ggml block type (d = m = 0), so the padded output features of the GEMM are exact zeros.  Returns false
+// unless rows % dh == 0 and dhp >= dh.
+bool pad_head_rows(const uint8_t* src, size_t row_bytes, int64_t rows, int dh, int dhp, uint8_t* dst);
+
 // Inverse (used by the unit tests to prove the re-tiling is lossless).
 bool wpack_unpack(int qtype, const uint8_t* packed, int64_t N, int64_t K, uint8_t* dst_ggml);
 

@@ -98,6 +98,14 @@ GEOMETRIES = {
     # over 257 positions, GELU
     "huge-w640": Geometry("huge-w640", image_size=224, patch_size=14, v_hidden=640, v_ff=1280, v_heads=8, v_layers=32,
                           t_hidden=128, t_ff=256, t_heads=2, t_layers=24, proj_dim=128, use_gelu=True),
+    # LAION ViT-bigG/14: vision head_dim 1664 / 16 = 104 (each head padded to 112 columns in the QKV projection at load), text
+    # head_dim 1280 / 20 = 64, GELU; 1 293 tensors, more than the reference accepts
+    "vit-bigg14": Geometry("vit-bigg14", patch_size=14, v_hidden=1664, v_ff=8192, v_heads=16, v_layers=48,
+                           t_hidden=1280, t_ff=5120, t_heads=20, t_layers=32, proj_dim=1280, use_gelu=True),
+    # the true bigG vision width and depth per layer with the huge tensor counts (32 + 24 layers, 909 tensors), so the reference
+    # accepts it: head_dim 104 over 257 positions next to a tiny text tower; ~2.5 GB as f16
+    "bigg-w1664": Geometry("bigg-w1664", image_size=224, patch_size=14, v_hidden=1664, v_ff=8192, v_heads=16, v_layers=32,
+                           t_hidden=128, t_ff=256, t_heads=2, t_layers=24, proj_dim=128, use_gelu=True),
 }
 
 

@@ -432,13 +432,15 @@ bool clip_b200_image_batch_preprocess_device(const struct clip_ctx * ctx, const 
  * use_legacy=1 runs the warp-level mma.sync kernel instead of the wgmma one.  ms (optional): device time of the last of 3 launches. */
 int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int causal, int use_legacy, const float * qkv, float * out,
                               float * ms);
-/* The same for head_dim 64 or 80: qkv [nseq*T, 3*H*head_dim], the 1/sqrt(head_dim) scale already applied to Q; out [nseq*T, H*head_dim].
- * Returns 2 with a message for any other head_dim, and for use_legacy=1 with head_dim 80 (the legacy kernel is head_dim 64 only). */
+/* The same for head_dim 64, 80 or 104: qkv [nseq*T, 3*H*head_dim], the 1/sqrt(head_dim) scale already applied to Q; out
+ * [nseq*T, H*head_dim].  At head_dim 104 the hook lays qkv out on the device as the loader lays out the QKV activations, each head
+ * padded to 112 columns with zeros.  Returns 2 with a message for any other head_dim, and for use_legacy=1 with head_dim 80 or 104
+ * (the legacy kernel is head_dim 64 only). */
 int clip_b200_debug_attention_hd(int operand_bf16, int nseq, int T, int H, int head_dim, int causal, int use_legacy, const float * qkv,
                                  float * out, float * ms);
 /* The attention probabilities of the same qkv (the kernel behind CLIP_B200_TOKENS_ATTENTION): out [nseq, H, R, T] with R = T, or 1
  * with cls_row (query row 0 only), of out_type (0 fp32, 1 fp16, 2 bf16: raw 16-bit values, not widened).  Runs on device 0.  Returns
- * 2 for bad arguments (head_dim other than 64 / 80, a non-positive size, an unknown out_type), 5 if the kernel wrote into the
+ * 2 for bad arguments (head_dim other than 64 / 80 / 104, a non-positive size, an unknown out_type), 5 if the kernel wrote into the
  * poisoned guard bytes that follow the output. */
 int clip_b200_debug_attention_probs(int operand_bf16, int nseq, int T, int H, int head_dim, int causal, int cls_row, int out_type,
                                     const float * qkv, void * out);
@@ -480,6 +482,10 @@ int clip_b200_debug_token_rows(int n, int T, int h, size_t in_stride, int no_cls
 /* CPU-only TEST HOOKS (no context, no GPU): lossless re-tiling check, tokenizer and preprocess without a model context */
 int clip_b200_debug_repack_roundtrip(int qtype, const void * rows, int N, int K);
 int clip_b200_debug_rendezvous(int rank, int world, const char * path, void * out128);     /* ranks-mode id exchange (csrc/dist.cpp) */
+/* the loader's QKV padding at head_dim 104: src = 3*H*dh rows of a [*, K] weight of ggml type qtype (0 f32, 1 f16, 2/3/6/7/8 the
+ * block types; qtype 0 with K = 1 is a bias) -> out = 3*H*dhp rows, each head's dh rows followed by dhp - dh rows of zero bytes.
+ * Returns 0, or 1 for bad arguments (dhp < dh, K not a whole number of blocks, an unknown type). */
+int clip_b200_debug_pad_qkv(int qtype, int H, int dh, int dhp, int K, const void * src, void * out);
 void clip_b200_debug_shard_bounds(size_t n, int r, int w, size_t * lo, size_t * hi);        /* devices-mode sharding rule */
 int clip_b200_debug_tokenize(const char * gguf_path, const char * text, int32_t * out, int cap);
 int clip_b200_debug_preprocess(const uint8_t * rgb, int nx, int ny, int out_size, const float * mean, const float * stdv,

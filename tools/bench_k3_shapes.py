@@ -4,7 +4,7 @@
     python tools/bench_k3_shapes.py [--lib PATH] [--reps 5]
 
 Each shape runs `reps` calls (the hook times the last of three launches per call); the line reports the median of all but the first
-call.  Useful FLOP: 4 T^2 dh per (sequence, head), halved for causal.  HBM bytes: the fused QKV matrix read once and O written
+call.  Useful FLOP: 4 T^2 dh per (sequence, head), halved for causal (dh the real head_dim: 104, not the 112 columns K3 multiplies).  HBM bytes: the fused QKV matrix read once and O written
 once (3 + 1 rows of H dh 16-bit values per token), against the H100 SXM data sheet's 3.35 TB/s.
 """
 import argparse
@@ -25,6 +25,7 @@ SHAPES = [("vit-l14 (headline, cfg3)", 256, 257, 16, 64, 0),
           ("vit-b32 (cfg2)", 256, 50, 12, 64, 0),
           ("text (cfg4)", 683, 77, 12, 64, 1),
           ("vit-h14", 256, 257, 16, 80, 0),
+          ("vit-bigg14", 256, 257, 16, 104, 0),
           ("vit-l14-336", 64, 577, 16, 64, 0)]
 
 
