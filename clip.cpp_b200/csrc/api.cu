@@ -87,7 +87,7 @@ struct Scope {
         }
     }
 };
-enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4, K_POS_RESAMPLE = 5, K_ATTN_PROBS = 6, K_KNN16 = 7 };
+enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4, K_POS_RESAMPLE = 5, K_ATTN_PROBS = 6, K_KNN16 = 7, K_KNN_I8 = 8 };
 
 // ---- tensor lookup helpers ---------------------------------------------------------------------------------
 const GgufTensor* need(const GgufFile& g, const std::string& name) {
@@ -1664,6 +1664,37 @@ bool clip_b200_topk_search(const struct clip_ctx* cctx, const void* d_queries, s
 }
 
 // ---- 16-bit nearest-neighbour search (K10, search.cu) ---------------------------------------------------------------
+// The pass driver of both K10 forms: launches of up to 32768 queries, each one K10 launch (`launch(r0, rows, k, plan, cand_ld)`,
+// timed as `kind`) into the grow-only workspace, the merge stages and the copies out.  Caller holds c->mu, has set the device and
+// has checked the arguments; n_queries, n_db > 0 and top_k in [1, 1024].
+extern "C++" {
+template <class Launch>
+static bool knn_search_locked(clip_ctx* c, const char* F, int kind, size_t n_queries, size_t n_db, int top_k, float* scores, int* indices,
+                              Launch launch) {
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
+    const int k = (int)std::min<size_t>((size_t)top_k, n_db), ndb = (int)n_db;
+    const size_t QB = 32768;                                              // queries per launch (the merge grid's row limit)
+    for (size_t r0 = 0; r0 < n_queries; r0 += QB) {
+        const int rows = (int)std::min(QB, n_queries - r0);
+        const Knn16Plan pl = knn16_plan(rows, ndb, k, sms);
+        const size_t cand_ld = (size_t)pl.parts * k;
+        if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * pl.buf_entries) || !ensure_cand(c, (size_t)rows * cand_ld)) return false;
+        {
+            Scope s(c, kind);
+            const cudaError_t e = launch(r0, rows, k, pl, cand_ld);
+            if (e != cudaSuccess) { set_err(std::string(F) + "launch: " + cudaGetErrorString(e)); return false; }
+        }
+        const int cur = merge_candidates(c, rows, cand_ld, (size_t)pl.parts, k);
+        CK(cudaMemcpy2DAsync(scores + r0 * k, (size_t)k * 4, c->d_cand_v[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpy2DAsync(indices + r0 * k, (size_t)k * 4, c->d_cand_i[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+    }
+    CK(cudaGetLastError());
+    return true;
+}
+}  // extern "C++"
+
 bool clip_b200_rows_to_16bit(const struct clip_ctx* cctx, const void* d_src, size_t n, int dim, int out_type, void* d_dst) {
     static const char* F = "clip_b200_rows_to_16bit: ";
     clip_ctx* c = const_cast<clip_ctx*>(cctx);
@@ -1696,29 +1727,54 @@ bool clip_b200_topk_search_16(const struct clip_ctx* cctx, const void* d_queries
     if (!scores || !indices) { set_err(std::string(F) + "null output"); return false; }
     std::lock_guard<std::mutex> lk(c->mu);
     CK(cudaSetDevice(c->device));
-    int sms = 0;
-    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
-    const int k = (int)std::min<size_t>((size_t)top_k, n_db), ndb = (int)n_db;
-    const size_t QB = 32768;                                              // queries per launch (the merge grid's row limit)
     const uint16_t* q16 = (const uint16_t*)d_queries;
-    for (size_t r0 = 0; r0 < n_queries; r0 += QB) {
-        const int rows = (int)std::min(QB, n_queries - r0);
-        const Knn16Plan pl = knn16_plan(rows, ndb, k, sms);
-        const size_t cand_ld = (size_t)pl.parts * k;
-        if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * pl.buf_entries) || !ensure_cand(c, (size_t)rows * cand_ld)) return false;
-        {
-            Scope s(c, K_KNN16);
-            const cudaError_t e = launch_knn16(q16 + r0 * dim, rows, d_db, ndb, dim, in_type == CLIP_B200_OUT_BF16, k, pl, c->d_knn,
-                                               c->d_cand_v[0], c->d_cand_i[0], cand_ld, c->stream);
-            if (e != cudaSuccess) { set_err(std::string(F) + "launch: " + cudaGetErrorString(e)); return false; }
-        }
-        const int cur = merge_candidates(c, rows, cand_ld, (size_t)pl.parts, k);
-        CK(cudaMemcpy2DAsync(scores + r0 * k, (size_t)k * 4, c->d_cand_v[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
-        CK(cudaMemcpy2DAsync(indices + r0 * k, (size_t)k * 4, c->d_cand_i[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
-        CK(cudaStreamSynchronize(c->stream));
+    const bool bf = in_type == CLIP_B200_OUT_BF16;
+    return knn_search_locked(c, F, K_KNN16, n_queries, n_db, top_k, scores, indices, [&](size_t r0, int rows, int k, const Knn16Plan& pl, size_t cand_ld) {
+        return launch_knn16(q16 + r0 * dim, rows, d_db, (int)n_db, dim, bf, k, pl, c->d_knn, c->d_cand_v[0], c->d_cand_i[0], cand_ld, c->stream);
+    });
+}
+
+// ---- int8 nearest-neighbour search (K10's s8 instance, search.cu) ---------------------------------------------------
+bool clip_b200_rows_to_int8(const struct clip_ctx* cctx, const void* d_src, size_t n, int dim, void* d_codes, void* d_scales) {
+    static const char* F = "clip_b200_rows_to_int8: ";
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    if (!c) { set_err(std::string(F) + "null context"); return false; }
+    if (dim < 16 || dim > 2048 || dim % 16) { set_err(std::string(F) + "dim must be a multiple of 16 in [16, 2048]"); return false; }
+    if (n > 0x7fffffffull) { set_err(std::string(F) + "n must be below 2^31"); return false; }
+    if (n == 0) return true;
+    if (!d_src || !d_codes || !d_scales || ((uintptr_t)d_src | (uintptr_t)d_codes | (uintptr_t)d_scales) % 16) {
+        set_err(std::string(F) + "null or not 16-byte aligned pointer"); return false;
     }
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    { Scope s(c, K_OTHER); launch_rows_to_int8((const float*)d_src, (int)n, dim, d_codes, (float*)d_scales, c->stream); }
     CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(c->stream));
     return true;
+}
+
+bool clip_b200_topk_search_i8(const struct clip_ctx* cctx, const void* d_q_codes, const void* d_q_scales, size_t n_queries,
+                              const void* d_db_codes, const void* d_db_scales, size_t n_db, int dim, int top_k, float* scores, int* indices) {
+    static const char* F = "clip_b200_topk_search_i8: ";
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    if (!c) { set_err(std::string(F) + "null context"); return false; }
+    if (dim < 16 || dim > 2048 || dim % 16) { set_err(std::string(F) + "dim must be a multiple of 16 in [16, 2048]"); return false; }
+    if (top_k < 1 || top_k > 1024) { set_err(std::string(F) + "top_k must be in [1, 1024]"); return false; }
+    if (n_queries > 0x7fffffffull || n_db > 0x7fffffffull) { set_err(std::string(F) + "n_queries and n_db must be below 2^31"); return false; }
+    if (n_queries == 0 || n_db == 0) return true;
+    if (!d_q_codes || !d_q_scales || !d_db_codes || !d_db_scales ||
+        ((uintptr_t)d_q_codes | (uintptr_t)d_q_scales | (uintptr_t)d_db_codes | (uintptr_t)d_db_scales) % 16) {
+        set_err(std::string(F) + "null or not 16-byte aligned device pointer"); return false;
+    }
+    if (!scores || !indices) { set_err(std::string(F) + "null output"); return false; }
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    const int8_t* qc = (const int8_t*)d_q_codes;
+    const float* qs = (const float*)d_q_scales;
+    return knn_search_locked(c, F, K_KNN_I8, n_queries, n_db, top_k, scores, indices, [&](size_t r0, int rows, int k, const Knn16Plan& pl, size_t cand_ld) {
+        return launch_knn_i8(qc + r0 * dim, qs + r0, rows, d_db_codes, (const float*)d_db_scales, (int)n_db, dim, k, pl, c->d_knn,
+                             c->d_cand_v[0], c->d_cand_i[0], cand_ld, c->stream);
+    });
 }
 
 // =====================================================================================================================

@@ -93,6 +93,13 @@ struct Knn16Plan {
 Knn16Plan knn16_plan(int nq, int ndb, int kk, int sms);
 cudaError_t launch_knn16(const void* q, int nq, const void* db, int ndb, int dim, int bf16, int kk, const Knn16Plan& pl, void* buf,
                          float* out_v, int* out_i, size_t out_ld, cudaStream_t st);
+// K10's int8 instance: q [nq, dim] and db [ndb, dim] int8 codes with f32 scales qs [nq] and xs [ndb], all 16-byte aligned, dim % 16
+// == 0, dim <= 2048; score = fp32(fp32(float(exact int32 dot) * qs) * xs).  The same plan, scratch and output as launch_knn16.
+cudaError_t launch_knn_i8(const void* q, const float* qs, int nq, const void* db, const float* xs, int ndb, int dim, int kk,
+                          const Knn16Plan& pl, void* buf, float* out_v, int* out_i, size_t out_ld, cudaStream_t st);
+// Q8 quantiser: x [n, dim] f32 -> codes [n, dim] int8 and scales [n] f32 by the rule of clip_b200_rows_to_int8 (clip_b200.h).
+// dim % 16 == 0, dim <= 2048, 16-byte aligned pointers; 64-bit offsets, so n * dim may pass 2^32.
+void launch_rows_to_int8(const float* x, int n, int dim, void* codes, float* scales, cudaStream_t st);
 
 }  // namespace cb
 struct clip_ctx;

@@ -7,13 +7,15 @@
 // move in the 4th digit, which bf16 tensor-core products would do.  Each dot product is ONE sequential fmaf chain over k, the same
 // order the reference's scalar loop uses.
 //
-// K10 (knn16_kernel, below) is the separate, opt-in search over a database stored in 16 bits: tensor-core scores and a top-k kept
-// inside the kernel, so no score matrix ever reaches memory.  It shares the candidate order and the merge stage with the fp32 path.
+// K10 (knn16_kernel, below) is the separate, opt-in search over a database stored in 16 bits or in int8 with a scale per row:
+// tensor-core scores and a top-k kept inside the kernel, so no score matrix ever reaches memory.  It shares the candidate order and
+// the merge stage with the fp32 path.
 #include <cuda.h>
 #include <float.h>
 #include <string.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -130,7 +132,7 @@ __global__ void __launch_bounds__(256) topk_stage_kernel(const float* __restrict
     }
 }
 
-// ---- K10: nearest-neighbour search over a 16-bit database on the tensor cores ---------------------------------------------------
+// ---- K10: nearest-neighbour search over a 16-bit or int8 database on the tensor cores --------------------------------------------
 // CTA = two consumer warpgroups (warps 0-7) + one producer warp (warp 8).  Work unit = (query tile of NQ = 8 NT <= 128 queries, database
 // partition of rows_per_part rows); the partition is walked in tiles of KB = 128 rows, 64 per consumer warpgroup.
 //   producer  one thread: per tile and per 64-column chunk of dim, the tile's database box [128 x 64] and the query box [NQ x 64]
@@ -147,11 +149,19 @@ __global__ void __launch_bounds__(256) topk_stage_kernel(const float* __restrict
 //             is compacted after the tile (bitonic sort in shared memory, best kk kept, theta raised), so one tile never overflows it.
 //   end       every query's buffer is sorted once more and its best kk (padded with (-inf, INT_MAX)) go to the candidate matrix at
 //             [query, partition * kk]; launch_topk_stage's merge passes finish the ranking across partitions.
-constexpr int KB = 128, KC = 64, KSTAGES = 4, KSORT = 2048;      // rows per tile, columns per chunk, ring depth, sort capacity
+// The int8 instance (KOp::S8) keeps all of this and changes three things.  A chunk is 128 bytes of a row either way, so 128 int8
+// columns instead of 64 16-bit ones, and the boxes, the swizzle and the descriptor steps are the same.  The MMA is m64nNk32 s8.s8
+// with int32 accumulators: exact sums, four k32 steps per chunk.  The score step turns each sum into
+// fp32(fp32(float_rn(acc) * s_q) * s_x) before the theta test: the query scales s_q are staged in shared memory once per CTA, and
+// each consumer thread loads the row scales s_x of its two rows per tile from global memory, guarded, so rows at or past row_end
+// never read the scale array.
+constexpr int KB = 128, KC = 64, KSTAGES = 4, KSORT = 2048;      // rows per tile, 16-bit columns per chunk, ring depth, sort capacity
 constexpr int KNN_THREADS = 288;
 constexpr uint32_t KDB_BYTES = KB * KC * 2;
 
-template <int NT>
+enum class KOp { F16, BF16, S8 };                                // K10's operand kinds
+
+template <KOp OP, int NT>
 struct KnnGeo {
     static constexpr int NQ = 8 * NT;
     static constexpr uint32_t Q_BYTES = NQ * KC * 2, STAGE = KDB_BYTES + Q_BYTES;
@@ -160,7 +170,8 @@ struct KnnGeo {
     static constexpr uint32_t CNT_OFF = THETA_OFF + 128 * 4;                  // int[128]
     static constexpr uint32_t FLAG_OFF = CNT_OFF + 128 * 4;                   // uint32[4]: queries to compact
     static constexpr uint32_t BAR_OFF = FLAG_OFF + 32;                        // full[KSTAGES], empty[KSTAGES]
-    static constexpr uint32_t SMEM = BAR_OFF + 16 * KSTAGES + 1024;
+    static constexpr uint32_t QS_OFF = BAR_OFF + 16 * KSTAGES;                // S8 only: float[NQ] query scales
+    static constexpr uint32_t SMEM = QS_OFF + (OP == KOp::S8 ? NQ * 4 : 0) + 1024;
     static_assert(Q_BYTES % 1024 == 0 && STAGE % 1024 == 0 && SMEM <= 227 * 1024, "K10 shared memory");
 };
 
@@ -170,17 +181,27 @@ struct KParams {
     float* out_v; int* out_i;       // [nq, parts * kk], row stride out_ld
     size_t out_ld;
     int nq, ndb, nchunks, rows_per_part, parts, kk, cap;
+    const float *qs, *xs;           // S8 only: query scales [nq], row scales [ndb]
 };
 
 CB_DEVINL void knn_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }        // both consumer warpgroups
 
-template <bool BF, int NT>
+template <KOp OP, int NT>
 CB_DEVINL void knn_mma(float (&d)[4 * NT], uint64_t da, uint64_t db, uint32_t accumulate) {
+    constexpr bool BF = OP == KOp::BF16;
     if constexpr (NT == 16) wgmma_ss_n128<BF>(d, da, db, accumulate);
     else if constexpr (NT == 8) wgmma_ss_n64<BF>(d, da, db, accumulate);
     else if constexpr (NT == 4) wgmma_ss_n32<BF>(d, da, db, accumulate);
     else if constexpr (NT == 2) wgmma_ss_n16<BF>(d, da, db, accumulate);
     else wgmma_ss_n8<BF>(d, da, db, accumulate);
+}
+template <KOp OP, int NT>
+CB_DEVINL void knn_mma(int (&d)[4 * NT], uint64_t da, uint64_t db, uint32_t accumulate) {
+    if constexpr (NT == 16) wgmma_ss_n128_s8(d, da, db, accumulate);
+    else if constexpr (NT == 8) wgmma_ss_n64_s8(d, da, db, accumulate);
+    else if constexpr (NT == 4) wgmma_ss_n32_s8(d, da, db, accumulate);
+    else if constexpr (NT == 2) wgmma_ss_n16_s8(d, da, db, accumulate);
+    else wgmma_ss_n8_s8(d, da, db, accumulate);
 }
 
 // Sort query q's n buffered candidates (256 consumer threads) and keep the best kk: back into the buffer with theta raised
@@ -213,10 +234,12 @@ CB_DEVINL void knn_sort_keep(Cand* sc, Cand* b, int n, int kk, bool final, float
     knn_bar();
 }
 
-template <bool BF, int NT>
+template <KOp OP, int NT>
 __global__ void __launch_bounds__(KNN_THREADS, 1) knn16_kernel(const __grid_constant__ KParams p) {
-    using G = KnnGeo<NT>;
+    using G = KnnGeo<OP, NT>;
     constexpr int NQ = G::NQ;
+    constexpr bool S8 = OP == KOp::S8;
+    constexpr int KCOL = S8 ? 2 * KC : KC;                         // elements in a chunk's 128 bytes
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     const uint32_t smem_base = smem_u32(smem);
@@ -225,6 +248,7 @@ __global__ void __launch_bounds__(KNN_THREADS, 1) knn16_kernel(const __grid_cons
     float* theta = reinterpret_cast<float*>(smem + G::THETA_OFF);
     int* cnt = reinterpret_cast<int*>(smem + G::CNT_OFF);
     uint32_t* flags = reinterpret_cast<uint32_t*>(smem + G::FLAG_OFF);
+    float* qscale = reinterpret_cast<float*>(smem + G::QS_OFF);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int qt = blockIdx.x / p.parts, part = blockIdx.x - qt * p.parts;
@@ -239,6 +263,8 @@ __global__ void __launch_bounds__(KNN_THREADS, 1) knn16_kernel(const __grid_cons
     }
     if (threadIdx.x < 128) { theta[threadIdx.x] = -INFINITY; cnt[threadIdx.x] = 0; }
     if (threadIdx.x < 4) flags[threadIdx.x] = 0;
+    if constexpr (S8)
+        if (threadIdx.x < NQ) qscale[threadIdx.x] = (int)threadIdx.x < nqv ? p.qs[q0 + threadIdx.x] : 0.f;
     __syncthreads();
 
     if (warp == 8) {
@@ -250,8 +276,8 @@ __global__ void __launch_bounds__(KNN_THREADS, 1) knn16_kernel(const __grid_cons
                     const uint32_t s = n % KSTAGES, st = smem_base + s * G::STAGE;
                     mbar_wait(empty + 8 * s, ((n / KSTAGES) & 1) ^ 1);
                     mbar_arrive_expect_tx(full + 8 * s, G::STAGE);
-                    tma_load_2d(st, &p.tm_db, c * KC, row_begin + t * KB, full + 8 * s);
-                    tma_load_2d(st + KDB_BYTES, &p.tm_q, c * KC, q0, full + 8 * s);
+                    tma_load_2d(st, &p.tm_db, c * KCOL, row_begin + t * KB, full + 8 * s);
+                    tma_load_2d(st + KDB_BYTES, &p.tm_q, c * KCOL, q0, full + 8 * s);
                 }
         }
         return;
@@ -261,9 +287,15 @@ __global__ void __launch_bounds__(KNN_THREADS, 1) knn16_kernel(const __grid_cons
     const int wg = warp >> 2, tc = 2 * (lane & 3);
     const int rr = wg * 64 + (warp & 3) * 16 + (lane >> 2);      // this thread: tile rows rr and rr + 8
     Cand* const bufq = p.buf + (size_t)blockIdx.x * NQ * p.cap;
-    float d[4 * NT];
+    std::conditional_t<S8, int, float> d[4 * NT];
     uint32_t n = 0;
     for (int t = 0; t < ntiles; t++) {
+        float xs[2] = {0.f, 0.f};                                  // S8: the scales of rows rr and rr + 8, loaded under the MMAs
+        if constexpr (S8) {
+            const int r = row_begin + t * KB + rr;
+            if (r < row_end) xs[0] = p.xs[r];
+            if (r + 8 < row_end) xs[1] = p.xs[r + 8];
+        }
         uint32_t prev = 0;
         for (int c = 0; c < p.nchunks; c++, n++) {
             const uint32_t s = n % KSTAGES, st = smem_base + s * G::STAGE;
@@ -271,7 +303,7 @@ __global__ void __launch_bounds__(KNN_THREADS, 1) knn16_kernel(const __grid_cons
             const uint64_t da = wgmma_desc_sw128(st + (uint32_t)wg * 64u * 128u), dq = wgmma_desc_sw128(st + KDB_BYTES);
             wgmma_fence();
             #pragma unroll
-            for (int k = 0; k < 4; k++) knn_mma<BF, NT>(d, da + 2 * k, dq + 2 * k, (uint32_t)(c | k));
+            for (int k = 0; k < 4; k++) knn_mma<OP, NT>(d, da + 2 * k, dq + 2 * k, (uint32_t)(c | k));
             wgmma_commit();
             if (c > 0) {                                           // the previous chunk's MMAs have read their stage
                 wgmma_wait<1>();
@@ -292,7 +324,9 @@ __global__ void __launch_bounds__(KNN_THREADS, 1) knn16_kernel(const __grid_cons
             #pragma unroll
             for (int e = 0; e < 4; e++) {
                 const int q = 8 * j + tc + (e & 1), row = row0 + 8 * (e >> 1);
-                float v = d[4 * j + e];
+                float v;
+                if constexpr (S8) v = __fmul_rn(__fmul_rn(__int2float_rn(d[4 * j + e]), qscale[q]), xs[e >> 1]);
+                else v = d[4 * j + e];
                 v = v != v ? -FLT_MAX : v;
                 if (q < nqv && row < row_end && v >= theta[q]) {
                     const int pos = atomicAdd(&cnt[q], 1);
@@ -327,8 +361,9 @@ typedef CUresult (*EncodeTiledFnK)(CUtensorMap*, CUtensorMapDataType, cuuint32_t
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// [rows, dim] 16-bit row-major, boxes of 64 columns x box_rows rows, 128-byte swizzle, zero fill past both ends
-bool make_rows_map(CUtensorMap* out, const void* base, int rows, int dim, int box_rows) {
+// [rows, dim] row-major 16-bit (elem_bytes 2) or int8 (1) elements, boxes of 128 bytes (64 or 128 columns) x box_rows rows,
+// 128-byte swizzle, zero fill past both ends
+bool make_rows_map(CUtensorMap* out, const void* base, int rows, int dim, int box_rows, int elem_bytes) {
     static EncodeTiledFnK enc = nullptr;
     if (!enc) {
         void* f = nullptr;
@@ -336,28 +371,94 @@ bool make_rows_map(CUtensorMap* out, const void* base, int rows, int dim, int bo
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) return false;
         enc = reinterpret_cast<EncodeTiledFnK>(f);
     }
-    const cuuint64_t dims[2] = {(cuuint64_t)dim, (cuuint64_t)rows}, strides[1] = {(cuuint64_t)dim * 2};
-    const cuuint32_t box[2] = {(cuuint32_t)KC, (cuuint32_t)box_rows}, estr[2] = {1, 1};
-    return enc(out, CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    const cuuint64_t dims[2] = {(cuuint64_t)dim, (cuuint64_t)rows}, strides[1] = {(cuuint64_t)dim * elem_bytes};
+    const cuuint32_t box[2] = {(cuuint32_t)(128 / elem_bytes), (cuuint32_t)box_rows}, estr[2] = {1, 1};
+    return enc(out, elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <bool BF, int NT>
+template <KOp OP, int NT>
 cudaError_t knn16_launch(const KParams& p, unsigned grid, cudaStream_t st) {
-    constexpr uint32_t smem = KnnGeo<NT>::SMEM;
-    cudaError_t e = cudaFuncSetAttribute(knn16_kernel<BF, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    constexpr uint32_t smem = KnnGeo<OP, NT>::SMEM;
+    cudaError_t e = cudaFuncSetAttribute(knn16_kernel<OP, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    knn16_kernel<BF, NT><<<grid, KNN_THREADS, smem, st>>>(p);
+    knn16_kernel<OP, NT><<<grid, KNN_THREADS, smem, st>>>(p);
     return cudaGetLastError();
 }
-template <bool BF>
+template <KOp OP>
 cudaError_t knn16_launch_nt(int nt, const KParams& p, unsigned grid, cudaStream_t st) {
     switch (nt) {
-        case 1: return knn16_launch<BF, 1>(p, grid, st);
-        case 2: return knn16_launch<BF, 2>(p, grid, st);
-        case 4: return knn16_launch<BF, 4>(p, grid, st);
-        case 8: return knn16_launch<BF, 8>(p, grid, st);
-        default: return knn16_launch<BF, 16>(p, grid, st);
+        case 1: return knn16_launch<OP, 1>(p, grid, st);
+        case 2: return knn16_launch<OP, 2>(p, grid, st);
+        case 4: return knn16_launch<OP, 4>(p, grid, st);
+        case 8: return knn16_launch<OP, 8>(p, grid, st);
+        default: return knn16_launch<OP, 16>(p, grid, st);
+    }
+}
+
+// K10's parameters for one launch: tensor maps over q and db of elem_bytes-wide elements, chunks of 128 bytes
+bool knn_params(KParams* p, const void* q, int nq, const void* db, int ndb, int dim, int elem_bytes, int kk, const Knn16Plan& pl,
+                void* buf, float* out_v, int* out_i, size_t out_ld) {
+    memset(p, 0, sizeof(*p));
+    if (!make_rows_map(&p->tm_db, db, ndb, dim, KB, elem_bytes) || !make_rows_map(&p->tm_q, q, nq, dim, 8 * pl.nt, elem_bytes)) return false;
+    p->buf = reinterpret_cast<Cand*>(buf);
+    p->out_v = out_v; p->out_i = out_i; p->out_ld = out_ld;
+    p->nq = nq; p->ndb = ndb;
+    p->nchunks = (dim * elem_bytes + 127) / 128;
+    p->rows_per_part = pl.rows_per_part; p->parts = pl.parts; p->kk = kk; p->cap = pl.cap;
+    return true;
+}
+
+// Q8 quantiser: one warp per row.  Lane l holds the 16-column groups l, l + 32, l + 64 and l + 96 that exist (dim % 16 == 0,
+// dim <= 2048), reduces max |x| exactly (fmaxf of magnitudes) and a finiteness flag over the warp, then writes its groups' codes
+// with 16-byte stores.  The arithmetic is the rule of clip_b200_rows_to_int8 (clip_b200.h): IEEE division, rint, clamp.
+__global__ void __launch_bounds__(256) quant_i8_kernel(const float* __restrict__ x, int n, int dim, int8_t* __restrict__ codes,
+                                                       float* __restrict__ scales) {
+    const int row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (row >= n) return;
+    const float4* xr = reinterpret_cast<const float4*>(x + (size_t)row * dim);
+    const int ng = dim / 16;
+    float4 v[16];
+    float m = 0.f;
+    bool fin = true;
+    #pragma unroll
+    for (int g = 0; g < 4; g++) {
+        const int gi = lane + 32 * g;
+        if (gi < ng) {
+            #pragma unroll
+            for (int u = 0; u < 4; u++) {
+                const float4 a = xr[4 * gi + u];
+                v[4 * g + u] = a;
+                m = fmaxf(m, fmaxf(fmaxf(fabsf(a.x), fabsf(a.y)), fmaxf(fabsf(a.z), fabsf(a.w))));
+                fin &= isfinite(a.x) && isfinite(a.y) && isfinite(a.z) && isfinite(a.w);
+            }
+        }
+    }
+    #pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    fin = __all_sync(0xffffffffu, fin);
+    float s = __fdiv_rn(m, 127.f);
+    if (!fin) s = __int_as_float(0x7fc00000);                      // NaN: a non-finite row's every score is NaN
+    const bool zero = !fin || s == 0.f;
+    if (lane == 0) scales[row] = s;
+    int4* cr = reinterpret_cast<int4*>(codes + (size_t)row * dim);
+    #pragma unroll
+    for (int g = 0; g < 4; g++) {
+        const int gi = lane + 32 * g;
+        if (gi >= ng) continue;
+        uint32_t w[4];
+        #pragma unroll
+        for (int u = 0; u < 4; u++) {
+            const float e[4] = {v[4 * g + u].x, v[4 * g + u].y, v[4 * g + u].z, v[4 * g + u].w};
+            uint32_t packed = 0;
+            #pragma unroll
+            for (int b = 0; b < 4; b++) {
+                const int c = zero ? 0 : min(127, max(-127, __float2int_rn(__fdiv_rn(e[b], s))));
+                packed |= (uint32_t)(c & 0xff) << (8 * b);
+            }
+            w[u] = packed;
+        }
+        cr[gi] = make_int4((int)w[0], (int)w[1], (int)w[2], (int)w[3]);
     }
 }
 
@@ -403,14 +504,22 @@ cudaError_t launch_knn16(const void* q, int nq, const void* db, int ndb, int dim
                          float* out_v, int* out_i, size_t out_ld, cudaStream_t st) {
     if (nq <= 0 || ndb <= 0) return cudaSuccess;
     KParams p;
-    memset(&p, 0, sizeof(p));
-    if (!make_rows_map(&p.tm_db, db, ndb, dim, KB) || !make_rows_map(&p.tm_q, q, nq, dim, 8 * pl.nt)) return cudaErrorInvalidValue;
-    p.buf = reinterpret_cast<Cand*>(buf);
-    p.out_v = out_v; p.out_i = out_i; p.out_ld = out_ld;
-    p.nq = nq; p.ndb = ndb;
-    p.nchunks = (dim + KC - 1) / KC;
-    p.rows_per_part = pl.rows_per_part; p.parts = pl.parts; p.kk = kk; p.cap = pl.cap;
-    return bf16 ? knn16_launch_nt<true>(pl.nt, p, (unsigned)pl.grid, st) : knn16_launch_nt<false>(pl.nt, p, (unsigned)pl.grid, st);
+    if (!knn_params(&p, q, nq, db, ndb, dim, 2, kk, pl, buf, out_v, out_i, out_ld)) return cudaErrorInvalidValue;
+    return bf16 ? knn16_launch_nt<KOp::BF16>(pl.nt, p, (unsigned)pl.grid, st) : knn16_launch_nt<KOp::F16>(pl.nt, p, (unsigned)pl.grid, st);
+}
+
+cudaError_t launch_knn_i8(const void* q, const float* qs, int nq, const void* db, const float* xs, int ndb, int dim, int kk,
+                          const Knn16Plan& pl, void* buf, float* out_v, int* out_i, size_t out_ld, cudaStream_t st) {
+    if (nq <= 0 || ndb <= 0) return cudaSuccess;
+    KParams p;
+    if (!knn_params(&p, q, nq, db, ndb, dim, 1, kk, pl, buf, out_v, out_i, out_ld)) return cudaErrorInvalidValue;
+    p.qs = qs; p.xs = xs;
+    return knn16_launch_nt<KOp::S8>(pl.nt, p, (unsigned)pl.grid, st);
+}
+
+void launch_rows_to_int8(const float* x, int n, int dim, void* codes, float* scales, cudaStream_t st) {
+    if (n <= 0) return;
+    quant_i8_kernel<<<(n + 7) / 8, 256, 0, st>>>(x, n, dim, reinterpret_cast<int8_t*>(codes), scales);
 }
 
 }  // namespace cb

@@ -19,6 +19,11 @@ CB_DEVINL void wgmma_fence_regs(float (&d)[R]) {
     #pragma unroll
     for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
+template <int R>
+CB_DEVINL void wgmma_fence_regs(int (&d)[R]) {
+    #pragma unroll
+    for (int i = 0; i < R; i++) asm volatile("" : "+r"(d[i])::"memory");
+}
 
 // Shared-memory matrix descriptor of a tile stored with the 128-byte swizzle (what TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): rows
 // of 128 B, 8-row groups 1024 B apart.  K-major operands use only the 8-row group stride; for an MN-major operand no wider than 64
@@ -184,6 +189,40 @@ CB_DEVINL void wgmma_ss_n8(float (&d)[4], uint64_t da, uint64_t db, uint32_t acc
     if constexpr (BF) CB_WGMMA_SS_N8("bf16");
     else CB_WGMMA_SS_N8("f16");
 #undef CB_WGMMA_SS_N8
+}
+
+// D[64 x N] (+)= A[64 x 32] . B[N x 32]^T for N = 128, 64, 32, 16 and 8: signed 8-bit operands, both K-major in shared memory
+// (128-byte swizzle: a k32 step is 32 B, as a k16 step of 16-bit operands), int32 accumulators in the fragment layout above.  The
+// integer products and sums are exact (no saturation: the int8 search keeps |D| below 2^31).  The int8 search kernel (search.cu).
+CB_DEVINL void wgmma_ss_n128_s8(int (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n\t}"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+                 : "l"(da), "l"(db), "r"(accumulate));
+}
+CB_DEVINL void wgmma_ss_n64_s8(int (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n\t}"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+                 : "l"(da), "l"(db), "r"(accumulate));
+}
+CB_DEVINL void wgmma_ss_n32_s8(int (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %18, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+                 : "l"(da), "l"(db), "r"(accumulate));
+}
+CB_DEVINL void wgmma_ss_n16_s8(int (&d)[8], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %10, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n16k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p;\n\t}"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+                 : "l"(da), "l"(db), "r"(accumulate));
+}
+CB_DEVINL void wgmma_ss_n8_s8(int (&d)[4], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %6, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n8k32.s32.s8.s8 {%0, %1, %2, %3}, %4, %5, p;\n\t}"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
+                 : "l"(da), "l"(db), "r"(accumulate));
 }
 
 }  // namespace cb

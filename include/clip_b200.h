@@ -333,6 +333,42 @@ bool clip_b200_rows_to_16bit(const struct clip_ctx * ctx, const void * d_src, si
 bool clip_b200_topk_search_16(const struct clip_ctx * ctx, const void * d_queries, size_t n_queries, const void * d_db, size_t n_db,
                               int dim, int in_type, int top_k, float * scores, int * indices);
 
+/* f32 rows -> scalar-quantised int8 rows (one signed byte per feature and one f32 scale per row, as FAISS SQ8 and USearch i8),
+ * device to device: how a database or query set is made for clip_b200_topk_search_i8.  It takes dim + 4 bytes a row.
+ * - d_src [n, dim] f32, d_codes [n, dim] int8, d_scales [n] f32, row-major, on the context's GPU, 16-byte aligned.  dim is a
+ *   multiple of 16 in [16, 2048]; n < 2^31 (n * dim may exceed 2^32).
+ * - The rule, per row, exactly: m = max_i |x_i|; s = m / 127 in f32, rounded to nearest; c_i = clamp(rint(x_i / s), -127, 127), the
+ *   division IEEE and correctly rounded, rint rounding half to even, nothing flushed to zero (the clamp matters when s is
+ *   subnormal).  A row whose s is 0 (all zeros, or m / 127 underflows) gets s = 0 and all-zero codes.  A row holding any NaN or
+ *   +-Inf gets s = NaN and all-zero codes.  No code is -128.
+ * - Refusals, with a message in clip_b200_last_error, in this order: null context; dim; n >= 2^31; then, when n > 0 (n == 0
+ *   returns true), null or misaligned pointers.  Returns once the rows are written.  Its time is kernel class 3. */
+bool clip_b200_rows_to_int8(const struct clip_ctx * ctx, const void * d_src, size_t n, int dim, void * d_codes, void * d_scales);
+
+/* Nearest-neighbour search over an int8 database (clip_b200_rows_to_int8's form) on the tensor cores: K10's s8 instance, the same
+ * kernel, plan and ranking as clip_b200_topk_search_16, reading half the bytes per row.
+ * - Inputs: query codes [n_queries, dim] and scales [n_queries], database codes [n_db, dim] and scales [n_db], as
+ *   clip_b200_rows_to_int8 writes them, on the context's GPU, 16-byte aligned.  dim is a multiple of 16 in [16, 2048].
+ * - Scores, exactly: acc = the int32 dot product of the codes (exact: |acc| <= 127^2 * 2048 < 2^31), then
+ *   score = fp32(fp32(float_rn(acc) * s_q) * s_x), both products rounded to nearest, in this order, not contracted.  A score
+ *   depends only on the query's and the row's codes and scales.  Against the exact dot product of the f32 rows q and x that
+ *   were quantised, a finite score lies within
+ *       |score - q.x| <= sum_i (|q_i| d_x + |x_i| d_q + d_q d_x) + 2^-22 |score| + 2^-149 (1 + s_x),
+ *   where d = s (1/2 + 2^-16) is how far a code times its scale can lie from the value (half a step, widened by the rounding of
+ *   x_i / s), or m - 127 s if that is larger, which happens only for subnormal s.  With normal scales that is about
+ *   sum_i (|q_i| s_x + |x_i| s_q) / 2 + dim s_q s_x / 4 + a few ulps of |score| (derived in tests/_search_i8.py).
+ * - Ranking: the best top_k of all n_db scores, score descending, then lower index first, host [n_queries, top_k], row i at
+ *   i * top_k.  A NaN score (a non-finite row or query) ranks last and is reported as -FLT_MAX.
+ * - top_k must be in [1, 1024]; a value above n_db means n_db.
+ * - Refusals, with a message in clip_b200_last_error, in this order: null context; dim; top_k; n_queries or n_db >= 2^31; then,
+ *   when there is work (n_queries == 0 or n_db == 0 returns true and writes nothing), null or misaligned device pointers and
+ *   null outputs.
+ * - Runs on the context's first GPU (in devices mode too); the database is not sharded.  Queries go in launches of up to 32768.
+ * - Workspace: clip_b200_topk_search_16's formula, in the same grow-only buffers.  Its kernel time is kernel class 8. */
+bool clip_b200_topk_search_i8(const struct clip_ctx * ctx, const void * d_q_codes, const void * d_q_scales, size_t n_queries,
+                              const void * d_db_codes, const void * d_db_scales, size_t n_db, int dim, int top_k,
+                              float * scores, int * indices);
+
 /* Batched zero-shot labelling, the batch form of clip_zero_shot_label_image (clip.h:106-107, clip.cpp:1624-1659): n images x
  * n_labels token sequences -> scores / indices [n, top_k], best first (p = (exp(s)+1e-9)/sum over ALL labels, clip.cpp:1591-1622).
  * normalize = false reproduces the reference (un-normalised embeddings).  Works in every multi-GPU mode (see below): in devices
@@ -396,7 +432,8 @@ uint64_t clip_b200_kernel_launches(const struct clip_ctx * ctx);   /* kernels la
 float    clip_b200_last_device_ms(const struct clip_ctx * ctx);    /* CUDA-event time of the last encode's kernels */
 /* per-kernel-class CUDA-event time accumulated since the last call with the same kind (0 GEMM, 1 attention,
  * 2 layernorm, 3 other, 4 the token-row kernel of the *_tokens calls, 5 the position-table resample of the *_hw calls, 6 the
- * attention-probability kernel of ATTENTION entries, 7 the 16-bit search kernel of clip_b200_topk_search_16); *count
+ * attention-probability kernel of ATTENTION entries, 7 the 16-bit search kernel of clip_b200_topk_search_16, 8 the int8 search
+ * kernel of clip_b200_topk_search_i8); *count
  * receives the number of launches.  Enabled by env CLIP_B200_PROFILE=1. */
 float    clip_b200_kernel_ms(const struct clip_ctx * ctx, int kind, uint64_t * count);
 /* CUDA-event stopwatch on the launch stream: mark(slot 0..3), then elapsed(a, b) in ms (-1 on error) */
