@@ -1581,200 +1581,200 @@ static bool ensure_cand(clip_ctx* c, size_t count) {
     return true;
 }
 
-// d_q [nq, d] x d_db [ndb, d] -> host scores / indices [nq, k], best first (ties: lower index first).  softmax: p = (exp(s)+1e-9)/sum
-// over the whole row first (clip.cpp:1591-1622); otherwise the raw dot products are ranked (nearest-neighbour search).
-// The stream is synchronised on return.  Caller holds c->mu and has set the device.
-static bool score_topk_locked(clip_ctx* c, const float* d_q, size_t nq, const float* d_db, size_t ndb, int d, int k, bool softmax,
-                              float* scores, int* indices) {
-    if (nq == 0 || ndb == 0) return true;
-    if (ndb > 0x7fffffffull || nq > 0x7fffffffull) { set_err("scoring: more than 2^31 rows"); return false; }
-    if (k <= 0 || (size_t)k > ndb) k = (int)ndb;
-    const int SL = topk_slice();
-    const size_t budget = (size_t)32 << 20;                               // floats of similarity scratch per pass (128 MB)
-    size_t CH = std::min(ndb, std::max<size_t>(budget / std::min<size_t>(nq, 256), (size_t)SL));
-    // whole rows: the normalisation needs them, and so does the host ranking taken when top_k > 1024 (a ranking per chunk would
-    // keep only the last chunk's best, numbered within that chunk)
-    if (softmax || k > 1024) CH = ndb;
-    const size_t RB = std::max<size_t>(1, std::min<size_t>({nq, budget / CH + 1, (size_t)32768}));
-    size_t nsl = 0;
-    for (size_t c0 = 0; c0 < ndb; c0 += CH) nsl += (std::min(CH, ndb - c0) + SL - 1) / SL;
-    const int kk = std::min(k, SL);
-    const bool device_select = nsl == 1 || k <= 1024;                    // each stage must shrink the candidate set
-    if (!ensure_buf(c, &c->d_logits, &c->d_logits_cap, RB * CH)) return false;
-    const size_t cand_ld = nsl * (size_t)kk;
-    if (device_select && !ensure_cand(c, RB * cand_ld)) return false;
+// What one call of the search family reads, as its public form received it: the four searches and the two row forms that make
+// their databases.  Each form fills one and calls search_call, so every form checks its arguments in the same order
+// (include/clip_b200.h), and the searches run the same pass driver.
+struct SearchCall {
+    enum Kind { SCORE, KNN16, KNN_I8, ROWS16, ROWS_I8 };
+    const char* who;                              // the public name, for messages
+    Kind kind;
+    const void* q = nullptr;                      // queries [nq, dim]; a row form: its f32 source rows [nq, dim]
+    const void* db = nullptr;                     // database rows [ndb, dim]; a row form: the rows it writes [nq, dim]
+    const void* xs = nullptr;                     // KNN_I8: database row scales [ndb]; ROWS_I8: the scales it writes [nq]
+    const void* qs = nullptr;                     // KNN_I8: query scales [nq]
+    size_t nq = 0, ndb = 0;                       // a row form: nq = n
+    int dim = 0;                                  // SCORE: the model's projection_dim, set by search_call
+    int type = 0;                                 // KNN16: in_type; ROWS16: out_type
+    int top_k = 0;                                // SCORE: <= 0 or > ndb means all ndb; KNN: [1, 1024], > ndb means ndb
+    bool softmax = false;                         // SCORE: rank p = (exp(s) + 1e-9) / sum over the row instead of s
+    float* scores = nullptr;                      // host outputs [nq, that top_k]
+    int* indices = nullptr;
+    bool search() const { return kind <= KNN_I8; }
+};
+
+// The pass driver of the four searches, for a checked call with nq, ndb > 0.  Per block of QB queries: the candidates into
+// d_cand_v/i[0] [rows, cand_ld] as `runs` sorted runs of kk, merge_candidates, the best k per row to the host, a synchronise.  Only
+// making the candidates differs: SCORE runs column chunks of CH rows through similarity [, softmax_with_sorting's p, clip.cpp:1591-1622]
+// and a top-k stage (a ranking above 1024 over more than one slice is made on the host instead); K10 is one launch per 32768 queries,
+// the merge grid's row limit.  Caller holds c->mu and has set the device.
+static bool search_locked(clip_ctx* c, const SearchCall& a) {
+    const size_t nq = a.nq, ndb = a.ndb;
+    const int k = a.top_k <= 0 || (size_t)a.top_k > ndb ? (int)ndb : a.top_k;
+    const int SL = topk_slice(), kk = std::min(k, SL);
+    const bool knn = a.kind != SearchCall::SCORE, i8 = a.kind == SearchCall::KNN_I8;
+    size_t QB = 32768, CH = ndb, nsl = 0;
+    bool device_select = true;
+    int sms = 0;
+    if (knn) {
+        CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
+    } else {
+        const size_t budget = (size_t)32 << 20;                           // floats of similarity scratch per pass (128 MB)
+        CH = std::min(ndb, std::max<size_t>(budget / std::min<size_t>(nq, 256), (size_t)SL));
+        // whole rows: the normalisation needs them, and so does the host ranking taken when top_k > 1024 (a ranking per chunk would
+        // keep only the last chunk's best, numbered within that chunk)
+        if (a.softmax || k > 1024) CH = ndb;
+        QB = std::max<size_t>(1, std::min<size_t>({nq, budget / CH + 1, (size_t)32768}));
+        for (size_t c0 = 0; c0 < ndb; c0 += CH) nsl += (std::min(CH, ndb - c0) + SL - 1) / SL;
+        device_select = nsl == 1 || k <= 1024;                            // each stage must shrink the candidate set
+        if (!ensure_buf(c, &c->d_logits, &c->d_logits_cap, QB * CH)) return false;
+        if (device_select && !ensure_cand(c, QB * nsl * kk)) return false;
+    }
     std::vector<float> hrow;
     std::vector<int> hidx;
-    for (size_t r0 = 0; r0 < nq; r0 += RB) {
-        const int rows = (int)std::min(RB, nq - r0);
-        size_t sl0 = 0;
-        for (size_t c0 = 0; c0 < ndb; c0 += CH) {
-            const int cols = (int)std::min(CH, ndb - c0);
-            { Scope s(c, K_OTHER); launch_similarity(d_q + r0 * d, d_db + c0 * d, c->d_logits, rows, cols, d, CH, c->stream); }
-            if (softmax) { Scope s(c, K_OTHER); launch_softmax_ref(c->d_logits, rows, cols, CH, c->stream); }
-            if (device_select) {
-                Scope s(c, K_OTHER);
-                launch_topk_stage(c->d_logits, nullptr, CH, rows, cols, (int)c0, kk, c->d_cand_v[0], c->d_cand_i[0], cand_ld, (int)(sl0 * kk), c->stream);
-                sl0 += ((size_t)cols + SL - 1) / SL;
-            } else {
-                // full ranking of rows longer than one sort slice (top_k > 1024): ranked on the host, as the reference does.  cols
-                // is the whole row (CH = ndb above) and k <= ndb.  NaN becomes -FLT_MAX as in topk_stage_kernel: it ranks last, ties
-                // by index, and the comparator stays a strict weak order.
-                hrow.resize((size_t)rows * cols);
-                CK(cudaMemcpy2DAsync(hrow.data(), (size_t)cols * 4, c->d_logits, CH * 4, (size_t)cols * 4, rows, cudaMemcpyDeviceToHost, c->stream));
-                CK(cudaStreamSynchronize(c->stream));
-                for (float& v : hrow) if (v != v) v = -FLT_MAX;
-                hidx.resize(cols);
-                for (int i = 0; i < rows; i++) {
-                    const float* r = hrow.data() + (size_t)i * cols;
-                    std::iota(hidx.begin(), hidx.end(), 0);
-                    std::partial_sort(hidx.begin(), hidx.begin() + k, hidx.end(), [&](int a, int b) { return r[a] > r[b] || (r[a] == r[b] && a < b); });
-                    for (int j = 0; j < k; j++) { scores[(r0 + i) * k + j] = r[hidx[j]]; indices[(r0 + i) * k + j] = hidx[j]; }
+    for (size_t r0 = 0; r0 < nq; r0 += QB) {
+        const int rows = (int)std::min(QB, nq - r0);
+        size_t runs = nsl, cand_ld = nsl * kk;
+        if (knn) {
+            const KnnPlan pl = knn_plan(rows, (int)ndb, k, sms);
+            runs = pl.parts;
+            cand_ld = (size_t)pl.parts * k;
+            if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * pl.buf_entries) || !ensure_cand(c, (size_t)rows * cand_ld)) return false;
+            const KOp op = i8 ? KOp::S8 : a.type == CLIP_B200_OUT_BF16 ? KOp::BF16 : KOp::F16;
+            const size_t q_row = i8 ? a.dim : 2 * (size_t)a.dim;               // bytes per query row
+            Scope s(c, i8 ? K_KNN_I8 : K_KNN16);
+            const cudaError_t e = launch_knn(op, (const uint8_t*)a.q + r0 * q_row, i8 ? (const float*)a.qs + r0 : nullptr, rows, a.db,
+                                             (const float*)a.xs, (int)ndb, a.dim, k, pl, c->d_knn, c->d_cand_v[0], c->d_cand_i[0], cand_ld,
+                                             c->stream);
+            if (e != cudaSuccess) { set_err(std::string(a.who) + ": launch: " + cudaGetErrorString(e)); return false; }
+        } else {
+            const float* q = (const float*)a.q + r0 * a.dim;
+            size_t sl0 = 0;
+            for (size_t c0 = 0; c0 < ndb; c0 += CH) {
+                const int cols = (int)std::min(CH, ndb - c0);
+                { Scope s(c, K_OTHER); launch_similarity(q, (const float*)a.db + c0 * a.dim, c->d_logits, rows, cols, a.dim, CH, c->stream); }
+                if (a.softmax) { Scope s(c, K_OTHER); launch_softmax_ref(c->d_logits, rows, cols, CH, c->stream); }
+                if (device_select) {
+                    Scope s(c, K_OTHER);
+                    launch_topk_stage(c->d_logits, nullptr, CH, rows, cols, (int)c0, kk, c->d_cand_v[0], c->d_cand_i[0], cand_ld, (int)(sl0 * kk), c->stream);
+                    sl0 += ((size_t)cols + SL - 1) / SL;
+                } else {
+                    // full ranking of rows longer than one sort slice (top_k > 1024): ranked on the host, as the reference does.  cols
+                    // is the whole row (CH = ndb above) and k <= ndb.  NaN becomes -FLT_MAX as in topk_stage_kernel: it ranks last, ties
+                    // by index, and the comparator stays a strict weak order.
+                    hrow.resize((size_t)rows * cols);
+                    CK(cudaMemcpy2DAsync(hrow.data(), (size_t)cols * 4, c->d_logits, CH * 4, (size_t)cols * 4, rows, cudaMemcpyDeviceToHost, c->stream));
+                    CK(cudaStreamSynchronize(c->stream));
+                    for (float& v : hrow) if (v != v) v = -FLT_MAX;
+                    hidx.resize(cols);
+                    for (int i = 0; i < rows; i++) {
+                        const float* r = hrow.data() + (size_t)i * cols;
+                        std::iota(hidx.begin(), hidx.end(), 0);
+                        std::partial_sort(hidx.begin(), hidx.begin() + k, hidx.end(), [&](int x, int y) { return r[x] > r[y] || (r[x] == r[y] && x < y); });
+                        for (int j = 0; j < k; j++) { a.scores[(r0 + i) * k + j] = r[hidx[j]]; a.indices[(r0 + i) * k + j] = hidx[j]; }
+                    }
                 }
             }
+            if (!device_select) continue;
         }
-        if (!device_select) continue;
-        const int cur = merge_candidates(c, rows, cand_ld, nsl, kk);
-        CK(cudaMemcpy2DAsync(scores + r0 * k, (size_t)k * 4, c->d_cand_v[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
-        CK(cudaMemcpy2DAsync(indices + r0 * k, (size_t)k * 4, c->d_cand_i[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
+        const int cur = merge_candidates(c, rows, cand_ld, runs, kk);
+        CK(cudaMemcpy2DAsync(a.scores + r0 * k, (size_t)k * 4, c->d_cand_v[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpy2DAsync(a.indices + r0 * k, (size_t)k * 4, c->d_cand_i[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
         CK(cudaStreamSynchronize(c->stream));
     }
     CK(cudaGetLastError());
+    return true;
+}
+
+// Every form of the family: the arguments checked in one order, the first fault refused (include/clip_b200.h), then the search pass or
+// the row kernel.
+static bool search_call(const clip_ctx* cctx, SearchCall a) {
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    const std::string who = a.who;
+    const SearchCall::Kind kind = a.kind;
+    if (!c) { set_err(who + ": null context"); return false; }
+    if ((kind == SearchCall::KNN16 || kind == SearchCall::ROWS16) && a.type != CLIP_B200_OUT_F16 && a.type != CLIP_B200_OUT_BF16) {
+        set_err(who + (kind == SearchCall::KNN16 ? ": in_type" : ": out_type") + " must be CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16");
+        return false;
+    }
+    const int step = kind == SearchCall::KNN16 ? 8 : kind == SearchCall::ROWS16 ? 4 : 16;     // SCORE's dim is the model's
+    if (kind != SearchCall::SCORE && (a.dim < step || a.dim > 2048 || a.dim % step)) {
+        set_err(who + ": dim must be a multiple of " + std::to_string(step) + " in [" + std::to_string(step) + ", 2048]");
+        return false;
+    }
+    const bool knn = kind == SearchCall::KNN16 || kind == SearchCall::KNN_I8;
+    if (knn && (a.top_k < 1 || a.top_k > 1024)) { set_err(who + ": top_k must be in [1, 1024]"); return false; }
+    if (a.nq > 0x7fffffffull || a.ndb > 0x7fffffffull) {
+        set_err(who + (a.search() ? ": n_queries and n_db must be below 2^31" : ": n must be below 2^31"));
+        return false;
+    }
+    if (a.nq == 0 || (a.search() && a.ndb == 0)) return true;
+    // the device pointers the kind reads or writes: q and db, then the int8 forms' scales.  K10 and the row kernels load and store
+    // 16 bytes at a time; the fp32 kernels read single floats.
+    const void* ptr[4] = {a.q, a.db, a.xs, a.qs};
+    const int n_ptr = kind == SearchCall::KNN_I8 ? 4 : kind == SearchCall::ROWS_I8 ? 3 : 2;
+    for (int i = 0; i < n_ptr; i++)
+        if (!ptr[i] || (kind != SearchCall::SCORE && (uintptr_t)ptr[i] % 16)) {
+            set_err(who + (kind == SearchCall::SCORE ? ": null device pointer" : ": null or not 16-byte aligned device pointer"));
+            return false;
+        }
+    if (a.search() && (!a.scores || !a.indices)) { set_err(who + ": null output"); return false; }
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    if (kind == SearchCall::SCORE) a.dim = c->has_vision ? c->vhp.projection_dim : c->thp.projection_dim;
+    if (a.search()) return search_locked(c, a);
+    if (kind == SearchCall::ROWS16) {
+        // K7 with one row per item, no CLS skip and no LayerNorm: an RNE copy.  Its offsets are size_t, so n * dim may pass 2^32.
+        Scope s(c, K_TOKEN_ROWS);
+        launch_token_rows((const float*)a.q, (size_t)a.dim, (int)a.nq, 1, 0, a.dim, nullptr, nullptr, 0.f, a.type, const_cast<void*>(a.db), c->stream);
+    } else {
+        Scope s(c, K_OTHER);
+        launch_rows_to_int8((const float*)a.q, (int)a.nq, a.dim, const_cast<void*>(a.db), (float*)const_cast<void*>(a.xs), c->stream);
+    }
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(c->stream));
     return true;
 }
 
 bool clip_b200_zero_shot_batch(const struct clip_ctx* cctx, const void* d_img, size_t n_img, const void* d_txt, size_t n_txt, float* scores,
                                int* indices, int top_k) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c) return false;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    const int d = c->has_vision ? c->vhp.projection_dim : c->thp.projection_dim;
-    return score_topk_locked(c, (const float*)d_img, n_img, (const float*)d_txt, n_txt, d, top_k, true, scores, indices);
+    SearchCall a{"clip_b200_zero_shot_batch", SearchCall::SCORE};
+    a.q = d_img; a.nq = n_img; a.db = d_txt; a.ndb = n_txt; a.top_k = top_k; a.softmax = true; a.scores = scores; a.indices = indices;
+    return search_call(cctx, a);
 }
 
 bool clip_b200_topk_search(const struct clip_ctx* cctx, const void* d_queries, size_t n_queries, const void* d_db, size_t n_db, int top_k,
                            float* scores, int* indices) {
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c) return false;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    const int d = c->has_vision ? c->vhp.projection_dim : c->thp.projection_dim;
-    return score_topk_locked(c, (const float*)d_queries, n_queries, (const float*)d_db, n_db, d, top_k, false, scores, indices);
+    SearchCall a{"clip_b200_topk_search", SearchCall::SCORE};
+    a.q = d_queries; a.nq = n_queries; a.db = d_db; a.ndb = n_db; a.top_k = top_k; a.scores = scores; a.indices = indices;
+    return search_call(cctx, a);
 }
-
-// ---- 16-bit nearest-neighbour search (K10, search.cu) ---------------------------------------------------------------
-// The pass driver of both K10 forms: launches of up to 32768 queries, each one K10 launch (`launch(r0, rows, k, plan, cand_ld)`,
-// timed as `kind`) into the grow-only workspace, the merge stages and the copies out.  Caller holds c->mu, has set the device and
-// has checked the arguments; n_queries, n_db > 0 and top_k in [1, 1024].
-extern "C++" {
-template <class Launch>
-static bool knn_search_locked(clip_ctx* c, const char* F, int kind, size_t n_queries, size_t n_db, int top_k, float* scores, int* indices,
-                              Launch launch) {
-    int sms = 0;
-    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
-    const int k = (int)std::min<size_t>((size_t)top_k, n_db), ndb = (int)n_db;
-    const size_t QB = 32768;                                              // queries per launch (the merge grid's row limit)
-    for (size_t r0 = 0; r0 < n_queries; r0 += QB) {
-        const int rows = (int)std::min(QB, n_queries - r0);
-        const Knn16Plan pl = knn16_plan(rows, ndb, k, sms);
-        const size_t cand_ld = (size_t)pl.parts * k;
-        if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * pl.buf_entries) || !ensure_cand(c, (size_t)rows * cand_ld)) return false;
-        {
-            Scope s(c, kind);
-            const cudaError_t e = launch(r0, rows, k, pl, cand_ld);
-            if (e != cudaSuccess) { set_err(std::string(F) + "launch: " + cudaGetErrorString(e)); return false; }
-        }
-        const int cur = merge_candidates(c, rows, cand_ld, (size_t)pl.parts, k);
-        CK(cudaMemcpy2DAsync(scores + r0 * k, (size_t)k * 4, c->d_cand_v[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
-        CK(cudaMemcpy2DAsync(indices + r0 * k, (size_t)k * 4, c->d_cand_i[cur], cand_ld * 4, (size_t)k * 4, rows, cudaMemcpyDeviceToHost, c->stream));
-        CK(cudaStreamSynchronize(c->stream));
-    }
-    CK(cudaGetLastError());
-    return true;
-}
-}  // extern "C++"
 
 bool clip_b200_rows_to_16bit(const struct clip_ctx* cctx, const void* d_src, size_t n, int dim, int out_type, void* d_dst) {
-    static const char* F = "clip_b200_rows_to_16bit: ";
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c) { set_err(std::string(F) + "null context"); return false; }
-    if (out_type != CLIP_B200_OUT_F16 && out_type != CLIP_B200_OUT_BF16) { set_err(std::string(F) + "out_type must be CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16"); return false; }
-    if (dim < 4 || dim > 2048 || dim % 4) { set_err(std::string(F) + "dim must be a multiple of 4 in [4, 2048]"); return false; }
-    if (n > 0x7fffffffull) { set_err(std::string(F) + "n must be below 2^31"); return false; }
-    if (n == 0) return true;
-    if (!d_src || !d_dst || ((uintptr_t)d_src | (uintptr_t)d_dst) % 16) { set_err(std::string(F) + "null or not 16-byte aligned pointer"); return false; }
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    // K7 with one row per item, no CLS skip and no LayerNorm: an RNE copy.  Its offsets are size_t, so n * dim may pass 2^32.
-    { Scope s(c, K_TOKEN_ROWS); launch_token_rows((const float*)d_src, (size_t)dim, (int)n, 1, 0, dim, nullptr, nullptr, 0.f, out_type, d_dst, c->stream); }
-    CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(c->stream));
-    return true;
+    SearchCall a{"clip_b200_rows_to_16bit", SearchCall::ROWS16};
+    a.q = d_src; a.nq = n; a.dim = dim; a.type = out_type; a.db = d_dst;
+    return search_call(cctx, a);
 }
 
 bool clip_b200_topk_search_16(const struct clip_ctx* cctx, const void* d_queries, size_t n_queries, const void* d_db, size_t n_db, int dim,
                               int in_type, int top_k, float* scores, int* indices) {
-    static const char* F = "clip_b200_topk_search_16: ";
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c) { set_err(std::string(F) + "null context"); return false; }
-    if (in_type != CLIP_B200_OUT_F16 && in_type != CLIP_B200_OUT_BF16) { set_err(std::string(F) + "in_type must be CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16"); return false; }
-    if (dim < 8 || dim > 2048 || dim % 8) { set_err(std::string(F) + "dim must be a multiple of 8 in [8, 2048]"); return false; }
-    if (top_k < 1 || top_k > 1024) { set_err(std::string(F) + "top_k must be in [1, 1024]"); return false; }
-    if (n_queries > 0x7fffffffull || n_db > 0x7fffffffull) { set_err(std::string(F) + "n_queries and n_db must be below 2^31"); return false; }
-    if (n_queries == 0 || n_db == 0) return true;
-    if (!d_queries || !d_db || ((uintptr_t)d_queries | (uintptr_t)d_db) % 16) { set_err(std::string(F) + "null or not 16-byte aligned device pointer"); return false; }
-    if (!scores || !indices) { set_err(std::string(F) + "null output"); return false; }
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    const uint16_t* q16 = (const uint16_t*)d_queries;
-    const bool bf = in_type == CLIP_B200_OUT_BF16;
-    return knn_search_locked(c, F, K_KNN16, n_queries, n_db, top_k, scores, indices, [&](size_t r0, int rows, int k, const Knn16Plan& pl, size_t cand_ld) {
-        return launch_knn16(q16 + r0 * dim, rows, d_db, (int)n_db, dim, bf, k, pl, c->d_knn, c->d_cand_v[0], c->d_cand_i[0], cand_ld, c->stream);
-    });
+    SearchCall a{"clip_b200_topk_search_16", SearchCall::KNN16};
+    a.q = d_queries; a.nq = n_queries; a.db = d_db; a.ndb = n_db; a.dim = dim; a.type = in_type; a.top_k = top_k;
+    a.scores = scores; a.indices = indices;
+    return search_call(cctx, a);
 }
 
-// ---- int8 nearest-neighbour search (K10's s8 instance, search.cu) ---------------------------------------------------
 bool clip_b200_rows_to_int8(const struct clip_ctx* cctx, const void* d_src, size_t n, int dim, void* d_codes, void* d_scales) {
-    static const char* F = "clip_b200_rows_to_int8: ";
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c) { set_err(std::string(F) + "null context"); return false; }
-    if (dim < 16 || dim > 2048 || dim % 16) { set_err(std::string(F) + "dim must be a multiple of 16 in [16, 2048]"); return false; }
-    if (n > 0x7fffffffull) { set_err(std::string(F) + "n must be below 2^31"); return false; }
-    if (n == 0) return true;
-    if (!d_src || !d_codes || !d_scales || ((uintptr_t)d_src | (uintptr_t)d_codes | (uintptr_t)d_scales) % 16) {
-        set_err(std::string(F) + "null or not 16-byte aligned pointer"); return false;
-    }
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    { Scope s(c, K_OTHER); launch_rows_to_int8((const float*)d_src, (int)n, dim, d_codes, (float*)d_scales, c->stream); }
-    CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(c->stream));
-    return true;
+    SearchCall a{"clip_b200_rows_to_int8", SearchCall::ROWS_I8};
+    a.q = d_src; a.nq = n; a.dim = dim; a.db = d_codes; a.xs = d_scales;
+    return search_call(cctx, a);
 }
 
 bool clip_b200_topk_search_i8(const struct clip_ctx* cctx, const void* d_q_codes, const void* d_q_scales, size_t n_queries,
                               const void* d_db_codes, const void* d_db_scales, size_t n_db, int dim, int top_k, float* scores, int* indices) {
-    static const char* F = "clip_b200_topk_search_i8: ";
-    clip_ctx* c = const_cast<clip_ctx*>(cctx);
-    if (!c) { set_err(std::string(F) + "null context"); return false; }
-    if (dim < 16 || dim > 2048 || dim % 16) { set_err(std::string(F) + "dim must be a multiple of 16 in [16, 2048]"); return false; }
-    if (top_k < 1 || top_k > 1024) { set_err(std::string(F) + "top_k must be in [1, 1024]"); return false; }
-    if (n_queries > 0x7fffffffull || n_db > 0x7fffffffull) { set_err(std::string(F) + "n_queries and n_db must be below 2^31"); return false; }
-    if (n_queries == 0 || n_db == 0) return true;
-    if (!d_q_codes || !d_q_scales || !d_db_codes || !d_db_scales ||
-        ((uintptr_t)d_q_codes | (uintptr_t)d_q_scales | (uintptr_t)d_db_codes | (uintptr_t)d_db_scales) % 16) {
-        set_err(std::string(F) + "null or not 16-byte aligned device pointer"); return false;
-    }
-    if (!scores || !indices) { set_err(std::string(F) + "null output"); return false; }
-    std::lock_guard<std::mutex> lk(c->mu);
-    CK(cudaSetDevice(c->device));
-    const int8_t* qc = (const int8_t*)d_q_codes;
-    const float* qs = (const float*)d_q_scales;
-    return knn_search_locked(c, F, K_KNN_I8, n_queries, n_db, top_k, scores, indices, [&](size_t r0, int rows, int k, const Knn16Plan& pl, size_t cand_ld) {
-        return launch_knn_i8(qc + r0 * dim, qs + r0, rows, d_db_codes, (const float*)d_db_scales, (int)n_db, dim, k, pl, c->d_knn,
-                             c->d_cand_v[0], c->d_cand_i[0], cand_ld, c->stream);
-    });
+    SearchCall a{"clip_b200_topk_search_i8", SearchCall::KNN_I8};
+    a.q = d_q_codes; a.qs = d_q_scales; a.nq = n_queries; a.db = d_db_codes; a.xs = d_db_scales; a.ndb = n_db; a.dim = dim;
+    a.top_k = top_k; a.scores = scores; a.indices = indices;
+    return search_call(cctx, a);
 }
 
 // =====================================================================================================================
@@ -1907,6 +1907,14 @@ bool clip_b200_zero_shot_images(const struct clip_ctx* cctx, const int n_threads
     ai.batch(imgs); ai.n_threads = n_threads; ai.normalize = normalize;
     at.in = labels; at.n = n_labels; at.normalize = normalize;
     const int d = c->vis.proj;
+    // the last phase on context r (caller holds r->mu and has set its device): its nq images against ndb labels, into the output
+    // rows from lo on
+    const auto score = [&](clip_ctx* r, size_t nq, size_t ndb, size_t lo) {
+        SearchCall s{who, SearchCall::SCORE};
+        s.q = r->d_emb[0]; s.nq = nq; s.db = r->d_emb[1]; s.ndb = ndb; s.dim = d; s.top_k = top_k; s.softmax = true;
+        s.scores = scores + lo * top_k; s.indices = indices + lo * top_k;
+        return search_locked(r, s);
+    };
     if (c->replicas.size() > 1) {
         const int w = (int)c->replicas.size();
         const size_t per = (n_labels + w - 1) / w, tot = (size_t)w * per;      // equal slots; only the last ones may be partly empty
@@ -1939,7 +1947,7 @@ bool clip_b200_zero_shot_images(const struct clip_ctx* cctx, const int n_threads
             if (hi == lo) return true;
             std::lock_guard<std::mutex> lk(r->mu);
             CK(cudaSetDevice(r->device));
-            return score_topk_locked(r, r->d_emb[0], hi - lo, r->d_emb[1], n_labels, d, top_k, true, scores + lo * top_k, indices + lo * top_k);
+            return score(r, hi - lo, n_labels, lo);
         });
     }
     const int w = ranks_mode(c) ? c->dist.world : 1, rank = ranks_mode(c) ? c->dist.rank : 0;
@@ -1954,7 +1962,7 @@ bool clip_b200_zero_shot_images(const struct clip_ctx* cctx, const int n_threads
     std::lock_guard<std::mutex> lk(c->mu);
     CK(cudaSetDevice(c->device));
     if (!gather_in_place(c, c->d_emb[1], n_labels, d)) return false;
-    return score_topk_locked(c, c->d_emb[0], n, c->d_emb[1], n_all, d, top_k, true, scores, indices);
+    return score(c, n, n_all, 0);
 }
 
 bool clip_model_quantize(const char* fname_inp, const char* fname_out, const int itype) {

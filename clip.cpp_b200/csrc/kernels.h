@@ -82,21 +82,21 @@ int topk_slice();
 void launch_topk_stage(const float* vals, const int* in_idx, size_t ld, int rows, int n, int idx_base, int kk, float* out_v, int* out_i,
                        size_t out_ld, int out_off, cudaStream_t st);
 
-// K10 16-bit nearest-neighbour search (search.cu): q [nq, dim] x db [ndb, dim], f16 or bf16, 16-byte aligned, dim % 8 == 0, dim <= 2048.
+// K10 nearest-neighbour search (search.cu): q [nq, dim] x db [ndb, dim] of operand kind op, 16-byte aligned, dim <= 2048.
+//   F16, BF16  dim % 8 == 0; qs and xs are unused (NULL)
+//   S8         int8 codes with f32 scales qs [nq] and xs [ndb], also 16-byte aligned, dim % 16 == 0;
+//              score = fp32(fp32(float(exact int32 dot) * qs) * xs)
 // Writes each query's best kk (<= 1024) per database partition, sorted, to out[query, partition * kk ...] (row stride out_ld >=
 // parts * kk); padding entries are (-inf, INT_MAX).  The plan fixes the query tile (8 nt queries), the partitions and the scratch
 // `buf` of buf_entries (value, index) pairs the launch needs.
-struct Knn16Plan {
+enum class KOp { F16, BF16, S8 };
+struct KnnPlan {
     int nt, parts, rows_per_part, grid, cap;
     size_t buf_entries;
 };
-Knn16Plan knn16_plan(int nq, int ndb, int kk, int sms);
-cudaError_t launch_knn16(const void* q, int nq, const void* db, int ndb, int dim, int bf16, int kk, const Knn16Plan& pl, void* buf,
-                         float* out_v, int* out_i, size_t out_ld, cudaStream_t st);
-// K10's int8 instance: q [nq, dim] and db [ndb, dim] int8 codes with f32 scales qs [nq] and xs [ndb], all 16-byte aligned, dim % 16
-// == 0, dim <= 2048; score = fp32(fp32(float(exact int32 dot) * qs) * xs).  The same plan, scratch and output as launch_knn16.
-cudaError_t launch_knn_i8(const void* q, const float* qs, int nq, const void* db, const float* xs, int ndb, int dim, int kk,
-                          const Knn16Plan& pl, void* buf, float* out_v, int* out_i, size_t out_ld, cudaStream_t st);
+KnnPlan knn_plan(int nq, int ndb, int kk, int sms);
+cudaError_t launch_knn(KOp op, const void* q, const float* qs, int nq, const void* db, const float* xs, int ndb, int dim, int kk,
+                       const KnnPlan& pl, void* buf, float* out_v, int* out_i, size_t out_ld, cudaStream_t st);
 // Q8 quantiser: x [n, dim] f32 -> codes [n, dim] int8 and scales [n] f32 by the rule of clip_b200_rows_to_int8 (clip_b200.h).
 // dim % 16 == 0, dim <= 2048, 16-byte aligned pointers; 64-bit offsets, so n * dim may pass 2^32.
 void launch_rows_to_int8(const float* x, int n, int dim, void* codes, float* scales, cudaStream_t st);

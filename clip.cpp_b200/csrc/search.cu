@@ -7,7 +7,7 @@
 // move in the 4th digit, which bf16 tensor-core products would do.  Each dot product is ONE sequential fmaf chain over k, the same
 // order the reference's scalar loop uses.
 //
-// K10 (knn16_kernel, below) is the separate, opt-in search over a database stored in 16 bits or in int8 with a scale per row:
+// K10 (knn_kernel, below) is the separate, opt-in search over a database stored in 16 bits or in int8 with a scale per row:
 // tensor-core scores and a top-k kept inside the kernel, so no score matrix ever reaches memory.  It shares the candidate order and
 // the merge stage with the fp32 path.
 #include <cuda.h>
@@ -93,6 +93,25 @@ constexpr int SL = 4096;
 struct Cand { float v; int i; };
 CB_DEVINL bool before(const Cand& a, const Cand& b) { return a.v > b.v || (a.v == b.v && a.i < b.i); }
 
+CB_DEVINL void knn_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }        // K10's two consumer warpgroups
+
+// Bitonic network over c[0, m) in shared memory, m a power of two, run by threads 0-255: best first in `before` order.  Each step
+// ends with a barrier of those threads: __syncthreads(), or knn_bar() (NAMED) where K10's producer warp does not take part.
+template <bool NAMED>
+CB_DEVINL void bitonic_sort(Cand* c, int m) {
+    for (int size = 2; size <= m; size <<= 1)
+        for (int stride = size >> 1; stride > 0; stride >>= 1) {
+            for (int t = threadIdx.x; t < (m >> 1); t += 256) {
+                const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
+                const bool desc = (lo & size) == 0;            // final order: best first
+                const Cand a = c[lo], b = c[hi];
+                if (before(b, a) == desc) { c[lo] = b; c[hi] = a; }
+            }
+            if (NAMED) knn_bar();
+            else __syncthreads();
+        }
+}
+
 __global__ void __launch_bounds__(256) topk_stage_kernel(const float* __restrict__ vals, const int* __restrict__ in_idx, size_t ld, int n,
                                                          int idx_base, int kk, float* __restrict__ out_v, int* __restrict__ out_i,
                                                          size_t out_ld, int out_off) {
@@ -113,16 +132,7 @@ __global__ void __launch_bounds__(256) topk_stage_kernel(const float* __restrict
         c[e] = x;
     }
     __syncthreads();
-    for (int size = 2; size <= m; size <<= 1)
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            for (int t = threadIdx.x; t < (m >> 1); t += 256) {
-                const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
-                const bool desc = (lo & size) == 0;            // final order: best first
-                const Cand a = c[lo], b = c[hi];
-                if (before(b, a) == desc) { c[lo] = b; c[hi] = a; }
-            }
-            __syncthreads();
-        }
+    bitonic_sort<false>(c, m);
     const int take = min(kk, cnt);
     float* ov = out_v + (size_t)row * out_ld + out_off + (size_t)blockIdx.x * kk;
     int* oi = out_i + (size_t)row * out_ld + out_off + (size_t)blockIdx.x * kk;
@@ -159,8 +169,6 @@ constexpr int KB = 128, KC = 64, KSTAGES = 4, KSORT = 2048;      // rows per til
 constexpr int KNN_THREADS = 288;
 constexpr uint32_t KDB_BYTES = KB * KC * 2;
 
-enum class KOp { F16, BF16, S8 };                                // K10's operand kinds
-
 template <KOp OP, int NT>
 struct KnnGeo {
     static constexpr int NQ = 8 * NT;
@@ -183,8 +191,6 @@ struct KParams {
     int nq, ndb, nchunks, rows_per_part, parts, kk, cap;
     const float *qs, *xs;           // S8 only: query scales [nq], row scales [ndb]
 };
-
-CB_DEVINL void knn_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }        // both consumer warpgroups
 
 template <KOp OP, int NT>
 CB_DEVINL void knn_mma(float (&d)[4 * NT], uint64_t da, uint64_t db, uint32_t accumulate) {
@@ -212,16 +218,7 @@ CB_DEVINL void knn_sort_keep(Cand* sc, Cand* b, int n, int kk, bool final, float
     while (m < n) m <<= 1;
     for (int e = t; e < m; e += 256) sc[e] = e < n ? b[e] : Cand{-INFINITY, 0x7fffffff};
     knn_bar();
-    for (int size = 2; size <= m; size <<= 1)
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            for (int u = t; u < (m >> 1); u += 256) {
-                const int lo = 2 * u - (u & (stride - 1)), hi = lo + stride;
-                const bool desc = (lo & size) == 0;
-                const Cand x = sc[lo], y = sc[hi];
-                if (before(y, x) == desc) { sc[lo] = y; sc[hi] = x; }
-            }
-            knn_bar();
-        }
+    bitonic_sort<true>(sc, m);
     if (final) {
         for (int e = t; e < kk; e += 256) {
             const Cand x = e < n ? sc[e] : Cand{-INFINITY, 0x7fffffff};
@@ -235,7 +232,7 @@ CB_DEVINL void knn_sort_keep(Cand* sc, Cand* b, int n, int kk, bool final, float
 }
 
 template <KOp OP, int NT>
-__global__ void __launch_bounds__(KNN_THREADS, 1) knn16_kernel(const __grid_constant__ KParams p) {
+__global__ void __launch_bounds__(KNN_THREADS, 1) knn_kernel(const __grid_constant__ KParams p) {
     using G = KnnGeo<OP, NT>;
     constexpr int NQ = G::NQ;
     constexpr bool S8 = OP == KOp::S8;
@@ -378,35 +375,22 @@ bool make_rows_map(CUtensorMap* out, const void* base, int rows, int dim, int bo
 }
 
 template <KOp OP, int NT>
-cudaError_t knn16_launch(const KParams& p, unsigned grid, cudaStream_t st) {
+cudaError_t knn_launch(const KParams& p, unsigned grid, cudaStream_t st) {
     constexpr uint32_t smem = KnnGeo<OP, NT>::SMEM;
-    cudaError_t e = cudaFuncSetAttribute(knn16_kernel<OP, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(knn_kernel<OP, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    knn16_kernel<OP, NT><<<grid, KNN_THREADS, smem, st>>>(p);
+    knn_kernel<OP, NT><<<grid, KNN_THREADS, smem, st>>>(p);
     return cudaGetLastError();
 }
 template <KOp OP>
-cudaError_t knn16_launch_nt(int nt, const KParams& p, unsigned grid, cudaStream_t st) {
+cudaError_t knn_launch_nt(int nt, const KParams& p, unsigned grid, cudaStream_t st) {
     switch (nt) {
-        case 1: return knn16_launch<OP, 1>(p, grid, st);
-        case 2: return knn16_launch<OP, 2>(p, grid, st);
-        case 4: return knn16_launch<OP, 4>(p, grid, st);
-        case 8: return knn16_launch<OP, 8>(p, grid, st);
-        default: return knn16_launch<OP, 16>(p, grid, st);
+        case 1: return knn_launch<OP, 1>(p, grid, st);
+        case 2: return knn_launch<OP, 2>(p, grid, st);
+        case 4: return knn_launch<OP, 4>(p, grid, st);
+        case 8: return knn_launch<OP, 8>(p, grid, st);
+        default: return knn_launch<OP, 16>(p, grid, st);
     }
-}
-
-// K10's parameters for one launch: tensor maps over q and db of elem_bytes-wide elements, chunks of 128 bytes
-bool knn_params(KParams* p, const void* q, int nq, const void* db, int ndb, int dim, int elem_bytes, int kk, const Knn16Plan& pl,
-                void* buf, float* out_v, int* out_i, size_t out_ld) {
-    memset(p, 0, sizeof(*p));
-    if (!make_rows_map(&p->tm_db, db, ndb, dim, KB, elem_bytes) || !make_rows_map(&p->tm_q, q, nq, dim, 8 * pl.nt, elem_bytes)) return false;
-    p->buf = reinterpret_cast<Cand*>(buf);
-    p->out_v = out_v; p->out_i = out_i; p->out_ld = out_ld;
-    p->nq = nq; p->ndb = ndb;
-    p->nchunks = (dim * elem_bytes + 127) / 128;
-    p->rows_per_part = pl.rows_per_part; p->parts = pl.parts; p->kk = kk; p->cap = pl.cap;
-    return true;
 }
 
 // Q8 quantiser: one warp per row.  Lane l holds the 16-column groups l, l + 32, l + 64 and l + 96 that exist (dim % 16 == 0,
@@ -484,8 +468,8 @@ void launch_topk_stage(const float* vals, const int* in_idx, size_t ld, int rows
     topk_stage_kernel<<<grid, 256, 0, st>>>(vals, in_idx, ld, n, idx_base, kk, out_v, out_i, out_ld, out_off);
 }
 
-Knn16Plan knn16_plan(int nq, int ndb, int kk, int sms) {
-    Knn16Plan pl;
+KnnPlan knn_plan(int nq, int ndb, int kk, int sms) {
+    KnnPlan pl;
     const int nqc = std::min(nq, 128);
     pl.nt = 1;
     while (8 * pl.nt < nqc) pl.nt <<= 1;
@@ -500,21 +484,24 @@ Knn16Plan knn16_plan(int nq, int ndb, int kk, int sms) {
     return pl;
 }
 
-cudaError_t launch_knn16(const void* q, int nq, const void* db, int ndb, int dim, int bf16, int kk, const Knn16Plan& pl, void* buf,
-                         float* out_v, int* out_i, size_t out_ld, cudaStream_t st) {
+cudaError_t launch_knn(KOp op, const void* q, const float* qs, int nq, const void* db, const float* xs, int ndb, int dim, int kk,
+                       const KnnPlan& pl, void* buf, float* out_v, int* out_i, size_t out_ld, cudaStream_t st) {
     if (nq <= 0 || ndb <= 0) return cudaSuccess;
+    const int eb = op == KOp::S8 ? 1 : 2;                          // element bytes; a chunk is 128 bytes of a row either way
     KParams p;
-    if (!knn_params(&p, q, nq, db, ndb, dim, 2, kk, pl, buf, out_v, out_i, out_ld)) return cudaErrorInvalidValue;
-    return bf16 ? knn16_launch_nt<KOp::BF16>(pl.nt, p, (unsigned)pl.grid, st) : knn16_launch_nt<KOp::F16>(pl.nt, p, (unsigned)pl.grid, st);
-}
-
-cudaError_t launch_knn_i8(const void* q, const float* qs, int nq, const void* db, const float* xs, int ndb, int dim, int kk,
-                          const Knn16Plan& pl, void* buf, float* out_v, int* out_i, size_t out_ld, cudaStream_t st) {
-    if (nq <= 0 || ndb <= 0) return cudaSuccess;
-    KParams p;
-    if (!knn_params(&p, q, nq, db, ndb, dim, 1, kk, pl, buf, out_v, out_i, out_ld)) return cudaErrorInvalidValue;
+    memset(&p, 0, sizeof(p));
+    if (!make_rows_map(&p.tm_db, db, ndb, dim, KB, eb) || !make_rows_map(&p.tm_q, q, nq, dim, 8 * pl.nt, eb)) return cudaErrorInvalidValue;
+    p.buf = reinterpret_cast<Cand*>(buf);
+    p.out_v = out_v; p.out_i = out_i; p.out_ld = out_ld;
+    p.nq = nq; p.ndb = ndb;
+    p.nchunks = (dim * eb + 127) / 128;
+    p.rows_per_part = pl.rows_per_part; p.parts = pl.parts; p.kk = kk; p.cap = pl.cap;
     p.qs = qs; p.xs = xs;
-    return knn16_launch_nt<KOp::S8>(pl.nt, p, (unsigned)pl.grid, st);
+    switch (op) {
+        case KOp::F16: return knn_launch_nt<KOp::F16>(pl.nt, p, (unsigned)pl.grid, st);
+        case KOp::BF16: return knn_launch_nt<KOp::BF16>(pl.nt, p, (unsigned)pl.grid, st);
+        default: return knn_launch_nt<KOp::S8>(pl.nt, p, (unsigned)pl.grid, st);
+    }
 }
 
 void launch_rows_to_int8(const float* x, int n, int dim, void* codes, float* scales, cudaStream_t st) {

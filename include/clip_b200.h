@@ -292,7 +292,15 @@ bool clip_b200_text_tokens_layers_device(const struct clip_ctx * ctx, const void
 /* Batched zero-shot scoring on the device (clip.cpp:1624-1659 semantics per image): d_img_vec [n_img, d], d_txt_vec [n_txt, d]
  * -> host scores/indices [n_img, top_k], best first; similarity matrix, softmax and top-k selection all run on the GPU.
  * Ranking (here and in clip_b200_topk_search): top_k <= 0 or top_k > n_txt means all n_txt, and row i of the output starts at
- * i * (that clamped top_k).  Equal scores are ordered by lower index first.  A NaN score ranks last and is reported as -FLT_MAX. */
+ * i * (that clamped top_k).  Equal scores are ordered by lower index first.  A NaN score ranks last and is reported as -FLT_MAX.
+ * Refusals (here and in clip_b200_topk_search), with a message in clip_b200_last_error that starts with the function's name, in
+ * this order: null context; a count (n_img / n_queries or n_txt / n_db) >= 2^31; then, when there is work (a count of 0 returns
+ * true and writes nothing), a null device pointer (no alignment is required) and null outputs.  These two forms used to check
+ * less, and differ from earlier versions in four ways:
+ * - a null context sets a message (it returned false without one);
+ * - the 2^31 message starts with the function's name (it started with "scoring:");
+ * - a null device pointer or null output is refused when there is work (the call used to fault on the device or fail later);
+ * - a call with one count 0 and the other >= 2^31 is refused (it returned true), the order of every search form. */
 bool clip_b200_zero_shot_batch(const struct clip_ctx * ctx, const void * d_img_vec, size_t n_img, const void * d_txt_vec,
                                size_t n_txt, float * scores, int * indices, int top_k);
 
@@ -300,7 +308,7 @@ bool clip_b200_zero_shot_batch(const struct clip_ctx * ctx, const void * d_img_v
  * (cosine similarity for normalised embeddings) of n_queries x n_db device-resident vectors, best top_k per query to the host.
  * Each score is one sequential fmaf chain over the d features.  top_k <= 0 or top_k > n_db means all n_db, and row i of the output
  * starts at i * (that clamped top_k).  Equal scores are ordered by lower index first.  A NaN score ranks last and is reported as
- * -FLT_MAX. */
+ * -FLT_MAX.  Refusals: those of clip_b200_zero_shot_batch, in the same order. */
 bool clip_b200_topk_search(const struct clip_ctx * ctx, const void * d_queries, size_t n_queries, const void * d_db, size_t n_db,
                            int top_k, float * scores, int * indices);
 

@@ -1,5 +1,5 @@
 """Device scoring checked exactly: csrc/search.cu (similarity, softmax_with_sorting arithmetic, bitonic top-k) as
-score_topk_locked in csrc/api.cu drives it, through clip_b200_topk_search and clip_b200_zero_shot_batch.
+search_locked in csrc/api.cu drives it, through clip_b200_topk_search and clip_b200_zero_shot_batch.
 
 - Similarity: each entry is one sequential fmaf chain over the features, bit for bit (_util.fmaf_chain_dot, whose fmaf is pinned
   to libm's below).  topk_search with top_k = n_db <= 4096 sorts the whole row in one device slice, so it returns every entry.
@@ -10,7 +10,7 @@ score_topk_locked in csrc/api.cu drives it, through clip_b200_topk_search and cl
 - NaN ranks last, ordered by index, and reads -FLT_MAX, on the device-selected (top_k <= 1024) and host-ranked paths alike.
 - top_k <= 0 or top_k > n means all n, and rows are packed at that stride.
 
-How score_topk_locked splits the work, for the cases below (SL = 4096 columns per sort slice):
+How search_locked splits the work of these two forms, for the cases below (SL = 4096 columns per sort slice):
   column chunk  CH = min(n_db, max(2^25 / min(n_q, 256), SL)); whole rows for softmax and for top_k > 1024
   row pass      RB = min(n_q, 2^25 / CH + 1, 32768)
   selection     on the device when the chunks hold one slice in all or top_k <= 1024 (one stage per slice, then merge stages

@@ -4,7 +4,8 @@
   so the 16-bit search must return what clip_b200_topk_search returns on the same values, byte for byte, across K10's tile (128
   rows), partition and candidate-buffer edges and the fp32 path's slice edges.
 - Random unit rows: every score within the bound of tests/_search_bound.py, and no row left out that could beat a returned one.
-- Scores depend on the query and the row alone; the contract's edges, refusals and guards.
+- Scores depend on the query and the row alone; the contract's edges and guards; refusals and empty calls through the table of
+  tests/test_gpu_search_forms.py.
 - rows_to_16bit equals numpy's round-to-nearest-even, including a call with n * dim > 2^32."""
 import ctypes as C
 import functools
@@ -14,6 +15,7 @@ import pytest
 
 from _search_bound import bits16, bound, exact, unit_rows
 from test_gpu_scoring_exact import GUARD, _Model, _assert_ranked, _tie_case, _tie_ints
+import test_gpu_search_forms as forms
 
 FLT_MAX = np.finfo(np.float32).max
 F16, BF16 = 1, 2
@@ -156,39 +158,9 @@ def test_nan_ranks_last_as_minus_flt_max(tiny):
 
 
 @pytest.mark.gpu
-def test_refusals_and_empty_calls(tiny):
-    L, ctx = tiny.prod.lib, tiny.ctx
-    q = np.zeros((4, 64), np.uint16)
-    d_q = _dev(tiny, q)
-    sc, ix = np.zeros(64, np.float32), np.zeros(64, np.int32)
-    sp, ip = sc.ctypes.data_as(C.POINTER(C.c_float)), ix.ctypes.data_as(C.POINTER(C.c_int))
-    try:
-        def call(*a):
-            return L.clip_b200_topk_search_16(*a)
-        cases = [
-            ((None, d_q, 4, d_q, 4, 64, F16, 1, sp, ip), "null context"),
-            ((ctx, d_q, 4, d_q, 4, 64, 0, 1, sp, ip), "in_type"),
-            ((ctx, d_q, 4, d_q, 4, 64, 3, 1, sp, ip), "in_type"),
-            ((ctx, d_q, 4, d_q, 4, 60, F16, 1, sp, ip), "dim"),
-            ((ctx, d_q, 4, d_q, 4, 0, F16, 1, sp, ip), "dim"),
-            ((ctx, d_q, 4, d_q, 4, 2056, F16, 1, sp, ip), "dim"),
-            ((ctx, d_q, 4, d_q, 4, 64, F16, 0, sp, ip), "top_k"),
-            ((ctx, d_q, 4, d_q, 4, 64, F16, 1025, sp, ip), "top_k"),
-            ((ctx, d_q, 1 << 31, d_q, 4, 64, F16, 1, sp, ip), "2^31"),
-            ((ctx, d_q, 4, d_q, 1 << 31, 64, F16, 1, sp, ip), "2^31"),
-            ((ctx, None, 4, d_q, 4, 64, F16, 1, sp, ip), "aligned"),
-            ((ctx, d_q, 4, d_q + 8, 3, 64, F16, 1, sp, ip), "aligned"),
-            ((ctx, d_q, 4, d_q, 4, 64, F16, 1, None, ip), "null output"),
-        ]
-        for args, word in cases:
-            assert not call(*args), (word, args[1:8])
-            assert word in tiny.prod.last_error(), (word, tiny.prod.last_error())
-        sc[:] = 7.0
-        assert call(ctx, d_q, 0, d_q, 4, 64, F16, 1, sp, ip) and call(ctx, d_q, 4, d_q, 0, 64, F16, 1, sp, ip)
-        assert call(ctx, None, 0, None, 0, 64, BF16, 1, None, None)
-        assert (sc == 7.0).all()
-    finally:
-        L.clip_b200_device_free(ctx, d_q)
+def test_refusals_and_empty_calls(prod):
+    """refusals, their order and empty calls: the table of the search forms (tests/test_gpu_search_forms.py) for this form"""
+    forms.check_form(prod, "clip_b200_topk_search_16")
 
 
 # ---- e. rows_to_16bit -------------------------------------------------------------------------------------------------------
@@ -217,11 +189,6 @@ def test_rows_to_16bit_is_rne(tiny, out_type):
     x.reshape(-1)[:5004] = np.concatenate([np.uint32(0x3F800000) | (t << np.uint32(3)), ties]).view(np.float32)
     got = _rows16(tiny, x, out_type)
     assert np.array_equal(got, bits16(x, out_type == BF16))
-    L = tiny.prod.lib
-    assert not L.clip_b200_rows_to_16bit(tiny.ctx, None, 4, 64, 0, None) and "out_type" in tiny.prod.last_error()
-    assert not L.clip_b200_rows_to_16bit(tiny.ctx, None, 4, 62, out_type, None) and "dim" in tiny.prod.last_error()
-    assert not L.clip_b200_rows_to_16bit(tiny.ctx, None, 4, 64, out_type, None) and "aligned" in tiny.prod.last_error()
-    assert L.clip_b200_rows_to_16bit(tiny.ctx, None, 0, 64, out_type, None)
 
 
 @pytest.mark.gpu

@@ -6,8 +6,8 @@ rule of tests/_search_i8.py.
   _tie_case's ranking and what clip_b200_topk_search returns on the same values, byte for byte.
 - Random unit rows quantised on the GPU: scores and indices equal the numpy emulation and ranking bit for bit; every score lies
   within the bound of the f32 dot product, and no row left out could beat a returned one.
-- Scores depend on the query and the row alone; non-finite rows and queries rank last; refusals, empty calls and output guards; a
-  database past 2^32 bytes."""
+- Scores depend on the query and the row alone; non-finite rows and queries rank last; refusals, empty calls and output guards
+  (the refusals through the table of tests/test_gpu_search_forms.py); a database past 2^32 bytes."""
 import ctypes as C
 
 import numpy as np
@@ -15,7 +15,8 @@ import pytest
 
 from _search_i8 import FLT_MAX, bound, emulate, exact, quantize, rank, unit_rows
 from test_gpu_scoring_exact import GUARD, _Model, _assert_ranked, _tie_case, _tie_ints
-from test_gpu_search_16 import EXACT_CASES
+from test_gpu_search_16 import EXACT_CASES, _dev
+import test_gpu_search_forms as forms
 
 
 @pytest.fixture(scope="module")
@@ -23,12 +24,6 @@ def tiny(prod):
     m = _Model(prod, "tiny", "f16")                    # projection dim 128: the fp32 path's d
     yield m
     prod.free(m.ctx)
-
-
-def _dev(m, a):
-    p = m.prod.lib.clip_b200_device_malloc(m.ctx, max(a.nbytes, 16))
-    assert p and m.prod.lib.clip_b200_memcpy_h2d(m.ctx, p, a.ctypes.data, a.nbytes), m.prod.last_error()
-    return p
 
 
 def _free(m, *ps):
@@ -110,28 +105,9 @@ def test_rows_to_int8_matches_rule(tiny, dim):
 
 
 @pytest.mark.gpu
-def test_rows_to_int8_refusals(tiny):
-    L, ctx = tiny.prod.lib, tiny.ctx
-    d = L.clip_b200_device_malloc(ctx, 4096)
-    try:
-        cases = [
-            ((None, d, 4, 64, d, d), "null context"),
-            ((ctx, None, 1 << 31, 24, None, None), "dim"),
-            ((ctx, d, 4, 0, d, d), "dim"),
-            ((ctx, d, 4, 2064, d, d), "dim"),
-            ((ctx, None, 1 << 31, 64, None, None), "2^31"),
-            ((ctx, None, 4, 64, d, d), "aligned"),
-            ((ctx, d, 4, 64, None, d), "aligned"),
-            ((ctx, d, 4, 64, d, None), "aligned"),
-            ((ctx, d, 4, 64, d, d + 4), "aligned"),
-            ((ctx, d + 8, 4, 64, d, d), "aligned"),
-        ]
-        for args, word in cases:
-            assert not L.clip_b200_rows_to_int8(*args), (word, args[2:4])
-            assert word in tiny.prod.last_error(), (word, tiny.prod.last_error())
-        assert L.clip_b200_rows_to_int8(ctx, None, 0, 64, None, None)
-    finally:
-        _free(tiny, d)
+def test_rows_to_int8_refusals(prod):
+    """refusals, their order and empty calls: the table of the search forms (tests/test_gpu_search_forms.py) for this form"""
+    forms.check_form(prod, "clip_b200_rows_to_int8")
 
 
 @pytest.mark.gpu
@@ -274,42 +250,9 @@ def test_non_finite_rows_and_queries_rank_last(tiny):
 
 # ---- 7. refusals, empty calls, guards ---------------------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_refusals_and_empty_calls(tiny):
-    L, ctx = tiny.prod.lib, tiny.ctx
-    d = _dev(tiny, np.zeros(4096, np.int8))
-    sc, ix = np.zeros(64, np.float32), np.zeros(64, np.int32)
-    sp, ip = sc.ctypes.data_as(C.POINTER(C.c_float)), ix.ctypes.data_as(C.POINTER(C.c_int))
-    try:
-        def call(*a):
-            return L.clip_b200_topk_search_i8(*a)
-        cases = [
-            ((None, d, d, 4, d, d, 4, 64, 1, sp, ip), "null context"),
-            ((ctx, d, d, 4, d, d, 4, 24, 0, sp, ip), "dim"),           # dim before top_k
-            ((ctx, d, d, 4, d, d, 4, 0, 1, sp, ip), "dim"),
-            ((ctx, d, d, 4, d, d, 4, 2064, 1, sp, ip), "dim"),
-            ((ctx, d, d, 1 << 31, d, d, 4, 64, 0, sp, ip), "top_k"),   # top_k before 2^31
-            ((ctx, d, d, 4, d, d, 4, 64, 1025, sp, ip), "top_k"),
-            ((ctx, None, d, 1 << 31, d, d, 4, 64, 1, sp, ip), "2^31"),  # 2^31 before pointers
-            ((ctx, d, d, 4, d, d, 1 << 31, 64, 1, sp, ip), "2^31"),
-            ((ctx, None, d, 4, d, d, 4, 64, 1, None, ip), "aligned"),  # pointers before outputs
-            ((ctx, d, None, 4, d, d, 4, 64, 1, sp, ip), "aligned"),
-            ((ctx, d, d, 4, None, d, 4, 64, 1, sp, ip), "aligned"),
-            ((ctx, d, d, 4, d, None, 4, 64, 1, sp, ip), "aligned"),
-            ((ctx, d, d + 4, 4, d, d, 4, 64, 1, sp, ip), "aligned"),
-            ((ctx, d, d, 4, d + 16, d + 8, 3, 64, 1, sp, ip), "aligned"),
-            ((ctx, d, d, 4, d, d, 4, 64, 1, None, ip), "null output"),
-            ((ctx, d, d, 4, d, d, 4, 64, 1, sp, None), "null output"),
-        ]
-        for args, word in cases:
-            assert not call(*args), (word, args[3:9])
-            assert word in tiny.prod.last_error(), (word, tiny.prod.last_error())
-        sc[:] = 7.0
-        ix[:] = -7
-        assert call(ctx, d, d, 0, d, d, 4, 64, 1, sp, ip) and call(ctx, d, d, 4, d, d, 0, 64, 1, sp, ip)
-        assert call(ctx, None, None, 0, None, None, 0, 64, 1, None, None)
-        assert (sc == 7.0).all() and (ix == -7).all()
-    finally:
-        _free(tiny, d)
+def test_refusals_and_empty_calls(prod):
+    """refusals, their order and empty calls: the table of the search forms (tests/test_gpu_search_forms.py) for this form"""
+    forms.check_form(prod, "clip_b200_topk_search_i8")
 
 
 # ---- 8. a database past 2^32 bytes ------------------------------------------------------------------------------------------
