@@ -6,7 +6,9 @@ and against emulated faults (tests/test_attention_long_bound.py).
 Notation: u = 2^-24 (fp32), u16 the unit roundoff of the 16-bit operand type (2^-8 for bf16: 8 significant bits; 2^-11 for
 fp16: 11 bits).  q, k, v are the 16-bit operands (exact in fp64), s_j = q.k_j the exact score, m = max_j s_j over the keys the
 row sees, pi_j = e^(s_j - m) / l with l = sum_j e^(s_j - m) >= 1, O = sum_j pi_j v_j, A = sum_j pi_j |v_j| >= |O|.  nb is the
-number of 128-key blocks the row's group visits and kend the keys it visits.
+number of key blocks the row's group visits -- blocks of the instance's width, keys_per_block(dh): 128 keys at head_dim 64 and 80,
+64 at 104 -- and kend the keys it visits.  dh is the width the kernel multiplies: at head_dim 104 the operands padded with zeros to
+112 columns, so S takes 7 k16 steps.
 
 Every error of the kernel is one of these, in the order it happens:
   1. S = Q.K^T on the tensor cores: products exact in fp32, dh/16 k16 steps accumulated in fp32.  As in test_gpu_gemm.py, with
@@ -27,9 +29,10 @@ Every error of the kernel is one of these, in the order it happens:
      P_abs = sum over keys with w_j < min normal of min(tiny, w_j) |v_j|.
   With numerator N' = sum w_j (1 + e_j + r_j) v_j (+ P_abs) and denominator l' = sum w_j (1 + e'_j):
      |N'/l' - O| <= ((2 E + u16) A + P_abs / l) / (1 - E).
-  6. The sums.  O: per block one rescale rounding and 8 k16 steps of P.V into fp32, i.e. (2 kend/16 + 4 + nb) u sum |p v|
-     (<= 1.01 A l).  l: 32 keys per thread and block summed in sequence (17 roundings deep: one pair, 16 chained adds), then one
-     multiply and one add per block, then 2 shuffles: (19 + 2 nb) u relative.
+  6. The sums.  O: per block one rescale rounding and a k16 step of P.V per 16 keys into fp32, i.e. (2 kend/16 + 4 + nb) u
+     sum |p v| (<= 1.01 A l).  l: per thread and block 32 keys summed in sequence at 128-key blocks (17 roundings deep: one pair,
+     16 chained adds; 16 keys and 9 deep at 64-key blocks, which the 17-deep term covers), then one multiply and one add per block,
+     then 2 shuffles: (19 + 2 nb) u relative.
   7. 1/l (correctly rounded; 2^-23 even for an approximate reciprocal) and o * (1/l): 3 u |O'|.
   8. The final 16-bit rounding: u16 |O'| (fp16 outputs below 2^-14: + 2^-25).
 The bound is the sum of 5-8, with O' = |O| + the error before step 8, and 1 % on top for second-order products (every term is far
@@ -42,6 +45,11 @@ MIN_NORMAL = {1: 2.0 ** -126, 0: 2.0 ** -14}
 TINY = {1: 2.0 ** -126, 0: 2.0 ** -25}
 EX2 = 2.0 ** -22
 AG, AK = 64, 128                                # query rows per group, keys per block (csrc/attention_tc.cu)
+
+
+def keys_per_block(dh):
+    """K3's key block at head_dim dh: 64 keys at 104 (a three-stage ring of 64-key blocks), 128 otherwise"""
+    return 64 if dh == 104 else AK
 
 
 def bf16(x):
@@ -62,12 +70,13 @@ def kend_of_rows(rows, T, causal):
     return np.minimum(T, (rows // AG + 1) * AG) if causal else np.full(rows.shape, T)
 
 
-def reference_rows(q, k, v, rows, causal, bf):
-    """fp64 attention of query rows `rows` over every key they see, and the element-wise bound of the module docstring.
-    q, k, v: [T, dh] of values exact in the 16-bit type (Q already scaled).  Returns (O [R, dh], bound [R, dh])."""
+def reference_rows(q, k, v, rows, causal, bf, kb=AK):
+    """fp64 attention of query rows `rows` over every key they see, and the element-wise bound of the module docstring for a
+    kernel of kb-key blocks.  q, k: [T, dh] and v: [T, dv] of values exact in the 16-bit type (Q already scaled); dh counts the
+    k16 steps of S, so at head_dim 104 q and k come padded to 112 columns and v does not.  Returns (O [R, dv], bound [R, dv])."""
     rows = np.asarray(rows)
     if len(rows) > 128:                         # keeps the [rows, T] fp64 intermediates to a few hundred MB at T = 85 265
-        parts = [reference_rows(q, k, v, rows[i:i + 128], causal, bf) for i in range(0, len(rows), 128)]
+        parts = [reference_rows(q, k, v, rows[i:i + 128], causal, bf, kb) for i in range(0, len(rows), 128)]
         return np.concatenate([p[0] for p in parts]), np.concatenate([p[1] for p in parts])
     T, dh = k.shape
     q = np.asarray(q, np.float64)[rows]
@@ -85,7 +94,7 @@ def reference_rows(q, k, v, rows, causal, bf):
     d = (2 * dh / 16 + 4) * U * np.where(vis, np.abs(q) @ np.abs(k).T, 0.0).max(-1, keepdims=True)
     smax = np.where(vis, np.abs(s), 0.0).max(-1, keepdims=True) + d
     kend = kend_of_rows(rows, T, causal)[:, None].astype(np.float64)
-    nb = np.ceil(kend / AK)
+    nb = np.ceil(kend / kb)
     e = np.expm1(d) + 12 * U * smax + EX2 * (1 + nb)
     u16 = U16[bf]
     small = w * np.exp(2 * d) < MIN_NORMAL[bf]
@@ -111,8 +120,8 @@ def pattern_head(pattern, T, dh, causal, rng):
     """(q, k, v) [T, dh] float32 for one (sequence, head), Q already scaled:
       random       scores of a few units, so a handful of keys carry each row
       needle       q_t = alpha k_pi(t): one key thousands of positions away dominates (score ~ 24 against a max of ~ 13 elsewhere)
-      ramp         the score grows by 0.25 per 128-key block (exactly, through two integer columns), so every block raises the
-                   running maximum and rescales O and l; half a unit more across each block
+      ramp         the score grows by 0.25 per key block of K3 at this head_dim (keys_per_block; exactly, through two integer
+                   columns), so every block raises the running maximum and rescales O and l; half a unit more across each block
       late_spike   a score of 60 at key T - 3 (in the last block), small noise elsewhere
       early_spike  a score of 60 at key 2
     """
@@ -129,9 +138,10 @@ def pattern_head(pattern, T, dh, causal, rng):
         k = rng.standard_normal((T, dh)) * 0.05
         j = np.arange(T)
         if pattern == "ramp":
-            kb = j // AK
+            w = keys_per_block(dh)
+            kb = j // w
             q[:, 0], q[:, 1], q[:, 2] = 26 * 0.25, 0.25, 0.5          # powers of two times small integers: exact in 16 bits
-            k[:, 0], k[:, 1], k[:, 2] = kb // 26, kb % 26, (j % AK) / AK
+            k[:, 0], k[:, 1], k[:, 2] = kb // 26, kb % 26, (j % w) / w
         else:
             q[:, 0] = 1.0
             k[:, 0] = np.where(j == (T - 3 if pattern == "late_spike" else 2), 60.0, 0.0)

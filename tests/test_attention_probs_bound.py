@@ -1,6 +1,7 @@
 """The bound of tests/_attention_probs_bound.py, checked without a GPU: it holds for a numpy emulation of K9's arithmetic at every
 block structure the kernel meets (one ragged block, exact multiples of 64 and 128, one key past them, several blocks, ViT-L/14@336's
-577 tokens), both operand types and both head dims, causal or not; and it is tight enough to reject two wrong results -- a softmax of
+577 tokens) and at any-resolution lengths (2049 causal, 4097), both operand types and head_dim 64, 80 and 104 (the operands padded
+to the 112 columns the kernel multiplies), causal or not; and it is tight enough to reject two wrong results -- a softmax of
 exponentials rounded to fp16 (what K3 multiplies V with) and a probability row shifted by one key."""
 import numpy as np
 import pytest
@@ -12,13 +13,17 @@ TS = [1, 17, 64, 65, 128, 129, 257, 577]
 
 
 def operands(T, dh, bf, causal, seed, pattern="random"):
+    """Q and K of one (sequence, head), rounded to the operand type; head_dim 104 padded with zeros to 112 columns"""
     rng = np.random.default_rng(seed)
     q, k, _ = pattern_head(pattern, T, dh, causal, rng)
-    return round16(q, bf), round16(k, bf)
+    q, k = round16(q, bf), round16(k, bf)
+    if dh == 104:
+        q, k = (np.concatenate([x, np.zeros((T, 8), np.float32)], 1) for x in (q, k))
+    return q, k
 
 
 @pytest.mark.parametrize("T", TS)
-@pytest.mark.parametrize("dh", [64, 80])
+@pytest.mark.parametrize("dh", [64, 80, 104])
 @pytest.mark.parametrize("bf", [0, 1])
 def test_bound_holds_for_the_emulation(T, dh, bf):
     causal = int(T in (65, 129))
@@ -27,6 +32,23 @@ def test_bound_holds_for_the_emulation(T, dh, bf):
     for out_type in (0, 1, 2):
         pi, bound = reference_probs(q, k, causal, bf, out_type)
         assert exceed(to_out(p32, out_type), pi, bound) <= 1.0, (T, dh, bf, out_type)
+
+
+@pytest.mark.parametrize("T,causal", [(2049, 1), (4097, 0)])
+@pytest.mark.parametrize("dh", [64, 104])
+@pytest.mark.parametrize("bf", [0, 1])
+def test_bound_holds_at_long_sequences(T, causal, dh, bf):
+    """17 and 33 blocks of 128 keys: l summed over many rescaled blocks, every row, every output type"""
+    q, k = operands(T, dh, bf, causal, 7 * T + dh + bf)
+    p32 = emulate(q, k, causal)
+    worst = 0.0
+    for r0 in range(0, T, 1024):                # row slices keep the fp64 [rows, T] intermediates small
+        rows = np.arange(r0, min(T, r0 + 1024))
+        for out_type in (0, 1, 2):
+            pi, bound = reference_probs(q, k, causal, bf, out_type, rows=rows)
+            worst = max(worst, exceed(to_out(p32[rows], out_type), pi, bound))
+    print("T=%d causal=%d dh=%d bf=%d: worst err/bound %.3f" % (T, causal, dh, bf, worst))
+    assert worst <= 1.0, worst
 
 
 @pytest.mark.parametrize("pattern", ["needle", "ramp", "late_spike", "early_spike"])

@@ -1,8 +1,9 @@
 """K3 (csrc/attention_tc.cu) at the sequence lengths any-resolution images and long text contexts reach, through the test hook
 clip_b200_debug_attention_hd: T up to 85 265 (a 4088 x 4088 image at patch 14), causal T up to 4096 (the longest context_length
-the loader takes).  Hundreds of 128-key blocks per group run the ring stages, the running max and the fp32 sums of l and O far
-past anything the 224 / 336 models reach, with TMA row coordinates far from 0.  nseq = 2 and H = 3 throughout, so that with an
-odd number of 64-row groups per head the warpgroup pairs straddle heads.
+the loader takes), at head_dim 64, 80 and 104.  Hundreds of key blocks per group -- 128 keys in a two-stage ring at 64 and 80, 64
+keys in a three-stage ring at 104 -- run the ring stages, the running max and the fp32 sums of l and O far past anything the
+224 / 336 models reach, with TMA row coordinates far from 0.  nseq = 2 and H = 3 throughout, so that with an odd number of 64-row
+groups per head the warpgroup pairs straddle heads.
 
   1. Counting: Q = 0 and V in {-1, 0, +1}, so every score is exactly 0 and every p exactly 1 (ex2.approx(0) = 1).  O is then an
      exact integer sum and l an exact key count, both below 2^24 and so exact in the fp32 accumulators whatever the summation
@@ -18,8 +19,9 @@ odd number of 64-row groups per head the warpgroup pairs straddle heads.
 import numpy as np
 import pytest
 
-from _attention_bound import PATTERNS, exceed, pattern_head, reference_rows, round16, sampled_rows
+from _attention_bound import PATTERNS, exceed, keys_per_block, pattern_head, reference_rows, round16, sampled_rows
 from test_gpu_attention_hd80 import run
+from test_gpu_attention_probs_hd104 import padded
 
 pytestmark = pytest.mark.gpu
 
@@ -27,7 +29,8 @@ NSEQ, H = 2, 3
 LONG = [(1025, 0), (2305, 0), (4097, 0), (16385, 0), (65537, 0), (85265, 0), (78, 1), (248, 1), (1000, 1), (2049, 1), (4096, 1)]
 # Column kinds: alternating +-1 (prefix sums 0 / +-1, so a causal off-by-one turns 0 into +-1 / (t + 1)); +-1 square waves whose
 # periods divide neither 64 nor 128 (a dropped, doubled or misplaced key block changes c_t); a random walk over {-1, 0, +1}; and a
-# constant +1 column, whose output must be exactly 1.
+# constant +1 column, whose output must be exactly 1.  Each (sequence, head) draws its own columns, so at head_dim 104 a store of
+# the 8 pad columns over the next head's columns 0-7, or a block read from another head's ring slot, shows.
 KINDS = ("alt", 3, 5, 7, 127, 129, 1000, "walk", "one")
 
 
@@ -60,7 +63,7 @@ def rounding_interval(c, l, bf):
 
 
 @pytest.mark.parametrize("T,causal", LONG)
-@pytest.mark.parametrize("dh", [64, 80])
+@pytest.mark.parametrize("dh", [64, 80, 104])
 @pytest.mark.parametrize("bf", [1, 0])
 def test_counting_every_row(prod, T, causal, dh, bf):
     rng = np.random.default_rng(T + dh)
@@ -86,7 +89,7 @@ def test_counting_every_row(prod, T, causal, dh, bf):
 
 
 @pytest.mark.parametrize("T,causal", LONG)
-@pytest.mark.parametrize("dh", [64, 80])
+@pytest.mark.parametrize("dh", [64, 80, 104])
 @pytest.mark.parametrize("bf", [1, 0])
 def test_sampled_rows_against_fp64(prod, T, causal, dh, bf):
     rng = np.random.default_rng(3 * T + dh + bf)
@@ -98,9 +101,12 @@ def test_sampled_rows_against_fp64(prod, T, causal, dh, bf):
     got = run(prod, qkv.reshape(NSEQ * T, -1), NSEQ, T, H, causal, bf, dh=dh).reshape(NSEQ, T, H, dh)
     assert np.isfinite(got).all()
     rows = sampled_rows(T, causal, rng, 256 if T <= 16385 else 64)       # the fp64 rows cost O(T) each
+    # the bound at the instance's key blocks, of the Q and K that S multiplies (head_dim 104: padded to 112 columns, 7 k16 steps)
+    pad = padded if dh == 104 else (lambda x: x)
     for i, pattern in enumerate(slots):
         s, h = i // H, i % H
-        want, bound = reference_rows(qkv[s, :, 0, h], qkv[s, :, 1, h], qkv[s, :, 2, h], rows, causal, bf)
+        want, bound = reference_rows(pad(qkv[s, :, 0, h]), pad(qkv[s, :, 1, h]), qkv[s, :, 2, h], rows, causal, bf,
+                                     keys_per_block(dh))
         r = exceed(got[s, rows, h], want, bound)
         print("T=%d causal=%d dh=%d bf=%d %-11s %d rows  err/bound %.3f" % (T, causal, dh, bf, pattern, len(rows), r))
         assert r <= 1.0, (pattern, r)

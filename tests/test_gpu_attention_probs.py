@@ -3,12 +3,21 @@ against an fp64 softmax of the 16-bit-rounded Q and K within the bound derived i
 that end a 64-row group or a 128-key block early, exactly or one past it, several sequences per launch (so groups end mid-sequence),
 one to sixteen heads, head_dim 64 and 80, both operand types.  Rows sum to 1 within the bound, causal entries above the diagonal are
 +0 bit for bit, the 16-bit outputs are the RNE of the f32 output bit for bit, the CLS row equals row 0 of the full map bit for bit,
-and the guard bytes after the output stay untouched (the hook returns 5 otherwise)."""
+and the guard bytes after the output stay untouched (the hook returns 5 otherwise).
+
+At the lengths any-resolution images and long text contexts reach (full maps at T = 2049 causal and 4097, CLS rows up to
+T = 85 265, where one (sequence, head) runs hundreds of 128-key blocks twice), at head_dim 64, 80 and 104:
+  1. Counting: Q = 0, so every score is exactly 0, every weight ex2(0) = 1 and l an exact key count (below 2^24, so exact in fp32
+     whatever the order of the sums).  Every visible entry of row t is then fl(1 / l) bit for bit, l = T (t + 1 when causal), every
+     masked entry +0, and the 16-bit outputs the RNE of that.  Every element of every row.
+  2. The score patterns of tests/_attention_bound.py, one per (sequence, head), against fp64 on sampled rows of the full maps
+     and on the CLS row, within the bound of tests/_attention_probs_bound.py."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
+from _attention_bound import PATTERNS, pattern_head, sampled_rows
 from _attention_probs_bound import exceed, reference_probs, round16
 
 pytestmark = pytest.mark.gpu
@@ -74,3 +83,101 @@ def test_bad_arguments(prod):
     assert "64 or 80" in prod.last_error()
     assert L.clip_b200_debug_attention_probs(1, 1, 5, 2, 64, 0, 0, 3, qkv.ctypes.data_as(fp), out.ctypes.data) == 2
     assert L.clip_b200_debug_attention_probs(1, 0, 5, 2, 64, 0, 0, 0, qkv.ctypes.data_as(fp), out.ctypes.data) == 2
+
+
+# ---- long sequences --------------------------------------------------------------------------------------------------------------
+NSEQ_L, H_L = 2, 3
+LONG_FULL = [(2049, 1), (4097, 0)]
+LONG_CLS = [(4097, 0), (16385, 0), (65537, 0), (85265, 0), (4096, 1)]
+
+
+def kernel_operand(x, dh):
+    """Q or K as the kernel multiplies it: at head_dim 104 padded with zeros to 112 columns (7 k16 steps of S)"""
+    from test_gpu_attention_probs_hd104 import padded       # imported here: that module imports this one
+    return padded(x) if dh == 104 else x
+
+
+def as_f32(out, out_type):
+    """the kernel's output as float32 values: f32 as it is, fp16 or bf16 bit patterns widened"""
+    if out_type == 0:
+        return out
+    return out.view(np.float16).astype(np.float32) if out_type == 1 else (out.astype(np.uint32) << 16).view(np.float32)
+
+
+@pytest.mark.parametrize("T,causal,cls_row", [(T, c, 0) for T, c in LONG_FULL] + [(T, c, 1) for T, c in LONG_CLS])
+@pytest.mark.parametrize("dh", [64, 80, 104])
+@pytest.mark.parametrize("bf", [1, 0])
+def test_counting_every_element(prod, T, causal, cls_row, dh, bf):
+    rng = np.random.default_rng(T + dh + bf)
+    qkv = np.zeros((NSEQ_L * T, 3, H_L, dh), np.float32)
+    qkv[:, 1] = rng.standard_normal((NSEQ_L * T, H_L, dh))          # K does not matter: every score is 0 * k
+    qkv = qkv.reshape(NSEQ_L * T, -1)
+    rows = np.arange(1 if cls_row else T)
+    l = (rows + 1 if causal else np.full(len(rows), T)).astype(np.float32)
+    vis = np.arange(T)[None, :] <= rows[:, None] if causal else np.ones((1, T), bool)
+    want = np.where(vis, (np.float32(1) / l)[:, None], np.float32(0)).astype(np.float32)
+    for out_type in (0, 1, 2):
+        got = run(prod, qkv, bf, NSEQ_L, T, H_L, dh, causal, cls_row, out_type)
+        w = want.view(np.uint32) if out_type == 0 else rne16(want, out_type)
+        bad = got.view(w.dtype) != w[None, None]
+        if bad.any():
+            s, h, r, j = (int(x[0]) for x in np.nonzero(bad))
+            raise AssertionError("out_type %d: %d of %d entries off; first at sequence %d head %d row %d key %d: %r, want %r (l = %d)" %
+                                 (out_type, bad.sum(), bad.size, s, h, r, j, as_f32(got, out_type)[s, h, r, j],
+                                  as_f32(want if out_type == 0 else w, out_type)[r, j], l[r]))
+    print("T=%d causal=%d cls=%d dh=%d bf=%d: all %d entries exact in every output type" % (T, causal, cls_row, dh, bf, got.size))
+
+
+def pattern_qkv(T, dh, causal, bf, rng):
+    """qkv [NSEQ_L * T, 3 H_L dh] with one pattern of tests/_attention_bound.py per (sequence, head), exact in the operand type"""
+    slots = PATTERNS + ("random",)
+    qkv = np.zeros((NSEQ_L, T, 3, H_L, dh), np.float32)
+    for i, pattern in enumerate(slots):
+        q, k, _ = pattern_head(pattern, T, dh, causal, rng)
+        qkv[i // H_L, :, 0, i % H_L], qkv[i // H_L, :, 1, i % H_L] = round16(q, bf), round16(k, bf)
+    return slots, qkv
+
+
+@pytest.mark.parametrize("T,causal", LONG_FULL)
+@pytest.mark.parametrize("dh", [64, 80, 104])
+@pytest.mark.parametrize("bf", [1, 0])
+def test_long_maps_against_fp64(prod, T, causal, dh, bf):
+    rng = np.random.default_rng(5 * T + dh + bf)
+    slots, qkv = pattern_qkv(T, dh, causal, bf, rng)
+    flat = qkv.reshape(NSEQ_L * T, -1)
+    p32 = run(prod, flat, bf, NSEQ_L, T, H_L, dh, causal, 0, 0)
+    assert np.isfinite(p32).all()
+    rows = sampled_rows(T, causal, rng)
+    for i, pattern in enumerate(slots):
+        s, h = i // H_L, i % H_L
+        pi, bound = reference_probs(kernel_operand(qkv[s, :, 0, h], dh), kernel_operand(qkv[s, :, 1, h], dh), causal, bf, rows=rows)
+        r = exceed(p32[s, h, rows], pi, bound)
+        print("T=%d causal=%d dh=%d bf=%d %-11s %d rows  err/bound %.3f" % (T, causal, dh, bf, pattern, len(rows), r))
+        assert r <= 1.0, (pattern, r)
+    for out_type in (0, 1, 2):
+        full = p32 if out_type == 0 else run(prod, flat, bf, NSEQ_L, T, H_L, dh, causal, 0, out_type)
+        if out_type:
+            assert np.array_equal(full, rne16(p32, out_type)), out_type
+        cls = run(prod, flat, bf, NSEQ_L, T, H_L, dh, causal, 1, out_type)
+        assert np.array_equal(cls.view(np.uint8), np.ascontiguousarray(full[:, :, :1]).view(np.uint8)), out_type
+
+
+@pytest.mark.parametrize("T,causal", LONG_CLS)
+@pytest.mark.parametrize("dh", [64, 80, 104])
+@pytest.mark.parametrize("bf", [1, 0])
+def test_long_cls_row_against_fp64(prod, T, causal, dh, bf):
+    rng = np.random.default_rng(7 * T + dh + bf)
+    slots, qkv = pattern_qkv(T, dh, causal, bf, rng)
+    flat = qkv.reshape(NSEQ_L * T, -1)
+    cls32 = run(prod, flat, bf, NSEQ_L, T, H_L, dh, causal, 1, 0)
+    for out_type in (0, 1, 2):
+        cls = cls32 if out_type == 0 else run(prod, flat, bf, NSEQ_L, T, H_L, dh, causal, 1, out_type)
+        if out_type:
+            assert np.array_equal(cls, rne16(cls32, out_type)), out_type
+        for i, pattern in enumerate(slots):
+            s, h = i // H_L, i % H_L
+            pi, bound = reference_probs(kernel_operand(qkv[s, :, 0, h], dh), kernel_operand(qkv[s, :, 1, h], dh), causal, bf,
+                                        out_type, rows=[0])
+            r = exceed(as_f32(cls[s, h], out_type), pi, bound)
+            print("T=%d causal=%d dh=%d bf=%d out_type=%d %-11s CLS row  err/bound %.3f" % (T, causal, dh, bf, out_type, pattern, r))
+            assert r <= 1.0, (pattern, out_type, r)

@@ -1,6 +1,7 @@
 """K3 is persistent: each CTA strides over pairs of 64-row query groups numbered in (sequence, head, group) order, and a pair may
 straddle two heads.  Where an item lands in that schedule -- which CTA, which iteration, which warpgroup, paired with which other
-group, which ring stage -- must not change a single bit of its output.  Each case runs a batch, the same sequences in permuted
+group, which ring stage (two stages of 128-key blocks at head_dim 64 and 80, three of 64-key blocks at 104) -- must not change a
+single bit of its output.  Each case runs a batch, the same sequences in permuted
 order, and a few of them alone, compares the bytes, and checks the sequences run alone against the fp64 restatement at the bound of
 tests/test_gpu_attention.py."""
 import numpy as np
@@ -21,7 +22,7 @@ GROUPS = {"below": 40, "at": 2 * SMS, "above": 8 * SMS}
 
 @pytest.mark.parametrize("load", list(GROUPS))
 @pytest.mark.parametrize("T,causal", CASES)
-@pytest.mark.parametrize("dh", [64, 80])
+@pytest.mark.parametrize("dh", [64, 80, 104])
 @pytest.mark.parametrize("bf", [1, 0])
 def test_output_independent_of_schedule(prod, T, causal, dh, bf, load):
     ngrp = -(-T // 64)
