@@ -72,6 +72,7 @@ EXTENSION_SYMBOLS = [
     "clip_b200_mark", "clip_b200_mark_elapsed_ms",
     # scoring + multi-GPU (round 2)
     "clip_b200_topk_search", "clip_b200_rows_to_16bit", "clip_b200_topk_search_16", "clip_b200_rows_to_int8", "clip_b200_topk_search_i8",
+    "clip_b200_rows_to_binary", "clip_b200_topk_search_b1", "clip_b200_topk_rescore",
     "clip_b200_zero_shot_images", "clip_b200_dist_unique_id", "clip_b200_dist_init_with_id",
     "clip_b200_dist_init", "clip_b200_dist_rank", "clip_b200_dist_world", "clip_b200_device_count", "clip_b200_nccl_version", "clip_b200_cuda_device_count",
     "clip_b200_dist_barrier", "clip_b200_dist_max_f64", "clip_b200_dist_all_gather", "clip_b200_image_encode_device_all",
@@ -270,6 +271,12 @@ class ClipLib:
             L.clip_b200_rows_to_int8.argtypes = [vp, vp, C.c_size_t, ip, vp, vp]
             L.clip_b200_topk_search_i8.restype = C.c_bool
             L.clip_b200_topk_search_i8.argtypes = [vp, vp, vp, C.c_size_t, vp, vp, C.c_size_t, ip, ip, fp, ipp]
+            L.clip_b200_rows_to_binary.restype = C.c_bool
+            L.clip_b200_rows_to_binary.argtypes = [vp, vp, C.c_size_t, ip, vp, vp]
+            L.clip_b200_topk_search_b1.restype = C.c_bool
+            L.clip_b200_topk_search_b1.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, ip, ip, fp, ipp]
+            L.clip_b200_topk_rescore.restype = C.c_bool
+            L.clip_b200_topk_rescore.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, ip, ip, ipp, ip, ip, fp, ipp]
             L.clip_b200_zero_shot_images.restype = C.c_bool
             L.clip_b200_zero_shot_images.argtypes = [vp, ip, C.POINTER(clip_image_f32_batch), C.POINTER(clip_tokens), C.c_size_t,
                                                      C.c_bool, ip, fp, ipp]

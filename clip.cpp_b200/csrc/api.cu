@@ -87,7 +87,7 @@ struct Scope {
         }
     }
 };
-enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4, K_POS_RESAMPLE = 5, K_ATTN_PROBS = 6, K_KNN16 = 7, K_KNN_I8 = 8 };
+enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4, K_POS_RESAMPLE = 5, K_ATTN_PROBS = 6, K_KNN16 = 7, K_KNN_I8 = 8, K_KNN_B1 = 9, K_RESCORE = 10 };
 
 // ---- tensor lookup helpers ---------------------------------------------------------------------------------
 const GgufTensor* need(const GgufFile& g, const std::string& name) {
@@ -1581,42 +1581,52 @@ static bool ensure_cand(clip_ctx* c, size_t count) {
     return true;
 }
 
-// What one call of the search family reads, as its public form received it: the four searches and the two row forms that make
-// their databases.  Each form fills one and calls search_call, so every form checks its arguments in the same order
+// What one call of the search family reads, as its public form received it: the five searches, the rescore and the three row forms
+// that make their databases.  Each form fills one and calls search_call, so every form checks its arguments in the same order
 // (include/clip_b200.h), and the searches run the same pass driver.
 struct SearchCall {
-    enum Kind { SCORE, KNN16, KNN_I8, ROWS16, ROWS_I8 };
+    enum Kind { SCORE, KNN16, KNN_I8, KNN_B1, RESCORE, ROWS16, ROWS_I8, ROWS_B1 };
     const char* who;                              // the public name, for messages
     Kind kind;
     const void* q = nullptr;                      // queries [nq, dim]; a row form: its f32 source rows [nq, dim]
     const void* db = nullptr;                     // database rows [ndb, dim]; a row form: the rows it writes [nq, dim]
-    const void* xs = nullptr;                     // KNN_I8: database row scales [ndb]; ROWS_I8: the scales it writes [nq]
+    const void* xs = nullptr;                     // KNN_I8: database row scales [ndb]; ROWS_I8: the scales it writes [nq];
+                                                  // ROWS_B1: the centre [dim] or NULL
     const void* qs = nullptr;                     // KNN_I8: query scales [nq]
     size_t nq = 0, ndb = 0;                       // a row form: nq = n
     int dim = 0;                                  // SCORE: the model's projection_dim, set by search_call
-    int type = 0;                                 // KNN16: in_type; ROWS16: out_type
-    int top_k = 0;                                // SCORE: <= 0 or > ndb means all ndb; KNN: [1, 1024], > ndb means ndb
+    int type = 0;                                 // KNN16, RESCORE: in_type; ROWS16: out_type
+    const int* cand = nullptr;                    // RESCORE: host candidates [nq, n_cand]
+    int n_cand = 0;
+    int top_k = 0;                                // SCORE: <= 0 or > ndb means all ndb; KNN: [1, 1024], > ndb means ndb;
+                                                  // RESCORE: [1, n_cand], padded past the valid candidates
     bool softmax = false;                         // SCORE: rank p = (exp(s) + 1e-9) / sum over the row instead of s
     float* scores = nullptr;                      // host outputs [nq, that top_k]
     int* indices = nullptr;
-    bool search() const { return kind <= KNN_I8; }
+    bool search() const { return kind <= RESCORE; }
+    bool knn() const { return kind == KNN16 || kind == KNN_I8 || kind == KNN_B1; }
 };
 
-// The pass driver of the four searches, for a checked call with nq, ndb > 0.  Per block of QB queries: the candidates into
+// The pass driver of the searches and the rescore, for a checked call with nq, ndb > 0.  Per block of QB queries: the candidates into
 // d_cand_v/i[0] [rows, cand_ld] as `runs` sorted runs of kk, merge_candidates, the best k per row to the host, a synchronise.  Only
 // making the candidates differs: SCORE runs column chunks of CH rows through similarity [, softmax_with_sorting's p, clip.cpp:1591-1622]
-// and a top-k stage (a ranking above 1024 over more than one slice is made on the host instead); K10 is one launch per 32768 queries,
-// the merge grid's row limit.  Caller holds c->mu and has set the device.
+// and a top-k stage (a ranking above 1024 over more than one slice is made on the host instead); K10 and K11 are one launch per 32768
+// queries, the merge grid's row limit; K12 is one launch per block of queries whose candidates (copied from the host) fit 2^22 ints,
+// writing one sorted run of top_k.  Caller holds c->mu and has set the device.
 static bool search_locked(clip_ctx* c, const SearchCall& a) {
     const size_t nq = a.nq, ndb = a.ndb;
-    const int k = a.top_k <= 0 || (size_t)a.top_k > ndb ? (int)ndb : a.top_k;
+    const bool rescore = a.kind == SearchCall::RESCORE;
+    const int k = rescore ? a.top_k : a.top_k <= 0 || (size_t)a.top_k > ndb ? (int)ndb : a.top_k;
     const int SL = topk_slice(), kk = std::min(k, SL);
-    const bool knn = a.kind != SearchCall::SCORE, i8 = a.kind == SearchCall::KNN_I8;
+    const bool knn = a.knn(), i8 = a.kind == SearchCall::KNN_I8, b1 = a.kind == SearchCall::KNN_B1;
     size_t QB = 32768, CH = ndb, nsl = 0;
     bool device_select = true;
     int sms = 0;
     if (knn) {
         CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
+    } else if (rescore) {
+        QB = std::min<size_t>(32768, ((size_t)1 << 22) / a.n_cand);
+        if (!ensure_buf(c, &c->d_rcand, &c->d_rcand_cap, std::min(QB, nq) * a.n_cand) || !ensure_cand(c, std::min(QB, nq) * k)) return false;
     } else {
         const size_t budget = (size_t)32 << 20;                           // floats of similarity scratch per pass (128 MB)
         CH = std::min(ndb, std::max<size_t>(budget / std::min<size_t>(nq, 256), (size_t)SL));
@@ -1634,7 +1644,25 @@ static bool search_locked(clip_ctx* c, const SearchCall& a) {
     for (size_t r0 = 0; r0 < nq; r0 += QB) {
         const int rows = (int)std::min(QB, nq - r0);
         size_t runs = nsl, cand_ld = nsl * kk;
-        if (knn) {
+        if (rescore) {
+            runs = 1;
+            cand_ld = k;
+            CK(cudaMemcpyAsync(c->d_rcand, a.cand + r0 * a.n_cand, (size_t)rows * a.n_cand * 4, cudaMemcpyHostToDevice, c->stream));
+            const size_t q_row = (size_t)a.dim * (a.type == CLIP_B200_OUT_F32 ? 4 : 2);
+            Scope s(c, K_RESCORE);
+            const cudaError_t e = launch_rescore(a.type, (const uint8_t*)a.q + r0 * q_row, rows, a.db, (int)ndb, a.dim, c->d_rcand, a.n_cand, k,
+                                                 c->d_cand_v[0], c->d_cand_i[0], cand_ld, c->stream);
+            if (e != cudaSuccess) { set_err(std::string(a.who) + ": launch: " + cudaGetErrorString(e)); return false; }
+        } else if (b1) {
+            const KnnPlan pl = knn_b1_plan(rows, (int)ndb, k, sms);
+            runs = pl.parts;
+            cand_ld = (size_t)pl.parts * k;
+            if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * pl.buf_entries) || !ensure_cand(c, (size_t)rows * cand_ld)) return false;
+            Scope s(c, K_KNN_B1);
+            const cudaError_t e = launch_knn_b1((const uint8_t*)a.q + r0 * (a.dim / 8), rows, a.db, (int)ndb, a.dim, k, pl, c->d_knn,
+                                                c->d_cand_v[0], c->d_cand_i[0], cand_ld, c->stream);
+            if (e != cudaSuccess) { set_err(std::string(a.who) + ": launch: " + cudaGetErrorString(e)); return false; }
+        } else if (knn) {
             const KnnPlan pl = knn_plan(rows, (int)ndb, k, sms);
             runs = pl.parts;
             cand_ld = (size_t)pl.parts * k;
@@ -1696,27 +1724,36 @@ static bool search_call(const clip_ctx* cctx, SearchCall a) {
         set_err(who + (kind == SearchCall::KNN16 ? ": in_type" : ": out_type") + " must be CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16");
         return false;
     }
-    const int step = kind == SearchCall::KNN16 ? 8 : kind == SearchCall::ROWS16 ? 4 : 16;     // SCORE's dim is the model's
+    if (kind == SearchCall::RESCORE && a.type != CLIP_B200_OUT_F32 && a.type != CLIP_B200_OUT_F16 && a.type != CLIP_B200_OUT_BF16) {
+        set_err(who + ": in_type must be CLIP_B200_OUT_F32, CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16");
+        return false;
+    }
+    const int step = kind == SearchCall::KNN16 || kind == SearchCall::RESCORE ? 8 : kind == SearchCall::ROWS16 ? 4
+                   : kind == SearchCall::KNN_B1 || kind == SearchCall::ROWS_B1 ? 128 : 16;     // SCORE's dim is the model's
     if (kind != SearchCall::SCORE && (a.dim < step || a.dim > 2048 || a.dim % step)) {
         set_err(who + ": dim must be a multiple of " + std::to_string(step) + " in [" + std::to_string(step) + ", 2048]");
         return false;
     }
-    const bool knn = kind == SearchCall::KNN16 || kind == SearchCall::KNN_I8;
-    if (knn && (a.top_k < 1 || a.top_k > 1024)) { set_err(who + ": top_k must be in [1, 1024]"); return false; }
+    if (kind == SearchCall::RESCORE) {
+        if (a.n_cand < 1 || a.n_cand > 2048) { set_err(who + ": n_cand must be in [1, 2048]"); return false; }
+        if (a.top_k < 1 || a.top_k > a.n_cand) { set_err(who + ": top_k must be in [1, n_cand]"); return false; }
+    }
+    if (a.knn() && (a.top_k < 1 || a.top_k > 1024)) { set_err(who + ": top_k must be in [1, 1024]"); return false; }
     if (a.nq > 0x7fffffffull || a.ndb > 0x7fffffffull) {
         set_err(who + (a.search() ? ": n_queries and n_db must be below 2^31" : ": n must be below 2^31"));
         return false;
     }
     if (a.nq == 0 || (a.search() && a.ndb == 0)) return true;
-    // the device pointers the kind reads or writes: q and db, then the int8 forms' scales.  K10 and the row kernels load and store
-    // 16 bytes at a time; the fp32 kernels read single floats.
+    // the device pointers the kind reads or writes: q and db, then the int8 forms' scales or ROWS_B1's optional centre.  K10, K11, K12
+    // and the row kernels load and store 16 bytes at a time; the fp32 kernels read single floats.
     const void* ptr[4] = {a.q, a.db, a.xs, a.qs};
-    const int n_ptr = kind == SearchCall::KNN_I8 ? 4 : kind == SearchCall::ROWS_I8 ? 3 : 2;
+    const int n_ptr = kind == SearchCall::KNN_I8 ? 4 : kind == SearchCall::ROWS_I8 || kind == SearchCall::ROWS_B1 ? 3 : 2;
     for (int i = 0; i < n_ptr; i++)
-        if (!ptr[i] || (kind != SearchCall::SCORE && (uintptr_t)ptr[i] % 16)) {
+        if ((!ptr[i] && !(kind == SearchCall::ROWS_B1 && i == 2)) || (kind != SearchCall::SCORE && (uintptr_t)ptr[i] % 16)) {
             set_err(who + (kind == SearchCall::SCORE ? ": null device pointer" : ": null or not 16-byte aligned device pointer"));
             return false;
         }
+    if (kind == SearchCall::RESCORE && !a.cand) { set_err(who + ": null cand"); return false; }
     if (a.search() && (!a.scores || !a.indices)) { set_err(who + ": null output"); return false; }
     std::lock_guard<std::mutex> lk(c->mu);
     CK(cudaSetDevice(c->device));
@@ -1726,9 +1763,12 @@ static bool search_call(const clip_ctx* cctx, SearchCall a) {
         // K7 with one row per item, no CLS skip and no LayerNorm: an RNE copy.  Its offsets are size_t, so n * dim may pass 2^32.
         Scope s(c, K_TOKEN_ROWS);
         launch_token_rows((const float*)a.q, (size_t)a.dim, (int)a.nq, 1, 0, a.dim, nullptr, nullptr, 0.f, a.type, const_cast<void*>(a.db), c->stream);
-    } else {
+    } else if (kind == SearchCall::ROWS_I8) {
         Scope s(c, K_OTHER);
         launch_rows_to_int8((const float*)a.q, (int)a.nq, a.dim, const_cast<void*>(a.db), (float*)const_cast<void*>(a.xs), c->stream);
+    } else {
+        Scope s(c, K_OTHER);
+        launch_rows_to_binary((const float*)a.q, (int)a.nq, a.dim, (const float*)a.xs, const_cast<void*>(a.db), c->stream);
     }
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(c->stream));
@@ -1773,6 +1813,27 @@ bool clip_b200_topk_search_i8(const struct clip_ctx* cctx, const void* d_q_codes
                               const void* d_db_codes, const void* d_db_scales, size_t n_db, int dim, int top_k, float* scores, int* indices) {
     SearchCall a{"clip_b200_topk_search_i8", SearchCall::KNN_I8};
     a.q = d_q_codes; a.qs = d_q_scales; a.nq = n_queries; a.db = d_db_codes; a.xs = d_db_scales; a.ndb = n_db; a.dim = dim;
+    a.top_k = top_k; a.scores = scores; a.indices = indices;
+    return search_call(cctx, a);
+}
+
+bool clip_b200_rows_to_binary(const struct clip_ctx* cctx, const void* d_src, size_t n, int dim, const void* d_center, void* d_bits) {
+    SearchCall a{"clip_b200_rows_to_binary", SearchCall::ROWS_B1};
+    a.q = d_src; a.nq = n; a.dim = dim; a.xs = d_center; a.db = d_bits;
+    return search_call(cctx, a);
+}
+
+bool clip_b200_topk_search_b1(const struct clip_ctx* cctx, const void* d_q_bits, size_t n_queries, const void* d_db_bits, size_t n_db,
+                              int dim, int top_k, float* scores, int* indices) {
+    SearchCall a{"clip_b200_topk_search_b1", SearchCall::KNN_B1};
+    a.q = d_q_bits; a.nq = n_queries; a.db = d_db_bits; a.ndb = n_db; a.dim = dim; a.top_k = top_k; a.scores = scores; a.indices = indices;
+    return search_call(cctx, a);
+}
+
+bool clip_b200_topk_rescore(const struct clip_ctx* cctx, const void* d_queries, size_t n_queries, const void* d_db, size_t n_db, int dim,
+                            int in_type, const int* cand, int n_cand, int top_k, float* scores, int* indices) {
+    SearchCall a{"clip_b200_topk_rescore", SearchCall::RESCORE};
+    a.q = d_queries; a.nq = n_queries; a.db = d_db; a.ndb = n_db; a.dim = dim; a.type = in_type; a.cand = cand; a.n_cand = n_cand;
     a.top_k = top_k; a.scores = scores; a.indices = indices;
     return search_call(cctx, a);
 }

@@ -101,6 +101,21 @@ cudaError_t launch_knn(KOp op, const void* q, const float* qs, int nq, const voi
 // dim % 16 == 0, dim <= 2048, 16-byte aligned pointers; 64-bit offsets, so n * dim may pass 2^32.
 void launch_rows_to_int8(const float* x, int n, int dim, void* codes, float* scales, cudaStream_t st);
 
+// K11 Hamming top-k (search.cu): q [nq, dim / 8] and db [ndb, dim / 8] bytes of sign bits (clip_b200_rows_to_binary), 16-byte
+// aligned, dim % 128 == 0, dim <= 2048; score = dim - 2 popc(q ^ x), exact.  Output as launch_knn's; the plan is knn_plan's on one or
+// two CTAs an SM (knn_b1_plan).
+KnnPlan knn_b1_plan(int nq, int ndb, int kk, int sms);
+cudaError_t launch_knn_b1(const void* q, int nq, const void* db, int ndb, int dim, int kk, const KnnPlan& pl, void* buf, float* out_v,
+                          int* out_i, size_t out_ld, cudaStream_t st);
+// K12 rescore (search.cu): per query, the distinct candidates of cand [nq, n_cand] (device) in [0, ndb), scored by one fmaf chain over
+// q [nq, dim] x db [ndb, dim] of type (0 f32, 1 f16, 2 bf16), 16-byte aligned, dim % 8 == 0, dim <= 2048, n_cand <= 2048; the best
+// kk (<= n_cand) to out [nq, out_ld], sorted, padded with (-inf, -1).
+cudaError_t launch_rescore(int type, const void* q, int nq, const void* db, int ndb, int dim, const int* cand, int n_cand, int kk,
+                           float* out_v, int* out_i, size_t out_ld, cudaStream_t st);
+// B1 quantiser: x [n, dim] f32 (center [dim] f32 or NULL) -> bits [n, dim / 8], bit i = x_i > center_i, LSB first; dim % 128 == 0,
+// dim <= 2048, 16-byte aligned; 64-bit offsets.
+void launch_rows_to_binary(const float* x, int n, int dim, const float* center, void* bits, cudaStream_t st);
+
 }  // namespace cb
 struct clip_ctx;
 struct clip_image_u8;

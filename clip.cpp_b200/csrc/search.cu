@@ -11,6 +11,7 @@
 // tensor-core scores and a top-k kept inside the kernel, so no score matrix ever reaches memory.  It shares the candidate order and
 // the merge stage with the fp32 path.
 #include <cuda.h>
+#include <cuda_fp16.h>
 #include <float.h>
 #include <string.h>
 
@@ -190,6 +191,8 @@ struct KParams {
     size_t out_ld;
     int nq, ndb, nchunks, rows_per_part, parts, kk, cap;
     const float *qs, *xs;           // S8 only: query scales [nq], row scales [ndb]
+    const uint4 *qb, *xb;           // K11 only: query and database bits [nq, dim / 128], [ndb, dim / 128], 16-byte words
+    int dim;                        // K11 only: bits per row
 };
 
 template <KOp OP, int NT>
@@ -229,6 +232,42 @@ CB_DEVINL void knn_sort_keep(Cand* sc, Cand* b, int n, int kk, bool final, float
         if (t == 0) { *theta = sc[kk - 1].v; *cnt = kk; }
     }
     knn_bar();
+}
+
+// The selection steps K10 and K11 share, run by their 256 consumer threads.  knn_push: a score v of (query q, row) that passed the
+// kernel's admission test against theta[q] goes into q's buffer; a query whose buffer passed kk + KB entries is flagged.
+CB_DEVINL void knn_push(const KParams& p, Cand* bufq, float v, int q, int row, int* cnt, uint32_t* flags) {
+    const int pos = atomicAdd(&cnt[q], 1);
+    *reinterpret_cast<float2*>(bufq + (size_t)q * p.cap + pos) = make_float2(v, __int_as_float(row));
+    if (pos == p.kk + KB) atomicOr(&flags[q >> 5], 1u << (q & 31));
+}
+
+// After a tile: compact every flagged query's buffer to its best kk and raise its theta.
+template <int NQ>
+CB_DEVINL void knn_compact(const KParams& p, Cand* sort_s, Cand* bufq, float* theta, int* cnt, uint32_t* flags) {
+    knn_bar();
+    uint32_t fl[(NQ + 31) / 32];
+    bool any = false;
+    #pragma unroll
+    for (int w = 0; w < (NQ + 31) / 32; w++) { fl[w] = flags[w]; any |= fl[w] != 0; }
+    knn_bar();
+    if (any) {                                                 // block-uniform
+        if (threadIdx.x < 4) flags[threadIdx.x] = 0;
+        #pragma unroll
+        for (int w = 0; w < (NQ + 31) / 32; w++)
+            for (uint32_t f = fl[w]; f; f &= f - 1) {
+                const int q = 32 * w + __ffs(f) - 1;
+                knn_sort_keep(sort_s, bufq + (size_t)q * p.cap, cnt[q], p.kk, false, &theta[q], &cnt[q], nullptr, nullptr);
+            }
+    }
+}
+
+// After the partition: each of the tile's nqv queries' best kk to the candidate matrix at [q0 + q, part * kk].
+CB_DEVINL void knn_finish(const KParams& p, Cand* sort_s, Cand* bufq, const int* cnt, int nqv, int q0, int part) {
+    for (int q = 0; q < nqv; q++) {
+        const size_t o = (size_t)(q0 + q) * p.out_ld + (size_t)part * p.kk;
+        knn_sort_keep(sort_s, bufq + (size_t)q * p.cap, cnt[q], p.kk, true, nullptr, nullptr, p.out_v + o, p.out_i + o);
+    }
 }
 
 template <KOp OP, int NT>
@@ -325,32 +364,248 @@ __global__ void __launch_bounds__(KNN_THREADS, 1) knn_kernel(const __grid_consta
                 if constexpr (S8) v = __fmul_rn(__fmul_rn(__int2float_rn(d[4 * j + e]), qscale[q]), xs[e >> 1]);
                 else v = d[4 * j + e];
                 v = v != v ? -FLT_MAX : v;
-                if (q < nqv && row < row_end && v >= theta[q]) {
-                    const int pos = atomicAdd(&cnt[q], 1);
-                    *reinterpret_cast<float2*>(bufq + (size_t)q * p.cap + pos) = make_float2(v, __int_as_float(row));
-                    if (pos == p.kk + KB) atomicOr(&flags[q >> 5], 1u << (q & 31));
-                }
+                if (q < nqv && row < row_end && v >= theta[q]) knn_push(p, bufq, v, q, row, cnt, flags);   // ties kept
             }
         }
-        knn_bar();
-        uint32_t fl[(NQ + 31) / 32];
-        bool any = false;
+        knn_compact<NQ>(p, sort_s, bufq, theta, cnt, flags);
+    }
+    knn_finish(p, sort_s, bufq, cnt, nqv, q0, part);
+}
+
+// ---- K11: Hamming top-k over a binary database on the tensor cores --------------------------------------------------------------
+// Same work unit, plan, candidate buffers and selection as K10 (KParams, knn_push / knn_compact / knn_finish); 256 threads, eight
+// warps of 16 rows each, so a tile is the same KB = 128 rows.  No TMA: each thread loads its rows' bits straight into registers.
+//   bits      a row is W = dim / 128 16-byte words, taken in blocks of four words (64 bytes, two k256 steps), blocks past the row's
+//             last word zero.  Thread (g = lane / 4, t = lane % 4) holds word 4 b + t of block b of rows g and g + 8: x, y of that word
+//             feed k-step 2 b as A's slots t and t + 4, z, w feed k-step 2 b + 1.  The query tile sits in shared memory in the same
+//             word order, so B's registers for query n are the same two words of that query: the k order is a permutation of the
+//             bits, which a sum of popcounts does not see, and zero words add nothing.
+//   MMA       mma.sync m16n8k256 b1.and.popc: a = popc(q & x), exact int32.  Hopper has no b1 wgmma; .xor.popc is not one native
+//             instruction on sm_90a, .and.popc is (BMMA.168256.AND.POPC).
+//   score     s = dim - 2 popc(q) - 2 popc(x) + 4 a = dim - 2 popc(q ^ x), the dot product of the +-1 vectors, an exact integer
+//             float; popc(x) from the thread's registers summed over its four lanes, popc(q) staged once per CTA.
+//   ties      scores take at most dim + 1 values, so ties are the normal case.  Rows reach a CTA in increasing index, so once a
+//             query's buffer has been compacted to its best kk, a later row with s == theta ranks after all kk of them (equal score,
+//             higher index) and can never enter: after the first compaction the admission test is s > theta, exactly.  Before it
+//             theta is -inf, which every (finite) score passes.  With K10's s >= theta an all-equal database would compact every tile.
+constexpr int B1_THREADS = 256;
+
+template <int NT>
+struct B1Geo {
+    static constexpr int NQ = 8 * NT;
+    static constexpr uint32_t SORT_OFF = 0;                                   // Cand[KSORT]
+    static constexpr uint32_t THETA_OFF = SORT_OFF + KSORT * 8;               // float[128]
+    static constexpr uint32_t CNT_OFF = THETA_OFF + 128 * 4;                  // int[128]
+    static constexpr uint32_t PQ_OFF = CNT_OFF + 128 * 4;                     // int[128]: popc of each query
+    static constexpr uint32_t FLAG_OFF = PQ_OFF + 128 * 4;                    // uint32[4]
+    static constexpr uint32_t Q_OFF = FLAG_OFF + 16;                          // uint4[NQ][qstride]
+    // query row stride in 16-byte words: 4 per block, an odd number of blocks, so that rows g and g + 1 of one 8-thread phase of a
+    // 16-byte shared load fall in different halves of the 32 banks
+    __host__ __device__ static int qstride(int nblk) { return 4 * (nblk | 1); }
+    static uint32_t smem(int nblk) { return Q_OFF + (uint32_t)NQ * qstride(nblk) * 16; }
+};
+
+CB_DEVINL void bmma_and_popc(int (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+    asm("mma.sync.aligned.m16n8k256.row.col.s32.b1.b1.s32.and.popc {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+                 "{%0, %1, %2, %3};"
+                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+CB_DEVINL int popc4(const uint4& v) { return __popc(v.x) + __popc(v.y) + __popc(v.z) + __popc(v.w); }
+
+template <int NT>
+__global__ void __launch_bounds__(B1_THREADS, NT >= 8 ? 1 : 2) knn_b1_kernel(const __grid_constant__ KParams p) {
+    using G = B1Geo<NT>;
+    constexpr int NQ = G::NQ;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 15) & ~(uintptr_t)15);
+    Cand* sort_s = reinterpret_cast<Cand*>(smem + G::SORT_OFF);
+    float* theta = reinterpret_cast<float*>(smem + G::THETA_OFF);
+    int* cnt = reinterpret_cast<int*>(smem + G::CNT_OFF);
+    int* pq = reinterpret_cast<int*>(smem + G::PQ_OFF);
+    uint32_t* flags = reinterpret_cast<uint32_t*>(smem + G::FLAG_OFF);
+    uint4* sq = reinterpret_cast<uint4*>(smem + G::Q_OFF);
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, tg = lane & 3;
+    const int qt = blockIdx.x / p.parts, part = blockIdx.x - qt * p.parts;
+    const int q0 = qt * NQ, nqv = min(NQ, p.nq - q0);
+    const int row_begin = part * p.rows_per_part, row_end = min(p.ndb, row_begin + p.rows_per_part);
+    const int ntiles = (row_end - row_begin + KB - 1) / KB;
+    const int W = p.dim / 128, nblk = (W + 3) / 4, qs = G::qstride(nblk);
+
+    if (threadIdx.x < 128) { theta[threadIdx.x] = -INFINITY; cnt[threadIdx.x] = 0; }
+    if (threadIdx.x < 4) flags[threadIdx.x] = 0;
+    for (int e = threadIdx.x; e < NQ * qs; e += B1_THREADS) {
+        const int q = e / qs, w = e - q * qs;
+        sq[e] = q < nqv && w < W ? p.qb[(size_t)(q0 + q) * W + w] : make_uint4(0, 0, 0, 0);
+    }
+    __syncthreads();
+    if (threadIdx.x < NQ) {
+        int s = 0;
+        for (int w = 0; w < W; w++) s += popc4(sq[threadIdx.x * qs + w]);
+        pq[threadIdx.x] = s;
+    }
+    __syncthreads();
+
+    Cand* const bufq = p.buf + (size_t)blockIdx.x * NQ * p.cap;
+    for (int t = 0; t < ntiles; t++) {
+        const int row0 = row_begin + t * KB + warp * 16 + g;           // this thread: rows row0 and row0 + 8
+        uint4 a[2][4];
         #pragma unroll
-        for (int w = 0; w < (NQ + 31) / 32; w++) { fl[w] = flags[w]; any |= fl[w] != 0; }
-        knn_bar();
-        if (any) {                                                 // block-uniform
-            if (threadIdx.x < 4) flags[threadIdx.x] = 0;
+        for (int h = 0; h < 2; h++)
             #pragma unroll
-            for (int w = 0; w < (NQ + 31) / 32; w++)
-                for (uint32_t f = fl[w]; f; f &= f - 1) {
-                    const int q = 32 * w + __ffs(f) - 1;
-                    knn_sort_keep(sort_s, bufq + (size_t)q * p.cap, cnt[q], p.kk, false, &theta[q], &cnt[q], nullptr, nullptr);
-                }
+            for (int b = 0; b < 4; b++) {
+                const int w = 4 * b + tg, r = row0 + 8 * h;
+                a[h][b] = b < nblk && w < W && r < row_end ? p.xb[(size_t)r * W + w] : make_uint4(0, 0, 0, 0);
+            }
+        int px[2];
+        #pragma unroll
+        for (int h = 0; h < 2; h++) {
+            px[h] = popc4(a[h][0]) + popc4(a[h][1]) + popc4(a[h][2]) + popc4(a[h][3]);
+            px[h] += __shfl_xor_sync(0xffffffffu, px[h], 1);
+            px[h] += __shfl_xor_sync(0xffffffffu, px[h], 2);
+        }
+        int d[NT][4];
+        #pragma unroll
+        for (int j = 0; j < NT; j++) d[j][0] = d[j][1] = d[j][2] = d[j][3] = 0;
+        #pragma unroll
+        for (int b = 0; b < 4; b++) {
+            if (b >= nblk) break;
+            #pragma unroll
+            for (int j = 0; j < NT; j++) {
+                const uint4 bq = sq[(8 * j + g) * qs + 4 * b + tg];
+                bmma_and_popc(d[j], a[0][b].x, a[1][b].x, a[0][b].y, a[1][b].y, bq.x, bq.y);
+                bmma_and_popc(d[j], a[0][b].z, a[1][b].z, a[0][b].w, a[1][b].w, bq.z, bq.w);
+            }
+        }
+        // candidates of this tile (accumulator layout: d[j][e] is row row0 + 8 (e >> 1), query 8 j + 2 tg + (e & 1))
+        #pragma unroll
+        for (int j = 0; j < NT; j++) {
+            #pragma unroll
+            for (int e = 0; e < 4; e++) {
+                const int q = 8 * j + 2 * tg + (e & 1), row = row0 + 8 * (e >> 1);
+                const float v = (float)(p.dim - 2 * pq[q] - 2 * px[e >> 1] + 4 * d[j][e]);
+                if (q < nqv && row < row_end && v > theta[q]) knn_push(p, bufq, v, q, row, cnt, flags);     // strict: see above
+            }
+        }
+        knn_compact<NQ>(p, sort_s, bufq, theta, cnt, flags);
+    }
+    knn_finish(p, sort_s, bufq, cnt, nqv, q0, part);
+}
+
+// ---- K12: exact rescoring of a candidate list --------------------------------------------------------------------------------------
+// One CTA per query: the query, widened to f32, in shared memory; the candidates sorted by index (bitonic_sort with equal values) so
+// that out-of-range entries (index INT_MAX after staging) go last and duplicates sit side by side, the first of each run kept; each
+// thread walks its candidates' rows with 16-byte loads, one fmaf chain per row from +0 over features 0 .. dim - 1 (sim_kernel's
+// order); then the family's order and the best kk.  A dropped entry is (-inf, INT_MAX) in the sort, after every valid candidate
+// (a valid -inf score has a lower index), and (-inf, -1) in the output.
+constexpr int RS_MAX = 2048, RS_PER = RS_MAX / 256;
+
+template <int T>   // element type: 0 f32, 1 f16, 2 bf16 (CLIP_B200_OUT_*)
+CB_DEVINL void widen8(const uint4& u, float (&f)[8]) {
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+    #pragma unroll
+    for (int i = 0; i < 4; i++) {
+        if constexpr (T == 1) {
+            const float2 h = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
+            f[2 * i] = h.x; f[2 * i + 1] = h.y;
+        } else {
+            f[2 * i] = __uint_as_float(w[i] << 16); f[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u);
         }
     }
-    for (int q = 0; q < nqv; q++) {
-        const size_t o = (size_t)(q0 + q) * p.out_ld + (size_t)part * p.kk;
-        knn_sort_keep(sort_s, bufq + (size_t)q * p.cap, cnt[q], p.kk, true, nullptr, nullptr, p.out_v + o, p.out_i + o);
+}
+
+template <int T>
+__global__ void __launch_bounds__(256) rescore_kernel(const void* __restrict__ q, const void* __restrict__ db, int ndb, int dim,
+                                                      const int* __restrict__ cand, int n_cand, int kk, float* __restrict__ out_v,
+                                                      int* __restrict__ out_i, size_t out_ld) {
+    __shared__ Cand c[RS_MAX];
+    __shared__ __align__(16) float sq[2048];
+    constexpr int ESZ = T == 0 ? 4 : 2, EPV = 16 / ESZ;             // element bytes, elements per 16-byte load
+    const int row = blockIdx.x;
+    const size_t rbytes = (size_t)dim * ESZ;
+    const uint4* qr = reinterpret_cast<const uint4*>(static_cast<const uint8_t*>(q) + row * rbytes);
+    for (int e = threadIdx.x; e < dim / EPV; e += 256) {
+        const uint4 u = qr[e];
+        if constexpr (T == 0) *reinterpret_cast<uint4*>(sq + 4 * e) = u;
+        else {
+            float f[8];
+            widen8<T>(u, f);
+            #pragma unroll
+            for (int i = 0; i < 8; i++) sq[8 * e + i] = f[i];
+        }
+    }
+    int m = 1;
+    while (m < n_cand) m <<= 1;
+    const int* cr = cand + (size_t)row * n_cand;
+    for (int e = threadIdx.x; e < m; e += 256) {
+        const int i = e < n_cand ? cr[e] : -1;
+        c[e] = Cand{0.f, i >= 0 && i < ndb ? i : 0x7fffffff};
+    }
+    __syncthreads();
+    bitonic_sort<false>(c, m);
+    Cand mine[RS_PER];
+    #pragma unroll
+    for (int u = 0; u < RS_PER; u++) {
+        const int e = threadIdx.x + 256 * u;
+        Cand x{-INFINITY, 0x7fffffff};
+        if (e < m) {
+            const int i = c[e].i;
+            if (i != 0x7fffffff && (e == 0 || c[e - 1].i != i)) {
+                const uint4* xr = reinterpret_cast<const uint4*>(static_cast<const uint8_t*>(db) + (size_t)i * rbytes);
+                float acc = 0.f;
+                #pragma unroll 4
+                for (int k = 0; k < dim / EPV; k++) {
+                    const uint4 v = xr[k];
+                    if constexpr (T == 0) {
+                        acc = fmaf(sq[4 * k], __uint_as_float(v.x), acc);
+                        acc = fmaf(sq[4 * k + 1], __uint_as_float(v.y), acc);
+                        acc = fmaf(sq[4 * k + 2], __uint_as_float(v.z), acc);
+                        acc = fmaf(sq[4 * k + 3], __uint_as_float(v.w), acc);
+                    } else {
+                        float f[8];
+                        widen8<T>(v, f);
+                        #pragma unroll
+                        for (int j = 0; j < 8; j++) acc = fmaf(sq[8 * k + j], f[j], acc);
+                    }
+                }
+                x = Cand{acc != acc ? -FLT_MAX : acc, i};
+            }
+        }
+        mine[u] = x;
+    }
+    __syncthreads();
+    #pragma unroll
+    for (int u = 0; u < RS_PER; u++)
+        if (threadIdx.x + 256 * u < m) c[threadIdx.x + 256 * u] = mine[u];
+    __syncthreads();
+    bitonic_sort<false>(c, m);
+    for (int e = threadIdx.x; e < kk; e += 256) {
+        const Cand x = e < m ? c[e] : Cand{-INFINITY, 0x7fffffff};
+        out_v[(size_t)row * out_ld + e] = x.i == 0x7fffffff ? -INFINITY : x.v;
+        out_i[(size_t)row * out_ld + e] = x.i == 0x7fffffff ? -1 : x.i;
+    }
+}
+
+// B1 quantiser: one warp per 128 features, which is one 16-byte output word: the rows are whole words, so word w of the flat
+// [n * dim / 128] array reads floats 128 w .. 128 w + 127 and centre features 128 (w % (dim / 128)) + ...  Lane l compares its
+// float4 (features 4 l .. 4 l + 3) with the centre, IEEE > with nothing flushed (the build has no -ftz), four bits LSB first; eight
+// lanes OR their nibbles into a 32-bit word and lane 0 stores the four words.
+__global__ void __launch_bounds__(256) quant_b1_kernel(const float4* __restrict__ x, size_t nwords, int wpr, const float4* __restrict__ center,
+                                                       uint4* __restrict__ bits) {
+    const int lane = threadIdx.x & 31;
+    const size_t step = (size_t)gridDim.x * 8;
+    for (size_t w = (size_t)blockIdx.x * 8 + (threadIdx.x >> 5); w < nwords; w += step) {
+        const float4 v = x[w * 32 + lane];
+        const float4 c = center ? center[(w % wpr) * 32 + lane] : make_float4(0.f, 0.f, 0.f, 0.f);
+        uint32_t nib = (v.x > c.x ? 1u : 0u) | (v.y > c.y ? 2u : 0u) | (v.z > c.z ? 4u : 0u) | (v.w > c.w ? 8u : 0u);
+        nib <<= 4 * (lane & 7);
+        nib |= __shfl_xor_sync(0xffffffffu, nib, 1);
+        nib |= __shfl_xor_sync(0xffffffffu, nib, 2);
+        nib |= __shfl_xor_sync(0xffffffffu, nib, 4);
+        const uint32_t w1 = __shfl_sync(0xffffffffu, nib, 8), w2 = __shfl_sync(0xffffffffu, nib, 16), w3 = __shfl_sync(0xffffffffu, nib, 24);
+        if (lane == 0) bits[w] = make_uint4(nib, w1, w2, w3);
     }
 }
 
@@ -507,6 +762,58 @@ cudaError_t launch_knn(KOp op, const void* q, const float* qs, int nq, const voi
 void launch_rows_to_int8(const float* x, int n, int dim, void* codes, float* scales, cudaStream_t st) {
     if (n <= 0) return;
     quant_i8_kernel<<<(n + 7) / 8, 256, 0, st>>>(x, n, dim, reinterpret_cast<int8_t*>(codes), scales);
+}
+
+KnnPlan knn_b1_plan(int nq, int ndb, int kk, int sms) {
+    const KnnPlan pl = knn_plan(nq, ndb, kk, sms);
+    return pl.nt < 8 ? knn_plan(nq, ndb, kk, 2 * sms) : pl;          // below 64-query tiles K11 runs two CTAs an SM
+}
+
+template <int NT>
+static cudaError_t knn_b1_launch(const KParams& p, unsigned grid, cudaStream_t st) {
+    const uint32_t smem = B1Geo<NT>::smem((p.dim / 128 + 3) / 4) + 16;
+    cudaError_t e = cudaFuncSetAttribute(knn_b1_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    knn_b1_kernel<NT><<<grid, B1_THREADS, smem, st>>>(p);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_knn_b1(const void* q, int nq, const void* db, int ndb, int dim, int kk, const KnnPlan& pl, void* buf, float* out_v,
+                          int* out_i, size_t out_ld, cudaStream_t st) {
+    if (nq <= 0 || ndb <= 0) return cudaSuccess;
+    KParams p;
+    memset(&p, 0, sizeof(p));
+    p.qb = reinterpret_cast<const uint4*>(q); p.xb = reinterpret_cast<const uint4*>(db); p.dim = dim;
+    p.buf = reinterpret_cast<Cand*>(buf);
+    p.out_v = out_v; p.out_i = out_i; p.out_ld = out_ld;
+    p.nq = nq; p.ndb = ndb;
+    p.rows_per_part = pl.rows_per_part; p.parts = pl.parts; p.kk = kk; p.cap = pl.cap;
+    switch (pl.nt) {
+        case 1: return knn_b1_launch<1>(p, (unsigned)pl.grid, st);
+        case 2: return knn_b1_launch<2>(p, (unsigned)pl.grid, st);
+        case 4: return knn_b1_launch<4>(p, (unsigned)pl.grid, st);
+        case 8: return knn_b1_launch<8>(p, (unsigned)pl.grid, st);
+        default: return knn_b1_launch<16>(p, (unsigned)pl.grid, st);
+    }
+}
+
+cudaError_t launch_rescore(int type, const void* q, int nq, const void* db, int ndb, int dim, const int* cand, int n_cand, int kk,
+                           float* out_v, int* out_i, size_t out_ld, cudaStream_t st) {
+    if (nq <= 0) return cudaSuccess;
+    switch (type) {
+        case 0: rescore_kernel<0><<<nq, 256, 0, st>>>(q, db, ndb, dim, cand, n_cand, kk, out_v, out_i, out_ld); break;
+        case 1: rescore_kernel<1><<<nq, 256, 0, st>>>(q, db, ndb, dim, cand, n_cand, kk, out_v, out_i, out_ld); break;
+        default: rescore_kernel<2><<<nq, 256, 0, st>>>(q, db, ndb, dim, cand, n_cand, kk, out_v, out_i, out_ld); break;
+    }
+    return cudaGetLastError();
+}
+
+void launch_rows_to_binary(const float* x, int n, int dim, const float* center, void* bits, cudaStream_t st) {
+    if (n <= 0) return;
+    const size_t nwords = (size_t)n * (dim / 128);
+    const unsigned grid = (unsigned)std::min<size_t>((nwords + 7) / 8, (size_t)1 << 20);
+    quant_b1_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const float4*>(x), nwords, dim / 128, reinterpret_cast<const float4*>(center),
+                                          reinterpret_cast<uint4*>(bits));
 }
 
 }  // namespace cb

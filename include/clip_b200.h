@@ -377,6 +377,59 @@ bool clip_b200_topk_search_i8(const struct clip_ctx * ctx, const void * d_q_code
                               const void * d_db_codes, const void * d_db_scales, size_t n_db, int dim, int top_k,
                               float * scores, int * indices);
 
+/* f32 rows -> binary rows (one sign bit per feature, as USearch b1 and FAISS binary indexes store them), device to device: how a
+ * database or query set is made for clip_b200_topk_search_b1.  A 768-d row takes 96 bytes.
+ * - d_src [n, dim] f32, d_center [dim] f32 or NULL (all zeros), d_bits [n, dim / 8] uint8, row-major, on the context's GPU,
+ *   16-byte aligned.  dim is a multiple of 128 in [128, 2048], so a row is whole 16-byte words; n < 2^31 (n * dim may exceed 2^32).
+ * - The rule, exactly: bit i is 1 iff x_i > c_i, an IEEE compare with nothing flushed to zero: a NaN gives 0, so does -0 against 0,
+ *   and a subnormal above 0 gives 1.  Feature i goes to byte i / 8, bit i % 8, least significant bit first
+ *   (numpy.packbits(bits, axis=1, bitorder="little")).
+ * - The centre: CLIP embeddings share a common mean direction, so the signs of raw coordinates spend bits on it.  Passing the
+ *   database's mean (of a sample) as d_center is the usual fix.
+ * - Refusals, with a message in clip_b200_last_error, in this order: null context; dim; n >= 2^31; then, when n > 0 (n == 0
+ *   returns true), null or misaligned d_src / d_bits, or a misaligned non-NULL d_center.  Returns once the rows are written.  Its
+ *   time is kernel class 3. */
+bool clip_b200_rows_to_binary(const struct clip_ctx * ctx, const void * d_src, size_t n, int dim, const void * d_center,
+                              void * d_bits);
+
+/* Nearest-neighbour search over a binary database (clip_b200_rows_to_binary's form) on the tensor cores (kernel K11): K10's plan,
+ * candidate buffers and merge, with 1-bit tensor-core products (mma m16n8k256 b1, AND + popcount).
+ * - Inputs: d_q_bits [n_queries, dim / 8] and d_db_bits [n_db, dim / 8], as clip_b200_rows_to_binary writes them, on the context's
+ *   GPU, 16-byte aligned.  dim is a multiple of 128 in [128, 2048].
+ * - Scores, exactly: s = dim - 2 popcount(q XOR x), the dot product of the +-1 vectors (bit 1 is +1): an integer in [-dim, dim],
+ *   returned as an exact float.  No NaN can occur.  A score depends only on the query's and the row's bits.
+ * - Ranking: the best top_k of all n_db scores, score descending, then lower index first, host [n_queries, top_k], row i at
+ *   i * top_k.  Scores take at most dim + 1 values, so ties are common; the index order settles them.
+ * - top_k must be in [1, 1024]; a value above n_db means n_db.
+ * - Refusals, with a message in clip_b200_last_error, in this order: null context; dim; top_k; n_queries or n_db >= 2^31; then,
+ *   when there is work (n_queries == 0 or n_db == 0 returns true and writes nothing), null or misaligned device pointers and
+ *   null outputs.
+ * - Runs on the context's first GPU (in devices mode too); the database is not sharded.  Queries go in launches of up to 32768.
+ * - Workspace: clip_b200_topk_search_16's formula, in the same grow-only buffers, except that with a query tile below 64 the plan
+ *   takes G <= 2 x #SMs CTAs.  Its kernel time is kernel class 9. */
+bool clip_b200_topk_search_b1(const struct clip_ctx * ctx, const void * d_q_bits, size_t n_queries, const void * d_db_bits,
+                              size_t n_db, int dim, int top_k, float * scores, int * indices);
+
+/* Exact rescoring of a shortlist (kernel K12), as FAISS IndexRefine and "binary + rescore" pipelines do it: per query, the
+ * candidates a cheaper search returned are scored again against full-precision rows and the best top_k kept.
+ * - Inputs: in_type is CLIP_B200_OUT_F32, CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16, for both d_queries [n_queries, dim] and d_db
+ *   [n_db, dim], row-major, on the context's GPU, 16-byte aligned.  dim is a multiple of 8 in [8, 2048].  cand is HOST memory
+ *   [n_queries, n_cand] int32, for example exactly what a search form wrote into its indices.  n_cand is in [1, 2048].
+ * - Scores, exactly: one sequential fmaf chain from +0 over features 0 .. dim - 1; 16-bit values are widened to f32 first (exact).
+ *   In F32 this is clip_b200_topk_search's chain, so every score has the same bits as that search's score for the pair.  With
+ *   16-bit rows each product is exact in f32 and only the sums round.  A NaN score ranks last among the valid candidates and is
+ *   reported as -FLT_MAX.
+ * - Candidates are a set: entries outside [0, n_db) (-1, INT_MAX, ...) are skipped and a duplicate counts once.  The best top_k
+ *   (top_k in [1, n_cand]) of the distinct valid candidates go to host [n_queries, top_k], score descending, then lower index
+ *   first; if fewer remain, the rest of the row is (-INFINITY, -1).
+ * - Refusals, with a message in clip_b200_last_error, in this order: null context; in_type; dim; n_cand; top_k; n_queries or n_db
+ *   >= 2^31; then, when there is work (n_queries == 0 or n_db == 0 returns true and writes nothing), null or misaligned device
+ *   pointers, null cand, null outputs.
+ * - Runs on the context's first GPU.  Workspace, grow-only: a device copy of the candidates of up to min(32768, 2^22 / n_cand)
+ *   queries at a time, and the merge buffers of clip_b200_topk_search.  Its kernel time is kernel class 10. */
+bool clip_b200_topk_rescore(const struct clip_ctx * ctx, const void * d_queries, size_t n_queries, const void * d_db, size_t n_db,
+                            int dim, int in_type, const int * cand, int n_cand, int top_k, float * scores, int * indices);
+
 /* Batched zero-shot labelling, the batch form of clip_zero_shot_label_image (clip.h:106-107, clip.cpp:1624-1659): n images x
  * n_labels token sequences -> scores / indices [n, top_k], best first (p = (exp(s)+1e-9)/sum over ALL labels, clip.cpp:1591-1622).
  * normalize = false reproduces the reference (un-normalised embeddings).  Works in every multi-GPU mode (see below): in devices
@@ -441,7 +494,8 @@ float    clip_b200_last_device_ms(const struct clip_ctx * ctx);    /* CUDA-event
 /* per-kernel-class CUDA-event time accumulated since the last call with the same kind (0 GEMM, 1 attention,
  * 2 layernorm, 3 other, 4 the token-row kernel of the *_tokens calls, 5 the position-table resample of the *_hw calls, 6 the
  * attention-probability kernel of ATTENTION entries, 7 the 16-bit search kernel of clip_b200_topk_search_16, 8 the int8 search
- * kernel of clip_b200_topk_search_i8); *count
+ * kernel of clip_b200_topk_search_i8, 9 the binary search kernel of clip_b200_topk_search_b1, 10 the rescore kernel of
+ * clip_b200_topk_rescore); *count
  * receives the number of launches.  Enabled by env CLIP_B200_PROFILE=1. */
 float    clip_b200_kernel_ms(const struct clip_ctx * ctx, int kind, uint64_t * count);
 /* CUDA-event stopwatch on the launch stream: mark(slot 0..3), then elapsed(a, b) in ms (-1 on error) */
