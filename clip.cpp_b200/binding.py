@@ -94,6 +94,9 @@ EXTENSION_SYMBOLS = [
     "clip_b200_debug_attention_probs",
     # head_dim 104 (ViT-bigG/14): the loader's QKV row padding
     "clip_b200_debug_pad_qkv",
+    # images of different sizes in one call (variable-length attention)
+    "clip_b200_image_batch_encode_mixed", "clip_b200_image_encode_device_mixed", "clip_b200_image_tokens_mixed",
+    "clip_b200_image_tokens_device_mixed", "clip_b200_debug_attention_mixed",
 ]
 
 # include/clip_b200.h: output types and flags of the *_tokens entry points
@@ -216,6 +219,8 @@ class ClipLib:
             L.clip_b200_debug_attention.argtypes = [ip, ip, ip, ip, ip, ip, fp, fp, C.POINTER(C.c_float)]
             L.clip_b200_debug_attention_hd.restype = C.c_int
             L.clip_b200_debug_attention_hd.argtypes = [ip, ip, ip, ip, ip, ip, ip, fp, fp, C.POINTER(C.c_float)]
+            L.clip_b200_debug_attention_mixed.restype = C.c_int
+            L.clip_b200_debug_attention_mixed.argtypes = [ip, ip, C.POINTER(C.c_int), ip, ip, fp, fp]
             L.clip_b200_debug_attention_probs.restype = C.c_int
             L.clip_b200_debug_attention_probs.argtypes = [ip, ip, ip, ip, ip, ip, ip, ip, fp, vp]
             L.clip_b200_debug_gemm.restype = C.c_int
@@ -252,6 +257,14 @@ class ClipLib:
             L.clip_b200_image_tokens_hw.restype = C.c_bool
             L.clip_b200_image_tokens_hw.argtypes = [vp, C.POINTER(clip_image_f32_batch), ip, ip, ip, vp]
             intp = C.POINTER(C.c_int)
+            L.clip_b200_image_batch_encode_mixed.restype = C.c_bool
+            L.clip_b200_image_batch_encode_mixed.argtypes = [vp, C.POINTER(clip_image_f32_batch), fp, C.c_bool]
+            L.clip_b200_image_encode_device_mixed.restype = C.c_bool
+            L.clip_b200_image_encode_device_mixed.argtypes = [vp, vp, C.c_size_t, intp, intp, vp, C.c_bool]
+            L.clip_b200_image_tokens_mixed.restype = C.c_bool
+            L.clip_b200_image_tokens_mixed.argtypes = [vp, C.POINTER(clip_image_f32_batch), ip, ip, ip, vp]
+            L.clip_b200_image_tokens_device_mixed.restype = C.c_bool
+            L.clip_b200_image_tokens_device_mixed.argtypes = [vp, vp, C.c_size_t, intp, intp, ip, ip, ip, vp]
             L.clip_b200_image_tokens_layers.restype = C.c_bool
             L.clip_b200_image_tokens_layers.argtypes = [vp, C.POINTER(clip_image_f32_batch), intp, intp, ip, ip, vp]
             L.clip_b200_image_tokens_layers_device.restype = C.c_bool
@@ -441,6 +454,41 @@ class ClipLib:
         if not self.lib.clip_b200_image_tokens_hw(ctx, C.byref(batch), layer, flags, out_type, out.ctypes.data):
             raise RuntimeError("clip_b200_image_tokens_hw failed: " + self.last_error())
         return out
+
+    # ---- images of different sizes in one call (include/clip_b200.h: *_mixed) -------------------------------------------------
+    @staticmethod
+    def make_mixed_batch(images):
+        """images: a list of [H_i, W_i, 3] float32 C-contiguous arrays -> (batch struct, keep-alive tuple)"""
+        arr = (clip_image_f32 * len(images))()
+        for i, im in enumerate(images):
+            assert im.dtype == np.float32 and im.flags["C_CONTIGUOUS"] and im.ndim == 3
+            arr[i].ny, arr[i].nx, arr[i].size = im.shape[0], im.shape[1], im.size
+            arr[i].data = C.cast(im.ctypes.data, C.POINTER(C.c_float))
+        return clip_image_f32_batch(arr, len(images)), (arr, images)
+
+    def mixed_token_rows(self, ctx, sizes, flags: int) -> list:
+        """rows per image of a *_tokens_mixed call: (H / P) * (W / P) + 1, less one with NO_CLS"""
+        P = self.vision_hparams(ctx).patch_size
+        return [(h // P) * (w // P) + 1 - (1 if flags & TOKENS_NO_CLS else 0) for h, w in sizes]
+
+    def image_batch_encode_mixed(self, ctx, images, normalize=True) -> np.ndarray:
+        """images: a list of [H_i, W_i, 3] float32 arrays, each its own patch-multiple size -> [n, projection_dim]"""
+        batch, keep = self.make_mixed_batch(images)
+        out = np.empty((len(images), self.vision_hparams(ctx).projection_dim), np.float32)
+        if not self.lib.clip_b200_image_batch_encode_mixed(ctx, C.byref(batch), out.ctypes.data_as(C.POINTER(C.c_float)), normalize):
+            raise RuntimeError("clip_b200_image_batch_encode_mixed failed: " + self.last_error())
+        return out
+
+    def image_tokens_mixed(self, ctx, images, layer: int = -1, flags: int = 0, out_type: int = OUT_F32) -> list:
+        """images: a list of [H_i, W_i, 3] float32 arrays -> a list of [T_i or T_i - 1, width] arrays (views of one ragged buffer)"""
+        batch, keep = self.make_mixed_batch(images)
+        hp = self.vision_hparams(ctx)
+        width = hp.projection_dim if flags & TOKENS_PROJECT else hp.hidden_size
+        rows = self.mixed_token_rows(ctx, [im.shape[:2] for im in images], flags)
+        flat = np.empty((sum(rows), width), OUT_DTYPES.get(out_type, np.float32))
+        if not self.lib.clip_b200_image_tokens_mixed(ctx, C.byref(batch), layer, flags, out_type, flat.ctypes.data):
+            raise RuntimeError("clip_b200_image_tokens_mixed failed: " + self.last_error())
+        return np.split(flat, np.cumsum(rows)[:-1])
 
     def text_tokens(self, ctx, ids: np.ndarray, layer: int = -1, flags: int = 0, out_type: int = OUT_F32) -> np.ndarray:
         """ids [n, seq_len] int32, padded by the caller -> [n, seq_len, width] of OUT_DTYPES[out_type]"""

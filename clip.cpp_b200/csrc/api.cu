@@ -10,6 +10,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <map>
 #include <memory>
 #include <numeric>
 #include <thread>
@@ -311,13 +312,20 @@ bool run_linear(clip_ctx* c, const Linear& L, const TmaMap* xmap, const void* xp
     return true;
 }
 
+// A mixed-size pass (the *_mixed calls): nseq sequences of different lengths packed back to back in `rows` rows; d_seq is K3's
+// varlen table on the device (launch_attention_tc_varlen), groups its 64-row groups per head.
+struct Packed {
+    int rows = 0, nseq = 0, groups = 0;
+    const int* d_seq = nullptr;
+};
+
 // The per-layer schedule shared by both towers (clip.cpp:1064-1143 text, 1342-1423 vision): blocks first .. end-1 on ws.x (a
-// multi-layer tokens call resumes where its previous stop left x).
-bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal, int first, int end) {
+// multi-layer tokens call resumes where its previous stop left x).  pk: a packed mixed-size pass instead of nseq x T rows.
+bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal, int first, int end, const Packed* pk = nullptr) {
     // The residual stream x stays fp32 (as in the reference).  The branch GEMMs (out-proj, FC2) add their result INTO x themselves
     // (EPI_REDADD32): LayerNorm then only reads x and writes its 16-bit output.
     Workspace& w = tw.ws;
-    const int M = nseq * T, h = tw.hidden;
+    const int M = pk ? pk->rows : nseq * T, h = tw.hidden;
     const int bf = c->operand_bf16 ? 1 : 0;
     const int dh = h / tw.heads;                      // 64, 80 or 104 (check_geometry)
     const float qscale = 1.0f / sqrtf((float)dh);     // clip.cpp:1082, 1363: the real head_dim, not the padded one
@@ -326,7 +334,8 @@ bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal, int first,
         const Layer& l = tw.L[il];
         { Scope s(c, K_LN); launch_layernorm(w.x, h, M, h, tw.eps, l.ln1_g, l.ln1_b, nullptr, w.a, bf, c->stream); }
         if (!run_linear(c, l.qkv, &w.map_a, w.a, bf, M, w.qkv, qw, EPI_STORE16, bf, qw / 3, qscale)) return false;
-        if (c->attn_tc) { Scope s(c, K_ATTN); CK(launch_attention_tc(w.qkv, w.a, nseq, T, tw.heads, dh, causal ? 1 : 0, bf, c->stream)); }
+        if (pk) { Scope s(c, K_ATTN); CK(launch_attention_tc_varlen(w.qkv, w.a, pk->rows, pk->nseq, pk->d_seq, pk->groups, tw.heads, dh, bf, c->stream)); }
+        else if (c->attn_tc) { Scope s(c, K_ATTN); CK(launch_attention_tc(w.qkv, w.a, nseq, T, tw.heads, dh, causal ? 1 : 0, bf, c->stream)); }
         else { Scope s(c, K_ATTN); launch_attention(w.qkv, w.a, nseq, T, tw.heads, causal ? 1 : 0, bf, c->stream); }
         if (!run_linear(c, l.out, &w.map_a, w.a, bf, M, w.x, h, EPI_REDADD32, 0)) return false;
         { Scope s(c, K_LN); launch_layernorm(w.x, h, M, h, tw.eps, l.ln2_g, l.ln2_b, nullptr, w.a, bf, c->stream); }
@@ -1464,6 +1473,251 @@ bool clip_b200_text_tokens_device(const struct clip_ctx* cctx, const void* d_ids
     return tokens_call(cctx, a);
 }
 
+// ---- images of different sizes in one call: the four clip_b200_*_mixed forms ----------------------------------------------------
+// What one mixed call reads, as its public form received it.
+struct MixedCall {
+    const char* who;                              // the public name, for messages
+    bool tokens, host;                            // per-token rows (else pooled); host images and output (else device)
+    const clip_image_f32_batch* imgs = nullptr;   // host: the images, each of its own ny x nx
+    const void* in = nullptr;                     // device: the NHWC f32 images back to back
+    const int *heights = nullptr, *widths = nullptr;
+    size_t n = 0;
+    int layer = 0, flags = 0, out_type = 0;       // tokens
+    void* out = nullptr;                          // tokens: the ragged rows (host or device)
+    float* vec = nullptr;                         // pooled, host
+    float* d_vec = nullptr;                       // pooled, device
+    bool normalize = true;
+    int H(size_t i) const { return host ? imgs->data[i].ny : heights[i]; }
+    int W(size_t i) const { return host ? imgs->data[i].nx : widths[i]; }
+};
+
+// check_hw_size for image i of a mixed call: the message names the image
+static bool check_mixed_size(const clip_ctx* c, size_t i, int H, int W, const char* who) {
+    const std::string w = std::string(who) + ": image " + std::to_string(i);
+    return check_hw_size(c, H, W, w.c_str());
+}
+
+// Rows of entry q for the images of a packed pass (T[i] rows each, `rows` in all) -> dst, item-major and ragged.  Without NO_CLS the
+// packed rows are already that layout, so the tail is token_rows_tail's on one item of `rows` rows.  With NO_CLS, K7 runs once per
+// image on that image's rows (after the same LN / projection / l2norm over all rows with PROJECT), as it runs on an image alone.
+static bool mixed_rows_tail(clip_ctx* c, Tower& tw, const std::vector<int>& T, int rows, const TokenReq& q, char* dst) {
+    if (!q.skip) return token_rows_tail(c, tw, 1, rows, q, dst);
+    Workspace& w = tw.ws;
+    const int h = tw.hidden, bf = c->operand_bf16 ? 1 : 0;
+    const float* src = w.x;
+    int width = h;
+    const float* gamma = (q.flags & CLIP_B200_TOKENS_POST_LN) ? tw.post_g : nullptr;
+    if (q.flags & CLIP_B200_TOKENS_PROJECT) {
+        float* p32 = reinterpret_cast<float*>(w.qkv);     // as token_rows_tail lays them out
+        float* n32 = reinterpret_cast<float*>(w.g);
+        { Scope s(c, K_LN); launch_layernorm(w.x, h, rows, h, tw.eps, tw.post_g, tw.post_b, nullptr, w.a, bf, c->stream); }
+        if (!run_linear(c, tw.proj_w, &w.map_a, w.a, bf, rows, p32, tw.proj, EPI_STORE32, 0)) return false;
+        if (q.flags & CLIP_B200_TOKENS_NORMALIZE) { Scope s(c, K_OTHER); launch_l2norm(p32, n32, rows, tw.proj, 1, c->stream); p32 = n32; }
+        src = p32; width = tw.proj; gamma = nullptr;
+    }
+    Scope s(c, K_TOKEN_ROWS);
+    size_t r0 = 0;
+    for (int t : T) {
+        launch_token_rows(src + r0 * width, width, 1, t, 1, width, gamma, tw.post_b, tw.eps, q.out_type, dst, c->stream);
+        r0 += (size_t)t;
+        dst += (size_t)(t - 1) * width * q.esize;
+    }
+    CK(cudaGetLastError());
+    return true;
+}
+
+// One GPU, images lo .. hi of a checked mixed call.  Position tables for every grid first, then passes of the longest prefix of the
+// remaining images that fits every workspace buffer, each one forward pass over its rows packed back to back.
+static bool mixed_pass(clip_ctx* c, const MixedCall& a, const TokenReq& q, size_t lo, size_t hi) {
+    Tower& tw = c->vis;
+    Workspace& w = tw.ws;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    if (!ensure_ws(c, tw, tw.micro_batch, tw.T, true)) return false;
+    const int P = tw.patch, h = tw.hidden, g = tw.image_size / P, bf = c->operand_bf16 ? 1 : 0;
+    const size_t n = hi - lo;
+    std::vector<int> T(n);
+    for (size_t i = 0; i < n; i++) {
+        const int H = a.H(lo + i), W = a.W(lo + i);
+        T[i] = (H / P) * (W / P) + 1;
+        if (T[i] > w.cap_rows || (size_t)(T[i] - 1) > (size_t)w.cap_items * tw.n_patches) {
+            set_err(std::string(a.who) + ": image " + std::to_string(lo + i) + ": one " + std::to_string(H) + " x " + std::to_string(W) +
+                    " image needs " + std::to_string(T[i]) + " rows, more than the workspace holds (" + std::to_string(w.cap_rows) +
+                    "); raise clip_b200_set_micro_batch before the first encode");
+            return false;
+        }
+    }
+    // one position table per grid: the loaded one at the model's own grid, the others resampled (K8) into one arena
+    std::map<std::pair<int, int>, size_t> table;
+    size_t floats = 0;
+    for (size_t i = 0; i < n; i++) {
+        const std::pair<int, int> gg(a.H(lo + i) / P, a.W(lo + i) / P);
+        if (gg != std::make_pair(g, g) && !table.count(gg)) { table[gg] = floats; floats += (size_t)T[i] * h; }
+    }
+    if (floats && !ensure_buf(c, &c->pos_mixed, &c->pos_mixed_cap, floats)) return false;
+    for (const auto& e : table) {
+        float* dst = c->pos_mixed + e.second;
+        CK(cudaMemcpyAsync(dst, tw.pos, (size_t)h * 4, cudaMemcpyDeviceToDevice, c->stream));     // the CLS row as it is
+        { Scope s(c, K_POS_RESAMPLE); launch_pos_resample(tw.pos + h, g, h, e.first.first, e.first.second, dst + h, c->stream); }
+    }
+    CK(cudaGetLastError());
+    // passes: total rows <= cap_rows, patch rows <= cap_items * n_patches, images <= cap_items (plan_call's limits)
+    std::vector<size_t> bounds{0};
+    {
+        size_t rows = 0, prows = 0, k = 0;
+        for (size_t i = 0; i < n; i++) {
+            if (k && (rows + T[i] > (size_t)w.cap_rows || prows + T[i] - 1 > (size_t)w.cap_items * tw.n_patches || k + 1 > (size_t)w.cap_items)) {
+                bounds.push_back(i);
+                rows = prows = k = 0;
+            }
+            rows += T[i]; prows += T[i] - 1; k++;
+        }
+        bounds.push_back(n);
+    }
+    size_t most = 0;
+    for (size_t b = 0; b + 1 < bounds.size(); b++) most = std::max(most, bounds[b + 1] - bounds[b]);
+    const size_t desc_bytes = (most * sizeof(MixedImage) + 2 * (most + 1) * sizeof(int) + 255) / 256 * 256;
+    if (!ensure_buf(c, &c->d_mixed, &c->d_mixed_cap, desc_bytes)) return false;
+    // where image lo + i starts: its pixels (floats from the call's first image) and its output (bytes from the call's out)
+    std::vector<size_t> px0(n + 1, 0), out0(n + 1, 0);
+    size_t px_lo = 0, out_lo = 0;
+    for (size_t i = 0; i < lo; i++) {
+        px_lo += (size_t)a.H(i) * a.W(i) * 3;
+        out_lo += (size_t)((a.H(i) / P) * (a.W(i) / P) + 1 - q.skip) * q.width * q.esize;
+    }
+    px0[0] = px_lo; out0[0] = out_lo;
+    for (size_t i = 0; i < n; i++) {
+        px0[i + 1] = px0[i] + (size_t)a.H(lo + i) * a.W(lo + i) * 3;
+        out0[i + 1] = out0[i] + (size_t)(T[i] - q.skip) * q.width * q.esize;
+    }
+    float* d_vec = a.d_vec;
+    if (!a.tokens && !d_vec) {
+        if (!ensure_out(c, n * tw.proj)) return false;
+        d_vec = c->d_out;
+    }
+    char* stage = nullptr;     // host tokens: one pass's rows on the device, then copied out
+    if (a.tokens && a.host) {
+        size_t widest = 0;
+        for (size_t b = 0; b + 1 < bounds.size(); b++) widest = std::max(widest, out0[bounds[b + 1]] - out0[bounds[b]]);
+        if (!ensure_buf(c, &c->d_ring, &c->d_ring_cap, widest)) return false;
+        stage = c->d_ring;
+    }
+    std::vector<char> blob(desc_bytes);
+    CK(cudaEventRecord(c->ev_t0, c->stream));
+    for (size_t b = 0; b + 1 < bounds.size(); b++) {
+        const size_t i0 = bounds[b], i1 = bounds[b + 1];
+        const int nb = (int)(i1 - i0);
+        MixedImage* im = reinterpret_cast<MixedImage*>(blob.data());
+        int* off = reinterpret_cast<int*>(blob.data() + nb * sizeof(MixedImage));
+        int* grp = off + nb + 1;
+        int rows = 0, prows = 0;
+        off[0] = grp[0] = 0;
+        for (int j = 0; j < nb; j++) {
+            const size_t i = i0 + j;
+            const int gh = a.H(lo + i) / P, gw = a.W(lo + i) / P;
+            const auto it = table.find(std::make_pair(gh, gw));
+            im[j].px = (long long)(px0[i] - px0[i0]);
+            im[j].pos = it == table.end() ? tw.pos : c->pos_mixed + it->second;
+            im[j].row = rows; im[j].prow = prows; im[j].gh = gh; im[j].gw = gw;
+            rows += T[i]; prows += T[i] - 1;
+            off[j + 1] = rows;
+            grp[j + 1] = grp[j] + (T[i] + 63) / 64;
+        }
+        const MixedImage* d_im = reinterpret_cast<const MixedImage*>(c->d_mixed);
+        const int* d_seq = reinterpret_cast<const int*>(c->d_mixed + nb * sizeof(MixedImage));
+        CK(cudaMemcpyAsync(c->d_mixed, blob.data(), nb * sizeof(MixedImage) + 2 * (nb + 1) * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+        const float* px;
+        if (a.host) {
+            for (int j = 0; j < nb; j++)
+                CK(cudaMemcpyAsync(w.pixels[0] + im[j].px, a.imgs->data[lo + i0 + j].data, (px0[i0 + j + 1] - px0[i0 + j]) * 4, cudaMemcpyHostToDevice, c->stream));
+            px = w.pixels[0];
+        } else {
+            px = (const float*)a.in + px0[i0];
+        }
+        { Scope s(c, K_OTHER); launch_im2col_mixed(px, d_im, nb, prows, P, tw.kpad, w.patches, c->stream); }
+        if (!run_linear(c, tw.patch_w, &w.map_patches, w.patches, false, prows, w.patch32, h, EPI_STORE32, 0)) return false;
+        { Scope s(c, K_OTHER); launch_assemble_mixed(w.patch32, tw.class_embd, d_im, nb, rows, h, tw.eps, tw.pre_g, tw.pre_b, w.x, c->stream); }
+        const Packed pk{rows, nb, grp[nb], d_seq};
+        if (a.tokens) {
+            if (!run_blocks(c, tw, nb, 0, false, 0, q.blocks, &pk)) return false;
+            char* dst = a.host ? stage : (char*)a.out + out0[i0];
+            if (!mixed_rows_tail(c, tw, std::vector<int>(T.begin() + i0, T.begin() + i1), rows, q, dst)) return false;
+            if (a.host) CK(cudaMemcpyAsync((char*)a.out + out0[i0], stage, out0[i1] - out0[i0], cudaMemcpyDeviceToHost, c->stream));
+        } else {
+            if (!run_blocks(c, tw, nb, 0, false, 0, tw.layers, &pk)) return false;
+            // CLS rows (off[j]) -> post-LN -> projection -> (L2 norm); the fp32 gather keeps the bits vision_forward's strided LN reads
+            { Scope s(c, K_OTHER); launch_gather_rows(w.x, w.sel32, nb, h, 0, d_seq, nullptr, bf, c->stream); }
+            { Scope s(c, K_LN); launch_layernorm(w.sel32, h, nb, h, tw.eps, tw.post_g, tw.post_b, nullptr, w.sel16, bf, c->stream); }
+            if (!run_linear(c, tw.proj_w, &w.map_sel, w.sel16, bf, nb, w.proj32, tw.proj, EPI_STORE32, 0)) return false;
+            { Scope s(c, K_OTHER); launch_l2norm(w.proj32, d_vec + i0 * tw.proj, nb, tw.proj, a.normalize ? 1 : 0, c->stream); }
+            CK(cudaGetLastError());
+        }
+    }
+    CK(cudaEventRecord(c->ev_t1, c->stream));
+    if (!a.tokens && a.vec) CK(cudaMemcpyAsync(a.vec + lo * tw.proj, d_vec, n * tw.proj * 4, cudaMemcpyDeviceToHost, c->stream));
+    return sync_and_time(c);
+}
+
+// Every mixed form: the arguments checked in one order, the first fault refused (include/clip_b200.h), then the passes; devices mode
+// shards the host forms' images over the GPUs as clip_image_batch_encode does.
+static bool mixed_call(const clip_ctx* cctx, MixedCall a) {
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    const std::string who = a.who;
+    if (!c) { set_err(who + ": null context"); return false; }
+    if (!c->vis.present) { set_err(who + ": this model has no vision encoder"); return false; }
+    if (!a.host && a.heights && a.widths)
+        for (size_t i = 0; i < a.n; i++)
+            if (!check_mixed_size(c, i, a.heights[i], a.widths[i], a.who)) return false;
+    if (a.host) a.n = a.imgs ? a.imgs->size : 0;     // a NULL batch is an empty one
+    if (a.n == 0) return true;
+    if (a.host) {
+        if (!a.imgs->data) { set_err(who + ": null input"); return false; }
+        if (!(a.tokens ? a.out : a.vec)) { set_err(who + ": null output"); return false; }
+        for (size_t i = 0; i < a.n; i++) {
+            if (!a.imgs->data[i].data) { set_err(who + ": image " + std::to_string(i) + " has no pixels"); return false; }
+            if (!check_mixed_size(c, i, a.imgs->data[i].ny, a.imgs->data[i].nx, a.who)) return false;
+        }
+    } else {
+        if (!a.in || !(a.tokens ? a.out : a.d_vec)) { set_err(who + ": null device pointer"); return false; }
+        if (!a.heights || !a.widths) { set_err(who + ": null heights or widths"); return false; }
+    }
+    TokenReq q;
+    if (a.tokens) {
+        if (!token_request(c, true, a.layer, a.flags, a.out_type, q, a.who)) return false;
+        if (q.attn) { set_err(who + ": CLIP_B200_TOKENS_ATTENTION is not supported at mixed sizes"); return false; }
+    }
+    if (a.host && c->replicas.size() > 1 && a.n >= c->replicas.size())
+        return for_each_replica(c, a.n, [&](clip_ctx* r, int, size_t lo, size_t hi) { return hi == lo || mixed_pass(r, a, q, lo, hi); });
+    return mixed_pass(c, a, q, 0, a.n);
+}
+
+bool clip_b200_image_batch_encode_mixed(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, float* vec, bool normalize) {
+    MixedCall a{"clip_b200_image_batch_encode_mixed", false, true};
+    a.imgs = imgs; a.vec = vec; a.normalize = normalize;
+    return mixed_call(cctx, a);
+}
+
+bool clip_b200_image_encode_device_mixed(const struct clip_ctx* cctx, const void* d_pixels, size_t n, const int* heights, const int* widths,
+                                         void* d_vec, bool normalize) {
+    MixedCall a{"clip_b200_image_encode_device_mixed", false, false};
+    a.in = d_pixels; a.n = n; a.heights = heights; a.widths = widths; a.d_vec = (float*)d_vec; a.normalize = normalize;
+    return mixed_call(cctx, a);
+}
+
+bool clip_b200_image_tokens_mixed(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, int layer, int flags, int out_type,
+                                  void* out) {
+    MixedCall a{"clip_b200_image_tokens_mixed", true, true};
+    a.imgs = imgs; a.layer = layer; a.flags = flags; a.out_type = out_type; a.out = out;
+    return mixed_call(cctx, a);
+}
+
+bool clip_b200_image_tokens_device_mixed(const struct clip_ctx* cctx, const void* d_pixels, size_t n, const int* heights, const int* widths,
+                                         int layer, int flags, int out_type, void* d_out) {
+    MixedCall a{"clip_b200_image_tokens_device_mixed", true, false};
+    a.in = d_pixels; a.n = n; a.heights = heights; a.widths = widths; a.layer = layer; a.flags = flags; a.out_type = out_type; a.out = d_out;
+    return mixed_call(cctx, a);
+}
+
 // ---- several layers from one forward pass (clip_b200_*_tokens_layers) ------------------------------------------------------------
 bool clip_b200_image_tokens_layers(const struct clip_ctx* cctx, const struct clip_image_f32_batch* imgs, const int* layers, const int* flags,
                                    int n_layers, int out_type, void* out) {
@@ -2331,6 +2585,39 @@ void from16(const uint16_t* x, size_t n, int bf16, float* out) {
 }  // namespace
 
 extern "C" {
+
+// TEST HOOK: K3's varlen instance on device 0.  nseq sequences of lens[s] rows packed back to back: qkv fp32 host [sum lens, 3*H*dh]
+// (laid out, rounded and padded as for clip_b200_debug_attention_hd), out fp32 host [sum lens, H*dh].  The qkv rows past the last
+// sequence and one 128-row block of guard rows after the output are poisoned (0xFF); a guard row written is an error (rc 6).
+int clip_b200_debug_attention_mixed(int operand_bf16, int nseq, const int* lens, int H, int head_dim, const float* qkv, float* out) {
+    g_err.clear();
+    if (head_dim != 64 && head_dim != 80 && head_dim != 104) { set_err("attention_mixed: head_dim must be 64, 80 or 104"); return 2; }
+    if (nseq <= 0 || H <= 0 || !lens) { set_err("attention_mixed: bad shape"); return 2; }
+    std::vector<int> seq(2 * ((size_t)nseq + 1), 0);
+    int* off = seq.data();
+    int* grp = off + nseq + 1;
+    for (int i = 0; i < nseq; i++) {
+        if (lens[i] <= 0) { set_err("attention_mixed: every length must be positive"); return 2; }
+        off[i + 1] = off[i] + lens[i];
+        grp[i + 1] = grp[i] + (lens[i] + 63) / 64;
+    }
+    if (attention_tc_init() != cudaSuccess) { set_err("attention_tc_init failed"); return 1; }
+    const size_t rows = (size_t)off[nseq], hid = (size_t)H * head_dim, qcols = (size_t)3 * H * qkv_head_cols(head_dim), guard = 128 * hid;
+    const std::vector<uint16_t> h16 = qkv_to16_padded(qkv, rows, H, head_dim, operand_bf16);
+    HookScratch s;
+    uint16_t* d_qkv = (uint16_t*)s.alloc((rows + 128) * qcols * 2, 0xff, h16.data(), h16.size() * 2);
+    uint16_t* d_out = (uint16_t*)s.alloc((rows * hid + guard) * 2, 0xff);
+    int* d_seq = (int*)s.alloc(seq.size() * 4, 0, seq.data(), seq.size() * 4);
+    if (!s.ok) return 3;
+    const cudaError_t e = launch_attention_tc_varlen(d_qkv, d_out, (int)rows, nseq, d_seq, grp[nseq], H, head_dim, operand_bf16, s.st);
+    if (e != cudaSuccess) { set_err(std::string("attention_mixed: ") + cudaGetErrorString(e)); return 5; }
+    if (!s.finish("attention_mixed")) return 5;
+    std::vector<uint16_t> o16(rows * hid + guard);
+    if (!s.copy_back(o16.data(), d_out, o16.size() * 2)) return 6;
+    if (std::any_of(o16.begin() + rows * hid, o16.end(), [](uint16_t b) { return b != 0xffff; })) { set_err("attention_mixed: a guard row was written"); return 6; }
+    from16(o16.data(), rows * hid, operand_bf16, out);
+    return 0;
+}
 
 int clip_b200_debug_layernorm(int rows, int h, size_t in_stride, float eps, const float* x, const float* gamma, const float* beta,
                               const float* delta, int operand_bf16, float* y_out, float* x_out) {

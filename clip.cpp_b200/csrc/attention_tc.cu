@@ -111,6 +111,37 @@ CB_DEVINL Group group_of(const AParams& p, int g) {
     return r;
 }
 
+// Packed sequences of different lengths (launch_attention_tc_varlen): sequence s is rows [off[s], off[s + 1]) of one [row][column]
+// view of the qkv matrix, and its groups are numbered from H * grp[s] (grp: prefix sums of the per-sequence group counts ceil(len / 64)).
+struct VarLen {
+    const int* off;
+    const int* grp;
+    int nseq;
+};
+
+// group_of for packed sequences.  Group::seq holds the sequence's first row (distinct for distinct sequences, so iter_var's test of a
+// shared (sequence, head) is iter_of's) and kend its length.  s: a sequence at or before group g's, advanced to g's.  A thread's
+// groups only increase, so the search gallops forward from the last sequence found (one load when g is still in it) and ends in a
+// binary search of the bracket.
+CB_DEVINL Group group_var(const AParams& p, const VarLen& v, int g, int& s) {
+    int lo = s, step = 1;
+    while (lo + step < v.nseq && __ldg(v.grp + lo + step) * p.H <= g) { lo += step; step *= 2; }
+    int hi = min(lo + step, v.nseq) - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (__ldg(v.grp + mid) * p.H <= g) lo = mid;
+        else hi = mid - 1;
+    }
+    s = lo;
+    const int ng = __ldg(v.grp + lo + 1) - __ldg(v.grp + lo), local = g - __ldg(v.grp + lo) * p.H;
+    Group r;
+    r.head = local / ng;
+    r.g0 = (local - r.head * ng) * AG;
+    r.seq = __ldg(v.off + lo);
+    r.kend = __ldg(v.off + lo + 1) - r.seq;
+    return r;
+}
+
 // The two groups of iteration `it` and what the K / V stages hold for them: slot 0 the first group's head (and the second's, when it
 // is the same (sequence, head) or there is no second group), slot 1 the second group's head otherwise.  kend0 / kend1: the keys a
 // slot must hold (0: slot unused); nkb: key blocks (of KB keys) of the iteration.
@@ -132,11 +163,46 @@ CB_DEVINL Iter iter_of(const AParams& p, int it) {
     return r;
 }
 
+// iter_of for packed sequences (s: group_var's)
+template <int KB>
+CB_DEVINL Iter iter_var(const AParams& p, const VarLen& v, int it, int& s) {
+    Iter r;
+    r.has_b = 2 * it + 1 < p.ngroups;
+    r.a = group_var(p, v, 2 * it, s);
+    r.b = r.has_b ? group_var(p, v, 2 * it + 1, s) : r.a;
+    r.shared = r.a.seq == r.b.seq && r.a.head == r.b.head;
+    r.kend0 = r.shared ? max(r.a.kend, r.b.kend) : r.a.kend;
+    r.kend1 = r.shared ? 0 : r.b.kend;
+    r.nkb = (max(r.kend0, r.kend1) + KB - 1) / KB;
+    return r;
+}
+
 // 64-row boxes of key block kb (KB keys) that a slot holding keys [0, kend) needs
 template <int KB>
 CB_DEVINL int kv_boxes(int kend, int kb) {
     const int key0 = kb * KB;
     return key0 >= kend ? 0 : (KB == ABOX || key0 + ABOX >= kend) ? 1 : 2;
+}
+
+// Rows of the last 64-row box a slot holding keys [0, kend) loads for block kb that lie past kend (0 when kb is not the slot's last
+// block).  In a packed view those rows belong to the next sequence.
+template <int KB>
+CB_DEVINL int kv_pad_rows(int kend, int kb) {
+    const int nb = kv_boxes<KB>(kend, kb);
+    return nb ? max(0, kb * KB + nb * ABOX - kend) : 0;
+}
+
+// Zero rows [r0, r1) of every piece of the KB-row tile at `tile`: each piece is row-major and its swizzle permutes 16-byte chunks
+// within a row, so a row's bytes are one contiguous range of the piece whatever the swizzle.  The calling warp's 32 lanes store.
+template <int DH>
+CB_DEVINL void zero_tile_rows(uint32_t tile, int r0, int r1, int lane) {
+    using G = AttnGeo<DH>;
+    auto zero = [&](uint32_t a0, uint32_t a1) {
+        for (uint32_t a = a0 + 16u * lane; a < a1; a += 512u) asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(a), "r"(0u) : "memory");
+    };
+    zero(tile + r0 * 128u, tile + r1 * 128u);
+    if constexpr (G::MID) zero(tile + G::mid_off(G::KB) + r0 * 64u, tile + G::mid_off(G::KB) + r1 * 64u);
+    if constexpr (G::TAIL) zero(tile + G::tail_off(G::KB) + r0 * 32u, tile + G::tail_off(G::KB) + r1 * 32u);
 }
 
 // one 64-row box (every piece) into box `b` of the `rows`-row tile at `tile`; tm_mid: the head_dim 104 map of columns 64-95
@@ -367,6 +433,175 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __gr
         }
     }
 }
+
+// K3 on packed sequences of different lengths (VarLen), non-causal: the kernel above with the maps viewing the packed rows as one
+// sequence.  A group's rows and keys are counted from its sequence's first row, its length takes the place of T, so every key block
+// and the width of the last one are those a fixed-T launch of that sequence alone takes, and each kept row has its arithmetic.  The box rows past a
+// sequence's end now hold the next sequence's rows instead of zeros: their scores are masked by select, their Q rows are never
+// stored, but P.V would turn a non-finite V row into NaN (0 * Inf), so the producer warp zeroes those V rows once the box has landed
+// and before the consumers may read the stage: such a stage lands on a barrier of the producer's own, and the producer arrives on
+// the stage's full barrier once the zeros are stored.
+template <bool BF, int DH>
+__global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(const __grid_constant__ AParams p, const __grid_constant__ CUtensorMap tm_mid,
+                                                                             const VarLen v) {
+    using G = AttnGeo<DH>;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    const uint32_t smem_base = smem_u32(smem);
+    // [i] = +8i bytes: Q tile full / empty (rings of two), K-V stage full / empty (rings of NST); kv_land: the producer's own barrier
+    // for a stage it zeroes before the consumers may read it
+    const uint32_t q_full = smem_base + G::BAR_OFF, q_empty = q_full + 16, kv_full = q_full + 32, kv_empty = kv_full + 8 * G::NST;
+    const uint32_t kv_land = kv_empty + 8 * G::NST;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < G::NST; i++) {
+            if (i < 2) { mbar_init(q_full + 8 * i, 1); mbar_init(q_empty + 8 * i, 8); }      // released by each consumer warp
+            mbar_init(kv_full + 8 * i, 1); mbar_init(kv_empty + 8 * i, 8);
+        }
+        mbar_init(kv_land, 1);
+        mbar_fence_init();
+        tma_prefetch_desc(&p.tm_qkv);
+        if constexpr (G::MID) tma_prefetch_desc(&tm_mid);
+        if constexpr (G::TAIL) tma_prefetch_desc(&p.tm_tail);
+    }
+    __syncthreads();
+    pdl_trigger();
+    pdl_wait();      // qkv is read (and the output written) only after the QKV GEMM grid has completed
+
+    const int hid = p.H * DH, qcols = p.H * G::DHP;           // output row, and Q / K / V part of a qkv row
+    // Ring positions run on across iterations: the i-th iteration of this CTA uses Q tile i % 2 (its (i / 2)-th use), the n-th key
+    // block of this CTA stage n % NST (its (n / NST)-th use).  A use waits for full with the use's parity and, in the producer, for the
+    // release of the previous use of the slot (parity flipped: the first wait on a fresh barrier passes).
+    if (warp == 8) {
+        // ------------------------------------------------------------------ producer (one warp)
+        // lane 0 issues the loads.  A stage that holds a sequence's last block lands on kv_land instead of kv_full; the whole warp
+        // waits for it, zeroes the V rows past the sequence's end and only then arrives on kv_full.  nz: such stages so far.
+        uint32_t n = 0, i = 0, nz = 0;
+        int sq = 0;
+        for (int it = blockIdx.x; it < p.niter; it += gridDim.x, i++) {
+            const Iter w = iter_var<G::KB>(p, v, it, sq);
+            const uint32_t qb = i & 1, q_s = smem_base + qb * G::TILE;
+            if (lane == 0) {
+                mbar_wait(q_empty + 8 * qb, ((i >> 1) & 1) ^ 1);
+                mbar_arrive_expect_tx(q_full + 8 * qb, (w.has_b ? 2 : 1) * G::BOX_BYTES);
+                load_box<DH, AK>(q_s, 0, p, tm_mid, w.a.head * G::DHP, w.a.seq + w.a.g0, 0, q_full + 8 * qb);
+                if (w.has_b) load_box<DH, AK>(q_s, 1, p, tm_mid, w.b.head * G::DHP, w.b.seq + w.b.g0, 0, q_full + 8 * qb);
+            }
+            for (int kb = 0; kb < w.nkb; kb++, n++) {
+                const uint32_t s = n % G::NST;
+                const int nb0 = kv_boxes<G::KB>(w.kend0, kb), nb1 = kv_boxes<G::KB>(w.kend1, kb);
+                const uint32_t slot0 = smem_base + G::KV_OFF + s * (4 * G::KTILE), slot1 = slot0 + 2 * G::KTILE;
+                const int z0 = kv_pad_rows<G::KB>(w.kend0, kb), z1 = kv_pad_rows<G::KB>(w.kend1, kb);
+                const uint32_t bar = (z0 || z1) ? kv_land : kv_full + 8 * s;
+                if (lane == 0) {
+                    mbar_wait(kv_empty + 8 * s, ((n / G::NST) & 1) ^ 1);
+                    mbar_arrive_expect_tx(bar, (uint32_t)(nb0 + nb1) * 2 * G::BOX_BYTES);
+                    for (int b = 0; b < nb0; b++) {
+                        load_box<DH, G::KB>(slot0, b, p, tm_mid, qcols + w.a.head * G::DHP, w.a.seq + kb * G::KB + b * ABOX, 0, bar);
+                        load_box<DH, G::KB>(slot0 + G::KTILE, b, p, tm_mid, 2 * qcols + w.a.head * G::DHP, w.a.seq + kb * G::KB + b * ABOX, 0, bar);
+                    }
+                    for (int b = 0; b < nb1; b++) {
+                        load_box<DH, G::KB>(slot1, b, p, tm_mid, qcols + w.b.head * G::DHP, w.b.seq + kb * G::KB + b * ABOX, 0, bar);
+                        load_box<DH, G::KB>(slot1 + G::KTILE, b, p, tm_mid, 2 * qcols + w.b.head * G::DHP, w.b.seq + kb * G::KB + b * ABOX, 0, bar);
+                    }
+                }
+                __syncwarp();
+                if (z0 || z1) {
+                    mbar_wait(kv_land, nz++ & 1);
+                    if (z0) zero_tile_rows<DH>(slot0 + G::KTILE, nb0 * ABOX - z0, nb0 * ABOX, lane);
+                    if (z1) zero_tile_rows<DH>(slot1 + G::KTILE, nb1 * ABOX - z1, nb1 * ABOX, lane);
+                    // the zeros (generic proxy) before the consumers' wgmma reads and the next TMA into the stage (async proxy)
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(kv_full + 8 * s);
+                }
+            }
+        }
+        return;
+    }
+
+    // ---------------------------------------------------------------------- consumers (fragment layout: wgmma.cuh)
+    const int wg = warp >> 2;
+    const int tc = 2 * (lane & 3);                             // this thread: columns 8j + tc + {0, 1}
+    uint32_t n = 0, i = 0;
+    int sq = 0;
+    for (int it = blockIdx.x; it < p.niter; it += gridDim.x, i++) {
+        const int sq_it = sq;                                  // at or before both groups' sequences
+        const Iter w = iter_var<G::KB>(p, v, it, sq);
+        const Group g = (wg == 0 || !w.has_b) ? w.a : w.b;
+        const bool live = wg == 0 || w.has_b;                  // warpgroup-uniform: only the launch's last, odd group leaves one idle
+        const uint32_t slot = (wg == 0 || w.shared) ? 0u : 1u;
+        const int nkb = (g.kend + G::KB - 1) / G::KB;
+        const int wrow0 = g.g0 + (warp & 3) * 16;              // first query row of this warp
+        const int r0 = wrow0 + (lane >> 2);                    // this thread: rows r0 and r0 + 8
+        // o: columns 0-63, om: 64-95 (head_dim 104 only), ot: the 16-column tail (head_dim 80, 104)
+        float o[32], om[16], ot[8], m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+        #pragma unroll
+        for (int j = 0; j < 32; j++) o[j] = 0.f;
+        #pragma unroll
+        for (int j = 0; j < 16; j++) om[j] = 0.f;
+        #pragma unroll
+        for (int j = 0; j < 8; j++) ot[j] = 0.f;
+        const uint32_t qb = i & 1, q_s = smem_base + qb * G::TILE;
+        mbar_wait(q_full + 8 * qb, (i >> 1) & 1);
+        const uint64_t dq = wgmma_desc_sw128(q_s + (uint32_t)wg * 64u * 128u);
+        const uint64_t dq_m = wgmma_desc_sw64(q_s + G::mid_off(AK) + (uint32_t)wg * 64u * 64u);
+        const uint64_t dq_t = wgmma_desc_sw32(q_s + G::tail_off(AK) + (uint32_t)wg * 64u * 32u);
+        for (int kb = 0; kb < w.nkb; kb++, n++) {
+            const uint32_t s = n % G::NST;
+            const uint32_t k_s = smem_base + G::KV_OFF + s * (4 * G::KTILE) + slot * (2 * G::KTILE), v_s = k_s + G::KTILE;
+            mbar_wait(kv_full + 8 * s, (n / G::NST) & 1);
+            if (live && kb < nkb) {
+                const int key0 = kb * G::KB, rem = g.kend - key0;
+                // S at the narrowest width that covers the keys left (a 64-key block never needs 128)
+                if (G::KB == 128 && rem > 64) attend_block<BF, DH, 16>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, g.kend, 0, wrow0, r0, tc);
+                else if (rem > 32) attend_block<BF, DH, 8>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, g.kend, 0, wrow0, r0, tc);
+                else if (rem > 16) attend_block<BF, DH, 4>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, g.kend, 0, wrow0, r0, tc);
+                else attend_block<BF, DH, 2>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, g.kend, 0, wrow0, r0, tc);
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(kv_empty + 8 * s);
+        }
+        // every S product that read this Q tile has completed (wgmma_wait<0> in attend_block)
+        __syncwarp();
+        if (lane == 0) mbar_arrive(q_empty + 8 * qb);
+        if (!live) continue;
+        // the group's first row and head looked up again rather than held in registers through the key loop (the head_dim 80
+        // instance has none to spare at 168, the most 288 threads can have)
+        int sq_e = sq_it;
+        const Group ge = group_var(p, v, 2 * it + wg, sq_e);
+        #pragma unroll
+        for (int h = 0; h < 2; h++) {
+            float l = l_run[h];
+            l += __shfl_xor_sync(0xffffffffu, l, 1);
+            l += __shfl_xor_sync(0xffffffffu, l, 2);
+            const float inv = 1.0f / l;
+            const int row = r0 + 8 * h;
+            if (row < g.kend) {
+                uint16_t* orow = p.out + ((size_t)ge.seq + row) * hid + ge.head * DH;
+                #pragma unroll
+                for (int j = 0; j < 8; j++)
+                    *reinterpret_cast<uint32_t*>(orow + 8 * j + tc) = pack2<BF>(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
+                if constexpr (G::MID) {
+                    #pragma unroll
+                    for (int j = 0; j < 4; j++)
+                        *reinterpret_cast<uint32_t*>(orow + 64 + 8 * j + tc) = pack2<BF>(om[4 * j + 2 * h] * inv, om[4 * j + 2 * h + 1] * inv);
+                }
+                if constexpr (G::TAIL) {
+                    // the real tail columns only: at head_dim 104, columns 104-111 are the padding
+                    #pragma unroll
+                    for (int j = 0; j < (DH - G::tail_col()) / 8; j++)
+                        *reinterpret_cast<uint32_t*>(orow + G::tail_col() + 8 * j + tc) = pack2<BF>(ot[4 * j + 2 * h] * inv, ot[4 * j + 2 * h + 1] * inv);
+                }
+            }
+        }
+    }
+}
+
+// the varlen kernel's shared memory: one more barrier (kv_land)
+template <int DH>
+constexpr uint32_t varlen_smem() { return AttnGeo<DH>::SMEM + 8; }
 
 // ---- K9: the attention probabilities themselves (the *_tokens calls' ATTENTION entries) ------------------------------------------
 // softmax(Q.K^T [causal]) of one block, recomputed from the qkv matrix K3 read (Q scaled by 1/sqrt(dh) and rounded, K 16-bit) through
@@ -628,6 +863,10 @@ cudaError_t set_smem() {
     if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(attention_tc_kernel<false, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AttnGeo<DH>::SMEM);
     if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(attention_tc_varlen_kernel<true, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)varlen_smem<DH>());
+    if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(attention_tc_varlen_kernel<false, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)varlen_smem<DH>());
+    if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(attention_probs_kernel<true, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ProbsGeo<DH>::SMEM);
     if (e != cudaSuccess) return e;
     return cudaFuncSetAttribute(attention_probs_kernel<false, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ProbsGeo<DH>::SMEM);
@@ -638,6 +877,14 @@ cudaError_t launch_dh(const AParams& p, const CUtensorMap& tm_mid, unsigned grid
     constexpr uint32_t smem = AttnGeo<DH>::SMEM;
     return bf16 ? launch_pdl(attention_tc_kernel<true, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid)
                 : launch_pdl(attention_tc_kernel<false, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid);
+}
+
+template <int DH>
+cudaError_t launch_varlen_dh(const AParams& p, const CUtensorMap& tm_mid, const VarLen& v, unsigned grid, int bf16, cudaStream_t st) {
+    static_assert(varlen_smem<DH>() <= 227 * 1024, "shared memory per block");
+    constexpr uint32_t smem = varlen_smem<DH>();
+    return bf16 ? launch_pdl(attention_tc_varlen_kernel<true, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid, v)
+                : launch_pdl(attention_tc_varlen_kernel<false, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid, v);
 }
 
 template <int DH>
@@ -677,6 +924,30 @@ cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T,
     if (e != cudaSuccess) return e;
     const unsigned grid = (unsigned)min(p.niter, sms);
     e = dh == 104 ? launch_dh<104>(p, tm_mid, grid, bf16, st) : dh == 80 ? launch_dh<80>(p, tm_mid, grid, bf16, st) : launch_dh<64>(p, tm_mid, grid, bf16, st);
+    return e != cudaSuccess ? e : cudaGetLastError();
+}
+
+cudaError_t launch_attention_tc_varlen(const void* qkv16, void* out16, int rows, int nseq, const int* d_seq, int groups, int H, int dh, int bf16,
+                                      cudaStream_t st) {
+    if (!supported_dh(dh)) return cudaErrorInvalidValue;
+    if (nseq <= 0) return cudaSuccess;
+    AParams p;
+    CUtensorMap tm_mid;
+    memset(&p, 0, sizeof(p));
+    if (!make_piece_maps(p, tm_mid, qkv16, 1, rows, H, dh)) return cudaErrorInvalidValue;
+    p.out = (uint16_t*)out16; p.T = rows; p.H = H; p.causal = 0;
+    const long long ngroups = (long long)groups * H;
+    if (ngroups > 0x7ffffffell) return cudaErrorInvalidValue;
+    p.ngroups = (int)ngroups;
+    p.niter = (p.ngroups + 1) / 2;
+    const VarLen v{d_seq, d_seq + nseq + 1, nseq};
+    int dev = 0, sms = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) return e;
+    const unsigned grid = (unsigned)min(p.niter, sms);
+    e = dh == 104 ? launch_varlen_dh<104>(p, tm_mid, v, grid, bf16, st) : dh == 80 ? launch_varlen_dh<80>(p, tm_mid, v, grid, bf16, st)
+                  : launch_varlen_dh<64>(p, tm_mid, v, grid, bf16, st);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 

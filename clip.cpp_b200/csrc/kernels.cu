@@ -4,6 +4,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 #include "kernels.h"
 
@@ -216,6 +218,23 @@ __global__ void __launch_bounds__(256) pos_resample_kernel(const float* __restri
     }
 }
 
+// One row of K4v for the mixed-size kernel: xr = LN(src + pr) * gamma + beta, one warp, expression for expression
+// assemble_preln_kernel's (which keeps its own copy, so that its code is unchanged)
+CB_DEVINL void assemble_row(const float* __restrict__ src, const float* __restrict__ pr, int h, float eps, const float* __restrict__ gamma,
+                            const float* __restrict__ beta, float* __restrict__ xr, int lane) {
+    const int h4 = h >> 2;
+    auto load = [&](int i) { return add4(ld4(src + 4 * i), ld4(pr + 4 * i)); };
+    float mean, rstd;
+    row_stats(load, h4, lane, 1.0f / (float)h, eps, mean, rstd);
+    for (int i = lane; i < h4; i += 32) {
+        const float4 v = load(i), g = ld4(gamma + 4 * i), bb = ld4(beta + 4 * i);
+        float4 o;
+        o.x = (v.x - mean) * rstd * g.x + bb.x; o.y = (v.y - mean) * rstd * g.y + bb.y;
+        o.z = (v.z - mean) * rstd * g.z + bb.z; o.w = (v.w - mean) * rstd * g.w + bb.w;
+        *reinterpret_cast<float4*>(xr + 4 * i) = o;
+    }
+}
+
 __global__ void __launch_bounds__(256) assemble_preln_kernel(const float* __restrict__ patch, const float* __restrict__ cls,
                                                              const float* __restrict__ pos, int B, int T, int h, float eps,
                                                              const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -237,6 +256,52 @@ __global__ void __launch_bounds__(256) assemble_preln_kernel(const float* __rest
         o.z = (v.z - mean) * rstd * g.z + bb.z; o.w = (v.w - mean) * rstd * g.w + bb.w;
         *reinterpret_cast<float4*>(xr + 4 * i) = o;
     }
+}
+
+// The image of a mixed-size pass that holds row `r` of the counter `field` (row or prow): images are in row order, so a binary
+// search of their first rows
+CB_DEVINL int image_of(const MixedImage* __restrict__ im, int n, int r, int MixedImage::*field) {
+    int lo = 0, hi = n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (im[mid].*field <= r) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+// K0a over the images of a mixed-size pass: patch row r of image i (r counted from the pass's first patch row) from its own grid,
+// element for element what im2col_kernel writes for that image alone.  One block per patch row at a time.
+__global__ void __launch_bounds__(256) im2col_mixed_kernel(const float* __restrict__ px, const MixedImage* __restrict__ im, int n, int prows,
+                                                           int P, int kpad, __half* __restrict__ out) {
+    const int K = 3 * P * P;
+    for (int rowi = blockIdx.x; rowi < prows; rowi += gridDim.x) {
+        const MixedImage d = im[image_of(im, n, rowi, &MixedImage::prow)];
+        const int p = rowi - d.prow, py = p / d.gw, pxx = p % d.gw, W = d.gw * P;
+        const float* img = px + d.px;
+        for (int k = threadIdx.x; k < kpad; k += blockDim.x) {
+            float v = 0.f;
+            if (k < K) {
+                const int c = k / (P * P), rem = k % (P * P), ky = rem / P, kx = rem % P;
+                v = img[((size_t)(py * P + ky) * W + (pxx * P + kx)) * 3 + c];
+            }
+            out[(size_t)rowi * kpad + k] = __float2half_rn(v);
+        }
+    }
+}
+
+// K4v over the images of a mixed-size pass: token row `row` is row t of image i, with i's position table; assemble_row as
+// assemble_preln_kernel runs it
+__global__ void __launch_bounds__(256) assemble_mixed_kernel(const float* __restrict__ patch, const float* __restrict__ cls,
+                                                             const MixedImage* __restrict__ im, int n, int rows, int h, float eps,
+                                                             const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                             float* __restrict__ x) {
+    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (row >= rows) return;
+    const MixedImage d = im[image_of(im, n, row, &MixedImage::row)];
+    const int t = row - d.row;
+    const float* src = (t == 0) ? cls : patch + ((size_t)d.prow + (t - 1)) * h;
+    assemble_row(src, d.pos + (size_t)t * h, h, eps, gamma, beta, x + (size_t)row * h, lane);
 }
 
 __global__ void __launch_bounds__(256) text_embed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ tok,
@@ -393,6 +458,17 @@ void launch_assemble_preln(const float* patch, const float* class_embd, const fl
                            const float* gamma, const float* beta, float* x, cudaStream_t st) {
     if (B * T <= 0) return;
     assemble_preln_kernel<<<rows_grid(B * T, 8), 256, 0, st>>>(patch, class_embd, pos, B, T, h, eps, gamma, beta, x);
+}
+
+void launch_im2col_mixed(const float* pixels, const MixedImage* im, int n, int prows, int P, int kpad, void* patches16, cudaStream_t st) {
+    if (n <= 0 || prows <= 0) return;
+    im2col_mixed_kernel<<<std::min(prows, 132 * 16), 256, 0, st>>>(pixels, im, n, prows, P, kpad, (__half*)patches16);
+}
+
+void launch_assemble_mixed(const float* patch, const float* class_embd, const MixedImage* im, int n, int rows, int h, float eps,
+                           const float* gamma, const float* beta, float* x, cudaStream_t st) {
+    if (n <= 0 || rows <= 0) return;
+    assemble_mixed_kernel<<<rows_grid(rows, 8), 256, 0, st>>>(patch, class_embd, im, n, rows, h, eps, gamma, beta, x);
 }
 
 void launch_text_embed(const int32_t* ids, const float* tok, const float* pos, int nseq, int T, int h, int n_vocab, float* x,

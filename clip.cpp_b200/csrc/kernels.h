@@ -34,6 +34,19 @@ void launch_pos_resample(const float* table, int g, int h, int gh, int gw, float
 void launch_assemble_preln(const float* patch, const float* class_embd, const float* pos, int B, int T, int h, float eps,
                            const float* gamma, const float* beta, float* x, cudaStream_t st);
 
+// One image of a mixed-size pass (the clip_b200_*_mixed calls): its rows are packed back to back with no padding.
+struct MixedImage {
+    long long px;          // its first pixel float, from the pass's pixel base (NHWC f32, gh*P x gw*P x 3)
+    const float* pos;      // its position table [gh*gw + 1, h]
+    int row, prow;         // its first token row (CLS) and first patch row in the pass
+    int gh, gw;            // its patch grid
+};
+// K0a and K4v over the n images of a mixed-size pass (im: device descriptors in row order): patches [prows, kpad] and x [rows, h]
+// hold each image's rows at its own offsets, bit for bit what launch_im2col / launch_assemble_preln write for that image alone.
+void launch_im2col_mixed(const float* pixels, const MixedImage* im, int n, int prows, int P, int kpad, void* patches16, cudaStream_t st);
+void launch_assemble_mixed(const float* patch, const float* class_embd, const MixedImage* im, int n, int rows, int h, float eps,
+                           const float* gamma, const float* beta, float* x, cudaStream_t st);
+
 // K4t text embed: x[s*T+t,:] = tok[ids[s*T+t],:] + pos[t,:]   (clip.cpp:1059-1061), tables fp32 (dequantised at load)
 void launch_text_embed(const int32_t* ids, const float* tok, const float* pos, int nseq, int T, int h, int n_vocab, float* x,
                        cudaStream_t st);
@@ -54,6 +67,11 @@ constexpr int qkv_head_cols(int dh) { return dh == 104 ? 112 : dh; }
 // each sequence's T tokens).
 cudaError_t attention_tc_init();
 cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T, int H, int dh, int causal, int bf16, cudaStream_t st);
+// K3 on nseq packed sequences of different lengths, non-causal: qkv16 [rows, 3*H*qkv_head_cols(dh)], out16 [rows, H*dh], sequence s
+// = rows off[s] .. off[s + 1] - 1.  d_seq (device): off [nseq + 1] (off[0] = 0, off[nseq] = rows), then grp [nseq + 1], the prefix
+// sums of ceil(len_s / 64); groups = grp[nseq].  Each sequence's rows equal, bit for bit, a launch_attention_tc of that sequence alone.
+cudaError_t launch_attention_tc_varlen(const void* qkv16, void* out16, int rows, int nseq, const int* d_seq, int groups, int H, int dh, int bf16,
+                                      cudaStream_t st);
 
 // K9 attention probabilities (attention_tc.cu): the softmax(Q K^T [causal]) K3 computes internally, from the same qkv16, written out:
 // out [nseq, H, R, T] of elem_type (0 fp32, 1 fp16, 2 bf16: RNE of the fp32 value), R = T, or 1 with cls_only (query row 0 alone).

@@ -117,6 +117,10 @@ struct clip_ctx {
     // the last position table resampled for a non-native image size (*_hw calls): CLS row + gh*gw patch rows [T, h], grow-only
     float* pos_hw = nullptr; size_t pos_hw_cap = 0;
     int pos_gh = 0, pos_gw = 0;
+    // the *_mixed calls: the position tables of every non-native grid of one call, back to back, and one pass's descriptors
+    // (MixedImage, then K3's varlen table), both grow-only
+    float* pos_mixed = nullptr; size_t pos_mixed_cap = 0;
+    char* d_mixed = nullptr; size_t d_mixed_cap = 0;
     double* d_scalars = nullptr;            // 16 doubles for the tiny all-reduces (barrier, max over ranks)
     // ---- multi-GPU (dist.h) ------------------------------------------------------------------------------------------
     cb::DistComm dist;                      // this replica's NCCL communicator (ranks mode or devices mode); world == 1: none

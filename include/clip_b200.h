@@ -259,6 +259,38 @@ bool clip_b200_image_batch_encode_hw(const struct clip_ctx * ctx, const struct c
 bool clip_b200_image_tokens_hw(const struct clip_ctx * ctx, const struct clip_image_f32_batch * imgs, int layer, int flags,
                                int out_type, void * out);
 
+/* Images of different sizes in one call (photos at their own aspect ratio, document pages): the *_hw entry points above with a
+ * height x width per image.  The images' rows are packed back to back into one forward pass, attention runs per image over packed
+ * sequences of different lengths, and each image gets the position table of its own grid.
+ *   sizes    every *_hw rule applies per image: positive multiples of patch_size, at most 4096.  Host forms read each image's size
+ *            from its ny / nx; device forms take heights[i] / widths[i], host arrays of n entries, and d_pixels holds the NHWC f32
+ *            images back to back (image i starts at float 3 * sum_{j<i} H_j W_j).  Images of one size, and images at image_size (the
+ *            loaded table, no resample), are valid calls.
+ *   vec      [n, projection_dim], as in the other pooled forms.
+ *   out      ragged, item-major: item i is T_i - skip rows of width elements, T_i = (H_i/P)(W_i/P) + 1, skip = 1 with NO_CLS, width =
+ *            hidden_size or projection_dim; it starts at byte sum_{j<i} (T_j - skip) * width * element size (16-byte aligned, as every
+ *            CLIP width is a multiple of 8).  layer, flags and out_type are those of clip_b200_image_tokens; the ATTENTION flags are
+ *            refused.
+ * Item i's outputs equal, byte for byte, those of image i passed alone to clip_b200_image_encode_device_hw /
+ * clip_b200_image_tokens_device_hw with the same arguments, whatever the other images, their order and how the call is split into
+ * passes: no value of one image reaches another image's outputs, and an image holding NaN or Inf leaves the others' bits unchanged.
+ * A pass holds the longest prefix of the remaining images that fits the workspace (sized for micro_batch images of the native size,
+ * as for the *_hw forms): its rows, patch rows and image count.
+ * Arguments are checked in this order, the first fault refused with a message in clip_b200_last_error(): 1. a null context; 2. the
+ * vision tower; 3. device forms: each image's size (the message names the first bad image; skipped while heights or widths is NULL);
+ * 4. n == 0 (a NULL batch is an empty one) returns true; 5. null pointers: host input and output, device pixels and output, then
+ * heights and widths; 6. host forms: each image's pixels and size; 7. tokens: the request, as clip_b200_image_tokens_hw refuses it,
+ * then ATTENTION; 8. an image whose rows alone exceed the workspace (the *_hw message, with the image's index).
+ * Host forms: devices mode (CLIP_B200_DEVICES) shards the images as clip_image_batch_encode does (by count); each pass's rows are
+ * copied to the host before the next pass runs. */
+bool clip_b200_image_batch_encode_mixed(const struct clip_ctx * ctx, const struct clip_image_f32_batch * imgs, float * vec, bool normalize);
+bool clip_b200_image_encode_device_mixed(const struct clip_ctx * ctx, const void * d_pixels, size_t n, const int * heights,
+                                         const int * widths, void * d_vec, bool normalize);
+bool clip_b200_image_tokens_mixed(const struct clip_ctx * ctx, const struct clip_image_f32_batch * imgs, int layer, int flags,
+                                  int out_type, void * out);
+bool clip_b200_image_tokens_device_mixed(const struct clip_ctx * ctx, const void * d_pixels, size_t n, const int * heights,
+                                         const int * widths, int layer, int flags, int out_type, void * d_out);
+
 /* Several layers' token rows from ONE forward pass of a tower (HF output_hidden_states returns all n_layer + 1; multi-layer VLM
  * connectors read 3 or 4 vision layers; SDXL reads layer -2 raw and the projected EOT row of layer -1 of the same text pass).
  *   layers[j], flags[j]  entry j: a layer and CLIP_B200_TOKENS_* flags exactly as `layer` / `flags` of the single-layer calls above.
@@ -537,6 +569,11 @@ int clip_b200_debug_attention(int operand_bf16, int nseq, int T, int H, int caus
  * (the legacy kernel is head_dim 64 only). */
 int clip_b200_debug_attention_hd(int operand_bf16, int nseq, int T, int H, int head_dim, int causal, int use_legacy, const float * qkv,
                                  float * out, float * ms);
+/* The variable-length instance behind the *_mixed calls: nseq non-causal sequences of lens[s] rows packed back to back, qkv
+ * [sum lens, 3*H*head_dim] and out [sum lens, H*head_dim], laid out and padded as for clip_b200_debug_attention_hd.  The qkv rows past
+ * the last sequence and 128 guard rows after the output are poisoned (0xFF).  Returns 2 for bad arguments, 5 for a launch or kernel
+ * error, 6 if a guard row was written. */
+int clip_b200_debug_attention_mixed(int operand_bf16, int nseq, const int * lens, int H, int head_dim, const float * qkv, float * out);
 /* The attention probabilities of the same qkv (the kernel behind CLIP_B200_TOKENS_ATTENTION): out [nseq, H, R, T] with R = T, or 1
  * with cls_row (query row 0 only), of out_type (0 fp32, 1 fp16, 2 bf16: raw 16-bit values, not widened).  Runs on device 0.  Returns
  * 2 for bad arguments (head_dim other than 64 / 80 / 104, a non-positive size, an unknown out_type), 5 if the kernel wrote into the
