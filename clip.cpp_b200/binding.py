@@ -97,6 +97,8 @@ EXTENSION_SYMBOLS = [
     # images of different sizes in one call (variable-length attention)
     "clip_b200_image_batch_encode_mixed", "clip_b200_image_encode_device_mixed", "clip_b200_image_tokens_mixed",
     "clip_b200_image_tokens_device_mixed", "clip_b200_debug_attention_mixed",
+    # inverted-file index over 16-bit databases
+    "clip_b200_ivf_train_16", "clip_b200_ivf_build_16", "clip_b200_ivf_search_16",
 ]
 
 # include/clip_b200.h: output types and flags of the *_tokens entry points
@@ -290,6 +292,12 @@ class ClipLib:
             L.clip_b200_topk_search_b1.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, ip, ip, fp, ipp]
             L.clip_b200_topk_rescore.restype = C.c_bool
             L.clip_b200_topk_rescore.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, ip, ip, ipp, ip, ip, fp, ipp]
+            L.clip_b200_ivf_train_16.restype = C.c_bool
+            L.clip_b200_ivf_train_16.argtypes = [vp, vp, C.c_size_t, ip, ip, ip, ip, vp]
+            L.clip_b200_ivf_build_16.restype = C.c_bool
+            L.clip_b200_ivf_build_16.argtypes = [vp, vp, C.c_size_t, ip, ip, vp, ip, vp, vp, vp]
+            L.clip_b200_ivf_search_16.restype = C.c_bool
+            L.clip_b200_ivf_search_16.argtypes = [vp, vp, C.c_size_t, ip, ip, vp, ip, vp, vp, vp, C.c_size_t, ip, ip, fp, ipp]
             L.clip_b200_zero_shot_images.restype = C.c_bool
             L.clip_b200_zero_shot_images.argtypes = [vp, ip, C.POINTER(clip_image_f32_batch), C.POINTER(clip_tokens), C.c_size_t,
                                                      C.c_bool, ip, fp, ipp]

@@ -88,7 +88,8 @@ struct Scope {
         }
     }
 };
-enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4, K_POS_RESAMPLE = 5, K_ATTN_PROBS = 6, K_KNN16 = 7, K_KNN_I8 = 8, K_KNN_B1 = 9, K_RESCORE = 10 };
+enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4, K_POS_RESAMPLE = 5, K_ATTN_PROBS = 6, K_KNN16 = 7, K_KNN_I8 = 8, K_KNN_B1 = 9, K_RESCORE = 10, K_IVF_SCAN = 11,
+       K_IVF_LAYOUT = 12 };
 
 // ---- tensor lookup helpers ---------------------------------------------------------------------------------
 const GgufTensor* need(const GgufFile& g, const std::string& name) {
@@ -1839,7 +1840,7 @@ static bool ensure_cand(clip_ctx* c, size_t count) {
 // that make their databases.  Each form fills one and calls search_call, so every form checks its arguments in the same order
 // (include/clip_b200.h), and the searches run the same pass driver.
 struct SearchCall {
-    enum Kind { SCORE, KNN16, KNN_I8, KNN_B1, RESCORE, ROWS16, ROWS_I8, ROWS_B1 };
+    enum Kind { SCORE, KNN16, KNN_I8, KNN_B1, RESCORE, ROWS16, ROWS_I8, ROWS_B1, IVF_TRAIN, IVF_BUILD, IVF_SEARCH };
     const char* who;                              // the public name, for messages
     Kind kind;
     const void* q = nullptr;                      // queries [nq, dim]; a row form: its f32 source rows [nq, dim]
@@ -1857,6 +1858,14 @@ struct SearchCall {
     bool softmax = false;                         // SCORE: rank p = (exp(s) + 1e-9) / sum over the row instead of s
     float* scores = nullptr;                      // host outputs [nq, that top_k]
     int* indices = nullptr;
+    // IVF_*: q holds the training rows, the database rows or the queries, nq their count; db is the list-ordered rows [ndb, dim]
+    // (IVF_BUILD writes them, with ndb = nq)
+    const void* cent = nullptr;                   // centroids [n_lists, dim] (IVF_TRAIN writes them)
+    int* offsets = nullptr;                       // [n_lists + 1] and [ndb]: IVF_BUILD writes them, IVF_SEARCH reads them
+    int* ids = nullptr;
+    int n_lists = 0;
+    int iters = 0;                                // IVF_TRAIN: n_iter; IVF_SEARCH: nprobe
+    bool ivf() const { return kind >= IVF_TRAIN; }
     bool search() const { return kind <= RESCORE; }
     bool knn() const { return kind == KNN16 || kind == KNN_I8 || kind == KNN_B1; }
 };
@@ -1967,6 +1976,248 @@ static bool search_locked(clip_ctx* c, const SearchCall& a) {
     return true;
 }
 
+// ---- the inverted-file index (clip_b200_ivf_*) ---------------------------------------------------------------------------------------
+// Carve the IVF arena into pieces of the given byte sizes, each 256-byte aligned, growing it first if it is too small.
+static bool ivf_arena(clip_ctx* c, std::initializer_list<size_t> sizes, std::initializer_list<void**> out) {
+    size_t total = 0;
+    for (size_t b : sizes) total += (b + 255) / 256 * 256;
+    if (!ensure_buf(c, &c->d_ivf, &c->d_ivf_cap, std::max<size_t>(total, 256))) return false;
+    size_t o = 0;
+    auto it = out.begin();
+    for (size_t b : sizes) { **it++ = c->d_ivf + o; o += (b + 255) / 256 * 256; }
+    return true;
+}
+
+// The list of each of the n rows x [n, dim]: K10 with top_k = 1 over the centroids, kept on the device through the merge, one
+// index per row to the host.  Blocks of 32768 rows, the merge grid's row limit.
+static bool ivf_assign(clip_ctx* c, const SearchCall& a, const void* x, size_t n, std::vector<int>& list) {
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
+    const KOp op = a.type == CLIP_B200_OUT_BF16 ? KOp::BF16 : KOp::F16;
+    list.resize(n);
+    for (size_t r0 = 0; r0 < n; r0 += 32768) {
+        const int rows = (int)std::min<size_t>(32768, n - r0);
+        const KnnPlan pl = knn_plan(rows, a.n_lists, 1, sms);
+        if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * pl.buf_entries) || !ensure_cand(c, (size_t)rows * pl.parts)) return false;
+        {
+            Scope s(c, K_KNN16);
+            const cudaError_t e = launch_knn(op, (const uint8_t*)x + r0 * a.dim * 2, nullptr, rows, a.cent, nullptr, a.n_lists, a.dim, 1, pl,
+                                             c->d_knn, c->d_cand_v[0], c->d_cand_i[0], pl.parts, c->stream);
+            if (e != cudaSuccess) { set_err(std::string(a.who) + ": launch: " + cudaGetErrorString(e)); return false; }
+        }
+        const int cur = merge_candidates(c, rows, pl.parts, pl.parts, 1);
+        CK(cudaMemcpy2DAsync(list.data() + r0, 4, c->d_cand_i[cur], (size_t)pl.parts * 4, 4, rows, cudaMemcpyDeviceToHost, c->stream));
+    }
+    CK(cudaStreamSynchronize(c->stream));
+    return true;
+}
+
+// The layout of an assignment: a counting sort, stable by row index.  off [n_lists + 1], ids [n].
+static void ivf_layout(const std::vector<int>& list, int n_lists, std::vector<int>& off, std::vector<int>& ids) {
+    off.assign(n_lists + 1, 0);
+    for (int l : list) off[l + 1]++;
+    for (int l = 0; l < n_lists; l++) off[l + 1] += off[l];
+    std::vector<int> pos(off.begin(), off.end() - 1);
+    ids.resize(list.size());
+    for (size_t i = 0; i < list.size(); i++) ids[pos[list[i]]++] = (int)i;
+}
+
+// k-means: initial centroids gathered from rows floor(i n / n_lists), then per iteration an assignment, its layout and the update
+// kernels (fp64 sums over chunks of IVF_CHUNK members, combined in chunk order).
+constexpr int IVF_CHUNK = 512;
+static bool ivf_train_locked(clip_ctx* c, const SearchCall& a) {
+    const size_t n = a.nq;
+    const int L = a.n_lists;
+    void* cent = const_cast<void*>(a.cent);
+    std::vector<int> list, off, ids, chunk_begin(L + 1);
+    std::vector<int2> chunks;
+    ids.resize(L);
+    for (int i = 0; i < L; i++) ids[i] = (int)((size_t)i * n / L);
+    {
+        int* d_init = nullptr;
+        if (!ivf_arena(c, {(size_t)L * 4}, {(void**)&d_init})) return false;
+        CK(cudaMemcpyAsync(d_init, ids.data(), (size_t)L * 4, cudaMemcpyHostToDevice, c->stream));
+        Scope s(c, K_IVF_LAYOUT);
+        launch_gather_rows16(a.q, d_init, L, a.dim, cent, c->stream);
+    }
+    for (int it = 0; it < a.iters; it++) {
+        if (!ivf_assign(c, a, a.q, n, list)) return false;
+        ivf_layout(list, L, off, ids);
+        chunks.clear();
+        for (int l = 0; l < L; l++) {
+            for (int b = off[l]; b < off[l + 1]; b += IVF_CHUNK) chunks.push_back(make_int2(b, std::min(b + IVF_CHUNK, off[l + 1])));
+            chunk_begin[l + 1] = (int)chunks.size();
+        }
+        int *d_ids = nullptr, *d_off = nullptr, *d_cb = nullptr;
+        int2* d_ch = nullptr;
+        double* d_part = nullptr;
+        if (!ivf_arena(c, {n * 4, (size_t)(L + 1) * 4, (size_t)(L + 1) * 4, chunks.size() * 8, chunks.size() * a.dim * 8},
+                       {(void**)&d_ids, (void**)&d_off, (void**)&d_cb, (void**)&d_ch, (void**)&d_part})) return false;
+        CK(cudaMemcpyAsync(d_ids, ids.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_off, off.data(), (size_t)(L + 1) * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_cb, chunk_begin.data(), (size_t)(L + 1) * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_ch, chunks.data(), chunks.size() * 8, cudaMemcpyHostToDevice, c->stream));
+        Scope s(c, K_IVF_LAYOUT);
+        launch_ivf_update(a.type == CLIP_B200_OUT_BF16, a.q, a.dim, d_ids, d_ch, (int)chunks.size(), d_cb, d_off, L, d_part, cent, c->stream);
+        CK(cudaGetLastError());
+    }
+    CK(cudaStreamSynchronize(c->stream));
+    return true;
+}
+
+static bool ivf_build_locked(clip_ctx* c, const SearchCall& a) {
+    std::vector<int> list, off, ids;
+    if (!ivf_assign(c, a, a.q, a.nq, list)) return false;
+    ivf_layout(list, a.n_lists, off, ids);
+    CK(cudaMemcpyAsync(a.offsets, off.data(), off.size() * 4, cudaMemcpyHostToDevice, c->stream));
+    CK(cudaMemcpyAsync(a.ids, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice, c->stream));
+    {
+        Scope s(c, K_IVF_LAYOUT);
+        launch_gather_rows16(a.q, a.ids, a.nq, a.dim, const_cast<void*>(a.db), c->stream);
+    }
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(c->stream));
+    return true;
+}
+
+// Search, per block of queries: the probes (K10 top-nprobe over the centroids, to the host), the host plan of the fine scan's work
+// units (include/clip_b200.h, clip_b200_ivf_search_16), the pairs' query rows gathered, K10's IVF instance, the merge.
+static bool ivf_search_locked(clip_ctx* c, const SearchCall& a, const std::vector<int>& off) {
+    const int L = a.n_lists, np = std::min(a.iters, L), w = (int)std::min<size_t>(a.top_k, a.ndb), KB = knn_tile_rows();
+    const bool bf = a.type == CLIP_B200_OUT_BF16;
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
+    const size_t QB = std::min<size_t>(32768, std::max<size_t>(1, ((size_t)1 << 24) / ((size_t)(w + 2 * KB) * np)));
+    std::vector<int> probes, cnt(L), pstart(L + 1), fill(L), pair_q, runs;
+    std::vector<size_t> slot;
+    std::vector<IvfUnit> units;
+    for (size_t r0 = 0; r0 < a.nq; r0 += QB) {
+        const int rows = (int)std::min(QB, a.nq - r0);
+        const uint8_t* q = (const uint8_t*)a.q + r0 * a.dim * 2;
+        // coarse: the best np lists of each query, best first
+        const KnnPlan pl = knn_plan(rows, L, np, sms);
+        if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * pl.buf_entries) || !ensure_cand(c, (size_t)rows * pl.parts * np)) return false;
+        {
+            Scope s(c, K_KNN16);
+            const cudaError_t e = launch_knn(bf ? KOp::BF16 : KOp::F16, q, nullptr, rows, a.cent, nullptr, L, a.dim, np, pl, c->d_knn,
+                                             c->d_cand_v[0], c->d_cand_i[0], (size_t)pl.parts * np, c->stream);
+            if (e != cudaSuccess) { set_err(std::string(a.who) + ": launch: " + cudaGetErrorString(e)); return false; }
+        }
+        const int pc = merge_candidates(c, rows, (size_t)pl.parts * np, pl.parts, np);
+        probes.resize((size_t)rows * np);
+        CK(cudaMemcpy2DAsync(probes.data(), (size_t)np * 4, c->d_cand_i[pc], (size_t)pl.parts * np * 4, (size_t)np * 4, rows,
+                             cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        // the plan: pairs (query, probed non-empty list) grouped by list, stable by query
+        std::fill(cnt.begin(), cnt.end(), 0);
+        for (int l : probes) if (off[l + 1] > off[l]) cnt[l]++;
+        int lists = 0;
+        for (int l = 0; l < L; l++) { pstart[l + 1] = pstart[l] + cnt[l]; lists += cnt[l] > 0; }
+        const int P = pstart[L];
+        pair_q.resize(P);
+        std::copy(pstart.begin(), pstart.end() - 1, fill.begin());
+        for (int r = 0; r < rows; r++)
+            for (int j = 0; j < np; j++) { const int l = probes[(size_t)r * np + j]; if (off[l + 1] > off[l]) pair_q[fill[l]++] = r; }
+        // query tile: the least 8 nt >= the mean pairs per probed list (at most 128); row ranges of R rows so that about 4 units per SM
+        const int mean = lists ? (P + lists - 1) / lists : 1;
+        int nt = 1;
+        while (8 * nt < std::min(mean, 128)) nt <<= 1;
+        const int N = 8 * nt;
+        size_t work = 0;
+        for (int l = 0; l < L; l++) work += (size_t)((cnt[l] + N - 1) / N) * (off[l + 1] - off[l]);
+        const size_t per = (work + 4 * (size_t)sms - 1) / (4 * (size_t)sms);
+        const int R = (int)std::min<size_t>((size_t)1 << 30, std::max<size_t>(KB, (per + KB - 1) / KB * KB));
+        units.clear();
+        for (int l = 0; l < L; l++)
+            for (int j = 0; j < cnt[l]; j += N)
+                for (int b = off[l], r = 0; b < off[l + 1]; b += R, r++)
+                    units.push_back(IvfUnit{pstart[l] + j, std::min(N, cnt[l] - j), b, (int)std::min<int64_t>((int64_t)b + R, off[l + 1]), r});
+        // run slots: query r's runs in probe order, one per row range of each probed list
+        runs.assign(rows, 0);
+        int runs_max = 1;
+        for (int r = 0; r < rows; r++) {
+            for (int j = 0; j < np; j++) { const int l = probes[(size_t)r * np + j]; runs[r] += (off[l + 1] - off[l] + R - 1) / R; }
+            runs_max = std::max(runs_max, runs[r]);
+        }
+        const size_t cand_ld = (size_t)runs_max * w;
+        slot.resize(P);
+        std::copy(pstart.begin(), pstart.end() - 1, fill.begin());
+        for (int r = 0; r < rows; r++)
+            for (int j = 0, run = 0; j < np; j++) {
+                const int l = probes[(size_t)r * np + j], nr = (off[l + 1] - off[l] + R - 1) / R;
+                if (nr) slot[fill[l]++] = (size_t)r * cand_ld + (size_t)run * w;
+                run += nr;
+            }
+        int* d_pq = nullptr;
+        IvfUnit* d_units = nullptr;
+        size_t* d_slot = nullptr;
+        void* d_pairs = nullptr;
+        if (!ivf_arena(c, {(size_t)P * 4, units.size() * sizeof(IvfUnit), (size_t)P * 8, (size_t)P * a.dim * 2},
+                       {(void**)&d_pq, (void**)&d_units, (void**)&d_slot, &d_pairs})) return false;
+        const size_t buf = units.size() * N * (size_t)(w + 2 * KB);
+        if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * buf) || !ensure_cand(c, (size_t)rows * cand_ld)) return false;
+        CK(cudaMemcpyAsync(d_pq, pair_q.data(), (size_t)P * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_units, units.data(), units.size() * sizeof(IvfUnit), cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_slot, slot.data(), (size_t)P * 8, cudaMemcpyHostToDevice, c->stream));
+        {
+            Scope s(c, K_OTHER);
+            launch_gather_rows16(q, d_pq, P, a.dim, d_pairs, c->stream);
+            launch_fill_cand(c->d_cand_v[0], c->d_cand_i[0], (size_t)rows * cand_ld, c->stream);
+        }
+        {
+            Scope s(c, K_IVF_SCAN);
+            const cudaError_t e = launch_knn_ivf(bf, d_pairs, P, a.db, (int)a.ndb, a.dim, w, nt, d_units, (int)units.size(), d_slot, a.ids,
+                                                 c->d_knn, c->d_cand_v[0], c->d_cand_i[0], c->stream);
+            if (e != cudaSuccess) { set_err(std::string(a.who) + ": launch: " + cudaGetErrorString(e)); return false; }
+        }
+        const int cur = merge_candidates(c, rows, cand_ld, runs_max, w);
+        float* os = a.scores + r0 * w;
+        int* oi = a.indices + r0 * w;
+        CK(cudaMemcpy2DAsync(os, (size_t)w * 4, c->d_cand_v[cur], cand_ld * 4, (size_t)w * 4, rows, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpy2DAsync(oi, (size_t)w * 4, c->d_cand_i[cur], cand_ld * 4, (size_t)w * 4, rows, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        for (size_t e = 0; e < (size_t)rows * w; e++)
+            if (oi[e] == 0x7fffffff) { oi[e] = -1; os[e] = -INFINITY; }
+    }
+    CK(cudaGetLastError());
+    return true;
+}
+
+// The IVF forms past the counts: empty calls, pointers, then the locked work.  IVF_SEARCH reads d_offsets first and refuses an index
+// whose offsets do not run non-decreasing from 0 to n_db, so a malformed index cannot send the scan out of d_rows.
+static bool ivf_call(clip_ctx* c, SearchCall& a) {
+    const std::string who = a.who;
+    const SearchCall::Kind kind = a.kind;
+    if (kind == SearchCall::IVF_TRAIN && a.nq < (size_t)a.n_lists) { set_err(who + ": n_train must be at least n_lists"); return false; }
+    if (kind == SearchCall::IVF_SEARCH && (a.nq == 0 || a.ndb == 0)) return true;
+    const bool empty_build = kind == SearchCall::IVF_BUILD && a.nq == 0;
+    // 16-byte aligned: the rows and centroids (TMA, 16-byte loads); 4-byte aligned: offsets and ids
+    const void* p16[3] = {a.q, a.cent, a.db};
+    const int n16 = empty_build ? 0 : kind == SearchCall::IVF_TRAIN ? 2 : 3;
+    for (int i = 0; i < n16; i++)
+        if (!p16[i] || (uintptr_t)p16[i] % 16) { set_err(who + ": null or not 16-byte aligned device pointer"); return false; }
+    const int* p4[2] = {a.offsets, a.ids};
+    const int n4 = kind == SearchCall::IVF_TRAIN ? 0 : empty_build ? 1 : 2;
+    for (int i = 0; i < n4; i++)
+        if (!p4[i] || (uintptr_t)p4[i] % 4) { set_err(who + ": null or not 4-byte aligned d_offsets or d_ids"); return false; }
+    if (kind == SearchCall::IVF_SEARCH && (!a.scores || !a.indices)) { set_err(who + ": null output"); return false; }
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    if (empty_build) {
+        CK(cudaMemsetAsync(a.offsets, 0, (size_t)(a.n_lists + 1) * 4, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        return true;
+    }
+    if (kind == SearchCall::IVF_TRAIN) return ivf_train_locked(c, a);
+    if (kind == SearchCall::IVF_BUILD) return ivf_build_locked(c, a);
+    std::vector<int> off(a.n_lists + 1);
+    CK(cudaMemcpy(off.data(), a.offsets, off.size() * 4, cudaMemcpyDeviceToHost));
+    bool ok = off[0] == 0 && (size_t)off[a.n_lists] == a.ndb;
+    for (int l = 0; ok && l < a.n_lists; l++) ok = off[l + 1] >= off[l];
+    if (!ok) { set_err(who + ": d_offsets must run non-decreasing from 0 to n_db"); return false; }
+    return ivf_search_locked(c, a, off);
+}
+
 // Every form of the family: the arguments checked in one order, the first fault refused (include/clip_b200.h), then the search pass or
 // the row kernel.
 static bool search_call(const clip_ctx* cctx, SearchCall a) {
@@ -1974,15 +2225,15 @@ static bool search_call(const clip_ctx* cctx, SearchCall a) {
     const std::string who = a.who;
     const SearchCall::Kind kind = a.kind;
     if (!c) { set_err(who + ": null context"); return false; }
-    if ((kind == SearchCall::KNN16 || kind == SearchCall::ROWS16) && a.type != CLIP_B200_OUT_F16 && a.type != CLIP_B200_OUT_BF16) {
-        set_err(who + (kind == SearchCall::KNN16 ? ": in_type" : ": out_type") + " must be CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16");
+    if ((kind == SearchCall::KNN16 || kind == SearchCall::ROWS16 || a.ivf()) && a.type != CLIP_B200_OUT_F16 && a.type != CLIP_B200_OUT_BF16) {
+        set_err(who + (kind == SearchCall::ROWS16 ? ": out_type" : ": in_type") + " must be CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16");
         return false;
     }
     if (kind == SearchCall::RESCORE && a.type != CLIP_B200_OUT_F32 && a.type != CLIP_B200_OUT_F16 && a.type != CLIP_B200_OUT_BF16) {
         set_err(who + ": in_type must be CLIP_B200_OUT_F32, CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16");
         return false;
     }
-    const int step = kind == SearchCall::KNN16 || kind == SearchCall::RESCORE ? 8 : kind == SearchCall::ROWS16 ? 4
+    const int step = kind == SearchCall::KNN16 || kind == SearchCall::RESCORE || a.ivf() ? 8 : kind == SearchCall::ROWS16 ? 4
                    : kind == SearchCall::KNN_B1 || kind == SearchCall::ROWS_B1 ? 128 : 16;     // SCORE's dim is the model's
     if (kind != SearchCall::SCORE && (a.dim < step || a.dim > 2048 || a.dim % step)) {
         set_err(who + ": dim must be a multiple of " + std::to_string(step) + " in [" + std::to_string(step) + ", 2048]");
@@ -1992,11 +2243,17 @@ static bool search_call(const clip_ctx* cctx, SearchCall a) {
         if (a.n_cand < 1 || a.n_cand > 2048) { set_err(who + ": n_cand must be in [1, 2048]"); return false; }
         if (a.top_k < 1 || a.top_k > a.n_cand) { set_err(who + ": top_k must be in [1, n_cand]"); return false; }
     }
-    if (a.knn() && (a.top_k < 1 || a.top_k > 1024)) { set_err(who + ": top_k must be in [1, 1024]"); return false; }
+    if (a.ivf() && (a.n_lists < 1 || a.n_lists > 65536)) { set_err(who + ": n_lists must be in [1, 65536]"); return false; }
+    if (kind == SearchCall::IVF_TRAIN && (a.iters < 1 || a.iters > 1000)) { set_err(who + ": n_iter must be in [1, 1000]"); return false; }
+    if (kind == SearchCall::IVF_SEARCH && (a.iters < 1 || a.iters > 1024)) { set_err(who + ": nprobe must be in [1, 1024]"); return false; }
+    if ((a.knn() || kind == SearchCall::IVF_SEARCH) && (a.top_k < 1 || a.top_k > 1024)) { set_err(who + ": top_k must be in [1, 1024]"); return false; }
     if (a.nq > 0x7fffffffull || a.ndb > 0x7fffffffull) {
-        set_err(who + (a.search() ? ": n_queries and n_db must be below 2^31" : ": n must be below 2^31"));
+        set_err(who + (a.search() || kind == SearchCall::IVF_SEARCH ? ": n_queries and n_db must be below 2^31"
+                       : kind == SearchCall::IVF_TRAIN ? ": n_train must be below 2^31" : kind == SearchCall::IVF_BUILD ? ": n_db must be below 2^31"
+                       : ": n must be below 2^31"));
         return false;
     }
+    if (a.ivf()) return ivf_call(c, a);
     if (a.nq == 0 || (a.search() && a.ndb == 0)) return true;
     // the device pointers the kind reads or writes: q and db, then the int8 forms' scales or ROWS_B1's optional centre.  K10, K11, K12
     // and the row kernels load and store 16 bytes at a time; the fp32 kernels read single floats.
@@ -2089,6 +2346,31 @@ bool clip_b200_topk_rescore(const struct clip_ctx* cctx, const void* d_queries, 
     SearchCall a{"clip_b200_topk_rescore", SearchCall::RESCORE};
     a.q = d_queries; a.nq = n_queries; a.db = d_db; a.ndb = n_db; a.dim = dim; a.type = in_type; a.cand = cand; a.n_cand = n_cand;
     a.top_k = top_k; a.scores = scores; a.indices = indices;
+    return search_call(cctx, a);
+}
+
+bool clip_b200_ivf_train_16(const struct clip_ctx* cctx, const void* d_train, size_t n_train, int dim, int in_type, int n_lists, int n_iter,
+                            void* d_centroids) {
+    SearchCall a{"clip_b200_ivf_train_16", SearchCall::IVF_TRAIN};
+    a.q = d_train; a.nq = n_train; a.dim = dim; a.type = in_type; a.n_lists = n_lists; a.iters = n_iter; a.cent = d_centroids;
+    return search_call(cctx, a);
+}
+
+bool clip_b200_ivf_build_16(const struct clip_ctx* cctx, const void* d_db, size_t n_db, int dim, int in_type, const void* d_centroids,
+                            int n_lists, int* d_offsets, int* d_ids, void* d_rows) {
+    SearchCall a{"clip_b200_ivf_build_16", SearchCall::IVF_BUILD};
+    a.q = d_db; a.nq = n_db; a.dim = dim; a.type = in_type; a.cent = d_centroids; a.n_lists = n_lists; a.offsets = d_offsets; a.ids = d_ids;
+    a.db = d_rows;
+    return search_call(cctx, a);
+}
+
+bool clip_b200_ivf_search_16(const struct clip_ctx* cctx, const void* d_queries, size_t n_queries, int dim, int in_type, const void* d_centroids,
+                             int n_lists, const int* d_offsets, const int* d_ids, const void* d_rows, size_t n_db, int nprobe, int top_k,
+                             float* scores, int* indices) {
+    SearchCall a{"clip_b200_ivf_search_16", SearchCall::IVF_SEARCH};
+    a.q = d_queries; a.nq = n_queries; a.dim = dim; a.type = in_type; a.cent = d_centroids; a.n_lists = n_lists;
+    a.offsets = const_cast<int*>(d_offsets); a.ids = const_cast<int*>(d_ids); a.db = d_rows; a.ndb = n_db; a.iters = nprobe; a.top_k = top_k;
+    a.scores = scores; a.indices = indices;
     return search_call(cctx, a);
 }
 

@@ -107,7 +107,7 @@ void launch_topk_stage(const float* vals, const int* in_idx, size_t ld, int rows
 // Writes each query's best kk (<= 1024) per database partition, sorted, to out[query, partition * kk ...] (row stride out_ld >=
 // parts * kk); padding entries are (-inf, INT_MAX).  The plan fixes the query tile (8 nt queries), the partitions and the scratch
 // `buf` of buf_entries (value, index) pairs the launch needs.
-enum class KOp { F16, BF16, S8 };
+enum class KOp { F16, BF16, S8, F16_IVF, BF16_IVF };      // the IVF instances: launch_knn_ivf only
 struct KnnPlan {
     int nt, parts, rows_per_part, grid, cap;
     size_t buf_entries;
@@ -115,6 +115,23 @@ struct KnnPlan {
 KnnPlan knn_plan(int nq, int ndb, int kk, int sms);
 cudaError_t launch_knn(KOp op, const void* q, const float* qs, int nq, const void* db, const float* xs, int ndb, int dim, int kk,
                        const KnnPlan& pl, void* buf, float* out_v, int* out_i, size_t out_ld, cudaStream_t st);
+// K10's IVF instances (kernel class 11): CTA u runs unit units[u], pairs p0 .. p0 + np - 1 (rows of pq [npairs, dim], the gathered
+// query of each (query, probed list) pair) against stored rows row_begin .. row_end - 1 of rows [ndb, dim], all in one list.  Pair
+// p's best kk of the unit go, sorted, to out[slot[p] + range * kk ...] with each row's original index ids[stored position]; padding
+// is (-inf, INT_MAX).  Query tile 8 nt; scratch `buf` of nunits * 8 nt * (kk + 256) (value, index) pairs.
+struct IvfUnit { int p0, np, row_begin, row_end, range; };
+cudaError_t launch_knn_ivf(bool bf, const void* pq, int npairs, const void* rows, int ndb, int dim, int kk, int nt, const IvfUnit* units,
+                           int nunits, const size_t* slot, const int* ids, void* buf, float* out_v, int* out_i, cudaStream_t st);
+int knn_tile_rows();                                                    // K10's KB: rows per tile
+// dst[p] = src[idx[p]], p < n, rows of dim 16-bit elements (dim % 8 == 0), 16-byte aligned; 64-bit offsets
+void launch_gather_rows16(const void* src, const int* idx, size_t n, int dim, void* dst, cudaStream_t st);
+// (v, i)[0 .. n) = (-inf, INT_MAX): the candidate matrix's unused runs
+void launch_fill_cand(float* v, int* i, size_t n, cudaStream_t st);
+// one k-means update (clip_b200_ivf_train_16's rule): x [n, dim] 16-bit (bf: bf16) in list order through ids; chunks[c] = (begin, end)
+// positions in ids, chunk_begin[l] .. chunk_begin[l + 1] - 1 the chunks of list l, offsets [n_lists + 1]; part [nchunks, dim] fp64
+// scratch.  Rewrites cent [n_lists, dim] in place, keeping the centroid of an empty list or of a zero mean.
+void launch_ivf_update(bool bf, const void* x, int dim, const int* ids, const int2* chunks, int nchunks, const int* chunk_begin,
+                       const int* offsets, int n_lists, double* part, void* cent, cudaStream_t st);
 // Q8 quantiser: x [n, dim] f32 -> codes [n, dim] int8 and scales [n] f32 by the rule of clip_b200_rows_to_int8 (clip_b200.h).
 // dim % 16 == 0, dim <= 2048, 16-byte aligned pointers; 64-bit offsets, so n * dim may pass 2^32.
 void launch_rows_to_int8(const float* x, int n, int dim, void* codes, float* scales, cudaStream_t st);

@@ -113,6 +113,7 @@ struct clip_ctx {
     float* d_cand_v[2] = {nullptr, nullptr}; int* d_cand_i[2] = {nullptr, nullptr}; size_t d_cand_cap = 0;
     uint32_t* d_knn = nullptr; size_t d_knn_cap = 0;    // clip_b200_topk_search_16: K10's per-CTA candidate buffers, 2 words per entry
     int* d_rcand = nullptr; size_t d_rcand_cap = 0;     // clip_b200_topk_rescore: the candidates of one block of queries
+    uint8_t* d_ivf = nullptr; size_t d_ivf_cap = 0;     // the clip_b200_ivf_* calls: host-planned tables and their scratch
     float* d_emb[2] = {nullptr, nullptr}; size_t d_emb_cap[2] = {0, 0};     // image / text embeddings kept on the device (zero-shot)
     // the last position table resampled for a non-native image size (*_hw calls): CLS row + gh*gw patch rows [T, h], grow-only
     float* pos_hw = nullptr; size_t pos_hw_cap = 0;

@@ -11,6 +11,7 @@
 // tensor-core scores and a top-k kept inside the kernel, so no score matrix ever reaches memory.  It shares the candidate order and
 // the merge stage with the fp32 path.
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <float.h>
 #include <string.h>
@@ -193,11 +194,14 @@ struct KParams {
     const float *qs, *xs;           // S8 only: query scales [nq], row scales [ndb]
     const uint4 *qb, *xb;           // K11 only: query and database bits [nq, dim / 128], [ndb, dim / 128], 16-byte words
     int dim;                        // K11 only: bits per row
+    const IvfUnit* units;           // IVF instances only: the work unit of each CTA,
+    const size_t* slot;             //   where pair p's run of range 0 starts in the candidate matrix (range r: + r * kk),
+    const int* ids;                 //   and the original index of each stored row
 };
 
 template <KOp OP, int NT>
 CB_DEVINL void knn_mma(float (&d)[4 * NT], uint64_t da, uint64_t db, uint32_t accumulate) {
-    constexpr bool BF = OP == KOp::BF16;
+    constexpr bool BF = OP == KOp::BF16 || OP == KOp::BF16_IVF;
     if constexpr (NT == 16) wgmma_ss_n128<BF>(d, da, db, accumulate);
     else if constexpr (NT == 8) wgmma_ss_n64<BF>(d, da, db, accumulate);
     else if constexpr (NT == 4) wgmma_ss_n32<BF>(d, da, db, accumulate);
@@ -270,11 +274,40 @@ CB_DEVINL void knn_finish(const KParams& p, Cand* sort_s, Cand* bufq, const int*
     }
 }
 
+// A CTA's work: queries q0 .. q0 + nqv - 1 (rows of the query map) against rows row_begin .. row_end - 1, its run written as
+// partition `part`.  K10 numbers its units from the plan; the IVF instances read them from the unit table.
+struct KnnWork { int q0, nqv, part, row_begin, row_end; };
+
+template <int NQ, bool IVF>
+CB_DEVINL KnnWork knn_work(const KParams& p) {
+    if constexpr (IVF) {
+        const IvfUnit u = p.units[blockIdx.x];
+        return KnnWork{u.p0, u.np, u.range, u.row_begin, u.row_end};
+    } else {
+        const int qt = blockIdx.x / p.parts, part = blockIdx.x - qt * p.parts;
+        const int q0 = qt * NQ, row_begin = part * p.rows_per_part;
+        return KnnWork{q0, min(NQ, p.nq - q0), part, row_begin, min(p.ndb, row_begin + p.rows_per_part)};
+    }
+}
+
+// The IVF instances' end: pair q0 + q's best kk go to its own run, p.slot[q0 + q] + part * kk, with each stored position that
+// knn_sort_keep wrote replaced by its original index (each thread rewrites the entries it wrote itself).
+CB_DEVINL void knn_finish_ivf(const KParams& p, Cand* sort_s, Cand* bufq, const int* cnt, int nqv, int q0, int part) {
+    for (int q = 0; q < nqv; q++) {
+        const size_t o = p.slot[q0 + q] + (size_t)part * p.kk;
+        knn_sort_keep(sort_s, bufq + (size_t)q * p.cap, cnt[q], p.kk, true, nullptr, nullptr, p.out_v + o, p.out_i + o);
+        for (int e = threadIdx.x; e < p.kk; e += 256) {
+            const int i = p.out_i[o + e];
+            if (i != 0x7fffffff) p.out_i[o + e] = p.ids[i];
+        }
+    }
+}
+
 template <KOp OP, int NT>
 __global__ void __launch_bounds__(KNN_THREADS, 1) knn_kernel(const __grid_constant__ KParams p) {
     using G = KnnGeo<OP, NT>;
     constexpr int NQ = G::NQ;
-    constexpr bool S8 = OP == KOp::S8;
+    constexpr bool S8 = OP == KOp::S8, IVF = OP == KOp::F16_IVF || OP == KOp::BF16_IVF;
     constexpr int KCOL = S8 ? 2 * KC : KC;                         // elements in a chunk's 128 bytes
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -287,9 +320,13 @@ __global__ void __launch_bounds__(KNN_THREADS, 1) knn_kernel(const __grid_consta
     float* qscale = reinterpret_cast<float*>(smem + G::QS_OFF);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int qt = blockIdx.x / p.parts, part = blockIdx.x - qt * p.parts;
-    const int q0 = qt * NQ, nqv = min(NQ, p.nq - q0);
-    const int row_begin = part * p.rows_per_part, row_end = min(p.ndb, row_begin + p.rows_per_part);
+    int qt = blockIdx.x / p.parts, part = blockIdx.x - qt * p.parts;
+    int q0 = qt * NQ, nqv = min(NQ, p.nq - q0);
+    int row_begin = part * p.rows_per_part, row_end = min(p.ndb, row_begin + p.rows_per_part);
+    if constexpr (IVF) {
+        const IvfUnit u = p.units[blockIdx.x];
+        q0 = u.p0; nqv = u.np; part = u.range; row_begin = u.row_begin; row_end = u.row_end;
+    }
     const int ntiles = (row_end - row_begin + KB - 1) / KB;
     if (threadIdx.x == 0) {
         for (int i = 0; i < KSTAGES; i++) { mbar_init(full + 8 * i, 1); mbar_init(empty + 8 * i, 8); }
@@ -369,7 +406,8 @@ __global__ void __launch_bounds__(KNN_THREADS, 1) knn_kernel(const __grid_consta
         }
         knn_compact<NQ>(p, sort_s, bufq, theta, cnt, flags);
     }
-    knn_finish(p, sort_s, bufq, cnt, nqv, q0, part);
+    if constexpr (IVF) knn_finish_ivf(p, sort_s, bufq, cnt, nqv, q0, part);
+    else knn_finish(p, sort_s, bufq, cnt, nqv, q0, part);
 }
 
 // ---- K11: Hamming top-k over a binary database on the tensor cores --------------------------------------------------------------
@@ -609,6 +647,74 @@ __global__ void __launch_bounds__(256) quant_b1_kernel(const float4* __restrict_
     }
 }
 
+// ---- IVF layout and k-means update -----------------------------------------------------------------------------------------------
+// Row gather: dst[p] = src[idx[p]], rows of w16 16-byte words, 64-bit offsets (n * dim * 2 may pass 2^32).
+__global__ void __launch_bounds__(256) gather_rows16_kernel(const uint4* __restrict__ src, const int* __restrict__ idx, size_t n, int w16,
+                                                            uint4* __restrict__ dst) {
+    const size_t total = n * (size_t)w16, step = (size_t)gridDim.x * 256;
+    for (size_t e = (size_t)blockIdx.x * 256 + threadIdx.x; e < total; e += step) {
+        const size_t r = e / w16, w = e - r * w16;
+        dst[e] = src[(size_t)idx[r] * w16 + w];
+    }
+}
+
+__global__ void __launch_bounds__(256) fill_cand_kernel(float* __restrict__ v, int* __restrict__ i, size_t n) {
+    const size_t step = (size_t)gridDim.x * 256;
+    for (size_t e = (size_t)blockIdx.x * 256 + threadIdx.x; e < n; e += step) { v[e] = -INFINITY; i[e] = 0x7fffffff; }
+}
+
+template <bool BF>
+CB_DEVINL double load16(const uint16_t* x, size_t e) {
+    const uint16_t h = x[e];
+    if constexpr (BF) return (double)__uint_as_float((uint32_t)h << 16);
+    else return (double)__half2float(__ushort_as_half(h));
+}
+
+// k-means sums, pass 1: chunk c = (the list-ordered members ids[begin .. end - 1]) -> part[c, dim], each feature summed in fp64 over
+// the chunk's members in order (one thread per feature, so the order is fixed).
+template <bool BF>
+__global__ void __launch_bounds__(256) ivf_chunk_sum_kernel(const uint16_t* __restrict__ x, int dim, const int* __restrict__ ids,
+                                                            const int2* __restrict__ chunks, double* __restrict__ part) {
+    const int2 ch = chunks[blockIdx.x];
+    for (int f = threadIdx.x; f < dim; f += 256) {
+        double s = 0.0;
+        for (int r = ch.x; r < ch.y; r++) s += load16<BF>(x, (size_t)ids[r] * dim + f);
+        part[(size_t)blockIdx.x * dim + f] = s;
+    }
+}
+
+// k-means sums, pass 2, one CTA per list: m = (the list's chunk sums added in chunk order) / count, then c = rne16(m / sqrt(sum m^2)),
+// in fp64, the squares summed by a fixed tree (each thread's features in order, then warps, then the eight warp sums in order).  An
+// empty list, or a mean that is exactly zero, leaves the centroid as it was.
+template <bool BF>
+__global__ void __launch_bounds__(256) ivf_update_kernel(const double* __restrict__ part, const int* __restrict__ chunk_begin,
+                                                         const int* __restrict__ offsets, int dim, uint16_t* __restrict__ cent) {
+    __shared__ double mean[2048], wsum[8];
+    const int l = blockIdx.x, count = offsets[l + 1] - offsets[l];
+    if (count == 0) return;
+    const int c0 = chunk_begin[l], c1 = chunk_begin[l + 1];
+    double sq = 0.0;
+    for (int f = threadIdx.x; f < dim; f += 256) {
+        double s = 0.0;
+        for (int c = c0; c < c1; c++) s += part[(size_t)c * dim + f];
+        const double m = s / (double)count;
+        mean[f] = m;
+        sq += m * m;
+    }
+    sq = warp_sum_d(sq);
+    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = sq;
+    __syncthreads();
+    double tot = 0.0;
+    #pragma unroll
+    for (int w = 0; w < 8; w++) tot += wsum[w];
+    if (tot == 0.0) return;
+    const double nrm = sqrt(tot);
+    for (int f = threadIdx.x; f < dim; f += 256) {
+        const double v = mean[f] / nrm;
+        cent[(size_t)l * dim + f] = BF ? __bfloat16_as_ushort(__double2bfloat16(v)) : __half_as_ushort(__double2half(v));
+    }
+}
+
 typedef CUresult (*EncodeTiledFnK)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -814,6 +920,45 @@ void launch_rows_to_binary(const float* x, int n, int dim, const float* center, 
     const unsigned grid = (unsigned)std::min<size_t>((nwords + 7) / 8, (size_t)1 << 20);
     quant_b1_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const float4*>(x), nwords, dim / 128, reinterpret_cast<const float4*>(center),
                                           reinterpret_cast<uint4*>(bits));
+}
+
+cudaError_t launch_knn_ivf(bool bf, const void* pq, int npairs, const void* rows, int ndb, int dim, int kk, int nt, const IvfUnit* units,
+                           int nunits, const size_t* slot, const int* ids, void* buf, float* out_v, int* out_i, cudaStream_t st) {
+    if (nunits <= 0) return cudaSuccess;
+    KParams p;
+    memset(&p, 0, sizeof(p));
+    if (!make_rows_map(&p.tm_db, rows, ndb, dim, KB, 2) || !make_rows_map(&p.tm_q, pq, npairs, dim, 8 * nt, 2)) return cudaErrorInvalidValue;
+    p.buf = reinterpret_cast<Cand*>(buf);
+    p.out_v = out_v; p.out_i = out_i;
+    p.nq = npairs; p.ndb = ndb;
+    p.nchunks = (dim * 2 + 127) / 128;
+    p.kk = kk; p.cap = kk + 2 * KB;
+    p.units = units; p.slot = slot; p.ids = ids;
+    return bf ? knn_launch_nt<KOp::BF16_IVF>(nt, p, (unsigned)nunits, st) : knn_launch_nt<KOp::F16_IVF>(nt, p, (unsigned)nunits, st);
+}
+
+int knn_tile_rows() { return KB; }
+
+void launch_gather_rows16(const void* src, const int* idx, size_t n, int dim, void* dst, cudaStream_t st) {
+    if (n == 0) return;
+    const int w16 = dim / 8;
+    const unsigned grid = (unsigned)std::min<size_t>((n * w16 + 255) / 256, (size_t)1 << 20);
+    gather_rows16_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const uint4*>(src), idx, n, w16, reinterpret_cast<uint4*>(dst));
+}
+
+void launch_fill_cand(float* v, int* i, size_t n, cudaStream_t st) {
+    if (n == 0) return;
+    fill_cand_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)1 << 16), 256, 0, st>>>(v, i, n);
+}
+
+void launch_ivf_update(bool bf, const void* x, int dim, const int* ids, const int2* chunks, int nchunks, const int* chunk_begin,
+                       const int* offsets, int n_lists, double* part, void* cent, cudaStream_t st) {
+    if (nchunks > 0) {
+        if (bf) ivf_chunk_sum_kernel<true><<<nchunks, 256, 0, st>>>((const uint16_t*)x, dim, ids, chunks, part);
+        else ivf_chunk_sum_kernel<false><<<nchunks, 256, 0, st>>>((const uint16_t*)x, dim, ids, chunks, part);
+    }
+    if (bf) ivf_update_kernel<true><<<n_lists, 256, 0, st>>>(part, chunk_begin, offsets, dim, (uint16_t*)cent);
+    else ivf_update_kernel<false><<<n_lists, 256, 0, st>>>(part, chunk_begin, offsets, dim, (uint16_t*)cent);
 }
 
 }  // namespace cb

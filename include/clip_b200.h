@@ -462,6 +462,65 @@ bool clip_b200_topk_search_b1(const struct clip_ctx * ctx, const void * d_q_bits
 bool clip_b200_topk_rescore(const struct clip_ctx * ctx, const void * d_queries, size_t n_queries, const void * d_db, size_t n_db,
                             int dim, int in_type, const int * cand, int n_cand, int top_k, float * scores, int * indices);
 
+/* ---- inverted-file index over a 16-bit database (FAISS IndexIVFFlat, spherical k-means) -------------------------------------
+ * k-means splits the database into n_lists lists; each row is stored with its list; a query scores the centroids and scans only
+ * its nprobe best lists.  At n_lists = 4096 and nprobe = 32 a query reads under 1 % of the rows.  The caller owns the index, four
+ * device buffers: centroids [n_lists, dim] of in_type, offsets [n_lists + 1] int32, ids [n_db] int32, rows [n_db, dim] of in_type.
+ * - Limits: in_type is CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16; dim is a multiple of 8 in [8, 2048]; n_lists in [1, 65536];
+ *   top_k in [1, 1024]; nprobe in [1, 1024], a value above n_lists meaning n_lists; n_iter in [1, 1000]; counts below 2^31.
+ *   Device pointers are 16-byte aligned, except d_offsets and d_ids, which need 4 bytes.  All three run on the context's first
+ *   GPU (in devices mode too).
+ * - Assignment: a row's list is its best centroid under clip_b200_topk_search_16's score and ranking (score descending, then the
+ *   lower list index), i.e. clip_b200_topk_search_16(row, centroids, top_k = 1).  Train and build assign alike.
+ * - Refusals, each with a message in clip_b200_last_error that starts with the function's name, in this order: null context;
+ *   in_type; dim; n_lists; n_iter / nprobe; top_k; a count >= 2^31 (train: then n_train < n_lists); then, when there is work,
+ *   null or misaligned device pointers, then null outputs.
+ * - Kernel time: the assignments and the probes are kernel class 7 (K10), the fine scan class 11, the k-means update and the
+ *   build's row gather class 12. */
+
+/* k-means (Lloyd, spherical) on the tensor cores: n_lists unit-norm centroids of in_type [n_lists, dim] to d_centroids.
+ * 1. The initial centroids are the training rows at indices floor(i * n_train / n_lists), so n_train >= n_lists is required (a
+ *    caller who wants a random start shuffles the training set).
+ * 2. Each of the n_iter iterations assigns every training row, then replaces the centroid c of each non-empty list by the mean m
+ *    of its members, L2-normalised: m_j = (fp64 sum of the members' values, exact when widened) / count in fp64, and
+ *    c_j = rne_16(m_j / sqrt(sum_j m_j^2)), in fp64, rounded once to in_type.  The sums run in a fixed order (members in row
+ *    order, in chunks of 512 whose sums are added in chunk order; the squares by a fixed tree), so a call gives the same bits
+ *    every time.  An empty list, and a list whose mean is exactly zero, keep their previous centroid.
+ * Workspace, grow-only: about n_train * 4 + (n_train / 512 + n_lists) * dim * 8 bytes, plus the K10 buffers of
+ * clip_b200_topk_search_16 at top_k = 1. */
+bool clip_b200_ivf_train_16(const struct clip_ctx * ctx, const void * d_train, size_t n_train, int dim, int in_type,
+                            int n_lists, int n_iter, void * d_centroids);
+
+/* Assign every row of d_db [n_db, dim] to its list and lay the database out list by list: d_offsets[l] .. d_offsets[l + 1] - 1 are
+ * the stored positions of list l, lists in list order, rows within a list in increasing original index; d_ids[p] is the original
+ * index at stored position p and d_rows[p] that row, byte for byte.  n_db == 0 writes n_lists + 1 zeros to d_offsets and nothing
+ * else.  Offsets of the copy are 64-bit, so n_db * dim * 2 may pass 2^32. */
+bool clip_b200_ivf_build_16(const struct clip_ctx * ctx, const void * d_db, size_t n_db, int dim, int in_type,
+                            const void * d_centroids, int n_lists, int * d_offsets, int * d_ids, void * d_rows);
+
+/* Probe the nprobe best lists of each query and return its best top_k rows, by original row index, to host [n_queries, w],
+ * w = min(top_k, n_db), row i at i * w.
+ * - The probes of query q are the best nprobe lists of clip_b200_topk_search_16(q, centroids, nprobe).  The result is the best w
+ *   rows of the union of the probed lists in clip_b200_topk_search_16's ranking: score descending, then the lower ORIGINAL index.
+ *   Each score has the bits clip_b200_topk_search_16 gives the pair (query, row): a score does not depend on the query's place in
+ *   a query tile nor on the tile's width.  A NaN score ranks last and is reported as -FLT_MAX.  When the probed lists hold fewer
+ *   than w rows, the rest of the row is (-INFINITY, -1), as clip_b200_topk_rescore pads.
+ * - Consequence: with nprobe >= n_lists the output equals clip_b200_topk_search_16 over the original database, byte for byte.
+ * - Before any device work d_offsets is read and must run non-decreasing from 0 to n_db; a malformed index is refused with a
+ *   message.  d_ids is only copied to the output, never dereferenced.  n_queries == 0 or n_db == 0 returns true and writes
+ *   nothing.
+ * - The fine scan is K10 run from a table of work units (list, up to N of its (query, list) pairs, a range of up to R of its
+ *   rows): N = 8 nt, the least power of two >= the mean pairs per probed list (8 to 128); R, a multiple of 128, so that the
+ *   units come to about 4 per SM.  Queries go in blocks of Q = min(32768, max(1, 2^24 / ((w + 256) * min(nprobe, n_lists))))
+ *   queries, P = Q * min(nprobe, n_lists) pairs at most.
+ * - Workspace, grow-only, per block: the K10 buffers of the probes (clip_b200_topk_search_16's formula at top_k = nprobe), then
+ *   U * N * (w + 256) * 8 bytes of per-unit candidates for U units (U * N < 3 P + 8 * lists probed + 512 * #SMs), P * (dim * 2 + 12)
+ *   bytes of gathered queries and tables, and 4 * Q * runs * w * 4 bytes of merge buffers, runs = the most row ranges one query
+ *   probes. */
+bool clip_b200_ivf_search_16(const struct clip_ctx * ctx, const void * d_queries, size_t n_queries, int dim, int in_type,
+                             const void * d_centroids, int n_lists, const int * d_offsets, const int * d_ids,
+                             const void * d_rows, size_t n_db, int nprobe, int top_k, float * scores, int * indices);
+
 /* Batched zero-shot labelling, the batch form of clip_zero_shot_label_image (clip.h:106-107, clip.cpp:1624-1659): n images x
  * n_labels token sequences -> scores / indices [n, top_k], best first (p = (exp(s)+1e-9)/sum over ALL labels, clip.cpp:1591-1622).
  * normalize = false reproduces the reference (un-normalised embeddings).  Works in every multi-GPU mode (see below): in devices
@@ -527,7 +586,8 @@ float    clip_b200_last_device_ms(const struct clip_ctx * ctx);    /* CUDA-event
  * 2 layernorm, 3 other, 4 the token-row kernel of the *_tokens calls, 5 the position-table resample of the *_hw calls, 6 the
  * attention-probability kernel of ATTENTION entries, 7 the 16-bit search kernel of clip_b200_topk_search_16, 8 the int8 search
  * kernel of clip_b200_topk_search_i8, 9 the binary search kernel of clip_b200_topk_search_b1, 10 the rescore kernel of
- * clip_b200_topk_rescore); *count
+ * clip_b200_topk_rescore, 11 the fine scan of clip_b200_ivf_search_16, 12 the k-means update of clip_b200_ivf_train_16 and the row
+ * gather of clip_b200_ivf_build_16); *count
  * receives the number of launches.  Enabled by env CLIP_B200_PROFILE=1. */
 float    clip_b200_kernel_ms(const struct clip_ctx * ctx, int kind, uint64_t * count);
 /* CUDA-event stopwatch on the launch stream: mark(slot 0..3), then elapsed(a, b) in ms (-1 on error) */
