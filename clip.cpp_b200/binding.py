@@ -97,6 +97,9 @@ EXTENSION_SYMBOLS = [
     # images of different sizes in one call (variable-length attention)
     "clip_b200_image_batch_encode_mixed", "clip_b200_image_encode_device_mixed", "clip_b200_image_tokens_mixed",
     "clip_b200_image_tokens_device_mixed", "clip_b200_debug_attention_mixed",
+    # token sequences of different lengths in one call (causal variable-length attention)
+    "clip_b200_text_batch_encode_packed", "clip_b200_text_encode_device_packed", "clip_b200_text_tokens_packed",
+    "clip_b200_text_tokens_device_packed", "clip_b200_debug_attention_mixed_causal",
     # inverted-file index over 16-bit databases
     "clip_b200_ivf_train_16", "clip_b200_ivf_build_16", "clip_b200_ivf_search_16",
 ]
@@ -223,6 +226,8 @@ class ClipLib:
             L.clip_b200_debug_attention_hd.argtypes = [ip, ip, ip, ip, ip, ip, ip, fp, fp, C.POINTER(C.c_float)]
             L.clip_b200_debug_attention_mixed.restype = C.c_int
             L.clip_b200_debug_attention_mixed.argtypes = [ip, ip, C.POINTER(C.c_int), ip, ip, fp, fp]
+            L.clip_b200_debug_attention_mixed_causal.restype = C.c_int
+            L.clip_b200_debug_attention_mixed_causal.argtypes = [ip, ip, C.POINTER(C.c_int), ip, ip, fp, fp]
             L.clip_b200_debug_attention_probs.restype = C.c_int
             L.clip_b200_debug_attention_probs.argtypes = [ip, ip, ip, ip, ip, ip, ip, ip, fp, vp]
             L.clip_b200_debug_gemm.restype = C.c_int
@@ -267,6 +272,14 @@ class ClipLib:
             L.clip_b200_image_tokens_mixed.argtypes = [vp, C.POINTER(clip_image_f32_batch), ip, ip, ip, vp]
             L.clip_b200_image_tokens_device_mixed.restype = C.c_bool
             L.clip_b200_image_tokens_device_mixed.argtypes = [vp, vp, C.c_size_t, intp, intp, ip, ip, ip, vp]
+            L.clip_b200_text_batch_encode_packed.restype = C.c_bool
+            L.clip_b200_text_batch_encode_packed.argtypes = [vp, C.POINTER(clip_tokens), C.c_size_t, fp, C.c_bool]
+            L.clip_b200_text_encode_device_packed.restype = C.c_bool
+            L.clip_b200_text_encode_device_packed.argtypes = [vp, vp, C.c_size_t, intp, vp, C.c_bool]
+            L.clip_b200_text_tokens_packed.restype = C.c_bool
+            L.clip_b200_text_tokens_packed.argtypes = [vp, C.POINTER(C.c_int32), C.c_size_t, intp, ip, ip, ip, vp]
+            L.clip_b200_text_tokens_device_packed.restype = C.c_bool
+            L.clip_b200_text_tokens_device_packed.argtypes = [vp, vp, C.c_size_t, intp, ip, ip, ip, vp]
             L.clip_b200_image_tokens_layers.restype = C.c_bool
             L.clip_b200_image_tokens_layers.argtypes = [vp, C.POINTER(clip_image_f32_batch), intp, intp, ip, ip, vp]
             L.clip_b200_image_tokens_layers_device.restype = C.c_bool
@@ -497,6 +510,32 @@ class ClipLib:
         if not self.lib.clip_b200_image_tokens_mixed(ctx, C.byref(batch), layer, flags, out_type, flat.ctypes.data):
             raise RuntimeError("clip_b200_image_tokens_mixed failed: " + self.last_error())
         return np.split(flat, np.cumsum(rows)[:-1])
+
+    # ---- token sequences of different lengths in one call (include/clip_b200.h: text *_packed) ----------------------------------
+    def text_batch_encode_packed(self, ctx, seqs, normalize=True) -> np.ndarray:
+        """seqs: a list of id lists / int32 arrays, each at its own length -> [n, projection_dim], packed with no padding"""
+        seqs = [np.ascontiguousarray(s, np.int32) for s in seqs]
+        arr = (clip_tokens * max(len(seqs), 1))()
+        for i, s in enumerate(seqs):
+            arr[i].data = s.ctypes.data_as(C.POINTER(C.c_int32))
+            arr[i].size = s.size
+        out = np.empty((len(seqs), self.text_hparams(ctx).projection_dim), np.float32)
+        if not self.lib.clip_b200_text_batch_encode_packed(ctx, arr, len(seqs), out.ctypes.data_as(C.POINTER(C.c_float)), normalize):
+            raise RuntimeError("clip_b200_text_batch_encode_packed failed: " + self.last_error())
+        return out
+
+    def text_tokens_packed(self, ctx, seqs, layer: int = -1, flags: int = 0, out_type: int = OUT_F32) -> list:
+        """seqs: a list of id lists / int32 arrays -> a list of [len_i, width] arrays (views of one ragged buffer)"""
+        seqs = [np.ascontiguousarray(s, np.int32) for s in seqs]
+        lens = np.array([s.size for s in seqs], np.int32)
+        ids = np.concatenate(seqs) if seqs else np.zeros(1, np.int32)
+        hp = self.text_hparams(ctx)
+        width = hp.projection_dim if flags & TOKENS_PROJECT else hp.hidden_size
+        flat = np.empty((int(lens.sum()), width), OUT_DTYPES.get(out_type, np.float32))
+        if not self.lib.clip_b200_text_tokens_packed(ctx, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(seqs),
+                                                     lens.ctypes.data_as(C.POINTER(C.c_int)), layer, flags, out_type, flat.ctypes.data):
+            raise RuntimeError("clip_b200_text_tokens_packed failed: " + self.last_error())
+        return np.split(flat, np.cumsum(lens)[:-1]) if seqs else []
 
     def text_tokens(self, ctx, ids: np.ndarray, layer: int = -1, flags: int = 0, out_type: int = OUT_F32) -> np.ndarray:
         """ids [n, seq_len] int32, padded by the caller -> [n, seq_len, width] of OUT_DTYPES[out_type]"""

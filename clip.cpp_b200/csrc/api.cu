@@ -313,15 +313,17 @@ bool run_linear(clip_ctx* c, const Linear& L, const TmaMap* xmap, const void* xp
     return true;
 }
 
-// A mixed-size pass (the *_mixed calls): nseq sequences of different lengths packed back to back in `rows` rows; d_seq is K3's
-// varlen table on the device (launch_attention_tc_varlen), groups its 64-row groups per head.
+// A packed pass (the image *_mixed and text *_packed calls): nseq sequences of different lengths packed back to back in `rows`
+// rows; d_seq is K3's varlen table on the device (launch_attention_tc_varlen), groups its 64-row groups per head; causal: the text
+// tower's mask.
 struct Packed {
     int rows = 0, nseq = 0, groups = 0;
     const int* d_seq = nullptr;
+    bool causal = false;
 };
 
 // The per-layer schedule shared by both towers (clip.cpp:1064-1143 text, 1342-1423 vision): blocks first .. end-1 on ws.x (a
-// multi-layer tokens call resumes where its previous stop left x).  pk: a packed mixed-size pass instead of nseq x T rows.
+// multi-layer tokens call resumes where its previous stop left x).  pk: a packed pass instead of nseq x T rows.
 bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal, int first, int end, const Packed* pk = nullptr) {
     // The residual stream x stays fp32 (as in the reference).  The branch GEMMs (out-proj, FC2) add their result INTO x themselves
     // (EPI_REDADD32): LayerNorm then only reads x and writes its 16-bit output.
@@ -335,13 +337,62 @@ bool run_blocks(clip_ctx* c, Tower& tw, int nseq, int T, bool causal, int first,
         const Layer& l = tw.L[il];
         { Scope s(c, K_LN); launch_layernorm(w.x, h, M, h, tw.eps, l.ln1_g, l.ln1_b, nullptr, w.a, bf, c->stream); }
         if (!run_linear(c, l.qkv, &w.map_a, w.a, bf, M, w.qkv, qw, EPI_STORE16, bf, qw / 3, qscale)) return false;
-        if (pk) { Scope s(c, K_ATTN); CK(launch_attention_tc_varlen(w.qkv, w.a, pk->rows, pk->nseq, pk->d_seq, pk->groups, tw.heads, dh, bf, c->stream)); }
+        if (pk) { Scope s(c, K_ATTN); CK(launch_attention_tc_varlen(w.qkv, w.a, pk->rows, pk->nseq, pk->d_seq, pk->groups, tw.heads, dh, pk->causal ? 1 : 0, bf, c->stream)); }
         else if (c->attn_tc) { Scope s(c, K_ATTN); CK(launch_attention_tc(w.qkv, w.a, nseq, T, tw.heads, dh, causal ? 1 : 0, bf, c->stream)); }
         else { Scope s(c, K_ATTN); launch_attention(w.qkv, w.a, nseq, T, tw.heads, causal ? 1 : 0, bf, c->stream); }
         if (!run_linear(c, l.out, &w.map_a, w.a, bf, M, w.x, h, EPI_REDADD32, 0)) return false;
         { Scope s(c, K_LN); launch_layernorm(w.x, h, M, h, tw.eps, l.ln2_g, l.ln2_b, nullptr, w.a, bf, c->stream); }
         if (!run_linear(c, l.fc1, &w.map_a, w.a, bf, M, w.g, tw.ff, c->use_gelu ? EPI_GELU16 : EPI_QGELU16, bf)) return false;
         if (!run_linear(c, l.fc2, &w.map_g, w.g, bf, M, w.x, h, EPI_REDADD32, 0)) return false;
+    }
+    CK(cudaGetLastError());
+    return true;
+}
+
+// ---- packed passes: what the image *_mixed and text *_packed forms share ------------------------------------------------------
+// Pass boundaries of a packed call whose item i has T[i] rows: each pass is the longest prefix of the remaining items that
+// fits(rows, items, t) admits (the pass's rows and items so far, the next item's rows), and holds at least one item.
+template <class F>
+std::vector<size_t> pack_passes(const std::vector<int>& T, F fits) {
+    std::vector<size_t> b{0};
+    size_t rows = 0, k = 0;
+    for (size_t i = 0; i < T.size(); i++) {
+        if (k && !fits(rows, k, T[i])) {
+            b.push_back(i);
+            rows = k = 0;
+        }
+        rows += (size_t)T[i]; k++;
+    }
+    b.push_back(T.size());
+    return b;
+}
+
+// K3's varlen table for the pass holding items i0 .. i1 - 1 (T[i] rows each) into seq [2 (i1 - i0 + 1)]: off (each item's first row,
+// then the pass's rows), then grp (prefix sums of the items' 64-row groups).  Returns the pass's rows.
+int varlen_table(const std::vector<int>& T, size_t i0, size_t i1, int* seq) {
+    const size_t nb = i1 - i0;
+    int* off = seq;
+    int* grp = seq + nb + 1;
+    off[0] = grp[0] = 0;
+    for (size_t j = 0; j < nb; j++) {
+        off[j + 1] = off[j] + T[i0 + j];
+        grp[j + 1] = grp[j] + (T[i0 + j] + 63) / 64;
+    }
+    return off[nb];
+}
+
+// The pooled tail of a packed pass: rows d_rows[0 .. nb) of ws.x (device, absolute rows) -> post-LN -> projection -> (L2 norm) ->
+// d_out [nb, proj], in chunks of at most cap_items rows (what the sel / proj buffers hold).  Every step works row by row, so the
+// chunks change no bits, and the fp32 gather keeps the bits the unpacked forms' LayerNorm reads.
+bool pooled_rows_tail(clip_ctx* c, Tower& tw, int nb, const int* d_rows, float* d_out, bool normalize) {
+    Workspace& w = tw.ws;
+    const int h = tw.hidden, bf = c->operand_bf16 ? 1 : 0;
+    for (int j0 = 0; j0 < nb; j0 += w.cap_items) {
+        const int k = std::min(w.cap_items, nb - j0);
+        { Scope s(c, K_OTHER); launch_gather_rows(w.x, w.sel32, k, h, 0, d_rows + j0, nullptr, bf, c->stream); }
+        { Scope s(c, K_LN); launch_layernorm(w.sel32, h, k, h, tw.eps, tw.post_g, tw.post_b, nullptr, w.sel16, bf, c->stream); }
+        if (!run_linear(c, tw.proj_w, &w.map_sel, w.sel16, bf, k, w.proj32, tw.proj, EPI_STORE32, 0)) return false;
+        { Scope s(c, K_OTHER); launch_l2norm(w.proj32, d_out + (size_t)j0 * tw.proj, k, tw.proj, normalize ? 1 : 0, c->stream); }
     }
     CK(cudaGetLastError());
     return true;
@@ -1535,7 +1586,7 @@ static bool mixed_pass(clip_ctx* c, const MixedCall& a, const TokenReq& q, size_
     std::lock_guard<std::mutex> lk(c->mu);
     CK(cudaSetDevice(c->device));
     if (!ensure_ws(c, tw, tw.micro_batch, tw.T, true)) return false;
-    const int P = tw.patch, h = tw.hidden, g = tw.image_size / P, bf = c->operand_bf16 ? 1 : 0;
+    const int P = tw.patch, h = tw.hidden, g = tw.image_size / P;
     const size_t n = hi - lo;
     std::vector<int> T(n);
     for (size_t i = 0; i < n; i++) {
@@ -1562,19 +1613,10 @@ static bool mixed_pass(clip_ctx* c, const MixedCall& a, const TokenReq& q, size_
         { Scope s(c, K_POS_RESAMPLE); launch_pos_resample(tw.pos + h, g, h, e.first.first, e.first.second, dst + h, c->stream); }
     }
     CK(cudaGetLastError());
-    // passes: total rows <= cap_rows, patch rows <= cap_items * n_patches, images <= cap_items (plan_call's limits)
-    std::vector<size_t> bounds{0};
-    {
-        size_t rows = 0, prows = 0, k = 0;
-        for (size_t i = 0; i < n; i++) {
-            if (k && (rows + T[i] > (size_t)w.cap_rows || prows + T[i] - 1 > (size_t)w.cap_items * tw.n_patches || k + 1 > (size_t)w.cap_items)) {
-                bounds.push_back(i);
-                rows = prows = k = 0;
-            }
-            rows += T[i]; prows += T[i] - 1; k++;
-        }
-        bounds.push_back(n);
-    }
+    // passes: total rows <= cap_rows, patch rows (one fewer per image) <= cap_items * n_patches, images <= cap_items (plan_call's limits)
+    const std::vector<size_t> bounds = pack_passes(T, [&](size_t rows, size_t k, int t) {
+        return rows + t <= (size_t)w.cap_rows && rows - k + t - 1 <= (size_t)w.cap_items * tw.n_patches && k + 1 <= (size_t)w.cap_items;
+    });
     size_t most = 0;
     for (size_t b = 0; b + 1 < bounds.size(); b++) most = std::max(most, bounds[b + 1] - bounds[b]);
     const size_t desc_bytes = (most * sizeof(MixedImage) + 2 * (most + 1) * sizeof(int) + 255) / 256 * 256;
@@ -1610,19 +1652,15 @@ static bool mixed_pass(clip_ctx* c, const MixedCall& a, const TokenReq& q, size_
         const int nb = (int)(i1 - i0);
         MixedImage* im = reinterpret_cast<MixedImage*>(blob.data());
         int* off = reinterpret_cast<int*>(blob.data() + nb * sizeof(MixedImage));
-        int* grp = off + nb + 1;
-        int rows = 0, prows = 0;
-        off[0] = grp[0] = 0;
+        const int* grp = off + nb + 1;
+        const int rows = varlen_table(T, i0, i1, off), prows = rows - nb;
         for (int j = 0; j < nb; j++) {
             const size_t i = i0 + j;
             const int gh = a.H(lo + i) / P, gw = a.W(lo + i) / P;
             const auto it = table.find(std::make_pair(gh, gw));
             im[j].px = (long long)(px0[i] - px0[i0]);
             im[j].pos = it == table.end() ? tw.pos : c->pos_mixed + it->second;
-            im[j].row = rows; im[j].prow = prows; im[j].gh = gh; im[j].gw = gw;
-            rows += T[i]; prows += T[i] - 1;
-            off[j + 1] = rows;
-            grp[j + 1] = grp[j] + (T[i] + 63) / 64;
+            im[j].row = off[j]; im[j].prow = off[j] - j; im[j].gh = gh; im[j].gw = gw;
         }
         const MixedImage* d_im = reinterpret_cast<const MixedImage*>(c->d_mixed);
         const int* d_seq = reinterpret_cast<const int*>(c->d_mixed + nb * sizeof(MixedImage));
@@ -1646,12 +1684,8 @@ static bool mixed_pass(clip_ctx* c, const MixedCall& a, const TokenReq& q, size_
             if (a.host) CK(cudaMemcpyAsync((char*)a.out + out0[i0], stage, out0[i1] - out0[i0], cudaMemcpyDeviceToHost, c->stream));
         } else {
             if (!run_blocks(c, tw, nb, 0, false, 0, tw.layers, &pk)) return false;
-            // CLS rows (off[j]) -> post-LN -> projection -> (L2 norm); the fp32 gather keeps the bits vision_forward's strided LN reads
-            { Scope s(c, K_OTHER); launch_gather_rows(w.x, w.sel32, nb, h, 0, d_seq, nullptr, bf, c->stream); }
-            { Scope s(c, K_LN); launch_layernorm(w.sel32, h, nb, h, tw.eps, tw.post_g, tw.post_b, nullptr, w.sel16, bf, c->stream); }
-            if (!run_linear(c, tw.proj_w, &w.map_sel, w.sel16, bf, nb, w.proj32, tw.proj, EPI_STORE32, 0)) return false;
-            { Scope s(c, K_OTHER); launch_l2norm(w.proj32, d_vec + i0 * tw.proj, nb, tw.proj, a.normalize ? 1 : 0, c->stream); }
-            CK(cudaGetLastError());
+            // the CLS rows (off[j]); a pass holds at most cap_items images, so this is one chunk
+            if (!pooled_rows_tail(c, tw, nb, d_seq, d_vec + i0 * tw.proj, a.normalize)) return false;
         }
     }
     CK(cudaEventRecord(c->ev_t1, c->stream));
@@ -1717,6 +1751,165 @@ bool clip_b200_image_tokens_device_mixed(const struct clip_ctx* cctx, const void
     MixedCall a{"clip_b200_image_tokens_device_mixed", true, false};
     a.in = d_pixels; a.n = n; a.heights = heights; a.widths = widths; a.layer = layer; a.flags = flags; a.out_type = out_type; a.out = d_out;
     return mixed_call(cctx, a);
+}
+
+// ---- token sequences of different lengths in one call: the four clip_b200_text_*_packed forms ----------------------------------
+// What one packed text call reads, as its public form received it.
+struct PackedTextCall {
+    const char* who;                              // the public name, for messages
+    bool tokens, host;                            // per-token rows (else pooled); host ids and output (else device)
+    const clip_tokens* seqs = nullptr;            // host pooled: the sequences
+    const int32_t* ids = nullptr;                 // the other forms: the sequences back to back (host or device)
+    const int* lens = nullptr;                    // with ids: host, n entries
+    size_t n = 0;
+    int layer = 0, flags = 0, out_type = 0;       // tokens
+    void* out = nullptr;                          // tokens: the ragged rows (host or device)
+    float* vec = nullptr;                         // pooled, host
+    float* d_vec = nullptr;                       // pooled, device
+    bool normalize = true;
+    int len(size_t i) const { return seqs ? (int)seqs[i].size : lens[i]; }
+};
+
+// One GPU, sequences lo .. hi of a checked packed call: passes of the longest prefix of the remaining sequences whose rows fit the
+// workspace (micro_batch x context_length rows), each one forward pass over its rows packed back to back.  Per pass, one upload of
+// K3's varlen table (whose off[] also places each row's position) and the EOT rows, the ids (read in place on the device, staged
+// into ws.ids from the host), one embedding, the blocks, then the tail.  Only the staging, the embedding and the pooled rows differ
+// from mixed_pass; the planner, the table, the blocks and the tails are the ones it runs.
+static bool text_packed_pass(clip_ctx* c, const PackedTextCall& a, const TokenReq& q, size_t lo, size_t hi) {
+    Tower& tw = c->txt;
+    Workspace& w = tw.ws;
+    const size_t n = hi - lo;
+    std::vector<int> T(n);
+    std::vector<size_t> id0(n + 1, 0), out0(n + 1, 0);     // sequence lo + i's first id and first output byte, from sequence lo's
+    for (size_t i = 0; i < n; i++) {
+        T[i] = a.len(lo + i);
+        id0[i + 1] = id0[i] + (size_t)T[i];
+        out0[i + 1] = out0[i] + (size_t)T[i] * q.width * q.esize;
+    }
+    size_t id_lo = 0;
+    for (size_t i = 0; i < lo; i++) id_lo += (size_t)a.len(i);
+    // host sequences: gathered into one pageable array, so that a pass's ids go up in one copy
+    std::vector<int32_t> gathered;
+    if (a.seqs) {
+        gathered.resize(id0[n]);
+        for (size_t i = 0; i < n; i++) memcpy(gathered.data() + id0[i], a.seqs[lo + i].data, (size_t)T[i] * 4);
+    }
+    const int32_t* ids = a.seqs ? gathered.data() : a.ids + id_lo;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    if (!ensure_ws(c, tw, tw.micro_batch, tw.n_ctx, false)) return false;
+    // every sequence fits a pass alone: its length is at most context_length
+    const std::vector<size_t> bounds = pack_passes(T, [&](size_t rows, size_t, int t) { return rows + t <= (size_t)w.cap_rows; });
+    size_t most = 0;
+    for (size_t b = 0; b + 1 < bounds.size(); b++) most = std::max(most, bounds[b + 1] - bounds[b]);
+    // one pass's descriptors: K3's varlen table [2 (nb + 1)], then the EOT rows [nb]
+    std::vector<int> blob(3 * most + 2);
+    if (!ensure_buf(c, &c->d_mixed, &c->d_mixed_cap, blob.size() * sizeof(int))) return false;
+    float* d_vec = a.d_vec;
+    if (!a.tokens && !d_vec) {
+        if (!ensure_out(c, n * tw.proj)) return false;
+        d_vec = c->d_out;
+    }
+    char* stage = nullptr;     // host tokens: one pass's rows on the device, then copied out
+    if (a.tokens && a.host) {
+        size_t widest = 0;
+        for (size_t b = 0; b + 1 < bounds.size(); b++) widest = std::max(widest, out0[bounds[b + 1]] - out0[bounds[b]]);
+        if (!ensure_buf(c, &c->d_ring, &c->d_ring_cap, widest)) return false;
+        stage = c->d_ring;
+    }
+    const size_t out_lo = id_lo * q.width * q.esize;
+    CK(cudaEventRecord(c->ev_t0, c->stream));
+    for (size_t b = 0; b + 1 < bounds.size(); b++) {
+        const size_t i0 = bounds[b], i1 = bounds[b + 1];
+        const int nb = (int)(i1 - i0);
+        int* off = blob.data();
+        const int rows = varlen_table(T, i0, i1, off);
+        int* eot = off + 2 * (nb + 1);
+        for (int j = 0; j < nb; j++) eot[j] = off[j + 1] - 1;     // the reference selects row N-1 (clip.cpp:1154-1155)
+        const int* d_seq = reinterpret_cast<const int*>(c->d_mixed);
+        CK(cudaMemcpyAsync(c->d_mixed, blob.data(), (size_t)(3 * nb + 2) * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+        const int32_t* d_ids = ids + id0[i0];
+        if (a.host) {
+            CK(cudaMemcpyAsync(w.ids, d_ids, (size_t)rows * 4, cudaMemcpyHostToDevice, c->stream));
+            d_ids = w.ids;
+        }
+        { Scope s(c, K_OTHER); launch_text_embed_packed(d_ids, tw.tok, tw.pos, d_seq, nb, rows, tw.hidden, tw.n_vocab, w.x, c->stream); }
+        const Packed pk{rows, nb, off[2 * nb + 1], d_seq, true};
+        if (!run_blocks(c, tw, nb, 0, true, 0, a.tokens ? q.blocks : tw.layers, &pk)) return false;
+        if (a.tokens) {
+            // text has no NO_CLS: the packed rows are already the ragged item-major layout
+            char* dst = a.host ? stage : (char*)a.out + out_lo + out0[i0];
+            if (!token_rows_tail(c, tw, 1, rows, q, dst)) return false;
+            if (a.host) CK(cudaMemcpyAsync((char*)a.out + out_lo + out0[i0], stage, out0[i1] - out0[i0], cudaMemcpyDeviceToHost, c->stream));
+        } else if (!pooled_rows_tail(c, tw, nb, d_seq + 2 * (nb + 1), d_vec + i0 * tw.proj, a.normalize)) {
+            return false;
+        }
+    }
+    CK(cudaEventRecord(c->ev_t1, c->stream));
+    if (!a.tokens && a.vec) CK(cudaMemcpyAsync(a.vec + lo * tw.proj, d_vec, n * tw.proj * 4, cudaMemcpyDeviceToHost, c->stream));
+    return sync_and_time(c);
+}
+
+// Every packed text form: the arguments checked in one order, the first fault refused (include/clip_b200.h), then the passes;
+// devices mode shards the host forms' sequences over the GPUs as clip_text_batch_encode does.
+static bool text_packed_call(const clip_ctx* cctx, PackedTextCall a) {
+    clip_ctx* c = const_cast<clip_ctx*>(cctx);
+    const std::string who = a.who;
+    if (!c) { set_err(who + ": null context"); return false; }
+    const Tower& tw = c->txt;
+    if (!tw.present) { set_err(who + ": this model has no text encoder"); return false; }
+    if (tw.hidden != 64 * tw.heads) {
+        set_err(who + ": packed sequences need a text tower of head_dim 64, not " + std::to_string(tw.hidden / tw.heads) + " (hidden " +
+                std::to_string(tw.hidden) + ", heads " + std::to_string(tw.heads) + ")");
+        return false;
+    }
+    if (a.n == 0) return true;
+    if (!(a.seqs || a.ids)) { set_err(who + ": null input"); return false; }
+    if (!a.seqs && !a.lens) { set_err(who + ": null lens"); return false; }
+    if (!(a.tokens ? a.out : a.host ? (void*)a.vec : (void*)a.d_vec)) { set_err(who + ": null output"); return false; }
+    for (size_t i = 0; i < a.n; i++) {
+        if (a.seqs && !a.seqs[i].data) { set_err(who + ": sequence " + std::to_string(i) + " has no tokens"); return false; }
+        const long long L = a.seqs ? (long long)std::min<size_t>(a.seqs[i].size, (size_t)INT_MAX) : (long long)a.lens[i];
+        if (L < 1 || L > tw.n_ctx) {
+            set_err(who + ": sequence " + std::to_string(i) + " has length " + std::to_string(L) + ", outside [1, context_length (" +
+                    std::to_string(tw.n_ctx) + ")]");
+            return false;
+        }
+    }
+    TokenReq q;
+    if (a.tokens) {
+        if (!token_request(c, false, a.layer, a.flags, a.out_type, q, a.who)) return false;
+        if (q.attn) { set_err(who + ": CLIP_B200_TOKENS_ATTENTION is not supported at packed lengths"); return false; }
+    }
+    if (a.host && c->replicas.size() > 1 && a.n >= TEXT_SHARD_MIN * c->replicas.size())
+        return for_each_replica(c, a.n, [&](clip_ctx* r, int, size_t lo, size_t hi) { return hi == lo || text_packed_pass(r, a, q, lo, hi); });
+    return text_packed_pass(c, a, q, 0, a.n);
+}
+
+bool clip_b200_text_batch_encode_packed(const struct clip_ctx* cctx, const struct clip_tokens* seqs, size_t n, float* vec, bool normalize) {
+    PackedTextCall a{"clip_b200_text_batch_encode_packed", false, true};
+    a.seqs = seqs; a.n = n; a.vec = vec; a.normalize = normalize;
+    return text_packed_call(cctx, a);
+}
+
+bool clip_b200_text_encode_device_packed(const struct clip_ctx* cctx, const void* d_ids, size_t n, const int* lens, void* d_vec, bool normalize) {
+    PackedTextCall a{"clip_b200_text_encode_device_packed", false, false};
+    a.ids = (const int32_t*)d_ids; a.n = n; a.lens = lens; a.d_vec = (float*)d_vec; a.normalize = normalize;
+    return text_packed_call(cctx, a);
+}
+
+bool clip_b200_text_tokens_packed(const struct clip_ctx* cctx, const int32_t* ids, size_t n, const int* lens, int layer, int flags, int out_type,
+                                  void* out) {
+    PackedTextCall a{"clip_b200_text_tokens_packed", true, true};
+    a.ids = ids; a.n = n; a.lens = lens; a.layer = layer; a.flags = flags; a.out_type = out_type; a.out = out;
+    return text_packed_call(cctx, a);
+}
+
+bool clip_b200_text_tokens_device_packed(const struct clip_ctx* cctx, const void* d_ids, size_t n, const int* lens, int layer, int flags,
+                                         int out_type, void* d_out) {
+    PackedTextCall a{"clip_b200_text_tokens_device_packed", true, false};
+    a.ids = (const int32_t*)d_ids; a.n = n; a.lens = lens; a.layer = layer; a.flags = flags; a.out_type = out_type; a.out = d_out;
+    return text_packed_call(cctx, a);
 }
 
 // ---- several layers from one forward pass (clip_b200_*_tokens_layers) ------------------------------------------------------------
@@ -2871,15 +3064,18 @@ extern "C" {
 // TEST HOOK: K3's varlen instance on device 0.  nseq sequences of lens[s] rows packed back to back: qkv fp32 host [sum lens, 3*H*dh]
 // (laid out, rounded and padded as for clip_b200_debug_attention_hd), out fp32 host [sum lens, H*dh].  The qkv rows past the last
 // sequence and one 128-row block of guard rows after the output are poisoned (0xFF); a guard row written is an error (rc 6).
-int clip_b200_debug_attention_mixed(int operand_bf16, int nseq, const int* lens, int H, int head_dim, const float* qkv, float* out) {
+static int debug_attention_varlen(const char* who, int operand_bf16, int nseq, const int* lens, int H, int head_dim, int causal,
+                                  const float* qkv, float* out) {
     g_err.clear();
-    if (head_dim != 64 && head_dim != 80 && head_dim != 104) { set_err("attention_mixed: head_dim must be 64, 80 or 104"); return 2; }
-    if (nseq <= 0 || H <= 0 || !lens) { set_err("attention_mixed: bad shape"); return 2; }
+    const std::string w = who;
+    if (causal && head_dim != 64) { set_err(w + ": head_dim must be 64"); return 2; }
+    if (head_dim != 64 && head_dim != 80 && head_dim != 104) { set_err(w + ": head_dim must be 64, 80 or 104"); return 2; }
+    if (nseq <= 0 || H <= 0 || !lens) { set_err(w + ": bad shape"); return 2; }
     std::vector<int> seq(2 * ((size_t)nseq + 1), 0);
     int* off = seq.data();
     int* grp = off + nseq + 1;
     for (int i = 0; i < nseq; i++) {
-        if (lens[i] <= 0) { set_err("attention_mixed: every length must be positive"); return 2; }
+        if (lens[i] <= 0) { set_err(w + ": every length must be positive"); return 2; }
         off[i + 1] = off[i] + lens[i];
         grp[i + 1] = grp[i] + (lens[i] + 63) / 64;
     }
@@ -2891,14 +3087,23 @@ int clip_b200_debug_attention_mixed(int operand_bf16, int nseq, const int* lens,
     uint16_t* d_out = (uint16_t*)s.alloc((rows * hid + guard) * 2, 0xff);
     int* d_seq = (int*)s.alloc(seq.size() * 4, 0, seq.data(), seq.size() * 4);
     if (!s.ok) return 3;
-    const cudaError_t e = launch_attention_tc_varlen(d_qkv, d_out, (int)rows, nseq, d_seq, grp[nseq], H, head_dim, operand_bf16, s.st);
-    if (e != cudaSuccess) { set_err(std::string("attention_mixed: ") + cudaGetErrorString(e)); return 5; }
-    if (!s.finish("attention_mixed")) return 5;
+    const cudaError_t e = launch_attention_tc_varlen(d_qkv, d_out, (int)rows, nseq, d_seq, grp[nseq], H, head_dim, causal, operand_bf16, s.st);
+    if (e != cudaSuccess) { set_err(w + ": " + cudaGetErrorString(e)); return 5; }
+    if (!s.finish(who)) return 5;
     std::vector<uint16_t> o16(rows * hid + guard);
     if (!s.copy_back(o16.data(), d_out, o16.size() * 2)) return 6;
-    if (std::any_of(o16.begin() + rows * hid, o16.end(), [](uint16_t b) { return b != 0xffff; })) { set_err("attention_mixed: a guard row was written"); return 6; }
+    if (std::any_of(o16.begin() + rows * hid, o16.end(), [](uint16_t b) { return b != 0xffff; })) { set_err(w + ": a guard row was written"); return 6; }
     from16(o16.data(), rows * hid, operand_bf16, out);
     return 0;
+}
+
+int clip_b200_debug_attention_mixed(int operand_bf16, int nseq, const int* lens, int H, int head_dim, const float* qkv, float* out) {
+    return debug_attention_varlen("attention_mixed", operand_bf16, nseq, lens, H, head_dim, 0, qkv, out);
+}
+
+// TEST HOOK: the same with the causal mask (the text tower's packed passes), head_dim 64 only
+int clip_b200_debug_attention_mixed_causal(int operand_bf16, int nseq, const int* lens, int H, int head_dim, const float* qkv, float* out) {
+    return debug_attention_varlen("attention_mixed_causal", operand_bf16, nseq, lens, H, head_dim, 1, qkv, out);
 }
 
 int clip_b200_debug_layernorm(int rows, int h, size_t in_stride, float eps, const float* x, const float* gamma, const float* beta,

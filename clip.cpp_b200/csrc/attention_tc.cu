@@ -32,6 +32,8 @@
 // Any T; a causal group stops at its own diagonal.
 #include <cuda.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "gemm.h"
 #include "kernels.h"
@@ -101,6 +103,15 @@ CB_DEVINL uint32_t pack2(float lo, float hi) {
 struct Group {
     int seq, head, g0, kend;
 };
+// A group of a packed causal sequence: its key end (min(len, g0 + 64)) and its sequence's length, which bounds the key mask and the
+// row stores, apart.  A type of its own, so that the non-causal varlen instances keep Group's layout and code.
+struct GroupLen : Group {
+    int len;
+};
+template <bool CAUSAL>
+using VarGroup = std::conditional_t<CAUSAL, GroupLen, Group>;
+CB_DEVINL int seq_len(const Group& g) { return g.kend; }         // non-causal: the key end is the length
+CB_DEVINL int seq_len(const GroupLen& g) { return g.len; }
 CB_DEVINL Group group_of(const AParams& p, int g) {
     const int sh = g / p.ngrp;
     Group r;
@@ -120,10 +131,11 @@ struct VarLen {
 };
 
 // group_of for packed sequences.  Group::seq holds the sequence's first row (distinct for distinct sequences, so iter_var's test of a
-// shared (sequence, head) is iter_of's) and kend its length.  s: a sequence at or before group g's, advanced to g's.  A thread's
-// groups only increase, so the search gallops forward from the last sequence found (one load when g is still in it) and ends in a
-// binary search of the bracket.
-CB_DEVINL Group group_var(const AParams& p, const VarLen& v, int g, int& s) {
+// shared (sequence, head) is iter_of's) and kend its length; causal, kend is the group's diagonal end as group_of has it and len the
+// length.  s: a sequence at or before group g's, advanced to g's.  A thread's groups only increase, so the search gallops forward from the
+// last sequence found (one load when g is still in it) and ends in a binary search of the bracket.
+template <bool CAUSAL>
+CB_DEVINL VarGroup<CAUSAL> group_var(const AParams& p, const VarLen& v, int g, int& s) {
     int lo = s, step = 1;
     while (lo + step < v.nseq && __ldg(v.grp + lo + step) * p.H <= g) { lo += step; step *= 2; }
     int hi = min(lo + step, v.nseq) - 1;
@@ -134,22 +146,28 @@ CB_DEVINL Group group_var(const AParams& p, const VarLen& v, int g, int& s) {
     }
     s = lo;
     const int ng = __ldg(v.grp + lo + 1) - __ldg(v.grp + lo), local = g - __ldg(v.grp + lo) * p.H;
-    Group r;
+    VarGroup<CAUSAL> r;
     r.head = local / ng;
     r.g0 = (local - r.head * ng) * AG;
     r.seq = __ldg(v.off + lo);
     r.kend = __ldg(v.off + lo + 1) - r.seq;
+    if constexpr (CAUSAL) {
+        r.len = r.kend;
+        r.kend = min(r.len, r.g0 + AG);
+    }
     return r;
 }
 
 // The two groups of iteration `it` and what the K / V stages hold for them: slot 0 the first group's head (and the second's, when it
 // is the same (sequence, head) or there is no second group), slot 1 the second group's head otherwise.  kend0 / kend1: the keys a
 // slot must hold (0: slot unused); nkb: key blocks (of KB keys) of the iteration.
-struct Iter {
-    Group a, b;
+template <class Gr>
+struct IterOf {
+    Gr a, b;
     bool has_b, shared;
     int kend0, kend1, nkb;
 };
+using Iter = IterOf<Group>;
 template <int KB>
 CB_DEVINL Iter iter_of(const AParams& p, int it) {
     Iter r;
@@ -164,12 +182,12 @@ CB_DEVINL Iter iter_of(const AParams& p, int it) {
 }
 
 // iter_of for packed sequences (s: group_var's)
-template <int KB>
-CB_DEVINL Iter iter_var(const AParams& p, const VarLen& v, int it, int& s) {
-    Iter r;
+template <int KB, bool CAUSAL>
+CB_DEVINL IterOf<VarGroup<CAUSAL>> iter_var(const AParams& p, const VarLen& v, int it, int& s) {
+    IterOf<VarGroup<CAUSAL>> r;
     r.has_b = 2 * it + 1 < p.ngroups;
-    r.a = group_var(p, v, 2 * it, s);
-    r.b = r.has_b ? group_var(p, v, 2 * it + 1, s) : r.a;
+    r.a = group_var<CAUSAL>(p, v, 2 * it, s);
+    r.b = r.has_b ? group_var<CAUSAL>(p, v, 2 * it + 1, s) : r.a;
     r.shared = r.a.seq == r.b.seq && r.a.head == r.b.head;
     r.kend0 = r.shared ? max(r.a.kend, r.b.kend) : r.a.kend;
     r.kend1 = r.shared ? 0 : r.b.kend;
@@ -434,14 +452,18 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __gr
     }
 }
 
-// K3 on packed sequences of different lengths (VarLen), non-causal: the kernel above with the maps viewing the packed rows as one
+// K3 on packed sequences of different lengths (VarLen): the kernel above with the maps viewing the packed rows as one
 // sequence.  A group's rows and keys are counted from its sequence's first row, its length takes the place of T, so every key block
 // and the width of the last one are those a fixed-T launch of that sequence alone takes, and each kept row has its arithmetic.  The box rows past a
 // sequence's end now hold the next sequence's rows instead of zeros: their scores are masked by select, their Q rows are never
 // stored, but P.V would turn a non-finite V row into NaN (0 * Inf), so the producer warp zeroes those V rows once the box has landed
 // and before the consumers may read the stage: such a stage lands on a barrier of the producer's own, and the producer arrives on
 // the stage's full barrier once the zeros are stored.
-template <bool BF, int DH>
+// CAUSAL (the text tower's packed passes, head_dim 64 only): a group's keys end at min(len, g0 + 64), as group_of has them, and
+// attend_block masks with T = len and causal = 1, as the fixed-T causal kernel calls it.  A key end before the sequence's end is
+// g0 + 64, a multiple of the 64-row box, so a slot's last box then ends exactly at its key end: box rows past a key end, the rows
+// the producer zeroes, still occur only at a sequence's end.
+template <bool BF, int DH, bool CAUSAL>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(const __grid_constant__ AParams p, const __grid_constant__ CUtensorMap tm_mid,
                                                                              const VarLen v) {
     using G = AttnGeo<DH>;
@@ -480,7 +502,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(con
         uint32_t n = 0, i = 0, nz = 0;
         int sq = 0;
         for (int it = blockIdx.x; it < p.niter; it += gridDim.x, i++) {
-            const Iter w = iter_var<G::KB>(p, v, it, sq);
+            const auto w = iter_var<G::KB, CAUSAL>(p, v, it, sq);
             const uint32_t qb = i & 1, q_s = smem_base + qb * G::TILE;
             if (lane == 0) {
                 mbar_wait(q_empty + 8 * qb, ((i >> 1) & 1) ^ 1);
@@ -528,11 +550,12 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(con
     int sq = 0;
     for (int it = blockIdx.x; it < p.niter; it += gridDim.x, i++) {
         const int sq_it = sq;                                  // at or before both groups' sequences
-        const Iter w = iter_var<G::KB>(p, v, it, sq);
-        const Group g = (wg == 0 || !w.has_b) ? w.a : w.b;
+        const auto w = iter_var<G::KB, CAUSAL>(p, v, it, sq);
+        const auto g = (wg == 0 || !w.has_b) ? w.a : w.b;
         const bool live = wg == 0 || w.has_b;                  // warpgroup-uniform: only the launch's last, odd group leaves one idle
         const uint32_t slot = (wg == 0 || w.shared) ? 0u : 1u;
         const int nkb = (g.kend + G::KB - 1) / G::KB;
+        const int len = seq_len(g);                            // the sequence's length: the key mask and the row stores
         const int wrow0 = g.g0 + (warp & 3) * 16;              // first query row of this warp
         const int r0 = wrow0 + (lane >> 2);                    // this thread: rows r0 and r0 + 8
         // o: columns 0-63, om: 64-95 (head_dim 104 only), ot: the 16-column tail (head_dim 80, 104)
@@ -555,10 +578,10 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(con
             if (live && kb < nkb) {
                 const int key0 = kb * G::KB, rem = g.kend - key0;
                 // S at the narrowest width that covers the keys left (a 64-key block never needs 128)
-                if (G::KB == 128 && rem > 64) attend_block<BF, DH, 16>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, g.kend, 0, wrow0, r0, tc);
-                else if (rem > 32) attend_block<BF, DH, 8>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, g.kend, 0, wrow0, r0, tc);
-                else if (rem > 16) attend_block<BF, DH, 4>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, g.kend, 0, wrow0, r0, tc);
-                else attend_block<BF, DH, 2>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, g.kend, 0, wrow0, r0, tc);
+                if (G::KB == 128 && rem > 64) attend_block<BF, DH, 16>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, len, CAUSAL ? 1 : 0, wrow0, r0, tc);
+                else if (rem > 32) attend_block<BF, DH, 8>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, len, CAUSAL ? 1 : 0, wrow0, r0, tc);
+                else if (rem > 16) attend_block<BF, DH, 4>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, len, CAUSAL ? 1 : 0, wrow0, r0, tc);
+                else attend_block<BF, DH, 2>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, len, CAUSAL ? 1 : 0, wrow0, r0, tc);
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(kv_empty + 8 * s);
@@ -570,7 +593,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(con
         // the group's first row and head looked up again rather than held in registers through the key loop (the head_dim 80
         // instance has none to spare at 168, the most 288 threads can have)
         int sq_e = sq_it;
-        const Group ge = group_var(p, v, 2 * it + wg, sq_e);
+        const auto ge = group_var<CAUSAL>(p, v, 2 * it + wg, sq_e);
         #pragma unroll
         for (int h = 0; h < 2; h++) {
             float l = l_run[h];
@@ -578,7 +601,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(con
             l += __shfl_xor_sync(0xffffffffu, l, 2);
             const float inv = 1.0f / l;
             const int row = r0 + 8 * h;
-            if (row < g.kend) {
+            if (row < len) {
                 uint16_t* orow = p.out + ((size_t)ge.seq + row) * hid + ge.head * DH;
                 #pragma unroll
                 for (int j = 0; j < 8; j++)
@@ -863,10 +886,16 @@ cudaError_t set_smem() {
     if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(attention_tc_kernel<false, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AttnGeo<DH>::SMEM);
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attention_tc_varlen_kernel<true, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)varlen_smem<DH>());
+    e = cudaFuncSetAttribute(attention_tc_varlen_kernel<true, DH, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)varlen_smem<DH>());
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attention_tc_varlen_kernel<false, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)varlen_smem<DH>());
+    e = cudaFuncSetAttribute(attention_tc_varlen_kernel<false, DH, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)varlen_smem<DH>());
     if (e != cudaSuccess) return e;
+    if constexpr (DH == 64) {
+        e = cudaFuncSetAttribute(attention_tc_varlen_kernel<true, DH, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)varlen_smem<DH>());
+        if (e != cudaSuccess) return e;
+        e = cudaFuncSetAttribute(attention_tc_varlen_kernel<false, DH, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)varlen_smem<DH>());
+        if (e != cudaSuccess) return e;
+    }
     e = cudaFuncSetAttribute(attention_probs_kernel<true, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ProbsGeo<DH>::SMEM);
     if (e != cudaSuccess) return e;
     return cudaFuncSetAttribute(attention_probs_kernel<false, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ProbsGeo<DH>::SMEM);
@@ -879,12 +908,12 @@ cudaError_t launch_dh(const AParams& p, const CUtensorMap& tm_mid, unsigned grid
                 : launch_pdl(attention_tc_kernel<false, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid);
 }
 
-template <int DH>
+template <int DH, bool CAUSAL>
 cudaError_t launch_varlen_dh(const AParams& p, const CUtensorMap& tm_mid, const VarLen& v, unsigned grid, int bf16, cudaStream_t st) {
     static_assert(varlen_smem<DH>() <= 227 * 1024, "shared memory per block");
     constexpr uint32_t smem = varlen_smem<DH>();
-    return bf16 ? launch_pdl(attention_tc_varlen_kernel<true, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid, v)
-                : launch_pdl(attention_tc_varlen_kernel<false, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid, v);
+    return bf16 ? launch_pdl(attention_tc_varlen_kernel<true, DH, CAUSAL>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid, v)
+                : launch_pdl(attention_tc_varlen_kernel<false, DH, CAUSAL>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid, v);
 }
 
 template <int DH>
@@ -927,15 +956,15 @@ cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T,
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 
-cudaError_t launch_attention_tc_varlen(const void* qkv16, void* out16, int rows, int nseq, const int* d_seq, int groups, int H, int dh, int bf16,
-                                      cudaStream_t st) {
-    if (!supported_dh(dh)) return cudaErrorInvalidValue;
+cudaError_t launch_attention_tc_varlen(const void* qkv16, void* out16, int rows, int nseq, const int* d_seq, int groups, int H, int dh, int causal,
+                                      int bf16, cudaStream_t st) {
+    if (!supported_dh(dh) || (causal && dh != 64)) return cudaErrorInvalidValue;
     if (nseq <= 0) return cudaSuccess;
     AParams p;
     CUtensorMap tm_mid;
     memset(&p, 0, sizeof(p));
     if (!make_piece_maps(p, tm_mid, qkv16, 1, rows, H, dh)) return cudaErrorInvalidValue;
-    p.out = (uint16_t*)out16; p.T = rows; p.H = H; p.causal = 0;
+    p.out = (uint16_t*)out16; p.T = rows; p.H = H; p.causal = causal;
     const long long ngroups = (long long)groups * H;
     if (ngroups > 0x7ffffffell) return cudaErrorInvalidValue;
     p.ngroups = (int)ngroups;
@@ -946,8 +975,9 @@ cudaError_t launch_attention_tc_varlen(const void* qkv16, void* out16, int rows,
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (e != cudaSuccess) return e;
     const unsigned grid = (unsigned)min(p.niter, sms);
-    e = dh == 104 ? launch_varlen_dh<104>(p, tm_mid, v, grid, bf16, st) : dh == 80 ? launch_varlen_dh<80>(p, tm_mid, v, grid, bf16, st)
-                  : launch_varlen_dh<64>(p, tm_mid, v, grid, bf16, st);
+    e = causal ? launch_varlen_dh<64, true>(p, tm_mid, v, grid, bf16, st)
+        : dh == 104 ? launch_varlen_dh<104, false>(p, tm_mid, v, grid, bf16, st) : dh == 80 ? launch_varlen_dh<80, false>(p, tm_mid, v, grid, bf16, st)
+                  : launch_varlen_dh<64, false>(p, tm_mid, v, grid, bf16, st);
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 

@@ -317,6 +317,27 @@ __global__ void __launch_bounds__(256) text_embed_kernel(const int32_t* __restri
     for (int i = lane; i < (h >> 2); i += 32) *reinterpret_cast<float4*>(xr + 4 * i) = add4(ld4(pr + 4 * i), ld4(tr + 4 * i));
 }
 
+// text_embed_kernel over the sequences of a packed pass: row `row` is token row - off[s] of sequence s (off in row order, so a binary
+// search of the first rows), with text_embed_kernel's clamp and sum
+__global__ void __launch_bounds__(256) text_embed_packed_kernel(const int32_t* __restrict__ ids, const float* __restrict__ tok,
+                                                                const float* __restrict__ pos, const int* __restrict__ off, int nseq,
+                                                                int rows, int h, int n_vocab, float* __restrict__ x) {
+    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (row >= rows) return;
+    int lo = 0, hi = nseq - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (off[mid] <= row) lo = mid;
+        else hi = mid - 1;
+    }
+    int id = ids[row];
+    id = id < 0 ? 0 : (id >= n_vocab ? n_vocab - 1 : id);
+    const float* tr = tok + (size_t)id * h;
+    const float* pr = pos + (size_t)(row - off[lo]) * h;
+    float* xr = x + (size_t)row * h;
+    for (int i = lane; i < (h >> 2); i += 32) *reinterpret_cast<float4*>(xr + 4 * i) = add4(ld4(pr + 4 * i), ld4(tr + 4 * i));
+}
+
 __global__ void __launch_bounds__(256) l2norm_kernel(const float* __restrict__ v, float* __restrict__ out, int rows, int d,
                                                      int normalize) {
     const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -475,6 +496,12 @@ void launch_text_embed(const int32_t* ids, const float* tok, const float* pos, i
                        cudaStream_t st) {
     if (nseq * T <= 0) return;
     text_embed_kernel<<<rows_grid(nseq * T, 8), 256, 0, st>>>(ids, tok, pos, nseq, T, h, n_vocab, x);
+}
+
+void launch_text_embed_packed(const int32_t* ids, const float* tok, const float* pos, const int* off, int nseq, int rows, int h, int n_vocab,
+                              float* x, cudaStream_t st) {
+    if (nseq <= 0 || rows <= 0) return;
+    text_embed_packed_kernel<<<rows_grid(rows, 8), 256, 0, st>>>(ids, tok, pos, off, nseq, rows, h, n_vocab, x);
 }
 
 void launch_l2norm(const float* v, float* out, int rows, int d, int normalize, cudaStream_t st) {

@@ -50,6 +50,10 @@ void launch_assemble_mixed(const float* patch, const float* class_embd, const Mi
 // K4t text embed: x[s*T+t,:] = tok[ids[s*T+t],:] + pos[t,:]   (clip.cpp:1059-1061), tables fp32 (dequantised at load)
 void launch_text_embed(const int32_t* ids, const float* tok, const float* pos, int nseq, int T, int h, int n_vocab, float* x,
                        cudaStream_t st);
+// K4t over the nseq sequences of a packed pass (the *_packed text calls): row r of sequence s = rows off[s] .. off[s + 1] - 1 (off:
+// device, nseq + 1 entries, off[nseq] = rows) is tok[ids[r]] + pos[r - off[s]], bit for bit what launch_text_embed writes for s alone
+void launch_text_embed_packed(const int32_t* ids, const float* tok, const float* pos, const int* off, int nseq, int rows, int h, int n_vocab,
+                              float* x, cudaStream_t st);
 
 // K3 attention: softmax(Q K^T [causal]) V per (sequence, head); qkv 16-bit [nseq*T, 3*H*dh] (Q pre-scaled by 1/sqrt(dh)),
 // out 16-bit [nseq*T, H*dh].  (clip.cpp:1100-1108, 1382-1388)
@@ -67,11 +71,12 @@ constexpr int qkv_head_cols(int dh) { return dh == 104 ? 112 : dh; }
 // each sequence's T tokens).
 cudaError_t attention_tc_init();
 cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T, int H, int dh, int causal, int bf16, cudaStream_t st);
-// K3 on nseq packed sequences of different lengths, non-causal: qkv16 [rows, 3*H*qkv_head_cols(dh)], out16 [rows, H*dh], sequence s
-// = rows off[s] .. off[s + 1] - 1.  d_seq (device): off [nseq + 1] (off[0] = 0, off[nseq] = rows), then grp [nseq + 1], the prefix
-// sums of ceil(len_s / 64); groups = grp[nseq].  Each sequence's rows equal, bit for bit, a launch_attention_tc of that sequence alone.
-cudaError_t launch_attention_tc_varlen(const void* qkv16, void* out16, int rows, int nseq, const int* d_seq, int groups, int H, int dh, int bf16,
-                                      cudaStream_t st);
+// K3 on nseq packed sequences of different lengths: qkv16 [rows, 3*H*qkv_head_cols(dh)], out16 [rows, H*dh], sequence s = rows
+// off[s] .. off[s + 1] - 1.  d_seq (device): off [nseq + 1] (off[0] = 0, off[nseq] = rows), then grp [nseq + 1], the prefix sums of
+// ceil(len_s / 64); groups = grp[nseq].  causal (the text tower): head_dim 64 only.  Each sequence's rows equal, bit for bit, a
+// launch_attention_tc of that sequence alone with the same causal.
+cudaError_t launch_attention_tc_varlen(const void* qkv16, void* out16, int rows, int nseq, const int* d_seq, int groups, int H, int dh, int causal,
+                                      int bf16, cudaStream_t st);
 
 // K9 attention probabilities (attention_tc.cu): the softmax(Q K^T [causal]) K3 computes internally, from the same qkv16, written out:
 // out [nseq, H, R, T] of elem_type (0 fp32, 1 fp16, 2 bf16: RNE of the fp32 value), R = T, or 1 with cls_only (query row 0 alone).

@@ -291,6 +291,37 @@ bool clip_b200_image_tokens_mixed(const struct clip_ctx * ctx, const struct clip
 bool clip_b200_image_tokens_device_mixed(const struct clip_ctx * ctx, const void * d_pixels, size_t n, const int * heights,
                                          const int * widths, int layer, int flags, int out_type, void * d_out);
 
+/* Token sequences of different lengths in one call, with no padding: clip_text_batch_encode, clip_b200_text_encode_device and
+ * clip_b200_text_tokens[_device] with every sequence at its own length.  The sequences' rows are packed back to back into one forward
+ * pass (every GEMM and LayerNorm runs on the real rows only) and causal attention runs per sequence over packed sequences of
+ * different lengths.  The unpadded forms above still accept ragged lengths; they pad every sequence to the longest of the call.
+ *   ids      ids / d_ids: int32, the sequences back to back; sequence i starts at element sum_{j<i} lens[j].  lens: a HOST array of n
+ *            lengths.  clip_b200_text_batch_encode_packed takes clip_tokens as clip_text_batch_encode does.
+ *   vec      vec / d_vec [n, projection_dim]: the EOT row of each sequence (row len - 1, as the reference selects it).
+ *   out      ragged, item-major: item i is lens[i] rows of width elements (hidden_size, or projection_dim with PROJECT); it starts at
+ *            byte sum_{j<i} lens[j] * width * element size (16-byte aligned, as every CLIP width is a multiple of 8).  layer, flags
+ *            and out_type are those of clip_b200_text_tokens, with the same refusals; the ATTENTION flags are refused.
+ * Item i's outputs equal, byte for byte, sequence i passed alone to clip_b200_text_encode_device / clip_b200_text_tokens_device at
+ * seq_len = lens[i], and clip_text_batch_encode's row i for the same sequences, whatever the other sequences, their order and how the
+ * call is split into passes: a sequence holding ids that lead to NaN or Inf leaves the others' bits unchanged.
+ * A pass holds the longest prefix of the remaining sequences whose rows fit the workspace (micro_batch x context_length rows,
+ * clip_b200_set_micro_batch), so short sequences take proportionally more per pass.
+ * Text towers of head_dim 64 only (every CLIP text tower: ViT-B, L, H/14 and bigG/14); others are refused.
+ * Arguments are checked in this order, the first fault refused with a message in clip_b200_last_error() that starts with the
+ * form's name: 1. a null context; 2. the text tower; 3. a text head_dim other than 64; 4. n == 0 returns true; 5. null pointers:
+ * input, lens, then output; 6. each sequence's length in [1, context_length] (the message names the first bad sequence; a
+ * clip_tokens with NULL data or size 0 fails here); 7. tokens forms: the request, as clip_b200_text_tokens refuses it, then ATTENTION.
+ * Host forms: devices mode (CLIP_B200_DEVICES) shards the sequences by count as clip_text_batch_encode does; each pass's rows are
+ * copied to the host before the next pass runs. */
+bool clip_b200_text_batch_encode_packed(const struct clip_ctx * ctx, const struct clip_tokens * seqs, size_t n, float * vec,
+                                        bool normalize);
+bool clip_b200_text_encode_device_packed(const struct clip_ctx * ctx, const void * d_ids, size_t n, const int * lens, void * d_vec,
+                                         bool normalize);
+bool clip_b200_text_tokens_packed(const struct clip_ctx * ctx, const int32_t * ids, size_t n, const int * lens, int layer, int flags,
+                                  int out_type, void * out);
+bool clip_b200_text_tokens_device_packed(const struct clip_ctx * ctx, const void * d_ids, size_t n, const int * lens, int layer,
+                                         int flags, int out_type, void * d_out);
+
 /* Several layers' token rows from ONE forward pass of a tower (HF output_hidden_states returns all n_layer + 1; multi-layer VLM
  * connectors read 3 or 4 vision layers; SDXL reads layer -2 raw and the projected EOT row of layer -1 of the same text pass).
  *   layers[j], flags[j]  entry j: a layer and CLIP_B200_TOKENS_* flags exactly as `layer` / `flags` of the single-layer calls above.
@@ -634,6 +665,9 @@ int clip_b200_debug_attention_hd(int operand_bf16, int nseq, int T, int H, int h
  * the last sequence and 128 guard rows after the output are poisoned (0xFF).  Returns 2 for bad arguments, 5 for a launch or kernel
  * error, 6 if a guard row was written. */
 int clip_b200_debug_attention_mixed(int operand_bf16, int nseq, const int * lens, int H, int head_dim, const float * qkv, float * out);
+/* The same with the causal mask (the instance behind the text *_packed calls): head_dim 64 only, anything else returns 2. */
+int clip_b200_debug_attention_mixed_causal(int operand_bf16, int nseq, const int * lens, int H, int head_dim, const float * qkv,
+                                           float * out);
 /* The attention probabilities of the same qkv (the kernel behind CLIP_B200_TOKENS_ATTENTION): out [nseq, H, R, T] with R = T, or 1
  * with cls_row (query row 0 only), of out_type (0 fp32, 1 fp16, 2 bf16: raw 16-bit values, not widened).  Runs on device 0.  Returns
  * 2 for bad arguments (head_dim other than 64 / 80 / 104, a non-positive size, an unknown out_type), 5 if the kernel wrote into the
