@@ -30,6 +30,10 @@
 // the next head.  S takes 4 + 2 + 1 k16 steps, O n64 + n32 + n16 per 16 keys (56 accumulators).  A 224-byte row makes a 128-key
 // K / V tile 28 KB, so this instance runs 64-key blocks in a ring of three stages (225 KB of shared memory in all).
 // Any T; a causal group stops at its own diagonal.
+// One kernel, two schedules (Sched, a template argument folded away per instance): FIXED takes nseq sequences of T rows through
+// the 3-D view above; PACKED / PACKED_CAUSAL take sequences of different lengths stored back to back (VarLen) through a view of the
+// packed rows as one sequence, find each group's sequence by a forward gallop, and have the producer warp zero the V rows a box
+// brings in from past a sequence's end.
 #include <cuda.h>
 
 #include <type_traits>
@@ -67,12 +71,10 @@ struct AttnGeo {
     static constexpr uint32_t BOX_BYTES = ABOX * ROW_BYTES;                    // one 64-row box, every piece
     static constexpr uint32_t KV_OFF = 2 * TILE;
     static constexpr uint32_t BAR_OFF = KV_OFF + NST * 4 * KTILE;
-    static constexpr uint32_t SMEM = BAR_OFF + 32 + 16 * NST + 1024;
     // offsets of the mid and tail pieces in a tile of `rows` rows
     static constexpr uint32_t mid_off(int rows) { return (uint32_t)rows * 128; }
     static constexpr uint32_t tail_off(int rows) { return (uint32_t)rows * (128 + (MID ? 64 : 0)); }
     static_assert(2 * AG == AK && 2 * ABOX == AK && MAIN % 1024 == 0 && TILE % 1024 == 0 && KTILE % 1024 == 0, "tile alignment");
-    static_assert(SMEM <= 227 * 1024, "shared memory per block");
 };
 
 struct AParams {
@@ -99,17 +101,22 @@ CB_DEVINL uint32_t pack2(float lo, float hi) {
     return r;
 }
 
+// K3's schedules.  FIXED: nseq sequences of T rows each, through the 3-D view [sequence][token][column].  PACKED: sequences of
+// different lengths stored back to back (VarLen), through the same maps viewing the packed rows as one sequence; PACKED_CAUSAL: the
+// same with the causal mask (the text tower's packed passes, head_dim 64 only).
+enum Sched { FIXED, PACKED, PACKED_CAUSAL };
+
 // One group of 64 query rows: its (sequence, head), first row and the end of the keys any of its rows can see
 struct Group {
     int seq, head, g0, kend;
 };
 // A group of a packed causal sequence: its key end (min(len, g0 + 64)) and its sequence's length, which bounds the key mask and the
-// row stores, apart.  A type of its own, so that the non-causal varlen instances keep Group's layout and code.
+// row stores, apart.  A type of its own, so that the non-causal packed instances keep Group's layout and code.
 struct GroupLen : Group {
     int len;
 };
-template <bool CAUSAL>
-using VarGroup = std::conditional_t<CAUSAL, GroupLen, Group>;
+template <Sched S>
+using GroupOf = std::conditional_t<S == PACKED_CAUSAL, GroupLen, Group>;
 CB_DEVINL int seq_len(const Group& g) { return g.kend; }         // non-causal: the key end is the length
 CB_DEVINL int seq_len(const GroupLen& g) { return g.len; }
 CB_DEVINL Group group_of(const AParams& p, int g) {
@@ -122,20 +129,20 @@ CB_DEVINL Group group_of(const AParams& p, int g) {
     return r;
 }
 
-// Packed sequences of different lengths (launch_attention_tc_varlen): sequence s is rows [off[s], off[s + 1]) of one [row][column]
-// view of the qkv matrix, and its groups are numbered from H * grp[s] (grp: prefix sums of the per-sequence group counts ceil(len / 64)).
+// The packed schedules' sequences (launch_attention_tc_varlen): sequence s is rows [off[s], off[s + 1]) of one [row][column] view of
+// the qkv matrix, and its groups are numbered from H * grp[s] (grp: prefix sums of the per-sequence group counts ceil(len / 64)).
 struct VarLen {
     const int* off;
     const int* grp;
     int nseq;
 };
 
-// group_of for packed sequences.  Group::seq holds the sequence's first row (distinct for distinct sequences, so iter_var's test of a
-// shared (sequence, head) is iter_of's) and kend its length; causal, kend is the group's diagonal end as group_of has it and len the
+// group_of for packed sequences.  Group::seq holds the sequence's first row (distinct for distinct sequences, so iter_of's test of a
+// shared (sequence, head) holds) and kend its length; causal, kend is the group's diagonal end as group_of has it and len the
 // length.  s: a sequence at or before group g's, advanced to g's.  A thread's groups only increase, so the search gallops forward from the
 // last sequence found (one load when g is still in it) and ends in a binary search of the bracket.
-template <bool CAUSAL>
-CB_DEVINL VarGroup<CAUSAL> group_var(const AParams& p, const VarLen& v, int g, int& s) {
+template <Sched S>
+CB_DEVINL GroupOf<S> group_var(const AParams& p, const VarLen& v, int g, int& s) {
     int lo = s, step = 1;
     while (lo + step < v.nseq && __ldg(v.grp + lo + step) * p.H <= g) { lo += step; step *= 2; }
     int hi = min(lo + step, v.nseq) - 1;
@@ -146,12 +153,12 @@ CB_DEVINL VarGroup<CAUSAL> group_var(const AParams& p, const VarLen& v, int g, i
     }
     s = lo;
     const int ng = __ldg(v.grp + lo + 1) - __ldg(v.grp + lo), local = g - __ldg(v.grp + lo) * p.H;
-    VarGroup<CAUSAL> r;
+    GroupOf<S> r;
     r.head = local / ng;
     r.g0 = (local - r.head * ng) * AG;
     r.seq = __ldg(v.off + lo);
     r.kend = __ldg(v.off + lo + 1) - r.seq;
-    if constexpr (CAUSAL) {
+    if constexpr (S == PACKED_CAUSAL) {
         r.len = r.kend;
         r.kend = min(r.len, r.g0 + AG);
     }
@@ -167,27 +174,20 @@ struct IterOf {
     bool has_b, shared;
     int kend0, kend1, nkb;
 };
-using Iter = IterOf<Group>;
-template <int KB>
-CB_DEVINL Iter iter_of(const AParams& p, int it) {
-    Iter r;
-    r.has_b = 2 * it + 1 < p.ngroups;
-    r.a = group_of(p, 2 * it);
-    r.b = group_of(p, r.has_b ? 2 * it + 1 : 2 * it);
-    r.shared = r.a.seq == r.b.seq && r.a.head == r.b.head;
-    r.kend0 = r.shared ? max(r.a.kend, r.b.kend) : r.a.kend;
-    r.kend1 = r.shared ? 0 : r.b.kend;
-    r.nkb = (max(r.kend0, r.kend1) + KB - 1) / KB;
-    return r;
+// group g of schedule S (s: group_var's cursor)
+template <Sched S>
+CB_DEVINL GroupOf<S> group_at(const AParams& p, const VarLen& v, int g, int& s) {
+    if constexpr (S == FIXED) return group_of(p, g);
+    else return group_var<S>(p, v, g, s);
 }
-
-// iter_of for packed sequences (s: group_var's)
-template <int KB, bool CAUSAL>
-CB_DEVINL IterOf<VarGroup<CAUSAL>> iter_var(const AParams& p, const VarLen& v, int it, int& s) {
-    IterOf<VarGroup<CAUSAL>> r;
+// s: group_var's sequence cursor (packed schedules only)
+template <int KB, Sched S>
+CB_DEVINL IterOf<GroupOf<S>> iter_of(const AParams& p, const VarLen& v, int it, int& s) {
+    IterOf<GroupOf<S>> r;
     r.has_b = 2 * it + 1 < p.ngroups;
-    r.a = group_var<CAUSAL>(p, v, 2 * it, s);
-    r.b = r.has_b ? group_var<CAUSAL>(p, v, 2 * it + 1, s) : r.a;
+    r.a = group_at<S>(p, v, 2 * it, s);
+    // with no second group, FIXED recomputes the first and the packed schedules copy it (each instance's code as it always was)
+    r.b = S == FIXED || r.has_b ? group_at<S>(p, v, r.has_b ? 2 * it + 1 : 2 * it, s) : r.a;
     r.shared = r.a.seq == r.b.seq && r.a.head == r.b.head;
     r.kend0 = r.shared ? max(r.a.kend, r.b.kend) : r.a.kend;
     r.kend1 = r.shared ? 0 : r.b.kend;
@@ -320,158 +320,30 @@ CB_DEVINL void attend_block(float (&o)[32], float (&om)[16], float (&ot)[8], flo
     if constexpr (G::TAIL) wgmma_fence_regs(ot);
 }
 
-// tm_mid: head_dim 104's map of columns 64-95 (unused otherwise; a parameter of its own, so AParams keeps its layout)
-template <bool BF, int DH>
-__global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __grid_constant__ AParams p, const __grid_constant__ CUtensorMap tm_mid) {
+// Row r of the sequence whose Group::seq is `seq` has box coordinates (r, seq) in FIXED's 3-D view, (seq + r, 0) in the packed rows' view
+template <Sched S> CB_DEVINL int box_row0(int seq) { return S == FIXED ? 0 : seq; }
+template <Sched S> CB_DEVINL int box_seq(int seq) { return S == FIXED ? seq : 0; }
+
+// K3, in either schedule.  The packed schedules count a group's rows and keys from its sequence's first row and take its length for
+// T, so every key block and the width of the last one are those a FIXED launch of that sequence alone takes, and each kept row has its
+// arithmetic.  Their box rows past a sequence's end hold the next sequence's rows instead of zeros: their scores are masked by
+// select, their Q rows are never stored, but P.V would turn a non-finite V row into NaN (0 * Inf), so the producer warp zeroes those
+// V rows once the box has landed and before the consumers may read the stage: such a stage lands on a barrier of the producer's own
+// (kv_land), and the producer arrives on the stage's full barrier once the zeros are stored.
+// PACKED_CAUSAL: a group's keys end at min(len, g0 + 64), as group_of has them, and attend_block masks with T = len and causal = 1,
+// as a causal FIXED launch calls it.  A key end before the sequence's end is g0 + 64, a multiple of the 64-row box, so a slot's last
+// box then ends exactly at its key end: box rows past a key end, the rows the producer zeroes, still occur only at a sequence's end.
+// tm_mid: head_dim 104's map of columns 64-95 (unused otherwise; a parameter of its own, so AParams keeps its layout); v: the packed
+// schedules' sequences (unused by FIXED).
+template <bool BF, int DH, Sched S>
+__global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_kernel(const __grid_constant__ AParams p, const __grid_constant__ CUtensorMap tm_mid,
+                                                                      const VarLen v) {
     using G = AttnGeo<DH>;
+    constexpr bool PACK = S != FIXED;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     const uint32_t smem_base = smem_u32(smem);
-    // [i] = +8i bytes: Q tile full / empty (rings of two), K-V stage full / empty (rings of NST)
-    const uint32_t q_full = smem_base + G::BAR_OFF, q_empty = q_full + 16, kv_full = q_full + 32, kv_empty = kv_full + 8 * G::NST;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < G::NST; i++) {
-            if (i < 2) { mbar_init(q_full + 8 * i, 1); mbar_init(q_empty + 8 * i, 8); }      // released by each consumer warp
-            mbar_init(kv_full + 8 * i, 1); mbar_init(kv_empty + 8 * i, 8);
-        }
-        mbar_fence_init();
-        tma_prefetch_desc(&p.tm_qkv);
-        if constexpr (G::MID) tma_prefetch_desc(&tm_mid);
-        if constexpr (G::TAIL) tma_prefetch_desc(&p.tm_tail);
-    }
-    __syncthreads();
-    pdl_trigger();
-    pdl_wait();      // qkv is read (and the output written) only after the QKV GEMM grid has completed
-
-    const int hid = p.H * DH, qcols = p.H * G::DHP;           // output row, and Q / K / V part of a qkv row
-    // Ring positions run on across iterations: the i-th iteration of this CTA uses Q tile i % 2 (its (i / 2)-th use), the n-th key
-    // block of this CTA stage n % NST (its (n / NST)-th use).  A use waits for full with the use's parity and, in the producer, for the
-    // release of the previous use of the slot (parity flipped: the first wait on a fresh barrier passes).
-    if (warp == 8) {
-        // ------------------------------------------------------------------ producer (one thread)
-        if (lane == 0) {
-            uint32_t n = 0, i = 0;
-            for (int it = blockIdx.x; it < p.niter; it += gridDim.x, i++) {
-                const Iter w = iter_of<G::KB>(p, it);
-                const uint32_t qb = i & 1, q_s = smem_base + qb * G::TILE;
-                mbar_wait(q_empty + 8 * qb, ((i >> 1) & 1) ^ 1);
-                mbar_arrive_expect_tx(q_full + 8 * qb, (w.has_b ? 2 : 1) * G::BOX_BYTES);
-                load_box<DH, AK>(q_s, 0, p, tm_mid, w.a.head * G::DHP, w.a.g0, w.a.seq, q_full + 8 * qb);
-                if (w.has_b) load_box<DH, AK>(q_s, 1, p, tm_mid, w.b.head * G::DHP, w.b.g0, w.b.seq, q_full + 8 * qb);
-                for (int kb = 0; kb < w.nkb; kb++, n++) {
-                    const uint32_t s = n % G::NST, bar = kv_full + 8 * s;
-                    const int nb0 = kv_boxes<G::KB>(w.kend0, kb), nb1 = kv_boxes<G::KB>(w.kend1, kb);
-                    mbar_wait(kv_empty + 8 * s, ((n / G::NST) & 1) ^ 1);
-                    mbar_arrive_expect_tx(bar, (uint32_t)(nb0 + nb1) * 2 * G::BOX_BYTES);
-                    const uint32_t slot0 = smem_base + G::KV_OFF + s * (4 * G::KTILE), slot1 = slot0 + 2 * G::KTILE;
-                    for (int b = 0; b < nb0; b++) {
-                        load_box<DH, G::KB>(slot0, b, p, tm_mid, qcols + w.a.head * G::DHP, kb * G::KB + b * ABOX, w.a.seq, bar);
-                        load_box<DH, G::KB>(slot0 + G::KTILE, b, p, tm_mid, 2 * qcols + w.a.head * G::DHP, kb * G::KB + b * ABOX, w.a.seq, bar);
-                    }
-                    for (int b = 0; b < nb1; b++) {
-                        load_box<DH, G::KB>(slot1, b, p, tm_mid, qcols + w.b.head * G::DHP, kb * G::KB + b * ABOX, w.b.seq, bar);
-                        load_box<DH, G::KB>(slot1 + G::KTILE, b, p, tm_mid, 2 * qcols + w.b.head * G::DHP, kb * G::KB + b * ABOX, w.b.seq, bar);
-                    }
-                }
-            }
-        }
-        return;
-    }
-
-    // ---------------------------------------------------------------------- consumers (fragment layout: wgmma.cuh)
-    const int wg = warp >> 2;
-    const int tc = 2 * (lane & 3);                             // this thread: columns 8j + tc + {0, 1}
-    uint32_t n = 0, i = 0;
-    for (int it = blockIdx.x; it < p.niter; it += gridDim.x, i++) {
-        const Iter w = iter_of<G::KB>(p, it);
-        const Group g = group_of(p, min(2 * it + wg, p.ngroups - 1));
-        const bool live = wg == 0 || w.has_b;                  // warpgroup-uniform: only the launch's last, odd group leaves one idle
-        const uint32_t slot = (wg == 0 || w.shared) ? 0u : 1u;
-        const int nkb = (g.kend + G::KB - 1) / G::KB;
-        const int wrow0 = g.g0 + (warp & 3) * 16;              // first query row of this warp
-        const int r0 = wrow0 + (lane >> 2);                    // this thread: rows r0 and r0 + 8
-        // o: columns 0-63, om: 64-95 (head_dim 104 only), ot: the 16-column tail (head_dim 80, 104)
-        float o[32], om[16], ot[8], m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-        #pragma unroll
-        for (int j = 0; j < 32; j++) o[j] = 0.f;
-        #pragma unroll
-        for (int j = 0; j < 16; j++) om[j] = 0.f;
-        #pragma unroll
-        for (int j = 0; j < 8; j++) ot[j] = 0.f;
-        const uint32_t qb = i & 1, q_s = smem_base + qb * G::TILE;
-        mbar_wait(q_full + 8 * qb, (i >> 1) & 1);
-        const uint64_t dq = wgmma_desc_sw128(q_s + (uint32_t)wg * 64u * 128u);
-        const uint64_t dq_m = wgmma_desc_sw64(q_s + G::mid_off(AK) + (uint32_t)wg * 64u * 64u);
-        const uint64_t dq_t = wgmma_desc_sw32(q_s + G::tail_off(AK) + (uint32_t)wg * 64u * 32u);
-        for (int kb = 0; kb < w.nkb; kb++, n++) {
-            const uint32_t s = n % G::NST;
-            const uint32_t k_s = smem_base + G::KV_OFF + s * (4 * G::KTILE) + slot * (2 * G::KTILE), v_s = k_s + G::KTILE;
-            mbar_wait(kv_full + 8 * s, (n / G::NST) & 1);
-            if (live && kb < nkb) {
-                const int key0 = kb * G::KB, rem = g.kend - key0;
-                // S at the narrowest width that covers the keys left (a 64-key block never needs 128)
-                if (G::KB == 128 && rem > 64) attend_block<BF, DH, 16>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
-                else if (rem > 32) attend_block<BF, DH, 8>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
-                else if (rem > 16) attend_block<BF, DH, 4>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
-                else attend_block<BF, DH, 2>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, p.T, p.causal, wrow0, r0, tc);
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(kv_empty + 8 * s);
-        }
-        // every S product that read this Q tile has completed (wgmma_wait<0> in attend_block)
-        __syncwarp();
-        if (lane == 0) mbar_arrive(q_empty + 8 * qb);
-        if (!live) continue;
-        #pragma unroll
-        for (int h = 0; h < 2; h++) {
-            float l = l_run[h];
-            l += __shfl_xor_sync(0xffffffffu, l, 1);
-            l += __shfl_xor_sync(0xffffffffu, l, 2);
-            const float inv = 1.0f / l;
-            const int row = r0 + 8 * h;
-            if (row < p.T) {
-                uint16_t* orow = p.out + ((size_t)g.seq * p.T + row) * hid + g.head * DH;
-                #pragma unroll
-                for (int j = 0; j < 8; j++)
-                    *reinterpret_cast<uint32_t*>(orow + 8 * j + tc) = pack2<BF>(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
-                if constexpr (G::MID) {
-                    #pragma unroll
-                    for (int j = 0; j < 4; j++)
-                        *reinterpret_cast<uint32_t*>(orow + 64 + 8 * j + tc) = pack2<BF>(om[4 * j + 2 * h] * inv, om[4 * j + 2 * h + 1] * inv);
-                }
-                if constexpr (G::TAIL) {
-                    // the real tail columns only: at head_dim 104, columns 104-111 are the padding
-                    #pragma unroll
-                    for (int j = 0; j < (DH - G::tail_col()) / 8; j++)
-                        *reinterpret_cast<uint32_t*>(orow + G::tail_col() + 8 * j + tc) = pack2<BF>(ot[4 * j + 2 * h] * inv, ot[4 * j + 2 * h + 1] * inv);
-                }
-            }
-        }
-    }
-}
-
-// K3 on packed sequences of different lengths (VarLen): the kernel above with the maps viewing the packed rows as one
-// sequence.  A group's rows and keys are counted from its sequence's first row, its length takes the place of T, so every key block
-// and the width of the last one are those a fixed-T launch of that sequence alone takes, and each kept row has its arithmetic.  The box rows past a
-// sequence's end now hold the next sequence's rows instead of zeros: their scores are masked by select, their Q rows are never
-// stored, but P.V would turn a non-finite V row into NaN (0 * Inf), so the producer warp zeroes those V rows once the box has landed
-// and before the consumers may read the stage: such a stage lands on a barrier of the producer's own, and the producer arrives on
-// the stage's full barrier once the zeros are stored.
-// CAUSAL (the text tower's packed passes, head_dim 64 only): a group's keys end at min(len, g0 + 64), as group_of has them, and
-// attend_block masks with T = len and causal = 1, as the fixed-T causal kernel calls it.  A key end before the sequence's end is
-// g0 + 64, a multiple of the 64-row box, so a slot's last box then ends exactly at its key end: box rows past a key end, the rows
-// the producer zeroes, still occur only at a sequence's end.
-template <bool BF, int DH, bool CAUSAL>
-__global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(const __grid_constant__ AParams p, const __grid_constant__ CUtensorMap tm_mid,
-                                                                             const VarLen v) {
-    using G = AttnGeo<DH>;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    const uint32_t smem_base = smem_u32(smem);
-    // [i] = +8i bytes: Q tile full / empty (rings of two), K-V stage full / empty (rings of NST); kv_land: the producer's own barrier
-    // for a stage it zeroes before the consumers may read it
+    // [i] = +8i bytes: Q tile full / empty (rings of two), K-V stage full / empty (rings of NST), then (packed) kv_land
     const uint32_t q_full = smem_base + G::BAR_OFF, q_empty = q_full + 16, kv_full = q_full + 32, kv_empty = kv_full + 8 * G::NST;
     const uint32_t kv_land = kv_empty + 8 * G::NST;
 
@@ -481,7 +353,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(con
             if (i < 2) { mbar_init(q_full + 8 * i, 1); mbar_init(q_empty + 8 * i, 8); }      // released by each consumer warp
             mbar_init(kv_full + 8 * i, 1); mbar_init(kv_empty + 8 * i, 8);
         }
-        mbar_init(kv_land, 1);
+        if constexpr (PACK) mbar_init(kv_land, 1);
         mbar_fence_init();
         tma_prefetch_desc(&p.tm_qkv);
         if constexpr (G::MID) tma_prefetch_desc(&tm_mid);
@@ -496,47 +368,65 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(con
     // block of this CTA stage n % NST (its (n / NST)-th use).  A use waits for full with the use's parity and, in the producer, for the
     // release of the previous use of the slot (parity flipped: the first wait on a fresh barrier passes).
     if (warp == 8) {
-        // ------------------------------------------------------------------ producer (one warp)
-        // lane 0 issues the loads.  A stage that holds a sequence's last block lands on kv_land instead of kv_full; the whole warp
-        // waits for it, zeroes the V rows past the sequence's end and only then arrives on kv_full.  nz: such stages so far.
+        // ------------------------------------------------------------------ producer
+        // FIXED: one thread.  Packed: one warp, of which lane 0 issues the loads.  A stage that holds a sequence's last block lands
+        // on kv_land instead of kv_full; the whole warp waits for it, zeroes the V rows past the sequence's end and only then arrives
+        // on kv_full.  nz: such stages so far.
+        if (!PACK && lane != 0) return;
         uint32_t n = 0, i = 0, nz = 0;
         int sq = 0;
         for (int it = blockIdx.x; it < p.niter; it += gridDim.x, i++) {
-            const auto w = iter_var<G::KB, CAUSAL>(p, v, it, sq);
+            const auto w = iter_of<G::KB, S>(p, v, it, sq);
             const uint32_t qb = i & 1, q_s = smem_base + qb * G::TILE;
             if (lane == 0) {
                 mbar_wait(q_empty + 8 * qb, ((i >> 1) & 1) ^ 1);
                 mbar_arrive_expect_tx(q_full + 8 * qb, (w.has_b ? 2 : 1) * G::BOX_BYTES);
-                load_box<DH, AK>(q_s, 0, p, tm_mid, w.a.head * G::DHP, w.a.seq + w.a.g0, 0, q_full + 8 * qb);
-                if (w.has_b) load_box<DH, AK>(q_s, 1, p, tm_mid, w.b.head * G::DHP, w.b.seq + w.b.g0, 0, q_full + 8 * qb);
+                load_box<DH, AK>(q_s, 0, p, tm_mid, w.a.head * G::DHP, box_row0<S>(w.a.seq) + w.a.g0, box_seq<S>(w.a.seq), q_full + 8 * qb);
+                if (w.has_b) load_box<DH, AK>(q_s, 1, p, tm_mid, w.b.head * G::DHP, box_row0<S>(w.b.seq) + w.b.g0, box_seq<S>(w.b.seq), q_full + 8 * qb);
             }
             for (int kb = 0; kb < w.nkb; kb++, n++) {
-                const uint32_t s = n % G::NST;
-                const int nb0 = kv_boxes<G::KB>(w.kend0, kb), nb1 = kv_boxes<G::KB>(w.kend1, kb);
-                const uint32_t slot0 = smem_base + G::KV_OFF + s * (4 * G::KTILE), slot1 = slot0 + 2 * G::KTILE;
-                const int z0 = kv_pad_rows<G::KB>(w.kend0, kb), z1 = kv_pad_rows<G::KB>(w.kend1, kb);
-                const uint32_t bar = (z0 || z1) ? kv_land : kv_full + 8 * s;
-                if (lane == 0) {
+                // the stage's slots and the barrier its loads land on, each schedule in its own order (FIXED's one thread takes
+                // the slots after the wait): the instances' register allocation depends on it.  z0 / z1: V rows the warp zeroes.
+                uint32_t s, bar, slot0, slot1;
+                int nb0, nb1, z0 = 0, z1 = 0;
+                if constexpr (!PACK) {
+                    s = n % G::NST; bar = kv_full + 8 * s;
+                    nb0 = kv_boxes<G::KB>(w.kend0, kb); nb1 = kv_boxes<G::KB>(w.kend1, kb);
                     mbar_wait(kv_empty + 8 * s, ((n / G::NST) & 1) ^ 1);
                     mbar_arrive_expect_tx(bar, (uint32_t)(nb0 + nb1) * 2 * G::BOX_BYTES);
+                    slot0 = smem_base + G::KV_OFF + s * (4 * G::KTILE); slot1 = slot0 + 2 * G::KTILE;
+                } else {
+                    s = n % G::NST;
+                    nb0 = kv_boxes<G::KB>(w.kend0, kb); nb1 = kv_boxes<G::KB>(w.kend1, kb);
+                    slot0 = smem_base + G::KV_OFF + s * (4 * G::KTILE); slot1 = slot0 + 2 * G::KTILE;
+                    z0 = kv_pad_rows<G::KB>(w.kend0, kb); z1 = kv_pad_rows<G::KB>(w.kend1, kb);
+                    bar = (z0 || z1) ? kv_land : kv_full + 8 * s;
+                }
+                if (lane == 0) {
+                    if constexpr (PACK) {
+                        mbar_wait(kv_empty + 8 * s, ((n / G::NST) & 1) ^ 1);
+                        mbar_arrive_expect_tx(bar, (uint32_t)(nb0 + nb1) * 2 * G::BOX_BYTES);
+                    }
                     for (int b = 0; b < nb0; b++) {
-                        load_box<DH, G::KB>(slot0, b, p, tm_mid, qcols + w.a.head * G::DHP, w.a.seq + kb * G::KB + b * ABOX, 0, bar);
-                        load_box<DH, G::KB>(slot0 + G::KTILE, b, p, tm_mid, 2 * qcols + w.a.head * G::DHP, w.a.seq + kb * G::KB + b * ABOX, 0, bar);
+                        load_box<DH, G::KB>(slot0, b, p, tm_mid, qcols + w.a.head * G::DHP, box_row0<S>(w.a.seq) + kb * G::KB + b * ABOX, box_seq<S>(w.a.seq), bar);
+                        load_box<DH, G::KB>(slot0 + G::KTILE, b, p, tm_mid, 2 * qcols + w.a.head * G::DHP, box_row0<S>(w.a.seq) + kb * G::KB + b * ABOX, box_seq<S>(w.a.seq), bar);
                     }
                     for (int b = 0; b < nb1; b++) {
-                        load_box<DH, G::KB>(slot1, b, p, tm_mid, qcols + w.b.head * G::DHP, w.b.seq + kb * G::KB + b * ABOX, 0, bar);
-                        load_box<DH, G::KB>(slot1 + G::KTILE, b, p, tm_mid, 2 * qcols + w.b.head * G::DHP, w.b.seq + kb * G::KB + b * ABOX, 0, bar);
+                        load_box<DH, G::KB>(slot1, b, p, tm_mid, qcols + w.b.head * G::DHP, box_row0<S>(w.b.seq) + kb * G::KB + b * ABOX, box_seq<S>(w.b.seq), bar);
+                        load_box<DH, G::KB>(slot1 + G::KTILE, b, p, tm_mid, 2 * qcols + w.b.head * G::DHP, box_row0<S>(w.b.seq) + kb * G::KB + b * ABOX, box_seq<S>(w.b.seq), bar);
                     }
                 }
-                __syncwarp();
-                if (z0 || z1) {
-                    mbar_wait(kv_land, nz++ & 1);
-                    if (z0) zero_tile_rows<DH>(slot0 + G::KTILE, nb0 * ABOX - z0, nb0 * ABOX, lane);
-                    if (z1) zero_tile_rows<DH>(slot1 + G::KTILE, nb1 * ABOX - z1, nb1 * ABOX, lane);
-                    // the zeros (generic proxy) before the consumers' wgmma reads and the next TMA into the stage (async proxy)
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                if constexpr (PACK) {
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(kv_full + 8 * s);
+                    if (z0 || z1) {
+                        mbar_wait(kv_land, nz++ & 1);
+                        if (z0) zero_tile_rows<DH>(slot0 + G::KTILE, nb0 * ABOX - z0, nb0 * ABOX, lane);
+                        if (z1) zero_tile_rows<DH>(slot1 + G::KTILE, nb1 * ABOX - z1, nb1 * ABOX, lane);
+                        // the zeros (generic proxy) before the consumers' wgmma reads and the next TMA into the stage (async proxy)
+                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(kv_full + 8 * s);
+                    }
                 }
             }
         }
@@ -550,12 +440,15 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(con
     int sq = 0;
     for (int it = blockIdx.x; it < p.niter; it += gridDim.x, i++) {
         const int sq_it = sq;                                  // at or before both groups' sequences
-        const auto w = iter_var<G::KB, CAUSAL>(p, v, it, sq);
-        const auto g = (wg == 0 || !w.has_b) ? w.a : w.b;
+        const auto w = iter_of<G::KB, S>(p, v, it, sq);
+        // this warpgroup's group: the same value either way, but each form gives its instances their register allocation
+        GroupOf<S> g;
+        if constexpr (PACK) g = (wg == 0 || !w.has_b) ? w.a : w.b;
+        else g = group_of(p, min(2 * it + wg, p.ngroups - 1));
         const bool live = wg == 0 || w.has_b;                  // warpgroup-uniform: only the launch's last, odd group leaves one idle
         const uint32_t slot = (wg == 0 || w.shared) ? 0u : 1u;
         const int nkb = (g.kend + G::KB - 1) / G::KB;
-        const int len = seq_len(g);                            // the sequence's length: the key mask and the row stores
+        const int len = PACK ? seq_len(g) : p.T;               // the sequence's length: the key mask and the row stores
         const int wrow0 = g.g0 + (warp & 3) * 16;              // first query row of this warp
         const int r0 = wrow0 + (lane >> 2);                    // this thread: rows r0 and r0 + 8
         // o: columns 0-63, om: 64-95 (head_dim 104 only), ot: the 16-column tail (head_dim 80, 104)
@@ -576,12 +469,12 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(con
             const uint32_t k_s = smem_base + G::KV_OFF + s * (4 * G::KTILE) + slot * (2 * G::KTILE), v_s = k_s + G::KTILE;
             mbar_wait(kv_full + 8 * s, (n / G::NST) & 1);
             if (live && kb < nkb) {
-                const int key0 = kb * G::KB, rem = g.kend - key0;
+                const int key0 = kb * G::KB, rem = g.kend - key0, causal = PACK ? S == PACKED_CAUSAL : p.causal;
                 // S at the narrowest width that covers the keys left (a 64-key block never needs 128)
-                if (G::KB == 128 && rem > 64) attend_block<BF, DH, 16>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, len, CAUSAL ? 1 : 0, wrow0, r0, tc);
-                else if (rem > 32) attend_block<BF, DH, 8>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, len, CAUSAL ? 1 : 0, wrow0, r0, tc);
-                else if (rem > 16) attend_block<BF, DH, 4>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, len, CAUSAL ? 1 : 0, wrow0, r0, tc);
-                else attend_block<BF, DH, 2>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, len, CAUSAL ? 1 : 0, wrow0, r0, tc);
+                if (G::KB == 128 && rem > 64) attend_block<BF, DH, 16>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, len, causal, wrow0, r0, tc);
+                else if (rem > 32) attend_block<BF, DH, 8>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, len, causal, wrow0, r0, tc);
+                else if (rem > 16) attend_block<BF, DH, 4>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, len, causal, wrow0, r0, tc);
+                else attend_block<BF, DH, 2>(o, om, ot, m_run, l_run, dq, dq_m, dq_t, k_s, v_s, key0, len, causal, wrow0, r0, tc);
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(kv_empty + 8 * s);
@@ -590,10 +483,16 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(con
         __syncwarp();
         if (lane == 0) mbar_arrive(q_empty + 8 * qb);
         if (!live) continue;
-        // the group's first row and head looked up again rather than held in registers through the key loop (the head_dim 80
+        // packed: the group's first row and head looked up again rather than held in registers through the key loop (the head_dim 80
         // instance has none to spare at 168, the most 288 threads can have)
-        int sq_e = sq_it;
-        const auto ge = group_var<CAUSAL>(p, v, 2 * it + wg, sq_e);
+        const auto ge = [&] {
+            if constexpr (PACK) {
+                int sq_e = sq_it;
+                return group_var<S>(p, v, 2 * it + wg, sq_e);
+            } else {
+                return g;
+            }
+        }();
         #pragma unroll
         for (int h = 0; h < 2; h++) {
             float l = l_run[h];
@@ -602,7 +501,7 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(con
             const float inv = 1.0f / l;
             const int row = r0 + 8 * h;
             if (row < len) {
-                uint16_t* orow = p.out + ((size_t)ge.seq + row) * hid + ge.head * DH;
+                uint16_t* orow = p.out + (PACK ? (size_t)ge.seq + row : (size_t)ge.seq * p.T + row) * hid + ge.head * DH;
                 #pragma unroll
                 for (int j = 0; j < 8; j++)
                     *reinterpret_cast<uint32_t*>(orow + 8 * j + tc) = pack2<BF>(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
@@ -622,9 +521,9 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attention_tc_varlen_kernel(con
     }
 }
 
-// the varlen kernel's shared memory: one more barrier (kv_land)
-template <int DH>
-constexpr uint32_t varlen_smem() { return AttnGeo<DH>::SMEM + 8; }
+// an instance's shared memory: AttnGeo's tiles, its barriers (the packed schedules' kv_land too) and the slack for 1024-byte alignment
+template <int DH, Sched S>
+constexpr uint32_t k3_smem() { return AttnGeo<DH>::BAR_OFF + 32 + 16 * AttnGeo<DH>::NST + (S == FIXED ? 0 : 8) + 1024; }
 
 // ---- K9: the attention probabilities themselves (the *_tokens calls' ATTENTION entries) ------------------------------------------
 // softmax(Q.K^T [causal]) of one block, recomputed from the qkv matrix K3 read (Q scaled by 1/sqrt(dh) and rounded, K 16-bit) through
@@ -880,40 +779,48 @@ bool make_piece_maps(AParams& p, CUtensorMap& tm_mid, const void* qkv16, int nse
     return dh == 64 || make_qkv_map(&p.tm_tail, qkv16, nseq, T, H, dh, 16, CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
+template <int DH, Sched S>
+cudaError_t set_k3_smem() {
+    const cudaError_t e = cudaFuncSetAttribute(attention_tc_kernel<true, DH, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k3_smem<DH, S>());
+    return e != cudaSuccess ? e : cudaFuncSetAttribute(attention_tc_kernel<false, DH, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k3_smem<DH, S>());
+}
+
 template <int DH>
 cudaError_t set_smem() {
-    cudaError_t e = cudaFuncSetAttribute(attention_tc_kernel<true, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AttnGeo<DH>::SMEM);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attention_tc_kernel<false, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AttnGeo<DH>::SMEM);
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attention_tc_varlen_kernel<true, DH, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)varlen_smem<DH>());
-    if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(attention_tc_varlen_kernel<false, DH, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)varlen_smem<DH>());
-    if (e != cudaSuccess) return e;
+    cudaError_t e = set_k3_smem<DH, FIXED>();
+    if (e == cudaSuccess) e = set_k3_smem<DH, PACKED>();
     if constexpr (DH == 64) {
-        e = cudaFuncSetAttribute(attention_tc_varlen_kernel<true, DH, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)varlen_smem<DH>());
-        if (e != cudaSuccess) return e;
-        e = cudaFuncSetAttribute(attention_tc_varlen_kernel<false, DH, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)varlen_smem<DH>());
-        if (e != cudaSuccess) return e;
+        if (e == cudaSuccess) e = set_k3_smem<DH, PACKED_CAUSAL>();
     }
-    e = cudaFuncSetAttribute(attention_probs_kernel<true, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ProbsGeo<DH>::SMEM);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(attention_probs_kernel<true, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ProbsGeo<DH>::SMEM);
+    return e != cudaSuccess ? e : cudaFuncSetAttribute(attention_probs_kernel<false, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ProbsGeo<DH>::SMEM);
+}
+
+template <int DH, Sched S>
+cudaError_t launch_dh(const AParams& p, const CUtensorMap& tm_mid, const VarLen& v, unsigned grid, int bf16, cudaStream_t st) {
+    constexpr uint32_t smem = k3_smem<DH, S>();
+    static_assert(smem <= 227 * 1024, "shared memory per block");
+    return bf16 ? launch_pdl(attention_tc_kernel<true, DH, S>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid, v)
+                : launch_pdl(attention_tc_kernel<false, DH, S>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid, v);
+}
+
+// What both K3 launchers share once p's maps, out, T, H and causal (and FIXED's ngrp) are set: the group count, the grid and the
+// dispatch on dh (PACKED_CAUSAL: 64 only) and bf16
+template <Sched S>
+cudaError_t launch_k3(AParams& p, const CUtensorMap& tm_mid, const VarLen& v, long long ngroups, int dh, int bf16, cudaStream_t st) {
+    if (ngroups > 0x7ffffffell) return cudaErrorInvalidValue;
+    p.ngroups = (int)ngroups;
+    p.niter = (p.ngroups + 1) / 2;
+    // persistent: at most one CTA per SM (the shared memory admits no second one)
+    int dev = 0, sms = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(attention_probs_kernel<false, DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ProbsGeo<DH>::SMEM);
-}
-
-template <int DH>
-cudaError_t launch_dh(const AParams& p, const CUtensorMap& tm_mid, unsigned grid, int bf16, cudaStream_t st) {
-    constexpr uint32_t smem = AttnGeo<DH>::SMEM;
-    return bf16 ? launch_pdl(attention_tc_kernel<true, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid)
-                : launch_pdl(attention_tc_kernel<false, DH>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid);
-}
-
-template <int DH, bool CAUSAL>
-cudaError_t launch_varlen_dh(const AParams& p, const CUtensorMap& tm_mid, const VarLen& v, unsigned grid, int bf16, cudaStream_t st) {
-    static_assert(varlen_smem<DH>() <= 227 * 1024, "shared memory per block");
-    constexpr uint32_t smem = varlen_smem<DH>();
-    return bf16 ? launch_pdl(attention_tc_varlen_kernel<true, DH, CAUSAL>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid, v)
-                : launch_pdl(attention_tc_varlen_kernel<false, DH, CAUSAL>, grid, (unsigned)ATT_THREADS, smem, st, 1, p, tm_mid, v);
+    const unsigned grid = (unsigned)min(p.niter, sms);
+    if constexpr (S == PACKED_CAUSAL) e = launch_dh<64, S>(p, tm_mid, v, grid, bf16, st);
+    else e = dh == 104 ? launch_dh<104, S>(p, tm_mid, v, grid, bf16, st) : dh == 80 ? launch_dh<80, S>(p, tm_mid, v, grid, bf16, st)
+                                                                         : launch_dh<64, S>(p, tm_mid, v, grid, bf16, st);
+    return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 template <int DH>
@@ -942,18 +849,7 @@ cudaError_t launch_attention_tc(const void* qkv16, void* out16, int nseq, int T,
     if (!make_piece_maps(p, tm_mid, qkv16, nseq, T, H, dh)) return cudaErrorInvalidValue;
     p.out = (uint16_t*)out16; p.T = T; p.H = H; p.causal = causal;
     p.ngrp = (T + AG - 1) / AG;
-    const long long ngroups = (long long)nseq * H * p.ngrp;
-    if (ngroups > 0x7ffffffell) return cudaErrorInvalidValue;
-    p.ngroups = (int)ngroups;
-    p.niter = (p.ngroups + 1) / 2;
-    // persistent: at most one CTA per SM (the shared memory admits no second one)
-    int dev = 0, sms = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (e != cudaSuccess) return e;
-    const unsigned grid = (unsigned)min(p.niter, sms);
-    e = dh == 104 ? launch_dh<104>(p, tm_mid, grid, bf16, st) : dh == 80 ? launch_dh<80>(p, tm_mid, grid, bf16, st) : launch_dh<64>(p, tm_mid, grid, bf16, st);
-    return e != cudaSuccess ? e : cudaGetLastError();
+    return launch_k3<FIXED>(p, tm_mid, VarLen{}, (long long)nseq * H * p.ngrp, dh, bf16, st);
 }
 
 cudaError_t launch_attention_tc_varlen(const void* qkv16, void* out16, int rows, int nseq, const int* d_seq, int groups, int H, int dh, int causal,
@@ -965,20 +861,9 @@ cudaError_t launch_attention_tc_varlen(const void* qkv16, void* out16, int rows,
     memset(&p, 0, sizeof(p));
     if (!make_piece_maps(p, tm_mid, qkv16, 1, rows, H, dh)) return cudaErrorInvalidValue;
     p.out = (uint16_t*)out16; p.T = rows; p.H = H; p.causal = causal;
-    const long long ngroups = (long long)groups * H;
-    if (ngroups > 0x7ffffffell) return cudaErrorInvalidValue;
-    p.ngroups = (int)ngroups;
-    p.niter = (p.ngroups + 1) / 2;
     const VarLen v{d_seq, d_seq + nseq + 1, nseq};
-    int dev = 0, sms = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (e != cudaSuccess) return e;
-    const unsigned grid = (unsigned)min(p.niter, sms);
-    e = causal ? launch_varlen_dh<64, true>(p, tm_mid, v, grid, bf16, st)
-        : dh == 104 ? launch_varlen_dh<104, false>(p, tm_mid, v, grid, bf16, st) : dh == 80 ? launch_varlen_dh<80, false>(p, tm_mid, v, grid, bf16, st)
-                  : launch_varlen_dh<64, false>(p, tm_mid, v, grid, bf16, st);
-    return e != cudaSuccess ? e : cudaGetLastError();
+    const long long ngroups = (long long)groups * H;
+    return causal ? launch_k3<PACKED_CAUSAL>(p, tm_mid, v, ngroups, dh, bf16, st) : launch_k3<PACKED>(p, tm_mid, v, ngroups, dh, bf16, st);
 }
 
 cudaError_t launch_attention_probs(const void* qkv16, void* out, int elem_type, int nseq, int T, int H, int dh, int causal, int cls_only,
