@@ -662,8 +662,9 @@ bool ensure_buf(clip_ctx* c, T** buf, size_t* cap, size_t count) {
 bool ensure_out(clip_ctx* c, size_t floats) { return ensure_buf(c, &c->d_out, &c->d_out_cap, floats); }
 
 int default_micro_batch(int T) {   // 33 token tiles = 132/4: every N/128 that is a multiple of 4 fills whole waves of the H100's SMs
-    // Fewer, longer launches: each launch pays a drain/fill gap of a few microseconds.  12 waves = 295 ViT-L/14 images = 1.7 GB of workspace.
-    int waves = 12;
+    // Fewer, longer launches: each launch pays a drain/fill gap of a few microseconds.  9 x 33 tiles of 256 rows = 295 ViT-L/14 images
+    // = 1.7 GB of workspace.
+    int waves = 9;
     if (const char* e = getenv("CLIP_B200_TOKEN_TILES_X33")) waves = std::max(1, atoi(e));
     const int mb = 33 * waves * GEMM_BN / T;
     return mb < 1 ? 1 : mb;

@@ -16,7 +16,7 @@ bool make_tma_2d_16bit(TmaMap* out, const void* gptr, uint64_t rows, uint64_t co
                        uint32_t box_rows);
 
 constexpr int GEMM_BM = 128;   // features per tile (two wgmma M = 64 warpgroups)
-constexpr int GEMM_BN = 192;   // tokens per tile   (wgmma N; 96 fp32 accumulator registers per thread)
+constexpr int GEMM_BN = 256;   // tokens per tile   (wgmma N; 128 fp32 accumulator registers per thread)
 constexpr int GEMM_BK = 64;
 
 struct GemmArgs {

@@ -6,14 +6,14 @@
 //   Y[token, feature] = sum_k X[token, k] * W[feature, k]  (+ bias, + epilogue)
 //
 // computed "swap-AB": the WEIGHT tile is the wgmma A operand (M = 128 features, 64 per consumer warpgroup), the ACTIVATION tile is
-// the B operand (N = 192 tokens); fp32 accumulators live in registers (96 per thread).  Persistent CTA, one per SM, 384 threads; the
+// the B operand (N = 256 tokens); fp32 accumulators live in registers (128 per thread).  Persistent CTA, one per SM, 384 threads; the
 // producer warpgroup hands its registers to the consumers (setmaxnreg 40 / 232):
 //   warp 8      producer, one thread: per k-block ONE 1-D bulk copy of the packed 32-weight blocks + scales of the [128 x 64] weight
-//               tile (wpack.h) into the Q ring, and a TMA box of the activation tile [192 tokens x 64 k] (128-B swizzle) into the X
+//               tile (wpack.h) into the Q ring, and a TMA box of the activation tile [256 tokens x 64 k] (128-B swizzle) into the X
 //               ring; unquantized f16 weights come as a second TMA box [128 features x 64 k] in the same X stage instead
 //   warps 0-7   two consumer warpgroups; group g owns features [64 g, 64 g + 64) of the tile.  Quantized weights never exist unpacked in
 //               shared memory: every lane dequantises exactly the 16-bit pairs of its own wgmma A fragments (2 rows x 16 k per k-block)
-//               from the packed chunk into registers, and the group issues 4 register-A wgmma m64n192k16 per k-block (B = activation
+//               from the packed chunk into registers, and the group issues 4 register-A wgmma m64n256k16 per k-block (B = activation
 //               tile from shared memory), keeping one k-block of MMAs in flight while it unpacks the next.  f16 weights: both operands
 //               from shared memory.  Epilogue: bias / scale / GELU computed from the accumulator registers, written in chunks into a
 //               ring of swizzled staging slots in shared memory and sent out by bulk tensor stores that drain while the group runs
@@ -33,7 +33,7 @@ namespace cb {
 namespace {
 
 constexpr int BM = GEMM_BM, BN = GEMM_BN, BK = GEMM_BK;
-constexpr int X_STAGE = BN * BK * 2;   // 24576 B
+constexpr int X_STAGE = BN * BK * 2;   // 32768 B
 constexpr int W_STAGE = BM * BK * 2;   // 16384 B (f16 path only)
 constexpr int THREADS = 384;           // 2 consumer warpgroups + 1 producer warpgroup (one thread of it issues the copies)
 static_assert(X_STAGE % 1024 == 0 && W_STAGE % 1024 == 0, "swizzled stage alignment");
@@ -42,20 +42,22 @@ __host__ __device__ constexpr uint32_t chunk_bytes(int qt) {
     return qt == 2 ? 4608u : qt == 3 ? 5120u : qt == 6 ? 5632u : qt == 7 ? 6144u : qt == 8 ? 8704u : 0u;
 }
 constexpr uint32_t E_SLOT = 4096;   // one epilogue staging slot (epilogue_staged)
-// shared-memory plan per weight type (fits the 227 KB carve-out): X ring, packed-weight ring, epilogue staging (SE slots per consumer
-// group, as many as the rings leave room for), barriers.  q8_0's Q ring is one chunk shallower than the others' to make room for two
-// slots per group: the producer issues Q(kb) just before it waits for X(kb)'s stage, and the consumers release a Q chunk a k-block
-// before its X stage, so with 6 X stages no more than 7 Q chunks are ever in use.
+// Shared-memory plan per weight type (fits the 227 KB carve-out): X ring, packed-weight ring, epilogue staging (SE slots per consumer
+// group, as many as the rings leave room for), barriers.  The producer issues Q(kb) just before it waits for X(kb)'s stage, and the
+// consumers release a Q chunk a k-block before its X stage, so no more than SX + 1 Q chunks are ever in use: the Q ring is that deep.
+//   q4_0  4 x 32 KB X + 5 x 4.5 KB Q + 2 x 9 x 4 KB        q5_1  4 x 32 KB X + 5 x 6 KB Q + 2 x 8 x 4 KB
+//   q4_1  4 x 32 KB X + 5 x 5 KB Q + 2 x 9 x 4 KB          q8_0  4 x 32 KB X + 5 x 8.5 KB Q + 2 x 6 x 4 KB
+//   q5_0  4 x 32 KB X + 5 x 5.5 KB Q + 2 x 8 x 4 KB        f16   4 x 48 KB (X + W) + 2 x 4 x 4 KB
 template <int QT>
 struct Cfg {
     static constexpr bool DQ = (QT != QT_F16);
     static constexpr uint32_t CHUNK = chunk_bytes(QT);
-    static constexpr int SX = DQ ? 6 : 5;                              // X ring (f16: X + W per stage)
-    static constexpr int SQ = !DQ ? 0 : QT == QT_Q8_0 ? 7 : 8;         // packed-weight ring
-    static constexpr int SE = !DQ ? 3 : QT == QT_Q8_0 ? 2 : (QT == QT_Q4_0 || QT == QT_Q4_1) ? 5 : 4;
+    static constexpr int SX = 4;                                       // X ring (f16: X + W per stage)
+    static constexpr int SQ = DQ ? SX + 1 : 0;                         // packed-weight ring
     static constexpr uint32_t XS = DQ ? (uint32_t)X_STAGE : (uint32_t)(X_STAGE + W_STAGE);
     static constexpr uint32_t Q_OFF = SX * XS;
     static constexpr uint32_t E_OFF = (Q_OFF + SQ * CHUNK + 1023) / 1024 * 1024;   // swizzled slots: 1024-byte aligned
+    static constexpr int SE = (232448 - 512 - 1024 - E_OFF) / (2 * E_SLOT);
     static constexpr uint32_t BAR_OFF = E_OFF + 2 * SE * E_SLOT;
     static constexpr uint32_t SMEM = BAR_OFF + 512 /*barriers*/ + 1024 /*align slack*/;
     static_assert(SMEM <= 232448, "shared memory plan exceeds 227 KB");
@@ -231,7 +233,7 @@ CB_DEVINL void stmatrix_x4_trans(uint32_t a, const uint32_t (&r)[4]) {
                  : "memory");
 }
 
-// Output rectangle of one consumer group: [192 tokens x 64 features] of Y, staged through a ring of SE slots of E_SLOT bytes in
+// Output rectangle of one consumer group: [256 tokens x 64 features] of Y, staged through a ring of SE slots of E_SLOT bytes in
 // shared memory, laid out [token][feature] with the 128-byte swizzle of the output tensor map (rows of 128 B, 16-byte piece p of row
 // r at p ^ (r & 7)).  A chunk fills one slot: 32 tokens x 64 features of 16-bit values (one box), or 16 tokens x 64 features of fp32
 // (two boxes of 32 features).  Chunks past the last token are skipped; the map's M rows clip the rest of a ragged tile.
@@ -268,7 +270,7 @@ CB_DEVINL void prefetch_x(const KParams& p, uint32_t ring, uint32_t full, uint32
     }
 }
 
-// Epilogue of one consumer group's [64 features x 192 tokens] accumulator (fragment layout: wgmma.cuh): this thread (warp w of the
+// Epilogue of one consumer group's [64 features x 256 tokens] accumulator (fragment layout: wgmma.cuh): this thread (warp w of the
 // group) owns features 16w + lane/4 (+ 8) and tokens 8j + 2 (lane % 4) + {0, 1}.  Per chunk: the values go into the slot, every
 // thread fences them to the async proxy, the group syncs and its leader thread issues the bulk store; nobody waits for the store.
 // A slot is written again only after the store that read it is past its source (the leader's wait_group.read before the group
@@ -369,7 +371,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_dq_kernel(const __grid_consta
     pdl_trigger();      // the next kernel of the stream may start placing CTAs as ours retire ...
     pdl_wait();         // ... and we touch global memory only after the previous grid has completed
 
-    // work units: [128 features x 192 tokens] tiles, feature tile fastest (CTAs running at the same time share their X tile in L2)
+    // work units: [128 features x 256 tokens] tiles, feature tile fastest (CTAs running at the same time share their X tile in L2)
     const int n_ft = p.N / BM, n_tt = (p.M + BN - 1) / BN, n_tiles = n_ft * n_tt, nkb = p.K / BK;
 
     if (warp >= 8) {
@@ -425,12 +427,12 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_dq_kernel(const __grid_consta
                 #pragma unroll
                 for (int k = 0; k < BK / 16; k++) {
                     const uint32_t ak[4] = {a[4 * k], a[4 * k + 1], a[4 * k + 2], a[4 * k + 3]};
-                    wgmma_rs_n192<BF>(acc, ak, db + 2 * k, (uint32_t)(kb | k));                      // B: +16 k = +32 B
+                    wgmma_rs_n256<BF>(acc, ak, db + 2 * k, (uint32_t)(kb | k));                      // B: +16 k = +32 B
                 }
             } else {
                 const uint64_t da = wgmma_desc_sw128(smem_base + s * C::XS + X_STAGE + (uint32_t)wg * 64u * 128u);
                 #pragma unroll
-                for (int k = 0; k < BK / 16; k++) wgmma_ss_n192<BF>(acc, da + 2 * k, db + 2 * k, (uint32_t)(kb | k));
+                for (int k = 0; k < BK / 16; k++) wgmma_ss_n256<BF>(acc, da + 2 * k, db + 2 * k, (uint32_t)(kb | k));
             }
             wgmma_commit();
             wgmma_wait<1>();            // the MMAs of k-block kb-1 are done: release its X stage, its A fragments may be overwritten

@@ -3,14 +3,19 @@
 
     python tools/bench_k1_shapes.py [--lib PATH] [--reps 5]
 
-M = 25344 tokens = 132 token tiles (whole waves on 132 SMs), q4_0 weights, bf16 operands.  Each shape runs `reps` times; the line
-reports the median of all but the first call.  REDADD32 and STORE32 at the same shape differ only in the epilogue (read-add-write of
-the fp32 residual against a plain fp32 store), so their gap is what the residual add costs.
+M = 25344 tokens = 99 token tiles of 256 (or 132 of 192): whole waves on 132 SMs for every shape below, q4_0 weights, bf16 operands.
+Each shape runs `reps` times; the line reports the median of all but the first call.  REDADD32 and STORE32 at the same shape differ
+only in the epilogue (read-add-write of the fp32 residual against a plain fp32 store), so their gap is what the residual add costs.
+
+Next to TFLOP/s each line gives the bytes the launch's tiles read from L2 and their rate: every feature tile reads the activations
+X once (M K 2 B), every token tile reads the packed weights once (N K / 32 blocks of 18 B), and the residual add reads x once (M N
+4 B).  The tile comes from csrc/gemm.h; --tile FxT gives it for a library built with another one (e.g. --tile 128x192).
 """
 import argparse
 import ctypes as C
 import json
 import os
+import re
 import sys
 
 import numpy as np
@@ -33,18 +38,34 @@ def q4_0_rows(N, K, rng):
     return blk.tobytes()
 
 
+def header_tile():
+    """(features, tokens) per CTA tile: GEMM_BM and GEMM_BN of csrc/gemm.h"""
+    src = open(os.path.join(ROOT, "clip.cpp_b200", "csrc", "gemm.h")).read()
+    return tuple(int(re.search(r"constexpr int %s = (\d+);" % n, src).group(1)) for n in ("GEMM_BM", "GEMM_BN"))
+
+
+def l2_read_bytes(M, N, K, epi, tile):
+    bf, bt = tile
+    x = -(-N // bf) * M * K * 2
+    w = -(-M // bt) * N * (K // 32) * 18
+    r = M * N * 4 if epi == "REDADD32" else 0
+    return x + w + r
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", default=binding.PRODUCT_LIB)
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--M", type=int, default=132 * 192)
+    ap.add_argument("--M", type=int, default=25344)
+    ap.add_argument("--tile", default="", help="FxT: the CTA tile (features x tokens) of the library under test (default: csrc/gemm.h)")
     ap.add_argument("--epi", default="", help="comma-separated epilogues to run (default: every shape)")
     args = ap.parse_args()
     lib = binding.ClipLib(args.lib)
     rng = np.random.default_rng(0)
     M = args.M
     fp = C.POINTER(C.c_float)
-    out = {"lib": os.path.basename(args.lib), "M": M, "shapes": []}
+    tile = tuple(int(v) for v in args.tile.split("x")) if args.tile else header_tile()
+    out = {"lib": os.path.basename(args.lib), "M": M, "tile": "%dx%d" % tile, "shapes": []}
     for N, K, epi in SHAPES:
         if args.epi and epi not in args.epi.split(","):
             continue
@@ -64,6 +85,8 @@ def main():
         med = float(np.median(ms[1:]))
         rec = {"N": N, "K": K, "epi": epi, "ms": [round(v, 4) for v in ms], "median_ms": round(med, 4),
                "tflops": round(2.0 * M * N * K / med / 1e9, 1)}
+        l2 = l2_read_bytes(M, N, K, epi, tile)
+        rec.update(l2_read_gb=round(l2 / 1e9, 3), l2_tbps=round(l2 / med / 1e9, 2))
         out["shapes"].append(rec)
         print(json.dumps(rec), flush=True)
     print(json.dumps(out))
