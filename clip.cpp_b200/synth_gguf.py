@@ -188,8 +188,15 @@ def _vocab(n):
     return toks
 
 
-def write_model(path: str, geom: Geometry, seed: int = 1234, ftype: int = 1) -> str:
-    """Write an f32 (ftype 0) or f16 (ftype 1) synthetic model; returns the sha256 of the file."""
+def write_model(path: str, geom: Geometry, seed: int = 1234, ftype: int = 1, qk_logit_std=None) -> str:
+    """Write an f32 (ftype 0) or f16 (ftype 1) synthetic model; returns the sha256 of the file.
+
+    qk_logit_std: draw each tower's attn_q / attn_k weights with std sqrt(qk_logit_std / hidden) instead of 0.03, so that the scaled
+    attention logits q.k / sqrt(head_dim) have a standard deviation of about qk_logit_std at any head_dim (LayerNorm outputs have
+    unit variance, so q and k entries have variance hidden std^2, and q.k / sqrt(head_dim) has standard deviation hidden std^2).
+    At 3 the softmax is peaked, so a wrong Q scale, mask or key moves the output; the default std 0.03 gives hidden 9e-4 (0.1 at
+    hidden 128), a nearly uniform softmax.  The
+    draws are the same, only scaled, so None writes the same bytes as before the keyword existed."""
     assert ftype in (0, 1)
     g = geom
     rng = np.random.Generator(np.random.PCG64(seed))
@@ -214,7 +221,10 @@ def write_model(path: str, geom: Geometry, seed: int = 1234, ftype: int = 1) -> 
         for il in range(layers):
             pre = "%s.blk.%d." % (p, il)
             for nm in ("attn_q", "attn_k", "attn_v", "attn_out"):
-                w.add_tensor(pre + nm + ".weight", normal((hid, hid), 0.03 if nm != "attn_out" else 0.02, wdt))
+                std = 0.02 if nm == "attn_out" else 0.03
+                if qk_logit_std is not None and nm in ("attn_q", "attn_k"):
+                    std = np.sqrt(qk_logit_std / hid)
+                w.add_tensor(pre + nm + ".weight", normal((hid, hid), std, wdt))
                 w.add_tensor(pre + nm + ".bias", normal((hid,), 0.02))
             w.add_tensor(pre + "ffn_down.weight", normal((ff, hid), 0.03, wdt))     # HF fc1 (h -> f)
             w.add_tensor(pre + "ffn_down.bias", normal((ff,), 0.02))
