@@ -102,6 +102,7 @@ EXTENSION_SYMBOLS = [
     "clip_b200_text_tokens_device_packed", "clip_b200_debug_attention_mixed_causal",
     # inverted-file index over 16-bit databases
     "clip_b200_ivf_train_16", "clip_b200_ivf_build_16", "clip_b200_ivf_search_16",
+    "clip_b200_ivfpq_train_16", "clip_b200_ivfpq_encode_16", "clip_b200_ivfpq_build", "clip_b200_ivfpq_search_16",
 ]
 
 # include/clip_b200.h: output types and flags of the *_tokens entry points
@@ -311,6 +312,14 @@ class ClipLib:
             L.clip_b200_ivf_build_16.argtypes = [vp, vp, C.c_size_t, ip, ip, vp, ip, vp, vp, vp]
             L.clip_b200_ivf_search_16.restype = C.c_bool
             L.clip_b200_ivf_search_16.argtypes = [vp, vp, C.c_size_t, ip, ip, vp, ip, vp, vp, vp, C.c_size_t, ip, ip, fp, ipp]
+            L.clip_b200_ivfpq_train_16.restype = C.c_bool
+            L.clip_b200_ivfpq_train_16.argtypes = [vp, vp, C.c_size_t, ip, ip, vp, ip, ip, ip, vp]
+            L.clip_b200_ivfpq_encode_16.restype = C.c_bool
+            L.clip_b200_ivfpq_encode_16.argtypes = [vp, vp, C.c_size_t, ip, ip, vp, ip, vp, ip, vp, vp]
+            L.clip_b200_ivfpq_build.restype = C.c_bool
+            L.clip_b200_ivfpq_build.argtypes = [vp, vp, vp, C.c_size_t, ip, ip, vp, vp, vp]
+            L.clip_b200_ivfpq_search_16.restype = C.c_bool
+            L.clip_b200_ivfpq_search_16.argtypes = [vp, vp, C.c_size_t, ip, ip, vp, ip, vp, ip, vp, vp, vp, C.c_size_t, ip, ip, fp, ipp]
             L.clip_b200_zero_shot_images.restype = C.c_bool
             L.clip_b200_zero_shot_images.argtypes = [vp, ip, C.POINTER(clip_image_f32_batch), C.POINTER(clip_tokens), C.c_size_t,
                                                      C.c_bool, ip, fp, ipp]

@@ -89,7 +89,7 @@ struct Scope {
     }
 };
 enum { K_GEMM = 0, K_ATTN = 1, K_LN = 2, K_OTHER = 3, K_TOKEN_ROWS = 4, K_POS_RESAMPLE = 5, K_ATTN_PROBS = 6, K_KNN16 = 7, K_KNN_I8 = 8, K_KNN_B1 = 9, K_RESCORE = 10, K_IVF_SCAN = 11,
-       K_IVF_LAYOUT = 12 };
+       K_IVF_LAYOUT = 12, K_ADC = 13, K_PQ = 14 };
 
 // ---- tensor lookup helpers ---------------------------------------------------------------------------------
 const GgufTensor* need(const GgufFile& g, const std::string& name) {
@@ -2034,7 +2034,8 @@ static bool ensure_cand(clip_ctx* c, size_t count) {
 // that make their databases.  Each form fills one and calls search_call, so every form checks its arguments in the same order
 // (include/clip_b200.h), and the searches run the same pass driver.
 struct SearchCall {
-    enum Kind { SCORE, KNN16, KNN_I8, KNN_B1, RESCORE, ROWS16, ROWS_I8, ROWS_B1, IVF_TRAIN, IVF_BUILD, IVF_SEARCH };
+    enum Kind { SCORE, KNN16, KNN_I8, KNN_B1, RESCORE, ROWS16, ROWS_I8, ROWS_B1, IVF_TRAIN, IVF_BUILD, IVF_SEARCH, PQ_TRAIN, PQ_ENCODE,
+                PQ_BUILD, PQ_SEARCH };
     const char* who;                              // the public name, for messages
     Kind kind;
     const void* q = nullptr;                      // queries [nq, dim]; a row form: its f32 source rows [nq, dim]
@@ -2059,7 +2060,13 @@ struct SearchCall {
     int* ids = nullptr;
     int n_lists = 0;
     int iters = 0;                                // IVF_TRAIN: n_iter; IVF_SEARCH: nprobe
-    bool ivf() const { return kind >= IVF_TRAIN; }
+    // PQ_*: q holds the training rows, the rows to encode, the codes to lay out (PQ_BUILD) or the queries; db the codes that PQ_ENCODE
+    // and PQ_BUILD write and PQ_SEARCH reads; cent, offsets, ids, n_lists and iters as IVF_*
+    const void* books = nullptr;                  // codebooks f32 [m, 256, dim / m] (PQ_TRAIN writes them)
+    int m = 0;                                    // subspaces
+    int* lists = nullptr;                         // [nq]: PQ_ENCODE writes them, PQ_BUILD reads them
+    bool ivf() const { return kind >= IVF_TRAIN && kind <= IVF_SEARCH; }
+    bool pq() const { return kind >= PQ_TRAIN; }
     bool search() const { return kind <= RESCORE; }
     bool knn() const { return kind == KNN16 || kind == KNN_I8 || kind == KNN_B1; }
 };
@@ -2274,21 +2281,40 @@ static bool ivf_build_locked(clip_ctx* c, const SearchCall& a) {
     return true;
 }
 
-// Search, per block of queries: the probes (K10 top-nprobe over the centroids, to the host), the host plan of the fine scan's work
-// units (include/clip_b200.h, clip_b200_ivf_search_16), the pairs' query rows gathered, K10's IVF instance, the merge.
-static bool ivf_search_locked(clip_ctx* c, const SearchCall& a, const std::vector<int>& off) {
+// One query block of an IVF search as its plan hands it to the form's scan: queries r0 .. r0 + rows - 1, P (query, probed list)
+// pairs grouped by list, each with its query row in the block (d_pq) and its coarse score (d_ps), the work units of query tile
+// 8 nt, each pair's run slot, and the form's own piece of the arena (`extra`).
+struct IvfBlock {
+    size_t r0;
+    int rows, P, nt, nunits;
+    const int* d_pq;
+    const float* d_ps;
+    const IvfUnit* d_units;
+    const size_t* d_slot;
+    void* extra;
+};
+
+// The plan both IVF searches run, per block of QB queries: the probes (K10 top-nprobe over the centroids, their ids and scores to
+// the host), the host plan of the fine scan's work units (include/clip_b200.h, clip_b200_ivf_search_16), the candidate pre-fill, the
+// form's scan (extra_bytes(P, rows) bytes of its own arena piece), the merge, the padding.  A unit holds at most 8 nt_max pairs:
+// K10 scores a unit's pairs together in its MMA, so up to 128; K13 scores them one after another, so a unit of np pairs costs np
+// times its rows, and 8 pairs a unit keep the plan's work estimate, and with it the units' balance, true to that cost.
+extern "C++" {
+template <class Extra, class Scan>
+static bool ivf_search_plan(clip_ctx* c, const SearchCall& a, const std::vector<int>& off, size_t QB, int nt_max, Extra extra_bytes,
+                            Scan scan) {
     const int L = a.n_lists, np = std::min(a.iters, L), w = (int)std::min<size_t>(a.top_k, a.ndb), KB = knn_tile_rows();
     const bool bf = a.type == CLIP_B200_OUT_BF16;
     int sms = 0;
     CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
-    const size_t QB = std::min<size_t>(32768, std::max<size_t>(1, ((size_t)1 << 24) / ((size_t)(w + 2 * KB) * np)));
     std::vector<int> probes, cnt(L), pstart(L + 1), fill(L), pair_q, runs;
+    std::vector<float> pscore, pair_s;
     std::vector<size_t> slot;
     std::vector<IvfUnit> units;
     for (size_t r0 = 0; r0 < a.nq; r0 += QB) {
         const int rows = (int)std::min(QB, a.nq - r0);
         const uint8_t* q = (const uint8_t*)a.q + r0 * a.dim * 2;
-        // coarse: the best np lists of each query, best first
+        // coarse: the best np lists of each query, best first, with their scores
         const KnnPlan pl = knn_plan(rows, L, np, sms);
         if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * pl.buf_entries) || !ensure_cand(c, (size_t)rows * pl.parts * np)) return false;
         {
@@ -2299,7 +2325,10 @@ static bool ivf_search_locked(clip_ctx* c, const SearchCall& a, const std::vecto
         }
         const int pc = merge_candidates(c, rows, (size_t)pl.parts * np, pl.parts, np);
         probes.resize((size_t)rows * np);
+        pscore.resize((size_t)rows * np);
         CK(cudaMemcpy2DAsync(probes.data(), (size_t)np * 4, c->d_cand_i[pc], (size_t)pl.parts * np * 4, (size_t)np * 4, rows,
+                             cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaMemcpy2DAsync(pscore.data(), (size_t)np * 4, c->d_cand_v[pc], (size_t)pl.parts * np * 4, (size_t)np * 4, rows,
                              cudaMemcpyDeviceToHost, c->stream));
         CK(cudaStreamSynchronize(c->stream));
         // the plan: pairs (query, probed non-empty list) grouped by list, stable by query
@@ -2309,13 +2338,18 @@ static bool ivf_search_locked(clip_ctx* c, const SearchCall& a, const std::vecto
         for (int l = 0; l < L; l++) { pstart[l + 1] = pstart[l] + cnt[l]; lists += cnt[l] > 0; }
         const int P = pstart[L];
         pair_q.resize(P);
+        pair_s.resize(P);
         std::copy(pstart.begin(), pstart.end() - 1, fill.begin());
         for (int r = 0; r < rows; r++)
-            for (int j = 0; j < np; j++) { const int l = probes[(size_t)r * np + j]; if (off[l + 1] > off[l]) pair_q[fill[l]++] = r; }
+            for (int j = 0; j < np; j++) {
+                const size_t e = (size_t)r * np + j;
+                const int l = probes[e];
+                if (off[l + 1] > off[l]) { pair_s[fill[l]] = pscore[e]; pair_q[fill[l]++] = r; }
+            }
         // query tile: the least 8 nt >= the mean pairs per probed list (at most 128); row ranges of R rows so that about 4 units per SM
         const int mean = lists ? (P + lists - 1) / lists : 1;
         int nt = 1;
-        while (8 * nt < std::min(mean, 128)) nt <<= 1;
+        while (8 * nt < std::min(mean, 128) && nt < nt_max) nt <<= 1;
         const int N = 8 * nt;
         size_t work = 0;
         for (int l = 0; l < L; l++) work += (size_t)((cnt[l] + N - 1) / N) * (off[l + 1] - off[l]);
@@ -2343,27 +2377,22 @@ static bool ivf_search_locked(clip_ctx* c, const SearchCall& a, const std::vecto
                 run += nr;
             }
         int* d_pq = nullptr;
+        float* d_ps = nullptr;
         IvfUnit* d_units = nullptr;
         size_t* d_slot = nullptr;
-        void* d_pairs = nullptr;
-        if (!ivf_arena(c, {(size_t)P * 4, units.size() * sizeof(IvfUnit), (size_t)P * 8, (size_t)P * a.dim * 2},
-                       {(void**)&d_pq, (void**)&d_units, (void**)&d_slot, &d_pairs})) return false;
-        const size_t buf = units.size() * N * (size_t)(w + 2 * KB);
-        if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * buf) || !ensure_cand(c, (size_t)rows * cand_ld)) return false;
+        void* extra = nullptr;
+        if (!ivf_arena(c, {(size_t)P * 4, (size_t)P * 4, units.size() * sizeof(IvfUnit), (size_t)P * 8, extra_bytes(P, rows)},
+                       {(void**)&d_pq, (void**)&d_ps, (void**)&d_units, (void**)&d_slot, &extra})) return false;
+        if (!ensure_cand(c, (size_t)rows * cand_ld)) return false;
         CK(cudaMemcpyAsync(d_pq, pair_q.data(), (size_t)P * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_ps, pair_s.data(), (size_t)P * 4, cudaMemcpyHostToDevice, c->stream));
         CK(cudaMemcpyAsync(d_units, units.data(), units.size() * sizeof(IvfUnit), cudaMemcpyHostToDevice, c->stream));
         CK(cudaMemcpyAsync(d_slot, slot.data(), (size_t)P * 8, cudaMemcpyHostToDevice, c->stream));
         {
             Scope s(c, K_OTHER);
-            launch_gather_rows16(q, d_pq, P, a.dim, d_pairs, c->stream);
             launch_fill_cand(c->d_cand_v[0], c->d_cand_i[0], (size_t)rows * cand_ld, c->stream);
         }
-        {
-            Scope s(c, K_IVF_SCAN);
-            const cudaError_t e = launch_knn_ivf(bf, d_pairs, P, a.db, (int)a.ndb, a.dim, w, nt, d_units, (int)units.size(), d_slot, a.ids,
-                                                 c->d_knn, c->d_cand_v[0], c->d_cand_i[0], c->stream);
-            if (e != cudaSuccess) { set_err(std::string(a.who) + ": launch: " + cudaGetErrorString(e)); return false; }
-        }
+        if (!scan(IvfBlock{r0, rows, P, nt, (int)units.size(), d_pq, d_ps, d_units, d_slot, extra})) return false;
         const int cur = merge_candidates(c, rows, cand_ld, runs_max, w);
         float* os = a.scores + r0 * w;
         int* oi = a.indices + r0 * w;
@@ -2375,6 +2404,189 @@ static bool ivf_search_locked(clip_ctx* c, const SearchCall& a, const std::vecto
     }
     CK(cudaGetLastError());
     return true;
+}
+}  // extern "C++"
+
+// IVF search over 16-bit rows: the pairs' query rows gathered, K10's IVF instance.
+static bool ivf_search_locked(clip_ctx* c, const SearchCall& a, const std::vector<int>& off) {
+    const int np = std::min(a.iters, a.n_lists), w = (int)std::min<size_t>(a.top_k, a.ndb), KB = knn_tile_rows();
+    const bool bf = a.type == CLIP_B200_OUT_BF16;
+    const size_t QB = std::min<size_t>(32768, std::max<size_t>(1, ((size_t)1 << 24) / ((size_t)(w + 2 * KB) * np)));
+    return ivf_search_plan(c, a, off, QB, 16, [&](int P, int) { return (size_t)P * a.dim * 2; }, [&](const IvfBlock& b) {
+        const size_t buf = (size_t)b.nunits * 8 * b.nt * (size_t)(w + 2 * KB);
+        if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * buf)) return false;
+        {
+            Scope s(c, K_OTHER);
+            launch_gather_rows16((const uint8_t*)a.q + b.r0 * a.dim * 2, b.d_pq, b.P, a.dim, b.extra, c->stream);
+        }
+        Scope s(c, K_IVF_SCAN);
+        const cudaError_t e = launch_knn_ivf(bf, b.extra, b.P, a.db, (int)a.ndb, a.dim, w, b.nt, b.d_units, b.nunits, b.d_slot, a.ids,
+                                             c->d_knn, c->d_cand_v[0], c->d_cand_i[0], c->stream);
+        if (e != cudaSuccess) { set_err(std::string(a.who) + ": launch: " + cudaGetErrorString(e)); return false; }
+        return true;
+    });
+}
+
+// ---- IVF with product-quantised residuals (clip_b200_ivfpq_*) -----------------------------------------------------------------
+// IVF-PQ search: each query's lookup tables, then K13 over the stored codes.  The query block also bounds the tables, Q * m KiB.
+static bool pq_search_locked(clip_ctx* c, const SearchCall& a, const std::vector<int>& off) {
+    const int np = std::min(a.iters, a.n_lists), w = (int)std::min<size_t>(a.top_k, a.ndb), KB = knn_tile_rows();
+    const bool bf = a.type == CLIP_B200_OUT_BF16;
+    const size_t QB = std::min<size_t>({32768, std::max<size_t>(1, ((size_t)1 << 24) / ((size_t)(w + 2 * KB) * np)), ((size_t)1 << 18) / a.m});
+    return ivf_search_plan(c, a, off, QB, 1, [&](int, int rows) { return (size_t)rows * a.m * 1024; }, [&](const IvfBlock& b) {
+        if (!ensure_buf(c, &c->d_knn, &c->d_knn_cap, 2 * (size_t)b.nunits * adc_cap(w))) return false;
+        float* tables = (float*)b.extra;
+        cudaError_t e;
+        {
+            Scope s(c, K_PQ);
+            e = launch_pq_tables(bf, (const uint8_t*)a.q + b.r0 * a.dim * 2, b.rows, a.dim, a.m, (const float*)a.books, tables, c->stream);
+        }
+        if (e == cudaSuccess) {
+            Scope s(c, K_ADC);
+            e = launch_adc(a.db, (int)a.ndb, a.m, tables, b.d_ps, b.d_pq, w, b.d_units, b.nunits, b.d_slot, a.ids, c->d_knn,
+                           c->d_cand_v[0], c->d_cand_i[0], c->stream);
+        }
+        if (e != cudaSuccess) { set_err(std::string(a.who) + ": launch: " + cudaGetErrorString(e)); return false; }
+        return true;
+    });
+}
+
+// Codebook k-means: the lists of the training rows (the build's assignment), the initial codewords, then per iteration the codes
+// of every residual, their layout per subspace (rows grouped by code, stable by row, on the host) and the update kernels (fp64
+// sums over chunks of IVF_CHUNK members, combined in chunk order).  The arena is carved once, at the most chunks a layout can have.
+static bool pq_train_locked(clip_ctx* c, const SearchCall& a) {
+    const size_t n = a.nq;
+    const int m = a.m, dsub = a.dim / m, NB = m * 256;
+    const bool bf = a.type == CLIP_B200_OUT_BF16;
+    std::vector<int> list;
+    if (!ivf_assign(c, a, a.q, n, list)) return false;
+    const size_t nch_max = (size_t)m * (n / IVF_CHUNK + 256);
+    int *d_lists = nullptr, *d_ids = nullptr, *d_cb = nullptr, *d_cnt = nullptr;
+    uint8_t* d_codes = nullptr;
+    longlong2* d_ch = nullptr;
+    double* d_part = nullptr;
+    if (!ivf_arena(c, {n * 4, n * m, n * m * 4, (size_t)(NB + 1) * 4, (size_t)NB * 4, nch_max * 16, nch_max * dsub * 8},
+                   {(void**)&d_lists, (void**)&d_codes, (void**)&d_ids, (void**)&d_cb, (void**)&d_cnt, (void**)&d_ch, (void**)&d_part})) return false;
+    CK(cudaMemcpyAsync(d_lists, list.data(), n * 4, cudaMemcpyHostToDevice, c->stream));
+    float* books = (float*)const_cast<void*>(a.books);
+    {
+        Scope s(c, K_PQ);
+        launch_pq_init(bf, a.q, n, a.dim, m, d_lists, a.cent, books, c->stream);
+    }
+    std::vector<uint8_t> codes(n * m);
+    std::vector<int> ids(n * m), cnt(NB), pos(NB), chunk_begin(NB + 1);
+    std::vector<longlong2> chunks;
+    for (int it = 0; it < a.iters; it++) {
+        {
+            Scope s(c, K_PQ);
+            const cudaError_t e = launch_pq_encode(bf, a.q, n, a.dim, m, d_lists, a.cent, books, d_codes, c->stream);
+            if (e != cudaSuccess) { set_err(std::string(a.who) + ": launch: " + cudaGetErrorString(e)); return false; }
+        }
+        CK(cudaMemcpyAsync(codes.data(), d_codes, n * m, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        std::fill(cnt.begin(), cnt.end(), 0);
+        for (size_t r = 0; r < n; r++)
+            for (int s = 0; s < m; s++) cnt[s * 256 + codes[r * m + s]]++;
+        chunks.clear();
+        for (int s = 0; s < m; s++)
+            for (int k = 0, p = 0; k < 256; k++) {
+                const int bk = s * 256 + k;
+                pos[bk] = p;
+                for (int b = p; b < p + cnt[bk]; b += IVF_CHUNK)
+                    chunks.push_back(make_longlong2((long long)s * n + b, (long long)s * n + std::min(b + IVF_CHUNK, p + cnt[bk])));
+                chunk_begin[bk + 1] = (int)chunks.size();
+                p += cnt[bk];
+            }
+        for (size_t r = 0; r < n; r++)
+            for (int s = 0; s < m; s++) { const int bk = s * 256 + codes[r * m + s]; ids[(size_t)s * n + pos[bk]++] = (int)r; }
+        CK(cudaMemcpyAsync(d_ids, ids.data(), n * m * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_cb, chunk_begin.data(), (size_t)(NB + 1) * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_cnt, cnt.data(), (size_t)NB * 4, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(d_ch, chunks.data(), chunks.size() * 16, cudaMemcpyHostToDevice, c->stream));
+        Scope s(c, K_PQ);
+        launch_pq_update(bf, a.q, n, a.dim, m, d_lists, a.cent, d_ids, d_ch, (int)chunks.size(), d_cb, d_cnt, d_part, books, c->stream);
+        CK(cudaGetLastError());
+    }
+    CK(cudaStreamSynchronize(c->stream));
+    return true;
+}
+
+static bool pq_encode_locked(clip_ctx* c, const SearchCall& a) {
+    std::vector<int> list;
+    if (!ivf_assign(c, a, a.q, a.nq, list)) return false;
+    CK(cudaMemcpyAsync(a.lists, list.data(), a.nq * 4, cudaMemcpyHostToDevice, c->stream));
+    {
+        Scope s(c, K_PQ);
+        const cudaError_t e = launch_pq_encode(a.type == CLIP_B200_OUT_BF16, a.q, a.nq, a.dim, a.m, a.lists, a.cent, (const float*)a.books,
+                                               const_cast<void*>(a.db), c->stream);
+        if (e != cudaSuccess) { set_err(std::string(a.who) + ": launch: " + cudaGetErrorString(e)); return false; }
+    }
+    CK(cudaStreamSynchronize(c->stream));
+    return true;
+}
+
+// The build reads the lists first and refuses a value outside [0, n_lists) before it writes anything.
+static bool pq_build_locked(clip_ctx* c, const SearchCall& a) {
+    std::vector<int> list(a.nq), off, ids;
+    CK(cudaMemcpy(list.data(), a.lists, a.nq * 4, cudaMemcpyDeviceToHost));
+    for (int l : list)
+        if (l < 0 || l >= a.n_lists) { set_err(std::string(a.who) + ": d_lists values must be in [0, n_lists)"); return false; }
+    ivf_layout(list, a.n_lists, off, ids);
+    CK(cudaMemcpyAsync(a.offsets, off.data(), off.size() * 4, cudaMemcpyHostToDevice, c->stream));
+    CK(cudaMemcpyAsync(a.ids, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice, c->stream));
+    {
+        Scope s(c, K_IVF_LAYOUT);
+        launch_gather_rows16(a.q, a.ids, a.nq, a.m / 2, const_cast<void*>(a.db), c->stream);       // a code row is m / 2 16-bit columns
+    }
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(c->stream));
+    return true;
+}
+
+// Reads d_offsets and refuses an index whose offsets do not run non-decreasing from 0 to n_db (the IVF searches' check).
+static bool ivf_offsets(clip_ctx* c, const SearchCall& a, std::vector<int>& off) {
+    off.resize(a.n_lists + 1);
+    CK(cudaMemcpy(off.data(), a.offsets, off.size() * 4, cudaMemcpyDeviceToHost));
+    bool ok = off[0] == 0 && (size_t)off[a.n_lists] == a.ndb;
+    for (int l = 0; ok && l < a.n_lists; l++) ok = off[l + 1] >= off[l];
+    if (!ok) set_err(std::string(a.who) + ": d_offsets must run non-decreasing from 0 to n_db");
+    return ok;
+}
+
+// The IVF-PQ forms past the counts: empty calls, pointers, then the locked work.
+static bool pq_call(clip_ctx* c, SearchCall& a) {
+    const std::string who = a.who;
+    const SearchCall::Kind kind = a.kind;
+    if ((kind == SearchCall::PQ_SEARCH && (a.nq == 0 || a.ndb == 0)) || (kind == SearchCall::PQ_ENCODE && a.nq == 0)) return true;
+    const bool empty_build = kind == SearchCall::PQ_BUILD && a.nq == 0;
+    // 16-byte aligned: rows, queries, centroids, codebooks and codes; 4-byte aligned: lists, offsets and ids
+    std::vector<const void*> p16, p4;
+    if (kind == SearchCall::PQ_BUILD) {
+        if (!empty_build) p16 = {a.q, a.db};
+        p4 = empty_build ? std::vector<const void*>{a.offsets} : std::vector<const void*>{a.lists, a.offsets, a.ids};
+    } else {
+        p16 = {a.q, a.cent, a.books};
+        if (kind != SearchCall::PQ_TRAIN) p16.push_back(a.db);
+        if (kind == SearchCall::PQ_ENCODE) p4 = {a.lists};
+        if (kind == SearchCall::PQ_SEARCH) p4 = {a.offsets, a.ids};
+    }
+    for (const void* p : p16)
+        if (!p || (uintptr_t)p % 16) { set_err(who + ": null or not 16-byte aligned device pointer"); return false; }
+    for (const void* p : p4)
+        if (!p || (uintptr_t)p % 4) { set_err(who + ": null or not 4-byte aligned d_lists, d_offsets or d_ids"); return false; }
+    if (kind == SearchCall::PQ_SEARCH && (!a.scores || !a.indices)) { set_err(who + ": null output"); return false; }
+    std::lock_guard<std::mutex> lk(c->mu);
+    CK(cudaSetDevice(c->device));
+    if (empty_build) {
+        CK(cudaMemsetAsync(a.offsets, 0, (size_t)(a.n_lists + 1) * 4, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        return true;
+    }
+    if (kind == SearchCall::PQ_TRAIN) return pq_train_locked(c, a);
+    if (kind == SearchCall::PQ_ENCODE) return pq_encode_locked(c, a);
+    if (kind == SearchCall::PQ_BUILD) return pq_build_locked(c, a);
+    std::vector<int> off;
+    return ivf_offsets(c, a, off) && pq_search_locked(c, a, off);
 }
 
 // The IVF forms past the counts: empty calls, pointers, then the locked work.  IVF_SEARCH reads d_offsets first and refuses an index
@@ -2404,12 +2616,8 @@ static bool ivf_call(clip_ctx* c, SearchCall& a) {
     }
     if (kind == SearchCall::IVF_TRAIN) return ivf_train_locked(c, a);
     if (kind == SearchCall::IVF_BUILD) return ivf_build_locked(c, a);
-    std::vector<int> off(a.n_lists + 1);
-    CK(cudaMemcpy(off.data(), a.offsets, off.size() * 4, cudaMemcpyDeviceToHost));
-    bool ok = off[0] == 0 && (size_t)off[a.n_lists] == a.ndb;
-    for (int l = 0; ok && l < a.n_lists; l++) ok = off[l + 1] >= off[l];
-    if (!ok) { set_err(who + ": d_offsets must run non-decreasing from 0 to n_db"); return false; }
-    return ivf_search_locked(c, a, off);
+    std::vector<int> off;
+    return ivf_offsets(c, a, off) && ivf_search_locked(c, a, off);
 }
 
 // Every form of the family: the arguments checked in one order, the first fault refused (include/clip_b200.h), then the search pass or
@@ -2419,7 +2627,8 @@ static bool search_call(const clip_ctx* cctx, SearchCall a) {
     const std::string who = a.who;
     const SearchCall::Kind kind = a.kind;
     if (!c) { set_err(who + ": null context"); return false; }
-    if ((kind == SearchCall::KNN16 || kind == SearchCall::ROWS16 || a.ivf()) && a.type != CLIP_B200_OUT_F16 && a.type != CLIP_B200_OUT_BF16) {
+    const bool typed = a.ivf() || (a.pq() && kind != SearchCall::PQ_BUILD);      // the IVF forms that read 16-bit rows
+    if ((kind == SearchCall::KNN16 || kind == SearchCall::ROWS16 || typed) && a.type != CLIP_B200_OUT_F16 && a.type != CLIP_B200_OUT_BF16) {
         set_err(who + (kind == SearchCall::ROWS16 ? ": out_type" : ": in_type") + " must be CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16");
         return false;
     }
@@ -2427,9 +2636,9 @@ static bool search_call(const clip_ctx* cctx, SearchCall a) {
         set_err(who + ": in_type must be CLIP_B200_OUT_F32, CLIP_B200_OUT_F16 or CLIP_B200_OUT_BF16");
         return false;
     }
-    const int step = kind == SearchCall::KNN16 || kind == SearchCall::RESCORE || a.ivf() ? 8 : kind == SearchCall::ROWS16 ? 4
+    const int step = kind == SearchCall::KNN16 || kind == SearchCall::RESCORE || typed ? 8 : kind == SearchCall::ROWS16 ? 4
                    : kind == SearchCall::KNN_B1 || kind == SearchCall::ROWS_B1 ? 128 : 16;     // SCORE's dim is the model's
-    if (kind != SearchCall::SCORE && (a.dim < step || a.dim > 2048 || a.dim % step)) {
+    if (kind != SearchCall::SCORE && kind != SearchCall::PQ_BUILD && (a.dim < step || a.dim > 2048 || a.dim % step)) {
         set_err(who + ": dim must be a multiple of " + std::to_string(step) + " in [" + std::to_string(step) + ", 2048]");
         return false;
     }
@@ -2437,17 +2646,25 @@ static bool search_call(const clip_ctx* cctx, SearchCall a) {
         if (a.n_cand < 1 || a.n_cand > 2048) { set_err(who + ": n_cand must be in [1, 2048]"); return false; }
         if (a.top_k < 1 || a.top_k > a.n_cand) { set_err(who + ": top_k must be in [1, n_cand]"); return false; }
     }
-    if (a.ivf() && (a.n_lists < 1 || a.n_lists > 65536)) { set_err(who + ": n_lists must be in [1, 65536]"); return false; }
-    if (kind == SearchCall::IVF_TRAIN && (a.iters < 1 || a.iters > 1000)) { set_err(who + ": n_iter must be in [1, 1000]"); return false; }
-    if (kind == SearchCall::IVF_SEARCH && (a.iters < 1 || a.iters > 1024)) { set_err(who + ": nprobe must be in [1, 1024]"); return false; }
-    if ((a.knn() || kind == SearchCall::IVF_SEARCH) && (a.top_k < 1 || a.top_k > 1024)) { set_err(who + ": top_k must be in [1, 1024]"); return false; }
+    // m: whole 16-byte words of codes per row (the build's copy is launch_gather_rows16 on m / 2 16-bit columns), dividing dim
+    if (a.pq() && (a.m < 16 || a.m > 256 || a.m % 16 || (kind != SearchCall::PQ_BUILD && a.dim % a.m))) {
+        set_err(who + (kind == SearchCall::PQ_BUILD ? ": m must be a multiple of 16 in [16, 256]" : ": m must be a multiple of 16 in [16, 256] that divides dim"));
+        return false;
+    }
+    const bool train = kind == SearchCall::IVF_TRAIN || kind == SearchCall::PQ_TRAIN, isearch = kind == SearchCall::IVF_SEARCH || kind == SearchCall::PQ_SEARCH;
+    if ((a.ivf() || a.pq()) && (a.n_lists < 1 || a.n_lists > 65536)) { set_err(who + ": n_lists must be in [1, 65536]"); return false; }
+    if (train && (a.iters < 1 || a.iters > 1000)) { set_err(who + ": n_iter must be in [1, 1000]"); return false; }
+    if (isearch && (a.iters < 1 || a.iters > 1024)) { set_err(who + ": nprobe must be in [1, 1024]"); return false; }
+    if ((a.knn() || isearch) && (a.top_k < 1 || a.top_k > 1024)) { set_err(who + ": top_k must be in [1, 1024]"); return false; }
     if (a.nq > 0x7fffffffull || a.ndb > 0x7fffffffull) {
-        set_err(who + (a.search() || kind == SearchCall::IVF_SEARCH ? ": n_queries and n_db must be below 2^31"
-                       : kind == SearchCall::IVF_TRAIN ? ": n_train must be below 2^31" : kind == SearchCall::IVF_BUILD ? ": n_db must be below 2^31"
+        set_err(who + (a.search() || isearch ? ": n_queries and n_db must be below 2^31"
+                       : train ? ": n_train must be below 2^31" : kind == SearchCall::IVF_BUILD || kind == SearchCall::PQ_BUILD ? ": n_db must be below 2^31"
                        : ": n must be below 2^31"));
         return false;
     }
+    if (kind == SearchCall::PQ_TRAIN && a.nq < 256) { set_err(who + ": n_train must be at least 256"); return false; }
     if (a.ivf()) return ivf_call(c, a);
+    if (a.pq()) return pq_call(c, a);
     if (a.nq == 0 || (a.search() && a.ndb == 0)) return true;
     // the device pointers the kind reads or writes: q and db, then the int8 forms' scales or ROWS_B1's optional centre.  K10, K11, K12
     // and the row kernels load and store 16 bytes at a time; the fp32 kernels read single floats.
@@ -2565,6 +2782,40 @@ bool clip_b200_ivf_search_16(const struct clip_ctx* cctx, const void* d_queries,
     a.q = d_queries; a.nq = n_queries; a.dim = dim; a.type = in_type; a.cent = d_centroids; a.n_lists = n_lists;
     a.offsets = const_cast<int*>(d_offsets); a.ids = const_cast<int*>(d_ids); a.db = d_rows; a.ndb = n_db; a.iters = nprobe; a.top_k = top_k;
     a.scores = scores; a.indices = indices;
+    return search_call(cctx, a);
+}
+
+bool clip_b200_ivfpq_train_16(const struct clip_ctx* cctx, const void* d_train, size_t n_train, int dim, int in_type, const void* d_centroids,
+                              int n_lists, int m, int n_iter, void* d_codebooks) {
+    SearchCall a{"clip_b200_ivfpq_train_16", SearchCall::PQ_TRAIN};
+    a.q = d_train; a.nq = n_train; a.dim = dim; a.type = in_type; a.cent = d_centroids; a.n_lists = n_lists; a.m = m; a.iters = n_iter;
+    a.books = d_codebooks;
+    return search_call(cctx, a);
+}
+
+bool clip_b200_ivfpq_encode_16(const struct clip_ctx* cctx, const void* d_rows, size_t n, int dim, int in_type, const void* d_centroids,
+                               int n_lists, const void* d_codebooks, int m, int* d_lists, void* d_codes) {
+    SearchCall a{"clip_b200_ivfpq_encode_16", SearchCall::PQ_ENCODE};
+    a.q = d_rows; a.nq = n; a.dim = dim; a.type = in_type; a.cent = d_centroids; a.n_lists = n_lists; a.books = d_codebooks; a.m = m;
+    a.lists = d_lists; a.db = d_codes;
+    return search_call(cctx, a);
+}
+
+bool clip_b200_ivfpq_build(const struct clip_ctx* cctx, const int* d_lists, const void* d_codes, size_t n_db, int n_lists, int m,
+                           int* d_offsets, int* d_ids, void* d_codes_out) {
+    SearchCall a{"clip_b200_ivfpq_build", SearchCall::PQ_BUILD};
+    a.lists = const_cast<int*>(d_lists); a.q = d_codes; a.nq = n_db; a.n_lists = n_lists; a.m = m; a.offsets = d_offsets; a.ids = d_ids;
+    a.db = d_codes_out;
+    return search_call(cctx, a);
+}
+
+bool clip_b200_ivfpq_search_16(const struct clip_ctx* cctx, const void* d_queries, size_t n_queries, int dim, int in_type,
+                               const void* d_centroids, int n_lists, const void* d_codebooks, int m, const int* d_offsets, const int* d_ids,
+                               const void* d_codes, size_t n_db, int nprobe, int top_k, float* scores, int* indices) {
+    SearchCall a{"clip_b200_ivfpq_search_16", SearchCall::PQ_SEARCH};
+    a.q = d_queries; a.nq = n_queries; a.dim = dim; a.type = in_type; a.cent = d_centroids; a.n_lists = n_lists; a.books = d_codebooks;
+    a.m = m; a.offsets = const_cast<int*>(d_offsets); a.ids = const_cast<int*>(d_ids); a.db = d_codes; a.ndb = n_db; a.iters = nprobe;
+    a.top_k = top_k; a.scores = scores; a.indices = indices;
     return search_call(cctx, a);
 }
 

@@ -137,6 +137,28 @@ void launch_fill_cand(float* v, int* i, size_t n, cudaStream_t st);
 // scratch.  Rewrites cent [n_lists, dim] in place, keeping the centroid of an empty list or of a zero mean.
 void launch_ivf_update(bool bf, const void* x, int dim, const int* ids, const int2* chunks, int nchunks, const int* chunk_begin,
                        const int* offsets, int n_lists, double* part, void* cent, cudaStream_t st);
+// IVF-PQ (clip_b200_ivfpq_*'s rule, clip_b200.h).  x and cent are 16-bit (bf: bf16) [n, dim] and [n_lists, dim]; lists [n] the list
+// of each row; books f32 [m, 256, dim / m]; codes uint8 [n, m], 16-byte aligned.  64-bit offsets throughout.
+// codes of each row's residual x - cent[list] (kernel class 14)
+cudaError_t launch_pq_encode(bool bf, const void* x, size_t n, int dim, int m, const int* lists, const void* cent, const float* books,
+                             void* codes, cudaStream_t st);
+// initial codebooks: codeword i of every subspace from the residual of row floor(i n / 256), n >= 256
+void launch_pq_init(bool bf, const void* x, size_t n, int dim, int m, const int* lists, const void* cent, float* books, cudaStream_t st);
+// one codebook update: ids [m][n] the rows of each subspace grouped by code (stable), chunks[c] = positions [begin, end) in that flat
+// array, chunk_begin [m * 256 + 1] the chunks of codeword s * 256 + k, count [m * 256] its members, part [nchunks, dim / m] fp64
+// scratch.  Rewrites each non-empty codeword with the fp64 mean of its members' residuals, rounded once to f32.
+void launch_pq_update(bool bf, const void* x, size_t n, int dim, int m, const int* lists, const void* cent, const int* ids,
+                      const longlong2* chunks, int nchunks, const int* chunk_begin, const int* count, double* part, float* books,
+                      cudaStream_t st);
+// lookup tables [nq, m, 256] f32 of queries q [nq, dim] 16-bit (kernel class 14)
+cudaError_t launch_pq_tables(bool bf, const void* q, int nq, int dim, int m, const float* books, float* tables, cudaStream_t st);
+// K13, the ADC scan (kernel class 13): CTA u runs unit units[u] of K10's IVF plan over stored codes [ndb, m].  Pair p (query
+// pair_q[p], coarse score pscore[p]) scores a row v = pscore[p] + T[s][code_s] for s in order, T = tables[pair_q[p]]; its best kk of
+// the unit go to out as launch_knn_ivf writes them.  Scratch `buf` of nunits * adc_cap(kk) (value, index) pairs.
+size_t adc_cap(int kk);
+cudaError_t launch_adc(const void* codes, int ndb, int m, const float* tables, const float* pscore, const int* pair_q, int kk,
+                       const IvfUnit* units, int nunits, const size_t* slot, const int* ids, void* buf, float* out_v, int* out_i,
+                       cudaStream_t st);
 // Q8 quantiser: x [n, dim] f32 -> codes [n, dim] int8 and scales [n] f32 by the rule of clip_b200_rows_to_int8 (clip_b200.h).
 // dim % 16 == 0, dim <= 2048, 16-byte aligned pointers; 64-bit offsets, so n * dim may pass 2^32.
 void launch_rows_to_int8(const float* x, int n, int dim, void* codes, float* scales, cudaStream_t st);

@@ -197,6 +197,11 @@ struct KParams {
     const IvfUnit* units;           // IVF instances only: the work unit of each CTA,
     const size_t* slot;             //   where pair p's run of range 0 starts in the candidate matrix (range r: + r * kk),
     const int* ids;                 //   and the original index of each stored row
+    const uint8_t* codes;           // K13 only: stored codes [ndb, m],
+    const float* tables;            //   each query's lookup tables [nq, m, 256],
+    const float* pscore;            //   each pair's coarse score [npairs],
+    const int* pair_q;              //   each pair's query [npairs],
+    int m;                          //   and the subspaces
 };
 
 template <KOp OP, int NT>
@@ -715,6 +720,171 @@ __global__ void __launch_bounds__(256) ivf_update_kernel(const double* __restric
     }
 }
 
+// ---- IVF-PQ: residual codebooks, encoding, lookup tables and the ADC scan (K13) ----------------------------------------------------
+template <bool BF>
+CB_DEVINL float widen16(uint16_t h) {
+    if constexpr (BF) return __uint_as_float((uint32_t)h << 16);
+    else return __half2float(__ushort_as_half(h));
+}
+
+// feature f of row `row`'s residual against its list's centroid: x - c in fp32, rounded to nearest, both widened exactly
+template <bool BF>
+CB_DEVINL float pq_residual(const uint16_t* x, const uint16_t* cent, const int* lists, size_t row, int dim, int f) {
+    return __fsub_rn(widen16<BF>(x[row * dim + f]), widen16<BF>(cent[(size_t)lists[row] * dim + f]));
+}
+
+// Codes, one thread per (row, subspace s = blockIdx.y): the residual's dsub features staged feature-major in shared memory (each
+// thread reads only its own column), then the 256 codewords of s in order, d = fmaf(t, t, d) with t = r_j - b_j from +0 in feature
+// order; a NaN distance is +inf; the least distance wins, the lower index on ties (strict <), so all-inf gives code 0.  Every thread
+// of a warp reads the same codeword element: one broadcast load.
+constexpr int PQ_ENC_THREADS = 128;
+template <bool BF>
+__global__ void __launch_bounds__(PQ_ENC_THREADS) pq_encode_kernel(const uint16_t* __restrict__ x, size_t n, int dim, int m,
+                                                                   const int* __restrict__ lists, const uint16_t* __restrict__ cent,
+                                                                   const float* __restrict__ books, uint8_t* __restrict__ codes) {
+    extern __shared__ float sr[];                                          // [dsub][PQ_ENC_THREADS]
+    const int s = blockIdx.y, dsub = dim / m, t = threadIdx.x;
+    const size_t row = (size_t)blockIdx.x * PQ_ENC_THREADS + t;
+    if (row >= n) return;
+    for (int j = 0; j < dsub; j++) sr[j * PQ_ENC_THREADS + t] = pq_residual<BF>(x, cent, lists, row, dim, s * dsub + j);
+    const float* b = books + (size_t)s * 256 * dsub;
+    float best = INFINITY;
+    int bi = 0;
+    for (int k = 0; k < 256; k++) {
+        float d = 0.f;
+        for (int j = 0; j < dsub; j++) {
+            const float e = __fsub_rn(sr[j * PQ_ENC_THREADS + t], __ldg(b + k * dsub + j));
+            d = fmaf(e, e, d);
+        }
+        if (d != d) d = INFINITY;
+        if (d < best) { best = d; bi = k; }
+    }
+    codes[row * m + s] = (uint8_t)bi;
+}
+
+// Initial codebooks, one CTA per subspace: codeword i of s is the residual of training row floor(i n / 256).
+template <bool BF>
+__global__ void __launch_bounds__(256) pq_init_kernel(const uint16_t* __restrict__ x, size_t n, int dim, int m, const int* __restrict__ lists,
+                                                      const uint16_t* __restrict__ cent, float* __restrict__ books) {
+    const int s = blockIdx.x, dsub = dim / m;
+    for (int e = threadIdx.x; e < 256 * dsub; e += 256) {
+        const int i = e / dsub, j = e - i * dsub;
+        books[(size_t)s * 256 * dsub + e] = pq_residual<BF>(x, cent, lists, (size_t)i * n / 256, dim, s * dsub + j);
+    }
+}
+
+// Codebook k-means sums, pass 1: chunk c = positions ch.x .. ch.y - 1 of the flat member array ids [m][n] (one codeword's members
+// of subspace s = ch.x / n, in row order) -> part[c, dsub], each feature's residual summed in fp64 over the chunk in order.
+template <bool BF>
+__global__ void __launch_bounds__(128) pq_chunk_sum_kernel(const uint16_t* __restrict__ x, size_t n, int dim, int m, const int* __restrict__ lists,
+                                                           const uint16_t* __restrict__ cent, const int* __restrict__ ids,
+                                                           const longlong2* __restrict__ chunks, double* __restrict__ part) {
+    const longlong2 ch = chunks[blockIdx.x];
+    const int dsub = dim / m, s = (int)(ch.x / (long long)n);
+    for (int j = threadIdx.x; j < dsub; j += 128) {
+        double acc = 0.0;
+        for (long long r = ch.x; r < ch.y; r++) acc += (double)pq_residual<BF>(x, cent, lists, (size_t)ids[r], dim, s * dsub + j);
+        part[(size_t)blockIdx.x * dsub + j] = acc;
+    }
+}
+
+// Pass 2, one CTA per (subspace, codeword) = blockIdx.x: the chunk sums added in chunk order, over the count in fp64, rounded once
+// to fp32.  An empty codeword keeps its value.
+__global__ void __launch_bounds__(128) pq_update_kernel(const double* __restrict__ part, const int* __restrict__ chunk_begin,
+                                                        const int* __restrict__ count, int dsub, float* __restrict__ books) {
+    const int bk = blockIdx.x, cnt = count[bk];
+    if (cnt == 0) return;
+    for (int j = threadIdx.x; j < dsub; j += 128) {
+        double acc = 0.0;
+        for (int c = chunk_begin[bk]; c < chunk_begin[bk + 1]; c++) acc += part[(size_t)c * dsub + j];
+        books[(size_t)bk * dsub + j] = __double2float_rn(acc / (double)cnt);
+    }
+}
+
+// Lookup tables, one CTA per (subspace s = blockIdx.x, PQ_TQ queries): codebook s staged [256][dsub | 1] (an odd row stride, so
+// thread k's reads of row k fall in distinct banks) and the queries' dsub features widened; thread k writes
+// T[q][s][k] = fmaf chain over j of q_j * b_kj from +0, in feature order.
+constexpr int PQ_TQ = 32;
+template <bool BF>
+__global__ void __launch_bounds__(256) pq_table_kernel(const uint16_t* __restrict__ q, int nq, int dim, int m, const float* __restrict__ books,
+                                                       float* __restrict__ tables) {
+    extern __shared__ float sm[];
+    const int s = blockIdx.x, q0 = blockIdx.y * PQ_TQ, nqv = min(PQ_TQ, nq - q0), dsub = dim / m, ld = dsub | 1, k = threadIdx.x;
+    float* sb = sm;
+    float* sq = sm + 256 * ld;
+    for (int e = threadIdx.x; e < 256 * dsub; e += 256) { const int i = e / dsub; sb[i * ld + e - i * dsub] = books[(size_t)s * 256 * dsub + e]; }
+    for (int e = threadIdx.x; e < nqv * dsub; e += 256) {
+        const int i = e / dsub;
+        sq[e] = widen16<BF>(q[(size_t)(q0 + i) * dim + s * dsub + e - i * dsub]);
+    }
+    __syncthreads();
+    for (int i = 0; i < nqv; i++) {
+        float acc = 0.f;
+        for (int j = 0; j < dsub; j++) acc = fmaf(sq[i * dsub + j], sb[k * ld + j], acc);
+        tables[((size_t)(q0 + i) * m + s) * 256 + k] = acc;
+    }
+}
+
+// ---- K13: the ADC scan over one IVF work unit ----------------------------------------------------------------------------------
+// The unit table of K10's IVF instances: CTA u runs unit u, pairs p0 .. p0 + np - 1 of one list against stored rows row_begin ..
+// row_end - 1.  256 threads over rows, one pair at a time:
+//   table    the pair's query's table T [m][256] fp32 in shared memory, in slices of up to PQ_SLICE subspaces (128 KiB).  With one
+//            slice it is staged once per pair; with more, once per slice per 256-row tile, each row's running sum carried in a
+//            register from slice to slice, so the sum's order is s = 0 .. m - 1 whatever the slicing.
+//   row      v = coarse score, then v += T[s][code_s] in fp32 for s in order; codes read 16 at a time (one 16-byte load).  Threads
+//            over rows look up random codes, so a lookup costs as many shared-memory wavefronts as its warp has codes in one bank.
+//   select   K10's steps on one query: admission v >= theta (NaN read as -FLT_MAX), knn_push / knn_compact after each 256-row
+//            tile, and knn_finish_ivf's end (the pair's best kk to its run, positions mapped to original indices).  A tile adds at
+//            most 256 entries to a buffer compacted past kk + KB, so cap = kk + KB + 256 <= KSORT.
+constexpr int ADC_THREADS = 256, PQ_SLICE = 128;
+
+__global__ void __launch_bounds__(ADC_THREADS, 2) adc_kernel(const __grid_constant__ KParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 15) & ~(uintptr_t)15);
+    Cand* sort_s = reinterpret_cast<Cand*>(smem);
+    float* theta = reinterpret_cast<float*>(smem + KSORT * 8);
+    int* cnt = reinterpret_cast<int*>(smem + KSORT * 8 + 16);
+    uint32_t* flags = reinterpret_cast<uint32_t*>(smem + KSORT * 8 + 32);
+    float* tab = reinterpret_cast<float*>(smem + KSORT * 8 + 64);
+    const IvfUnit u = p.units[blockIdx.x];
+    const int m = p.m, nsl = (m + PQ_SLICE - 1) / PQ_SLICE;
+    Cand* const bufq = p.buf + (size_t)blockIdx.x * p.cap;
+    for (int j = 0; j < u.np; j++) {
+        const int pair = u.p0 + j;
+        const float4* T = reinterpret_cast<const float4*>(p.tables + (size_t)p.pair_q[pair] * m * 256);
+        const float s_c = p.pscore[pair];
+        if (threadIdx.x == 0) { theta[0] = -INFINITY; cnt[0] = 0; }
+        if (threadIdx.x < 4) flags[threadIdx.x] = 0;
+        for (int t0 = u.row_begin; t0 < u.row_end; t0 += ADC_THREADS) {
+            const int row = t0 + threadIdx.x;
+            float v = s_c;
+            for (int sl = 0; sl < nsl; sl++) {
+                const int sb = sl * PQ_SLICE, ns = min(PQ_SLICE, m - sb);
+                if (nsl > 1 || t0 == u.row_begin) {                // block-uniform
+                    __syncthreads();                                // every lookup of the previous slice is done
+                    float4* t4 = reinterpret_cast<float4*>(tab);
+                    for (int e = threadIdx.x; e < ns * 64; e += ADC_THREADS) t4[e] = T[sb * 64 + e];
+                    __syncthreads();
+                }
+                if (row < u.row_end) {
+                    const uint4* cr = reinterpret_cast<const uint4*>(p.codes + (size_t)row * m + sb);
+                    for (int g = 0; g < ns / 16; g++) {
+                        const uint4 w = cr[g];
+                        const uint32_t wd[4] = {w.x, w.y, w.z, w.w};
+                        const float* tg = tab + g * 16 * 256;
+                        #pragma unroll
+                        for (int b = 0; b < 16; b++) v = __fadd_rn(v, tg[b * 256 + ((wd[b >> 2] >> (8 * (b & 3))) & 0xff)]);
+                    }
+                }
+            }
+            v = v != v ? -FLT_MAX : v;
+            if (row < u.row_end && v >= theta[0]) knn_push(p, bufq, v, 0, row, cnt, flags);     // ties kept
+            knn_compact<1>(p, sort_s, bufq, theta, cnt, flags);
+        }
+        knn_finish_ivf(p, sort_s, bufq, cnt, 1, pair, u.range);
+    }
+}
+
 typedef CUresult (*EncodeTiledFnK)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -959,6 +1129,70 @@ void launch_ivf_update(bool bf, const void* x, int dim, const int* ids, const in
     }
     if (bf) ivf_update_kernel<true><<<n_lists, 256, 0, st>>>(part, chunk_begin, offsets, dim, (uint16_t*)cent);
     else ivf_update_kernel<false><<<n_lists, 256, 0, st>>>(part, chunk_begin, offsets, dim, (uint16_t*)cent);
+}
+
+template <class K>
+static cudaError_t set_smem(K k, size_t smem) {
+    return smem > 48 * 1024 ? cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) : cudaSuccess;
+}
+
+cudaError_t launch_pq_encode(bool bf, const void* x, size_t n, int dim, int m, const int* lists, const void* cent, const float* books,
+                             void* codes, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    const dim3 grid((unsigned)((n + PQ_ENC_THREADS - 1) / PQ_ENC_THREADS), (unsigned)m);
+    const size_t smem = (size_t)(dim / m) * PQ_ENC_THREADS * 4;
+    cudaError_t e = bf ? set_smem(pq_encode_kernel<true>, smem) : set_smem(pq_encode_kernel<false>, smem);
+    if (e != cudaSuccess) return e;
+    if (bf) pq_encode_kernel<true><<<grid, PQ_ENC_THREADS, smem, st>>>((const uint16_t*)x, n, dim, m, lists, (const uint16_t*)cent, books, (uint8_t*)codes);
+    else pq_encode_kernel<false><<<grid, PQ_ENC_THREADS, smem, st>>>((const uint16_t*)x, n, dim, m, lists, (const uint16_t*)cent, books, (uint8_t*)codes);
+    return cudaGetLastError();
+}
+
+void launch_pq_init(bool bf, const void* x, size_t n, int dim, int m, const int* lists, const void* cent, float* books, cudaStream_t st) {
+    if (bf) pq_init_kernel<true><<<m, 256, 0, st>>>((const uint16_t*)x, n, dim, m, lists, (const uint16_t*)cent, books);
+    else pq_init_kernel<false><<<m, 256, 0, st>>>((const uint16_t*)x, n, dim, m, lists, (const uint16_t*)cent, books);
+}
+
+void launch_pq_update(bool bf, const void* x, size_t n, int dim, int m, const int* lists, const void* cent, const int* ids,
+                      const longlong2* chunks, int nchunks, const int* chunk_begin, const int* count, double* part, float* books,
+                      cudaStream_t st) {
+    if (nchunks > 0) {
+        if (bf) pq_chunk_sum_kernel<true><<<nchunks, 128, 0, st>>>((const uint16_t*)x, n, dim, m, lists, (const uint16_t*)cent, ids, chunks, part);
+        else pq_chunk_sum_kernel<false><<<nchunks, 128, 0, st>>>((const uint16_t*)x, n, dim, m, lists, (const uint16_t*)cent, ids, chunks, part);
+    }
+    pq_update_kernel<<<m * 256, 128, 0, st>>>(part, chunk_begin, count, dim / m, books);
+}
+
+cudaError_t launch_pq_tables(bool bf, const void* q, int nq, int dim, int m, const float* books, float* tables, cudaStream_t st) {
+    if (nq <= 0) return cudaSuccess;
+    const int dsub = dim / m;
+    const size_t smem = ((size_t)256 * (dsub | 1) + (size_t)PQ_TQ * dsub) * 4;
+    cudaError_t e = bf ? set_smem(pq_table_kernel<true>, smem) : set_smem(pq_table_kernel<false>, smem);
+    if (e != cudaSuccess) return e;
+    const dim3 grid((unsigned)m, (unsigned)((nq + PQ_TQ - 1) / PQ_TQ));
+    if (bf) pq_table_kernel<true><<<grid, 256, smem, st>>>((const uint16_t*)q, nq, dim, m, books, tables);
+    else pq_table_kernel<false><<<grid, 256, smem, st>>>((const uint16_t*)q, nq, dim, m, books, tables);
+    return cudaGetLastError();
+}
+
+size_t adc_cap(int kk) { return (size_t)kk + KB + ADC_THREADS; }
+
+cudaError_t launch_adc(const void* codes, int ndb, int m, const float* tables, const float* pscore, const int* pair_q, int kk,
+                       const IvfUnit* units, int nunits, const size_t* slot, const int* ids, void* buf, float* out_v, int* out_i,
+                       cudaStream_t st) {
+    if (nunits <= 0) return cudaSuccess;
+    KParams p;
+    memset(&p, 0, sizeof(p));
+    p.buf = reinterpret_cast<Cand*>(buf);
+    p.out_v = out_v; p.out_i = out_i;
+    p.ndb = ndb; p.kk = kk; p.cap = (int)adc_cap(kk);
+    p.units = units; p.slot = slot; p.ids = ids;
+    p.codes = reinterpret_cast<const uint8_t*>(codes); p.tables = tables; p.pscore = pscore; p.pair_q = pair_q; p.m = m;
+    const size_t smem = 16 + KSORT * 8 + 64 + (size_t)std::min(m, PQ_SLICE) * 256 * 4;
+    cudaError_t e = set_smem(adc_kernel, smem);
+    if (e != cudaSuccess) return e;
+    adc_kernel<<<(unsigned)nunits, ADC_THREADS, smem, st>>>(p);
+    return cudaGetLastError();
 }
 
 }  // namespace cb

@@ -545,12 +545,84 @@ bool clip_b200_ivf_build_16(const struct clip_ctx * ctx, const void * d_db, size
  *   units come to about 4 per SM.  Queries go in blocks of Q = min(32768, max(1, 2^24 / ((w + 256) * min(nprobe, n_lists))))
  *   queries, P = Q * min(nprobe, n_lists) pairs at most.
  * - Workspace, grow-only, per block: the K10 buffers of the probes (clip_b200_topk_search_16's formula at top_k = nprobe), then
- *   U * N * (w + 256) * 8 bytes of per-unit candidates for U units (U * N < 3 P + 8 * lists probed + 512 * #SMs), P * (dim * 2 + 12)
+ *   U * N * (w + 256) * 8 bytes of per-unit candidates for U units (U * N < 3 P + 8 * lists probed + 512 * #SMs), P * (dim * 2 + 16)
  *   bytes of gathered queries and tables, and 4 * Q * runs * w * 4 bytes of merge buffers, runs = the most row ranges one query
  *   probes. */
 bool clip_b200_ivf_search_16(const struct clip_ctx * ctx, const void * d_queries, size_t n_queries, int dim, int in_type,
                              const void * d_centroids, int n_lists, const int * d_offsets, const int * d_ids,
                              const void * d_rows, size_t n_db, int nprobe, int top_k, float * scores, int * indices);
+
+/* ---- inverted-file index with product-quantised residuals (FAISS IndexIVFPQ, by residual, 8-bit codes) ----------------------
+ * The lists of clip_b200_ivf_*, but each row is stored as m one-byte codes of its residual against its list's centroid: m bytes a
+ * row instead of dim * 2, so 10^8 768-d rows take 9.6 GB of codes at m = 96.  The residual's dim features are split into m
+ * subspaces of dsub = dim / m features, and each subspace has its own 256 codewords.  The caller owns the index: centroids
+ * [n_lists, dim] of in_type (from clip_b200_ivf_train_16, for example), codebooks f32 [m, 256, dsub], and from the build offsets
+ * [n_lists + 1] int32, ids [n_db] int32 and codes uint8 [n_db, m].  Encode and build are separate calls, so a database larger than
+ * device memory is encoded in chunks of rows; only its codes and lists need to be resident at build time.
+ * - Limits: in_type, dim, n_lists, nprobe, n_iter and top_k as clip_b200_ivf_*.  m is a multiple of 16 in [16, 256] that divides
+ *   dim, so a code row is whole 16-byte words.  Training needs n_train >= 256.  Counts below 2^31; offsets into the codes are 64-bit,
+ *   so n_db * m may pass 2^32.  Device pointers are 16-byte aligned, except d_lists, d_offsets and d_ids, which need 4 bytes.  All
+ *   four run on the context's first GPU.
+ * - The rule; every step is exact, so a restatement in numpy reproduces every output bit for bit (tests/_search_ivfpq.py):
+ *   1. A row's list is its best centroid under clip_b200_ivf_build_16's rule: clip_b200_topk_search_16(row, centroids, 1).
+ *   2. Its residual r_j = x_j - c_j in fp32, rounded to nearest, both values widened exactly from in_type.
+ *   3. The distance of r to codeword b of subspace s: t = r_j - b_j in fp32, d = fmaf(t, t, d), over the subspace's features in
+ *      order, from +0.  A NaN distance counts as +inf.
+ *   4. The code of subspace s is the codeword with the least distance, the lower index on ties.  So a row holding NaN or +-Inf
+ *      gets code 0 in every subspace it touches.
+ * - Refusals, each with a message in clip_b200_last_error that starts with the function's name, in the order of the steps that
+ *   apply to the form: null context; in_type; dim; m; n_lists; n_iter / nprobe; top_k; a count >= 2^31 (train: then n_train < 256);
+ *   then, when there is work, null or misaligned device pointers, then null outputs.
+ * - Kernel time: the assignments and the probes are kernel class 7 (K10), the ADC scan class 13, the lookup tables, the codebook
+ *   k-means and the encoding class 14, the build's code gather class 12. */
+
+/* Codebook k-means (Lloyd, Euclidean) over the residuals of d_train [n_train, dim] -> d_codebooks f32 [m, 256, dsub].
+ * 1. Every training row is assigned to its list (rule 1) and its residual taken (rule 2).
+ * 2. The initial codeword i of every subspace is the residual of training row floor(i * n_train / 256).
+ * 3. Each of the n_iter iterations assigns every residual in every subspace (rules 3 and 4), then replaces each non-empty codeword
+ *    by the fp64 mean of its members' residuals, rounded once to fp32.  The members are summed in row order, in chunks of 512 whose
+ *    sums are added in chunk order, as clip_b200_ivf_train_16 sums, so a call gives the same bits every time.  An empty codeword
+ *    keeps its value.  There is no normalisation.
+ * Workspace, grow-only: about n_train * (5 m + 4) + (n_train / 512 + 256) * dim * 8 bytes, plus the K10 buffers of
+ * clip_b200_topk_search_16 at top_k = 1; the host holds n_train * 5 m bytes. */
+bool clip_b200_ivfpq_train_16(const struct clip_ctx * ctx, const void * d_train, size_t n_train, int dim, int in_type,
+                              const void * d_centroids, int n_lists, int m, int n_iter, void * d_codebooks);
+
+/* Encode d_rows [n, dim]: each row's list (rule 1) to d_lists [n] int32 and its codes (rules 2-4) to d_codes uint8 [n, m].  Chunks
+ * of a database encoded by separate calls give the bytes one call gives.  n == 0 returns true and writes nothing. */
+bool clip_b200_ivfpq_encode_16(const struct clip_ctx * ctx, const void * d_rows, size_t n, int dim, int in_type,
+                               const void * d_centroids, int n_lists, const void * d_codebooks, int m,
+                               int * d_lists, void * d_codes);
+
+/* Lay encoded rows out list by list: d_offsets and d_ids are the stable layout by original index that clip_b200_ivf_build_16 writes
+ * for the same lists, and stored position p of d_codes_out [n_db, m] holds the codes of row d_ids[p], byte for byte.  d_lists is
+ * read first: a value outside [0, n_lists) is refused before anything is written.  n_db == 0 writes n_lists + 1 zeros to d_offsets
+ * and nothing else. */
+bool clip_b200_ivfpq_build(const struct clip_ctx * ctx, const int * d_lists, const void * d_codes, size_t n_db, int n_lists, int m,
+                           int * d_offsets, int * d_ids, void * d_codes_out);
+
+/* Probe the nprobe best lists of each query and return its best top_k stored rows, by original row index, to host [n_queries, w],
+ * w = min(top_k, n_db), row i at i * w.
+ * - The probes and their coarse scores s_c are exactly what clip_b200_topk_search_16(q, centroids, nprobe) returns, NaN read as
+ *   -FLT_MAX included.
+ * - The lookup table of a query: T[s][k] = the fmaf chain over subspace s's features j of q_j * b_kj, from +0, in order, with q
+ *   widened exactly.  A stored row with codes c in list l scores v = s_c, then v = v + T[s][c_s] in fp32 for s = 0 .. m - 1 in
+ *   order.  For inner product this is FAISS's by-residual IVFPQ score <q, c_l> + <q, r^>; the table depends on the query alone.
+ * - Ranking, padding and d_offsets' check are clip_b200_ivf_search_16's: score descending, then the lower original index; a NaN
+ *   score ranks last and is reported as -FLT_MAX; (-INFINITY, -1) past the probed rows; a malformed d_offsets is refused before
+ *   any device work.  n_queries == 0 or n_db == 0 returns true and writes nothing.
+ * - The scan (K13) runs clip_b200_ivf_search_16's work units with at most N = 8 pairs a unit (K13 scores a unit's pairs one after
+ *   another, so a unit costs its pairs times its rows), 256 threads over rows, one pair at a time, with the pair's table in shared
+ *   memory in slices of up to 128 subspaces.  Queries go in blocks of
+ *   Q = min(32768, max(1, 2^24 / ((w + 256) * min(nprobe, n_lists))), 2^18 / m), so the tables of a block, Q * m KiB, stay within
+ *   256 MiB.
+ * - Workspace, grow-only, per block: the K10 buffers of the probes, Q * m KiB of tables, U * (w + 384) * 8 bytes of per-unit
+ *   candidates for U units (U < 3 P + lists probed + 512 * #SMs, P = Q * min(nprobe, n_lists) pairs at most), P * 16 + U * 20 bytes
+ *   of plan, and 4 * Q * runs * w * 4 bytes of merge buffers, runs = the most row ranges one query probes. */
+bool clip_b200_ivfpq_search_16(const struct clip_ctx * ctx, const void * d_queries, size_t n_queries, int dim, int in_type,
+                               const void * d_centroids, int n_lists, const void * d_codebooks, int m,
+                               const int * d_offsets, const int * d_ids, const void * d_codes, size_t n_db,
+                               int nprobe, int top_k, float * scores, int * indices);
 
 /* Batched zero-shot labelling, the batch form of clip_zero_shot_label_image (clip.h:106-107, clip.cpp:1624-1659): n images x
  * n_labels token sequences -> scores / indices [n, top_k], best first (p = (exp(s)+1e-9)/sum over ALL labels, clip.cpp:1591-1622).
@@ -618,7 +690,8 @@ float    clip_b200_last_device_ms(const struct clip_ctx * ctx);    /* CUDA-event
  * attention-probability kernel of ATTENTION entries, 7 the 16-bit search kernel of clip_b200_topk_search_16, 8 the int8 search
  * kernel of clip_b200_topk_search_i8, 9 the binary search kernel of clip_b200_topk_search_b1, 10 the rescore kernel of
  * clip_b200_topk_rescore, 11 the fine scan of clip_b200_ivf_search_16, 12 the k-means update of clip_b200_ivf_train_16 and the row
- * gather of clip_b200_ivf_build_16); *count
+ * gather of clip_b200_ivf_build_16 and clip_b200_ivfpq_build, 13 the ADC scan of clip_b200_ivfpq_search_16, 14 its lookup tables,
+ * the codebook k-means of clip_b200_ivfpq_train_16 and the encoding of clip_b200_ivfpq_encode_16); *count
  * receives the number of launches.  Enabled by env CLIP_B200_PROFILE=1. */
 float    clip_b200_kernel_ms(const struct clip_ctx * ctx, int kind, uint64_t * count);
 /* CUDA-event stopwatch on the launch stream: mark(slot 0..3), then elapsed(a, b) in ms (-1 on error) */
